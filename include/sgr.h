@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define SGR_ABI_VERSION 4
+#define SGR_ABI_VERSION 5
 
 #define SGR_OK 0
 #define SGR_EINVAL (-1)   /* bad argument combination / shape                     */
@@ -308,6 +308,24 @@ int sgr_image_loss(int32_t C, int32_t H, int32_t W, const float *image, const fl
  * scalars (device, 2 floats): {weight * mean, mean}; dL_dacc[N] (or NULL) = weight * d mean / d acc.  scratch: >= 8 bytes. */
 int sgr_sky_loss(int64_t N, const float *acc, const uint8_t *sky_mask, float weight, float *dL_dacc, float *scalars, void *scratch,
                  void *stream);
+/* Object-accumulation loss (train.py:114-122, on the acc of the objects-only render): acc clamped to [1e-6, 1-1e-6], mean over the
+ * N pixels of obj_bound ? -(acc log acc + (1-acc) log(1-acc)) : -log(1-acc).  scalars (device, 2 floats): {weight * mean, mean};
+ * dL_dacc[N] (or NULL) = weight * d mean / d acc, zero where the clamp is active.  scratch: >= 8 bytes. */
+int sgr_obj_acc_loss(int64_t N, const float *acc, const uint8_t *obj_bound, float weight, float *dL_dacc, float *scalars, void *scratch,
+                     void *stream);
+/* LiDAR depth loss (train.py:124-132): on the valid pixels (lidar_depth > 0 and mask, mask uint8 [N] or NULL = all),
+ * err = |depth / (acc + 1e-10) - lidar_depth|; value = mean of the k = int(keep * n) smallest err (n = valid pixels, k formed in
+ * double and truncated like Python's int(0.95 * n)).  acc is the UNCLAMPED accumulation (render_pkg['acc']), not the sky loss's
+ * clamped copy.  The k smallest are found on the device by an exact radix select, so nothing is read back to the host and the grid
+ * sizes depend on N only (the call can be captured in a CUDA graph).  NaN errors order above every number, like torch.topk.
+ * Gradients (either pointer may be NULL): the k selected pixels get g = weight * sign(e - lidar_depth) / k with sign(0) = 0,
+ * dL_ddepth = g / (acc + 1e-10), dL_dacc = -g * e / (acc + 1e-10); all other pixels 0.  Of the pixels tied at the k-th value, those
+ * with the lowest flat index are taken.  k == 0 (n <= 1 at keep = 0.95) gives a NaN value and all-zero gradients.
+ *   depth, acc, lidar_depth: [N] fp32 device; 0 < keep <= 1; N < 2^31.
+ *   scalars (device, 4 floats): {weight * mean, mean, n, k}.  scratch: sgr_lidar_depth_loss_scratch_bytes(N) bytes. */
+size_t sgr_lidar_depth_loss_scratch_bytes(int64_t N);
+int sgr_lidar_depth_loss(int64_t N, const float *depth, const float *acc, const float *lidar_depth, const uint8_t *mask, double keep,
+                         float weight, float *dL_ddepth, float *dL_dacc, float *scalars, void *scratch, size_t scratch_bytes, void *stream);
 
 /* ---- Post-backward bookkeeping of a training iteration (SURVEY.md §8 row f3) ----
  * Densification statistics of StreetGaussianModel.set_max_radii2D + add_densification_stats

@@ -8,7 +8,7 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libsgr.so")
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_state_sizes", "sgr_binning_bytes", "sgr_forward", "sgr_forward_bounded",
            "sgr_forward_status", "sgr_forward_status_async", "sgr_backward_blend",
@@ -16,7 +16,7 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_state_s
            "sgr_knn_mean_dist2", "sgr_record_bytes", "sgr_project", "sgr_forward_records",
            "sgr_scatter_records", "sgr_gather_grad2d", "sgr_peer_barrier", "sgr_sharded_forward", "sgr_sharded_backward",
            "sgr_compose_forward", "sgr_compose_backward", "sgr_image_loss_scratch_bytes", "sgr_image_loss", "sgr_sky_loss",
-           "sgr_densify_stats", "sgr_adam_step"]
+           "sgr_obj_acc_loss", "sgr_lidar_depth_loss_scratch_bytes", "sgr_lidar_depth_loss", "sgr_densify_stats", "sgr_adam_step"]
 
 
 class SgrFrame(C.Structure):
@@ -128,6 +128,12 @@ def lib():
     L.sgr_image_loss.argtypes = [C.c_int32] * 3 + [vp, vp, vp, C.c_float, C.c_float, vp, vp, vp, C.c_size_t, vp]
     L.sgr_sky_loss.restype = C.c_int
     L.sgr_sky_loss.argtypes = [C.c_int64, vp, vp, C.c_float, vp, vp, vp, vp]
+    L.sgr_obj_acc_loss.restype = C.c_int
+    L.sgr_obj_acc_loss.argtypes = [C.c_int64, vp, vp, C.c_float, vp, vp, vp, vp]
+    L.sgr_lidar_depth_loss_scratch_bytes.restype = C.c_size_t
+    L.sgr_lidar_depth_loss_scratch_bytes.argtypes = [C.c_int64]
+    L.sgr_lidar_depth_loss.restype = C.c_int
+    L.sgr_lidar_depth_loss.argtypes = [C.c_int64, vp, vp, vp, vp, C.c_double, C.c_float, vp, vp, vp, vp, C.c_size_t, vp]
     L.sgr_densify_stats.restype = C.c_int
     L.sgr_densify_stats.argtypes = [C.POINTER(SgrStatSegment), C.c_int32, vp, vp, vp]
     L.sgr_adam_step.restype = C.c_int

@@ -659,6 +659,33 @@ int sgr_sky_loss(int64_t N, const float *acc, const uint8_t *sky_mask, float wei
 	return SGR_OK;
 }
 
+// replaces train.py:114-122 (clamp / where / entropy / mean on the objects-only render's acc)
+int sgr_obj_acc_loss(int64_t N, const float *acc, const uint8_t *obj_bound, float weight, float *dL_dacc, float *scalars, void *scratch, void *stream) {
+	if (N <= 0) return fail(SGR_EINVAL, "N must be positive");
+	if (!acc || !obj_bound || !scalars || !scratch) return fail(SGR_EINVAL, "NULL pointer passed to sgr_obj_acc_loss");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_obj_acc_loss((size_t)N, acc, obj_bound, weight, dL_dacc, scalars, scratch, st), "obj_acc_loss");
+	return SGR_OK;
+}
+
+// replaces train.py:124-132 (boolean index, torch.topk with a host-side k, mean) and its autograd replay
+size_t sgr_lidar_depth_loss_scratch_bytes(int64_t N) { return (N > 0 && N < ((int64_t)1 << 31)) ? lidar_depth_loss_scratch_bytes((size_t)N) : 0; }
+
+int sgr_lidar_depth_loss(int64_t N, const float *depth, const float *acc, const float *lidar_depth, const uint8_t *mask, double keep, float weight,
+                         float *dL_ddepth, float *dL_dacc, float *scalars, void *scratch, size_t scratch_bytes, void *stream) {
+	if (N <= 0 || N >= ((int64_t)1 << 31)) return fail(SGR_EINVAL, "N must be in [1, 2^31), got %lld", (long long)N);
+	if (!(keep > 0.0 && keep <= 1.0)) return fail(SGR_EINVAL, "keep must be in (0, 1], got %g", keep);
+	if (!depth || !acc || !lidar_depth || !scalars) return fail(SGR_EINVAL, "NULL pointer passed to sgr_lidar_depth_loss");
+	if (!scratch || scratch_bytes < lidar_depth_loss_scratch_bytes((size_t)N))
+		return fail(SGR_ENOMEM, "lidar depth loss scratch too small: %zu < %zu", scratch_bytes, lidar_depth_loss_scratch_bytes((size_t)N));
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_lidar_depth_loss((size_t)N, depth, acc, lidar_depth, mask, keep, weight, dL_ddepth, dL_dacc, scalars, scratch, st),
+	        "lidar_depth_loss");
+	return SGR_OK;
+}
+
 int sgr_densify_stats(const SgrStatSegment *segments, int32_t num_segments, const int32_t *radii, const float *means2D_grad, void *stream) {
 	if (!segments || num_segments <= 0) return fail(SGR_EINVAL, "segment table is empty");
 	int64_t at = 0;

@@ -177,9 +177,27 @@ __global__ void __launch_bounds__(256) ssim_grad_kernel(const int C, const int H
 	grad[o] = g;
 }
 
-// sky / accumulation loss (train.py:107-113): acc clamped to [1e-6, 1 - 1e-6]; mean of  sky ? -log(1 - acc) : -log(acc).
-// out[0] += sum; grad = weight / N * d/dacc (zero where the clamp is active, like torch.clamp's backward).
-__global__ void __launch_bounds__(256) sky_loss_kernel(const size_t N, const float *__restrict__ accm, const uint8_t *__restrict__ sky, const float weight,
+// Per-pixel losses of an accumulation map clamped to [1e-6, 1 - 1e-6], selected per pixel by a uint8 flag.
+// sky (train.py:107-108):          sky ? -log(1 - acc) : -log(acc)
+struct SkyForm {
+	static __device__ __forceinline__ float value(float ac, bool s) { return s ? -logf(1.f - ac) : -logf(ac); }
+	static __device__ __forceinline__ float deriv(float ac, bool s) { return s ? 1.f / (1.f - ac) : -1.f / ac; }
+};
+// object accumulation (train.py:117-120): obj_bound ? -(acc log acc + (1 - acc) log(1 - acc)) : -log(1 - acc)
+struct ObjForm {
+	static __device__ __forceinline__ float value(float ac, bool b) {
+		const float om = 1.f - ac;
+		return b ? -__fadd_rn(__fmul_rn(ac, logf(ac)), __fmul_rn(om, logf(om))) : -logf(om);  // two roundings, as torch does them
+	}
+	static __device__ __forceinline__ float deriv(float ac, bool b) {
+		const float om = 1.f - ac;
+		return b ? logf(om) - logf(ac) : 1.f / om;
+	}
+};
+
+// out[0] += sum of Form::value; grad = weight / N * d/dacc (zero where the clamp is active, like torch.clamp's backward).
+template <class Form>
+__global__ void __launch_bounds__(256) acc_loss_kernel(const size_t N, const float *__restrict__ accm, const uint8_t *__restrict__ flag, const float weight,
                                                       float *__restrict__ grad, double *__restrict__ out) {
 	__shared__ float red[8];
 	float v = 0.f;
@@ -187,9 +205,9 @@ __global__ void __launch_bounds__(256) sky_loss_kernel(const size_t N, const flo
 		const float a = accm[i];
 		const float ac = fminf(fmaxf(a, 1e-6f), 1.f - 1e-6f);
 		const bool inside = a >= 1e-6f && a <= 1.f - 1e-6f;
-		const bool s = sky[i] != 0;
-		v += s ? -logf(1.f - ac) : -logf(ac);
-		if (grad) grad[i] = inside ? (weight / (float)N) * (s ? 1.f / (1.f - ac) : -1.f / ac) : 0.f;
+		const bool s = flag[i] != 0;
+		v += Form::value(ac, s);
+		if (grad) grad[i] = inside ? (weight / (float)N) * Form::deriv(ac, s) : 0.f;
 	}
 #pragma unroll
 	for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -201,7 +219,7 @@ __global__ void __launch_bounds__(256) sky_loss_kernel(const size_t N, const flo
 		atomicAdd(out, s);
 	}
 }
-__global__ void sky_finalize_kernel(const size_t N, const float weight, const double *__restrict__ sum, float *__restrict__ scalars) {
+__global__ void acc_loss_finalize_kernel(const size_t N, const float weight, const double *__restrict__ sum, float *__restrict__ scalars) {
 	scalars[0] = (float)((double)weight * (*sum / (double)N));
 	scalars[1] = (float)(*sum / (double)N);
 }
@@ -223,14 +241,273 @@ cudaError_t launch_image_loss(int C, int H, int W, const float *img, const float
 	return cudaGetLastError();
 }
 
-cudaError_t launch_sky_loss(size_t N, const float *accm, const uint8_t *sky, float weight, float *grad, float *scalars, void *scratch, cudaStream_t st) {
+template <class Form>
+static cudaError_t launch_acc_loss(size_t N, const float *accm, const uint8_t *flag, float weight, float *grad, float *scalars, void *scratch,
+                                   cudaStream_t st) {
 	double *sum = reinterpret_cast<double *>(scratch);
 	cudaError_t e = cudaMemsetAsync(sum, 0, sizeof(double), st);
 	if (e != cudaSuccess) return e;
 	const unsigned nblk = (unsigned)((N + 255) / 256 < kNumSMs * 8 ? (N + 255) / 256 : kNumSMs * 8);
 	count_launch(2);
-	sky_loss_kernel<<<nblk ? nblk : 1, 256, 0, st>>>(N, accm, sky, weight, grad, sum);
-	sky_finalize_kernel<<<1, 1, 0, st>>>(N, weight, sum, scalars);
+	acc_loss_kernel<Form><<<nblk ? nblk : 1, 256, 0, st>>>(N, accm, flag, weight, grad, sum);
+	acc_loss_finalize_kernel<<<1, 1, 0, st>>>(N, weight, sum, scalars);
+	return cudaGetLastError();
+}
+
+cudaError_t launch_sky_loss(size_t N, const float *accm, const uint8_t *sky, float weight, float *grad, float *scalars, void *scratch, cudaStream_t st) {
+	return launch_acc_loss<SkyForm>(N, accm, sky, weight, grad, scalars, scratch, st);
+}
+
+cudaError_t launch_obj_acc_loss(size_t N, const float *accm, const uint8_t *obj_bound, float weight, float *grad, float *scalars, void *scratch,
+                                cudaStream_t st) {
+	return launch_acc_loss<ObjForm>(N, accm, obj_bound, weight, grad, scalars, scratch, st);
+}
+
+// ---- LiDAR depth loss (train.py:124-132) ----
+// Radix digits of the 32-bit keys: bits 31..21, 20..10, 9..0.  Valid errors are >= 0 (NaN included, |x| clears the sign), so the
+// unsigned order of their bit patterns is the float order with NaN above +inf, as torch.topk orders it.
+constexpr int kLidarBins = 2048;
+struct LidarState {
+	uint32_t n;       // valid pixels
+	uint32_t k;       // int(keep * n)
+	uint32_t prefix;  // digits selected so far; after the last level the k-th smallest key t
+	uint32_t rank;    // 1-based rank of the k-th smallest key among the keys carrying `prefix`; in the end the number of ties taken
+	double sum_lt;    // sum of the errors whose key is < t
+	uint32_t hist[3][kLidarBins];
+};
+// Every pass splits the image into the same lidar_grid(N) blocks of contiguous pixel ranges (the grid depends on N only, so the call
+// can be captured in a CUDA graph); the k smallest errors are found by an exact radix select on their fp32 bit patterns.
+struct LidarGrid {
+	unsigned blocks;
+	size_t chunk;  // pixels per block, a multiple of 256
+};
+static LidarGrid lidar_grid(size_t N) {
+	const size_t tiles = (N + 255) / 256;
+	const size_t blocks = tiles < kNumSMs * 4 ? tiles : kNumSMs * 4;
+	return LidarGrid{(unsigned)(blocks ? blocks : 1), ((tiles + blocks - 1) / (blocks ? blocks : 1)) * 256};
+}
+
+size_t lidar_depth_loss_scratch_bytes(size_t N) {
+	return align_up(sizeof(LidarState)) + align_up((size_t)lidar_grid(N).blocks * sizeof(uint32_t)) + align_up(N * sizeof(uint32_t));
+}
+
+// pass 1: e = depth / (acc + 1e-10), key = bits of |e - lidar| on valid pixels (0xFFFFFFFF elsewhere), n, histogram of key >> 21
+__global__ void __launch_bounds__(256) lidar_key_kernel(const size_t N, const size_t chunk, const float *__restrict__ depth,
+                                                       const float *__restrict__ acc, const float *__restrict__ lidar,
+                                                       const uint8_t *__restrict__ mask, uint32_t *__restrict__ keys, LidarState *__restrict__ s) {
+	__shared__ uint32_t hist[kLidarBins];
+	__shared__ uint32_t nblk;
+	for (int b = threadIdx.x; b < kLidarBins; b += 256) hist[b] = 0;
+	if (threadIdx.x == 0) nblk = 0;
+	__syncthreads();
+	const size_t lo = (size_t)blockIdx.x * chunk, hi = lo + chunk < N ? lo + chunk : N;
+	uint32_t cnt = 0;
+	for (size_t i = lo + threadIdx.x; i < hi; i += 256) {
+		const float l = lidar[i];
+		uint32_t key = 0xFFFFFFFFu;
+		if (l > 0.f && (mask == nullptr || mask[i])) {
+			const float e = __fdiv_rn(depth[i], __fadd_rn(acc[i], 1e-10f));
+			key = __float_as_uint(fabsf(__fsub_rn(e, l)));
+			atomicAdd(&hist[key >> 21], 1u);
+			cnt++;
+		}
+		keys[i] = key;
+	}
+#pragma unroll
+	for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+	if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(&nblk, cnt);
+	__syncthreads();
+	for (int b = threadIdx.x; b < kLidarBins; b += 256)
+		if (hist[b]) atomicAdd(&s->hist[0][b], hist[b]);
+	if (threadIdx.x == 0 && nblk) atomicAdd(&s->n, nblk);
+}
+
+// passes 2 and 3: histogram of the next digit of the keys that carry the prefix selected so far
+//   level 1: keys with key >> 21 == prefix, digit (key >> 10) & 2047;  level 2: key >> 10 == prefix, digit key & 1023
+__global__ void __launch_bounds__(256) lidar_hist_kernel(const size_t N, const size_t chunk, const int level, const uint32_t *__restrict__ keys,
+                                                        LidarState *__restrict__ s) {
+	__shared__ uint32_t hist[kLidarBins];
+	if (s->k == 0) return;
+	for (int b = threadIdx.x; b < kLidarBins; b += 256) hist[b] = 0;
+	__syncthreads();
+	const uint32_t prefix = s->prefix;
+	const int shift = level == 1 ? 21 : 10, dshift = level == 1 ? 10 : 0;
+	const uint32_t dmask = level == 1 ? 2047u : 1023u;
+	const size_t lo = (size_t)blockIdx.x * chunk, hi = lo + chunk < N ? lo + chunk : N;
+	for (size_t i = lo + threadIdx.x; i < hi; i += 256) {
+		const uint32_t key = keys[i];
+		if (key != 0xFFFFFFFFu && (key >> shift) == prefix) atomicAdd(&hist[(key >> dshift) & dmask], 1u);
+	}
+	__syncthreads();
+	for (int b = threadIdx.x; b < kLidarBins; b += 256)
+		if (hist[b]) atomicAdd(&s->hist[level][b], hist[b]);
+}
+
+// One block of 1024 threads: finds the digit of the level's histogram that holds the rank-th smallest key and narrows the prefix and the
+// rank to that bin.  Level 0 first forms k = int(keep * n) in fp64, exactly Python's int(0.95 * n).
+__global__ void __launch_bounds__(1024) lidar_select_kernel(const int level, const double keep, LidarState *__restrict__ s) {
+	__shared__ uint32_t warp_sum[32];
+	__shared__ uint32_t k_sh;
+	if (threadIdx.x == 0) {
+		if (level == 0) s->k = (uint32_t)(keep * (double)s->n);
+		k_sh = s->k;
+	}
+	__syncthreads();
+	if (k_sh == 0) return;
+	const uint32_t rank = level == 0 ? k_sh : s->rank;  // 1-based rank among the keys that carry the prefix
+	constexpr int kPer = kLidarBins / 1024;
+	const uint32_t *h = s->hist[level];
+	uint32_t c[kPer], own = 0;
+#pragma unroll
+	for (int j = 0; j < kPer; j++) own += (c[j] = h[threadIdx.x * kPer + j]);
+	// block inclusive scan of `own`
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	uint32_t inc = own;
+#pragma unroll
+	for (int o = 1; o < 32; o <<= 1) {
+		const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
+		if (lane >= o) inc += t;
+	}
+	if (lane == 31) warp_sum[warp] = inc;
+	__syncthreads();
+	if (warp == 0) {
+		uint32_t w = warp_sum[lane];
+#pragma unroll
+		for (int o = 1; o < 32; o <<= 1) {
+			const uint32_t t = __shfl_up_sync(0xffffffffu, w, o);
+			if (lane >= o) w += t;
+		}
+		warp_sum[lane] = w;
+	}
+	__syncthreads();
+	if (warp > 0) inc += warp_sum[warp - 1];
+	const uint32_t exc = inc - own;
+	if (own == 0 || rank <= exc || rank > inc) return;  // exactly one thread holds the rank
+	static_assert(kPer == 2, "two bins per thread");
+	uint32_t below = exc, d = 0;
+	if (rank > below + c[0]) {  // then the rank lies in the second bin, since rank <= inc
+		below += c[0];
+		d = 1;
+	}
+	const uint32_t digit = threadIdx.x * kPer + d;
+	const int bits = level == 2 ? 10 : 11;
+	s->prefix = level == 0 ? digit : ((s->prefix << bits) | digit);
+	s->rank = rank - below;
+}
+
+// pass 4: t = prefix (the k-th smallest key).  sum of err over keys < t (fp64) and the number of keys == t in each block
+__global__ void __launch_bounds__(256) lidar_sum_kernel(const size_t N, const size_t chunk, const uint32_t *__restrict__ keys,
+                                                       LidarState *__restrict__ s, uint32_t *__restrict__ block_ties) {
+	__shared__ double red_s[8];
+	__shared__ uint32_t red_t[8];
+	if (s->k == 0) return;
+	const uint32_t t = s->prefix;
+	const size_t lo = (size_t)blockIdx.x * chunk, hi = lo + chunk < N ? lo + chunk : N;
+	double sum = 0.0;
+	uint32_t ties = 0;
+	for (size_t i = lo + threadIdx.x; i < hi; i += 256) {
+		const uint32_t key = keys[i];
+		if (key < t) sum += (double)__uint_as_float(key);
+		ties += key == t;
+	}
+#pragma unroll
+	for (int o = 16; o > 0; o >>= 1) {
+		sum += __shfl_xor_sync(0xffffffffu, sum, o);
+		ties += __shfl_xor_sync(0xffffffffu, ties, o);
+	}
+	if ((threadIdx.x & 31) == 0) { red_s[threadIdx.x >> 5] = sum; red_t[threadIdx.x >> 5] = ties; }
+	__syncthreads();
+	if (threadIdx.x == 0) {
+		double bs = 0.0;
+		uint32_t bt = 0;
+		for (int w = 0; w < 8; w++) { bs += red_s[w]; bt += red_t[w]; }
+		if (bs != 0.0) atomicAdd(&s->sum_lt, bs);
+		block_ties[blockIdx.x] = bt;
+	}
+}
+
+// pass 5: the k selected pixels (keys < t, plus the s->rank tied pixels of lowest flat index) get g = weight * sign(e - lidar) / k,
+//   dL/ddepth = g / (acc + 1e-10), dL/dacc = -g * (e / (acc + 1e-10)) (torch's div backward); every other pixel 0.
+//   Block 0 writes scalars {weight * mean, mean, n, k}; k == 0 gives NaN and all-zero gradients, like the mean of an empty top-k.
+__global__ void __launch_bounds__(256) lidar_grad_kernel(const size_t N, const size_t chunk, const float *__restrict__ depth,
+                                                        const float *__restrict__ acc, const float *__restrict__ lidar,
+                                                        const uint32_t *__restrict__ keys, const LidarState *__restrict__ s,
+                                                        const uint32_t *__restrict__ block_ties, const float weight, float *__restrict__ dL_ddepth,
+                                                        float *__restrict__ dL_dacc, float *__restrict__ scalars) {
+	__shared__ uint32_t warp_cnt[8];
+	__shared__ uint32_t base_sh;
+	const uint32_t k = s->k, t = s->prefix, take = s->rank;
+	if (blockIdx.x == 0 && threadIdx.x == 0) {
+		const double mean = k ? (s->sum_lt + (double)take * (double)__uint_as_float(t)) / (double)k : 0.0 / 0.0;
+		scalars[0] = (float)((double)weight * mean);
+		scalars[1] = (float)mean;
+		scalars[2] = (float)s->n;
+		scalars[3] = (float)k;
+	}
+	if (dL_ddepth == nullptr && dL_dacc == nullptr) return;
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	// ties in the blocks before this one
+	uint32_t before = 0;
+	if (k) {
+		for (unsigned b = threadIdx.x; b < blockIdx.x; b += 256) before += block_ties[b];
+#pragma unroll
+		for (int o = 16; o > 0; o >>= 1) before += __shfl_xor_sync(0xffffffffu, before, o);
+		if (lane == 0) warp_cnt[warp] = before;
+		__syncthreads();
+		if (threadIdx.x == 0) {
+			uint32_t b = 0;
+			for (int w = 0; w < 8; w++) b += warp_cnt[w];
+			base_sh = b;
+		}
+		__syncthreads();
+		before = base_sh;
+	}
+	const float gk = k ? weight / (float)k : 0.f;
+	const size_t lo = (size_t)blockIdx.x * chunk, hi = lo + chunk < N ? lo + chunk : N;
+	for (size_t i0 = lo; i0 < hi; i0 += 256) {  // block-uniform trip count: the tie scan below needs every thread
+		const size_t i = i0 + threadIdx.x;
+		const uint32_t key = (k && i < hi) ? keys[i] : 0xFFFFFFFFu;
+		const bool tie = k && key == t;
+		const unsigned ballot = __ballot_sync(0xffffffffu, tie);
+		__syncthreads();  // warp_cnt of the previous tile has been read
+		if (lane == 0) warp_cnt[warp] = __popc(ballot);
+		__syncthreads();
+		uint32_t rank = before + __popc(ballot & ((1u << lane) - 1u));
+		for (int w = 0; w < warp; w++) rank += warp_cnt[w];
+		for (int w = 0; w < 8; w++) before += warp_cnt[w];
+		if (i >= hi) continue;
+		float gd = 0.f, ga = 0.f;
+		if (key < t || (tie && rank < take)) {
+			const float l = lidar[i], b = __fadd_rn(acc[i], 1e-10f);
+			const float e = __fdiv_rn(depth[i], b), df = __fsub_rn(e, l);
+			const float g = (df > 0.f ? 1.f : (df < 0.f ? -1.f : 0.f)) * gk;  // torch.abs backward: sign(0) = sign(NaN) = 0
+			gd = __fdiv_rn(g, b);
+			ga = -g * __fdiv_rn(e, b);
+		}
+		if (dL_ddepth) dL_ddepth[i] = gd;
+		if (dL_dacc) dL_dacc[i] = ga;
+	}
+}
+
+cudaError_t launch_lidar_depth_loss(size_t N, const float *depth, const float *acc, const float *lidar, const uint8_t *mask, double keep, float weight,
+                                    float *dL_ddepth, float *dL_dacc, float *scalars, void *scratch, cudaStream_t st) {
+	const LidarGrid G = lidar_grid(N);
+	char *p = reinterpret_cast<char *>(scratch);
+	LidarState *s = reinterpret_cast<LidarState *>(p);
+	uint32_t *block_ties = reinterpret_cast<uint32_t *>(p + align_up(sizeof(LidarState)));
+	uint32_t *keys = reinterpret_cast<uint32_t *>(p + align_up(sizeof(LidarState)) + align_up((size_t)G.blocks * sizeof(uint32_t)));
+	cudaError_t e = cudaMemsetAsync(s, 0, sizeof(LidarState), st);
+	if (e != cudaSuccess) return e;
+	count_launch(8);
+	lidar_key_kernel<<<G.blocks, 256, 0, st>>>(N, G.chunk, depth, acc, lidar, mask, keys, s);
+	lidar_select_kernel<<<1, 1024, 0, st>>>(0, keep, s);
+	lidar_hist_kernel<<<G.blocks, 256, 0, st>>>(N, G.chunk, 1, keys, s);
+	lidar_select_kernel<<<1, 1024, 0, st>>>(1, keep, s);
+	lidar_hist_kernel<<<G.blocks, 256, 0, st>>>(N, G.chunk, 2, keys, s);
+	lidar_select_kernel<<<1, 1024, 0, st>>>(2, keep, s);
+	lidar_sum_kernel<<<G.blocks, 256, 0, st>>>(N, G.chunk, keys, s, block_ties);
+	lidar_grad_kernel<<<(dL_ddepth || dL_dacc) ? G.blocks : 1, 256, 0, st>>>(N, G.chunk, depth, acc, lidar, keys, s, block_ties, weight, dL_ddepth,
+	                                                                        dL_dacc, scalars);
 	return cudaGetLastError();
 }
 
