@@ -8,7 +8,7 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libsgr.so")
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_state_sizes", "sgr_binning_bytes", "sgr_forward", "sgr_forward_bounded",
            "sgr_forward_status", "sgr_forward_status_async", "sgr_backward_blend",
@@ -16,7 +16,8 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_state_s
            "sgr_knn_mean_dist2", "sgr_record_bytes", "sgr_project", "sgr_forward_records",
            "sgr_scatter_records", "sgr_gather_grad2d", "sgr_peer_barrier", "sgr_sharded_forward", "sgr_sharded_backward",
            "sgr_compose_forward", "sgr_compose_backward", "sgr_image_loss_scratch_bytes", "sgr_image_loss", "sgr_sky_loss",
-           "sgr_obj_acc_loss", "sgr_lidar_depth_loss_scratch_bytes", "sgr_lidar_depth_loss", "sgr_densify_stats", "sgr_adam_step"]
+           "sgr_obj_acc_loss", "sgr_lidar_depth_loss_scratch_bytes", "sgr_lidar_depth_loss", "sgr_densify_stats", "sgr_adam_step",
+           "sgr_densify_scratch_bytes", "sgr_densify_plan", "sgr_densify_apply", "sgr_reset_opacity"]
 
 
 class SgrFrame(C.Structure):
@@ -55,6 +56,26 @@ class SgrStatSegment(C.Structure):
 class SgrAdamTensor(C.Structure):
     _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p), ("numel", C.c_int64),
                 ("lr", C.c_float), ("step", C.c_int32)]
+
+
+DENSIFY_TENSORS = 7   # _xyz, _features_dc, _features_rest, _opacity, _scaling, _rotation, _semantic
+DENSIFY_DRAWS = 18
+DENSIFY_RESULT = 8
+DENSIFY_BACKGROUND, DENSIFY_ACTOR = 0, 1
+
+
+class SgrDensifySegment(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("count", C.c_int32), ("dc_width", C.c_int32), ("rest_width", C.c_int32), ("semantic_width", C.c_int32),
+                ("grad_col", C.c_int32), ("prune_big", C.c_int32), ("reserved", C.c_int32), ("param", C.c_void_p * DENSIFY_TENSORS),
+                ("exp_avg", C.c_void_p * DENSIFY_TENSORS), ("exp_avg_sq", C.c_void_p * DENSIFY_TENSORS), ("max_radii2D", C.c_void_p),
+                ("xyz_gradient_accum", C.c_void_p), ("denom", C.c_void_p), ("grad_threshold", C.c_float), ("dense_threshold", C.c_float),
+                ("big_threshold", C.c_float), ("min_opacity", C.c_float), ("sphere_center", C.c_float * 3), ("sphere_diameter", C.c_float),
+                ("min_xyz", C.c_float * 3), ("max_xyz", C.c_float * 3)]
+
+
+class SgrDensifyOutput(C.Structure):
+    _fields_ = [("count", C.c_int32), ("reserved", C.c_int32), ("param", C.c_void_p * DENSIFY_TENSORS), ("exp_avg", C.c_void_p * DENSIFY_TENSORS),
+                ("exp_avg_sq", C.c_void_p * DENSIFY_TENSORS), ("max_radii2D", C.c_void_p), ("xyz_gradient_accum", C.c_void_p), ("denom", C.c_void_p)]
 
 
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
@@ -138,6 +159,14 @@ def lib():
     L.sgr_densify_stats.argtypes = [C.POINTER(SgrStatSegment), C.c_int32, vp, vp, vp]
     L.sgr_adam_step.restype = C.c_int
     L.sgr_adam_step.argtypes = [C.POINTER(SgrAdamTensor), C.c_int32, C.c_double, C.c_double, C.c_double, vp]
+    L.sgr_densify_scratch_bytes.restype = C.c_size_t
+    L.sgr_densify_scratch_bytes.argtypes = [C.c_int32, C.c_int64]
+    L.sgr_densify_plan.restype = C.c_int
+    L.sgr_densify_plan.argtypes = [C.POINTER(SgrDensifySegment), C.c_int32, C.c_uint64, vp, vp, C.c_size_t, C.POINTER(C.c_int64), vp]
+    L.sgr_densify_apply.restype = C.c_int
+    L.sgr_densify_apply.argtypes = [C.POINTER(SgrDensifySegment), C.POINTER(SgrDensifyOutput), C.c_int32, C.c_uint64, vp, vp, C.c_size_t, vp]
+    L.sgr_reset_opacity.restype = C.c_int
+    L.sgr_reset_opacity.argtypes = [C.POINTER(SgrDensifySegment), C.c_int32, vp]
     L.sgr_backward_blend.restype = C.c_int
     L.sgr_backward_blend.argtypes = [C.POINTER(SgrFrame), C.c_int64] + [vp] * 12
     L.sgr_backward_geom.restype = C.c_int

@@ -717,6 +717,106 @@ int sgr_adam_step(const SgrAdamTensor *tensors, int32_t num_tensors, double beta
 	return SGR_OK;
 }
 
+// ---- densification ----
+static const char *const kDensifyTensor[SGR_DENSIFY_TENSORS] = {"xyz", "features_dc", "features_rest", "opacity", "scaling", "rotation", "semantic"};
+
+static int densify_width(const SgrDensifySegment &s, int a) {
+	const int fixed[SGR_DENSIFY_TENSORS] = {3, s.dc_width, s.rest_width, 1, 3, 4, s.semantic_width};
+	return fixed[a];
+}
+
+// validates the input table; *P receives the total Gaussian count
+static int check_densify_segments(const SgrDensifySegment *segments, int32_t num_segments, int64_t *P) {
+	if (!segments || num_segments <= 0) return fail(SGR_EINVAL, "segment table is empty");
+	int64_t at = 0;
+	for (int k = 0; k < num_segments; k++) {
+		const SgrDensifySegment &s = segments[k];
+		if (s.kind != SGR_DENSIFY_BACKGROUND && s.kind != SGR_DENSIFY_ACTOR) return fail(SGR_EINVAL, "segment %d: unknown kind %d", k, s.kind);
+		if (s.count < 0) return fail(SGR_EINVAL, "segment %d: count %d", k, s.count);
+		if (s.dc_width <= 0 || s.rest_width < 0 || s.semantic_width < 0)
+			return fail(SGR_EINVAL, "segment %d: bad row widths dc=%d rest=%d semantic=%d", k, s.dc_width, s.rest_width, s.semantic_width);
+		if (s.grad_col != 0 && s.grad_col != 1) return fail(SGR_EINVAL, "segment %d: grad_col must be 0 or 1, got %d", k, s.grad_col);
+		if (s.count > 0) {
+			for (int a = 0; a < SGR_DENSIFY_TENSORS; a++) {
+				const bool has = densify_width(s, a) > 0;
+				if (has != (s.param[a] != nullptr))
+					return fail(SGR_EINVAL, "segment %d: %s is %s", k, kDensifyTensor[a], has ? "NULL" : "given for a zero row width");
+				if ((s.exp_avg[a] == nullptr) != (s.exp_avg_sq[a] == nullptr) || (!has && s.exp_avg[a]))
+					return fail(SGR_EINVAL, "segment %d: %s needs both Adam moments or neither", k, kDensifyTensor[a]);
+			}
+			if (!s.max_radii2D || !s.xyz_gradient_accum || !s.denom) return fail(SGR_EINVAL, "segment %d has a NULL statistics array", k);
+		}
+		at += s.count;
+	}
+	if (at >= 0x7fffffffLL) return fail(SGR_EUNSUPPORTED, "%lld Gaussians in all exceed 2^31-2", (long long)at);
+	*P = at;
+	return SGR_OK;
+}
+
+size_t sgr_densify_scratch_bytes(int32_t num_segments, int64_t P) {
+	return num_segments > 0 && P >= 0 ? densify_scratch_bytes(num_segments, (long long)P) : 0;
+}
+
+int sgr_densify_plan(const SgrDensifySegment *segments, int32_t num_segments, uint64_t seed, const float *draws, void *scratch,
+                     size_t scratch_bytes, int64_t *result, void *stream) {
+	int64_t P = 0;
+	const int rc = check_densify_segments(segments, num_segments, &P);
+	if (rc != SGR_OK) return rc;
+	if (!result) return fail(SGR_EINVAL, "result is NULL");
+	const size_t need = densify_scratch_bytes(num_segments, (long long)P);
+	if (!scratch || scratch_bytes < need) return fail(SGR_ENOMEM, "densify scratch too small: %zu < %zu", scratch_bytes, need);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_densify_plan(segments, num_segments, (unsigned long long)seed, draws, scratch, reinterpret_cast<long long *>(result), st),
+	        "densify_plan");
+	return SGR_OK;
+}
+
+int sgr_densify_apply(const SgrDensifySegment *segments, const SgrDensifyOutput *outputs, int32_t num_segments, uint64_t seed,
+                      const float *draws, void *scratch, size_t scratch_bytes, void *stream) {
+	int64_t P = 0;
+	const int rc = check_densify_segments(segments, num_segments, &P);
+	if (rc != SGR_OK) return rc;
+	if (!outputs) return fail(SGR_EINVAL, "output table is NULL");
+	for (int k = 0; k < num_segments; k++) {
+		const SgrDensifySegment &s = segments[k];
+		const SgrDensifyOutput &o = outputs[k];
+		if (o.count < 0) return fail(SGR_EINVAL, "output %d: count %d", k, o.count);
+		if (o.count == 0) continue;
+		for (int a = 0; a < SGR_DENSIFY_TENSORS; a++) {
+			const bool has = densify_width(s, a) > 0;
+			if (has != (o.param[a] != nullptr)) return fail(SGR_EINVAL, "output %d: %s is %s", k, kDensifyTensor[a], has ? "NULL" : "given for a zero row width");
+			const bool moments = s.count > 0 && s.exp_avg[a] != nullptr;
+			if (moments != (o.exp_avg[a] != nullptr) || moments != (o.exp_avg_sq[a] != nullptr))
+				return fail(SGR_EINVAL, "output %d: the Adam moments of %s must be given exactly where the input has them", k, kDensifyTensor[a]);
+		}
+		if (!o.max_radii2D || !o.xyz_gradient_accum || !o.denom) return fail(SGR_EINVAL, "output %d has a NULL statistics array", k);
+	}
+	const size_t need = densify_scratch_bytes(num_segments, (long long)P);
+	if (!scratch || scratch_bytes < need) return fail(SGR_ENOMEM, "densify scratch too small: %zu < %zu", scratch_bytes, need);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_densify_apply(segments, outputs, num_segments, (unsigned long long)seed, draws, scratch, st), "densify_apply");
+	return SGR_OK;
+}
+
+int sgr_reset_opacity(const SgrDensifySegment *segments, int32_t num_segments, void *stream) {
+	if (!segments || num_segments <= 0) return fail(SGR_EINVAL, "segment table is empty");
+	int64_t at = 0;
+	for (int k = 0; k < num_segments; k++) {
+		const SgrDensifySegment &s = segments[k];
+		if (s.count < 0) return fail(SGR_EINVAL, "segment %d: count %d", k, s.count);
+		if (s.count > 0 && !s.param[3]) return fail(SGR_EINVAL, "segment %d: opacity is NULL", k);
+		if ((s.exp_avg[3] == nullptr) != (s.exp_avg_sq[3] == nullptr)) return fail(SGR_EINVAL, "segment %d: opacity needs both Adam moments or neither", k);
+		at += s.count;
+	}
+	if (at >= 0x7fffffffLL) return fail(SGR_EUNSUPPORTED, "%lld Gaussians in all exceed 2^31-2", (long long)at);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_reset_opacity(segments, num_segments, st), "reset_opacity");
+	return SGR_OK;
+}
+
 size_t sgr_knn_scratch_bytes(int32_t P) { return knn_scratch_bytes(P); }
 
 int sgr_knn_mean_dist2(int32_t P, const float *points, float *mean_dist2, void *scratch, size_t scratch_bytes, void *stream) {

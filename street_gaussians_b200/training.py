@@ -8,11 +8,18 @@
         torch.optim.Adam's interface (param_groups with per-group "lr" / "name", .step(), .zero_grad(), state_dict) for the way the
         reference uses it (gaussian_model.py:300-303: lr per group, eps=1e-15, no weight decay / amsgrad); ONE kernel updates every
         tensor of every group — pass the groups of all sub-models to a single FusedAdam to get a single launch per iteration.
+    densify_and_prune(models, max_grad, min_opacity, prune_big_points, optimizer=None, *, grad_abs=False, seed=None, noise=None)
+        = StreetGaussianModel.densify_and_prune (lib/models/street_gaussian_model.py:573-586) over GaussianModelBkgd /
+        GaussianModelActor.densify_and_prune: clone, split and prune every sub-model in two kernels around ONE host read-back of the
+        new sizes, resizing the parameters together with their Adam moments.  Works with one shared FusedAdam over all sub-models.
+    reset_opacity(models, optimizer=None)
+        = StreetGaussianModel.reset_opacity (:597-602 -> lib/models/gaussian_model.py:410-414), in place, one kernel.
 CUDA tensors only; there is no CPU fallback.
 """
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import Iterable, Sequence
 
 import torch
@@ -95,3 +102,254 @@ class FusedAdam(torch.optim.Optimizer):
             _capi.check(rc, "sgr_adam_step")
             del keep
         return loss
+
+
+# ---- densification ----
+PARAM_NAMES = ("_xyz", "_features_dc", "_features_rest", "_opacity", "_scaling", "_rotation", "_semantic")
+SCALAR_NAMES = ("points_total", "points_clone", "points_split", "points_below_min_opacity", "points_big_ws", "points_pruned")
+
+
+def _has(model, name):
+    return name in model if isinstance(model, dict) else hasattr(model, name)
+
+
+def _set(model, name, value):
+    if isinstance(model, dict):
+        model[name] = value
+    else:
+        setattr(model, name, value)
+
+
+def _per_model(v, n, what):
+    if isinstance(v, (list, tuple)):
+        if len(v) != n:
+            raise ValueError(f"{what}: {len(v)} values for {n} models")
+        return list(v)
+    return [v] * n
+
+
+def _f32(v) -> float:
+    return float(torch.as_tensor(v, dtype=torch.float32).reshape(-1)[0])
+
+
+def _times(t, f: float) -> float:
+    """fp32 tensor x Python float, formed the way torch forms the reference's thresholds (percent_dense * extent, ...)."""
+    return float((torch.as_tensor(t, dtype=torch.float32).detach().cpu().reshape(-1)[:1] * f)[0])
+
+
+def _param_slots(optimizer):
+    """id(param) -> (group, position): groups are matched by parameter identity, never by group['name'], so one optimizer over
+    all sub-models (whose groups repeat the names "xyz", "f_dc", ...) works as well as one per sub-model."""
+    slots = {}
+    opts = [] if optimizer is None else list(optimizer) if isinstance(optimizer, (list, tuple)) else [optimizer]
+    for opt in opts:
+        for g in opt.param_groups:
+            for j, p in enumerate(g["params"]):
+                slots[id(p)] = (opt, g, j)
+    return slots
+
+
+def _moments(optimizer, slots, p):
+    if id(p) not in slots:
+        return None
+    st = slots[id(p)][0].state.get(p, None)
+    if not st or "exp_avg" not in st:
+        return None
+    return st["exp_avg"], st["exp_avg_sq"]
+
+
+def _check_tensor(t, dev, what):
+    if not t.is_cuda or t.device != dev:
+        raise _capi.SgrError(f"{what} must be a CUDA tensor on {dev} (there is no CPU fallback)")
+    if t.dtype != torch.float32 or not t.is_contiguous():
+        raise _capi.SgrError(f"{what} must be a contiguous fp32 tensor")
+
+
+def _segment(model, k, optimizer, slots, dev):
+    seg = _capi.SgrDensifySegment()
+    params = [_attr(model, n) for n in PARAM_NAMES]
+    n = int(params[0].shape[0])
+    seg.count = n
+    widths = [int(math.prod(p.shape[1:])) for p in params]
+    seg.dc_width, seg.rest_width, seg.semantic_width = widths[1], widths[2], widths[6]
+    moments = []
+    for a, p in enumerate(params):
+        _check_tensor(p, dev, f"model {k}: {PARAM_NAMES[a]}")
+        if p.shape[0] != n:
+            raise ValueError(f"model {k}: {PARAM_NAMES[a]} has {p.shape[0]} rows, _xyz {n}")
+        mv = _moments(optimizer, slots, p)
+        if mv is not None:
+            for t in mv:
+                _check_tensor(t, dev, f"model {k}: Adam state of {PARAM_NAMES[a]}")
+                if t.shape != p.shape:
+                    raise ValueError(f"model {k}: Adam state of {PARAM_NAMES[a]} has shape {tuple(t.shape)}, the parameter {tuple(p.shape)}")
+        moments.append(mv)
+        if n and widths[a]:
+            seg.param[a] = p.data_ptr()
+            if mv is not None:
+                seg.exp_avg[a], seg.exp_avg_sq[a] = mv[0].data_ptr(), mv[1].data_ptr()
+    return seg, params, moments, widths
+
+
+def _densify(models, max_grad, min_opacity, prune_big_points, optimizer=None, grad_abs=False, seed=None, noise=None, keep_masks=False):
+    L = _capi.lib()
+    models = list(models)
+    nm = len(models)
+    if nm == 0:
+        return [], None
+    dev = _attr(models[0], "_xyz").device
+    slots = _param_slots(optimizer)
+    max_grads, grad_abss = _per_model(max_grad, nm, "max_grad"), _per_model(grad_abs, nm, "grad_abs")
+    segs = (_capi.SgrDensifySegment * nm)()
+    infos = []
+    for k, m in enumerate(models):
+        seg, params, moments, widths = _segment(m, k, optimizer, slots, dev)
+        n = seg.count
+        stats = [_attr(m, s) for s in ("max_radii2D", "xyz_gradient_accum", "denom")]
+        for t, w in zip(stats, (1, 2, 1)):
+            _check_tensor(t, dev, f"model {k}: densification statistics")
+            if t.numel() != w * n:
+                raise ValueError(f"model {k}: max_radii2D must be [{n}], xyz_gradient_accum [{n}, 2] and denom [{n}, 1]")
+        if n:
+            seg.max_radii2D, seg.xyz_gradient_accum, seg.denom = (t.data_ptr() for t in stats)
+        if _has(m, "scene_radius"):       # GaussianModelBkgd (gaussian_model_bkgd.py:21-23, 86-98)
+            seg.kind, extent = _capi.DENSIFY_BACKGROUND, _attr(m, "scene_radius")
+            c = torch.as_tensor(_attr(m, "sphere_center"), dtype=torch.float32).detach().cpu().reshape(-1)
+            for a in range(3):
+                seg.sphere_center[a] = float(c[a])
+            seg.sphere_diameter = _f32(2 * torch.as_tensor(_attr(m, "sphere_radius"), dtype=torch.float32).detach().cpu().reshape(-1)[:1])
+        elif _has(m, "extent"):           # GaussianModelActor (gaussian_model_actor.py:37-40, 218-247)
+            seg.kind, extent = _capi.DENSIFY_ACTOR, _attr(m, "extent")
+            lo = torch.as_tensor(_attr(m, "min_xyz"), dtype=torch.float32).detach().cpu().reshape(-1)
+            hi = torch.as_tensor(_attr(m, "max_xyz"), dtype=torch.float32).detach().cpu().reshape(-1)
+            for a in range(3):
+                seg.min_xyz[a], seg.max_xyz[a] = float(lo[a]), float(hi[a])
+        else:
+            raise ValueError(f"model {k} has neither scene_radius (background) nor extent (actor)")
+        seg.grad_col = 1 if grad_abss[k] else 0
+        seg.prune_big = 1 if prune_big_points else 0
+        seg.grad_threshold = _f32(max_grads[k])
+        seg.dense_threshold = _times(extent, _attr(m, "percent_dense"))
+        seg.big_threshold = _times(extent, _attr(m, "percent_big_ws"))
+        seg.min_opacity = _f32(min_opacity)
+        segs[k] = seg
+        infos.append((params, moments, widths))
+    P = sum(s.count for s in segs)
+    if noise is not None:
+        if tuple(noise.shape) != (P, _capi.DENSIFY_DRAWS):
+            raise ValueError(f"noise must be [{P}, {_capi.DENSIFY_DRAWS}]")
+        _check_tensor(noise, dev, "noise")
+    if seed is None:
+        seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+    nbytes = L.sgr_densify_scratch_bytes(nm, P)
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    result = (C.c_int64 * (nm * _capi.DENSIFY_RESULT))()
+    npp = _ptr(noise) if noise is not None else None
+    with torch.cuda.device(dev):
+        rc = L.sgr_densify_plan(segs, nm, C.c_uint64(seed), npp, scratch.data_ptr(), nbytes, result, _stream(dev))
+    _capi.check(rc, "sgr_densify_plan")
+    outs = (_capi.SgrDensifyOutput * nm)()
+    new = []
+    for k, (params, moments, widths) in enumerate(infos):
+        n_new = int(result[k * _capi.DENSIFY_RESULT])
+        o = outs[k]
+        o.count = n_new
+        np_, nmom = [], []
+        for a, p in enumerate(params):
+            t = torch.empty((n_new,) + tuple(p.shape[1:]), dtype=torch.float32, device=dev)
+            mv = None if moments[a] is None else (torch.empty_like(t), torch.empty_like(t))
+            if n_new and widths[a]:
+                o.param[a] = t.data_ptr()
+                if mv is not None and segs[k].count:
+                    o.exp_avg[a], o.exp_avg_sq[a] = mv[0].data_ptr(), mv[1].data_ptr()
+            if mv is not None and segs[k].count == 0:
+                mv = (torch.zeros_like(t), torch.zeros_like(t))
+            np_.append(t)
+            nmom.append(mv)
+        stats = (torch.empty(n_new, device=dev), torch.empty(n_new, 2, device=dev), torch.empty(n_new, 1, device=dev))
+        if n_new:
+            o.max_radii2D, o.xyz_gradient_accum, o.denom = (t.data_ptr() for t in stats)
+        new.append((np_, nmom, stats))
+    with torch.cuda.device(dev):
+        rc = L.sgr_densify_apply(segs, outs, nm, C.c_uint64(seed), npp, scratch.data_ptr(), nbytes, _stream(dev))
+    _capi.check(rc, "sgr_densify_apply")
+    scalars = []
+    for k, m in enumerate(models):
+        params, moments, _ = infos[k]
+        np_, nmom, stats = new[k]
+        for a, (old, t) in enumerate(zip(params, np_)):
+            p = torch.nn.Parameter(t, requires_grad=old.requires_grad)
+            if id(old) in slots:
+                opt, g, j = slots[id(old)]
+                g["params"][j] = p
+                st = opt.state.pop(old, None)
+                if st is not None:
+                    if nmom[a] is not None:
+                        st["exp_avg"], st["exp_avg_sq"] = nmom[a]
+                    opt.state[p] = st
+            _set(m, PARAM_NAMES[a], p)
+        for name, t in zip(("max_radii2D", "xyz_gradient_accum", "denom"), stats):
+            _set(m, name, t)
+        r = result[k * _capi.DENSIFY_RESULT:(k + 1) * _capi.DENSIFY_RESULT]
+        d = dict(zip(SCALAR_NAMES, (int(v) for v in r[1:7])))
+        if not prune_big_points:
+            d.pop("points_big_ws")
+        scalars.append(d)
+    masks = None
+    if keep_masks:  # the plan's per-parent 4-bit section masks (for tests): in the scratch, after the two tables and two start arrays
+        al = lambda b: (b + 255) // 256 * 256
+        off = al(C.sizeof(_capi.SgrDensifySegment) * nm) + al(C.sizeof(_capi.SgrDensifyOutput) * nm) + 2 * al(4 * (nm + 1))
+        masks = scratch[off:off + P].clone()
+    return scalars, masks
+
+
+def densify_and_prune(models: Sequence, max_grad, min_opacity: float, prune_big_points: bool, optimizer=None, *, grad_abs=False,
+                      seed=None, noise=None) -> list:
+    """Clone, split and prune every sub-model (background and actors, in composition order) in one pass, as
+    GaussianModelBkgd.densify_and_prune (lib/models/gaussian_model_bkgd.py:74-114) and GaussianModelActor.densify_and_prune
+    (lib/models/gaussian_model_actor.py:204-261) do one model at a time.
+
+    models: objects or mappings with the reference's attributes: the parameters _xyz, _features_dc, _features_rest, _opacity,
+      _scaling, _rotation, _semantic; the statistics max_radii2D, xyz_gradient_accum, denom; percent_dense and percent_big_ws; and
+      either scene_radius, sphere_center, sphere_radius (a background) or extent, min_xyz, max_xyz (an actor).
+    max_grad, grad_abs: one value, or one per model.  The reference reads them from the config per kind
+      (cfg.optim.densify_grad_threshold_bkgd / _obj and densify_grad_abs_bkgd / _obj); grad_abs selects column 1 of
+      xyz_gradient_accum.  An actor with random_initialization or deformable uses the caller's max_grad with grad_abs=False.
+    optimizer: one optimizer (e.g. a FusedAdam over all models) or a list of them (e.g. the reference's torch.optim.Adam per model).  Each parameter's group is found by identity, the
+      parameter is replaced by a new nn.Parameter in that group, and its state (step unchanged) moves to the new key with the
+      moments of surviving rows carried and zero moments for clones and children.
+    seed: key of the Philox normal draws (None: drawn from torch's default generator).  noise: [P, 18] draws per parent instead
+      (a test seam; see include/sgr.h).
+
+    Returns one dict per model with points_total, points_clone, points_split, points_below_min_opacity, points_big_ws (with
+    prune_big_points) and points_pruned.  The only host synchronisation is one read-back of the new sizes.  Unlike the reference it
+    does not call torch.cuda.empty_cache(): the freed blocks stay in PyTorch's cache for the next iterations.  The number of
+    Gaussians changes, so a CUDA graph that captured a training step must be captured again after this call."""
+    return _densify(models, max_grad, min_opacity, prune_big_points, optimizer, grad_abs, seed, noise)[0]
+
+
+def reset_opacity(models: Sequence, optimizer=None) -> None:
+    """GaussianModel.reset_opacity (lib/models/gaussian_model.py:410-414) for every model in one kernel:
+    _opacity = inverse_sigmoid(min(sigmoid(_opacity), 0.01)) and the opacity's Adam moments zeroed, in place (the parameter
+    objects stay the same, so the optimizer needs no update)."""
+    L = _capi.lib()
+    models = list(models)
+    if not models:
+        return
+    slots = _param_slots(optimizer)
+    segs = (_capi.SgrDensifySegment * len(models))()
+    dev = _attr(models[0], "_opacity").device
+    for k, m in enumerate(models):
+        op = _attr(m, "_opacity")
+        _check_tensor(op, dev, f"model {k}: _opacity")
+        segs[k].count = int(op.numel())
+        if op.numel():
+            segs[k].param[3] = op.data_ptr()
+            mv = _moments(optimizer, slots, op)
+            if mv is not None:
+                for t in mv:
+                    _check_tensor(t, dev, f"model {k}: Adam state of _opacity")
+                segs[k].exp_avg[3], segs[k].exp_avg_sq[3] = mv[0].data_ptr(), mv[1].data_ptr()
+    with torch.cuda.device(dev):
+        rc = L.sgr_reset_opacity(segs, len(models), _stream(dev))
+    _capi.check(rc, "sgr_reset_opacity")
