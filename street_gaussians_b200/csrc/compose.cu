@@ -16,6 +16,7 @@
 namespace sgr {
 
 constexpr int kMaxSeg = SGR_MAX_SEGMENTS_PER_LAUNCH;
+static_assert(kMaxSeg <= 32, "compose_pose_finalize_kernel takes the posed flags of a group as one 32-bit mask");
 
 struct SegDev {
 	const float *xyz, *rotation, *scaling, *opacity, *fdc, *frest;
@@ -288,12 +289,19 @@ __global__ void __launch_bounds__(256) compose_bwd_kernel(const SegTable t, cons
 	}
 }
 
-// acc[16] -> d pose (4 + 3, padded to 8): the matrix path goes through quaternion_to_matrix's normalisation
-__global__ void compose_pose_finalize_kernel(const int n, const float *__restrict__ poses, const float *__restrict__ acc,
-                                             float *__restrict__ dposes) {
-	const int s = blockIdx.x * blockDim.x + threadIdx.x;
-	if (s >= n) return;
-	const float *a = acc + (size_t)s * 16, *ps = poses + (size_t)s * 8;
+// acc[16] -> d pose (4 + 3, padded to 8): the matrix path goes through quaternion_to_matrix's normalisation.  One warp per group of
+// kMaxSeg segments; bit k of `posed` is segment first + k.  Rows of unposed segments are written as zeros: their pose row is not
+// read by the other kernels and may hold anything, a zero quaternion included (composer.py leaves the background's row zero).
+__global__ void compose_pose_finalize_kernel(const int first, const int n, const unsigned posed, const float *__restrict__ poses,
+                                             const float *__restrict__ acc, float *__restrict__ dposes) {
+	if ((int)threadIdx.x >= n) return;
+	const size_t s = (size_t)first + threadIdx.x;
+	float *o = dposes + s * 8;
+	if (!((posed >> threadIdx.x) & 1u)) {
+		for (int k = 0; k < 8; k++) o[k] = 0.f;
+		return;
+	}
+	const float *a = acc + s * 16, *ps = poses + s * 8;
 	const float nr = sqrtf(ps[0] * ps[0] + ps[1] * ps[1] + ps[2] * ps[2] + ps[3] * ps[3]);
 	const float w = ps[0] / nr, x = ps[1] / nr, y = ps[2] / nr, z = ps[3] / nr;
 	const float G00 = a[0], G01 = a[1], G02 = a[2], G10 = a[3], G11 = a[4], G12 = a[5], G20 = a[6], G21 = a[7], G22 = a[8];
@@ -302,7 +310,6 @@ __global__ void compose_pose_finalize_kernel(const int n, const float *__restric
 	const float dy = 2.f * (-2.f * y * G00 + x * G01 + w * G02 + x * G10 + z * G12 - w * G20 + z * G21 - 2.f * y * G22);
 	const float dz = 2.f * (-2.f * z * G00 - w * G01 + x * G02 + w * G10 - 2.f * z * G11 + y * G12 + x * G20 + y * G21);
 	const float dot = w * dw + x * dx + y * dy + z * dz;
-	float *o = dposes + (size_t)s * 8;
 	o[0] = a[9] + (dw - w * dot) / nr; o[1] = a[10] + (dx - x * dot) / nr; o[2] = a[11] + (dy - y * dot) / nr; o[3] = a[12] + (dz - z * dot) / nr;
 	o[4] = a[13]; o[5] = a[14]; o[6] = a[15]; o[7] = 0.f;
 }
@@ -352,8 +359,13 @@ cudaError_t launch_compose_bwd(const SgrSegment *segs, const SgrSegmentGrads *gr
 		count_launch();
 		compose_bwd_kernel<<<(count + 255) / 256, 256, 0, st>>>(t, gt, M, poses, idft, flip, flip_quat, g_xyz, g_rot, g_scale, g_opac, g_sh, acc);
 	}
-	count_launch();
-	compose_pose_finalize_kernel<<<(nseg + 63) / 64, 64, 0, st>>>(nseg, poses, acc, dposes);
+	for (int first = 0; first < nseg; first += kMaxSeg) {
+		const int n = nseg - first < kMaxSeg ? nseg - first : kMaxSeg;
+		unsigned posed = 0;
+		for (int k = 0; k < n; k++) posed |= (segs[first + k].posed ? 1u : 0u) << k;
+		count_launch();
+		compose_pose_finalize_kernel<<<1, kMaxSeg, 0, st>>>(first, n, posed, poses, acc, dposes);
+	}
 	return cudaGetLastError();
 }
 

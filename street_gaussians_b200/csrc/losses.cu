@@ -21,15 +21,18 @@ constexpr int kWin = 11, kHalo = 5, kTileL = 16, kExt = kTileL + 2 * kHalo;  // 
 struct GaussWin {
 	float w[kWin];
 };
-// loss_utils.py:84-86: exp(-(x - 5)^2 / (2 * 1.5^2)) normalised (float32, like torch.Tensor([...]) / sum)
+// loss_utils.py:84-86: exp(-(x - 5)^2 / (2 * 1.5^2)) normalised (float32, like torch.Tensor([...]) / sum).  The sum is the fp32
+// rounding of the exact sum, as torch's sum gives for these 11 values; a sequential fp32 sum is one ulp low and would move 9 of the
+// 11 weights by one ulp.
 static GaussWin make_window() {
 	GaussWin g;
-	float s = 0.f;
+	double s = 0.0;
 	for (int k = 0; k < kWin; k++) {
 		g.w[k] = (float)exp(-(double)((k - kWin / 2) * (k - kWin / 2)) / (2.0 * 1.5 * 1.5));
-		s += g.w[k];
+		s += (double)g.w[k];
 	}
-	for (int k = 0; k < kWin; k++) g.w[k] /= s;
+	const float sf = (float)s;
+	for (int k = 0; k < kWin; k++) g.w[k] /= sf;
 	return g;
 }
 
@@ -129,7 +132,8 @@ __global__ void __launch_bounds__(256) ssim_grad_kernel(const int C, const int H
 	if (blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 0 && scalars != nullptr) {
 		const double l1 = n_l1 > 0.0 ? acc[1] / n_l1 : 0.0 / 0.0;  // (an empty mask is a NaN mean in the reference as well)
 		const double ss = acc[0] / n_el;
-		scalars[0] = (float)((double)w_l1 * l1 + (double)w_ssim * ss);
+		// a term with weight 0 is absent, not 0 * NaN: ssim() under an empty mask is 1, as in the reference
+		scalars[0] = (float)((w_l1 != 0.f ? (double)w_l1 * l1 : 0.0) + (double)w_ssim * ss);
 		scalars[1] = (float)l1;
 		scalars[2] = (float)ss;
 		scalars[3] = (float)acc[2];
