@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define SGR_ABI_VERSION 6
+#define SGR_ABI_VERSION 7
 
 #define SGR_OK 0
 #define SGR_EINVAL (-1)   /* bad argument combination / shape                     */
@@ -414,6 +414,32 @@ int sgr_densify_apply(const SgrDensifySegment *segments, const SgrDensifyOutput 
 /* GaussianModel.reset_opacity (lib/models/gaussian_model.py:410-414) in place: _opacity = inverse_sigmoid(min(sigmoid(_opacity), 0.01))
  * and the opacity tensor's exp_avg / exp_avg_sq (when non-NULL) zeroed.  Reads count, param[3], exp_avg[3], exp_avg_sq[3] only. */
 int sgr_reset_opacity(const SgrDensifySegment *segments, int32_t num_segments, void *stream);
+
+/* ---- Visibility-masked ("sparse") Adam: an OPT-IN deviation from the reference (no counterpart there) ----
+ * One Adam step that updates only the rows of the Gaussians this frame rendered.  Segments are the sub-models in composition order
+ * (ascending, gap-free, as for sgr_densify_stats); row l of segment k is VISIBLE iff radii[start_k + l] > 0 (the reference's
+ * visibility_filter, street_gaussian_renderer.py:274).  For each tensor a with width[a] > 0:
+ *   visible rows:   exactly sgr_adam_step's update (same arithmetic, same rounding: bit-equal), with that tensor's lr and step;
+ *   invisible rows: param, exp_avg and exp_avg_sq are not written and grad is not read.
+ * `step` is the tensor's 1-based step count after this update, as for sgr_adam_step; there are no per-row step counts.  A tensor with
+ * width 0 is not touched (pointers may be NULL); widths above SGR_SPARSE_ADAM_MAX_WIDTH return SGR_EUNSUPPORTED.  Traffic: 4 B per row of radii + 28 B per element of a visible row, rounded up to
+ * 32-B sectors; a 256-row tile with no visible row costs only its radii.  No host synchronisation.
+ * segments: HOST array; every pointer device, fp32, rows of `width` floats; radii[sum of counts] int32 device.
+ * betas / eps are doubles for the same reason as in sgr_adam_step. */
+#define SGR_SPARSE_ADAM_MAX_WIDTH 8388607   /* 2^23 - 1 floats per row: a 256-row tile spans fewer than 2^31 floats */
+typedef struct SgrSparseAdamSegment {
+	int32_t start, count;                       /* range in the composed index space                      */
+	float *param[SGR_DENSIFY_TENSORS];          /* _xyz, _features_dc, _features_rest, _opacity, _scaling, _rotation, _semantic */
+	const float *grad[SGR_DENSIFY_TENSORS];
+	float *exp_avg[SGR_DENSIFY_TENSORS];
+	float *exp_avg_sq[SGR_DENSIFY_TENSORS];
+	int32_t width[SGR_DENSIFY_TENSORS];         /* floats per row; 0 = not updated by this call           */
+	float lr[SGR_DENSIFY_TENSORS];
+	int32_t step[SGR_DENSIFY_TENSORS];
+	int32_t reserved;
+} SgrSparseAdamSegment;
+int sgr_sparse_adam_step(const SgrSparseAdamSegment *segments, int32_t num_segments, const int32_t *radii, double beta1, double beta2,
+                         double eps, void *stream);
 
 /* present[P] (uint8 0/1) = view-space z > 0.2.  Replaces markVisible -> checkFrustum
  * (DGR/rasterize_points.cu:222-241, rasterizer_impl.cu:54-66, 141-153; pybind `mark_visible`, DGR/ext.cpp:18). */

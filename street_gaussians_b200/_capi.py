@@ -8,7 +8,7 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libsgr.so")
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_state_sizes", "sgr_binning_bytes", "sgr_forward", "sgr_forward_bounded",
            "sgr_forward_status", "sgr_forward_status_async", "sgr_backward_blend",
@@ -17,7 +17,7 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_state_s
            "sgr_scatter_records", "sgr_gather_grad2d", "sgr_peer_barrier", "sgr_sharded_forward", "sgr_sharded_backward",
            "sgr_compose_forward", "sgr_compose_backward", "sgr_image_loss_scratch_bytes", "sgr_image_loss", "sgr_sky_loss",
            "sgr_obj_acc_loss", "sgr_lidar_depth_loss_scratch_bytes", "sgr_lidar_depth_loss", "sgr_densify_stats", "sgr_adam_step",
-           "sgr_densify_scratch_bytes", "sgr_densify_plan", "sgr_densify_apply", "sgr_reset_opacity"]
+           "sgr_densify_scratch_bytes", "sgr_densify_plan", "sgr_densify_apply", "sgr_reset_opacity", "sgr_sparse_adam_step"]
 
 
 class SgrFrame(C.Structure):
@@ -76,6 +76,15 @@ class SgrDensifySegment(C.Structure):
 class SgrDensifyOutput(C.Structure):
     _fields_ = [("count", C.c_int32), ("reserved", C.c_int32), ("param", C.c_void_p * DENSIFY_TENSORS), ("exp_avg", C.c_void_p * DENSIFY_TENSORS),
                 ("exp_avg_sq", C.c_void_p * DENSIFY_TENSORS), ("max_radii2D", C.c_void_p), ("xyz_gradient_accum", C.c_void_p), ("denom", C.c_void_p)]
+
+
+SPARSE_ADAM_MAX_WIDTH = 8388607   # floats per row
+
+
+class SgrSparseAdamSegment(C.Structure):
+    _fields_ = [("start", C.c_int32), ("count", C.c_int32), ("param", C.c_void_p * DENSIFY_TENSORS), ("grad", C.c_void_p * DENSIFY_TENSORS),
+                ("exp_avg", C.c_void_p * DENSIFY_TENSORS), ("exp_avg_sq", C.c_void_p * DENSIFY_TENSORS), ("width", C.c_int32 * DENSIFY_TENSORS),
+                ("lr", C.c_float * DENSIFY_TENSORS), ("step", C.c_int32 * DENSIFY_TENSORS), ("reserved", C.c_int32)]
 
 
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
@@ -167,6 +176,8 @@ def lib():
     L.sgr_densify_apply.argtypes = [C.POINTER(SgrDensifySegment), C.POINTER(SgrDensifyOutput), C.c_int32, C.c_uint64, vp, vp, C.c_size_t, vp]
     L.sgr_reset_opacity.restype = C.c_int
     L.sgr_reset_opacity.argtypes = [C.POINTER(SgrDensifySegment), C.c_int32, vp]
+    L.sgr_sparse_adam_step.restype = C.c_int
+    L.sgr_sparse_adam_step.argtypes = [C.POINTER(SgrSparseAdamSegment), C.c_int32, vp, C.c_double, C.c_double, C.c_double, vp]
     L.sgr_backward_blend.restype = C.c_int
     L.sgr_backward_blend.argtypes = [C.POINTER(SgrFrame), C.c_int64] + [vp] * 12
     L.sgr_backward_geom.restype = C.c_int

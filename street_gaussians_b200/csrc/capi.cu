@@ -1,5 +1,6 @@
 // capi.cu — the extern "C" surface of libsgr.so (include/sgr.h): argument validation, state carving, launch order.
 // Host-side only; every device kernel lives in its own translation unit.
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -814,6 +815,37 @@ int sgr_reset_opacity(const SgrDensifySegment *segments, int32_t num_segments, v
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 	const bool debug = false;
 	SGR_TRY(launch_reset_opacity(segments, num_segments, st), "reset_opacity");
+	return SGR_OK;
+}
+
+int sgr_sparse_adam_step(const SgrSparseAdamSegment *segments, int32_t num_segments, const int32_t *radii, double beta1, double beta2,
+                         double eps, void *stream) {
+	if (!segments || num_segments <= 0) return fail(SGR_EINVAL, "segment table is empty");
+	int64_t at = 0;
+	for (int k = 0; k < num_segments; k++) {
+		const SgrSparseAdamSegment &s = segments[k];
+		if (s.start != at || s.count < 0) return fail(SGR_EINVAL, "segment %d: start %d (expected %lld), count %d", k, s.start, (long long)at, s.count);
+		for (int a = 0; a < SGR_DENSIFY_TENSORS; a++) {
+			const int w = s.width[a];
+			if (w < 0) return fail(SGR_EINVAL, "segment %d: %s has width %d", k, kDensifyTensor[a], w);
+			// the kernel indexes a 256-row tile's span [0, 256 w) with int
+			if (w > SGR_SPARSE_ADAM_MAX_WIDTH)
+				return fail(SGR_EUNSUPPORTED, "segment %d: %s has width %d > %d floats per row", k, kDensifyTensor[a], w, SGR_SPARSE_ADAM_MAX_WIDTH);
+			if (w == 0) continue;
+			if (s.count > 0 && (!s.param[a] || !s.grad[a] || !s.exp_avg[a] || !s.exp_avg_sq[a]))
+				return fail(SGR_EINVAL, "segment %d: %s has a NULL pointer", k, kDensifyTensor[a]);
+			if (s.step[a] < 1) return fail(SGR_EINVAL, "segment %d: %s has step %d (step counts from 1)", k, kDensifyTensor[a], s.step[a]);
+			if (!std::isfinite(s.lr[a])) return fail(SGR_EINVAL, "segment %d: %s has a non-finite lr", k, kDensifyTensor[a]);
+		}
+		at += s.count;
+	}
+	if (at >= 0x7fffffffLL) return fail(SGR_EUNSUPPORTED, "%lld Gaussians in all exceed 2^31-2", (long long)at);
+	if (!(beta1 >= 0.0 && beta1 < 1.0) || !(beta2 >= 0.0 && beta2 < 1.0)) return fail(SGR_EINVAL, "betas must lie in [0, 1)");
+	if (at == 0) return SGR_OK;
+	if (!radii) return fail(SGR_EINVAL, "radii is NULL");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_sparse_adam(segments, num_segments, radii, beta1, beta2, eps, st), "sparse_adam");
 	return SGR_OK;
 }
 

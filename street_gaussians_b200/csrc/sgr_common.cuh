@@ -359,6 +359,8 @@ cudaError_t launch_lidar_depth_loss(size_t N, const float *depth, const float *a
                                     float *dL_ddepth, float *dL_dacc, float *scalars, void *scratch, cudaStream_t st);
 cudaError_t launch_densify_stats(const SgrStatSegment *segs, int nseg, const int32_t *radii, const float *grad2d, cudaStream_t st);
 cudaError_t launch_adam(const SgrAdamTensor *ts, int n_tensors, double beta1, double beta2, double eps, cudaStream_t st);
+cudaError_t launch_sparse_adam(const SgrSparseAdamSegment *segs, int nseg, const int32_t *radii, double beta1, double beta2, double eps,
+                               cudaStream_t st);
 size_t densify_scratch_bytes(int nseg, long long P);
 cudaError_t launch_densify_plan(const SgrDensifySegment *segs, int nseg, unsigned long long seed, const float *draws, void *scratch,
                                 long long *result_host, cudaStream_t st);

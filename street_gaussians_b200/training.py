@@ -14,6 +14,9 @@
         new sizes, resizing the parameters together with their Adam moments.  Works with one shared FusedAdam over all sub-models.
     reset_opacity(models, optimizer=None)
         = StreetGaussianModel.reset_opacity (:597-602 -> lib/models/gaussian_model.py:410-414), in place, one kernel.
+    SparseAdam(param_groups, ...).step(models, radii)
+        opt-in visibility-masked Adam (no reference counterpart; it deviates from the reference): FusedAdam's update on the rows
+        with radii > 0 only, every other row's parameter and moments left untouched.
 CUDA tensors only; there is no CPU fallback.
 """
 from __future__ import annotations
@@ -62,6 +65,16 @@ def add_densification_stats(models: Sequence, radii: torch.Tensor, viewspace_poi
     _capi.check(rc, "sgr_densify_stats")
 
 
+def _advance_state(st, p):
+    """torch.optim.Adam's per-parameter state {step, exp_avg, exp_avg_sq}, created at zero on first use, with step incremented."""
+    if len(st) == 0:
+        st["step"] = 0
+        st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+        st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+    st["step"] = int(st["step"]) + 1
+    return st
+
+
 class FusedAdam(torch.optim.Optimizer):
     """torch.optim.Adam(params, lr, betas=(0.9, 0.999), eps) semantics, every parameter of every group updated by one kernel."""
 
@@ -86,12 +99,7 @@ class FusedAdam(torch.optim.Optimizer):
             tab = (_capi.SgrAdamTensor * len(items))()
             keep = []
             for k, (p, group) in enumerate(items):
-                st = self.state[p]
-                if len(st) == 0:
-                    st["step"] = 0
-                    st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
-                    st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
-                st["step"] = int(st["step"]) + 1
+                st = _advance_state(self.state[p], p)
                 g = p.grad if (p.grad.dtype == torch.float32 and p.grad.is_contiguous()) else p.grad.to(torch.float32).contiguous()
                 keep.append(g)
                 t = tab[k]
@@ -353,3 +361,118 @@ def reset_opacity(models: Sequence, optimizer=None) -> None:
     with torch.cuda.device(dev):
         rc = L.sgr_reset_opacity(segs, len(models), _stream(dev))
     _capi.check(rc, "sgr_reset_opacity")
+
+
+# ---- visibility-masked Adam ----
+class SparseAdam(torch.optim.Optimizer):
+    """Visibility-masked ("sparse") Adam: an OPT-IN alternative to FusedAdam that updates only the rows of the Gaussians the frame
+    rendered.  It changes training results against the reference (whose torch.optim.Adam also moves invisible rows on their decaying
+    momentum), so FusedAdam stays the drop-in; use this one when the optimizer step's cost matters more than matching the reference.
+
+    step(models, radii) — models: the frame's sub-models in composition order (background, then the frame's actors), the same list
+    and radii [sum of rows] int32 (the rasterizer's output) that add_densification_stats gets.  Each model's per-Gaussian tensors are
+    found by identity among _xyz, _features_dc, _features_rest, _opacity, _scaling, _rotation, _semantic.  For every such tensor this
+    optimizer holds and that has a .grad:
+      * row l of model k is visible iff radii[start_k + l] > 0 (the reference's visibility_filter);
+      * visible rows get FusedAdam's update bit for bit, with the tensor's group lr / betas / eps and its step count;
+      * invisible rows keep their parameter, exp_avg and exp_avg_sq, and their gradient is not read;
+      * state["step"] goes up by one, as in FusedAdam: there are no per-row step counts.
+    Rows that receive gradient from anything other than this frame's render (a regulariser, another camera's loss) are still
+    skipped when their radii is 0.  Tensors held by this optimizer that belong to no model passed in this call (actors absent from
+    the frame) keep their bits and their step count.  So do non-per-Gaussian parameters such as actor poses: put those in a
+    FusedAdam.  The state stays {step, exp_avg, exp_avg_sq}, so densify_and_prune, reset_opacity, state_dict and load_state_dict
+    work unchanged, and a state dict moves between FusedAdam and SparseAdam in either direction.  One kernel launch per (betas, eps)
+    bucket; no host synchronisation.  CUDA tensors only."""
+
+    def __init__(self, params, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8):
+        super().__init__(params, dict(lr=lr, betas=betas, eps=eps))
+
+    @torch.no_grad()
+    def step(self, models: Sequence = None, radii: torch.Tensor = None, closure=None):
+        if models is None or radii is None:
+            raise TypeError("SparseAdam.step(models, radii) needs the frame's models and radii; it has no dense fallback "
+                            "(use FusedAdam for a dense update)")
+        loss = closure() if closure is not None else None
+        models = list(models)
+        params, rows = [], []
+        for k, m in enumerate(models):
+            ps = [_attr(m, n) for n in PARAM_NAMES]
+            n = int(ps[0].shape[0])
+            for a, p in enumerate(ps):
+                if p.dim() == 0 or p.shape[0] != n:
+                    raise ValueError(f"model {k}: {PARAM_NAMES[a]} has shape {tuple(p.shape)}, _xyz has {n} rows")
+            params.append(ps)
+            rows.append(n)
+        if radii.dtype != torch.int32 or tuple(radii.shape) != (sum(rows),):
+            raise ValueError(f"radii must be an int32 tensor of shape [{sum(rows)}] for these models, got {radii.dtype} {tuple(radii.shape)}")
+        if not radii.is_cuda:
+            raise _capi.SgrError("SparseAdam needs CUDA tensors (there is no CPU fallback)")
+        dev = radii.device
+        # What sgr_sparse_adam_step would reject is checked here, before any state changes, so that a bad group or tensor cannot
+        # leave other tensors stepped.  Hyper-parameters once per group; the messages are only formatted on failure.
+        hyper = {}  # id(group) -> (lr, (betas, eps))
+        for g in self.param_groups:
+            lr, betas = float(g["lr"]), tuple(float(b) for b in g["betas"])
+            if not math.isfinite(lr):
+                raise ValueError(f"a parameter group has a non-finite lr {lr}")
+            if not all(0.0 <= b < 1.0 for b in betas):
+                raise ValueError(f"a parameter group has betas {betas} outside [0, 1)")
+            hyper[id(g)] = (lr, (betas, float(g["eps"])))
+        group_of = {id(p): g for g in self.param_groups for p in g["params"]}
+        f32 = torch.float32
+        ok = lambda t: t.is_cuda and t.dtype == f32 and t.device == dev and t.is_contiguous()
+        buckets = {}  # (betas, eps) -> [(model, tensor, param, lr, width)]; every tensor is on radii's device
+        for k, ps in enumerate(params):
+            for a, p in enumerate(ps):
+                g = group_of.get(id(p))
+                if g is None or p.grad is None:
+                    continue
+                if not ok(p):
+                    _check_tensor(p, dev, f"model {k}: {PARAM_NAMES[a]}")
+                st = self.state[p]
+                if st:
+                    m, v = st["exp_avg"], st["exp_avg_sq"]
+                    if not (ok(m) and ok(v) and m.shape == p.shape and v.shape == p.shape):
+                        for t in (m, v):
+                            _check_tensor(t, dev, f"model {k}: Adam state of {PARAM_NAMES[a]}")
+                        raise ValueError(f"model {k}: Adam state of {PARAM_NAMES[a]} has shapes {tuple(m.shape)} / {tuple(v.shape)}, "
+                                         f"the parameter {tuple(p.shape)}")
+                w = math.prod(p.shape[1:])
+                if w > _capi.SPARSE_ADAM_MAX_WIDTH:
+                    raise _capi.SgrError(f"model {k}: {PARAM_NAMES[a]} has {w} floats per row, more than {_capi.SPARSE_ADAM_MAX_WIDTH}")
+                lr, key = hyper[id(g)]
+                buckets.setdefault(key, []).append((k, a, p, lr, w))
+        if not buckets:
+            return loss
+        L = _capi.lib()
+        r = radii.contiguous()
+        for (betas, eps), items in buckets.items():
+            # per model: param, grad, exp_avg, exp_avg_sq, width, lr, step of its 7 tensors, written into the ctypes record at once
+            fields = [None] * len(models)
+            keep = []
+            for k, a, p, lr, w in items:
+                st = _advance_state(self.state[p], p)
+                if w == 0:
+                    continue
+                f = fields[k]
+                if f is None:
+                    f = fields[k] = [[None] * 7, [None] * 7, [None] * 7, [None] * 7, [0] * 7, [0.0] * 7, [0] * 7]
+                f[4][a], f[5][a], f[6][a] = w, lr, st["step"]
+                if p.numel():
+                    g = p.grad if (p.grad.dtype == torch.float32 and p.grad.is_contiguous()) else p.grad.to(torch.float32).contiguous()
+                    keep.append(g)
+                    f[0][a], f[1][a], f[2][a], f[3][a] = p.data_ptr(), g.data_ptr(), st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr()
+            segs = (_capi.SgrSparseAdamSegment * len(models))()
+            start = 0
+            for k, n in enumerate(rows):
+                s = segs[k]
+                s.start, s.count = start, n
+                start += n
+                f = fields[k]
+                if f is not None:
+                    s.param[:], s.grad[:], s.exp_avg[:], s.exp_avg_sq[:], s.width[:], s.lr[:], s.step[:] = f
+            with torch.cuda.device(dev):
+                rc = L.sgr_sparse_adam_step(segs, len(models), _ptr(r), float(betas[0]), float(betas[1]), eps, _stream(dev))
+            _capi.check(rc, "sgr_sparse_adam_step")
+            del keep
+        return loss
