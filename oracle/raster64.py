@@ -96,12 +96,15 @@ def _instances(rec, radii, W, H):
 
 # ----------------------------------------------------------------------------------------------- blend
 def blend64(rec, radii, W: int, H: int, bg, semantics=None, upstream: Optional[Dict] = None, alpha_img=None,
-            max_pairs: int = 1 << 21):
+            max_pairs: int = 1 << 21, decisions=None):
     """Blend per-Gaussian records [P, 12] (the GaussRec layout: px, py, conic xx, xy, opacity-free yy ... see below) in fp64.
 
     rec columns: 0 px, 1 py, 2 conic.xx, 3 conic.xy, 4 conic.yy, 5 opacity, 6 (unused), 7 view depth, 8..10 rgb, 11 clamp bits.
     upstream: dict(color [3,H,W], depth [1,H,W], alpha [1,H,W], semantic [S,H,W]) -> also the backward.
     alpha_img: the alpha image the backward reads T_final = 1 - alpha from (backward.cu:468); default: this forward's.
+    decisions: (pix, gid, take) — flat pixel indices, Gaussian indices and bools: those pairs pass (take) or skip the two
+      per-pair tests (power > 0, alpha < 1/255) as given instead of as fp64 decides; a forced pass blends alpha =
+      min(0.99, o exp(min(power, 0))).  Every other pair, and the T < 1e-4 stop, keep fp64's decision.
 
     Error model (units of 2^-24, the fp32 unit roundoff).  For a pair i of pixel p the fp32 code computes
       power with absolute error ~ pm_i = 0.5 (|a| dx^2 + |c| dy^2) + |b dx dy| (the terms it sums), so G and alpha carry a relative
@@ -164,6 +167,11 @@ def blend64(rec, radii, W: int, H: int, bg, semantics=None, upstream: Optional[D
         chunks = []
     lx = torch.arange(256, device=dev) % TILE
     ly = torch.arange(256, device=dev) // TILE
+    dec_key = dec_take = None
+    if decisions is not None:
+        dpix, dgid, dtake = (torch.as_tensor(v, device=dev) for v in decisions)
+        dec_key, o_ = torch.sort(dpix.to(torch.int64) * P + dgid.to(torch.int64))
+        dec_take = dtake.to(torch.bool)[o_]
 
     def evaluate(chunk):
         ci = torch.tensor(chunk, device=dev)
@@ -185,6 +193,11 @@ def blend64(rec, radii, W: int, H: int, bg, semantics=None, upstream: Optional[D
         G = torch.exp(torch.clamp(power, max=0.0))
         alpha = torch.clamp(o * G, max=ALPHA_CAP)
         ok = present[..., None] & inside[:, None, :] & ~(power > 0) & ~(alpha < ALPHA_MIN)
+        if dec_key is not None and len(dec_key):
+            key = (pix[:, None, :] * P + gid[:, :, None]).reshape(-1)
+            pos = torch.searchsorted(dec_key, key).clamp(max=len(dec_key) - 1)
+            hit = (dec_key[pos] == key).reshape(ok.shape) & present[..., None] & inside[:, None, :]
+            ok = torch.where(hit, dec_take[pos].reshape(ok.shape), ok)
         A = torch.where(ok, alpha, torch.zeros_like(alpha))
         Tincl = torch.cumprod(1 - A, 1)
         keep = ok & ~(Tincl < T_STOP)
@@ -327,6 +340,81 @@ def blend64(rec, radii, W: int, H: int, bg, semantics=None, upstream: Optional[D
     out.update(grad2d=g2d, mass_grad2d=g2m, kmass_grad2d=g2k, grad_semantics=gsem, mass_grad_semantics=gsem_m,
                kmass_grad_semantics=gsem_k, ntiles=ntiles)
     return out
+
+
+# ----------------------------------------------------------------------------------------------- near-threshold decisions
+# Rounding counts (units of 2^-24) of the two values the reference's per-pair tests read (forward.cu:420-430), see power_interval.
+EPS_POWER = 8.0
+EPS_ALPHA = 8.0
+
+
+def power_interval(rec, px, py):
+    """fp64 power of the pairs (records `rec` [..., 12] against pixel coordinates px, py, broadcast) and a bound `err` with
+    |fp32 power - fp64 power| <= err for the reference's expression -0.5 (a dx dx + c dy dy) - b dx dy evaluated in fp32 on the
+    same fp32 record, with or without contraction to FMAs.  Returns (power, err, pm).
+
+    Derivation (u = 2^-24, pm = 0.5 (|a| dx^2 + |c| dy^2) + |b dx dy|): dx = x - px rounds once (u |dx|), as does dy.  Each of
+    a dx dx, c dy dy, b dx dy then takes two products: 2 u from the rounded coordinates plus 2 roundings, 4 u of its magnitude.
+    The sum a dx dx + c dy dy adds one rounding of a value <= |a| dx^2 + |c| dy^2, so -0.5 (...) is off by 5 u of its terms, and the
+    final difference adds u |power| <= u pm:  |err| <= 5 u pm + u pm = 6 u pm to first order.  A contracted FMA drops a rounding,
+    never adds one.  EPS_POWER = 8 covers the second-order terms."""
+    dx = rec[..., 0].to(F64) - px
+    dy = rec[..., 1].to(F64) - py
+    a, b, c = rec[..., 2].to(F64), rec[..., 3].to(F64), rec[..., 4].to(F64)
+    power = -0.5 * (a * dx * dx + c * dy * dy) - b * dx * dy
+    pm = 0.5 * (a.abs() * dx * dx + c.abs() * dy * dy) + (b * dx * dy).abs()
+    return power, EPS_POWER * EPS32 * pm, pm
+
+
+def pair_decisions(rec, px, py):
+    """The reference's blend decision of pairs (power > 0 skips, o exp(power) < 1/255 skips) judged on the interval of
+    power_interval and on EPS_ALPHA u of relative error in alpha (expf is within 2 ulp = 4 u, the product with the opacity one
+    rounding).  'may': some fp32 evaluation within the bounds blends the pair;  'must': every one does."""
+    power, err, pm = power_interval(rec, px, py)
+    o = rec[..., 5].to(F64)
+    lo, hi = power - err, power + err
+    ae = EPS_ALPHA * EPS32
+    may = (lo <= 0) & (o * torch.exp(torch.clamp(hi, max=0.0)) * (1 + ae) >= ALPHA_MIN)
+    must = (hi <= 0) & (o * torch.exp(torch.clamp(lo, max=0.0)) * (1 - ae) >= ALPHA_MIN)
+    return dict(power=power, err=err, pm=pm, may=may, must=must & may)
+
+
+def instance_pixels(rec, radii, W, H, max_pairs: int = 1 << 22):
+    """Yields the (tile, Gaussian) instances of the reference's rectangles in chunks, each with its 256 pixels:
+    dict(tile [n], gid [n], pix [n, 256] flat index, inside [n, 256], px, py [n, 256], dec = pair_decisions of every pixel)."""
+    tiles, ids, _, _ = _instances(rec, radii, W, H)
+    gx = (W + TILE - 1) // TILE
+    dev = rec.device
+    lx = torch.arange(256, device=dev) % TILE
+    ly = torch.arange(256, device=dev) // TILE
+    step = max(1, max_pairs // 256)
+    for s in range(0, len(tiles), step):
+        t, g = tiles[s:s + step], ids[s:s + step]
+        pxi = (t % gx)[:, None] * TILE + lx[None, :]
+        pyi = (t // gx)[:, None] * TILE + ly[None, :]
+        inside = (pxi < W) & (pyi < H)
+        pix = torch.where(inside, pyi * W + pxi, torch.zeros_like(pxi))
+        dec = pair_decisions(rec[g][:, None, :], pxi.to(F64), pyi.to(F64))
+        dec["may"] &= inside
+        dec["must"] &= inside
+        yield dict(tile=t, gid=g, pix=pix, inside=inside, px=pxi, py=pyi, dec=dec)
+
+
+def ambiguous_pairs(rec, radii, W, H):
+    """(flat pixel, Gaussian) of every pair of the reference's rectangles that may blend but need not: its decision is left to
+    fp32 rounding.  Returns dict(pix, gid, power, err) sorted by (pix, gid)."""
+    pix, gid, pw, er = [], [], [], []
+    for ch in instance_pixels(rec.to(F64), radii, W, H):
+        d = ch["dec"]
+        amb = d["may"] & ~d["must"]
+        n, i = torch.nonzero(amb, as_tuple=True)
+        pix.append(ch["pix"][n, i]); gid.append(ch["gid"][n]); pw.append(d["power"][n, i]); er.append(d["err"][n, i])
+    if not pix:
+        z = torch.zeros(0, dtype=torch.int64, device=rec.device)
+        return dict(pix=z, gid=z, power=z.to(F64), err=z.to(F64))
+    pix, gid, pw, er = torch.cat(pix), torch.cat(gid), torch.cat(pw), torch.cat(er)
+    o = torch.argsort(pix * rec.shape[0] + gid)
+    return dict(pix=pix[o], gid=gid[o], power=pw[o], err=er[o])
 
 
 def bound(kmass, mass=None, ntiles=None, extra: float = 0.0):

@@ -22,12 +22,16 @@
 // not help either: the kernel is bound by the NUMBER of instructions it issues, not by latency.
 // What did pay: cutting instructions.  Phase 2 accumulates the moments in chunk-local integer pixel coordinates
 // (compile-time constants of a fully unrolled loop: 3 FMAs per pixel instead of 8, no coordinate loads, no index rotation — the shared
-// arrays are padded instead) and re-centres them once per thread; phase 1 takes exp() as ex2.approx.
+// arrays are padded instead) and re-centres them once per thread; phase 1 takes exp() as ex2.approx, and falls back to the
+// forward's expf only for pairs within a few 2^-22 of alpha = 1/255, so that it blends exactly the pairs the forward blended.
 #include "sgr_common.cuh"
 
 namespace sgr {
 
 constexpr int kB2 = 32;  // splats per batch
+// o G with ex2.approx: at or above kAlphaPass the forward's expf surely gives alpha >= 1/255, below kAlphaSkip surely not
+constexpr float kAlphaPass = (1.0f / 255.0f) * (1.0f + 0x1p-16f);
+constexpr float kAlphaSkip = (1.0f / 255.0f) * (1.0f - 0x1p-16f);
 constexpr uint32_t kRec2 = 48;
 // Shared-memory map.  Phase 2 reads pixel i of chunk c (= the 8x4 block of warp c) at a COMPILE-TIME offset, so the 8 chunk-threads
 // of a splat (consecutive lanes) must land in different banks by layout, not by rotating the index: each 32-pixel chunk is padded by one
@@ -156,15 +160,28 @@ __global__ void __launch_bounds__(256, 3) blend_bwd2_kernel(const FrameDev f, co
 				if (valid) {
 					float G;
 					if (kFastExp) {
-						// ex2.approx of power * log2(e): 2 instructions instead of expf's 10.  G is ~4e-7 relative off the forward's
-						// expf — the same order as the reciprocal below, far inside the 1e-3 gradient bar.  SGR_BWD2_EXPF=1 selects expf.
+						// ex2.approx of power * log2(e): 2 instructions instead of expf's 10.  Its VALUE is within
+						// 2^-21 + |power| 2^-23 relative of the forward's expf (ex2.approx and expf 2^-22 each, the rounded argument
+						// and log2(e) |power| 2^-24 each), inside the gradient bounds.  But the forward's DECISION alpha < 1/255
+						// must be taken again exactly: a pair the forward blended and this kernel skipped (or the reverse) drops (or
+						// invents) its own gradient and puts T off by ~1/255 for every pair in front of it.  So a pair passes at once
+						// only when o G clears 1/255 by 2^-16 relative (more than the difference for |power| <= 28, i.e. for any
+						// opacity below ~5e9, since |power| = ln(255 o) at the threshold); below that window it is skipped, and
+						// inside it G is recomputed with the forward's expf.  The window test costs blend_bwd2 about 3.5 % on config C.
+						// (fminf(0.99, .) does not move a decision against 1/255; NaN passes in both kernels.)
+						// SGR_BWD2_EXPF=1 selects expf everywhere.
 						asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(G) : "f"(power * 1.4426950408889634f));
+						valid = !(q1.y * G < kAlphaPass);
+						if (!valid && !(q1.y * G < kAlphaSkip)) {
+							G = expf(power);
+							valid = !(q1.y * G < 1.0f / 255.0f);
+						}
 					} else {
 						G = expf(power);
+						valid = !(fminf(0.99f, q1.y * G) < 1.0f / 255.0f);
 					}
-					const float alpha = fminf(0.99f, q1.y * G);
-					valid = !(alpha < 1.0f / 255.0f);
 					if (valid) {
+						const float alpha = fminf(0.99f, q1.y * G);
 						const float4 q2 = ld4(a + 32);  // r, g, b, clamp bits
 						// 1/(1-alpha), alpha <= 0.99: hardware reciprocal + one Newton step (<= 1 ulp) = 3 instructions instead of
 						// the ~8 of an IEEE division with its special-case path; serves both T/(1-a) and T_final/(1-a)

@@ -198,15 +198,27 @@ __device__ __forceinline__ void bulk_wait_all_read() { asm volatile("cp.async.bu
 // of the tile passes the reference's two per-pixel tests (forward.cu:420-430):  power <= 0  and  o*exp(power) >= 1/255.
 // With q(d) = a dx^2 + 2b dx dy + c dy^2 = -2*power this is  q <= 2*ln(255*o) =: qmax, i.e. the pixel lies inside an
 // ellipse.  tile_visit.cuh intersects that ellipse with each tile row in closed form.  Everything is evaluated
-// conservatively (slack far above fp32 rounding, "keep" on NaN / non-PD input).
+// conservatively ("keep" on NaN / non-PD input), with two slacks on qmax:
+//   0.02 + 1e-3 |tau|        the approximate log and the culling's own fast division / square root;
+//   2^-17 (a c / det) |2 tau| the fp32 rounding of `power` itself.  The reference sums terms of magnitude up to
+//                            |a| dx^2 + |c| dy^2 + 2 |b dx dy| <= 4 (a c / det) q on the ellipse, with ~6 roundings, and det = a c - b^2
+//                            cancels by the same ratio.  For a thin diagonal splat (conic condition number kappa, a c / det ~ kappa / 4)
+//                            that error is ~1e-2 q at kappa = 1e5 and comparable to q at kappa = 1e6, far above the constant slack:
+//                            without this term tiles holding pairs the reference blends were dropped.  Round or axis-aligned splats
+//                            (a c / det ~ 1) are not affected.
+// So a dropped tile receives nothing from any fp32 evaluation of the reference's expression within those rounding bounds.
 struct CullParams {
 	float mx, my, a, b, c, qmax;  // qmax < 0 => nothing can pass; qmax = +inf => keep all of the rectangle
 };
 __device__ __forceinline__ CullParams make_cull(float mx, float my, float a, float b, float c, float opacity) {
 	CullParams cp{mx, my, a, b, c, __int_as_float(0x7f800000)};
-	const bool pd = (a > 0.f) && (c > 0.f) && (a * c - b * b > 0.f);
+	const float det = a * c - b * b;
+	const bool pd = (a > 0.f) && (c > 0.f) && (det > 0.f);
 	const float tau = __logf(255.0f * opacity);  // (approximate log: the slack below dwarfs its error) NaN for negative / NaN opacity -> keep
-	if (pd && tau == tau) cp.qmax = 2.0f * tau + (0.02f + 1e-3f * fabsf(tau));
+	if (pd && tau == tau) {
+		const float ratio = __fdividef(a * c, det);  // >= 1
+		cp.qmax = 2.0f * tau + (0.02f + 1e-3f * fabsf(tau)) + 0x1p-17f * ratio * fabsf(2.0f * tau);
+	}
 	return cp;
 }
 // state carving (host) — implemented in capi.cu

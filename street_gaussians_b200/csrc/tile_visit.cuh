@@ -7,7 +7,8 @@
 // tile columns it touches form ONE interval whose ends follow in closed form from the ellipse's x-extent inside the
 // strip (two square roots per row).  A tile (full strip height) intersects the convex set iff its x-range intersects
 // that interval, so this is exactly the per-tile test, at O(rows) instead of O(rows x cols) cost, with the same
-// conservative slack (a tile that is kept needlessly only costs time; a dropped tile provably receives nothing).
+// conservative slack (a tile that is kept needlessly only costs time; a dropped tile receives nothing from any fp32
+// evaluation of the reference's `power` within the rounding bound that make_cull's qmax slack covers).
 //
 // (Tried and removed: an extra 8-bit mask per instance of the tile's eight 8x4-pixel blocks so that the blend warps could
 // skip splats that miss their block.  On the BASELINE config-C frame pixels saturate on large near splats, so few
@@ -24,7 +25,7 @@ namespace sgr {
 constexpr int kCoopArea = 64;
 
 // Approximate (MUFU-based, ~2 ulp) division / square root: this file only decides which tiles are KEPT, with slack
-// (0.05 px on the interval ends, 0.02 + 1e-3|tau| on qmax) that is orders of magnitude above their error, and count and emit
+// (0.05 px on the interval ends, 0.02 + 1e-3|tau| on qmax, plus make_cull's term for thin splats) above their error, and count and emit
 // evaluate the identical code, so the IEEE versions (10-15 dependent instructions each) buy nothing here.
 __device__ __forceinline__ float fast_sqrt(float x) { return x * __frsqrt_rn(fmaxf(x, 1e-30f)); }
 __device__ __forceinline__ float fast_div(float x, float y) { return __fdividef(x, y); }
