@@ -10,8 +10,13 @@ INFRASTRUCTURE, not product code (nothing under street_gaussians_b200/ may impor
                 lib/models/gaussian_model.py:300-303, 316-318)
   stats64       the densification statistics (csrc/optim.cu densify_stats_kernel; reference lib/models/street_gaussian_model.py:
                 551-571)
+  acc_loss64    the sky loss and the object-accumulation loss, value and dL/dacc (csrc/losses.cu acc_loss_kernel<SkyForm / ObjForm>;
+                reference train.py:107-122)
+  lidar64       the LiDAR depth loss: the exact top-k selection, value and fp32 gradients in the kernel's order (csrc/losses.cu
+                lidar_*_kernel; reference train.py:124-132)
 
-Every function returns, for each output element, the fp64 value and an absolute bound on |fp32 kernel - fp64 value|, built from the
+Every function returns, for each output element, the fp64 value and an absolute bound on |fp32 kernel - fp64 value| (lidar64's
+gradients are instead an fp32 restatement the kernel must match bit for bit), built from the
 magnitudes the fp32 code actually combines.  u = 2^-24 is the unit roundoff of fp32; a rounding whose result can be subnormal adds
 an absolute 2^-149.  The bounds are first order (products of two error terms are dropped); each constant is a count of roundings,
 derived in the docstring of the function that uses it and rounded up, never fitted to observed errors.
@@ -343,3 +348,144 @@ def stats64(max_radii2D, grad_accum, denom, radii, grad2d) -> Dict[str, torch.Te
     b = torch.where(vis[:, None], 3 * U * torch.stack([hyp, torch.zeros_like(hyp)], 1) + U * ga1.abs() + 2 * TINY, 0.0)
     return dict(max_radii2D=torch.where(vis, torch.maximum(mr, r), mr), denom=torch.where(vis[:, None], dn.reshape(-1, 1) + 1, dn.reshape(-1, 1)),
                 xyz_gradient_accum=ga1, b_xyz_gradient_accum=b)
+
+
+# ----------------------------------------------------------------------------------------------- sky / object accumulation losses
+ACC_LO = float(np.float32(1e-6))                               # the kernel's clamp edges 1e-6f and 1.f - 1e-6f; torch.clamp casts
+ACC_HI = float(np.float32(np.float32(1.0) - np.float32(1e-6)))  # min=1e-6, max=1 - 1e-6 to the same two floats
+ACC_MAX_BLOCKS = 1056                                           # launch_acc_loss: min(ceil(N / 256), kNumSMs * 8) blocks
+
+
+def acc_blocks(N: int) -> int:
+    return max(1, min(-(-N // 256), ACC_MAX_BLOCKS))
+
+
+def acc_loss64(kind: str, acc, flag, weight: float) -> Dict[str, torch.Tensor]:
+    """kind "sky" (train.py:107-113): mean(flag ? -log(1 - a) : -log(a)); kind "obj" (train.py:114-122): mean(flag ? -(a log a +
+    (1 - a) log(1 - a)) : -log(1 - a)); a = clamp(acc, 1e-6, 1 - 1e-6), times weight.  acc fp32, flag bool, any shape.
+    Returns grad (dL/dacc, flat), value and their bounds b_grad, b_value; "inside" marks the pixels where the clamp passes the
+    gradient (a in [1e-6f, 1 - 1e-6f], inclusive like torch.clamp's backward).  A NaN in acc is kept by the clamp, as torch.clamp
+    keeps it: the value is NaN and that pixel's gradient is 0.
+
+    Everything is computed in fp64 from the fp32 acc (the clamp is exact in fp32).  Bounds (u = 2^-24; CUDA's logf is within 1 ulp,
+    i.e. 2 u of its result; om = 1 - ac is one fp32 rounding, exact for ac >= 0.5, and log(om (1 + d)) = log(om) + d moves a log by
+    at most u absolutely):
+      gradient   the kernel forms (weight / (float)N) * deriv:  the fp32 weight, (float)N, the division and the product are 4 u on
+                 |grad|; deriv adds  sky: 1 / (1 - ac) 2 u |deriv| (om, the division), -1 / ac  u |deriv|;  obj: logf(om) - logf(ac)
+                 2 u (|log om| + |log ac|) + u (om's rounding) + u |deriv| (the subtraction) - absolute, since the two logs cancel
+                 near ac = 0.5 -, 1 / om 2 u |deriv|.  Each times |weight| / N; plus 2^-149.
+                 The obj entropy bound also covers autograd's order of the same expression, so that the fp32 torch restatement can
+                 stand in for the kernel on the CPU: with G the incoming gradient, torch adds -G log ac (3 u |G log ac|), -(G ac) / ac
+                 (2 u |G|), G log om (|G| (3 u |log om| + u)) and (G om) / om (2 u |G|), whose +-G cancel, in 3 additions of partial
+                 sums up to |G| (|log ac| + |log om| + 2) (3 u each): in all |G| u (6 (|log om| + |log ac|) + 11), which is larger
+                 than the kernel's count and is the one used.
+      values     per pixel  sky: -logf(om) u + 2 u |v|, -logf(ac) 2 u |v|;  obj: -(ac logf(ac) + om logf(om)) with t1 = ac log ac,
+                 t2 = om log om: 3 u |t1| (logf, product) + 4 u |t2| + u om (om's rounding, through both factors of t2) + u |v| (the
+                 sum), rounded up to 4 u (|t1| + |t2|) + u om + u |v|;  -logf(om) u + 2 u |v|.
+      value      each thread adds its m = ceil(N / (blocks 256)) values in fp32 ((m - 1) u on sum |v|), then 5 shuffle levels (5 u),
+                 then fp64 (the 8 warp sums and one atomic per block: (blocks + 8) 2^-53); the mean and weight in fp64 and one
+                 rounding to fp32, with the fp32 weight: 2 u |value|."""
+    a = acc.detach().reshape(-1).to(F64)
+    f = flag.detach().reshape(-1).to(a.device).bool()
+    N = a.numel()
+    nan = torch.isnan(a)
+    ac = torch.where(nan, a, a.clamp(ACC_LO, ACC_HI))
+    inside = (a >= ACC_LO) & (a <= ACC_HI)
+    om = 1.0 - ac
+    la, lo = torch.log(ac), torch.log(om)
+    if kind == "sky":
+        v = torch.where(f, -lo, -la)
+        dv = torch.where(f, 1.0 / om, -1.0 / ac)
+        e_v = torch.where(f, U + 2 * U * v.abs(), 2 * U * v.abs())
+        e_d = torch.where(f, 2 * U * dv.abs(), U * dv.abs())
+    elif kind == "obj":
+        t1, t2 = ac * la, om * lo
+        v = torch.where(f, -(t1 + t2), -lo)
+        dv = torch.where(f, lo - la, 1.0 / om)
+        e_v = torch.where(f, 4 * U * (t1.abs() + t2.abs()) + U * om + U * v.abs(), U + 2 * U * v.abs())
+        e_d = torch.where(f, 6 * U * (la.abs() + lo.abs()) + 11 * U, 2 * U * dv.abs())
+    else:
+        raise ValueError(kind)
+    c = weight / N
+    grad = torch.where(inside, c * dv, 0.0)
+    b_grad = torch.where(inside, abs(c) * e_d + 4 * U * grad.abs() + TINY, 0.0)
+    blocks = acc_blocks(N)
+    m = -(-N // (blocks * 256))
+    s_abs = float(v.abs().sum())
+    value = weight * float(v.sum()) / N
+    b_value = abs(weight) / N * (float(e_v.sum()) + (m - 1 + 5) * U * s_abs + (blocks + 8) * 2.0 ** -53 * s_abs) + 2 * U * abs(value) + TINY
+    return dict(grad=grad, b_grad=b_grad, value=value, b_value=b_value, inside=inside, blocks=blocks, terms_per_thread=m)
+
+
+# ----------------------------------------------------------------------------------------------- LiDAR depth loss
+LIDAR_MAX_BLOCKS = 528         # lidar_grid: min(ceil(N / 256), kNumSMs * 4) blocks of contiguous pixel ranges
+NAN_KEY = 0x7FC00000           # every NaN key, whatever its bits, as one class above +inf (0x7F800000)
+
+
+def lidar_grid(N: int):
+    """(blocks, chunk): chunk = ceil(tiles / blocks) 256 pixels per block; blocks past ceil(N / chunk) are empty."""
+    tiles = -(-N // 256)
+    blocks = max(1, min(tiles, LIDAR_MAX_BLOCKS))
+    return blocks, -(-tiles // blocks) * 256
+
+
+def _f32(t):
+    return np.ascontiguousarray(t.detach().cpu().reshape(-1).numpy() if torch.is_tensor(t) else np.asarray(t).reshape(-1), np.float32)
+
+
+def lidar_keys(depth, acc, lidar):
+    """err = |depth / (acc + 1e-10f) - lidar| in fp32 (numpy's fp32 add, division and subtraction are IEEE and keep subnormals, as
+    the library's build does) and the sort key of each pixel: err's bit pattern, NaN mapped to NAN_KEY.  CUDA writes the canonical NaN
+    0x7FFFFFFF and x86 does not, so only NaN-ness, not the bits, is comparable."""
+    d, a, l = _f32(depth), _f32(acc), _f32(lidar)
+    with np.errstate(all="ignore"):
+        b = a + np.float32(1e-10)
+        e = d / b
+        df = e - l
+        err = np.abs(df)
+    key = np.where(np.isnan(err), NAN_KEY, err.view(np.uint32).astype(np.int64))
+    return dict(b=b, e=e, df=df, err=err, key=key, lidar=l)
+
+
+def lidar64(depth, acc, lidar, mask, weight: float, keep: float) -> dict:
+    """The LiDAR depth loss, weight * mean of the k = int(keep n) smallest err over the n pixels with lidar > 0 and mask.
+
+    Selection: the first k of the valid pixels stably sorted by (key, flat index) - exactly the kernel's radix select with ties taken
+    at the lowest flat indices.  value: the fp64 mean of the selected err times the fp32 weight the kernel receives; the kernel sums in
+    fp64 (at most k roundings of 2^-53 on a sum of non-negative terms, then the division and the weight) and rounds once to fp32, which
+    can be subnormal:  b_value = (u + (k + 2) 2^-53) |value| + 2^-149.
+    NaN for k = 0, and for a selected NaN.  Gradients (flat fp32, 0 off the selection) restate lidar_grad_kernel in its own order:
+    gk = w32 / (float)k, g = sign(df) gk with sign(0) = sign(NaN) = 0, gd = g / b, ga = -g (e / b); the kernel must match them bit
+    for bit."""
+    r = lidar_keys(depth, acc, lidar)
+    l, key = r["lidar"], r["key"]
+    valid = l > 0
+    if mask is not None:
+        valid &= _f32(mask.to(torch.float32) if torch.is_tensor(mask) else mask) != 0
+    n = int(valid.sum())
+    k = int(keep * n)
+    idx = np.nonzero(valid)[0]
+    order = idx[np.argsort(key[idx], kind="stable")]
+    sel = np.zeros(key.size, bool)
+    sel[order[:k]] = True
+    w32 = np.float32(weight)
+    gd = np.zeros(key.size, np.float32)
+    ga = np.zeros(key.size, np.float32)
+    if k:
+        t = int(key[order[k - 1]])
+        mean = float(r["err"][order[:k]].astype(np.float64).sum()) / k
+        value = float(w32) * mean
+        gk = w32 / np.float32(k)
+        df, b, e = r["df"][sel], r["b"][sel], r["e"][sel]
+        sg = np.where(df > 0, np.float32(1), np.where(df < 0, np.float32(-1), np.float32(0))).astype(np.float32)
+        g = sg * gk
+        with np.errstate(all="ignore"):
+            gd[sel] = g / b
+            ga[sel] = -g * (e / b)
+    else:
+        t, value = None, float("nan")
+    lt = int((valid & (key < t)).sum()) if k else 0
+    ties = int((valid & (key == t)).sum()) if k else 0
+    b_value = (U + (k + 2) * 2.0 ** -53) * abs(value) + TINY
+    return dict(valid=valid, n=n, k=k, sel=sel, key=key, t=t, lt=lt, ties=ties, take=k - lt, value=value, b_value=b_value, gd=gd, ga=ga,
+                err=r["err"], df=r["df"])

@@ -200,6 +200,8 @@ struct ObjForm {
 };
 
 // out[0] += sum of Form::value; grad = weight / N * d/dacc (zero where the clamp is active, like torch.clamp's backward).
+// A NaN acc stays NaN through the clamp, as in torch.clamp (fmaxf alone would turn it into 1e-6): the value reports the diverged
+// render, and the pixel's gradient is 0 since `inside` is false for NaN.
 template <class Form>
 __global__ void __launch_bounds__(256) acc_loss_kernel(const size_t N, const float *__restrict__ accm, const uint8_t *__restrict__ flag, const float weight,
                                                       float *__restrict__ grad, double *__restrict__ out) {
@@ -207,7 +209,7 @@ __global__ void __launch_bounds__(256) acc_loss_kernel(const size_t N, const flo
 	float v = 0.f;
 	for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += (size_t)gridDim.x * blockDim.x) {
 		const float a = accm[i];
-		const float ac = fminf(fmaxf(a, 1e-6f), 1.f - 1e-6f);
+		const float ac = a != a ? a : fminf(fmaxf(a, 1e-6f), 1.f - 1e-6f);
 		const bool inside = a >= 1e-6f && a <= 1.f - 1e-6f;
 		const bool s = flag[i] != 0;
 		v += Form::value(ac, s);
