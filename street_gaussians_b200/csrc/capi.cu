@@ -374,7 +374,10 @@ static int make_total_frame(const SgrFrame *frame, const SgrPeers *peers, FrameD
 	if (fl.S != 0) return fail(SGR_EUNSUPPORTED, "the fused Gaussian-sharded step supports S == 0 only (use the staged calls for feature channels)");
 	for (int p = 0; p < pt.world; p++)
 		if (pt.world > 1 && !pt.flags[p]) return fail(SGR_EINVAL, "peer table entry %d has no barrier pad", p);
-	if (pt.world > 1 && !(fl.band.step == pt.world && fl.band.begin == pt.rank))
+	// a rank past the last tile row (more ranks than tile rows) owns no row: its cyclic band is empty (cyclic_band passes [0, 0)), it
+	// receives no record and renders nothing, but it still projects, scatters and gathers its own Gaussians and takes every barrier
+	const bool no_rows = pt.rank >= fl.gy && band_rows(fl.band) == 0;
+	if (pt.world > 1 && !no_rows && !(fl.band.step == pt.world && fl.band.begin == pt.rank))
 		return fail(SGR_EINVAL, "the peer exchange needs the cyclic band of this rank: begin == rank, step == world (got [%d,%d) step %d)",
 		            fl.band.begin, fl.band.end, fl.band.step);
 	ft = fl;
