@@ -158,6 +158,49 @@ int sgr_backward(const SgrFrame *frame, int64_t num_instances, const float *mean
                  float *dL_dcolors_precomp, float *dL_dsemantics, float *dL_dopacity, float *dL_dscales,
                  float *dL_drotations, float *dL_dcov3D, float *grad2d_scratch, void *stream);
 
+/* ---- Render layers: row ranges of the same call rendered alongside the full frame (whole image, one GPU) ----------------------
+ * A layer is the half-open row range [begin, end) of the call's Gaussians plus a background colour; its images are bit-identical
+ * to a separate sgr_forward on the sliced arrays with that background and S = 0 (colour, depth, alpha only).  That is the
+ * reference's objects-only / background-only render with parse_camera_again=False (render_object / render_background,
+ * lib/models/street_gaussian_renderer.py:13-40, train.py:114-122), which rasterises the actor rows [n_bkgd, P) of the tensors the
+ * full render used.  Per tile the separate call's list is the subsequence of the main list with ids in the range (stable depth
+ * pre-sort, stable tile sort), so the layer's list is compacted out of the main call's list and blended with the main call's
+ * per-Gaussian records: nothing is projected, sorted or read back again, and the bounded mode stays free of host synchronisation.
+ * An empty range (begin == end, also with P == 0) gives colour bg and zero depth and alpha, as render_kernel's empty branch
+ * (street_gaussian_renderer.py:138-151) does — not the zero colour of sgr_forward's P == 0 short-circuit. */
+typedef struct SgrLayer {
+	int32_t begin, end;  /* 0 <= begin <= end <= frame.P */
+	const float *bg;     /* [3] device */
+} SgrLayer;
+/* Bytes of one layer's caller-owned state (per-tile ranges, per-pixel contributor counts and the layer's tile lists) for a main call
+ * whose sgr_backward_* calls take num_instances: the instance count of sgr_forward, or the capacity of sgr_forward_bounded. */
+int sgr_layer_state_sizes(const SgrFrame *frame, int64_t num_instances, size_t *layer_bytes);
+/* Renders `layer` from the state a whole-image sgr_forward / sgr_forward_bounded left in geom / binning / img state (frame == that
+ * call's frame, num_instances == the value its backward takes).  out_color[3,H,W], out_depth[1,H,W], out_alpha[1,H,W]: every pixel
+ * written.  With an empty range no state is read (geom / binning / img state may be NULL). */
+int sgr_forward_layer(const SgrFrame *frame, const SgrLayer *layer, int64_t num_instances, const void *geom_state, const void *binning_state,
+                      const void *img_state, void *layer_state, size_t layer_bytes, float *out_color, float *out_depth, float *out_alpha,
+                      void *stream);
+/* Backward blend of one layer (its sgr_forward_layer state): grad2d[end-begin, 12] (row r = Gaussian begin + r, same columns as
+ * sgr_backward_blend) is ZEROED and accumulated.  Nothing is done for an empty range. */
+int sgr_backward_blend_layer(const SgrFrame *frame, const SgrLayer *layer, const void *geom_state, const void *layer_state, const float *out_alpha,
+                             const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha, float *grad2d, void *stream);
+typedef struct SgrLayerGrad {
+	int32_t begin, end;
+	const float *grad2d;  /* [end-begin, 12] device (sgr_backward_blend_layer's output), or NULL: this layer has no gradient */
+	float *dL_dmeans2D;   /* [end-begin, 3] device or NULL: receives this layer's own screen-space gradient ([0:3] of its grad2d) */
+} SgrLayerGrad;
+/* sgr_backward_geom for a layered call: the chain rule runs once on the main sums plus every layer's sums (all 12 columns), while
+ * dL_dmeans2D receives the MAIN sums only, as a separate call would leave it (the densification statistics read it); each layer's
+ * own [0:3] goes to its dL_dmeans2D sink.  grad2d[P,12] (the main sums) is CONSUMED: the layer rows are added into it in place.
+ * layers: HOST array.  scratch: 3 floats per row of [lo, hi), the smallest range that covers every layer with a gradient (3 * P
+ * floats always suffice).  Outputs and their rules as in sgr_backward_geom. */
+int sgr_backward_geom_layered(const SgrFrame *frame, const float *means3D, const float *shs, const float *colors_precomp,
+                              const float *scales, const float *rotations, const float *cov3D_precomp, const int32_t *radii,
+                              const void *geom_state, float *grad2d, const SgrLayerGrad *layers, int32_t num_layers, float *scratch,
+                              float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors_precomp, float *dL_dopacity,
+                              float *dL_dscales, float *dL_drotations, float *dL_dcov3D, void *stream);
+
 /* ---- Gaussian-sharded rendering (multi-GPU; no reference counterpart — the reference is single-GPU.  SURVEY.md §8e
  * "variant A": every rank owns P/N Gaussians AND a tile-row band) --------------------------------------------------
  * The forward of DGR/cuda_rasterizer/rasterizer_impl.cu:197-343 is split at the point where the per-Gaussian work

@@ -10,13 +10,13 @@ from __future__ import annotations
 import os
 import sys
 
-from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, InstanceCapacity, TileRowBand,  # noqa: F401
+from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, InstanceCapacity, RenderLayer, TileRowBand,  # noqa: F401
                          distCUDA2, rasterize_gaussians)
 
 from .composer import compose  # noqa: E402,F401
 from . import losses, training  # noqa: E402,F401
 
-__all__ = ["compose", "GaussianRasterizationSettings", "GaussianRasterizer", "TileRowBand", "InstanceCapacity", "rasterize_gaussians", "distCUDA2",
+__all__ = ["compose", "GaussianRasterizationSettings", "GaussianRasterizer", "TileRowBand", "InstanceCapacity", "RenderLayer", "rasterize_gaussians", "distCUDA2",
            "install_shims"]
 
 _SHIMS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "shims")

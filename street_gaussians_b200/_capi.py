@@ -17,7 +17,8 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_state_s
            "sgr_scatter_records", "sgr_gather_grad2d", "sgr_peer_barrier", "sgr_sharded_forward", "sgr_sharded_backward",
            "sgr_compose_forward", "sgr_compose_backward", "sgr_image_loss_scratch_bytes", "sgr_image_loss", "sgr_sky_loss",
            "sgr_obj_acc_loss", "sgr_lidar_depth_loss_scratch_bytes", "sgr_lidar_depth_loss", "sgr_densify_stats", "sgr_adam_step",
-           "sgr_densify_scratch_bytes", "sgr_densify_plan", "sgr_densify_apply", "sgr_reset_opacity", "sgr_sparse_adam_step"]
+           "sgr_densify_scratch_bytes", "sgr_densify_plan", "sgr_densify_apply", "sgr_reset_opacity", "sgr_sparse_adam_step",
+           "sgr_layer_state_sizes", "sgr_forward_layer", "sgr_backward_blend_layer", "sgr_backward_geom_layered"]
 
 
 class SgrFrame(C.Structure):
@@ -85,6 +86,14 @@ class SgrSparseAdamSegment(C.Structure):
     _fields_ = [("start", C.c_int32), ("count", C.c_int32), ("param", C.c_void_p * DENSIFY_TENSORS), ("grad", C.c_void_p * DENSIFY_TENSORS),
                 ("exp_avg", C.c_void_p * DENSIFY_TENSORS), ("exp_avg_sq", C.c_void_p * DENSIFY_TENSORS), ("width", C.c_int32 * DENSIFY_TENSORS),
                 ("lr", C.c_float * DENSIFY_TENSORS), ("step", C.c_int32 * DENSIFY_TENSORS), ("reserved", C.c_int32)]
+
+
+class SgrLayer(C.Structure):
+    _fields_ = [("begin", C.c_int32), ("end", C.c_int32), ("bg", C.c_void_p)]
+
+
+class SgrLayerGrad(C.Structure):
+    _fields_ = [("begin", C.c_int32), ("end", C.c_int32), ("grad2d", C.c_void_p), ("dL_dmeans2D", C.c_void_p)]
 
 
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
@@ -178,6 +187,14 @@ def lib():
     L.sgr_reset_opacity.argtypes = [C.POINTER(SgrDensifySegment), C.c_int32, vp]
     L.sgr_sparse_adam_step.restype = C.c_int
     L.sgr_sparse_adam_step.argtypes = [C.POINTER(SgrSparseAdamSegment), C.c_int32, vp, C.c_double, C.c_double, C.c_double, vp]
+    L.sgr_layer_state_sizes.restype = C.c_int
+    L.sgr_layer_state_sizes.argtypes = [C.POINTER(SgrFrame), C.c_int64, C.POINTER(C.c_size_t)]
+    L.sgr_forward_layer.restype = C.c_int
+    L.sgr_forward_layer.argtypes = [C.POINTER(SgrFrame), C.POINTER(SgrLayer), C.c_int64, vp, vp, vp, vp, C.c_size_t, vp, vp, vp, vp]
+    L.sgr_backward_blend_layer.restype = C.c_int
+    L.sgr_backward_blend_layer.argtypes = [C.POINTER(SgrFrame), C.POINTER(SgrLayer)] + [vp] * 8
+    L.sgr_backward_geom_layered.restype = C.c_int
+    L.sgr_backward_geom_layered.argtypes = [C.POINTER(SgrFrame)] + [vp] * 9 + [C.POINTER(SgrLayerGrad), C.c_int32, vp] + [vp] * 8 + [vp]
     L.sgr_backward_blend.restype = C.c_int
     L.sgr_backward_blend.argtypes = [C.POINTER(SgrFrame), C.c_int64] + [vp] * 12
     L.sgr_backward_geom.restype = C.c_int

@@ -355,6 +355,12 @@ cudaError_t launch_preprocess_bwd(const FrameDev &f, const float *means3D, const
                                   const int32_t *radii, GeomView g, const float *grad2d, float *dL_dmeans3D,
                                   float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity,
                                   float *dL_dscales, float *dL_drot, float *dL_dcov3D, cudaStream_t st);
+// render layers (layers.cu)
+cudaError_t launch_layer_lists(const FrameDev &f, ImgView main_img, BinView main_bin, int begin, int end, ImgView layer_img, uint32_t *layer_list,
+                               cudaStream_t st);
+cudaError_t launch_layer_fill(const FrameDev &f, const float *bg, float *color, float *depth, float *alpha, cudaStream_t st);
+cudaError_t launch_layer_stash(const float *grad2d, int lo, int hi, float *stash, bool restore, float *dL_dmeans2D, cudaStream_t st);
+cudaError_t launch_layer_merge(float *grad2d, const SgrLayerGrad *layers, int n, cudaStream_t st);
 cudaError_t launch_compose_fwd(const SgrSegment *segs, int nseg, int M, const float *poses, const float *idft, const uint8_t *flip,
                                const float *flip_quat, float *xyz, float *rot, float *scale, float *opac, float *sh, cudaStream_t st);
 cudaError_t launch_compose_bwd(const SgrSegment *segs, const SgrSegmentGrads *grads, int nseg, int M, const float *poses, const float *idft,

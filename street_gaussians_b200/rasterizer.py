@@ -300,22 +300,27 @@ def _backward_geom_impl(settings, band, st: _ForwardState, tensors, radii, grad2
     return g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rots, g_cov
 
 
+def _forward_or_dump(means3D, sh, colors_precomp, semantics, opacities, scales, rotations, cov3Ds_precomp, raster_settings, band, capacity):
+    try:
+        return _forward_impl(means3D, sh, colors_precomp, semantics, opacities, scales, rotations, cov3Ds_precomp, raster_settings, band,
+                             capacity)
+    except Exception:
+        if raster_settings.debug:  # same post-mortem as the reference (DGR/diff_gaussian_rasterization/__init__.py:87-94)
+            _dump("snapshot_fw.dump", (raster_settings.bg, means3D, colors_precomp, semantics, opacities, scales, rotations,
+                                       raster_settings.scale_modifier, cov3Ds_precomp, raster_settings.viewmatrix,
+                                       raster_settings.projmatrix, raster_settings.tanfovx, raster_settings.tanfovy,
+                                       raster_settings.image_height, raster_settings.image_width, sh, raster_settings.sh_degree,
+                                       raster_settings.campos, raster_settings.prefiltered, raster_settings.debug))
+            print("\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
+        raise
+
+
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, semantics, opacities, scales, rotations, cov3Ds_precomp,
                 raster_settings, band=None, grad_reduce=None, capacity=None):
-        try:
-            color, radii, depth, alpha, semantic, st, tensors = _forward_impl(means3D, sh, colors_precomp, semantics, opacities, scales,
-                                                                              rotations, cov3Ds_precomp, raster_settings, band, capacity)
-        except Exception:
-            if raster_settings.debug:  # same post-mortem as the reference (DGR/diff_gaussian_rasterization/__init__.py:87-94)
-                _dump("snapshot_fw.dump", (raster_settings.bg, means3D, colors_precomp, semantics, opacities, scales, rotations,
-                                           raster_settings.scale_modifier, cov3Ds_precomp, raster_settings.viewmatrix,
-                                           raster_settings.projmatrix, raster_settings.tanfovx, raster_settings.tanfovy,
-                                           raster_settings.image_height, raster_settings.image_width, sh, raster_settings.sh_degree,
-                                           raster_settings.campos, raster_settings.prefiltered, raster_settings.debug))
-                print("\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
-            raise
+        color, radii, depth, alpha, semantic, st, tensors = _forward_or_dump(means3D, sh, colors_precomp, semantics, opacities, scales,
+                                                                             rotations, cov3Ds_precomp, raster_settings, band, capacity)
         ctx.raster_settings, ctx.band, ctx.state, ctx.grad_reduce = raster_settings, band, st, grad_reduce
         ctx.shapes = tuple(None if t is None else (tuple(t.shape), t.device, t.dtype)
                            for t in (means3D, means2D, sh, colors_precomp, semantics, opacities, scales, rotations, cov3Ds_precomp))
@@ -382,6 +387,161 @@ class _RasterizeGaussians(torch.autograd.Function):
                 fit(g_opac, 5), fit(g_scales, 6), fit(g_rots, 7), fit(g_cov, 8), None, None, None, None)
 
 
+class RenderLayer(NamedTuple):
+    """Rows [begin, end) of the call's Gaussians, rendered in the same call as the full frame over background `bg` (3 floats).
+    The reference's objects-only render (render_object with parse_camera_again=False, train.py:114-122) is
+    ``RenderLayer(n_bkgd, P, (1, 1, 1))`` on the composed tensors, its background-only render ``RenderLayer(0, n_bkgd, (1, 1, 1))``.
+    The layer's (color, depth, alpha) equal a separate GaussianRasterizer call on the sliced tensors with this `bg` and no
+    semantics; an empty range gives colour `bg` with zero depth and alpha.  `means2D` ([end - begin, 3], optional) receives the
+    layer's own screen-space gradient, as the separate call's means2D would; the main call's means2D receives the main images' only."""
+    begin: int
+    end: int
+    bg: object
+    means2D: Optional[torch.Tensor] = None
+
+
+def _check_layers(layers, P: int):
+    """(begin, end, bg as a float32 tensor, means2D) per layer; raises ValueError before anything touches the GPU."""
+    out = []
+    for i, l in enumerate(layers):
+        if not isinstance(l, RenderLayer):
+            l = RenderLayer(*l)
+        b, e = int(l.begin), int(l.end)
+        if not 0 <= b <= e <= P:
+            raise ValueError(f"layer {i}: range [{b}, {e}) is not inside [0, {P}]")
+        bg = l.bg.detach() if isinstance(l.bg, torch.Tensor) else torch.as_tensor(l.bg, dtype=torch.float32)
+        if bg.numel() != 3 or not (bg.is_floating_point() or bg.dtype in (torch.int32, torch.int64)):
+            raise ValueError(f"layer {i}: bg must hold 3 floats, got shape {tuple(bg.shape)} of {bg.dtype}")
+        if l.means2D is not None and tuple(l.means2D.shape) != (e - b, 3):
+            raise ValueError(f"layer {i}: means2D must have shape ({e - b}, 3), got {tuple(l.means2D.shape)}")
+        out.append((b, e, bg.reshape(3), l.means2D))
+    return out
+
+
+class _RasterizeLayered(torch.autograd.Function):
+    """The whole-image call with render layers (include/sgr.h, SgrLayer): outputs (color, radii, depth, alpha, semantic) and then
+    (color, depth, alpha) per layer.  Inputs as _RasterizeGaussians, then the layer sinks (means2D of each layer, or None)."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, sh, colors_precomp, semantics, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
+                capacity, layers, *sinks):
+        ctx.set_materialize_grads(False)  # a layer without upstream gradient costs nothing in backward
+        color, radii, depth, alpha, semantic, st, tensors = _forward_or_dump(means3D, sh, colors_precomp, semantics, opacities, scales,
+                                                                             rotations, cov3Ds_precomp, raster_settings, None, capacity)
+        L = _capi.lib()
+        device, P = means3D.device, int(means3D.shape[0])
+        H, W = int(raster_settings.image_height), int(raster_settings.image_width)
+        M = int(tensors["sh"].shape[1]) if tensors is not None and tensors["sh"] is not None else 0
+        S = int(tensors["semantics"].shape[1]) if tensors is not None and tensors["semantics"] is not None else 0
+        fr, keep = _make_frame(raster_settings, P, M, S, device, None)
+        f32 = dict(device=device, dtype=torch.float32)
+        bgs, states, outs = [], [], []
+        for b, e, bg, _ in layers:
+            bg = _dev_f32(bg, device)
+            c, d, a = torch.empty((3, H, W), **f32), torch.empty((1, H, W), **f32), torch.empty((1, H, W), **f32)
+            lay = _capi.SgrLayer(b, e, bg.data_ptr())
+            ls, nbytes = None, 0
+            if e > b:
+                nb = C.c_size_t(0)
+                _capi.check(L.sgr_layer_state_sizes(C.byref(fr), st.num_instances, C.byref(nb)), "sgr_layer_state_sizes")
+                ls, nbytes = torch.empty((nb.value,), device=device, dtype=torch.uint8), nb.value
+            with torch.cuda.device(device):
+                rc = L.sgr_forward_layer(C.byref(fr), C.byref(lay), st.num_instances, _ptr(st.geom), _ptr(st.binning), _ptr(st.img), _ptr(ls),
+                                         nbytes, _ptr(c), _ptr(d), _ptr(a), _stream(device))
+            _capi.check(rc, "sgr_forward_layer")
+            bgs.append(bg)
+            states.append(ls)
+            outs += [c, d, a]
+        del keep
+        ctx.raster_settings, ctx.state, ctx.layers, ctx.layer_bgs, ctx.layer_states = raster_settings, st, layers, bgs, states
+        ctx.shapes = tuple(None if t is None else (tuple(t.shape), t.device, t.dtype)
+                           for t in (means3D, means2D, sh, colors_precomp, semantics, opacities, scales, rotations, cov3Ds_precomp))
+        ctx.tensor_keys = None if tensors is None else tuple(k for k, v in tensors.items() if v is not None)
+        ctx.tensor_none = None if tensors is None else tuple(k for k, v in tensors.items() if v is None)
+        layer_alphas = outs[2::3]
+        ctx.save_for_backward(radii, alpha, *layer_alphas, *([] if tensors is None else [tensors[k] for k in ctx.tensor_keys]))
+        ctx.mark_non_differentiable(radii)
+        return (color, radii, depth, alpha, semantic, *outs)
+
+    @staticmethod
+    def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha, grad_semantic, *grad_layers):
+        n = len(ctx.layers)
+        radii, alpha, *rest = ctx.saved_tensors
+        layer_alphas, saved = rest[:n], rest[n:]
+        shapes, settings, st = ctx.shapes, ctx.raster_settings, ctx.state
+        nones = (None, None, None)
+
+        def fit(g, i):
+            if shapes[i] is None:
+                return None
+            shape, device, dtype = shapes[i]
+            if g is None:
+                return torch.zeros(shape, device=device, dtype=dtype)
+            return g.reshape(shape).to(device=device, dtype=dtype)
+
+        if ctx.tensor_keys is None:  # P == 0: every range is empty
+            sink_grads = tuple(None if s is None else torch.zeros((0, 3), device=s.device, dtype=s.dtype) for _, _, _, s in ctx.layers)
+            return tuple(fit(None, i) for i in range(9)) + nones + sink_grads
+        tensors = dict(zip(ctx.tensor_keys, saved))
+        tensors.update({k: None for k in ctx.tensor_none})
+        means3D = tensors["means3D"]
+        dev, P = means3D.device, int(means3D.shape[0])
+        H, W = int(settings.image_height), int(settings.image_width)
+        S = int(tensors["semantics"].shape[1]) if tensors["semantics"] is not None else 0
+        zimg = lambda c: torch.zeros((c, H, W), device=dev, dtype=torch.float32)
+        # the main images: as the unlayered backward (an output without upstream gradient contributes zeros)
+        grad2d, g_sem = _backward_blend_impl(settings, None, st, tensors, alpha,
+                                             grad_color if grad_color is not None else zimg(3),
+                                             grad_depth if grad_depth is not None else zimg(1),
+                                             grad_alpha if grad_alpha is not None else zimg(1),
+                                             grad_semantic if grad_semantic is not None else zimg(S))
+        L = _capi.lib()
+        M = int(tensors["sh"].shape[1]) if tensors["sh"] is not None else 0
+        fr, keep = _make_frame(settings, P, M, S, dev, None)
+        table, sink_grads, keep_alive = [], [], []
+        for k, (b, e, _, sink) in enumerate(ctx.layers):
+            gc, gd, ga = grad_layers[3 * k: 3 * k + 3]
+            lg = _capi.SgrLayerGrad(b, e, None, None)
+            sg = None
+            if (gc is not None or gd is not None or ga is not None) and e > b:
+                gc = _dev_f32(gc, dev) if gc is not None else zimg(3)
+                gd = _dev_f32(gd, dev) if gd is not None else zimg(1)
+                ga = _dev_f32(ga, dev) if ga is not None else zimg(1)
+                g2 = torch.empty((e - b, 12), device=dev, dtype=torch.float32)
+                lay = _capi.SgrLayer(b, e, ctx.layer_bgs[k].data_ptr())
+                with torch.cuda.device(dev):
+                    rc = L.sgr_backward_blend_layer(C.byref(fr), C.byref(lay), _ptr(st.geom), _ptr(ctx.layer_states[k]), _ptr(layer_alphas[k]),
+                                                    _ptr(gc), _ptr(gd), _ptr(ga), _ptr(g2), _stream(dev))
+                _capi.check(rc, "sgr_backward_blend_layer")
+                lg.grad2d = g2.data_ptr()
+                keep_alive += [gc, gd, ga, g2]
+                if sink is not None and ctx.needs_input_grad[12 + k]:
+                    sg = torch.empty((e - b, 3), device=dev, dtype=torch.float32)
+                    lg.dL_dmeans2D = sg.data_ptr()
+            table.append(lg)
+            sink_grads.append(None if sg is None else sg.to(dtype=sink.dtype, device=sink.device))
+        live = [lg for lg in table if lg.grad2d]
+        if not live:  # no layer output has a gradient: the unlayered chain rule
+            grads = _backward_geom_impl(settings, None, st, tensors, radii, grad2d)
+        else:
+            lo, hi = min(lg.begin for lg in live), max(lg.end for lg in live)
+            scratch = torch.empty((3 * (hi - lo),), device=dev, dtype=torch.float32)
+            sh, colors, scales, rots, cov = (tensors[k] for k in ("sh", "colors_precomp", "scales", "rotations", "cov3Ds_precomp"))
+            e_ = lambda *shape: torch.empty(shape, device=dev, dtype=torch.float32)
+            grads = (e_(P, 3), e_(P, 3), e_(P, M, 3) if sh is not None else None, e_(P, 3) if colors is not None else None, e_(P, 1),
+                     e_(P, 3) if cov is None else None, e_(P, 4) if cov is None else None, e_(P, 6) if cov is not None else None)
+            arr = (_capi.SgrLayerGrad * len(table))(*table)
+            with torch.cuda.device(dev):
+                rc = L.sgr_backward_geom_layered(C.byref(fr), _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(scales), _ptr(rots), _ptr(cov),
+                                                 _ptr(radii), _ptr(st.geom), _ptr(grad2d), arr, len(table), _ptr(scratch),
+                                                 *(_ptr(g) for g in grads), _stream(dev))
+            _capi.check(rc, "sgr_backward_geom_layered")
+        del keep, keep_alive
+        g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rots, g_cov = grads
+        return (fit(g_means3D, 0), fit(g_means2D, 1), fit(g_sh, 2), fit(g_colors, 3), fit(g_sem if S > 0 else None, 4),
+                fit(g_opac, 5), fit(g_scales, 6), fit(g_rots, 7), fit(g_cov, 8)) + nones + tuple(sink_grads)
+
+
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, semantics, opacities, scales, rotations, cov3Ds_precomp,
                         raster_settings):
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, semantics, opacities, scales, rotations,
@@ -425,7 +585,22 @@ class GaussianRasterizer(nn.Module):
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                 cov3D_precomp=None, semantics=None):
+        return self._forward(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp, semantics, None)
+
+    def forward_layers(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
+                       cov3D_precomp=None, semantics=None, *, layers):
+        """forward() plus render layers: ``layers`` is a sequence of RenderLayer, and the result gains a 6th element holding one
+        (color[3,H,W], depth[1,H,W], alpha[1,H,W]) per layer, rendered from this call's tile lists (whole image on one GPU, default
+        and InstanceCapacity modes).  The first five elements are what forward() returns.  (forward() itself keeps the
+        reference's exact signature.)"""
+        return self._forward(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp, semantics, layers)
+
+    def _forward(self, means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp, semantics, layers):
         raster_settings = self.raster_settings
+        if layers is not None:
+            if self.band is not None or self.grad_reduce is not None:
+                raise _capi.SgrError("render layers need the whole image on one GPU (this rasterizer has a tile-row band / gradient reduction)")
+            layers = tuple(_check_layers(layers, int(means3D.shape[0])))
         if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
             raise Exception('Please provide excatly one of either SHs or precomputed colors!')
         if ((scales is None or rotations is None) and cov3D_precomp is None) or \
@@ -439,6 +614,12 @@ class GaussianRasterizer(nn.Module):
         cov3D_precomp = empty() if cov3D_precomp is None else cov3D_precomp
         if semantics is None:
             semantics = torch.zeros(means3D.shape[0], 0, dtype=torch.float32, device=means3D.device)
+        if layers is not None:
+            if not means3D.is_cuda:
+                raise _capi.SgrError("street_gaussians_b200 rasterizer needs CUDA tensors (there is no CPU fallback)")
+            out = _RasterizeLayered.apply(means3D, means2D, shs, colors_precomp, semantics, opacities, scales, rotations, cov3D_precomp,
+                                          raster_settings, self.capacity, layers, *(l[3] for l in layers))
+            return tuple(out[:5]) + (tuple(tuple(out[5 + 3 * k: 8 + 3 * k]) for k in range(len(layers))),)
         return _RasterizeGaussians.apply(means3D, means2D, shs, colors_precomp, semantics, opacities, scales, rotations,
                                          cov3D_precomp, raster_settings, self.band, self.grad_reduce, self.capacity)
 

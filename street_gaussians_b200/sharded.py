@@ -69,6 +69,9 @@ class ShardedGaussianRasterizer(GaussianRasterizer):
         super().__init__(raster_settings, band=band, grad_reduce=reduce, capacity=capacity)
         self.group, self.world, self.rank = group, world, rank
 
+    def forward_layers(self, *args, **kwargs):
+        raise _capi.SgrError("render layers are single-GPU only: use GaussianRasterizer")
+
     def gather_images(self, *images: torch.Tensor):
         """Sum the zero-padded per-band images into full frames on every rank (only needed when a full image is wanted
         on one device; the loss can be evaluated band-locally)."""
@@ -629,6 +632,9 @@ class GaussianShardedRasterizer(nn.Module):
     def synchronize_capacity(self):
         if self.capacity is not None:
             self.capacity.check(wait=True)
+
+    def forward_layers(self, *args, **kwargs):
+        raise _capi.SgrError("render layers are single-GPU only: use GaussianRasterizer")
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None,
                 semantics=None):
