@@ -156,6 +156,28 @@ static cudaError_t read_back_u32(uint32_t *dst, const uint32_t *src_dev, cudaStr
 		if (rc_ != SGR_OK) return rc_;                                  \
 	} while (0)
 
+// colour and covariance inputs of a projection: exactly one source of each, and SH coefficients only with M > 0
+static int check_gaussian_inputs(const FrameDev &f, const float *shs, const float *colors_precomp, const float *scales,
+                                 const float *rotations, const float *cov3D_precomp) {
+	if ((shs == nullptr) == (colors_precomp == nullptr)) return fail(SGR_EINVAL, "provide exactly one of shs / colors_precomp");
+	const bool sr = scales != nullptr && rotations != nullptr;
+	if (sr == (cov3D_precomp != nullptr) || ((scales != nullptr) != (rotations != nullptr)))
+		return fail(SGR_EINVAL, "provide exactly one of (scales, rotations) / cov3D_precomp");
+	if (shs && f.M <= 0) return fail(SGR_EINVAL, "shs given but M == 0");
+	return SGR_OK;
+}
+
+// pointers of the per-Gaussian chain rule; `inputs_ok` is the caller's check of its own input pointers
+static int check_geom_grads(const char *fn, bool inputs_ok, const float *shs, const float *scales, const float *rotations,
+                            const float *cov3D_precomp, const float *dL_dmeans3D, const float *dL_dmeans2D, const float *dL_dsh,
+                            const float *dL_dopacity, const float *dL_dscales, const float *dL_drotations) {
+	if (!inputs_ok || !dL_dmeans3D || !dL_dmeans2D || !dL_dopacity) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	if (shs && !dL_dsh) return fail(SGR_EINVAL, "shs given but dL_dsh is NULL");
+	if (!cov3D_precomp && (!scales || !rotations || !dL_dscales || !dL_drotations))
+		return fail(SGR_EINVAL, "scale/rotation path needs scales, rotations, dL_dscales, dL_drotations");
+	return SGR_OK;
+}
+
 }  // namespace sgr
 
 using namespace sgr;
@@ -200,11 +222,7 @@ static int forward_impl(const SgrFrame *frame, const float *means3D, const float
 		if (f.S > 0 && !semantics) return fail(SGR_EINVAL, "S > 0 but semantics is NULL");
 	} else if (f.P > 0) {
 		if (!means3D || !opacities || !radii) return fail(SGR_EINVAL, "means3D / opacities / radii is NULL");
-		if ((shs == nullptr) == (colors_precomp == nullptr)) return fail(SGR_EINVAL, "provide exactly one of shs / colors_precomp");
-		const bool sr = scales != nullptr && rotations != nullptr;
-		if (sr == (cov3D_precomp != nullptr) || ((scales != nullptr) != (rotations != nullptr)))
-			return fail(SGR_EINVAL, "provide exactly one of (scales, rotations) / cov3D_precomp");
-		if (shs && f.M <= 0) return fail(SGR_EINVAL, "shs given but M == 0");
+		if ((rc = check_gaussian_inputs(f, shs, colors_precomp, scales, rotations, cov3D_precomp)) != SGR_OK) return rc;
 		if (f.S > 0 && !semantics) return fail(SGR_EINVAL, "S > 0 but semantics is NULL");
 	}
 	const GeomView g = carve_geom(geom_state, f.P);
@@ -286,11 +304,7 @@ int sgr_project(const SgrFrame *frame, const float *means3D, const float *shs, c
 	if (f.P == 0) return SGR_OK;
 	if (!f.view || !f.proj || !f.campos) return fail(SGR_EINVAL, "camera pointer (viewmatrix/projmatrix/campos) is NULL");
 	if (!means3D || !opacities || !radii || !records) return fail(SGR_EINVAL, "means3D / opacities / radii / records is NULL");
-	if ((shs == nullptr) == (colors_precomp == nullptr)) return fail(SGR_EINVAL, "provide exactly one of shs / colors_precomp");
-	const bool sr = scales != nullptr && rotations != nullptr;
-	if (sr == (cov3D_precomp != nullptr) || ((scales != nullptr) != (rotations != nullptr)))
-		return fail(SGR_EINVAL, "provide exactly one of (scales, rotations) / cov3D_precomp");
-	if (shs && f.M <= 0) return fail(SGR_EINVAL, "shs given but M == 0");
+	if ((rc = check_gaussian_inputs(f, shs, colors_precomp, scales, rotations, cov3D_precomp)) != SGR_OK) return rc;
 	SGR_TRY(launch_project(f, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, radii,
 	                       reinterpret_cast<GaussRec *>(records), st),
 	        "project");
@@ -402,11 +416,7 @@ int sgr_sharded_forward(const SgrFrame *frame, const SgrPeers *peers, const floa
 	if (pt.chunk > 0 && (!radii_local || !records_local)) return fail(SGR_EINVAL, "radii_local / records_local is NULL");
 	if (fl.P > 0) {
 		if (!means3D || !opacities) return fail(SGR_EINVAL, "means3D / opacities is NULL");
-		if ((shs == nullptr) == (colors_precomp == nullptr)) return fail(SGR_EINVAL, "provide exactly one of shs / colors_precomp");
-		const bool sr = scales != nullptr && rotations != nullptr;
-		if (sr == (cov3D_precomp != nullptr) || ((scales != nullptr) != (rotations != nullptr)))
-			return fail(SGR_EINVAL, "provide exactly one of (scales, rotations) / cov3D_precomp");
-		if (shs && fl.M <= 0) return fail(SGR_EINVAL, "shs given but M == 0");
+		if ((rc = check_gaussian_inputs(fl, shs, colors_precomp, scales, rotations, cov3D_precomp)) != SGR_OK) return rc;
 	}
 	void *geom_state = pt.rec[pt.rank];  // this rank's gathered records ARE the head of its geom state
 	const GeomView g = carve_geom(geom_state, ft.P);
@@ -450,13 +460,9 @@ int sgr_sharded_backward(const SgrFrame *frame, const SgrPeers *peers, int64_t c
 	const bool debug = frame->debug != 0;
 	if (!img_state || !out_alpha || !dL_dcolor || !dL_ddepth || !dL_dalpha) return fail(SGR_EINVAL, "NULL pointer passed to sgr_sharded_backward");
 	if (capacity > 0 && !binning_state) return fail(SGR_EINVAL, "capacity > 0 but binning_state is NULL");
-	if (fl.P > 0) {
-		if (!means3D || !radii_local || !records_local || !dL_dmeans3D || !dL_dmeans2D || !dL_dopacity)
-			return fail(SGR_EINVAL, "NULL pointer passed to sgr_sharded_backward");
-		if (shs && !dL_dsh) return fail(SGR_EINVAL, "shs given but dL_dsh is NULL");
-		if (!cov3D_precomp && (!scales || !rotations || !dL_dscales || !dL_drotations))
-			return fail(SGR_EINVAL, "scale/rotation path needs scales, rotations, dL_dscales, dL_drotations");
-	}
+	if (fl.P > 0 && (rc = check_geom_grads("sgr_sharded_backward", means3D && radii_local && records_local, shs, scales, rotations, cov3D_precomp,
+	                                       dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dopacity, dL_dscales, dL_drotations)) != SGR_OK)
+		return rc;
 	const GeomView g = carve_geom(pt.rec[pt.rank], ft.P);
 	const ImgView img = carve_img(const_cast<void *>(img_state), ft.W, ft.H);
 	const BinView b = carve_bin(const_cast<void *>(binning_state), capacity);
@@ -519,28 +525,55 @@ int sgr_backward_blend(const SgrFrame *frame, int64_t num_instances, const float
 	return SGR_OK;
 }
 
-int sgr_backward_geom(const SgrFrame *frame, const float *means3D, const float *shs, const float *colors_precomp,
-                      const float *scales, const float *rotations, const float *cov3D_precomp, const int32_t *radii,
-                      const void *geom_state, const float *grad2d, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh,
-                      float *dL_dcolors_precomp, float *dL_dopacity, float *dL_dscales, float *dL_drotations,
-                      float *dL_dcov3D, void *stream) {
+// shared body of sgr_backward_geom (no layer table) and sgr_backward_geom_layered; `fn` names the entry point in error messages.
+// With a live layer (grad2d set, non-empty range) the layers' rows are merged into grad2d before the chain rule, and the main
+// dL_dmeans2D of their range is restored from the pre-merge rows afterwards.
+static int backward_geom(const char *fn, const SgrFrame *frame, const float *means3D, const float *shs, const float *colors_precomp,
+                         const float *scales, const float *rotations, const float *cov3D_precomp, const int32_t *radii,
+                         const void *geom_state, float *grad2d, const SgrLayerGrad *layers, int32_t num_layers, float *scratch,
+                         float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors_precomp, float *dL_dopacity,
+                         float *dL_dscales, float *dL_drotations, float *dL_dcov3D, void *stream) {
 	FrameDev f;
 	int rc = make_frame(frame, f);
 	if (rc) return rc;
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 	const bool debug = frame->debug != 0;
+	if (num_layers < 0 || (num_layers > 0 && !layers)) return fail(SGR_EINVAL, "bad layer table");
+	int lo = 0x7fffffff, hi = 0;
+	for (int k = 0; k < num_layers; k++) {
+		const SgrLayerGrad &l = layers[k];
+		if (l.begin < 0 || l.begin > l.end || l.end > f.P) return fail(SGR_EINVAL, "bad layer %d range [%d, %d) for P = %d", k, l.begin, l.end, f.P);
+		if (!l.grad2d || l.end == l.begin) continue;
+		lo = l.begin < lo ? l.begin : lo;
+		hi = l.end > hi ? l.end : hi;
+	}
 	if (f.P == 0) return SGR_OK;
-	if (!means3D || !radii || !geom_state || !grad2d || !dL_dmeans3D || !dL_dmeans2D || !dL_dopacity)
-		return fail(SGR_EINVAL, "NULL pointer passed to sgr_backward_geom");
-	if (shs && !dL_dsh) return fail(SGR_EINVAL, "shs given but dL_dsh is NULL");
-	if (!cov3D_precomp && (!scales || !rotations || !dL_dscales || !dL_drotations))
-		return fail(SGR_EINVAL, "scale/rotation path needs scales, rotations, dL_dscales, dL_drotations");
+	if ((rc = check_geom_grads(fn, means3D && radii && geom_state && grad2d, shs, scales, rotations, cov3D_precomp, dL_dmeans3D,
+	                           dL_dmeans2D, dL_dsh, dL_dopacity, dL_dscales, dL_drotations)) != SGR_OK)
+		return rc;
+	if (hi > lo && !scratch) return fail(SGR_EINVAL, "scratch is NULL");
 	const GeomView g = carve_geom(const_cast<void *>(geom_state), f.P);
+	if (hi > lo) {
+		SGR_TRY(launch_layer_stash(grad2d, lo, hi, scratch, false, nullptr, st), "layer stash");
+		SGR_TRY(launch_layer_merge(grad2d, layers, num_layers, st), "layer merge");
+	}
 	SGR_TRY(launch_preprocess_bwd(f, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii, g, grad2d, dL_dmeans3D,
 	                              dL_dmeans2D, shs ? dL_dsh : nullptr, dL_dcolors_precomp, dL_dopacity,
 	                              cov3D_precomp ? nullptr : dL_dscales, cov3D_precomp ? nullptr : dL_drotations, dL_dcov3D, st),
 	        "preprocess_bwd");
+	if (hi > lo) SGR_TRY(launch_layer_stash(grad2d, lo, hi, scratch, true, dL_dmeans2D, st), "layer restore");
 	return SGR_OK;
+}
+
+int sgr_backward_geom(const SgrFrame *frame, const float *means3D, const float *shs, const float *colors_precomp,
+                      const float *scales, const float *rotations, const float *cov3D_precomp, const int32_t *radii,
+                      const void *geom_state, const float *grad2d, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh,
+                      float *dL_dcolors_precomp, float *dL_dopacity, float *dL_dscales, float *dL_drotations,
+                      float *dL_dcov3D, void *stream) {
+	// without layers grad2d is only read
+	return backward_geom("sgr_backward_geom", frame, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii, geom_state,
+	                     const_cast<float *>(grad2d), nullptr, 0, nullptr, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors_precomp, dL_dopacity,
+	                     dL_dscales, dL_drotations, dL_dcov3D, stream);
 }
 
 int sgr_backward(const SgrFrame *frame, int64_t num_instances, const float *means3D, const float *shs,
@@ -653,36 +686,9 @@ int sgr_backward_geom_layered(const SgrFrame *frame, const float *means3D, const
                               const void *geom_state, float *grad2d, const SgrLayerGrad *layers, int32_t num_layers, float *scratch,
                               float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors_precomp, float *dL_dopacity,
                               float *dL_dscales, float *dL_drotations, float *dL_dcov3D, void *stream) {
-	FrameDev f;
-	int rc = make_frame(frame, f);
-	if (rc) return rc;
-	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-	const bool debug = frame->debug != 0;
-	if (num_layers < 0 || (num_layers > 0 && !layers)) return fail(SGR_EINVAL, "bad layer table");
-	int lo = 0x7fffffff, hi = 0;
-	for (int k = 0; k < num_layers; k++) {
-		const SgrLayerGrad &l = layers[k];
-		if (l.begin < 0 || l.begin > l.end || l.end > f.P) return fail(SGR_EINVAL, "bad layer %d range [%d, %d) for P = %d", k, l.begin, l.end, f.P);
-		if (!l.grad2d || l.end == l.begin) continue;
-		lo = l.begin < lo ? l.begin : lo;
-		hi = l.end > hi ? l.end : hi;
-	}
-	if (f.P == 0) return SGR_OK;
-	if (!means3D || !radii || !geom_state || !grad2d || !dL_dmeans3D || !dL_dmeans2D || !dL_dopacity)
-		return fail(SGR_EINVAL, "NULL pointer passed to sgr_backward_geom_layered");
-	if (shs && !dL_dsh) return fail(SGR_EINVAL, "shs given but dL_dsh is NULL");
-	if (!cov3D_precomp && (!scales || !rotations || !dL_dscales || !dL_drotations))
-		return fail(SGR_EINVAL, "scale/rotation path needs scales, rotations, dL_dscales, dL_drotations");
-	if (hi > lo && !scratch) return fail(SGR_EINVAL, "scratch is NULL");
-	const GeomView g = carve_geom(const_cast<void *>(geom_state), f.P);
-	SGR_TRY(launch_layer_stash(grad2d, lo, hi, scratch, false, nullptr, st), "layer stash");
-	SGR_TRY(launch_layer_merge(grad2d, layers, num_layers, st), "layer merge");
-	SGR_TRY(launch_preprocess_bwd(f, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii, g, grad2d, dL_dmeans3D,
-	                              dL_dmeans2D, shs ? dL_dsh : nullptr, dL_dcolors_precomp, dL_dopacity,
-	                              cov3D_precomp ? nullptr : dL_dscales, cov3D_precomp ? nullptr : dL_drotations, dL_dcov3D, st),
-	        "preprocess_bwd");
-	SGR_TRY(launch_layer_stash(grad2d, lo, hi, scratch, true, dL_dmeans2D, st), "layer restore");
-	return SGR_OK;
+	return backward_geom("sgr_backward_geom_layered", frame, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii,
+	                     geom_state, grad2d, layers, num_layers, scratch, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors_precomp, dL_dopacity,
+	                     dL_dscales, dL_drotations, dL_dcov3D, stream);
 }
 
 int sgr_mark_visible(int32_t P, const float *means3D, const float *viewmatrix, const float *projmatrix, uint8_t *present,

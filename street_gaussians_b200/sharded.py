@@ -31,8 +31,9 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from . import _capi
-from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, InstanceCapacity, TileRowBand, _ForwardState,
-                         _backward_blend_impl, _backward_geom_impl, _dev_f32, _make_frame, _none_if_empty, _ptr, _stream)
+from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, InstanceCapacity, TileRowBand, _copy_status, _ForwardState,
+                         _backward_blend_impl, _backward_geom_impl, _dev_f32, _fit_grads, _fp32_inputs, _geom_grad_buffers, _image_grads,
+                         _input_shapes, _make_frame, _ptr, _reference_inputs, _stream)
 
 
 def cyclic_band(image_height: int, rank: int, world: int) -> TileRowBand:
@@ -108,19 +109,7 @@ def chunk_size(P_local: int, group=None) -> int:
     return int(t.item())
 
 
-def _local_tensors(means3D, sh, colors_precomp, semantics, opacities, scales, rotations, cov3Ds_precomp):
-    if means3D.dim() != 2 or means3D.shape[1] != 3:
-        raise RuntimeError("means3D must have dimensions (num_points, 3)")
-    if not means3D.is_cuda:
-        raise _capi.SgrError("street_gaussians_b200 rasterizer needs CUDA tensors (there is no CPU fallback)")
-    device = means3D.device
-    S = int(semantics.shape[1]) if (semantics is not None and semantics.dim() == 2) else 0
-    tensors = dict(means3D=_dev_f32(means3D, device), opacities=_dev_f32(opacities, device))
-    for name, t in (("sh", _none_if_empty(sh)), ("colors_precomp", _none_if_empty(colors_precomp)), ("scales", _none_if_empty(scales)),
-                    ("rotations", _none_if_empty(rotations)), ("cov3Ds_precomp", _none_if_empty(cov3Ds_precomp)),
-                    ("semantics", semantics if S > 0 else None)):
-        tensors[name] = _dev_f32(t, device) if t is not None else None
-    return tensors
+_local_tensors = _fp32_inputs  # step 0: the local Gaussians as the kernels read them
 
 
 def project_records(tensors, settings: GaussianRasterizationSettings, chunk: int):
@@ -193,12 +182,7 @@ def forward_records(settings: GaussianRasterizationSettings, band: Optional[Tile
                                    _ptr(st.binning) if bounded else None, nbytes, cap, _stream(device))
         _capi.check(rc, "sgr_forward_records")
         if bounded:
-            host_status = capacity.status_word()
-            rc = L.sgr_forward_status_async(C.byref(fr), _ptr(st.geom), C.c_void_p(host_status.data_ptr()), _stream(device))
-            _capi.check(rc, "sgr_forward_status_async")
-            ev = torch.cuda.Event()
-            ev.record(torch.cuda.current_stream(device))
-            capacity.track(host_status, ev)
+            capacity.record_status(fr, st.geom, device)
             st.num_instances = cap
         else:
             st.num_instances = int(n_inst.value)
@@ -399,8 +383,7 @@ class _GaussianShardedRasterize(torch.autograd.Function):
         color, depth, alpha, semantic = forward_records(settings, owner.band, st, (gb, ib), radii_all, sem_all, owner.capacity)
         ctx.settings, ctx.owner, ctx.state, ctx.tensors = settings, owner, st, tensors
         ctx.sem_all, ctx.P_total, ctx.chunk, ctx.ws = sem_all, P_total, chunk, ws
-        ctx.shapes = tuple(None if t is None else (tuple(t.shape), t.device, t.dtype)
-                           for t in (means3D, means2D, sh, colors_precomp, semantics, opacities, scales, rotations, cov3Ds_precomp))
+        ctx.shapes = _input_shapes(means3D, means2D, sh, colors_precomp, semantics, opacities, scales, rotations, cov3Ds_precomp)
         ctx.save_for_backward(rec, radii, alpha)
         radii_out = radii[:P]
         ctx.mark_non_differentiable(radii_out)
@@ -415,14 +398,10 @@ class _GaussianShardedRasterize(torch.autograd.Function):
         rec, radii, alpha = ctx.saved_tensors
         settings, owner, st, tensors, shapes = ctx.settings, ctx.owner, ctx.state, ctx.tensors, ctx.shapes
         dev = alpha.device
-        H, W = int(settings.image_height), int(settings.image_width)
         S = int(ctx.sem_all.shape[1]) if ctx.sem_all is not None else 0
         P = int(tensors["means3D"].shape[0])
-        zimg = lambda c: torch.zeros((c, H, W), device=dev, dtype=torch.float32)
-        grad_color = grad_color if grad_color is not None else zimg(3)
-        grad_depth = grad_depth if grad_depth is not None else zimg(1)
-        grad_alpha = grad_alpha if grad_alpha is not None else zimg(1)
-        grad_semantic = grad_semantic if grad_semantic is not None else zimg(S)
+        grad_color, grad_depth, grad_alpha, grad_semantic = _image_grads(settings, dev, (grad_color, grad_depth, grad_alpha, grad_semantic),
+                                                                         (3, 1, 1, S))
         ws = ctx.ws
         grad2d, g_sem = backward_blend_records(settings, owner.band, st, ctx.P_total, ctx.sem_all, alpha, grad_color, grad_depth,
                                                grad_alpha, grad_semantic, grad2d_out=ws.grad2d if ws is not None else None)
@@ -448,17 +427,8 @@ class _GaussianShardedRasterize(torch.autograd.Function):
         else:
             g = backward_geom_local(settings, tensors, rec, radii, grad2d)
         g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rots, g_cov = g
-
-        def fit(t, i):
-            if shapes[i] is None:
-                return None
-            shape, device, dtype = shapes[i]
-            if t is None:
-                return torch.zeros(shape, device=device, dtype=dtype)
-            return t.reshape(shape).to(device=device, dtype=dtype)
-
-        return (fit(g_means3D, 0), fit(g_means2D, 1), fit(g_sh, 2), fit(g_colors, 3), fit(g_sem[:P] if S > 0 else None, 4),
-                fit(g_opac, 5), fit(g_scales, 6), fit(g_rots, 7), fit(g_cov, 8), None, None, None)
+        return _fit_grads(shapes, (g_means3D, g_means2D, g_sh, g_colors, g_sem[:P] if S > 0 else None, g_opac, g_scales, g_rots,
+                                   g_cov)) + (None, None, None)
 
 
 def sharded_forward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, capacity: int, gaussian_capacity: int, status_word=None):
@@ -483,10 +453,9 @@ def sharded_forward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, ca
                                    _ptr(bufs["img"]), ws.img_bytes, _ptr(bufs["binning"]), nbytes, capacity, gaussian_capacity, epoch, pre,
                                    _stream(device))
         _capi.check(rc, "sgr_sharded_forward")
-        if status_word is not None:
+        if status_word is not None:  # the status of the gathered frame (P_total slots)
             frt, keep2 = _make_frame(settings, ws.P_total, 0, 0, device, band)
-            rc = L.sgr_forward_status_async(C.byref(frt), _ptr(ws.geom), C.c_void_p(status_word.data_ptr()), _stream(device))
-            _capi.check(rc, "sgr_forward_status_async")
+            _copy_status(frt, ws.geom, status_word, device)
             del keep2
     del keep
     ws.fwd_pending = True
@@ -499,13 +468,7 @@ def sharded_backward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, c
     dev = alpha.device
     sh, colors, scales, rots, cov = (tensors[k] for k in ("sh", "colors_precomp", "scales", "rotations", "cov3Ds_precomp"))
     M = int(sh.shape[1]) if sh is not None else 0
-    e = lambda *shape: torch.empty(shape, device=dev, dtype=torch.float32)
-    g_means3D, g_means2D, g_opac = e(P, 3), e(P, 3), e(P, 1)
-    g_sh = e(P, M, 3) if sh is not None else None
-    g_colors = e(P, 3) if colors is not None else None
-    g_scales = e(P, 3) if cov is None else None
-    g_rots = e(P, 4) if cov is None else None
-    g_cov = e(P, 6) if cov is not None else None
+    g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rots, g_cov = _geom_grad_buffers(tensors, P, dev)
     bufs = ws.step_buffers(0)
     fr, keep = _make_frame(settings, P, M, 0, dev, band)
     ws.next_epochs(1)
@@ -534,15 +497,14 @@ def _fused_forward(ctx, tensors, settings, owner, ws: "PeerWorkspace", P: int, c
     capacity = int(cap.capacity)
     # depth-order slots: learnt from the previous frames (status word 4); the first fused frame compacts into all slots
     gcap = int(cap.gaussian_capacity) if cap.gaussian_capacity is not None else ws.P_total
-    host_status = None if cap.frozen else cap.status_word()
-    color, depth, alpha, bufs = sharded_forward_raw(settings, owner.band, ws, tensors, P, capacity, gcap, host_status)
-    if host_status is not None:
-        ev = torch.cuda.Event()
-        ev.record(torch.cuda.current_stream(device))
-        cap.track(host_status, ev)
+    color, depth, alpha, bufs = sharded_forward_raw(settings, owner.band, ws, tensors, P, capacity, gcap)
+    if not cap.frozen:  # the status of the gathered frame (P_total slots)
+        frt, keep = _make_frame(settings, ws.P_total, 0, 0, device, owner.band)
+        cap.record_status(frt, ws.geom, device)
+        del keep
     ws.in_flight = bool(differentiable)
     ctx.fused, ctx.settings, ctx.owner, ctx.ws, ctx.P, ctx.capacity, ctx.tensors = True, settings, owner, ws, P, capacity, tensors
-    ctx.shapes = tuple(None if t is None else (tuple(t.shape), t.device, t.dtype) for t in inputs)
+    ctx.shapes = _input_shapes(*inputs)
     ctx.save_for_backward(alpha)
     radii_out = bufs["radii"][:P]
     ctx.mark_non_differentiable(radii_out)
@@ -554,25 +516,11 @@ def _fused_backward(ctx, grad_color, grad_depth, grad_alpha):
     (alpha,) = ctx.saved_tensors
     settings, owner, ws, P, tensors, shapes = ctx.settings, ctx.owner, ctx.ws, ctx.P, ctx.tensors, ctx.shapes
     dev = alpha.device
-    H, W = int(settings.image_height), int(settings.image_width)
-    zimg = lambda c: torch.zeros((c, H, W), device=dev, dtype=torch.float32)
-    gc = _dev_f32(grad_color, dev) if grad_color is not None else zimg(3)
-    gd = _dev_f32(grad_depth, dev) if grad_depth is not None else zimg(1)
-    ga = _dev_f32(grad_alpha, dev) if grad_alpha is not None else zimg(1)
+    gc, gd, ga = (_dev_f32(g, dev) for g in _image_grads(settings, dev, (grad_color, grad_depth, grad_alpha), (3, 1, 1)))
     g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rots, g_cov = sharded_backward_raw(settings, owner.band, ws, tensors, P,
                                                                                                    ctx.capacity, alpha, gc, gd, ga)
     ws.in_flight = False
-
-    def fit(t, i):
-        if shapes[i] is None:
-            return None
-        shape, device, dtype = shapes[i]
-        if t is None:
-            return torch.zeros(shape, device=device, dtype=dtype)
-        return t.reshape(shape).to(device=device, dtype=dtype)
-
-    return (fit(g_means3D, 0), fit(g_means2D, 1), fit(g_sh, 2), fit(g_colors, 3), fit(None, 4), fit(g_opac, 5), fit(g_scales, 6),
-            fit(g_rots, 7), fit(g_cov, 8), None, None, None)
+    return _fit_grads(shapes, (g_means3D, g_means2D, g_sh, g_colors, None, g_opac, g_scales, g_rots, g_cov)) + (None, None, None)
 
 
 class GaussianShardedRasterizer(nn.Module):
@@ -638,19 +586,8 @@ class GaussianShardedRasterizer(nn.Module):
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None,
                 semantics=None):
-        if (shs is None) == (colors_precomp is None):
-            raise Exception('Please provide excatly one of either SHs or precomputed colors!')
-        if ((scales is None or rotations is None) and cov3D_precomp is None) or \
-                ((scales is not None or rotations is not None) and cov3D_precomp is not None):
-            raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
-        e = torch.Tensor([])
-        shs = e if shs is None else shs
-        colors_precomp = e if colors_precomp is None else colors_precomp
-        scales = e if scales is None else scales
-        rotations = e if rotations is None else rotations
-        cov3D_precomp = e if cov3D_precomp is None else cov3D_precomp
-        if semantics is None:
-            semantics = torch.zeros((means3D.shape[0], 0), device=means3D.device)
+        shs, colors_precomp, scales, rotations, cov3D_precomp, semantics = _reference_inputs(means3D, shs, colors_precomp, scales, rotations,
+                                                                                             cov3D_precomp, semantics)
         args = (means3D, means2D, shs, colors_precomp, semantics, opacities, scales, rotations, cov3D_precomp)
         differentiable = torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in args)
         return _GaussianShardedRasterize.apply(*args, self.raster_settings, self, differentiable)
