@@ -470,10 +470,10 @@ int sgr_sharded_backward(const SgrFrame *frame, const SgrPeers *peers, int64_t c
 	if (ft.P > 0)
 		SGR_TRY(launch_blend_bwd(ft, g, b, img, nullptr, out_alpha, dL_dcolor, dL_ddepth, dL_dalpha, nullptr, grad2d, nullptr, st, true), "blend_bwd");
 	SGR_TRY(launch_peer_barrier(pt, barrier_epoch, ft.P > 0 ? g.big_count : nullptr, st), "barrier");
-	SGR_TRY(launch_preprocess_bwd_gather(fl, pt, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii_local,
-	                                     reinterpret_cast<const GaussRec *>(records_local), dL_dmeans3D, dL_dmeans2D, shs ? dL_dsh : nullptr,
-	                                     dL_dcolors_precomp, dL_dopacity, cov3D_precomp ? nullptr : dL_dscales,
-	                                     cov3D_precomp ? nullptr : dL_drotations, dL_dcov3D, g.depth_key, st),
+	SGR_TRY(launch_preprocess_bwd(fl, &pt, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii_local,
+	                              reinterpret_cast<const GaussRec *>(records_local), reinterpret_cast<const float *>(g.depth_key), dL_dmeans3D,
+	                              dL_dmeans2D, shs ? dL_dsh : nullptr, dL_dcolors_precomp, dL_dopacity, cov3D_precomp ? nullptr : dL_dscales,
+	                              cov3D_precomp ? nullptr : dL_drotations, dL_dcov3D, st),
 	        "preprocess_bwd+gather");
 	return SGR_OK;
 }
@@ -557,7 +557,7 @@ static int backward_geom(const char *fn, const SgrFrame *frame, const float *mea
 		SGR_TRY(launch_layer_stash(grad2d, lo, hi, scratch, false, nullptr, st), "layer stash");
 		SGR_TRY(launch_layer_merge(grad2d, layers, num_layers, st), "layer merge");
 	}
-	SGR_TRY(launch_preprocess_bwd(f, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii, g, grad2d, dL_dmeans3D,
+	SGR_TRY(launch_preprocess_bwd(f, nullptr, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii, g.rec, grad2d, dL_dmeans3D,
 	                              dL_dmeans2D, shs ? dL_dsh : nullptr, dL_dcolors_precomp, dL_dopacity,
 	                              cov3D_precomp ? nullptr : dL_dscales, cov3D_precomp ? nullptr : dL_drotations, dL_dcov3D, st),
 	        "preprocess_bwd");

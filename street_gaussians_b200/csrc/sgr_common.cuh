@@ -325,13 +325,6 @@ cudaError_t launch_project_scatter(const FrameDev &f, const PeerTable &pt, const
                                    const float *colors_precomp, const float *opacities, const float *scales, const float *rotations,
                                    const float *cov3D_precomp, int32_t *radii_local, GaussRec *rec_local, uint32_t *masks_local,
                                    size_t cnt_offset, cudaStream_t st);
-// sgr_gather_grad2d fused into sgr_backward_geom: the 12 screen-space sums of each local Gaussian are summed from the ranks
-// that rendered it while the chain rule runs
-cudaError_t launch_preprocess_bwd_gather(const FrameDev &f, const PeerTable &pt, const float *means3D, const float *shs,
-                                         const float *colors_precomp, const float *scales, const float *rotations,
-                                         const float *cov3D_precomp, const int32_t *radii, const GaussRec *rec, float *dL_dmeans3D,
-                                         float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity, float *dL_dscales,
-                                         float *dL_drot, float *dL_dcov3D, const uint32_t *masks_local, cudaStream_t st);
 cudaError_t launch_scatter_records(const FrameDev &f, const PeerTable &pt, const GaussRec *rec, const int32_t *radii, cudaStream_t st);
 cudaError_t launch_gather_grad2d(const FrameDev &f, const PeerTable &pt, const GaussRec *rec, const int32_t *radii, float *out,
                                  cudaStream_t st);
@@ -350,11 +343,13 @@ cudaError_t launch_blend_bwd(const FrameDev &f, GeomView g, BinView b, ImgView i
                              const float *dL_dsem, float *grad2d, float *dL_dsemantics, cudaStream_t st, bool grad2d_zeroed = false);
 cudaError_t launch_blend_bwd2(const FrameDev &f, GeomView g, BinView b, ImgView img, const float *out_alpha, const float *dL_dcolor,
                               const float *dL_ddepth, const float *dL_dalpha, float *grad2d, cudaStream_t st, bool grad2d_zeroed = false);
-cudaError_t launch_preprocess_bwd(const FrameDev &f, const float *means3D, const float *shs, const float *colors_precomp,
-                                  const float *scales, const float *rotations, const float *cov3D_precomp,
-                                  const int32_t *radii, GeomView g, const float *grad2d, float *dL_dmeans3D,
-                                  float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors, float *dL_dopacity,
-                                  float *dL_dscales, float *dL_drot, float *dL_dcov3D, cudaStream_t st);
+// pt == nullptr: grad2d holds the f.P x 12 screen-space sums of this process.  With a peer table (sgr_sharded_backward, with
+// sgr_gather_grad2d fused in) the sums of each local Gaussian are summed from the ranks that rendered it while the chain rule runs,
+// and grad2d carries instead the destination masks (u32[f.P]) the forward stored.
+cudaError_t launch_preprocess_bwd(const FrameDev &f, const PeerTable *pt, const float *means3D, const float *shs, const float *colors_precomp,
+                                  const float *scales, const float *rotations, const float *cov3D_precomp, const int32_t *radii,
+                                  const GaussRec *rec, const float *grad2d, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh,
+                                  float *dL_dcolors, float *dL_dopacity, float *dL_dscales, float *dL_drot, float *dL_dcov3D, cudaStream_t st);
 // render layers (layers.cu)
 cudaError_t launch_layer_lists(const FrameDev &f, ImgView main_img, BinView main_bin, int begin, int end, ImgView layer_img, uint32_t *layer_list,
                                cudaStream_t st);

@@ -95,7 +95,7 @@ def _single(scene, st, band=None, semantics=None):
 
 
 def gather_variant(lt, g_sh, no_tma):
-    """Which kernel launch_preprocess_bwd_gather runs (bwd_rows_fit_tma restated): TMA rows for M in {4, 8, 12, 16} with 16-B aligned
+    """Which kernel launch_preprocess_bwd runs with a peer table (bwd_rows_fit_tma restated): TMA rows for M in {4, 8, 12, 16} with 16-B aligned
     SH in / out, the staged kernel for the other M <= 16 (and under SGR_NO_TMA), the unstaged one without SH (colors_precomp)."""
     sh = lt["sh"]
     if sh is None:
