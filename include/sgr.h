@@ -13,6 +13,11 @@
  *    (DGR/diff_gaussian_rasterization/__init__.py:197-233): means3D[P,3], shs[P,M,3], colors_precomp[P,3],
  *    semantics[P,S], opacities[P,1], scales[P,3], rotations[P,4] (w,x,y,z), cov3D_precomp[P,6],
  *    images [C,H,W].  A NULL pointer plays the role of the reference's empty tensor.
+ *  - shs, rotations and their gradients dL_dsh, dL_drotations must be 16-byte aligned (the kernels move those rows with
+ *    16-byte vector accesses); every entry point that takes them returns SGR_EINVAL otherwise.  A fresh allocation is;
+ *    a view at an odd float offset into a larger buffer may not be.
+ *  - with shs, M >= (D + 1)^2: the active degree never evaluates coefficients that are not stored (SGR_EINVAL otherwise;
+ *    the reference reads past the row).  Coefficients beyond (D + 1)^2 are never read and get zero gradient.
  *  - the CALLER owns all memory, including the forward->backward state buffers and scratch; the library is
  *    stateless between calls, re-entrant and thread-safe; every kernel is enqueued on `stream` (a cudaStream_t
  *    passed as void*).  The only host synchronisations are one 8-byte read-back of the instance count inside

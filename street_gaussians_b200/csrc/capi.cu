@@ -156,7 +156,15 @@ static cudaError_t read_back_u32(uint32_t *dst, const uint32_t *src_dev, cudaStr
 		if (rc_ != SGR_OK) return rc_;                                  \
 	} while (0)
 
-// colour and covariance inputs of a projection: exactly one source of each, and SH coefficients only with M > 0
+// The kernels read rotation rows and SH rows with 16-B vector loads (and store their gradients so); a pointer into the middle of
+// a larger buffer can break that alignment, which faults on the device.  NULL passes.
+static int check_aligned16(const char *what, const void *p) {
+	if ((reinterpret_cast<uintptr_t>(p) & 15u) != 0) return fail(SGR_EINVAL, "%s is not 16-byte aligned (%p)", what, p);
+	return SGR_OK;
+}
+
+// colour and covariance inputs of a projection: exactly one source of each, SH coefficients only with M > 0 and at least the
+// (D + 1)^2 the active degree evaluates, and the rows read as float4 aligned
 static int check_gaussian_inputs(const FrameDev &f, const float *shs, const float *colors_precomp, const float *scales,
                                  const float *rotations, const float *cov3D_precomp) {
 	if ((shs == nullptr) == (colors_precomp == nullptr)) return fail(SGR_EINVAL, "provide exactly one of shs / colors_precomp");
@@ -164,17 +172,27 @@ static int check_gaussian_inputs(const FrameDev &f, const float *shs, const floa
 	if (sr == (cov3D_precomp != nullptr) || ((scales != nullptr) != (rotations != nullptr)))
 		return fail(SGR_EINVAL, "provide exactly one of (scales, rotations) / cov3D_precomp");
 	if (shs && f.M <= 0) return fail(SGR_EINVAL, "shs given but M == 0");
-	return SGR_OK;
+	if (shs && f.M < (f.D + 1) * (f.D + 1))
+		return fail(SGR_EINVAL, "SH degree %d needs %d coefficients per Gaussian, shs has M = %d", f.D, (f.D + 1) * (f.D + 1), f.M);
+	int rc;
+	if ((rc = check_aligned16("shs", shs)) != SGR_OK) return rc;
+	return check_aligned16("rotations", rotations);
 }
 
 // pointers of the per-Gaussian chain rule; `inputs_ok` is the caller's check of its own input pointers
-static int check_geom_grads(const char *fn, bool inputs_ok, const float *shs, const float *scales, const float *rotations,
+static int check_geom_grads(const char *fn, const FrameDev &f, bool inputs_ok, const float *shs, const float *scales, const float *rotations,
                             const float *cov3D_precomp, const float *dL_dmeans3D, const float *dL_dmeans2D, const float *dL_dsh,
                             const float *dL_dopacity, const float *dL_dscales, const float *dL_drotations) {
 	if (!inputs_ok || !dL_dmeans3D || !dL_dmeans2D || !dL_dopacity) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
 	if (shs && !dL_dsh) return fail(SGR_EINVAL, "shs given but dL_dsh is NULL");
 	if (!cov3D_precomp && (!scales || !rotations || !dL_dscales || !dL_drotations))
 		return fail(SGR_EINVAL, "scale/rotation path needs scales, rotations, dL_dscales, dL_drotations");
+	if (shs && f.M < (f.D + 1) * (f.D + 1))
+		return fail(SGR_EINVAL, "SH degree %d needs %d coefficients per Gaussian, shs has M = %d", f.D, (f.D + 1) * (f.D + 1), f.M);
+	int rc;
+	if ((rc = check_aligned16("shs", shs)) != SGR_OK || (rc = check_aligned16("rotations", rotations)) != SGR_OK) return rc;
+	if (shs && (rc = check_aligned16("dL_dsh", dL_dsh)) != SGR_OK) return rc;
+	if (!cov3D_precomp && (rc = check_aligned16("dL_drotations", dL_drotations)) != SGR_OK) return rc;
 	return SGR_OK;
 }
 
@@ -460,7 +478,7 @@ int sgr_sharded_backward(const SgrFrame *frame, const SgrPeers *peers, int64_t c
 	const bool debug = frame->debug != 0;
 	if (!img_state || !out_alpha || !dL_dcolor || !dL_ddepth || !dL_dalpha) return fail(SGR_EINVAL, "NULL pointer passed to sgr_sharded_backward");
 	if (capacity > 0 && !binning_state) return fail(SGR_EINVAL, "capacity > 0 but binning_state is NULL");
-	if (fl.P > 0 && (rc = check_geom_grads("sgr_sharded_backward", means3D && radii_local && records_local, shs, scales, rotations, cov3D_precomp,
+	if (fl.P > 0 && (rc = check_geom_grads("sgr_sharded_backward", fl, means3D && radii_local && records_local, shs, scales, rotations, cov3D_precomp,
 	                                       dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dopacity, dL_dscales, dL_drotations)) != SGR_OK)
 		return rc;
 	const GeomView g = carve_geom(pt.rec[pt.rank], ft.P);
@@ -548,7 +566,7 @@ static int backward_geom(const char *fn, const SgrFrame *frame, const float *mea
 		hi = l.end > hi ? l.end : hi;
 	}
 	if (f.P == 0) return SGR_OK;
-	if ((rc = check_geom_grads(fn, means3D && radii && geom_state && grad2d, shs, scales, rotations, cov3D_precomp, dL_dmeans3D,
+	if ((rc = check_geom_grads(fn, f, means3D && radii && geom_state && grad2d, shs, scales, rotations, cov3D_precomp, dL_dmeans3D,
 	                           dL_dmeans2D, dL_dsh, dL_dopacity, dL_dscales, dL_drotations)) != SGR_OK)
 		return rc;
 	if (hi > lo && !scratch) return fail(SGR_EINVAL, "scratch is NULL");
@@ -713,6 +731,7 @@ int sgr_visible_filter(const SgrFrame *frame, const float *means3D, const float 
 	if (f.P == 0) return SGR_OK;
 	if (!means3D || !radii || !means2D || !f.view || !f.proj) return fail(SGR_EINVAL, "NULL pointer passed to sgr_visible_filter");
 	if (!cov3D_precomp && (!scales || !rotations)) return fail(SGR_EINVAL, "provide (scales, rotations) or cov3D_precomp");
+	if ((rc = check_aligned16("rotations", cov3D_precomp ? nullptr : rotations)) != SGR_OK) return rc;
 	SGR_TRY(launch_filter(f, means3D, scales, rotations, cov3D_precomp, radii, means2D, st), "visible_filter");
 	return SGR_OK;
 }

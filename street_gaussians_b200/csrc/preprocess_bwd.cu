@@ -442,9 +442,12 @@ __global__ void __launch_bounds__(256, 3) preprocess_bwd_tma_kernel(
 #pragma unroll
 				for (int tt = 0; tt < 4; tt++) {
 					const int e = 4 * j + tt, k = e / 3, ch = e % 3;  // compile-time after unrolling
-					const float cg = cv[tt] * dRGB[ch];
+					// coefficients beyond the active degree are never read (a NaN or Inf stored there must not reach dL/dmean3D)
+					// and get +0 (B[k] = 0 times a negative dL/dRGB would store -0)
+					const bool active = k < ncoef;
+					const float cg = active ? cv[tt] * dRGB[ch] : 0.f;
 					ddx += Bx[k] * cg; ddy += By[k] * cg; ddz += Bz[k] * cg;
-					o[tt] = B[k] * dRGB[ch];
+					o[tt] = active ? B[k] * dRGB[ch] : 0.f;
 				}
 				asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(row + 16u * j), "f"(o[0]), "f"(o[1]), "f"(o[2]), "f"(o[3]) : "memory");
 			}

@@ -52,10 +52,13 @@ def _ptr(t: Optional[torch.Tensor]):
 
 
 def _dev_f32(t: torch.Tensor, device) -> torch.Tensor:
-    """contiguous fp32 on `device` (the reference calls .contiguous() on every argument, DGR/rasterize_points.cu:92-118)."""
+    """contiguous fp32 on `device` (the reference calls .contiguous() on every argument, DGR/rasterize_points.cu:92-118), at a
+    16-byte aligned address: a contiguous view keeps its storage offset (a slice of a flat parameter buffer), and the library
+    reads rotation and SH rows with 16-byte loads (include/sgr.h).  Such a view is copied."""
     if t.device != device or t.dtype != torch.float32:
         t = t.to(device=device, dtype=torch.float32)
-    return t.contiguous()
+    t = t.contiguous()
+    return t.clone() if t.data_ptr() % 16 else t
 
 
 def _none_if_empty(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:

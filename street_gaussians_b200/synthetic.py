@@ -25,14 +25,41 @@ def projection_matrix(znear: float, zfar: float, tanx: float, tany: float) -> to
     return P
 
 
+def projection_matrix_k(znear: float, zfar: float, fx: float, fy: float, cx: float, cy: float, skew: float, width: int,
+                        height: int) -> torch.Tensor:
+    """Same matrix as lib/utils/graphics_utils.py:72-94 (getProjectionMatrixK): principal point and skew from K, OpenGL depth row."""
+    P = torch.zeros(4, 4, dtype=torch.float32)
+    P[0, 0] = 2 * fx / width
+    P[0, 1] = 2 * skew / width
+    P[0, 2] = -1 + 2 * (cx / width)
+    P[1, 1] = 2 * fy / height
+    P[1, 2] = -1 + 2 * (cy / height)
+    P[2, 2] = (zfar + znear) / (zfar - znear)
+    P[2, 3] = -1 * 2 * zfar * znear / (zfar - znear)
+    P[3, 2] = 1.0
+    return P
+
+
 def make_camera(width: int, height: int, fovx_deg: float = 50.0, w2c: Optional[torch.Tensor] = None,
-                sh_degree: int = 3, bg=(0.0, 0.0, 0.0), scale_modifier: float = 1.0) -> Dict:
-    tanx = math.tan(math.radians(fovx_deg) * 0.5)
-    tany = tanx * height / width
+                sh_degree: int = 3, bg=(0.0, 0.0, 0.0), scale_modifier: float = 1.0, intrinsics=None) -> Dict:
+    """intrinsics = (fx, fy, cx, cy, skew) in pixels: the camera of a Waymo frame (lib/datasets/waymo_full_readers.py:100-102,
+    lib/utils/camera_utils.py:52-55, 208-209).  The projection comes from K, while tan(fov / 2) comes from the reader's FoVs,
+    which pair fx with the height and fy with the width.  So the rasterizer derives its x focal length from fy and its y focal
+    length from fx, as the reference does.  fovx_deg is then unused."""
+    if intrinsics is None:
+        tanx = math.tan(math.radians(fovx_deg) * 0.5)
+        tany = tanx * height / width
+    else:
+        fx, fy, cx, cy, skew = (float(v) for v in intrinsics)
+        focal2fov = lambda focal, pixels: 2 * math.atan(pixels / (2 * focal))  # lib/utils/graphics_utils.py:99-100
+        tanx = math.tan(focal2fov(fy, width) * 0.5)
+        tany = math.tan(focal2fov(fx, height) * 0.5)
     if w2c is None:
         w2c = torch.eye(4, dtype=torch.float32)
     view_t = w2c.t().contiguous()  # world_view_transform
-    proj_t = projection_matrix(0.001, 1000.0, tanx, tany).t().contiguous()
+    proj = (projection_matrix(0.001, 1000.0, tanx, tany) if intrinsics is None else
+            projection_matrix_k(0.001, 1000.0, fx, fy, cx, cy, skew, width, height))
+    proj_t = proj.t().contiguous()
     full = (view_t.unsqueeze(0).bmm(proj_t.unsqueeze(0))).squeeze(0).contiguous()
     campos = view_t.inverse()[3, :3].contiguous()
     return dict(image_height=int(height), image_width=int(width), tanfovx=tanx, tanfovy=tany,
@@ -79,15 +106,18 @@ def _field(gen, n, tanx, tany, zmin=2.0, zmax=80.0, near_frac=0.02, scale_med=0.
 
 def make_scene(P: int, width: int, height: int, sh_degree: int = 3, seed: int = 0, n_vehicles: int = 0,
                per_vehicle: int = 0, semantics: int = 0, pose: bool = False, fovx_deg: float = 50.0,
-               bg=(0.0, 0.0, 0.0), scale_med: float = 0.007, with_raw: bool = False) -> Dict:
+               bg=(0.0, 0.0, 0.0), scale_med: float = 0.007, with_raw: bool = False, sh_coeffs: Optional[int] = None,
+               intrinsics=None, scale_modifier: float = 1.0) -> Dict:
     """P background Gaussians (+ n_vehicles x per_vehicle posed 'vehicle' clusters, composed the way
     lib/models/street_gaussian_model.py:335-363 does: x_world = R_obj x_local + t_obj, q_world = q_obj * q_local).
     with_raw: also return out["raw"] = dict(models=[background, vehicle_0, ...] of RAW parameters (local frame, log scale, logit
     opacity, features_dc / features_rest split; the layout street_gaussians_b200.compose consumes), poses [n_vehicles, 7], idft
-    [n_vehicles, 1]) whose composition reproduces the composed arrays above up to fp32 rounding."""
+    [n_vehicles, 1]) whose composition reproduces the composed arrays above up to fp32 rounding.
+    sh_coeffs: coefficients stored per Gaussian (default (sh_degree + 1)^2, as many as the active degree evaluates; more is what a
+    model trained towards a higher degree holds before it gets there).  intrinsics, scale_modifier: see make_camera."""
     gen = torch.Generator().manual_seed(seed)
     w2c = random_pose(gen) if pose else None
-    cam = make_camera(width, height, fovx_deg, w2c, sh_degree, bg)
+    cam = make_camera(width, height, fovx_deg, w2c, sh_degree, bg, scale_modifier, intrinsics)
     tanx, tany = cam["tanfovx"], cam["tanfovy"]
     means, scales, rot, opac = _field(gen, P, tanx, tany, scale_med=scale_med)
     raw_local, raw_pose = [], []
@@ -116,7 +146,7 @@ def make_scene(P: int, width: int, height: int, sh_degree: int = 3, seed: int = 
     if w2c is not None:  # express the field in world coordinates so that W2C brings it back in front of the camera
         c2w = torch.linalg.inv(w2c)
         means = means @ c2w[:3, :3].t() + c2w[:3, 3]
-    M = (sh_degree + 1) ** 2
+    M = (sh_degree + 1) ** 2 if sh_coeffs is None else int(sh_coeffs)
     shs = torch.randn(n, M, 3, generator=gen) * 0.2
     shs[:, 0, :] = torch.randn(n, 3, generator=gen)
     out = dict(cam=cam, means3D=means.float().contiguous(), scales=scales.float().contiguous(),

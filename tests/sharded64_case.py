@@ -105,9 +105,11 @@ def total_classes(totals, world):
     return cl
 
 
-def _pool(W, H, world, seed, D, n_small, n_wide, n_ties):
-    """Candidates: class-k splats span exactly k tile rows (k = 1, 2, 3), wide faint splats span every row, tie pairs.  n_small: {1: n, 2: n, 3: n} candidates per class."""
+def _pool(W, H, world, seed, D, n_small, n_wide, n_ties, camera=None):
+    """Candidates: class-k splats span exactly k tile rows (k = 1, 2, 3), wide faint splats span every row, tie pairs.  n_small: {1: n, 2: n, 3: n} candidates per class.
+    camera: (W, H, D) -> camera dict of synthetic.make_camera to build the splats under (default: the identity camera)."""
     g = torch.Generator().manual_seed(seed)
+    kw = dict(sh_degree=D) if camera is None else dict(cam=camera(W, H, D))
     gy = (H + TILE - 1) // TILE
     U = lambda n, lo, hi: torch.rand(n, generator=g, dtype=F64) * (hi - lo) + lo
     row = lambda n, top: torch.randint(0, max(1, top), (n,), generator=g).to(F64)
@@ -118,10 +120,10 @@ def _pool(W, H, world, seed, D, n_small, n_wide, n_ties):
             continue
         n = n_small[k]
         py = TILE * row(n, gy - k + 1) + off + U(n, -jit, jit)
-        parts.append(RC.screen_scene(W, H, U(n, 0, W), py, U(n, *sig), U(n, 3.0, 30.0), U(n, 0.05, 0.5), sh_degree=D, seed=seed + k))
+        parts.append(RC.screen_scene(W, H, U(n, 0, W), py, U(n, *sig), U(n, 3.0, 30.0), U(n, 0.05, 0.5), seed=seed + k, **kw))
         tags += [f"c{k}"] * n
     if n_wide:
-        parts.append(RC.stack(W, H, W / 2, H / 2, n_wide, seed=seed + 7, opac=(0.004, 0.008), sigma=40.0, z0=2.0, sh_degree=D))
+        parts.append(RC.stack(W, H, W / 2, H / 2, n_wide, seed=seed + 7, opac=(0.004, 0.008), sigma=40.0, z0=2.0, **kw))
         tags += ["wide"] * n_wide
     for i in range(n_ties):  # two splats 1 px apart, bit-identical z, opacity 0.6, red against blue
         y = int(torch.randint(0, max(1, H // TILE), (1,), generator=g))  # a full tile row: the pair blends on visible pixels
@@ -150,9 +152,10 @@ def _classify(sc, tags, world, device):
     return m, popcount(m)
 
 
-def build(name, seed=0, D=3, device="cpu", max_tries=4):
+def build(name, seed=0, D=3, device="cpu", max_tries=4, camera=None):
     """The case `name` of CASES: returns dict(scene (global, rank-major), P_r, chunk, world, W, H, mask, totals, ties [(a, b) global
-    indices], owner_of [global index -> rank], tags)."""
+    indices], owner_of [global index -> rank], tags).  camera: see _pool; under a posed camera the two splats of a pair do not keep
+    bit-identical view depths, so such a case has no tie pairs."""
     spec = CASES[name]
     world, W, H, chunk = spec["world"], spec["W"], spec["H"], spec["chunk"]
     P_r = owned_counts(spec["layout"], world, chunk)
@@ -182,9 +185,10 @@ def build(name, seed=0, D=3, device="cpu", max_tries=4):
             need["c2"] += 256
         elif rc == "t768":
             need["c3"] += 256
-    n_ties = 2 if sum(1 for p in P_r if p > 0) >= 2 else 0
+    n_ties = 2 if sum(1 for p in P_r if p > 0) >= 2 and camera is None else 0
     n_small = {k: int(1.3 * need[f"c{k}"]) + 40 for k in (1, 2, 3)}
-    pool, tags = _pool(W, H, world, seed * 7919 + len(name), D, n_small, need["wide"] + 80 if need["wide"] else 0, n_ties)
+    pool, tags = _pool(W, H, world, seed * 7919 + len(name), D, n_small, need["wide"] + 80 if need["wide"] else 0, n_ties,
+                        camera)
     excluded = torch.zeros(len(tags), dtype=torch.bool)
     for _ in range(max_tries):
         keep0 = torch.nonzero(~excluded).reshape(-1)

@@ -257,6 +257,45 @@ def test_gaussian_sharded_entry_points_validate_before_touching_cuda():
     assert L.sgr_scatter_records(C.byref(fr), C.byref(pe), None, None, None) == -1 and "entry 0 is NULL" in err()
 
 
+def test_sh_degree_and_alignment_validated_before_touching_cuda():
+    """An active SH degree with more coefficients than stored (the kernels would evaluate uninitialised ones), and rotation / SH
+    rows or their gradients off 16-byte alignment (16-byte vector loads and stores would fault), come back as SGR_EINVAL from
+    every entry point that takes them.  The pointers are never dereferenced: validation precedes any CUDA call."""
+    L = _capi.lib()
+    err = lambda: L.sgr_last_error().decode()
+    ok, off = C.c_void_p(1 << 20), C.c_void_p((1 << 20) + 4)  # 16-byte aligned, one float past it
+    fr = _capi.SgrFrame()
+    fr.P, fr.width, fr.height, fr.D, fr.M = 100, 64, 64, 1, 16
+    fr.tan_fovx, fr.tan_fovy, fr.scale_modifier = 0.5, 0.5, 1.0
+    fr.bg = fr.viewmatrix = fr.projmatrix = fr.campos = ok.value
+
+    def project(shs, rot):
+        return L.sgr_project(C.byref(fr), ok, shs, None, ok, ok, rot, None, ok, ok, None)
+
+    for D, M in ((3, 9), (2, 4), (1, 1), (3, 15)):
+        fr.D, fr.M = D, M
+        assert project(ok, ok) == -1 and "SH degree" in err(), (D, M)
+    fr.D, fr.M = 1, 16
+    assert project(off, ok) == -1 and "shs is not 16-byte aligned" in err()
+    assert project(ok, off) == -1 and "rotations is not 16-byte aligned" in err()
+    for M in (4, 9, 25):  # whatever the row width: the staged and unstaged paths read rotations as float4 too
+        fr.M = M
+        assert project(ok, off) == -1 and "rotations" in err(), M
+    fr.M = 16
+    assert L.sgr_forward_bounded(C.byref(fr), ok, ok, None, None, ok, ok, off, None, ok, ok, ok, None, ok, ok, 1 << 30, ok, 1 << 30,
+                                 ok, 1 << 30, 0, None) == -1 and "rotations" in err()
+    assert L.sgr_visible_filter(C.byref(fr), ok, ok, off, None, ok, ok, None) == -1 and "rotations" in err()
+
+    def backward(shs, rot, dsh, drot, D=1, M=16):
+        fr.D, fr.M = D, M
+        return L.sgr_backward_geom(C.byref(fr), ok, shs, None, ok, rot, None, ok, ok, ok, ok, ok, dsh, None, ok, ok, drot, None, None)
+
+    assert backward(ok, ok, ok, ok, D=3, M=9) == -1 and "SH degree" in err()
+    for args, what in (((off, ok, ok, ok), "shs"), ((ok, off, ok, ok), "rotations"), ((ok, ok, off, ok), "dL_dsh"),
+                       ((ok, ok, ok, off), "dL_drotations")):
+        assert backward(*args) == -1 and f"{what} is not 16-byte aligned" in err(), what
+
+
 def test_peer_workspace_layout_is_aligned_and_ordered():
     from street_gaussians_b200.sharded import PeerWorkspace
     st = sgb.GaussianRasterizationSettings(480, 640, 0.5, 0.4, torch.zeros(3), 1.0, torch.eye(4), torch.eye(4), 3, torch.zeros(3), False, False)

@@ -270,8 +270,12 @@ def test_layered_gradients_per_element_vs_float64():
     import raster64_case as RC
     import test_raster64_gpu as T
     sc = RC.cat_scenes(T.preprocess_scene(D=3, seed=51), T.preprocess_scene(D=3, seed=52))
-    b0 = T.preprocess_scene(D=3, seed=51)["means3D"].shape[0]
-    sc["cam"]["bg"] = torch.tensor([0.1, 0.2, 0.3])
+    check_layered(sc, T.preprocess_scene(D=3, seed=51)["means3D"].shape[0])
+
+
+def check_layered(sc, b0):
+    """test_layered_gradients_per_element_vs_float64 on the scene `sc`, with the layer [b0, P) (before the margin passes)."""
+    sc["cam"] = dict(sc["cam"], bg=torch.tensor([0.1, 0.2, 0.3]))
     sc, b = _margin_pair(sc, b0)
     P = sc["means3D"].shape[0]
     assert 0 < b < P

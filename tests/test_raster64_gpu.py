@@ -232,25 +232,45 @@ def test_band_and_bounded_modes():
 
 
 # ------------------------------------------------------------------------------------------------ C. preprocess
-def preprocess_scene(D, seed, colors_precomp=False, cov3d=False):
+def preprocess_scene(D, seed, colors_precomp=False, cov3d=False, cam=None, sh_coeffs=None):
     """Splats on screen plus centres outside 1.3 tan(fov) whose splats reach into the image (the Jacobian clamp and its zero
-    gradient), SH colours driven below 0 (clamp bits), anisotropic covariances from raw, non-normalised quaternions."""
+    gradient), SH colours driven below 0 (clamp bits), anisotropic covariances from raw, non-normalised quaternions.
+    cam: a 96 x 64 camera (synthetic.make_camera; its sh_degree replaces D) — the clamp cases are then placed by tx/tz against
+    1.3 tan(fov / 2), wherever that falls in the image.  sh_coeffs: coefficients stored beyond the active degree's."""
     W, H = 96, 64
     g = torch.Generator().manual_seed(seed)
     n = 80
     r = lambda lo, hi, m=n: torch.rand(m, generator=g, dtype=torch.float64) * (hi - lo) + lo
-    a = RC.screen_scene(W, H, r(0, W), r(0, H), r(2.0, 7.0), r(3.0, 20.0), r(0.1, 0.9), sh_degree=D, seed=seed)
-    # |ndc| up to 1.9 (|tx/tz| > 1.3 tan) with splats of 25-40 px reaching in: left, right, above, below
+    kw = dict(sh_degree=D) if cam is None else dict(cam=cam, sh_coeffs=sh_coeffs)
+    a = RC.screen_scene(W, H, r(0, W), r(0, H), r(2.0, 7.0), r(3.0, 20.0), r(0.1, 0.9), seed=seed, **kw)
+    # |tx/tz| between 1.45 and 1.9 tan (clamped at 1.3 tan) with splats of 25-40 px reaching in: left, right, above, below
     m = 8
     ndc = r(1.45, 1.9, m)
     sx = torch.tensor([1, -1, 0, 0, 1, -1, 1, -1], dtype=torch.float64)
     sy = torch.tensor([0, 0, 1, -1, 1, 1, -1, -1], dtype=torch.float64)
-    cx = torch.where(sx != 0, ((sx * ndc + 1) * W - 1) / 2, r(10, W - 10, m))
-    cy = torch.where(sy != 0, ((sy * ndc + 1) * H - 1) / 2, r(10, H - 10, m))
-    b = RC.screen_scene(W, H, cx, cy, r(25.0, 40.0, m), r(4.0, 8.0, m), r(0.3, 0.8, m), sh_degree=D, seed=seed + 1)
-    c = RC.screen_scene(W, H, r(0, W, 12), r(0, H, 12), r(2.0, 5.0, 12), r(3.0, 20.0, 12), r(0.3, 0.8, 12), sh_degree=D, seed=seed + 2,
-                        rgb=torch.tensor([-0.4, 0.6, -0.3], dtype=torch.float64))
+    if cam is None:
+        cx = torch.where(sx != 0, ((sx * ndc + 1) * W - 1) / 2, r(10, W - 10, m))
+        cy = torch.where(sy != 0, ((sy * ndc + 1) * H - 1) / 2, r(10, H - 10, m))
+    else:
+        u0, v0 = RC.ratio_of(cam, r(10, W - 10, m), r(10, H - 10, m))
+        u = torch.where(sx != 0, sx * ndc * cam["tanfovx"], u0)
+        v = torch.where(sy != 0, sy * ndc * cam["tanfovy"], v0)
+        cx, cy = RC.pixel_of(cam, u, v)
+    b = RC.screen_scene(W, H, cx, cy, r(25.0, 40.0, m), r(4.0, 8.0, m), r(0.3, 0.8, m), seed=seed + 1, **kw)
+    c = RC.screen_scene(W, H, r(0, W, 12), r(0, H, 12), r(2.0, 5.0, 12), r(3.0, 20.0, 12), r(0.3, 0.8, 12), seed=seed + 2,
+                        rgb=torch.tensor([-0.4, 0.6, -0.3], dtype=torch.float64), **kw)
     sc = RC.cat_scenes(RC.cat_scenes(a, b), c)
+    if cam is not None:
+        # centres past the x clamp that still lie inside the image, where the camera puts 1.3 tan(fov / 2) inside it
+        limx = 1.3 * cam["tanfovx"]
+        u_edge = float(RC.ratio_of(cam, W - 4.0, H / 2)[0])
+        if u_edge > 1.1 * limx:
+            k = 10
+            vv = RC.ratio_of(cam, r(0, W, k), r(8, H - 8, k))[1]
+            uu = limx * 1.02 + r(0, 1, k) * (u_edge - limx * 1.05)
+            ix, iy = RC.pixel_of(cam, uu, vv)
+            d = RC.screen_scene(W, H, ix, iy, r(3.0, 8.0, k), r(3.0, 20.0, k), r(0.3, 0.8, k), seed=seed + 3, **kw)
+            sc = RC.cat_scenes(sc, d)
     P = sc["means3D"].shape[0]
     q = torch.randn(P, 4, generator=g)
     sc["rotations"] = (q / q.norm(dim=1, keepdim=True) * (0.8 + 0.4 * torch.rand(P, 1, generator=g))).float()
@@ -352,11 +372,15 @@ def test_end_to_end_autograd():
     fp32 records rather than fp64 ones: the records differ by the bounds of check_preprocess, which move a pair's power by at most
     64 2^-24 (1 + cond) (1 + max(W, H)) relative to the terms it sums.  Catches plumbing errors: argument order, the means2D leaf,
     semantics, bands of the result tuple."""
-    sc = RC.cat_scenes(preprocess_scene(D=3, seed=31), preprocess_scene(D=3, seed=32))
+    check_end_to_end("end_to_end", RC.cat_scenes(preprocess_scene(D=3, seed=31), preprocess_scene(D=3, seed=32)))
+
+
+def check_end_to_end(name, sc):
+    """test_end_to_end_autograd on the 96 x 64 scene `sc` (4 semantic channels and a background are added)."""
     gen = torch.Generator().manual_seed(33)
     sc["semantics"] = torch.rand(sc["means3D"].shape[0], 4, generator=gen)
     sc["grad_semantic"] = torch.randn(4, 64, 96, generator=gen) / (64 * 96)
-    sc["cam"]["bg"] = torch.tensor([0.1, 0.2, 0.3])
+    sc["cam"] = dict(sc["cam"], bg=torch.tensor([0.1, 0.2, 0.3]))
     sc, removed, _ = R64.margin_scene(sc, device=DEV)
     mine = util.run_api(sgb, sc)
     r = R64.render64(sc, DEV, alpha_img=torch.from_numpy(mine["alpha"]))
@@ -383,8 +407,8 @@ def test_end_to_end_autograd():
         err = (got - ref).abs()
         worst[key] = float((err / bnd).max())
         assert (err <= bnd).all(), (key, worst[key])
-    REPORT["end_to_end"] = dict(removed=removed, t_rec=t_rec, **{kk: round(v, 4) for kk, v in worst.items()})
-    print("end_to_end", REPORT["end_to_end"])
+    REPORT[name] = dict(removed=removed, t_rec=t_rec, **{kk: round(v, 4) for kk, v in worst.items()})
+    print(name, REPORT[name])
 
 
 VARIANT_SCRIPT = r"""

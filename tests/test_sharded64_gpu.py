@@ -159,11 +159,11 @@ def tie_check(case, rec, radii, bl, alpha):
         assert gap > 1e3, ("tie swap is not detectable", a, b, gap)
 
 
-def run_fused(name, D=3, precomp=False, compact=True, frames=2, no_tma=False, expect=None):
+def run_fused(name, D=3, precomp=False, compact=True, frames=2, no_tma=False, expect=None, camera=None):
     """Two frames of `name` (seeds 0, 1; same chunk), each forward + backward on emulated ranks (compact: first with every
-    depth-order slot, then with the learnt n_sel + 16), then two forwards in a row."""
+    depth-order slot, then with the learnt n_sel + 16), then two forwards in a row.  camera: see sharded64_case.build."""
     _warm_up_fused_path(DEV)
-    cases = [SC.build(name, seed=f, D=D, device=DEV) for f in range(frames)]
+    cases = [SC.build(name, seed=f, D=D, device=DEV, camera=camera) for f in range(frames)]
     world, chunk, W, H = cases[0]["world"], cases[0]["chunk"], cases[0]["W"], cases[0]["H"]
     st = util.settings_from(sgb, cases[0]["scene"]["cam"], DEV)
     wss = SH.PeerWorkspace.emulate(st, chunk, world, DEV)
