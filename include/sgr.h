@@ -342,6 +342,37 @@ int sgr_compose_backward(const SgrSegment *segments, const SgrSegmentGrads *grad
                          const float *idft, const uint8_t *flip, const float *flip_quat, const float *dL_dmeans3D,
                          const float *dL_drotations, const float *dL_dscales, const float *dL_dopacities, const float *dL_dshs,
                          float *dposes, float *pose_scratch, void *stream);
+/* The same two calls with the learned background pose correction of lib/models/camera_pose.py:89-114
+ * (cfg.model.use_pose_correction; street_gaussian_model.py:311-312, 340-341) applied to every segment with posed == 0.
+ * bkgd_correction (device, 8 floats): qw qx qy qz tx ty tz pad — the caller's rows pose_correction_rots[id] / pose_correction_trans[id].
+ * With q = c / max(|c|, 1e-12) (F.normalize) and R = quaternion_to_matrix(q) (which normalises q once more, with no clamp, so a zero
+ * correction gives NaN like the reference): xyz' = R xyz + t and rotation' = q (x) normalize(_rotation), NOT normalised again.
+ * Backward: dcorrection (device, 8 floats: d q, d t, 0) receives the gradient of every unposed row, through both normalisations on
+ * the matrix path and through F.normalize alone on the rotation path; pose_scratch must hold (num_segments + 1) * 16 floats. */
+int sgr_compose_forward_corrected(const SgrSegment *segments, int32_t num_segments, int32_t M, const float *poses, const float *idft,
+                                  const uint8_t *flip, const float *flip_quat, const float *bkgd_correction, float *means3D, float *rotations,
+                                  float *scales, float *opacities, float *shs, void *stream);
+int sgr_compose_backward_corrected(const SgrSegment *segments, const SgrSegmentGrads *grads, int32_t num_segments, int32_t M,
+                                   const float *poses, const float *idft, const uint8_t *flip, const float *flip_quat,
+                                   const float *bkgd_correction, const float *dL_dmeans3D, const float *dL_drotations, const float *dL_dscales,
+                                   const float *dL_dopacities, const float *dL_dshs, float *dposes, float *dcorrection, float *pose_scratch,
+                                   void *stream);
+
+/* ---- Colour correction (lib/models/color_correction.py:129-140, cfg.model.use_color_correction) ----
+ * out[i] = A[i,0] image[0] + A[i,1] image[1] + A[i,2] image[2] + A[i,3] per pixel: the products in einsum's order, then the bias.
+ * image, out, dL_dout, dL_dimage: [3,H,W] fp32 device; affine, dL_daffine: [3,4] fp32 device (row-major).
+ * Backward: dL_dimage = A^T dL_dout per pixel (may be NULL), dL_daffine[i,j] = sum over pixels of dL_dout[i] [image[j], 1], reduced in
+ * a fixed order, so repeated calls give bit-identical results; grid sizes depend on H*W only (no host synchronisation).
+ * scratch: sgr_color_correct_scratch_bytes(H, W) bytes. */
+int sgr_color_correct_forward(int32_t H, int32_t W, const float *image, const float *affine, float *out, void *stream);
+size_t sgr_color_correct_scratch_bytes(int32_t H, int32_t W);
+int sgr_color_correct_backward(int32_t H, int32_t W, const float *image, const float *affine, const float *dL_dout, float *dL_dimage,
+                               float *dL_daffine, void *scratch, size_t scratch_bytes, void *stream);
+/* Regularisation of the colour correction (color_correction.py:134-140 as train.py:135-138 uses it):
+ * value (device, 1 float) = weight * mean(|A - I| + |A_sky - I|) over the 12 entries (|A_sky - I| left out when affine_sky is NULL);
+ * g_affine / g_affine_sky (device, 12 floats, either may be NULL) = weight / 12 * sign(A - I), 0 where A == I. */
+int sgr_color_correction_reg(const float *affine, const float *affine_sky, float weight, float *value, float *g_affine, float *g_affine_sky,
+                             void *stream);
 
 /* ---- Image-space losses with their gradient (SURVEY.md §8 row f2) ----
  * value = w_l1 * L1(image, gt, mask) + w_ssim * SSIM(image, gt, mask)  and  dL_dimage = d value / d image  in two kernels.

@@ -14,9 +14,10 @@ from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, Inst
                          distCUDA2, rasterize_gaussians)
 
 from .composer import compose  # noqa: E402,F401
-from . import losses, training  # noqa: E402,F401
+from .corrections import color_correct, color_correction_reg_loss  # noqa: E402,F401
+from . import corrections, losses, training  # noqa: E402,F401
 
-__all__ = ["compose", "GaussianRasterizationSettings", "GaussianRasterizer", "TileRowBand", "InstanceCapacity", "RenderLayer", "rasterize_gaussians", "distCUDA2",
+__all__ = ["compose", "color_correct", "color_correction_reg_loss", "GaussianRasterizationSettings", "GaussianRasterizer", "TileRowBand", "InstanceCapacity", "RenderLayer", "rasterize_gaussians", "distCUDA2",
            "install_shims"]
 
 _SHIMS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "shims")

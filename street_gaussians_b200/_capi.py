@@ -18,7 +18,9 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_state_s
            "sgr_compose_forward", "sgr_compose_backward", "sgr_image_loss_scratch_bytes", "sgr_image_loss", "sgr_sky_loss",
            "sgr_obj_acc_loss", "sgr_lidar_depth_loss_scratch_bytes", "sgr_lidar_depth_loss", "sgr_densify_stats", "sgr_adam_step",
            "sgr_densify_scratch_bytes", "sgr_densify_plan", "sgr_densify_apply", "sgr_reset_opacity", "sgr_sparse_adam_step",
-           "sgr_layer_state_sizes", "sgr_forward_layer", "sgr_backward_blend_layer", "sgr_backward_geom_layered"]
+           "sgr_layer_state_sizes", "sgr_forward_layer", "sgr_backward_blend_layer", "sgr_backward_geom_layered",
+           "sgr_compose_forward_corrected", "sgr_compose_backward_corrected", "sgr_color_correct_forward", "sgr_color_correct_scratch_bytes",
+           "sgr_color_correct_backward", "sgr_color_correction_reg"]
 
 
 class SgrFrame(C.Structure):
@@ -161,6 +163,18 @@ def lib():
     L.sgr_compose_forward.argtypes = [C.POINTER(SgrSegment), C.c_int32, C.c_int32] + [vp] * 10
     L.sgr_compose_backward.restype = C.c_int
     L.sgr_compose_backward.argtypes = [C.POINTER(SgrSegment), C.POINTER(SgrSegmentGrads), C.c_int32, C.c_int32] + [vp] * 12
+    L.sgr_compose_forward_corrected.restype = C.c_int
+    L.sgr_compose_forward_corrected.argtypes = [C.POINTER(SgrSegment), C.c_int32, C.c_int32] + [vp] * 11
+    L.sgr_compose_backward_corrected.restype = C.c_int
+    L.sgr_compose_backward_corrected.argtypes = [C.POINTER(SgrSegment), C.POINTER(SgrSegmentGrads), C.c_int32, C.c_int32] + [vp] * 14
+    L.sgr_color_correct_forward.restype = C.c_int
+    L.sgr_color_correct_forward.argtypes = [C.c_int32, C.c_int32, vp, vp, vp, vp]
+    L.sgr_color_correct_scratch_bytes.restype = C.c_size_t
+    L.sgr_color_correct_scratch_bytes.argtypes = [C.c_int32, C.c_int32]
+    L.sgr_color_correct_backward.restype = C.c_int
+    L.sgr_color_correct_backward.argtypes = [C.c_int32, C.c_int32, vp, vp, vp, vp, vp, vp, C.c_size_t, vp]
+    L.sgr_color_correction_reg.restype = C.c_int
+    L.sgr_color_correction_reg.argtypes = [vp, vp, C.c_float, vp, vp, vp, vp]
     L.sgr_image_loss_scratch_bytes.restype = C.c_size_t
     L.sgr_image_loss_scratch_bytes.argtypes = [C.c_int32] * 3
     L.sgr_image_loss.restype = C.c_int

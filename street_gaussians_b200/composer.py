@@ -8,15 +8,18 @@ sgr_compose_forward / sgr_compose_backward (include/sgr.h).
     poses  : [num_actors, 7] = (qw, qx, qy, qz, tx, ty, tz): the rows parse_camera expands into obj_rots / obj_trans (:258-273)
     idft   : [num_actors, C] IDFT(t, C) rows (lib/utils/sh_utils.py:120-130)
     flip   : optional bool [sum of actor counts] (the flip_mask of :275-284) with flip_quat [4] (the reference's flip_matrix)
+    pose_correction : optional (rot [4], trans [3]), the caller's rows pose_correction_rots[id] / pose_correction_trans[id] of
+             lib/models/camera_pose.py; the background is moved by them as correct_gaussian_xyz / correct_gaussian_rotation do
+             (street_gaussian_model.py:311-312, 340-341).  None (the reference's 'test' mode) composes without a correction.
 
 `compose(...)` returns (means3D, rotations, scales, opacities, shs) ready for GaussianRasterizer.forward; gradients flow to every
-raw parameter and to `poses`.  PyTorch is plumbing (allocation, autograd bookkeeping); all arithmetic is in libsgr.so, and there
+raw parameter, to `poses` and to the two correction rows.  PyTorch is plumbing (allocation, autograd bookkeeping); all arithmetic is in libsgr.so, and there
 is no CPU fallback.
 """
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional, Sequence
+from typing import Optional, Sequence, Tuple
 
 import torch
 
@@ -38,7 +41,7 @@ def _f32c(t: torch.Tensor) -> torch.Tensor:
 
 class _Compose(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, poses, idft, flip, flip_quat, n_models, *raw):
+    def forward(ctx, poses, idft, flip, flip_quat, corr_rot, corr_trans, n_models, *raw):
         L = _capi.lib()
         if not raw[0].is_cuda:
             raise _capi.SgrError("street_gaussians_b200 composer needs CUDA tensors (there is no CPU fallback)")
@@ -69,15 +72,28 @@ class _Compose(torch.autograd.Function):
             flip_full = torch.zeros((P,), device=dev, dtype=torch.uint8)
             flip_full[int(models[0][0].shape[0]):] = flip.to(device=dev, dtype=torch.uint8)
             flip_quat = _f32c(flip_quat.to(dev).reshape(4))
+        corr = None
+        if corr_rot is not None:
+            corr = torch.zeros((8,), device=dev, dtype=torch.float32)
+            corr[:4] = corr_rot.reshape(4).to(device=dev, dtype=torch.float32)
+            corr[4:7] = corr_trans.reshape(3).to(device=dev, dtype=torch.float32)
         e = lambda *shape: torch.empty(shape, device=dev, dtype=torch.float32)
         xyz, rot, scale, opac, sh = e(P, 3), e(P, 4), e(P, 3), e(P, 1), e(P, M, 3)
+        fq = _ptr(flip_quat) if flip_full is not None else None
         with torch.cuda.device(dev):
-            rc = L.sgr_compose_forward(segs, nseg, M, _ptr(pose_tab), _ptr(idft_tab), _ptr(flip_full), _ptr(flip_quat) if flip_full is not None else None,
-                                       _ptr(xyz), _ptr(rot), _ptr(scale), _ptr(opac), _ptr(sh), _stream(dev))
-        _capi.check(rc, "sgr_compose_forward")
+            if corr is None:
+                rc = L.sgr_compose_forward(segs, nseg, M, _ptr(pose_tab), _ptr(idft_tab), _ptr(flip_full), fq, _ptr(xyz), _ptr(rot), _ptr(scale),
+                                           _ptr(opac), _ptr(sh), _stream(dev))
+            else:
+                rc = L.sgr_compose_forward_corrected(segs, nseg, M, _ptr(pose_tab), _ptr(idft_tab), _ptr(flip_full), fq, _ptr(corr), _ptr(xyz),
+                                                     _ptr(rot), _ptr(scale), _ptr(opac), _ptr(sh), _stream(dev))
+        _capi.check(rc, "sgr_compose_forward" if corr is None else "sgr_compose_forward_corrected")
         ctx.segs, ctx.nseg, ctx.M, ctx.n_models = segs, nseg, M, n_models
         ctx.flip_full, ctx.flip_quat = flip_full, (flip_quat if flip_full is not None else None)
         ctx.pose_shape = None if poses is None else (tuple(poses.shape), poses.dtype, poses.device)
+        ctx.corr_meta = None if corr is None else ((tuple(corr_rot.shape), corr_rot.dtype, corr_rot.device),
+                                                   (tuple(corr_trans.shape), corr_trans.dtype, corr_trans.device))
+        ctx.corr = corr
         ctx.save_for_backward(pose_tab, idft_tab, *raw)
         return xyz, rot, scale, opac, sh
 
@@ -96,22 +112,35 @@ class _Compose(torch.autograd.Function):
             g = gtab[k]
             g.xyz, g.rotation, g.scaling, g.opacity, g.features_dc, g.features_rest = (t.data_ptr() if t.numel() else None for t in grads[6 * k: 6 * k + 6])
         dposes = torch.empty((nseg, 8), device=dev, dtype=torch.float32)
-        scratch = torch.empty((nseg, 16), device=dev, dtype=torch.float32)
+        corr = ctx.corr
         with torch.cuda.device(dev):
-            rc = L.sgr_compose_backward(ctx.segs, gtab, nseg, M, _ptr(pose_tab), _ptr(idft_tab), _ptr(ctx.flip_full), _ptr(ctx.flip_quat),
-                                        _ptr(g_xyz), _ptr(g_rot), _ptr(g_scale), _ptr(g_opac), _ptr(g_sh), _ptr(dposes), _ptr(scratch),
-                                        _stream(dev))
-        _capi.check(rc, "sgr_compose_backward")
-        g_poses = None
+            if corr is None:
+                scratch = torch.empty((nseg, 16), device=dev, dtype=torch.float32)
+                rc = L.sgr_compose_backward(ctx.segs, gtab, nseg, M, _ptr(pose_tab), _ptr(idft_tab), _ptr(ctx.flip_full), _ptr(ctx.flip_quat),
+                                            _ptr(g_xyz), _ptr(g_rot), _ptr(g_scale), _ptr(g_opac), _ptr(g_sh), _ptr(dposes), _ptr(scratch),
+                                            _stream(dev))
+            else:
+                scratch = torch.empty((nseg + 1, 16), device=dev, dtype=torch.float32)
+                dcorr = torch.empty((8,), device=dev, dtype=torch.float32)
+                rc = L.sgr_compose_backward_corrected(ctx.segs, gtab, nseg, M, _ptr(pose_tab), _ptr(idft_tab), _ptr(ctx.flip_full),
+                                                      _ptr(ctx.flip_quat), _ptr(corr), _ptr(g_xyz), _ptr(g_rot), _ptr(g_scale), _ptr(g_opac),
+                                                      _ptr(g_sh), _ptr(dposes), _ptr(dcorr), _ptr(scratch), _stream(dev))
+        _capi.check(rc, "sgr_compose_backward" if corr is None else "sgr_compose_backward_corrected")
+        g_poses = g_crot = g_ctrans = None
         if ctx.pose_shape is not None:
             shape, dtype, device = ctx.pose_shape
             g_poses = dposes[1:, :7].to(device=device, dtype=dtype).reshape(shape)
-        return (g_poses, None, None, None, None) + tuple(grads)
+        if corr is not None:
+            (rs, rd, rdev), (ts, td, tdev) = ctx.corr_meta
+            g_crot, g_ctrans = dcorr[:4].to(device=rdev, dtype=rd).reshape(rs), dcorr[4:7].to(device=tdev, dtype=td).reshape(ts)
+        return (g_poses, None, None, None, g_crot, g_ctrans, None) + tuple(grads)
 
 
 def compose(models: Sequence, poses: Optional[torch.Tensor] = None, idft: Optional[torch.Tensor] = None,
-            flip: Optional[torch.Tensor] = None, flip_quat: Optional[torch.Tensor] = None):
-    """-> (means3D[P,3], rotations[P,4], scales[P,3], opacities[P,1], shs[P,M,3]) of background + actors, differentiable."""
+            flip: Optional[torch.Tensor] = None, flip_quat: Optional[torch.Tensor] = None, *,
+            pose_correction: Optional[Tuple[torch.Tensor, torch.Tensor]] = None):
+    """-> (means3D[P,3], rotations[P,4], scales[P,3], opacities[P,1], shs[P,M,3]) of background + actors, differentiable.
+    pose_correction = (rot [4], trans [3]) moves the background by the learned per-image correction; gradients return to both."""
     raw = [_raw(m, k) for m in models for k in RAW_KEYS]
     n_act = len(models) - 1
     if n_act > 0:
@@ -121,4 +150,9 @@ def compose(models: Sequence, poses: Optional[torch.Tensor] = None, idft: Option
             raise ValueError(f"idft must be [{n_act}, fourier_dim]")
     if flip is not None and flip_quat is None:
         raise ValueError("flip mask given without flip_quat (the reference's flip_matrix)")
-    return _Compose.apply(poses, idft, flip, flip_quat, len(models), *raw)
+    corr_rot = corr_trans = None
+    if pose_correction is not None:
+        corr_rot, corr_trans = pose_correction
+        if corr_rot.numel() != 4 or corr_trans.numel() != 3:
+            raise ValueError("pose_correction must be (rot [4] = qw, qx, qy, qz; trans [3])")
+    return _Compose.apply(poses, idft, flip, flip_quat, corr_rot, corr_trans, len(models), *raw)

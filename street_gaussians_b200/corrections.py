@@ -1,0 +1,103 @@
+"""The per-camera colour correction of the reference (lib/models/color_correction.py, cfg.model.use_color_correction) over
+sgr_color_correct_forward / sgr_color_correct_backward / sgr_color_correction_reg (include/sgr.h).
+
+    color_correct(image, affine)                          color_correction.py:129-132, street_gaussian_renderer.py:113-114
+    color_correction_reg_loss(affine, affine_sky, weight)  color_correction.py:134-140 as train.py:135-138 adds it
+
+`affine` is the [3, 4] matrix ColorCorrection.get_affine_trans(camera) returns, in its embedding or its MLP mode (the MLP stays the
+caller's torch module; its output is differentiable like any other tensor).  The background pose correction is not here: pass its
+two rows to `compose(..., pose_correction=...)`.  CUDA tensors only: there is no CPU fallback.
+"""
+from __future__ import annotations
+
+from typing import Optional
+
+import torch
+
+from . import _capi
+from .rasterizer import _ptr, _stream
+
+
+def _prep(t: torch.Tensor, what: str) -> torch.Tensor:
+    if not t.is_cuda:
+        raise _capi.SgrError(f"street_gaussians_b200.corrections needs CUDA tensors ({what} is on {t.device}; there is no CPU fallback)")
+    return t if (t.dtype == torch.float32 and t.is_contiguous()) else t.to(torch.float32).contiguous()
+
+
+def _affine(a: torch.Tensor, what: str, dev) -> torch.Tensor:
+    if tuple(a.shape) != (3, 4):
+        raise ValueError(f"{what} must be [3, 4], got {tuple(a.shape)}")
+    a = _prep(a, what)
+    if a.device != dev:
+        raise ValueError(f"{what} is on {a.device}, the image on {dev}")
+    return a
+
+
+class _ColorCorrect(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, image, affine):
+        L = _capi.lib()
+        img = _prep(image, "image")
+        if img.dim() != 3 or img.shape[0] != 3:
+            raise ValueError(f"image must be [3, H, W], got {tuple(image.shape)}")
+        A = _affine(affine, "affine", img.device)
+        H, W = int(img.shape[1]), int(img.shape[2])
+        out = torch.empty_like(img)
+        with torch.cuda.device(img.device):
+            rc = L.sgr_color_correct_forward(H, W, _ptr(img), _ptr(A), _ptr(out), _stream(img.device))
+        _capi.check(rc, "sgr_color_correct_forward")
+        ctx.save_for_backward(img, A)
+        ctx.dtypes = (image.dtype, affine.dtype)
+        return out
+
+    @staticmethod
+    def backward(ctx, g_out):
+        L = _capi.lib()
+        img, A = ctx.saved_tensors
+        dev = img.device
+        H, W = int(img.shape[1]), int(img.shape[2])
+        g = _prep(g_out, "dL/dout")
+        g_img = torch.empty_like(img) if ctx.needs_input_grad[0] else None
+        g_A = torch.empty((3, 4), device=dev, dtype=torch.float32)
+        nbytes = int(L.sgr_color_correct_scratch_bytes(H, W))
+        scratch = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+        with torch.cuda.device(dev):
+            rc = L.sgr_color_correct_backward(H, W, _ptr(img), _ptr(A), _ptr(g), _ptr(g_img), _ptr(g_A), _ptr(scratch), nbytes, _stream(dev))
+        _capi.check(rc, "sgr_color_correct_backward")
+        return (g_img.to(ctx.dtypes[0]) if g_img is not None else None), (g_A.to(ctx.dtypes[1]) if ctx.needs_input_grad[1] else None)
+
+
+def color_correct(image: torch.Tensor, affine: torch.Tensor) -> torch.Tensor:
+    """einsum('ij,jhw->ihw', affine[:3, :3], image) + affine[:3, 3, None, None] for image [3, H, W]; differentiable in both."""
+    return _ColorCorrect.apply(image, affine)
+
+
+class _Reg(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, affine, affine_sky, weight: float):
+        L = _capi.lib()
+        A = _affine(affine, "affine", affine.device)
+        S = _affine(affine_sky, "affine_sky", A.device) if affine_sky is not None else None
+        dev = A.device
+        value = torch.empty((), device=dev, dtype=torch.float32)
+        gA = torch.empty((3, 4), device=dev, dtype=torch.float32)
+        gS = torch.empty((3, 4), device=dev, dtype=torch.float32) if S is not None else None
+        with torch.cuda.device(dev):
+            rc = L.sgr_color_correction_reg(_ptr(A), _ptr(S), float(weight), _ptr(value), _ptr(gA), _ptr(gS), _stream(dev))
+        _capi.check(rc, "sgr_color_correction_reg")
+        ctx.save_for_backward(gA, gS if gS is not None else gA)
+        ctx.has_sky = S is not None
+        ctx.dtypes = (affine.dtype, affine_sky.dtype if affine_sky is not None else None)
+        return value
+
+    @staticmethod
+    def backward(ctx, g_out):
+        gA, gS = ctx.saved_tensors
+        g_sky = (gS * g_out).to(ctx.dtypes[1]) if ctx.has_sky else None
+        return (gA * g_out).to(ctx.dtypes[0]), g_sky, None
+
+
+def color_correction_reg_loss(affine: torch.Tensor, affine_sky: Optional[torch.Tensor] = None, weight: float = 1.0) -> torch.Tensor:
+    """weight * mean(|affine - I| + |affine_sky - I|) over the 12 entries (only |affine - I| without affine_sky): the regularisation
+    train.py:135-138 adds with weight = lambda_color_correction.  Returns a 0-dim CUDA tensor; gradients reach both matrices."""
+    return _Reg.apply(affine, affine_sky, weight)

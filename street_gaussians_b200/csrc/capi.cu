@@ -754,29 +754,45 @@ static int check_segments(const SgrSegment *segs, int32_t n, int32_t M, int64_t 
 	return SGR_OK;
 }
 
-int sgr_compose_forward(const SgrSegment *segments, int32_t num_segments, int32_t M, const float *poses, const float *idft,
-                        const uint8_t *flip, const float *flip_quat, float *means3D, float *rotations, float *scales, float *opacities,
-                        float *shs, void *stream) {
+static int compose_forward_impl(const char *fn, const SgrSegment *segments, int32_t num_segments, int32_t M, const float *poses,
+                                const float *idft, const uint8_t *flip, const float *flip_quat, float *means3D, float *rotations, float *scales,
+                                float *opacities, float *shs, const float *correction, void *stream) {
 	int64_t P = 0;
 	int rc = check_segments(segments, num_segments, M, P);
 	if (rc) return rc;
 	if (P == 0) return SGR_OK;
-	if (!poses || !idft || !means3D || !rotations || !scales || !opacities || !shs) return fail(SGR_EINVAL, "NULL pointer passed to sgr_compose_forward");
+	if (!poses || !idft || !means3D || !rotations || !scales || !opacities || !shs) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
 	if (flip && !flip_quat) return fail(SGR_EINVAL, "flip mask given without flip_quat");
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 	const bool debug = false;
-	SGR_TRY(launch_compose_fwd(segments, num_segments, M, poses, idft, flip, flip_quat, means3D, rotations, scales, opacities, shs, st), "compose_fwd");
+	SGR_TRY(launch_compose_fwd(segments, num_segments, M, poses, idft, flip, flip_quat, means3D, rotations, scales, opacities, shs, correction, st),
+	        "compose_fwd");
 	return SGR_OK;
 }
 
-int sgr_compose_backward(const SgrSegment *segments, const SgrSegmentGrads *grads, int32_t num_segments, int32_t M, const float *poses,
-                         const float *idft, const uint8_t *flip, const float *flip_quat, const float *dL_dmeans3D,
-                         const float *dL_drotations, const float *dL_dscales, const float *dL_dopacities, const float *dL_dshs,
-                         float *dposes, float *pose_scratch, void *stream) {
+int sgr_compose_forward(const SgrSegment *segments, int32_t num_segments, int32_t M, const float *poses, const float *idft,
+                        const uint8_t *flip, const float *flip_quat, float *means3D, float *rotations, float *scales, float *opacities,
+                        float *shs, void *stream) {
+	return compose_forward_impl("sgr_compose_forward", segments, num_segments, M, poses, idft, flip, flip_quat, means3D, rotations, scales,
+	                            opacities, shs, nullptr, stream);
+}
+
+int sgr_compose_forward_corrected(const SgrSegment *segments, int32_t num_segments, int32_t M, const float *poses, const float *idft,
+                                  const uint8_t *flip, const float *flip_quat, const float *bkgd_correction, float *means3D, float *rotations,
+                                  float *scales, float *opacities, float *shs, void *stream) {
+	if (!bkgd_correction) return fail(SGR_EINVAL, "NULL bkgd_correction passed to sgr_compose_forward_corrected");
+	return compose_forward_impl("sgr_compose_forward_corrected", segments, num_segments, M, poses, idft, flip, flip_quat, means3D, rotations,
+	                            scales, opacities, shs, bkgd_correction, stream);
+}
+
+static int compose_backward_impl(const char *fn, const SgrSegment *segments, const SgrSegmentGrads *grads, int32_t num_segments, int32_t M,
+                                 const float *poses, const float *idft, const uint8_t *flip, const float *flip_quat, const float *correction,
+                                 const float *dL_dmeans3D, const float *dL_drotations, const float *dL_dscales, const float *dL_dopacities,
+                                 const float *dL_dshs, float *dposes, float *dcorrection, float *pose_scratch, void *stream) {
 	int64_t P = 0;
 	int rc = check_segments(segments, num_segments, M, P);
 	if (rc) return rc;
-	if (!grads || !dposes || !pose_scratch || !poses || !idft) return fail(SGR_EINVAL, "NULL pointer passed to sgr_compose_backward");
+	if (!grads || !dposes || !pose_scratch || !poses || !idft) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
 	if (P > 0 && (!dL_dmeans3D || !dL_drotations || !dL_dscales || !dL_dopacities || !dL_dshs)) return fail(SGR_EINVAL, "NULL upstream gradient");
 	if (flip && !flip_quat) return fail(SGR_EINVAL, "flip mask given without flip_quat");
 	for (int k = 0; k < num_segments; k++) {
@@ -787,8 +803,60 @@ int sgr_compose_backward(const SgrSegment *segments, const SgrSegmentGrads *grad
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 	const bool debug = false;
 	SGR_TRY(launch_compose_bwd(segments, grads, num_segments, M, poses, idft, flip, flip_quat, dL_dmeans3D, dL_drotations, dL_dscales,
-	                           dL_dopacities, dL_dshs, pose_scratch, dposes, st),
+	                           dL_dopacities, dL_dshs, pose_scratch, dposes, correction, dcorrection, st),
 	        "compose_bwd");
+	return SGR_OK;
+}
+
+int sgr_compose_backward(const SgrSegment *segments, const SgrSegmentGrads *grads, int32_t num_segments, int32_t M, const float *poses,
+                         const float *idft, const uint8_t *flip, const float *flip_quat, const float *dL_dmeans3D,
+                         const float *dL_drotations, const float *dL_dscales, const float *dL_dopacities, const float *dL_dshs,
+                         float *dposes, float *pose_scratch, void *stream) {
+	return compose_backward_impl("sgr_compose_backward", segments, grads, num_segments, M, poses, idft, flip, flip_quat, nullptr, dL_dmeans3D,
+	                             dL_drotations, dL_dscales, dL_dopacities, dL_dshs, dposes, nullptr, pose_scratch, stream);
+}
+
+int sgr_compose_backward_corrected(const SgrSegment *segments, const SgrSegmentGrads *grads, int32_t num_segments, int32_t M,
+                                   const float *poses, const float *idft, const uint8_t *flip, const float *flip_quat,
+                                   const float *bkgd_correction, const float *dL_dmeans3D, const float *dL_drotations, const float *dL_dscales,
+                                   const float *dL_dopacities, const float *dL_dshs, float *dposes, float *dcorrection, float *pose_scratch,
+                                   void *stream) {
+	if (!bkgd_correction || !dcorrection) return fail(SGR_EINVAL, "NULL bkgd_correction / dcorrection passed to sgr_compose_backward_corrected");
+	return compose_backward_impl("sgr_compose_backward_corrected", segments, grads, num_segments, M, poses, idft, flip, flip_quat, bkgd_correction,
+	                             dL_dmeans3D, dL_drotations, dL_dscales, dL_dopacities, dL_dshs, dposes, dcorrection, pose_scratch, stream);
+}
+
+int sgr_color_correct_forward(int32_t H, int32_t W, const float *image, const float *affine, float *out, void *stream) {
+	if (H <= 0 || W <= 0) return fail(SGR_EINVAL, "bad image size H=%d W=%d", H, W);
+	if (!image || !affine || !out) return fail(SGR_EINVAL, "NULL pointer passed to sgr_color_correct_forward");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_color_correct_fwd((int64_t)H * W, image, affine, out, st), "color_correct_fwd");
+	return SGR_OK;
+}
+
+size_t sgr_color_correct_scratch_bytes(int32_t H, int32_t W) { return (H > 0 && W > 0) ? color_correct_scratch_bytes((int64_t)H * W) : 0; }
+
+int sgr_color_correct_backward(int32_t H, int32_t W, const float *image, const float *affine, const float *dL_dout, float *dL_dimage,
+                               float *dL_daffine, void *scratch, size_t scratch_bytes, void *stream) {
+	if (H <= 0 || W <= 0) return fail(SGR_EINVAL, "bad image size H=%d W=%d", H, W);
+	if (!image || !affine || !dL_dout || !dL_daffine) return fail(SGR_EINVAL, "NULL pointer passed to sgr_color_correct_backward");
+	const int64_t N = (int64_t)H * W;
+	if (!scratch || scratch_bytes < color_correct_scratch_bytes(N))
+		return fail(SGR_ENOMEM, "colour correction scratch too small: %zu < %zu", scratch_bytes, color_correct_scratch_bytes(N));
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_color_correct_bwd(N, image, affine, dL_dout, dL_dimage, dL_daffine, scratch, st), "color_correct_bwd");
+	return SGR_OK;
+}
+
+int sgr_color_correction_reg(const float *affine, const float *affine_sky, float weight, float *value, float *g_affine, float *g_affine_sky,
+                             void *stream) {
+	if (!affine || !value) return fail(SGR_EINVAL, "NULL pointer passed to sgr_color_correction_reg");
+	if (affine_sky == nullptr && g_affine_sky != nullptr) return fail(SGR_EINVAL, "g_affine_sky given without affine_sky");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_color_correction_reg(affine, affine_sky, weight, value, g_affine, g_affine_sky, st), "color_correction_reg");
 	return SGR_OK;
 }
 

@@ -101,11 +101,22 @@ __device__ __forceinline__ void warp_copy_rows(const float *__restrict__ src, fl
 	}
 }
 
+// The learned per-image pose correction of the background (lib/models/camera_pose.py:89-114): q = F.normalize(corr[0:4]), then
+// quaternion_to_matrix normalises q a second time (no clamp: a zero correction gives NaN like the reference).
+__device__ __forceinline__ float4 correction_quat(const float *__restrict__ corr) {
+	const float4 c = make_float4(corr[0], corr[1], corr[2], corr[3]);
+	const float cn = qnorm_clamped(c);
+	return make_float4(c.x / cn, c.y / cn, c.z / cn, c.w / cn);
+}
+
+// CORRECTED: rows of unposed segments are moved by the correction `corr` (8 floats: q, t, pad); the other instantiation never
+// reads it, so its code is the composer's without a correction.
+template <bool CORRECTED>
 __global__ void __launch_bounds__(256) compose_fwd_kernel(const SegTable t, const int M, const float *__restrict__ poses,
                                                          const float *__restrict__ idft, const uint8_t *__restrict__ flip,
                                                          const float *__restrict__ flip_quat, float *__restrict__ o_xyz,
                                                          float *__restrict__ o_rot, float *__restrict__ o_scale, float *__restrict__ o_opac,
-                                                         float *__restrict__ o_sh) {
+                                                         float *__restrict__ o_sh, const float *__restrict__ corr) {
 	const int i = t.start[0] + blockIdx.x * blockDim.x + threadIdx.x;
 	const bool active = i < t.start[t.n];
 	const int lane = threadIdx.x & 31;
@@ -140,6 +151,14 @@ __global__ void __launch_bounds__(256) compose_fwd_kernel(const SegTable t, cons
 			q = qmul(qo, q);  // raw product with the (un-normalised) actor quaternion, then normalise (:324-325)
 			const float n2 = qnorm_clamped(q);
 			q = make_float4(q.x / n2, q.y / n2, q.z / n2, q.w / n2);
+		} else if (CORRECTED) {
+			// xyz' = [xyz, 1] @ [[R, t], [0, 0, 0, 1]]^T; rot' = qc (x) normalize(rot), not normalised again (camera_pose.py:89-114)
+			const float4 qc = correction_quat(corr);
+			float R[9];
+			quat_to_rot(qc, R);
+			p = make_float3(R[0] * p.x + R[1] * p.y + R[2] * p.z + corr[4], R[3] * p.x + R[4] * p.y + R[5] * p.z + corr[5],
+			                R[6] * p.x + R[7] * p.y + R[8] * p.z + corr[6]);
+			q = qmul(qc, q);
 		}
 		o_xyz[3 * g] = p.x; o_xyz[3 * g + 1] = p.y; o_xyz[3 * g + 2] = p.z;
 		*reinterpret_cast<float4 *>(o_rot + 4 * g) = q;
@@ -171,13 +190,15 @@ __global__ void __launch_bounds__(256) compose_fwd_kernel(const SegTable t, cons
 	}
 }
 
-// acc[16] per segment: G = sum g_xyz (x) x_local (9, row-major), g_a = sum over the rotation path (4), sum g_xyz (3)
+// acc[16] per segment: G = sum g_xyz (x) x_local (9, row-major), g_a = sum over the rotation path (4), sum g_xyz (3).
+// CORRECTED: the unposed rows add the same 16 sums for the correction into row `corr_row` of acc.
+template <bool CORRECTED>
 __global__ void __launch_bounds__(256) compose_bwd_kernel(const SegTable t, const SegGradTable gt, const int M, const float *__restrict__ poses,
                                                          const float *__restrict__ idft, const uint8_t *__restrict__ flip,
                                                          const float *__restrict__ flip_quat, const float *__restrict__ g_xyz,
                                                          const float *__restrict__ g_rot, const float *__restrict__ g_scale,
                                                          const float *__restrict__ g_opac, const float *__restrict__ g_sh,
-                                                         float *__restrict__ acc) {
+                                                         float *__restrict__ acc, const float *__restrict__ corr, const int corr_row) {
 	const int i = t.start[0] + blockIdx.x * blockDim.x + threadIdx.x;
 	const bool active = i < t.start[t.n];
 	const int lane = threadIdx.x & 31;
@@ -202,7 +223,7 @@ __global__ void __launch_bounds__(256) compose_bwd_kernel(const SegTable t, cons
 		const float4 raw = *reinterpret_cast<const float4 *>(sg.rotation + 4 * l);
 		float4 gn = *reinterpret_cast<const float4 *>(g_rot + 4 * g);  // gradient w.r.t. the composed (unit) rotation
 		float3 gx = make_float3(g_xyz[3 * g], g_xyz[3 * g + 1], g_xyz[3 * g + 2]);
-		float3 xl = posed ? make_float3(sg.xyz[3 * l], sg.xyz[3 * l + 1], sg.xyz[3 * l + 2]) : make_float3(0.f, 0.f, 0.f);
+		float3 xl = (posed || CORRECTED) ? make_float3(sg.xyz[3 * l], sg.xyz[3 * l + 1], sg.xyz[3 * l + 2]) : make_float3(0.f, 0.f, 0.f);
 		// activations (gaussian_model.py:224-251): d exp = exp, d sigmoid = o (1 - o)
 		og.scaling[3 * l] = gs.x * expf(ls.x); og.scaling[3 * l + 1] = gs.y * expf(ls.y); og.scaling[3 * l + 2] = gs.z * expf(ls.z);
 		const float o = 1.0f / (1.0f + expf(-lo));
@@ -251,6 +272,20 @@ __global__ void __launch_bounds__(256) compose_bwd_kernel(const SegTable t, cons
 			                        R[2] * gx.x + R[5] * gx.y + R[8] * gx.z);  // R^T g
 			if (fl) gl.y = -gl.y;
 			gx = gl;
+		} else if (CORRECTED) {
+			// rot' = qc (x) n without a final normalisation, xyz' = R(qc) x + t
+			const float4 qc = correction_quat(corr);
+			const float4 ga = qmul(gn, qconj(n));  // d/d qc
+			gn = qmul(qconj(qc), gn);              // d/d n
+			a16[9] = ga.x; a16[10] = ga.y; a16[11] = ga.z; a16[12] = ga.w;
+			float R[9];
+			quat_to_rot(qc, R);
+			a16[0] = gx.x * xl.x; a16[1] = gx.x * xl.y; a16[2] = gx.x * xl.z;
+			a16[3] = gx.y * xl.x; a16[4] = gx.y * xl.y; a16[5] = gx.y * xl.z;
+			a16[6] = gx.z * xl.x; a16[7] = gx.z * xl.y; a16[8] = gx.z * xl.z;
+			a16[13] = gx.x; a16[14] = gx.y; a16[15] = gx.z;
+			gx = make_float3(R[0] * gx.x + R[3] * gx.y + R[6] * gx.z, R[1] * gx.x + R[4] * gx.y + R[7] * gx.z,
+			                 R[2] * gx.x + R[5] * gx.y + R[8] * gx.z);
 		}
 		og.xyz[3 * l] = gx.x; og.xyz[3 * l + 1] = gx.y; og.xyz[3 * l + 2] = gx.z;
 		const float dn = n.x * gn.x + n.y * gn.y + n.z * gn.z + n.w * gn.w;  // through n = raw / max(|raw|, eps)
@@ -259,8 +294,44 @@ __global__ void __launch_bounds__(256) compose_bwd_kernel(const SegTable t, cons
 	}
 	// tracked-pose sums: one atomic per (warp, component) when the whole warp sits in one actor
 	const bool contiguous = warp_is_contiguous(s, li, active);
-	const bool any_posed = __any_sync(full, posed);
-	if (any_posed) {
+	if (CORRECTED) {
+		// Every active row contributes: actors to their own row, unposed rows to corr_row.  All background warps share corr_row, so
+		// the warps' sums are added per block first (in warp order) and a block issues one atomic per component and row.
+		__shared__ float wsum[8][16];
+		__shared__ int wrow[8];
+		const int warp = threadIdx.x >> 5;
+		const int row = posed ? t.first + s : corr_row;
+		const int r0 = __shfl_sync(full, row, 0);
+		const bool uniform = __all_sync(full, !active || row == r0) && __any_sync(full, active);
+#pragma unroll
+		for (int k = 0; k < 16; k++) {
+			float v = a16[k];
+#pragma unroll
+			for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(full, v, o);
+			if (lane == k) wsum[warp][k] = v;
+		}
+		if (lane == 0) wrow[warp] = uniform ? r0 : -1;
+		if (!uniform && active) {
+#pragma unroll
+			for (int k = 0; k < 16; k++) atomicAdd(acc + (size_t)row * 16 + k, a16[k]);
+		}
+		__syncthreads();
+		if (threadIdx.x < 16) {
+			const int k = threadIdx.x, nw = blockDim.x >> 5;
+			int cur = -1;
+			float v = 0.f;
+			for (int w = 0; w < nw; w++) {
+				if (wrow[w] < 0) continue;
+				if (wrow[w] != cur) {
+					if (cur >= 0) atomicAdd(acc + (size_t)cur * 16 + k, v);
+					cur = wrow[w];
+					v = 0.f;
+				}
+				v += wsum[w][k];
+			}
+			if (cur >= 0) atomicAdd(acc + (size_t)cur * 16 + k, v);
+		}
+	} else if (__any_sync(full, posed)) {
 		const int s0 = __shfl_sync(full, s, 0);
 		const bool uniform = __all_sync(full, !active || s == s0);
 		if (uniform) {
@@ -292,8 +363,43 @@ __global__ void __launch_bounds__(256) compose_bwd_kernel(const SegTable t, cons
 // acc[16] -> d pose (4 + 3, padded to 8): the matrix path goes through quaternion_to_matrix's normalisation.  One warp per group of
 // kMaxSeg segments; bit k of `posed` is segment first + k.  Rows of unposed segments are written as zeros: their pose row is not
 // read by the other kernels and may hold anything, a zero quaternion included (composer.py leaves the background's row zero).
+// d/d ps of the matrix part: G through quaternion_to_matrix(ps) and its normalisation of ps.  The actor rows below write the same
+// map out in place: moving them onto this function reorders their instructions, and the plain composer's code stays as it was.
+__device__ __forceinline__ float4 matrix_path_grad(const float *__restrict__ a, const float *__restrict__ ps) {
+	const float nr = sqrtf(ps[0] * ps[0] + ps[1] * ps[1] + ps[2] * ps[2] + ps[3] * ps[3]);
+	const float w = ps[0] / nr, x = ps[1] / nr, y = ps[2] / nr, z = ps[3] / nr;
+	const float G00 = a[0], G01 = a[1], G02 = a[2], G10 = a[3], G11 = a[4], G12 = a[5], G20 = a[6], G21 = a[7], G22 = a[8];
+	const float dw = 2.f * (-z * G01 + y * G02 + z * G10 - x * G12 - y * G20 + x * G21);
+	const float dx = 2.f * (y * G01 + z * G02 + y * G10 - 2.f * x * G11 - w * G12 + z * G20 + w * G21 - 2.f * x * G22);
+	const float dy = 2.f * (-2.f * y * G00 + x * G01 + w * G02 + x * G10 + z * G12 - w * G20 + z * G21 - 2.f * y * G22);
+	const float dz = 2.f * (-2.f * z * G00 - w * G01 + x * G02 + w * G10 - 2.f * z * G11 + y * G12 + x * G20 + y * G21);
+	const float dot = w * dw + x * dx + y * dy + z * dz;
+	return make_float4((dw - w * dot) / nr, (dx - x * dot) / nr, (dy - y * dot) / nr, (dz - z * dot) / nr);
+}
+
+// CORRECTED: thread kMaxSeg of the launch that gets a non-NULL `dcorr` turns acc row `corr_row` into the correction's gradient
+// (8 floats: q, t, pad).  The rotation path's sums are already d/d qc; qc = F.normalize(corr[0:4]) is the one extra stage.
+template <bool CORRECTED>
 __global__ void compose_pose_finalize_kernel(const int first, const int n, const unsigned posed, const float *__restrict__ poses,
-                                             const float *__restrict__ acc, float *__restrict__ dposes) {
+                                             const float *__restrict__ acc, float *__restrict__ dposes, const float *__restrict__ corr,
+                                             float *__restrict__ dcorr, const int corr_row) {
+	if (CORRECTED && threadIdx.x == kMaxSeg) {
+		if (dcorr == nullptr) return;
+		const float *a = acc + (size_t)corr_row * 16;
+		const float4 qc = correction_quat(corr);
+		const float qv[4] = {qc.x, qc.y, qc.z, qc.w};
+		const float4 m = matrix_path_grad(a, qv);
+		const float4 gq = make_float4(a[9] + m.x, a[10] + m.y, a[11] + m.z, a[12] + m.w);  // d/d qc
+		const float cn = sqrtf(corr[0] * corr[0] + corr[1] * corr[1] + corr[2] * corr[2] + corr[3] * corr[3]);
+		if (cn >= 1e-12f) {  // F.normalize's backward; below its clamp the norm is a constant
+			const float dot = qc.x * gq.x + qc.y * gq.y + qc.z * gq.z + qc.w * gq.w;
+			dcorr[0] = (gq.x - qc.x * dot) / cn; dcorr[1] = (gq.y - qc.y * dot) / cn; dcorr[2] = (gq.z - qc.z * dot) / cn; dcorr[3] = (gq.w - qc.w * dot) / cn;
+		} else {
+			dcorr[0] = gq.x / 1e-12f; dcorr[1] = gq.y / 1e-12f; dcorr[2] = gq.z / 1e-12f; dcorr[3] = gq.w / 1e-12f;
+		}
+		dcorr[4] = a[13]; dcorr[5] = a[14]; dcorr[6] = a[15]; dcorr[7] = 0.f;
+		return;
+	}
 	if ((int)threadIdx.x >= n) return;
 	const size_t s = (size_t)first + threadIdx.x;
 	float *o = dposes + s * 8;
@@ -328,22 +434,28 @@ static void fill_table(SegTable &t, const SgrSegment *segs, int first, int n) {
 }
 
 cudaError_t launch_compose_fwd(const SgrSegment *segs, int nseg, int M, const float *poses, const float *idft, const uint8_t *flip,
-                               const float *flip_quat, float *xyz, float *rot, float *scale, float *opac, float *sh, cudaStream_t st) {
+                               const float *flip_quat, float *xyz, float *rot, float *scale, float *opac, float *sh, const float *corr,
+                               cudaStream_t st) {
 	for (int first = 0; first < nseg; first += kMaxSeg) {
 		SegTable t;
 		fill_table(t, segs, first, nseg - first < kMaxSeg ? nseg - first : kMaxSeg);
 		const int count = t.start[t.n] - t.start[0];
 		if (count <= 0) continue;
 		count_launch();
-		compose_fwd_kernel<<<(count + 255) / 256, 256, 0, st>>>(t, M, poses, idft, flip, flip_quat, xyz, rot, scale, opac, sh);
+		if (corr)
+			compose_fwd_kernel<true><<<(count + 255) / 256, 256, 0, st>>>(t, M, poses, idft, flip, flip_quat, xyz, rot, scale, opac, sh, corr);
+		else
+			compose_fwd_kernel<false><<<(count + 255) / 256, 256, 0, st>>>(t, M, poses, idft, flip, flip_quat, xyz, rot, scale, opac, sh, nullptr);
 	}
 	return cudaGetLastError();
 }
 
 cudaError_t launch_compose_bwd(const SgrSegment *segs, const SgrSegmentGrads *grads, int nseg, int M, const float *poses, const float *idft,
                                const uint8_t *flip, const float *flip_quat, const float *g_xyz, const float *g_rot, const float *g_scale,
-                               const float *g_opac, const float *g_sh, float *acc, float *dposes, cudaStream_t st) {
-	cudaError_t e = cudaMemsetAsync(acc, 0, (size_t)nseg * 16 * sizeof(float), st);
+                               const float *g_opac, const float *g_sh, float *acc, float *dposes, const float *corr, float *dcorr,
+                               cudaStream_t st) {
+	// with a correction, acc has one more row (index nseg) for the sums of the unposed rows
+	cudaError_t e = cudaMemsetAsync(acc, 0, (size_t)(nseg + (corr ? 1 : 0)) * 16 * sizeof(float), st);
 	if (e != cudaSuccess) return e;
 	for (int first = 0; first < nseg; first += kMaxSeg) {
 		SegTable t;
@@ -357,14 +469,23 @@ cudaError_t launch_compose_bwd(const SgrSegment *segs, const SgrSegmentGrads *gr
 		const int count = t.start[t.n] - t.start[0];
 		if (count <= 0) continue;
 		count_launch();
-		compose_bwd_kernel<<<(count + 255) / 256, 256, 0, st>>>(t, gt, M, poses, idft, flip, flip_quat, g_xyz, g_rot, g_scale, g_opac, g_sh, acc);
+		if (corr)
+			compose_bwd_kernel<true><<<(count + 255) / 256, 256, 0, st>>>(t, gt, M, poses, idft, flip, flip_quat, g_xyz, g_rot, g_scale, g_opac, g_sh,
+			                                                               acc, corr, nseg);
+		else
+			compose_bwd_kernel<false><<<(count + 255) / 256, 256, 0, st>>>(t, gt, M, poses, idft, flip, flip_quat, g_xyz, g_rot, g_scale, g_opac,
+			                                                                g_sh, acc, nullptr, 0);
 	}
 	for (int first = 0; first < nseg; first += kMaxSeg) {
 		const int n = nseg - first < kMaxSeg ? nseg - first : kMaxSeg;
 		unsigned posed = 0;
 		for (int k = 0; k < n; k++) posed |= (segs[first + k].posed ? 1u : 0u) << k;
 		count_launch();
-		compose_pose_finalize_kernel<<<1, kMaxSeg, 0, st>>>(first, n, posed, poses, acc, dposes);
+		if (corr)  // the last group's extra thread finalizes the correction
+			compose_pose_finalize_kernel<true><<<1, kMaxSeg + 1, 0, st>>>(first, n, posed, poses, acc, dposes, corr,
+			                                                              first + n == nseg ? dcorr : nullptr, nseg);
+		else
+			compose_pose_finalize_kernel<false><<<1, kMaxSeg, 0, st>>>(first, n, posed, poses, acc, dposes, nullptr, nullptr, 0);
 	}
 	return cudaGetLastError();
 }

@@ -357,10 +357,18 @@ cudaError_t launch_layer_fill(const FrameDev &f, const float *bg, float *color, 
 cudaError_t launch_layer_stash(const float *grad2d, int lo, int hi, float *stash, bool restore, float *dL_dmeans2D, cudaStream_t st);
 cudaError_t launch_layer_merge(float *grad2d, const SgrLayerGrad *layers, int n, cudaStream_t st);
 cudaError_t launch_compose_fwd(const SgrSegment *segs, int nseg, int M, const float *poses, const float *idft, const uint8_t *flip,
-                               const float *flip_quat, float *xyz, float *rot, float *scale, float *opac, float *sh, cudaStream_t st);
+                               const float *flip_quat, float *xyz, float *rot, float *scale, float *opac, float *sh, const float *corr,
+                               cudaStream_t st);
 cudaError_t launch_compose_bwd(const SgrSegment *segs, const SgrSegmentGrads *grads, int nseg, int M, const float *poses, const float *idft,
                                const uint8_t *flip, const float *flip_quat, const float *g_xyz, const float *g_rot, const float *g_scale,
-                               const float *g_opac, const float *g_sh, float *acc, float *dposes, cudaStream_t st);
+                               const float *g_opac, const float *g_sh, float *acc, float *dposes, const float *corr, float *dcorr,
+                               cudaStream_t st);
+cudaError_t launch_color_correct_fwd(int64_t N, const float *image, const float *affine, float *out, cudaStream_t st);
+size_t color_correct_scratch_bytes(int64_t N);
+cudaError_t launch_color_correct_bwd(int64_t N, const float *image, const float *affine, const float *g_out, float *g_image, float *g_affine,
+                                     void *scratch, cudaStream_t st);
+cudaError_t launch_color_correction_reg(const float *affine, const float *affine_sky, float weight, float *value, float *g_affine,
+                                        float *g_affine_sky, cudaStream_t st);
 size_t image_loss_scratch_bytes(int C, int H, int W);
 cudaError_t launch_image_loss(int C, int H, int W, const float *img, const float *gt, const uint8_t *mask, float w_l1, float w_ssim, float *grad,
                               float *scalars, void *scratch, cudaStream_t st);

@@ -38,6 +38,18 @@ poses = torch.randn(3, 7, device=dev, requires_grad=True)
 out = sgb.compose(models, poses, torch.randn(3, 5, device=dev), torch.rand(538, device=dev) < 0.5, torch.tensor([0.0, 0.0, 1.0, 0.0], device=dev))
 sum(o.sum() for o in out).backward()
 print("compose ok", float(out[0].abs().sum()), float(poses.grad.abs().sum()))
+# the corrected composer (background pose correction, 40 actors: two segment groups) and the colour correction with its regularisation
+models = [{k: v.to(dev).requires_grad_(True) for k, v in m.items()} for m in CC.make_case(4, 777, [13] * 40, 9, 3)]
+poses = torch.randn(40, 7, device=dev, requires_grad=True)
+corr = (torch.tensor([0.9, 0.1, -0.2, 0.3], device=dev, requires_grad=True), torch.randn(3, device=dev, requires_grad=True))
+out = sgb.compose(models, poses, torch.randn(40, 3, device=dev), torch.rand(520, device=dev) < 0.5, torch.tensor([0.0, 0.0, 1.0, 0.0], device=dev),
+                  pose_correction=corr)
+sum(o.sum() for o in out).backward()
+aff = (torch.eye(4, device=dev)[:3] + 0.1).requires_grad_(True)
+for hw in ((70, 93), (64, 96)):
+    img = torch.rand(3, *hw, device=dev, requires_grad=True)
+    (sgb.color_correct(img, aff).sum() + sgb.color_correction_reg_loss(aff, aff * 0.5, 0.1)).backward()
+print("corrections ok", float(corr[0].grad.abs().sum()), float(aff.grad.abs().sum()))
 img = torch.rand(3, 70, 93, device=dev, requires_grad=True)
 l = losses.photometric_loss(img, torch.rand(3, 70, 93, device=dev), torch.rand(1, 70, 93, device=dev) > 0.3) + losses.sky_loss(img[:1], torch.rand(1, 70, 93, device=dev) > 0.5)
 l.backward()
