@@ -1,4 +1,4 @@
-// binning.cu — depth pre-sort, instance offsets, (tile, gaussian) pair emission, 2-pass stable tile sort, per-tile ranges.
+// binning.cu — depth pre-sort, instance offsets, (tile, gaussian) pair emission, stable tile bucketing, per-tile ranges.
 //
 // Replaces the reference's cub InclusiveSum + duplicateWithKeys + 64-bit cub SortPairs + identifyTileRanges
 // (DGR/cuda_rasterizer/rasterizer_impl.cu:278-321, 70-138).  The reference sorts all R instances on a 46-bit
@@ -6,10 +6,14 @@
 // where they are cheapest:
 //   1. the P Gaussians are sorted ONCE by their 32-bit depth bits (stable radix sort, ties keep ascending index);
 //   2. instances are emitted in that order, so the unsorted list is already depth-ordered;
-//   3. a STABLE radix sort on the tile id alone (<= 16 bits -> 2 passes, 16 B per instance per pass) then yields exactly
-//      the reference's order: ascending tile, within a tile ascending depth bits, ties by ascending Gaussian index.
+//   3. a STABLE sort on the tile id alone then yields exactly the reference's order: ascending tile, within a tile ascending
+//      depth bits, ties by ascending Gaussian index.  Frames of at most kBucketMaxTiles tiles bucket the emitted instances
+//      (launch_bucketing: two 7-bit digit passes, ranges from the tile histogram); larger ones take a cub radix sort over the
+//      whole list and find the ranges in the sorted keys.
 // Integer / bit work: the resulting per-tile lists equal the reference's lists minus the instances removed by the
 // exact cull (tile_visit.cuh); tests/test_parity_gpu.py checks images bit-for-bit / to 1e-6 against the reference.
+#include <cub/block/block_radix_rank.cuh>
+#include <cub/block/block_scan.cuh>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
@@ -34,6 +38,10 @@ struct WasDelivered {  // (predicate of the round-2 second-cut stream compaction
 	__host__ __device__ __forceinline__ bool operator()(int i) const { return radii[i] > 0; }
 };
 using CountIter = cub::TransformInputIterator<uint32_t, GatherCount, cub::CountingInputIterator<int>>;
+
+// Frames of up to this many tiles bucket their instances by tile (launch_bucketing below): the per-tile histogram and cursors
+// live in shared memory (64 KB).  Larger frames take the tile radix sort.
+constexpr int kBucketMaxTiles = 16384;
 
 size_t geom_temp_bytes(int P) {
 	const int n = P > 0 ? P : 1;
@@ -370,6 +378,299 @@ static int bits_for(uint32_t n) {  // smallest b with (1 << b) >= n, i.e. enough
 	return b > 0 ? b : 1;
 }
 
+// ---- tile bucketing: the per-tile lists as a stable LSD radix sort of the EMITTED instances [0, E) on two 7-bit digits ----
+// Emission already writes the instances in their final within-tile order (ascending depth bits, ties by ascending index), so a
+// stable bucketing by tile id gives exactly the list the tile radix sort gives, over E instead of the whole capacity and without
+// padding.  A single ranked scatter straight into the ~10^4 tile buckets writes isolated words (a partition holds ~3 instances of
+// a tile); on config C it took 0.40 ms on an H100, more than the radix sort it replaces.  Two passes over 128 buckets write runs.
+//   1. bucket_count<TILES>:  [0, E) is cut into partitions of kBucketPart instances; CTA p counts its partition's tile ids in a
+//                            shared-memory histogram, writes row p of the (partition x tile) matrix and of the (partition x low
+//                            digit) matrix;
+//   2. bucket_columns:       per column, the total over the partitions (the tile totals -> ranges[t].y; the digit totals), and
+//                            for the digit matrices the exclusive prefix over the partitions, in place;
+//   3. bucket_ranges:        one CTA scans the tile totals into `ranges` ((0, 0) for a tile without instances);
+//   4. bucket_pass<false>:   CTA p walks its partition in rounds; a stable match-based block rank of the round on the low digit
+//                            gives every instance its position among equal digits, added to the digit's running cursor in shared
+//                            memory; the Gaussian index with the high digit in its top 7 bits goes to the digit-ordered
+//                            intermediate array (frames of at most 2^25 Gaussians; larger ones take the radix sort);
+//   5. bucket_count<false>, bucket_columns, bucket_pass<true>: the same on the high digit of the intermediate array, writing the
+//                            Gaussian indices into vals_out.
+// Positions come from ranks and prefix sums only, never from the order of atomics.  E is read on the device (status[3]) and the
+// grids are sized from the capacity, so the bounded mode stays free of host synchronisation.
+constexpr uint32_t kBucketPart = 32768;  // instances per partition (whole rounds)
+constexpr int kBucketThreads = 512;  // histogram CTAs
+constexpr int kPassThreads = 256;    // rank-and-scatter CTAs: 72 registers, 3 CTAs per SM
+constexpr int kDigitBits = 7, kDigits = 1 << kDigitBits;
+constexpr int kPassItems = 8;
+constexpr uint32_t kPassRound = kPassThreads * kPassItems;
+static_assert(kBucketPart % kPassRound == 0, "partitions are whole rounds");
+static_assert(kBucketMaxTiles <= (1 << (2 * kDigitBits)), "two digits cover every tile id of a bucketed frame");
+constexpr uint32_t kNoGaussian = 0xffffffffu;  // value of the slots of the last round past E
+// the intermediate words carry the high digit in their top 7 bits, so a bucketed frame has at most 2^25 Gaussians
+constexpr int kPackShift = 32 - kDigitBits;
+constexpr uint32_t kPackMask = (1u << kPackShift) - 1u;
+
+// the bucketing scratch behind the cub temp of the binning state (carve_bin): the count matrices and the digit totals.  Sized for
+// kBucketMaxTiles tiles, so that it does not depend on the frame.
+struct BucketScratch {
+	uint32_t *tile_counts, *digit_counts[2], *digit_totals[2];
+	size_t bytes;
+};
+static BucketScratch carve_bucket(void *base, int64_t slots) {
+	BucketScratch s;
+	char *p = reinterpret_cast<char *>(base);
+	const size_t n = slots > 0 ? (size_t)slots : 1, nparts = (n + kBucketPart - 1) / kBucketPart;
+	auto take = [&](size_t bytes) { char *r = p; p += align_up(bytes); return r; };
+	s.tile_counts = reinterpret_cast<uint32_t *>(take(nparts * kBucketMaxTiles * sizeof(uint32_t)));
+	for (int i = 0; i < 2; i++) s.digit_counts[i] = reinterpret_cast<uint32_t *>(take(nparts * kDigits * sizeof(uint32_t)));
+	for (int i = 0; i < 2; i++) s.digit_totals[i] = reinterpret_cast<uint32_t *>(take(kDigits * sizeof(uint32_t)));
+	s.bytes = (size_t)(p - reinterpret_cast<char *>(base));
+	return s;
+}
+size_t bucket_scratch_bytes(int64_t slots) { return carve_bucket(nullptr, slots).bytes; }
+
+template <bool TILES>
+__global__ void __launch_bounds__(kBucketThreads) bucket_count_kernel(const uint16_t *__restrict__ keys, const uint32_t *__restrict__ status,
+                                                                    const uint32_t ntile, uint32_t *__restrict__ tile_counts,
+                                                                    uint32_t *__restrict__ digit_counts) {
+	extern __shared__ uint32_t s_hist[];  // TILES: per tile id of keys_in; else per high digit of the intermediate words
+	const uint32_t E = status[3];
+	const uint32_t begin = blockIdx.x * kBucketPart;
+	if (begin >= E) return;  // (rows past the last partition are never read)
+	const uint32_t end = min(begin + kBucketPart, E);
+	const uint32_t nbin = TILES ? ntile : (uint32_t)kDigits;
+	for (uint32_t t = threadIdx.x; t < nbin; t += kBucketThreads) s_hist[t] = 0u;
+	__syncthreads();
+	if (!TILES) {
+		const uint32_t *words = reinterpret_cast<const uint32_t *>(keys);
+		for (uint32_t i = begin + threadIdx.x * 4u; i < end; i += kBucketThreads * 4u) {
+			if (i + 4u <= end) {
+				const uint4 v = *reinterpret_cast<const uint4 *>(words + i);
+				atomicAdd(&s_hist[v.x >> kPackShift], 1u); atomicAdd(&s_hist[v.y >> kPackShift], 1u);
+				atomicAdd(&s_hist[v.z >> kPackShift], 1u); atomicAdd(&s_hist[v.w >> kPackShift], 1u);
+			} else {
+				for (uint32_t j = i; j < end; j++) atomicAdd(&s_hist[words[j] >> kPackShift], 1u);
+			}
+		}
+	} else
+	for (uint32_t i = begin + threadIdx.x * 8u; i < end; i += kBucketThreads * 8u) {
+		if (i + 8u <= end) {  // begin is a multiple of 8 and keys is 256-B aligned: one 16-B load of 8 tile ids
+			const uint4 v = *reinterpret_cast<const uint4 *>(keys + i);
+			atomicAdd(&s_hist[v.x & 0xffffu], 1u); atomicAdd(&s_hist[v.x >> 16], 1u);
+			atomicAdd(&s_hist[v.y & 0xffffu], 1u); atomicAdd(&s_hist[v.y >> 16], 1u);
+			atomicAdd(&s_hist[v.z & 0xffffu], 1u); atomicAdd(&s_hist[v.z >> 16], 1u);
+			atomicAdd(&s_hist[v.w & 0xffffu], 1u); atomicAdd(&s_hist[v.w >> 16], 1u);
+		} else {
+			for (uint32_t j = i; j < end; j++) atomicAdd(&s_hist[keys[j]], 1u);
+		}
+	}
+	__syncthreads();
+	uint32_t *drow = digit_counts + (size_t)blockIdx.x * kDigits;
+	if (TILES) {
+		uint32_t *row = tile_counts + (size_t)blockIdx.x * ntile;
+		for (uint32_t t = threadIdx.x; t < ntile; t += kBucketThreads) row[t] = s_hist[t];
+		for (uint32_t d = threadIdx.x; d < (uint32_t)kDigits; d += kBucketThreads) {  // low digit = tile id mod 128
+			uint32_t sum = 0u;
+			for (uint32_t t = d; t < ntile; t += kDigits) sum += s_hist[t];
+			drow[d] = sum;
+		}
+	} else {
+		for (uint32_t d = threadIdx.x; d < (uint32_t)kDigits; d += kBucketThreads) drow[d] = s_hist[d];
+	}
+}
+
+// 32 columns per CTA (one per lane: coalesced rows), the partitions split into 32 contiguous slices (one per warp).  Each warp sums
+// its slice and the slice totals are scanned across the warps in shared memory: totals[c * stride] = the column total and, with
+// `prefix`, the slice is rewritten as the exclusive prefix over the partitions.
+__global__ void __launch_bounds__(1024) bucket_columns_kernel(uint32_t *__restrict__ counts, const uint32_t *__restrict__ status,
+                                                             const uint32_t ncol, uint32_t *__restrict__ totals, const uint32_t stride,
+                                                             const bool prefix) {
+	__shared__ uint32_t s_tot[32][33];
+	const uint32_t nparts = (status[3] + kBucketPart - 1) / kBucketPart;
+	const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+	const uint32_t c = blockIdx.x * 32u + lane;
+	const uint32_t per = (nparts + 31u) / 32u;
+	const uint32_t p0 = min(w * per, nparts), p1 = min(p0 + per, nparts);
+	uint32_t sum = 0u;
+	if (c < ncol) {
+#pragma unroll 4
+		for (uint32_t p = p0; p < p1; p++) sum += counts[(size_t)p * ncol + c];
+	}
+	s_tot[w][lane] = sum;
+	__syncthreads();
+	uint32_t run = 0u;
+	for (uint32_t v = 0; v < w; v++) run += s_tot[v][lane];
+	if (c >= ncol) return;
+	if (w == 31u) totals[(size_t)c * stride] = run + sum;
+	if (!prefix) return;
+	for (uint32_t p = p0; p < p1; p++) {
+		const uint32_t x = counts[(size_t)p * ncol + c];
+		counts[(size_t)p * ncol + c] = run;
+		run += x;
+	}
+}
+
+// one CTA: ranges[t] = (start, start + total) from the exclusive scan of the tile totals in ranges[t].y, (0, 0) for a tile without
+// instances.  Warp w owns tiles [512 w, 512 w + 512), read and written 32 consecutive tiles at a time.
+constexpr int kRangesPerLane = kBucketMaxTiles / (32 * 32);
+__global__ void __launch_bounds__(1024) bucket_ranges_kernel(uint2 *__restrict__ ranges, const uint32_t ntile) {
+	__shared__ uint32_t s_warp[32];
+	const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+	const uint32_t seg = w * 32u * kRangesPerLane;
+	uint32_t tot[kRangesPerLane], excl[kRangesPerLane];
+#pragma unroll
+	for (int j = 0; j < kRangesPerLane; j++) {
+		const uint32_t t = seg + j * 32u + lane;
+		tot[j] = t < ntile ? ranges[t].y : 0u;
+	}
+	uint32_t carry = 0u;
+#pragma unroll
+	for (int j = 0; j < kRangesPerLane; j++) {
+		uint32_t inc = tot[j];
+#pragma unroll
+		for (int o = 1; o < 32; o <<= 1) {
+			const uint32_t y = __shfl_up_sync(0xffffffffu, inc, o);
+			if (lane >= (uint32_t)o) inc += y;
+		}
+		excl[j] = carry + inc - tot[j];
+		carry += __shfl_sync(0xffffffffu, inc, 31);
+	}
+	if (lane == 0) s_warp[w] = carry;
+	__syncthreads();
+	if (w == 0) {
+		const uint32_t x = s_warp[lane];
+		uint32_t inc = x;
+#pragma unroll
+		for (int o = 1; o < 32; o <<= 1) {
+			const uint32_t y = __shfl_up_sync(0xffffffffu, inc, o);
+			if (lane >= (uint32_t)o) inc += y;
+		}
+		s_warp[lane] = inc - x;
+	}
+	__syncthreads();
+	const uint32_t base = s_warp[w];
+#pragma unroll
+	for (int j = 0; j < kRangesPerLane; j++) {
+		const uint32_t t = seg + j * 32u + lane;
+		if (t < ntile) ranges[t] = tot[j] ? make_uint2(base + excl[j], base + excl[j] + tot[j]) : make_uint2(0u, 0u);
+	}
+}
+
+struct TileDigit {
+	int shift;
+	__device__ __forceinline__ uint32_t Digit(uint32_t key) const { return (key >> shift) & (kDigits - 1); }
+};
+
+// HIGH = false: (keys, vals) -> out by the low digit, out = Gaussian | high digit << 25; HIGH = true: (-, vals = those words) -> out
+// = Gaussian by the high digit.
+// prefix[p * 128 + d] = instances of digit d in the partitions before p; totals[d] = instances of digit d.
+// A round is held warp-striped (warp w: instances base + 256 w + 32 j + lane), the order in which the match-based block rank
+// counts, so the ranks are stable; the round is then staged in shared memory in digit order and written out in runs.
+template <bool HIGH>
+__global__ void __launch_bounds__(kPassThreads) bucket_pass_kernel(const uint16_t *__restrict__ keys, const uint32_t *__restrict__ vals,
+                                                                   const uint32_t *__restrict__ status, const uint32_t *__restrict__ prefix,
+                                                                   const uint32_t *__restrict__ totals, uint32_t *__restrict__ out) {
+	constexpr int kShift = HIGH ? kDigitBits : 0;
+	using Rank = cub::BlockRadixRankMatch<kPassThreads, kDigitBits, false>;
+	__shared__ typename Rank::TempStorage tmp;
+	__shared__ uint32_t s_vals[kPassRound];
+	__shared__ uint16_t s_keys[kPassRound];
+	__shared__ uint32_t s_cursor[kDigits];  // per digit: output position of the first instance of this round
+	__shared__ uint32_t s_pref[kDigits];    // per digit: its first position in the round's digit order
+	const uint32_t E = status[3];
+	const uint32_t begin = blockIdx.x * kBucketPart;
+	if (begin >= E) return;
+	const uint32_t end = min(begin + kBucketPart, E);
+	const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+	if (threadIdx.x < 32) {  // digit starts (exclusive scan of the totals, 4 digits per lane) + this partition's prefix
+		const uint4 t4 = reinterpret_cast<const uint4 *>(totals)[lane];
+		const uint32_t sum = t4.x + t4.y + t4.z + t4.w;
+		uint32_t inc = sum;
+#pragma unroll
+		for (int o = 1; o < 32; o <<= 1) {
+			const uint32_t y = __shfl_up_sync(0xffffffffu, inc, o);
+			if (lane >= (uint32_t)o) inc += y;
+		}
+		const uint4 p4 = reinterpret_cast<const uint4 *>(prefix + (size_t)blockIdx.x * kDigits)[lane];
+		uint32_t x = inc - sum;
+		s_cursor[4 * lane + 0] = x + p4.x; x += t4.x;
+		s_cursor[4 * lane + 1] = x + p4.y; x += t4.y;
+		s_cursor[4 * lane + 2] = x + p4.z; x += t4.z;
+		s_cursor[4 * lane + 3] = x + p4.w;
+	}
+	uint32_t k[kPassItems], v[kPassItems];
+	// the round's instances, warp-striped; called for the next round as soon as this one is staged in shared memory, so that the
+	// loads overlap the stores
+	auto load = [&](const uint32_t base) {
+#pragma unroll
+		for (int j = 0; j < kPassItems; j++) {
+			const uint32_t i = base + warp * (32u * kPassItems) + j * 32u + lane;
+			const bool in = i < end;  // slots past E: the largest digit, behind every real instance of it, written nowhere
+			if (HIGH) {
+				const uint32_t x = in ? vals[i] : 0u;
+				k[j] = in ? (x >> kPackShift) << kDigitBits : 0xffffu;
+				v[j] = in ? x & kPackMask : kNoGaussian;
+			} else {
+				k[j] = in ? (uint32_t)keys[i] : 0xffffu;
+				v[j] = in ? vals[i] : kNoGaussian;
+			}
+		}
+	};
+	load(begin);
+	for (uint32_t base = begin; base < end; base += kPassRound) {
+		int rank[kPassItems];
+		int pref[Rank::BINS_TRACKED_PER_THREAD];
+		Rank(tmp).RankKeys(k, rank, TileDigit{kShift}, pref);
+		if (threadIdx.x < kDigits) s_pref[threadIdx.x] = (uint32_t)pref[0];
+#pragma unroll
+		for (int j = 0; j < kPassItems; j++) {
+			s_vals[rank[j]] = v[j];
+			s_keys[rank[j]] = (uint16_t)k[j];
+		}
+		if (base + kPassRound < end) load(base + kPassRound);
+		__syncthreads();
+		// position q of the round's digit order holds the (q - pref[d])-th instance of digit d in this round
+#pragma unroll
+		for (int j = 0; j < kPassItems; j++) {
+			const uint32_t q = j * kPassThreads + threadIdx.x;
+			const uint32_t val = s_vals[q];
+			if (val == kNoGaussian) continue;
+			const uint32_t key = s_keys[q], d = (key >> kShift) & (kDigits - 1);
+			const uint32_t pos = s_cursor[d] + q - s_pref[d];
+			out[pos] = HIGH ? val : val | (key >> kDigitBits) << kPackShift;
+		}
+		__syncthreads();
+		if (threadIdx.x < kDigits)
+			s_cursor[threadIdx.x] += (threadIdx.x + 1 < kDigits ? s_pref[threadIdx.x + 1] : kPassRound) - s_pref[threadIdx.x];
+		__syncthreads();
+	}
+}
+
+// 16-bit tile ids, at most kBucketMaxTiles tiles and 2^25 Gaussians.  The intermediate words live in keys_out, the count matrices
+// and totals in the bucketing scratch.
+static cudaError_t launch_bucketing(const BinView &b, ImgView img, const uint32_t *status, int ntile, int64_t slots, cudaStream_t st) {
+	static std::atomic<uint64_t> smem_count{0};
+	cudaError_t e;
+	if ((e = ensure_dynamic_smem(bucket_count_kernel<true>, kBucketMaxTiles * sizeof(uint32_t), smem_count)) != cudaSuccess) return e;
+	const BucketScratch sc = carve_bucket(b.bucket, slots);
+	const unsigned nparts = (unsigned)((slots + kBucketPart - 1) / kBucketPart);
+	const uint16_t *keys = reinterpret_cast<const uint16_t *>(b.keys_in);
+	count_launch(8);
+	bucket_count_kernel<true><<<nparts, kBucketThreads, (size_t)ntile * sizeof(uint32_t), st>>>(keys, status, (uint32_t)ntile, sc.tile_counts,
+	                                                                                          sc.digit_counts[0]);
+	bucket_columns_kernel<<<(unsigned)((ntile + 31) / 32), 1024, 0, st>>>(sc.tile_counts, status, (uint32_t)ntile,
+	                                                                      reinterpret_cast<uint32_t *>(img.ranges) + 1, 2u, false);
+	bucket_ranges_kernel<<<1, 1024, 0, st>>>(img.ranges, (uint32_t)ntile);
+	bucket_columns_kernel<<<kDigits / 32, 1024, 0, st>>>(sc.digit_counts[0], status, kDigits, sc.digit_totals[0], 1u, true);
+	uint32_t *mid = b.keys_out;
+	bucket_pass_kernel<false><<<nparts, kPassThreads, 0, st>>>(keys, b.vals_in, status, sc.digit_counts[0], sc.digit_totals[0], mid);
+	bucket_count_kernel<false><<<nparts, kBucketThreads, kDigits * sizeof(uint32_t), st>>>(reinterpret_cast<const uint16_t *>(mid), status,
+	                                                                                     0u, nullptr, sc.digit_counts[1]);
+	bucket_columns_kernel<<<kDigits / 32, 1024, 0, st>>>(sc.digit_counts[1], status, kDigits, sc.digit_totals[1], 1u, true);
+	bucket_pass_kernel<true><<<nparts, kPassThreads, 0, st>>>(nullptr, mid, status, sc.digit_counts[1], sc.digit_totals[1], b.vals_out);
+	return cudaGetLastError();
+}
+
 cudaError_t launch_binning(const FrameDev &f, GeomView g, const int32_t *radii, BinView b, ImgView img, int64_t R, cudaStream_t st,
                            int64_t cap, int n_order) {
 	if (n_order < 0) n_order = f.P;
@@ -390,7 +691,15 @@ cudaError_t launch_binning(const FrameDev &f, GeomView g, const int32_t *radii, 
 	if ((e = cudaMemsetAsync(g.big_count, 0, sizeof(uint32_t), st)) != cudaSuccess) return e;
 	const unsigned npad_blk = bounded ? (unsigned)(cap / 256 + 1 < kNumSMs * 8 ? cap / 256 + 1 : kNumSMs * 8) : 0u;
 	const int sort_bits = bounded ? (ntile <= 65535 ? 16 : 32) : bits_for(ntile);
-	if (ntile <= 65535 || (!bounded && ntile <= 65536)) {  // 16-bit tile ids (the key arrays are allocated for 32-bit ids either way)
+	if (ntile <= kBucketMaxTiles && (uint32_t)f.P <= kPackMask + 1u) {  // tile bucketing of the emitted instances (16-bit tile ids)
+		uint16_t *kin = reinterpret_cast<uint16_t *>(b.keys_in);
+		count_launch();
+		emit_pairs_kernel<uint16_t><<<nblk, 256, 0, st>>>(f, g.rec, radii, g.tiles_touched, g.perm, g.offsets, kin, b.vals_in, g.big_list, g.big_count, cap32, n_order);
+		count_launch();
+		emit_big_kernel<uint16_t><<<nbig_blk, 256, 0, st>>>(f, g.rec, radii, g.perm, g.offsets, kin, b.vals_in, g.big_list, g.big_count, cap32);
+		if ((e = cudaGetLastError()) != cudaSuccess) return e;
+		return launch_bucketing(b, img, g.big_count, ntile, R, st);
+	} else if (ntile <= 65535 || (!bounded && ntile <= 65536)) {  // 16-bit tile ids (the key arrays are allocated for 32-bit ids either way)
 		uint16_t *kin = reinterpret_cast<uint16_t *>(b.keys_in), *kout = reinterpret_cast<uint16_t *>(b.keys_out);
 		count_launch();
 		emit_pairs_kernel<uint16_t><<<nblk, 256, 0, st>>>(f, g.rec, radii, g.tiles_touched, g.perm, g.offsets, kin, b.vals_in, g.big_list, g.big_count, cap32, n_order);

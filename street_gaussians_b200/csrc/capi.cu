@@ -82,6 +82,8 @@ BinView carve_bin(void *base, int64_t R) {
 	b.vals_out = take<uint32_t>(p, n);
 	b.sort_temp_bytes = memo_bytes(R, [](int64_t n) { return sort_temp_bytes(n); });
 	b.sort_temp = take<char>(p, b.sort_temp_bytes);
+	b.bucket_bytes = bucket_scratch_bytes(R);
+	b.bucket = take<char>(p, b.bucket_bytes);
 	b.total_bytes = (size_t)(p - reinterpret_cast<char *>(base));
 	return b;
 }

@@ -6,7 +6,7 @@
 //                  (u32[P] each) and cub temp storage.
 //   img state    : ranges uint2[Ntile], n_contrib u32[H*W], block-max n_contrib u32[Ntile]
 //   binning state: keys_in u32[R], keys_out u32[R] (tile ids), vals_in u32[R], vals_out u32[R] (= tile-ordered,
-//                  depth-sorted point list), sort temp
+//                  depth-sorted point list), sort temp, tile-bucketing scratch
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -59,6 +59,8 @@ struct BinView {
 	uint32_t *vals_in, *vals_out;  // Gaussian indices; vals_out is the tile-ordered, depth-sorted point list
 	void *sort_temp;
 	size_t sort_temp_bytes;
+	void *bucket;  // tile-bucketing scratch (binning.cu carve_bucket): count matrices, digit totals
+	size_t bucket_bytes;
 	size_t total_bytes;
 };
 
@@ -332,6 +334,7 @@ cudaError_t launch_gather_grad2d(const FrameDev &f, const PeerTable &pt, const G
 cudaError_t launch_count_tiles(const FrameDev &f, GeomView g, const int32_t *radii, cudaStream_t st, float *zero_rows = nullptr);
 size_t geom_temp_bytes(int P);
 size_t sort_temp_bytes(int64_t R);
+size_t bucket_scratch_bytes(int64_t R);
 // cap < 0: exact mode, R is the host-known instance count.  cap >= 0: bounded mode, R is ignored, the arrays hold `cap`
 // slots and the true count lives in g.big_count[1..3].
 cudaError_t launch_binning(const FrameDev &f, GeomView g, const int32_t *radii, BinView b, ImgView img, int64_t R,
