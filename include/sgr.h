@@ -374,6 +374,25 @@ int sgr_color_correct_backward(int32_t H, int32_t W, const float *image, const f
 int sgr_color_correction_reg(const float *affine, const float *affine_sky, float weight, float *value, float *g_affine, float *g_affine_sky,
                              void *stream);
 
+/* ---- Sky cube map composite (lib/models/sky_cubemap.py:77-123 at street_gaussian_renderer.py:107-111, model.nsg.include_sky) ----
+ * rgb_out = rgb + sky (1 - acc) per pixel.  A pixel of column i, row j looks along Rm^T K^-1 (i + jitter_x, j + jitter_y, 1)
+ * (Rm = w2c[:3, :3]; both jitters NULL: 0.5 each).  Pixels the mode selects take the cube map's bilinear lookup with edge wrap
+ * (a tap past a cube corner takes the mean of the three taps that exist; DESIGN.md §2), clamped to [0, 1]; the others take `fill`.
+ *   SGR_SKY_MASK_ACC    pixels with 1 - acc > 1e-3 (fp32)
+ *   SGR_SKY_MASK_GIVEN  pixels with sky_mask != 0, and every pixel of rows 0-49; sky_mask is only read
+ * rgb, rgb_out, dL_dout: [3,H,W]; acc, dL_dacc, jitter_x, jitter_y: [H,W]; sky_mask: [H,W] bytes (NULL for SGR_SKY_MASK_ACC);
+ * cube_map, dL_dcube: [6,R,R,3] (face 0:+x 1:-x 2:+y 3:-y 4:+z 5:-z, then row, column, channel); K: [3,3]; w2c: [4,4] row-major.
+ * All fp32 device memory.  Backward: dL_dacc = -sum_c sky_c dL_dout_c (may be NULL); dL_dcube is ADDED to (the caller zeroes it;
+ * may be NULL); dL/drgb is dL_dout itself.  One kernel each way, grid sizes depend on H*W only (no host synchronisation). */
+#define SGR_SKY_MASK_ACC 0
+#define SGR_SKY_MASK_GIVEN 1
+int sgr_sky_composite_forward(int32_t H, int32_t W, int32_t R, int32_t mode, float fill, const float *rgb, const float *acc,
+                              const uint8_t *sky_mask, const float *cube_map, const float *K, const float *w2c, const float *jitter_x,
+                              const float *jitter_y, float *rgb_out, void *stream);
+int sgr_sky_composite_backward(int32_t H, int32_t W, int32_t R, int32_t mode, float fill, const float *acc, const uint8_t *sky_mask,
+                               const float *cube_map, const float *K, const float *w2c, const float *jitter_x, const float *jitter_y,
+                               const float *dL_dout, float *dL_dacc, float *dL_dcube, void *stream);
+
 /* ---- Image-space losses with their gradient (SURVEY.md §8 row f2) ----
  * value = w_l1 * L1(image, gt, mask) + w_ssim * SSIM(image, gt, mask)  and  dL_dimage = d value / d image  in two kernels.
  * Replaces l1_loss (lib/utils/loss_utils.py:21-37), ssim / _ssim (:91-126: 11x11 Gaussian window, sigma 1.5, zero padding, C1 = 0.01^2,

@@ -862,6 +862,40 @@ int sgr_color_correction_reg(const float *affine, const float *affine_sky, float
 	return SGR_OK;
 }
 
+static int sky_check(const char *fn, int32_t H, int32_t W, int32_t R, int32_t mode, const uint8_t *sky_mask) {
+	// texel indices are int: 6 R^2 < 2^31
+	if (H <= 0 || W <= 0 || R <= 0 || R > 16384) return fail(SGR_EINVAL, "%s: bad sizes H=%d W=%d R=%d", fn, H, W, R);
+	if (mode != SGR_SKY_MASK_ACC && mode != SGR_SKY_MASK_GIVEN) return fail(SGR_EINVAL, "%s: unknown mask mode %d", fn, mode);
+	if (mode == SGR_SKY_MASK_GIVEN && !sky_mask) return fail(SGR_EINVAL, "%s: SGR_SKY_MASK_GIVEN needs sky_mask", fn);
+	return SGR_OK;
+}
+
+int sgr_sky_composite_forward(int32_t H, int32_t W, int32_t R, int32_t mode, float fill, const float *rgb, const float *acc,
+                              const uint8_t *sky_mask, const float *cube_map, const float *K, const float *w2c, const float *jitter_x,
+                              const float *jitter_y, float *rgb_out, void *stream) {
+	if (int rc = sky_check("sgr_sky_composite_forward", H, W, R, mode, sky_mask)) return rc;
+	if (!rgb || !acc || !cube_map || !K || !w2c || !rgb_out) return fail(SGR_EINVAL, "NULL pointer passed to sgr_sky_composite_forward");
+	if (!jitter_x != !jitter_y) return fail(SGR_EINVAL, "sgr_sky_composite_forward: give both jitters or neither");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_sky_composite_fwd(H, W, R, mode, fill, rgb, acc, sky_mask, cube_map, K, w2c, jitter_x, jitter_y, rgb_out, st), "sky_composite_fwd");
+	return SGR_OK;
+}
+
+int sgr_sky_composite_backward(int32_t H, int32_t W, int32_t R, int32_t mode, float fill, const float *acc, const uint8_t *sky_mask,
+                               const float *cube_map, const float *K, const float *w2c, const float *jitter_x, const float *jitter_y,
+                               const float *dL_dout, float *dL_dacc, float *dL_dcube, void *stream) {
+	if (int rc = sky_check("sgr_sky_composite_backward", H, W, R, mode, sky_mask)) return rc;
+	if (!acc || !cube_map || !K || !w2c || !dL_dout) return fail(SGR_EINVAL, "NULL pointer passed to sgr_sky_composite_backward");
+	if (!jitter_x != !jitter_y) return fail(SGR_EINVAL, "sgr_sky_composite_backward: give both jitters or neither");
+	if (!dL_dacc && !dL_dcube) return SGR_OK;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_sky_composite_bwd(H, W, R, mode, fill, acc, sky_mask, cube_map, K, w2c, jitter_x, jitter_y, dL_dout, dL_dacc, dL_dcube, st),
+	        "sky_composite_bwd");
+	return SGR_OK;
+}
+
 size_t sgr_image_loss_scratch_bytes(int32_t C, int32_t H, int32_t W) { return (C > 0 && H > 0 && W > 0) ? image_loss_scratch_bytes(C, H, W) : 0; }
 
 int sgr_image_loss(int32_t C, int32_t H, int32_t W, const float *image, const float *gt, const uint8_t *mask, float w_l1, float w_ssim,

@@ -372,6 +372,12 @@ cudaError_t launch_color_correct_bwd(int64_t N, const float *image, const float 
                                      void *scratch, cudaStream_t st);
 cudaError_t launch_color_correction_reg(const float *affine, const float *affine_sky, float weight, float *value, float *g_affine,
                                         float *g_affine_sky, cudaStream_t st);
+cudaError_t launch_sky_composite_fwd(int H, int W, int R, int mode, float fill, const float *rgb, const float *acc, const uint8_t *mask,
+                                     const float *cube, const float *K, const float *w2c, const float *jx, const float *jy, float *out,
+                                     cudaStream_t st);
+cudaError_t launch_sky_composite_bwd(int H, int W, int R, int mode, float fill, const float *acc, const uint8_t *mask, const float *cube,
+                                     const float *K, const float *w2c, const float *jx, const float *jy, const float *gout, float *gacc,
+                                     float *gcube, cudaStream_t st);
 size_t image_loss_scratch_bytes(int C, int H, int W);
 cudaError_t launch_image_loss(int C, int H, int W, const float *img, const float *gt, const uint8_t *mask, float w_l1, float w_ssim, float *grad,
                               float *scalars, void *scratch, cudaStream_t st);

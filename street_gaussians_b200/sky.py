@@ -1,0 +1,98 @@
+"""The sky cube map of the reference (lib/models/sky_cubemap.py:77-123, model.nsg.include_sky) composited onto the rendered frame
+(street_gaussian_renderer.py:107-111) over sgr_sky_composite_forward / sgr_sky_composite_backward (include/sgr.h).
+
+    sky_composite(rgb, acc, cube_map, K, w2c, sky_mask=..., perturb=..., white_background=...)
+        == rgb + SkyCubeMap(camera, acc.detach()) * (1 - acc)
+
+`cube_map` is SkyCubeMap.sky_cube_map [6, R, R, 3]; `w2c` is camera.world_view_transform.transpose(0, 1).  With `sky_mask` (training
+with the guidance mask) the cube is sampled where the mask is set and on rows 0-49; without it, where 1 - acc > 1e-3.  The caller's
+mask is only read: the reference sets its rows 0-49 in place, which the sky loss then sees, so a caller who wants that loss input
+sets those rows itself.  `perturb` jitters each pixel's sample point as get_rays_torch(perturb=True) does, with two torch.rand(H, W)
+draws on the current CUDA generator.  CUDA tensors only: there is no CPU fallback.
+"""
+from __future__ import annotations
+
+from typing import Optional
+
+import torch
+
+from . import _capi
+from .rasterizer import _ptr, _stream
+
+
+def _check(rgb, acc, cube_map, K, w2c, sky_mask):
+    if rgb.dim() != 3 or rgb.shape[0] != 3:
+        raise ValueError(f"rgb must be [3, H, W], got {tuple(rgb.shape)}")
+    H, W = int(rgb.shape[1]), int(rgb.shape[2])
+    if tuple(acc.shape) != (1, H, W):
+        raise ValueError(f"acc must be [1, {H}, {W}], got {tuple(acc.shape)}")
+    if cube_map.dim() != 4 or cube_map.shape[0] != 6 or cube_map.shape[3] != 3:
+        raise ValueError(f"cube_map must be [6, R, R, 3], got {tuple(cube_map.shape)}")
+    if cube_map.shape[1] != cube_map.shape[2]:
+        raise ValueError(f"cube_map faces must be square, got {cube_map.shape[1]} x {cube_map.shape[2]}")
+    if tuple(K.shape) != (3, 3) or tuple(w2c.shape) != (4, 4):
+        raise ValueError(f"K must be [3, 3] and w2c [4, 4], got {tuple(K.shape)} and {tuple(w2c.shape)}")
+    if sky_mask is not None:
+        if tuple(sky_mask.shape) not in ((1, H, W), (H, W)) or sky_mask.dtype != torch.bool:
+            raise ValueError(f"sky_mask must be a bool [1, {H}, {W}] or [{H}, {W}], got {sky_mask.dtype} {tuple(sky_mask.shape)}")
+    named = dict(rgb=rgb, acc=acc, cube_map=cube_map, K=K, w2c=w2c)
+    for what, t in named.items():
+        if t.dtype != torch.float32:
+            raise ValueError(f"{what} must be float32, got {t.dtype}")
+    if sky_mask is not None:
+        named["sky_mask"] = sky_mask
+    for what, t in named.items():
+        if not t.is_cuda:
+            raise _capi.SgrError(f"street_gaussians_b200.sky needs CUDA tensors ({what} is on {t.device}; there is no CPU fallback)")
+        if t.device != rgb.device:
+            raise ValueError(f"{what} is on {t.device}, rgb on {rgb.device}")
+    return H, W, int(cube_map.shape[1])
+
+
+class _SkyComposite(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, rgb, acc, cube_map, K, w2c, sky_mask, perturb: bool, fill: float):
+        H, W, R = _check(rgb, acc, cube_map, K, w2c, sky_mask)
+        L = _capi.lib()
+        dev = rgb.device
+        rgb_c, acc_c, cube = rgb.contiguous(), acc.contiguous(), cube_map.contiguous()
+        Kc, Tc = K.contiguous(), w2c.contiguous()
+        mask = sky_mask.contiguous() if sky_mask is not None else None
+        mode = _capi.SKY_MASK_GIVEN if mask is not None else _capi.SKY_MASK_ACC
+        if perturb:  # graphics_utils.py:195-196, in that order
+            jx = torch.rand(H, W, device=dev)
+            jy = torch.rand(H, W, device=dev)
+        else:
+            jx = jy = None
+        out = torch.empty_like(rgb_c)
+        with torch.cuda.device(dev):
+            rc = L.sgr_sky_composite_forward(H, W, R, mode, float(fill), _ptr(rgb_c), _ptr(acc_c), _ptr(mask), _ptr(cube), _ptr(Kc), _ptr(Tc),
+                                             _ptr(jx), _ptr(jy), _ptr(out), _stream(dev))
+        _capi.check(rc, "sgr_sky_composite_forward")
+        ctx.save_for_backward(acc_c, cube, Kc, Tc, mask, jx, jy)
+        ctx.args = (H, W, R, mode, float(fill))
+        return out
+
+    @staticmethod
+    def backward(ctx, g_out):
+        L = _capi.lib()
+        acc, cube, Kc, Tc, mask, jx, jy = ctx.saved_tensors
+        H, W, R, mode, fill = ctx.args
+        dev = acc.device
+        g = g_out.contiguous()
+        need_rgb, need_acc, need_cube = ctx.needs_input_grad[:3]
+        g_acc = torch.empty_like(acc) if need_acc else None
+        g_cube = torch.zeros_like(cube) if need_cube else None
+        with torch.cuda.device(dev):
+            rc = L.sgr_sky_composite_backward(H, W, R, mode, fill, _ptr(acc), _ptr(mask), _ptr(cube), _ptr(Kc), _ptr(Tc), _ptr(jx), _ptr(jy),
+                                              _ptr(g), _ptr(g_acc), _ptr(g_cube), _stream(dev))
+        _capi.check(rc, "sgr_sky_composite_backward")
+        return (g_out if need_rgb else None), g_acc, g_cube, None, None, None, None, None
+
+
+def sky_composite(rgb: torch.Tensor, acc: torch.Tensor, cube_map: torch.Tensor, K: torch.Tensor, w2c: torch.Tensor, *,
+                  sky_mask: Optional[torch.Tensor] = None, perturb: bool = False, white_background: bool = True) -> torch.Tensor:
+    """rgb [3, H, W] + sky * (1 - acc [1, H, W]) with the sky sampled from cube_map [6, R, R, 3] along the rays of K [3, 3] and
+    w2c [4, 4], clamped to [0, 1]; pixels the mask rule leaves out take 1 (white_background) or 0.  Differentiable in rgb, acc and
+    cube_map.  sky_mask: bool [1, H, W] or [H, W] (training with the guidance mask), None for the acc rule.  All fp32 CUDA tensors."""
+    return _SkyComposite.apply(rgb, acc, cube_map, K, w2c, sky_mask, bool(perturb), 1.0 if white_background else 0.0)
