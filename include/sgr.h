@@ -393,6 +393,34 @@ int sgr_sky_composite_backward(int32_t H, int32_t W, int32_t R, int32_t mode, fl
                                const float *cube_map, const float *K, const float *w2c, const float *jitter_x, const float *jitter_y,
                                const float *dL_dout, float *dL_dacc, float *dL_dcube, void *stream);
 
+/* ---- Tracked actor poses (lib/models/actor_pose.py as StreetGaussianModel.parse_camera uses it, street_gaussian_model.py:257-271) ----
+ * poses[a] = (qw, qx, qy, qz, tx, ty, tz) of visible actor a on one camera, the rows sgr_compose_forward takes:
+ * matrix_to_quaternion(R_ego) (x) rot and R_ego trans + t_ego, with rot / trans interpolated between the two tracklet entries of the
+ * actor's track nearest `timestamp` (ties: the entry first in the track's order), each entry's translation plus opt_trans and its
+ * rotation turned by opt_rots about z; with opt_trans / opt_rots given and is_val set, interpolated again between the poses at the two
+ * training timestamps of camera `cam` nearest `timestamp` inside the track's span (DESIGN.md §5 lists the reference's quirks kept).
+ * idft[a, fourier_dim] (may be NULL) = IDFT(fourier_scale (frame - start_frame) / (end_frame - start_frame), fourier_dim).
+ * The track table (device, built once): track t owns entries [track_off[t], track_off[t+1]) of entry_fc [E, 2] int32 (frame, column:
+ * the track's argwhere order) and entry_ts [E] float64 (the frame's tracklet timestamp); track_span [T, 2] float64 (start, end
+ * timestamp); track_frames [T, 2] int32 (start, end frame); camera c owns cam_ts[cam_off[c], cam_off[c+1]) float64, its training
+ * timestamps in order (may be NULL with num_cams == 0).  input_trans [F, K, 3], input_rots [F, K, 4] (w, x, y, z) fp32 device.
+ * Per call: tracks (HOST, n_act int32 in [0, num_tracks)); ego_pose [4, 4] row-major fp32 device; opt_trans [F, K, 3] and opt_rots
+ * [F, K] fp32 device, both or neither (model.nsg.opt_track); poses [n_act, 7] fp32 device.  Every track used must have >= 2 entries.
+ * Backward: dL_dopt_trans / dL_dopt_rots are ADDED to (the caller zeroes them); each actor touches at most 4 rows of each (8 on the
+ * validation path), summed per row in actor order so repeated calls agree bit for bit.  scratch: sgr_actor_pose_scratch_bytes(n_act).
+ * Grid sizes depend on n_act only and nothing is read back to the host. */
+int sgr_actor_pose_forward(int32_t num_tracks, int32_t K, const int32_t *track_off, const int32_t *entry_fc, const double *entry_ts,
+                           const double *track_span, const int32_t *track_frames, int32_t num_cams, const int32_t *cam_off, const double *cam_ts,
+                           const float *input_trans, const float *input_rots, int32_t n_act, const int32_t *tracks, double timestamp, int32_t cam,
+                           int32_t is_val, const float *ego_pose, const float *opt_trans, const float *opt_rots, int32_t frame, double fourier_scale,
+                           int32_t fourier_dim, float *poses, float *idft, void *stream);
+size_t sgr_actor_pose_scratch_bytes(int32_t n_act);
+int sgr_actor_pose_backward(int32_t num_tracks, int32_t K, const int32_t *track_off, const int32_t *entry_fc, const double *entry_ts,
+                            const double *track_span, const int32_t *track_frames, int32_t num_cams, const int32_t *cam_off, const double *cam_ts,
+                            const float *input_trans, const float *input_rots, int32_t n_act, const int32_t *tracks, double timestamp, int32_t cam,
+                            int32_t is_val, const float *ego_pose, const float *opt_trans, const float *opt_rots, const float *dL_dposes,
+                            float *dL_dopt_trans, float *dL_dopt_rots, void *scratch, size_t scratch_bytes, void *stream);
+
 /* ---- Image-space losses with their gradient (SURVEY.md §8 row f2) ----
  * value = w_l1 * L1(image, gt, mask) + w_ssim * SSIM(image, gt, mask)  and  dL_dimage = d value / d image  in two kernels.
  * Replaces l1_loss (lib/utils/loss_utils.py:21-37), ssim / _ssim (:91-126: 11x11 Gaussian window, sigma 1.5, zero padding, C1 = 0.01^2,

@@ -16,9 +16,10 @@ from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, Inst
 from .composer import compose  # noqa: E402,F401
 from .corrections import color_correct, color_correction_reg_loss  # noqa: E402,F401
 from .sky import sky_composite  # noqa: E402,F401
+from .actor_pose import ActorPose  # noqa: E402,F401
 from . import corrections, losses, sky, training  # noqa: E402,F401
 
-__all__ = ["compose", "color_correct", "color_correction_reg_loss", "sky_composite", "GaussianRasterizationSettings", "GaussianRasterizer", "TileRowBand", "InstanceCapacity", "RenderLayer", "rasterize_gaussians", "distCUDA2",
+__all__ = ["compose", "ActorPose", "color_correct", "color_correction_reg_loss", "sky_composite", "GaussianRasterizationSettings", "GaussianRasterizer", "TileRowBand", "InstanceCapacity", "RenderLayer", "rasterize_gaussians", "distCUDA2",
            "install_shims"]
 
 _SHIMS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "shims")

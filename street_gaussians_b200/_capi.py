@@ -20,7 +20,8 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_state_s
            "sgr_densify_scratch_bytes", "sgr_densify_plan", "sgr_densify_apply", "sgr_reset_opacity", "sgr_sparse_adam_step",
            "sgr_layer_state_sizes", "sgr_forward_layer", "sgr_backward_blend_layer", "sgr_backward_geom_layered",
            "sgr_compose_forward_corrected", "sgr_compose_backward_corrected", "sgr_color_correct_forward", "sgr_color_correct_scratch_bytes",
-           "sgr_color_correct_backward", "sgr_color_correction_reg", "sgr_sky_composite_forward", "sgr_sky_composite_backward"]
+           "sgr_color_correct_backward", "sgr_color_correction_reg", "sgr_sky_composite_forward", "sgr_sky_composite_backward",
+           "sgr_actor_pose_forward", "sgr_actor_pose_scratch_bytes", "sgr_actor_pose_backward"]
 
 SKY_MASK_ACC, SKY_MASK_GIVEN = 0, 1
 
@@ -181,6 +182,14 @@ def lib():
     L.sgr_sky_composite_forward.argtypes = [C.c_int32] * 4 + [C.c_float] + [vp] * 10
     L.sgr_sky_composite_backward.restype = C.c_int
     L.sgr_sky_composite_backward.argtypes = [C.c_int32] * 4 + [C.c_float] + [vp] * 11
+    track_table = [C.c_int32, C.c_int32, vp, vp, vp, vp, vp, C.c_int32, vp, vp, vp, vp]
+    pose_call = [C.c_int32, vp, C.c_double, C.c_int32, C.c_int32, vp, vp, vp]
+    L.sgr_actor_pose_forward.restype = C.c_int
+    L.sgr_actor_pose_forward.argtypes = track_table + pose_call + [C.c_int32, C.c_double, C.c_int32, vp, vp, vp]
+    L.sgr_actor_pose_scratch_bytes.restype = C.c_size_t
+    L.sgr_actor_pose_scratch_bytes.argtypes = [C.c_int32]
+    L.sgr_actor_pose_backward.restype = C.c_int
+    L.sgr_actor_pose_backward.argtypes = track_table + pose_call + [vp, vp, vp, vp, C.c_size_t, vp]
     L.sgr_image_loss_scratch_bytes.restype = C.c_size_t
     L.sgr_image_loss_scratch_bytes.argtypes = [C.c_int32] * 3
     L.sgr_image_loss.restype = C.c_int

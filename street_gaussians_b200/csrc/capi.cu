@@ -896,6 +896,76 @@ int sgr_sky_composite_backward(int32_t H, int32_t W, int32_t R, int32_t mode, fl
 	return SGR_OK;
 }
 
+static int actor_pose_check(const char *fn, int32_t num_tracks, int32_t K, const int32_t *track_off, const int32_t *entry_fc, const double *entry_ts,
+                            const double *track_span, const int32_t *track_frames, int32_t num_cams, const int32_t *cam_off, const double *cam_ts,
+                            const float *input_trans, const float *input_rots, int32_t n_act, const int32_t *tracks, int32_t cam, int32_t is_val,
+                            const float *ego_pose, const float *opt_trans, const float *opt_rots) {
+	if (num_tracks < 0 || K <= 0 || num_cams < 0 || n_act < 0) return fail(SGR_EINVAL, "%s: bad sizes tracks=%d K=%d cams=%d actors=%d", fn, num_tracks, K, num_cams, n_act);
+	if (!track_off || !entry_fc || !entry_ts || !track_span || !track_frames || !input_trans || !input_rots || !ego_pose)
+		return fail(SGR_EINVAL, "%s: NULL track table or ego pose", fn);
+	if (n_act > 0 && !tracks) return fail(SGR_EINVAL, "%s: tracks is NULL", fn);
+	for (int32_t a = 0; a < n_act; a++)
+		if (tracks[a] < 0 || tracks[a] >= num_tracks) return fail(SGR_EINVAL, "%s: track slot %d of actor %d is outside [0, %d)", fn, tracks[a], a, num_tracks);
+	if ((opt_trans == nullptr) != (opt_rots == nullptr)) return fail(SGR_EINVAL, "%s: give both opt_trans and opt_rots or neither", fn);
+	if (opt_trans && is_val) {
+		if (cam < 0 || cam >= num_cams) return fail(SGR_EINVAL, "%s: camera %d is outside [0, %d)", fn, cam, num_cams);
+		if (!cam_off || !cam_ts) return fail(SGR_EINVAL, "%s: NULL camera timestamps", fn);
+	}
+	return SGR_OK;
+}
+
+static ActorPoseTable actor_pose_table(int32_t num_tracks, int32_t K, const int32_t *track_off, const int32_t *entry_fc, const double *entry_ts,
+                                       const double *track_span, const int32_t *track_frames, int32_t num_cams, const int32_t *cam_off,
+                                       const double *cam_ts, const float *input_trans, const float *input_rots) {
+	return ActorPoseTable{num_tracks, K, num_cams, track_off, entry_fc, track_frames, cam_off, entry_ts, track_span, cam_ts, input_trans, input_rots};
+}
+
+int sgr_actor_pose_forward(int32_t num_tracks, int32_t K, const int32_t *track_off, const int32_t *entry_fc, const double *entry_ts,
+                           const double *track_span, const int32_t *track_frames, int32_t num_cams, const int32_t *cam_off, const double *cam_ts,
+                           const float *input_trans, const float *input_rots, int32_t n_act, const int32_t *tracks, double timestamp, int32_t cam,
+                           int32_t is_val, const float *ego_pose, const float *opt_trans, const float *opt_rots, int32_t frame, double fourier_scale,
+                           int32_t fourier_dim, float *poses, float *idft, void *stream) {
+	const char *fn = "sgr_actor_pose_forward";
+	if (int rc = actor_pose_check(fn, num_tracks, K, track_off, entry_fc, entry_ts, track_span, track_frames, num_cams, cam_off, cam_ts, input_trans,
+	                              input_rots, n_act, tracks, cam, is_val, ego_pose, opt_trans, opt_rots))
+		return rc;
+	if (n_act > 0 && !poses) return fail(SGR_EINVAL, "%s: poses is NULL", fn);
+	if (idft && (fourier_dim <= 0 || fourier_dim > SGR_MAX_FOURIER)) return fail(SGR_EINVAL, "%s: fourier_dim %d is outside [1, %d]", fn, fourier_dim, SGR_MAX_FOURIER);
+	if (n_act == 0) return SGR_OK;
+	const ActorPoseTable T = actor_pose_table(num_tracks, K, track_off, entry_fc, entry_ts, track_span, track_frames, num_cams, cam_off, cam_ts,
+	                                          input_trans, input_rots);
+	const ActorPoseCall c{timestamp, fourier_scale, cam, is_val != 0, opt_trans != nullptr, frame, fourier_dim, ego_pose, opt_trans, opt_rots};
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_actor_pose_fwd(T, c, tracks, n_act, poses, idft, st), "actor_pose_fwd");
+	return SGR_OK;
+}
+
+size_t sgr_actor_pose_scratch_bytes(int32_t n_act) { return n_act > 0 ? actor_pose_scratch_bytes(n_act) : 0; }
+
+int sgr_actor_pose_backward(int32_t num_tracks, int32_t K, const int32_t *track_off, const int32_t *entry_fc, const double *entry_ts,
+                            const double *track_span, const int32_t *track_frames, int32_t num_cams, const int32_t *cam_off, const double *cam_ts,
+                            const float *input_trans, const float *input_rots, int32_t n_act, const int32_t *tracks, double timestamp, int32_t cam,
+                            int32_t is_val, const float *ego_pose, const float *opt_trans, const float *opt_rots, const float *dL_dposes,
+                            float *dL_dopt_trans, float *dL_dopt_rots, void *scratch, size_t scratch_bytes, void *stream) {
+	const char *fn = "sgr_actor_pose_backward";
+	if (int rc = actor_pose_check(fn, num_tracks, K, track_off, entry_fc, entry_ts, track_span, track_frames, num_cams, cam_off, cam_ts, input_trans,
+	                              input_rots, n_act, tracks, cam, is_val, ego_pose, opt_trans, opt_rots))
+		return rc;
+	if (!opt_trans) return fail(SGR_EINVAL, "%s: without opt_trans / opt_rots the poses have no parameters", fn);
+	if (n_act == 0) return SGR_OK;
+	if (!dL_dposes || !dL_dopt_trans || !dL_dopt_rots) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	if (!scratch || scratch_bytes < actor_pose_scratch_bytes(n_act))
+		return fail(SGR_EINVAL, "%s: scratch of %zu bytes, needs %zu", fn, scratch_bytes, actor_pose_scratch_bytes(n_act));
+	const ActorPoseTable T = actor_pose_table(num_tracks, K, track_off, entry_fc, entry_ts, track_span, track_frames, num_cams, cam_off, cam_ts,
+	                                          input_trans, input_rots);
+	const ActorPoseCall c{timestamp, 0.0, cam, is_val != 0, 1, 0, 0, ego_pose, opt_trans, opt_rots};
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_actor_pose_bwd(T, c, tracks, n_act, dL_dposes, dL_dopt_trans, dL_dopt_rots, scratch, st), "actor_pose_bwd");
+	return SGR_OK;
+}
+
 size_t sgr_image_loss_scratch_bytes(int32_t C, int32_t H, int32_t W) { return (C > 0 && H > 0 && W > 0) ? image_loss_scratch_bytes(C, H, W) : 0; }
 
 int sgr_image_loss(int32_t C, int32_t H, int32_t W, const float *image, const float *gt, const uint8_t *mask, float w_l1, float w_ssim,

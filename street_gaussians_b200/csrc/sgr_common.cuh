@@ -378,6 +378,24 @@ cudaError_t launch_sky_composite_fwd(int H, int W, int R, int mode, float fill, 
 cudaError_t launch_sky_composite_bwd(int H, int W, int R, int mode, float fill, const float *acc, const uint8_t *mask, const float *cube,
                                      const float *K, const float *w2c, const float *jx, const float *jy, const float *gout, float *gacc,
                                      float *gcube, cudaStream_t st);
+// tracked actor poses (actor_pose.cu): the device-resident track table and one call's camera
+constexpr int kActorPoseChunk = 256;  // actors per launch: their track slots travel as a kernel parameter
+struct ActorPoseTable {
+	int num_tracks, K, num_cams;
+	const int32_t *track_off, *entry_fc, *track_frames, *cam_off;
+	const double *entry_ts, *track_span, *cam_ts;
+	const float *input_trans, *input_rots;
+};
+struct ActorPoseCall {
+	double timestamp, fourier_scale;
+	int cam, is_val, opt_track, frame, fourier_dim;
+	const float *ego_pose, *opt_trans, *opt_rots;
+};
+size_t actor_pose_scratch_bytes(int n);
+cudaError_t launch_actor_pose_fwd(const ActorPoseTable &T, const ActorPoseCall &c, const int32_t *slots, int n, float *poses, float *idft,
+                                  cudaStream_t st);
+cudaError_t launch_actor_pose_bwd(const ActorPoseTable &T, const ActorPoseCall &c, const int32_t *slots, int n, const float *g_poses, float *g_trans,
+                                  float *g_rots, void *scratch, cudaStream_t st);
 size_t image_loss_scratch_bytes(int C, int H, int W);
 cudaError_t launch_image_loss(int C, int H, int W, const float *img, const float *gt, const uint8_t *mask, float w_l1, float w_ssim, float *grad,
                               float *scalars, void *scratch, cudaStream_t st);
