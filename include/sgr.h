@@ -421,6 +421,43 @@ int sgr_actor_pose_backward(int32_t num_tracks, int32_t K, const int32_t *track_
                             int32_t is_val, const float *ego_pose, const float *opt_trans, const float *opt_rots, const float *dL_dposes,
                             float *dL_dopt_trans, float *dL_dopt_rots, void *scratch, size_t scratch_bytes, void *stream);
 
+/* ---- Feature channels (street_gaussian_renderer.py:206-264: cfg.render.render_normal, cfg.data.use_semantic) ----
+ * Per-Gaussian normals (GaussianModel.get_normals, gaussian_model.py:256-269) of the COMPOSED rows sgr_compose_forward writes:
+ * n = quaternion_to_matrix(rotations[i])[:, argmin(scales[i])] (the matrix with its own normalisation by sqrt(q.q); the lowest index
+ * wins ties, a NaN scale counts as the minimum), kept if sum(-d n) >= 0 with d = (means3D[i] - camera_center) / |...|, else -n (a NaN
+ * dot product takes -n).  means3D, scales, normals: [P,3]; rotations, dL_drotations: [P,4] (16-B aligned); camera_center: [3]; all fp32
+ * device.  decision: [P] bytes device, written by the forward (bits 0-1 the column, bit 2 the negation) and applied by the backward,
+ * which writes dL_drotations (fully written) through both of the matrix's normalisation and the column; the column and the sign
+ * pass no gradient, and nothing reaches means3D or scales.  One kernel each way; grids depend on P only. */
+int sgr_gaussian_normals_forward(int32_t P, const float *means3D, const float *rotations, const float *scales, const float *camera_center,
+                                 float *normals, uint8_t *decision, void *stream);
+int sgr_gaussian_normals_backward(int32_t P, const float *rotations, const uint8_t *decision, const float *dL_dnormals, float *dL_drotations,
+                                  void *stream);
+/* Composed semantics (StreetGaussianModel.get_semantic, street_gaussian_model.py:417-431) over [background, actor_0, ...]:
+ *   background rows (bg_semantic [n_bg,K]):   'logits' the rows;  'probabilities' softmax over each row
+ *   actor a's rows (actor_semantic[a] [n,1]):  zeros except column class_label[a] = the value ('logits') or its sigmoid
+ * Rows come out in compose's order into semantics [n_bg + sum counts, K].  actor_count, class_label (in [0, K)) and the pointer
+ * arrays actor_semantic / dL_dactor_semantic are HOST arrays of n_act entries; every tensor is fp32 device.  The backward reads the
+ * forward's output `semantics`; dL_dbg (may be NULL) and each dL_dactor_semantic[a] are fully written (dL_dactor_semantic may be NULL).
+ * Grids depend on the row counts only. */
+#define SGR_SEMANTIC_LOGITS 0
+#define SGR_SEMANTIC_PROBABILITIES 1
+int sgr_compose_semantics_forward(int32_t K, int32_t mode, int32_t n_bg, const float *bg_semantic, int32_t n_act, const int32_t *actor_count,
+                                  const int32_t *class_label, const float *const *actor_semantic, float *semantics, void *stream);
+int sgr_compose_semantics_backward(int32_t K, int32_t mode, int32_t n_bg, int32_t n_act, const int32_t *actor_count, const int32_t *class_label,
+                                   const float *semantics, const float *dL_dsemantics, float *dL_dbg, float *const *dL_dactor_semantic,
+                                   void *stream);
+/* Finishing of the rendered feature image rendered [S,H,W] (street_gaussian_renderer.py:245-264), channels [0, normal_channels) the
+ * normals (normal_channels 0 or 3) and the K = S - normal_channels others the semantics:
+ *   normals [3,H,W]  = x / max(|x|, 1e-12) per pixel (F.normalize(dim=0))
+ *   semantic [K,H,W] = 'probabilities' log(x / (sum_c x_c + 1e-8) + 1e-8);  'logits' x
+ * normals / semantic may be NULL only where they have no channel.  Backward: dL_drendered [S,H,W] fully written; dL_dnormals and
+ * dL_dsemantic may be NULL (zero).  One thread per pixel, one kernel each way. */
+int sgr_finish_features_forward(int32_t S, int32_t H, int32_t W, int32_t normal_channels, int32_t mode, const float *rendered, float *normals,
+                                float *semantic, void *stream);
+int sgr_finish_features_backward(int32_t S, int32_t H, int32_t W, int32_t normal_channels, int32_t mode, const float *rendered,
+                                 const float *dL_dnormals, const float *dL_dsemantic, float *dL_drendered, void *stream);
+
 /* ---- Image-space losses with their gradient (SURVEY.md §8 row f2) ----
  * value = w_l1 * L1(image, gt, mask) + w_ssim * SSIM(image, gt, mask)  and  dL_dimage = d value / d image  in two kernels.
  * Replaces l1_loss (lib/utils/loss_utils.py:21-37), ssim / _ssim (:91-126: 11x11 Gaussian window, sigma 1.5, zero padding, C1 = 0.01^2,

@@ -21,9 +21,12 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_state_s
            "sgr_layer_state_sizes", "sgr_forward_layer", "sgr_backward_blend_layer", "sgr_backward_geom_layered",
            "sgr_compose_forward_corrected", "sgr_compose_backward_corrected", "sgr_color_correct_forward", "sgr_color_correct_scratch_bytes",
            "sgr_color_correct_backward", "sgr_color_correction_reg", "sgr_sky_composite_forward", "sgr_sky_composite_backward",
-           "sgr_actor_pose_forward", "sgr_actor_pose_scratch_bytes", "sgr_actor_pose_backward"]
+           "sgr_actor_pose_forward", "sgr_actor_pose_scratch_bytes", "sgr_actor_pose_backward", "sgr_gaussian_normals_forward",
+           "sgr_gaussian_normals_backward", "sgr_compose_semantics_forward", "sgr_compose_semantics_backward", "sgr_finish_features_forward",
+           "sgr_finish_features_backward"]
 
 SKY_MASK_ACC, SKY_MASK_GIVEN = 0, 1
+SEMANTIC_LOGITS, SEMANTIC_PROBABILITIES = 0, 1
 
 
 class SgrFrame(C.Structure):
@@ -190,6 +193,19 @@ def lib():
     L.sgr_actor_pose_scratch_bytes.argtypes = [C.c_int32]
     L.sgr_actor_pose_backward.restype = C.c_int
     L.sgr_actor_pose_backward.argtypes = track_table + pose_call + [vp, vp, vp, vp, C.c_size_t, vp]
+    L.sgr_gaussian_normals_forward.restype = C.c_int
+    L.sgr_gaussian_normals_forward.argtypes = [C.c_int32] + [vp] * 7
+    L.sgr_gaussian_normals_backward.restype = C.c_int
+    L.sgr_gaussian_normals_backward.argtypes = [C.c_int32] + [vp] * 5
+    i32p = C.POINTER(C.c_int32)
+    L.sgr_compose_semantics_forward.restype = C.c_int
+    L.sgr_compose_semantics_forward.argtypes = [C.c_int32, C.c_int32, C.c_int32, vp, C.c_int32, i32p, i32p, C.POINTER(vp), vp, vp]
+    L.sgr_compose_semantics_backward.restype = C.c_int
+    L.sgr_compose_semantics_backward.argtypes = [C.c_int32] * 4 + [i32p, i32p, vp, vp, vp, C.POINTER(vp), vp]
+    L.sgr_finish_features_forward.restype = C.c_int
+    L.sgr_finish_features_forward.argtypes = [C.c_int32] * 5 + [vp] * 4
+    L.sgr_finish_features_backward.restype = C.c_int
+    L.sgr_finish_features_backward.argtypes = [C.c_int32] * 5 + [vp] * 5
     L.sgr_image_loss_scratch_bytes.restype = C.c_size_t
     L.sgr_image_loss_scratch_bytes.argtypes = [C.c_int32] * 3
     L.sgr_image_loss.restype = C.c_int

@@ -5,6 +5,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <vector>
 
 #include "sgr_common.cuh"
 
@@ -963,6 +964,117 @@ int sgr_actor_pose_backward(int32_t num_tracks, int32_t K, const int32_t *track_
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 	const bool debug = false;
 	SGR_TRY(launch_actor_pose_bwd(T, c, tracks, n_act, dL_dposes, dL_dopt_trans, dL_dopt_rots, scratch, st), "actor_pose_bwd");
+	return SGR_OK;
+}
+
+int sgr_gaussian_normals_forward(int32_t P, const float *means3D, const float *rotations, const float *scales, const float *camera_center,
+                                 float *normals, uint8_t *decision, void *stream) {
+	const char *fn = "sgr_gaussian_normals_forward";
+	if (P < 0) return fail(SGR_EINVAL, "%s: bad size P=%d", fn, P);
+	if (P == 0) return SGR_OK;
+	if (!means3D || !rotations || !scales || !camera_center || !normals || !decision) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	if (reinterpret_cast<uintptr_t>(rotations) % 16) return fail(SGR_EINVAL, "%s: rotations must be 16-byte aligned", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_gaussian_normals_fwd(P, means3D, rotations, scales, camera_center, normals, decision, st), "gaussian_normals_fwd");
+	return SGR_OK;
+}
+
+int sgr_gaussian_normals_backward(int32_t P, const float *rotations, const uint8_t *decision, const float *dL_dnormals, float *dL_drotations,
+                                  void *stream) {
+	const char *fn = "sgr_gaussian_normals_backward";
+	if (P < 0) return fail(SGR_EINVAL, "%s: bad size P=%d", fn, P);
+	if (P == 0) return SGR_OK;
+	if (!rotations || !decision || !dL_dnormals || !dL_drotations) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	if (reinterpret_cast<uintptr_t>(rotations) % 16 || reinterpret_cast<uintptr_t>(dL_drotations) % 16)
+		return fail(SGR_EINVAL, "%s: rotations and dL_drotations must be 16-byte aligned", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_gaussian_normals_bwd(P, rotations, decision, dL_dnormals, dL_drotations, st), "gaussian_normals_bwd");
+	return SGR_OK;
+}
+
+// Checks what both semantic entries share and builds the actors' composed row starts (starts[a] = n_bg + counts before a).
+static int semantics_check(const char *fn, int32_t K, int32_t mode, int32_t n_bg, int32_t n_act, const int32_t *actor_count,
+                           const int32_t *class_label, std::vector<int32_t> &starts) {
+	if (K < 1) return fail(SGR_EINVAL, "%s: K = %d, need at least one class", fn, K);
+	if (mode != SGR_SEMANTIC_LOGITS && mode != SGR_SEMANTIC_PROBABILITIES) return fail(SGR_EINVAL, "%s: unknown semantic mode %d", fn, mode);
+	if (n_bg < 0 || n_act < 0) return fail(SGR_EINVAL, "%s: bad sizes n_bg=%d n_act=%d", fn, n_bg, n_act);
+	if (n_act > 0 && (!actor_count || !class_label)) return fail(SGR_EINVAL, "%s: NULL actor table", fn);
+	starts.assign((size_t)n_act + 1, 0);
+	long long at = n_bg;
+	for (int32_t a = 0; a < n_act; a++) {
+		if (actor_count[a] < 0) return fail(SGR_EINVAL, "%s: actor %d has %d rows", fn, a, actor_count[a]);
+		if (class_label[a] < 0 || class_label[a] >= K) return fail(SGR_EINVAL, "%s: class label %d of actor %d is outside [0, %d)", fn, class_label[a], a, K);
+		starts[a] = (int32_t)at;
+		at += actor_count[a];
+		if (at > 0x7fffffffLL) return fail(SGR_EUNSUPPORTED, "%s: composed row count exceeds 2^31-1", fn);
+	}
+	starts[n_act] = (int32_t)at;
+	return SGR_OK;
+}
+
+int sgr_compose_semantics_forward(int32_t K, int32_t mode, int32_t n_bg, const float *bg_semantic, int32_t n_act, const int32_t *actor_count,
+                                  const int32_t *class_label, const float *const *actor_semantic, float *semantics, void *stream) {
+	const char *fn = "sgr_compose_semantics_forward";
+	std::vector<int32_t> starts;
+	if (int rc = semantics_check(fn, K, mode, n_bg, n_act, actor_count, class_label, starts)) return rc;
+	if (starts[n_act] == 0) return SGR_OK;
+	if (!semantics || (n_bg > 0 && !bg_semantic)) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	for (int32_t a = 0; a < n_act; a++)
+		if (actor_count[a] > 0 && (!actor_semantic || !actor_semantic[a])) return fail(SGR_EINVAL, "%s: NULL semantic of actor %d", fn, a);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_compose_semantics_fwd(n_bg, K, mode, bg_semantic, n_act, starts.data(), class_label, actor_semantic, semantics, st),
+	        "compose_semantics_fwd");
+	return SGR_OK;
+}
+
+int sgr_compose_semantics_backward(int32_t K, int32_t mode, int32_t n_bg, int32_t n_act, const int32_t *actor_count, const int32_t *class_label,
+                                   const float *semantics, const float *dL_dsemantics, float *dL_dbg, float *const *dL_dactor_semantic,
+                                   void *stream) {
+	const char *fn = "sgr_compose_semantics_backward";
+	std::vector<int32_t> starts;
+	if (int rc = semantics_check(fn, K, mode, n_bg, n_act, actor_count, class_label, starts)) return rc;
+	if (starts[n_act] == 0) return SGR_OK;
+	if (!semantics || !dL_dsemantics) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	if (dL_dactor_semantic)
+		for (int32_t a = 0; a < n_act; a++)
+			if (actor_count[a] > 0 && !dL_dactor_semantic[a]) return fail(SGR_EINVAL, "%s: NULL gradient of actor %d", fn, a);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_compose_semantics_bwd(n_bg, K, mode, semantics, dL_dsemantics, dL_dbg, n_act, starts.data(), class_label, dL_dactor_semantic, st),
+	        "compose_semantics_bwd");
+	return SGR_OK;
+}
+
+static int finish_check(const char *fn, int32_t S, int32_t H, int32_t W, int32_t normal_channels, int32_t mode) {
+	if (S < 1 || H <= 0 || W <= 0) return fail(SGR_EINVAL, "%s: bad sizes S=%d H=%d W=%d", fn, S, H, W);
+	if (normal_channels != 0 && normal_channels != 3) return fail(SGR_EINVAL, "%s: normal_channels must be 0 or 3, got %d", fn, normal_channels);
+	if (normal_channels > S) return fail(SGR_EINVAL, "%s: %d normal channels but S = %d", fn, normal_channels, S);
+	if (mode != SGR_SEMANTIC_LOGITS && mode != SGR_SEMANTIC_PROBABILITIES) return fail(SGR_EINVAL, "%s: unknown semantic mode %d", fn, mode);
+	return SGR_OK;
+}
+
+int sgr_finish_features_forward(int32_t S, int32_t H, int32_t W, int32_t normal_channels, int32_t mode, const float *rendered, float *normals,
+                                float *semantic, void *stream) {
+	const char *fn = "sgr_finish_features_forward";
+	if (int rc = finish_check(fn, S, H, W, normal_channels, mode)) return rc;
+	if (!rendered || (normal_channels > 0 && !normals) || (S > normal_channels && !semantic)) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_finish_features_fwd(S, H, W, normal_channels, mode, rendered, normals, semantic, st), "finish_features_fwd");
+	return SGR_OK;
+}
+
+int sgr_finish_features_backward(int32_t S, int32_t H, int32_t W, int32_t normal_channels, int32_t mode, const float *rendered,
+                                 const float *dL_dnormals, const float *dL_dsemantic, float *dL_drendered, void *stream) {
+	const char *fn = "sgr_finish_features_backward";
+	if (int rc = finish_check(fn, S, H, W, normal_channels, mode)) return rc;
+	if (!rendered || !dL_drendered) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_finish_features_bwd(S, H, W, normal_channels, mode, rendered, dL_dnormals, dL_dsemantic, dL_drendered, st), "finish_features_bwd");
 	return SGR_OK;
 }
 

@@ -396,6 +396,17 @@ cudaError_t launch_actor_pose_fwd(const ActorPoseTable &T, const ActorPoseCall &
                                   cudaStream_t st);
 cudaError_t launch_actor_pose_bwd(const ActorPoseTable &T, const ActorPoseCall &c, const int32_t *slots, int n, const float *g_poses, float *g_trans,
                                   float *g_rots, void *scratch, cudaStream_t st);
+// feature channels (features.cu)
+cudaError_t launch_gaussian_normals_fwd(int P, const float *means, const float *rots, const float *scales, const float *center, float *normals,
+                                        uint8_t *decision, cudaStream_t st);
+cudaError_t launch_gaussian_normals_bwd(int P, const float *rots, const uint8_t *decision, const float *g_normals, float *g_rots, cudaStream_t st);
+cudaError_t launch_compose_semantics_fwd(int n_bg, int K, int mode, const float *bg, int n_act, const int32_t *start, const int32_t *label,
+                                         const float *const *actor, float *out, cudaStream_t st);
+cudaError_t launch_compose_semantics_bwd(int n_bg, int K, int mode, const float *out, const float *g, float *g_bg, int n_act, const int32_t *start,
+                                         const int32_t *label, float *const *g_actor, cudaStream_t st);
+cudaError_t launch_finish_features_fwd(int S, int H, int W, int nc, int mode, const float *in, float *nout, float *sout, cudaStream_t st);
+cudaError_t launch_finish_features_bwd(int S, int H, int W, int nc, int mode, const float *in, const float *gn, const float *gs, float *gin,
+                                       cudaStream_t st);
 size_t image_loss_scratch_bytes(int C, int H, int W);
 cudaError_t launch_image_loss(int C, int H, int W, const float *img, const float *gt, const uint8_t *mask, float w_l1, float w_ssim, float *grad,
                               float *scalars, void *scratch, cudaStream_t st);
