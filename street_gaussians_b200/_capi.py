@@ -1,10 +1,14 @@
-"""ctypes loader for libsgr.so (include/sgr.h).  The product path has NO fallback: if the CUDA library is missing or
-does not export the ABI, importing / calling raises — it never routes through a CPU implementation.
+"""ctypes loader for libsgr.so (include/sgr.h), and how the package calls it: `call` (device guard, current stream, error
+check) and `f32` (the contiguous fp32 form the entries read).  The product path has NO fallback: if the CUDA library is
+missing or does not export the ABI, importing / calling raises — it never routes through a CPU implementation.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
+from typing import Optional
+
+import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libsgr.so")
@@ -262,3 +266,37 @@ def check(rc: int, what: str) -> None:
     if rc != 0:
         msg = lib().sgr_last_error()
         raise SgrError(f"{what} failed (code {rc}): {msg.decode() if msg else '?'}")
+
+
+def ptr(t: Optional[torch.Tensor]):
+    """The tensor's device address for a `void*` argument; NULL for None or an empty tensor."""
+    if t is None or t.numel() == 0:
+        return None
+    return C.c_void_p(t.data_ptr())
+
+
+def stream(device) -> C.c_void_p:
+    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+
+
+def call(name: str, device, *args) -> None:
+    """Call the entry `name` with `args` and raise SgrError if it fails.  With a `device`, the call runs with that device current
+    (work the library enqueues and the ALLOC_FN callbacks it makes target it) and gets the device's current stream as its last
+    argument.  device=None is for the entries that take no stream (sgr_state_sizes, sgr_layer_state_sizes)."""
+    fn = getattr(_lib or lib(), name)
+    if device is None:
+        rc = fn(*args)
+    else:
+        with torch.cuda.device(device):
+            rc = fn(*args, stream(device))
+    check(rc, name)
+
+
+def f32(t: torch.Tensor, device=None, align16: bool = False) -> torch.Tensor:
+    """`t` as a contiguous fp32 tensor, on `device` if one is given; copied only when it has to be.  align16: also copy a view
+    whose address is not 16-byte aligned (a contiguous view keeps its storage offset, e.g. a slice of a flat parameter buffer),
+    for the arguments the library reads with 16-byte loads (rotation and SH rows, include/sgr.h)."""
+    if t.dtype != torch.float32 or (device is not None and t.device != device):
+        t = t.to(device=device, dtype=torch.float32)
+    t = t.contiguous()
+    return t.clone() if align16 and t.data_ptr() % 16 else t

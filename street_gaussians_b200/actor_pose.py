@@ -21,7 +21,7 @@ import torch
 import torch.nn as nn
 
 from . import _capi
-from .rasterizer import _ptr, _stream
+from ._capi import ptr
 
 
 def track_table(tracklets, tracklet_timestamps, camera_timestamps, obj_meta) -> dict:
@@ -56,18 +56,15 @@ def track_table(tracklets, tracklet_timestamps, camera_timestamps, obj_meta) -> 
 class _PoseFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, opt_trans, opt_rots, module, slots, timestamp, cam, is_val, ego, frame):
-        L = _capi.lib()
         n = len(slots)
         slots = slots if n else None
         dev = module.input_trans.device
         poses = torch.empty((n, 7), device=dev, dtype=torch.float32)
         idft = torch.empty((n, module.fourier_dim), device=dev, dtype=torch.float32) if frame is not None else None
         opt = opt_trans is not None
-        with torch.cuda.device(dev):
-            rc = L.sgr_actor_pose_forward(*module._table_args(), n, slots, timestamp, cam, int(is_val), _ptr(ego),
-                                          _ptr(opt_trans) if opt else None, _ptr(opt_rots) if opt else None, int(frame or 0),
-                                          module.fourier_scale, module.fourier_dim, _ptr(poses), _ptr(idft), _stream(dev))
-        _capi.check(rc, "sgr_actor_pose_forward")
+        _capi.call("sgr_actor_pose_forward", dev, *module._table_args(), n, slots, timestamp, cam, int(is_val), ptr(ego),
+                   ptr(opt_trans) if opt else None, ptr(opt_rots) if opt else None, int(frame or 0), module.fourier_scale,
+                   module.fourier_dim, ptr(poses), ptr(idft))
         ctx.module, ctx.args = module, (n, slots, timestamp, cam, is_val)
         if opt:
             ctx.save_for_backward(opt_trans, opt_rots, ego)
@@ -83,13 +80,11 @@ class _PoseFn(torch.autograd.Function):
         dev = opt_trans.device
         g_trans, g_rots = torch.zeros_like(opt_trans), torch.zeros_like(opt_rots)
         if n and g_poses is not None:
-            g = g_poses.to(torch.float32).contiguous()
+            g = _capi.f32(g_poses)
             nbytes = int(L.sgr_actor_pose_scratch_bytes(n))
             scratch = torch.empty((nbytes,), device=dev, dtype=torch.uint8)
-            with torch.cuda.device(dev):
-                rc = L.sgr_actor_pose_backward(*ctx.module._table_args(), n, slots, timestamp, cam, int(is_val), _ptr(ego), _ptr(opt_trans),
-                                               _ptr(opt_rots), _ptr(g), _ptr(g_trans), _ptr(g_rots), _ptr(scratch), nbytes, _stream(dev))
-            _capi.check(rc, "sgr_actor_pose_backward")
+            _capi.call("sgr_actor_pose_backward", dev, *ctx.module._table_args(), n, slots, timestamp, cam, int(is_val), ptr(ego), ptr(opt_trans),
+                       ptr(opt_rots), ptr(g), ptr(g_trans), ptr(g_rots), ptr(scratch), nbytes)
         return g_trans, g_rots, None, None, None, None, None, None, None
 
 
@@ -126,8 +121,8 @@ class ActorPose(nn.Module):
             self.opt_rots = nn.Parameter(torch.zeros_like(self.input_rots[..., :1]))
 
     def _table_args(self):
-        return (len(self._counts), self.max_obj, _ptr(self._track_off), _ptr(self._entry_fc), _ptr(self._entry_ts), _ptr(self._track_span),
-                _ptr(self._track_frames), len(self._cam), _ptr(self._cam_off), _ptr(self._cam_ts), _ptr(self.input_trans), _ptr(self.input_rots))
+        return (len(self._counts), self.max_obj, ptr(self._track_off), ptr(self._entry_fc), ptr(self._entry_ts), ptr(self._track_span),
+                ptr(self._track_frames), len(self._cam), ptr(self._cam_off), ptr(self._cam_ts), ptr(self.input_trans), ptr(self.input_rots))
 
     def forward(self, track_ids: Sequence, timestamp: float, cam=0, is_val: bool = False, ego_pose: Optional[torch.Tensor] = None,
                 frame: Optional[int] = None):
@@ -157,7 +152,7 @@ class ActorPose(nn.Module):
             raise ValueError(f"ego_pose must be [4, 4], got {tuple(ego_pose.shape)}")
         if ego_pose.device != dev:
             raise ValueError(f"ego_pose is on {ego_pose.device}, the track table on {dev}")
-        ego = ego_pose.detach().to(torch.float32).contiguous()
+        ego = _capi.f32(ego_pose.detach())
         arr = (C.c_int32 * len(slots))(*slots)
         ot, orr = (self.opt_trans, self.opt_rots) if self.opt_track else (None, None)
         return _PoseFn.apply(ot, orr, self, arr, float(timestamp), c, val, ego, frame)

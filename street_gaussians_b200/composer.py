@@ -24,7 +24,7 @@ from typing import Optional, Sequence, Tuple
 import torch
 
 from . import _capi
-from .rasterizer import _ptr, _stream
+from ._capi import ptr
 
 RAW_KEYS = ("xyz", "rotation", "scaling", "opacity", "features_dc", "features_rest")
 
@@ -35,18 +35,13 @@ def _raw(model, key):
     return getattr(model, "_" + key)
 
 
-def _f32c(t: torch.Tensor) -> torch.Tensor:
-    return t if (t.dtype == torch.float32 and t.is_contiguous()) else t.to(torch.float32).contiguous()
-
-
 class _Compose(torch.autograd.Function):
     @staticmethod
     def forward(ctx, poses, idft, flip, flip_quat, corr_rot, corr_trans, n_models, *raw):
-        L = _capi.lib()
         if not raw[0].is_cuda:
             raise _capi.SgrError("street_gaussians_b200 composer needs CUDA tensors (there is no CPU fallback)")
         dev = raw[0].device
-        raw = tuple(_f32c(t) for t in raw)
+        raw = tuple(_capi.f32(t) for t in raw)
         models = [raw[6 * k: 6 * k + 6] for k in range(n_models)]
         M = int(models[0][5].shape[1]) + 1
         nseg = n_models
@@ -71,7 +66,7 @@ class _Compose(torch.autograd.Function):
         if flip is not None and nseg > 1:
             flip_full = torch.zeros((P,), device=dev, dtype=torch.uint8)
             flip_full[int(models[0][0].shape[0]):] = flip.to(device=dev, dtype=torch.uint8)
-            flip_quat = _f32c(flip_quat.to(dev).reshape(4))
+            flip_quat = _capi.f32(flip_quat.reshape(4), dev)
         corr = None
         if corr_rot is not None:
             corr = torch.zeros((8,), device=dev, dtype=torch.float32)
@@ -79,15 +74,13 @@ class _Compose(torch.autograd.Function):
             corr[4:7] = corr_trans.reshape(3).to(device=dev, dtype=torch.float32)
         e = lambda *shape: torch.empty(shape, device=dev, dtype=torch.float32)
         xyz, rot, scale, opac, sh = e(P, 3), e(P, 4), e(P, 3), e(P, 1), e(P, M, 3)
-        fq = _ptr(flip_quat) if flip_full is not None else None
-        with torch.cuda.device(dev):
-            if corr is None:
-                rc = L.sgr_compose_forward(segs, nseg, M, _ptr(pose_tab), _ptr(idft_tab), _ptr(flip_full), fq, _ptr(xyz), _ptr(rot), _ptr(scale),
-                                           _ptr(opac), _ptr(sh), _stream(dev))
-            else:
-                rc = L.sgr_compose_forward_corrected(segs, nseg, M, _ptr(pose_tab), _ptr(idft_tab), _ptr(flip_full), fq, _ptr(corr), _ptr(xyz),
-                                                     _ptr(rot), _ptr(scale), _ptr(opac), _ptr(sh), _stream(dev))
-        _capi.check(rc, "sgr_compose_forward" if corr is None else "sgr_compose_forward_corrected")
+        fq = ptr(flip_quat) if flip_full is not None else None
+        if corr is None:
+            _capi.call("sgr_compose_forward", dev, segs, nseg, M, ptr(pose_tab), ptr(idft_tab), ptr(flip_full), fq, ptr(xyz), ptr(rot),
+                       ptr(scale), ptr(opac), ptr(sh))
+        else:
+            _capi.call("sgr_compose_forward_corrected", dev, segs, nseg, M, ptr(pose_tab), ptr(idft_tab), ptr(flip_full), fq, ptr(corr),
+                       ptr(xyz), ptr(rot), ptr(scale), ptr(opac), ptr(sh))
         ctx.segs, ctx.nseg, ctx.M, ctx.n_models = segs, nseg, M, n_models
         ctx.flip_full, ctx.flip_quat = flip_full, (flip_quat if flip_full is not None else None)
         ctx.pose_shape = None if poses is None else (tuple(poses.shape), poses.dtype, poses.device)
@@ -99,12 +92,11 @@ class _Compose(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_xyz, g_rot, g_scale, g_opac, g_sh):
-        L = _capi.lib()
         pose_tab, idft_tab, *raw = ctx.saved_tensors
         dev = pose_tab.device
         nseg, M = ctx.nseg, ctx.M
         P = sum(int(raw[6 * k].shape[0]) for k in range(nseg))
-        z = lambda g, *shape: _f32c(g) if g is not None else torch.zeros(shape, device=dev, dtype=torch.float32)
+        z = lambda g, *shape: _capi.f32(g) if g is not None else torch.zeros(shape, device=dev, dtype=torch.float32)
         g_xyz, g_rot, g_scale, g_opac, g_sh = z(g_xyz, P, 3), z(g_rot, P, 4), z(g_scale, P, 3), z(g_opac, P, 1), z(g_sh, P, M, 3)
         grads = [torch.empty_like(t) for t in raw]
         gtab = (_capi.SgrSegmentGrads * nseg)()
@@ -113,19 +105,16 @@ class _Compose(torch.autograd.Function):
             g.xyz, g.rotation, g.scaling, g.opacity, g.features_dc, g.features_rest = (t.data_ptr() if t.numel() else None for t in grads[6 * k: 6 * k + 6])
         dposes = torch.empty((nseg, 8), device=dev, dtype=torch.float32)
         corr = ctx.corr
-        with torch.cuda.device(dev):
-            if corr is None:
-                scratch = torch.empty((nseg, 16), device=dev, dtype=torch.float32)
-                rc = L.sgr_compose_backward(ctx.segs, gtab, nseg, M, _ptr(pose_tab), _ptr(idft_tab), _ptr(ctx.flip_full), _ptr(ctx.flip_quat),
-                                            _ptr(g_xyz), _ptr(g_rot), _ptr(g_scale), _ptr(g_opac), _ptr(g_sh), _ptr(dposes), _ptr(scratch),
-                                            _stream(dev))
-            else:
-                scratch = torch.empty((nseg + 1, 16), device=dev, dtype=torch.float32)
-                dcorr = torch.empty((8,), device=dev, dtype=torch.float32)
-                rc = L.sgr_compose_backward_corrected(ctx.segs, gtab, nseg, M, _ptr(pose_tab), _ptr(idft_tab), _ptr(ctx.flip_full),
-                                                      _ptr(ctx.flip_quat), _ptr(corr), _ptr(g_xyz), _ptr(g_rot), _ptr(g_scale), _ptr(g_opac),
-                                                      _ptr(g_sh), _ptr(dposes), _ptr(dcorr), _ptr(scratch), _stream(dev))
-        _capi.check(rc, "sgr_compose_backward" if corr is None else "sgr_compose_backward_corrected")
+        if corr is None:
+            scratch = torch.empty((nseg, 16), device=dev, dtype=torch.float32)
+            _capi.call("sgr_compose_backward", dev, ctx.segs, gtab, nseg, M, ptr(pose_tab), ptr(idft_tab), ptr(ctx.flip_full), ptr(ctx.flip_quat),
+                       ptr(g_xyz), ptr(g_rot), ptr(g_scale), ptr(g_opac), ptr(g_sh), ptr(dposes), ptr(scratch))
+        else:
+            scratch = torch.empty((nseg + 1, 16), device=dev, dtype=torch.float32)
+            dcorr = torch.empty((8,), device=dev, dtype=torch.float32)
+            _capi.call("sgr_compose_backward_corrected", dev, ctx.segs, gtab, nseg, M, ptr(pose_tab), ptr(idft_tab), ptr(ctx.flip_full),
+                       ptr(ctx.flip_quat), ptr(corr), ptr(g_xyz), ptr(g_rot), ptr(g_scale), ptr(g_opac), ptr(g_sh), ptr(dposes), ptr(dcorr),
+                       ptr(scratch))
         g_poses = g_crot = g_ctrans = None
         if ctx.pose_shape is not None:
             shape, dtype, device = ctx.pose_shape

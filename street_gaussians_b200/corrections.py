@@ -15,19 +15,19 @@ from typing import Optional
 import torch
 
 from . import _capi
-from .rasterizer import _ptr, _stream
+from ._capi import ptr
 
 
-def _prep(t: torch.Tensor, what: str) -> torch.Tensor:
+def _check_cuda(t: torch.Tensor, what: str) -> None:
     if not t.is_cuda:
         raise _capi.SgrError(f"street_gaussians_b200.corrections needs CUDA tensors ({what} is on {t.device}; there is no CPU fallback)")
-    return t if (t.dtype == torch.float32 and t.is_contiguous()) else t.to(torch.float32).contiguous()
 
 
 def _affine(a: torch.Tensor, what: str, dev) -> torch.Tensor:
     if tuple(a.shape) != (3, 4):
         raise ValueError(f"{what} must be [3, 4], got {tuple(a.shape)}")
-    a = _prep(a, what)
+    _check_cuda(a, what)
+    a = _capi.f32(a)
     if a.device != dev:
         raise ValueError(f"{what} is on {a.device}, the image on {dev}")
     return a
@@ -36,16 +36,14 @@ def _affine(a: torch.Tensor, what: str, dev) -> torch.Tensor:
 class _ColorCorrect(torch.autograd.Function):
     @staticmethod
     def forward(ctx, image, affine):
-        L = _capi.lib()
-        img = _prep(image, "image")
+        _check_cuda(image, "image")
+        img = _capi.f32(image)
         if img.dim() != 3 or img.shape[0] != 3:
             raise ValueError(f"image must be [3, H, W], got {tuple(image.shape)}")
         A = _affine(affine, "affine", img.device)
         H, W = int(img.shape[1]), int(img.shape[2])
         out = torch.empty_like(img)
-        with torch.cuda.device(img.device):
-            rc = L.sgr_color_correct_forward(H, W, _ptr(img), _ptr(A), _ptr(out), _stream(img.device))
-        _capi.check(rc, "sgr_color_correct_forward")
+        _capi.call("sgr_color_correct_forward", img.device, H, W, ptr(img), ptr(A), ptr(out))
         ctx.save_for_backward(img, A)
         ctx.dtypes = (image.dtype, affine.dtype)
         return out
@@ -56,14 +54,13 @@ class _ColorCorrect(torch.autograd.Function):
         img, A = ctx.saved_tensors
         dev = img.device
         H, W = int(img.shape[1]), int(img.shape[2])
-        g = _prep(g_out, "dL/dout")
+        _check_cuda(g_out, "dL/dout")
+        g = _capi.f32(g_out)
         g_img = torch.empty_like(img) if ctx.needs_input_grad[0] else None
         g_A = torch.empty((3, 4), device=dev, dtype=torch.float32)
         nbytes = int(L.sgr_color_correct_scratch_bytes(H, W))
         scratch = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-        with torch.cuda.device(dev):
-            rc = L.sgr_color_correct_backward(H, W, _ptr(img), _ptr(A), _ptr(g), _ptr(g_img), _ptr(g_A), _ptr(scratch), nbytes, _stream(dev))
-        _capi.check(rc, "sgr_color_correct_backward")
+        _capi.call("sgr_color_correct_backward", dev, H, W, ptr(img), ptr(A), ptr(g), ptr(g_img), ptr(g_A), ptr(scratch), nbytes)
         return (g_img.to(ctx.dtypes[0]) if g_img is not None else None), (g_A.to(ctx.dtypes[1]) if ctx.needs_input_grad[1] else None)
 
 
@@ -75,16 +72,13 @@ def color_correct(image: torch.Tensor, affine: torch.Tensor) -> torch.Tensor:
 class _Reg(torch.autograd.Function):
     @staticmethod
     def forward(ctx, affine, affine_sky, weight: float):
-        L = _capi.lib()
         A = _affine(affine, "affine", affine.device)
         S = _affine(affine_sky, "affine_sky", A.device) if affine_sky is not None else None
         dev = A.device
         value = torch.empty((), device=dev, dtype=torch.float32)
         gA = torch.empty((3, 4), device=dev, dtype=torch.float32)
         gS = torch.empty((3, 4), device=dev, dtype=torch.float32) if S is not None else None
-        with torch.cuda.device(dev):
-            rc = L.sgr_color_correction_reg(_ptr(A), _ptr(S), float(weight), _ptr(value), _ptr(gA), _ptr(gS), _stream(dev))
-        _capi.check(rc, "sgr_color_correction_reg")
+        _capi.call("sgr_color_correction_reg", dev, ptr(A), ptr(S), float(weight), ptr(value), ptr(gA), ptr(gS))
         ctx.save_for_backward(gA, gS if gS is not None else gA)
         ctx.has_sky = S is not None
         ctx.dtypes = (affine.dtype, affine_sky.dtype if affine_sky is not None else None)

@@ -21,8 +21,8 @@ from typing import Optional, Sequence, Tuple
 import torch
 
 from . import _capi
+from ._capi import ptr
 from .composer import _raw
-from .rasterizer import _ptr, _stream
 
 MODES = {"logits": _capi.SEMANTIC_LOGITS, "probabilities": _capi.SEMANTIC_PROBABILITIES}
 
@@ -44,22 +44,15 @@ def _cuda_f32(what: str, named: dict, device=None):
             raise ValueError(f"{name} is on {t.device}, expected {device}")
 
 
-def _aligned16(t: torch.Tensor) -> torch.Tensor:
-    t = t.contiguous()
-    return t if t.data_ptr() % 16 == 0 else t.clone()
-
-
 class _GaussianNormals(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, rotations, scales, camera_center):
         P = int(means3D.shape[0])
         dev = means3D.device
-        m, r, s, c = means3D.contiguous(), _aligned16(rotations), scales.contiguous(), camera_center.reshape(3).contiguous()
+        m, r, s, c = means3D.contiguous(), _capi.f32(rotations, align16=True), scales.contiguous(), camera_center.reshape(3).contiguous()
         normals = torch.empty((P, 3), device=dev, dtype=torch.float32)
         decision = torch.empty((P,), device=dev, dtype=torch.uint8)
-        with torch.cuda.device(dev):
-            rc = _capi.lib().sgr_gaussian_normals_forward(P, _ptr(m), _ptr(r), _ptr(s), _ptr(c), _ptr(normals), _ptr(decision), _stream(dev))
-        _capi.check(rc, "sgr_gaussian_normals_forward")
+        _capi.call("sgr_gaussian_normals_forward", dev, P, ptr(m), ptr(r), ptr(s), ptr(c), ptr(normals), ptr(decision))
         ctx.save_for_backward(r, decision)
         return normals
 
@@ -71,9 +64,7 @@ class _GaussianNormals(torch.autograd.Function):
         dev = r.device
         g = g_normals.contiguous()
         g_rot = torch.empty_like(r)
-        with torch.cuda.device(dev):
-            rc = _capi.lib().sgr_gaussian_normals_backward(int(r.shape[0]), _ptr(r), _ptr(decision), _ptr(g), _ptr(g_rot), _stream(dev))
-        _capi.check(rc, "sgr_gaussian_normals_backward")
+        _capi.call("sgr_gaussian_normals_backward", dev, int(r.shape[0]), ptr(r), ptr(decision), ptr(g), ptr(g_rot))
         return None, g_rot, None, None
 
 
@@ -105,9 +96,7 @@ class _ComposeSemantics(torch.autograd.Function):
         ptrs = (C.c_void_p * max(n_act, 1))(*[a.data_ptr() if a.numel() else None for a in act_c])
         P = n_bg + sum(int(a.shape[0]) for a in act_c)
         out = torch.empty((P, K), device=dev, dtype=torch.float32)
-        with torch.cuda.device(dev):
-            rc = _capi.lib().sgr_compose_semantics_forward(K, mode, n_bg, _ptr(bg_c), n_act, counts, lab, ptrs, _ptr(out), _stream(dev))
-        _capi.check(rc, "sgr_compose_semantics_forward")
+        _capi.call("sgr_compose_semantics_forward", dev, K, mode, n_bg, ptr(bg_c), n_act, counts, lab, ptrs, ptr(out))
         ctx.args = (mode, K, n_bg, n_act, counts, lab, [tuple(a.shape) for a in act_c])
         ctx.save_for_backward(out)
         return out
@@ -123,9 +112,7 @@ class _ComposeSemantics(torch.autograd.Function):
         g_bg = torch.empty((n_bg, K), device=dev, dtype=torch.float32) if need_bg else None
         g_act = [torch.empty(s, device=dev, dtype=torch.float32) for s in shapes] if need_act else None
         gptrs = (C.c_void_p * max(n_act, 1))(*[t.data_ptr() if t.numel() else None for t in g_act]) if need_act else None
-        with torch.cuda.device(dev):
-            rc = _capi.lib().sgr_compose_semantics_backward(K, mode, n_bg, n_act, counts, lab, _ptr(out), _ptr(g), _ptr(g_bg), gptrs, _stream(dev))
-        _capi.check(rc, "sgr_compose_semantics_backward")
+        _capi.call("sgr_compose_semantics_backward", dev, K, mode, n_bg, n_act, counts, lab, ptr(out), ptr(g), ptr(g_bg), gptrs)
         return (None, None, g_bg) + (tuple(g_act) if need_act else (None,) * n_act)
 
 
@@ -160,9 +147,7 @@ class _FinishFeatures(torch.autograd.Function):
         x = rendered.contiguous()
         normals = torch.empty((nc, H, W), device=dev, dtype=torch.float32)
         semantic = torch.empty((S - nc, H, W), device=dev, dtype=torch.float32)
-        with torch.cuda.device(dev):
-            rc = _capi.lib().sgr_finish_features_forward(S, H, W, nc, mode, _ptr(x), _ptr(normals), _ptr(semantic), _stream(dev))
-        _capi.check(rc, "sgr_finish_features_forward")
+        _capi.call("sgr_finish_features_forward", dev, S, H, W, nc, mode, ptr(x), ptr(normals), ptr(semantic))
         ctx.save_for_backward(x)
         ctx.args = (S, H, W, nc, mode)
         return normals, semantic
@@ -175,9 +160,7 @@ class _FinishFeatures(torch.autograd.Function):
         gn = g_normals.contiguous() if g_normals is not None else None
         gs = g_semantic.contiguous() if g_semantic is not None else None
         g = torch.empty_like(x)
-        with torch.cuda.device(dev):
-            rc = _capi.lib().sgr_finish_features_backward(S, H, W, nc, mode, _ptr(x), _ptr(gn), _ptr(gs), _ptr(g), _stream(dev))
-        _capi.check(rc, "sgr_finish_features_backward")
+        _capi.call("sgr_finish_features_backward", dev, S, H, W, nc, mode, ptr(x), ptr(gn), ptr(gs), ptr(g))
         return g, None, None
 
 

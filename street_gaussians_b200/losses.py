@@ -21,20 +21,20 @@ from typing import Optional
 import torch
 
 from . import _capi
-from .rasterizer import _ptr, _stream
+from ._capi import ptr
 
 
-def _prep(img: torch.Tensor) -> torch.Tensor:
-    if not img.is_cuda:
+def _check_cuda(*ts: torch.Tensor) -> None:
+    if not all(t.is_cuda for t in ts):
         raise _capi.SgrError("street_gaussians_b200.losses needs CUDA tensors (there is no CPU fallback)")
-    return img if (img.dtype == torch.float32 and img.is_contiguous()) else img.to(torch.float32).contiguous()
 
 
 class _ImageLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, image, gt, mask, w_l1: float, w_ssim: float, which: int):
         L = _capi.lib()
-        img, g = _prep(image), _prep(gt.detach())
+        _check_cuda(image, gt)
+        img, g = _capi.f32(image), _capi.f32(gt.detach())
         if img.dim() != 3 or img.shape != g.shape:
             raise ValueError(f"image / gt must both be [C, H, W], got {tuple(image.shape)} and {tuple(gt.shape)}")
         Cn, H, W = (int(v) for v in img.shape)
@@ -49,10 +49,8 @@ class _ImageLoss(torch.autograd.Function):
         scalars = torch.empty(4, device=dev, dtype=torch.float32)
         nbytes = int(L.sgr_image_loss_scratch_bytes(Cn, H, W))
         scratch = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-        with torch.cuda.device(dev):
-            rc = L.sgr_image_loss(Cn, H, W, _ptr(img), _ptr(g), _ptr(m), float(w_l1), float(w_ssim), _ptr(grad), _ptr(scalars), _ptr(scratch),
-                                  nbytes, _stream(dev))
-        _capi.check(rc, "sgr_image_loss")
+        _capi.call("sgr_image_loss", dev, Cn, H, W, ptr(img), ptr(g), ptr(m), float(w_l1), float(w_ssim), ptr(grad), ptr(scalars),
+                   ptr(scratch), nbytes)
         ctx.save_for_backward(grad) if need_grad else None
         ctx.has_grad, ctx.in_dtype = need_grad, image.dtype
         return scalars[which]
@@ -94,8 +92,8 @@ class _AccLoss(torch.autograd.Function):
     """A per-pixel loss of an accumulation map selected by a bool mask: sgr_sky_loss or sgr_obj_acc_loss (same C signature)."""
     @staticmethod
     def forward(ctx, acc, flag_mask, weight: float, entry: str):
-        L = _capi.lib()
-        a = _prep(acc)
+        _check_cuda(acc)
+        a = _capi.f32(acc)
         dev = a.device
         m = flag_mask.reshape(-1).to(device=dev, dtype=torch.uint8).contiguous()
         if m.numel() != a.numel():
@@ -104,9 +102,7 @@ class _AccLoss(torch.autograd.Function):
         grad = torch.empty_like(a) if need_grad else None
         scalars = torch.empty(2, device=dev, dtype=torch.float32)
         scratch = torch.empty(64, device=dev, dtype=torch.uint8)
-        with torch.cuda.device(dev):
-            rc = getattr(L, entry)(a.numel(), _ptr(a), _ptr(m), float(weight), _ptr(grad), _ptr(scalars), _ptr(scratch), _stream(dev))
-        _capi.check(rc, entry)
+        _capi.call(entry, dev, a.numel(), ptr(a), ptr(m), float(weight), ptr(grad), ptr(scalars), ptr(scratch))
         ctx.save_for_backward(grad) if need_grad else None
         ctx.has_grad, ctx.in_dtype = need_grad, acc.dtype
         return scalars[0]
@@ -134,7 +130,8 @@ class _LidarDepthLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, depth, acc, lidar_depth, mask, weight: float, keep: float):
         L = _capi.lib()
-        d, a, ld = _prep(depth), _prep(acc), _prep(lidar_depth.detach())
+        _check_cuda(depth, acc, lidar_depth)
+        d, a, ld = _capi.f32(depth), _capi.f32(acc), _capi.f32(lidar_depth.detach())
         N = d.numel()
         if a.numel() != N or ld.numel() != N:
             raise ValueError(f"depth, acc and lidar_depth must have one shape, got {tuple(depth.shape)}, {tuple(acc.shape)}, "
@@ -151,10 +148,8 @@ class _LidarDepthLoss(torch.autograd.Function):
         scalars = torch.empty(4, device=dev, dtype=torch.float32)
         nbytes = int(L.sgr_lidar_depth_loss_scratch_bytes(N))
         scratch = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-        with torch.cuda.device(dev):
-            rc = L.sgr_lidar_depth_loss(N, _ptr(d), _ptr(a), _ptr(ld), _ptr(m), float(keep), float(weight), _ptr(g_depth), _ptr(g_acc),
-                                        _ptr(scalars), _ptr(scratch), nbytes, _stream(dev))
-        _capi.check(rc, "sgr_lidar_depth_loss")
+        _capi.call("sgr_lidar_depth_loss", dev, N, ptr(d), ptr(a), ptr(ld), ptr(m), float(keep), float(weight), ptr(g_depth), ptr(g_acc),
+                   ptr(scalars), ptr(scratch), nbytes)
         ctx.save_for_backward(g_depth, g_acc)
         ctx.dtypes = (depth.dtype, acc.dtype)
         return scalars[0]

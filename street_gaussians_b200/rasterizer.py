@@ -21,6 +21,10 @@ import torch
 import torch.nn as nn
 
 from . import _capi
+from ._capi import ptr
+
+# ptr and stream live in _capi; these names keep working for test and tool scripts that import them from the rasterizer
+_ptr, _stream = ptr, _capi.stream
 
 
 class GaussianRasterizationSettings(NamedTuple):
@@ -45,28 +49,12 @@ class TileRowBand(NamedTuple):
     step: int = 1
 
 
-def _ptr(t: Optional[torch.Tensor]):
-    if t is None or t.numel() == 0:
-        return None
-    return C.c_void_p(t.data_ptr())
-
-
-def _dev_f32(t: torch.Tensor, device) -> torch.Tensor:
-    """contiguous fp32 on `device` (the reference calls .contiguous() on every argument, DGR/rasterize_points.cu:92-118), at a
-    16-byte aligned address: a contiguous view keeps its storage offset (a slice of a flat parameter buffer), and the library
-    reads rotation and SH rows with 16-byte loads (include/sgr.h).  Such a view is copied."""
-    if t.device != device or t.dtype != torch.float32:
-        t = t.to(device=device, dtype=torch.float32)
-    t = t.contiguous()
-    return t.clone() if t.data_ptr() % 16 else t
-
-
 def _none_if_empty(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
     return None if t is None or t.numel() == 0 else t
 
 
 def _make_frame(s: GaussianRasterizationSettings, P: int, M: int, S: int, device, band: Optional[TileRowBand]):
-    keep = [_dev_f32(s.bg, device), _dev_f32(s.viewmatrix, device), _dev_f32(s.projmatrix, device), _dev_f32(s.campos, device)]
+    keep = [_capi.f32(t, device, align16=True) for t in (s.bg, s.viewmatrix, s.projmatrix, s.campos)]
     fr = _capi.SgrFrame()
     fr.P, fr.D, fr.M, fr.S = int(P), int(s.sh_degree), int(M), int(S)
     fr.width, fr.height = int(s.image_width), int(s.image_height)
@@ -78,10 +66,6 @@ def _make_frame(s: GaussianRasterizationSettings, P: int, M: int, S: int, device
         fr.row_begin, fr.row_end, fr.row_step = int(band.begin), int(band.end), int(band.step)
     fr.bg, fr.viewmatrix, fr.projmatrix, fr.campos = (k.data_ptr() for k in keep)
     return fr, keep
-
-
-def _stream(device) -> C.c_void_p:
-    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
 def _dump(path: str, args) -> None:
@@ -113,19 +97,19 @@ def _reference_inputs(means3D, shs, colors_precomp, scales, rotations, cov3D_pre
 
 
 def _fp32_inputs(means3D, sh, colors_precomp, semantics, opacities, scales, rotations, cov3Ds_precomp):
-    """The kernels' inputs as contiguous fp32 on means3D's device; an absent or empty optional input, and semantics without
-    channels, is None."""
+    """The kernels' inputs as contiguous fp32 on means3D's device (the reference calls .contiguous() on every argument,
+    DGR/rasterize_points.cu:92-118), 16-byte aligned; an absent or empty optional input, and semantics without channels, is None."""
     if means3D.dim() != 2 or means3D.shape[1] != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")  # DGR/rasterize_points.cu:58-60
     if not means3D.is_cuda:
         raise _capi.SgrError("street_gaussians_b200 rasterizer needs CUDA tensors (there is no CPU fallback)")
     device = means3D.device
     S = int(semantics.shape[1]) if (semantics is not None and semantics.dim() == 2) else 0
-    tensors = dict(means3D=_dev_f32(means3D, device), opacities=_dev_f32(opacities, device))
+    tensors = dict(means3D=_capi.f32(means3D, device, align16=True), opacities=_capi.f32(opacities, device, align16=True))
     for name, t in (("sh", _none_if_empty(sh)), ("colors_precomp", _none_if_empty(colors_precomp)), ("scales", _none_if_empty(scales)),
                     ("rotations", _none_if_empty(rotations)), ("cov3Ds_precomp", _none_if_empty(cov3Ds_precomp)),
                     ("semantics", semantics if S > 0 else None)):
-        tensors[name] = _dev_f32(t, device) if t is not None else None
+        tensors[name] = _capi.f32(t, device, align16=True) if t is not None else None
     return tensors
 
 
@@ -164,8 +148,7 @@ def _geom_grad_buffers(tensors, P: int, device):
 
 def _copy_status(fr, geom, host_status: torch.Tensor, device):
     """sgr_forward_status_async: the status words of the forward just enqueued into pinned `host_status`, on the current stream."""
-    rc = _capi.lib().sgr_forward_status_async(C.byref(fr), _ptr(geom), C.c_void_p(host_status.data_ptr()), _stream(device))
-    _capi.check(rc, "sgr_forward_status_async")
+    _capi.call("sgr_forward_status_async", device, C.byref(fr), ptr(geom), C.c_void_p(host_status.data_ptr()))
 
 
 class InstanceCapacity:
@@ -276,7 +259,7 @@ def _forward_impl(means3D, sh, colors_precomp, semantics, opacities, scales, rot
 
     fr, keep = _make_frame(settings, P, M, S, device, band)
     gb, ib = C.c_size_t(0), C.c_size_t(0)
-    _capi.check(L.sgr_state_sizes(C.byref(fr), C.byref(gb), C.byref(ib)), "sgr_state_sizes")
+    _capi.call("sgr_state_sizes", None, C.byref(fr), C.byref(gb), C.byref(ib))
     st.geom = torch.empty((gb.value,), device=device, dtype=torch.uint8)
     st.img = torch.empty((ib.value,), device=device, dtype=torch.uint8)
 
@@ -287,15 +270,12 @@ def _forward_impl(means3D, sh, colors_precomp, semantics, opacities, scales, rot
         cap = int(capacity.capacity)
         nbytes = int(L.sgr_binning_bytes(cap))
         st.binning = torch.empty((nbytes,), device=device, dtype=torch.uint8)
-        with torch.cuda.device(device):
-            rc = L.sgr_forward_bounded(C.byref(fr), _ptr(tensors["means3D"]), _ptr(tensors["sh"]), _ptr(tensors["colors_precomp"]),
-                                       _ptr(tensors["semantics"]), _ptr(tensors["opacities"]), _ptr(tensors["scales"]),
-                                       _ptr(tensors["rotations"]), _ptr(tensors["cov3Ds_precomp"]), _ptr(color), _ptr(depth), _ptr(alpha),
-                                       _ptr(semantic), _ptr(radii), _ptr(st.geom), gb.value, _ptr(st.img), ib.value, _ptr(st.binning), nbytes,
-                                       cap, _stream(device))
-            _capi.check(rc, "sgr_forward_bounded")
-            if not capacity.frozen:
-                capacity.record_status(fr, st.geom, device)
+        _capi.call("sgr_forward_bounded", device, C.byref(fr), ptr(tensors["means3D"]), ptr(tensors["sh"]), ptr(tensors["colors_precomp"]),
+                   ptr(tensors["semantics"]), ptr(tensors["opacities"]), ptr(tensors["scales"]), ptr(tensors["rotations"]),
+                   ptr(tensors["cov3Ds_precomp"]), ptr(color), ptr(depth), ptr(alpha), ptr(semantic), ptr(radii), ptr(st.geom), gb.value,
+                   ptr(st.img), ib.value, ptr(st.binning), nbytes, cap)
+        if not capacity.frozen:
+            capacity.record_status(fr, st.geom, device)
         st.num_instances = cap
         del keep
         return color, radii, depth, alpha, semantic, st, tensors
@@ -306,13 +286,10 @@ def _forward_impl(means3D, sh, colors_precomp, semantics, opacities, scales, rot
 
     cb = _capi.ALLOC_FN(_alloc)
     bin_ptr, n_inst = C.c_void_p(), C.c_int64(0)
-    with torch.cuda.device(device):
-        rc = L.sgr_forward(C.byref(fr), _ptr(tensors["means3D"]), _ptr(tensors["sh"]), _ptr(tensors["colors_precomp"]),
-                           _ptr(tensors["semantics"]), _ptr(tensors["opacities"]), _ptr(tensors["scales"]),
-                           _ptr(tensors["rotations"]), _ptr(tensors["cov3Ds_precomp"]), _ptr(color), _ptr(depth), _ptr(alpha),
-                           _ptr(semantic), _ptr(radii), _ptr(st.geom), gb.value, _ptr(st.img), ib.value, cb, None,
-                           C.byref(bin_ptr), C.byref(n_inst), _stream(device))
-    _capi.check(rc, "sgr_forward")
+    _capi.call("sgr_forward", device, C.byref(fr), ptr(tensors["means3D"]), ptr(tensors["sh"]), ptr(tensors["colors_precomp"]),
+               ptr(tensors["semantics"]), ptr(tensors["opacities"]), ptr(tensors["scales"]), ptr(tensors["rotations"]),
+               ptr(tensors["cov3Ds_precomp"]), ptr(color), ptr(depth), ptr(alpha), ptr(semantic), ptr(radii), ptr(st.geom), gb.value,
+               ptr(st.img), ib.value, cb, None, C.byref(bin_ptr), C.byref(n_inst))
     st.num_instances = int(n_inst.value)
     if capacity is not None:
         capacity.observe(st.num_instances)
@@ -324,7 +301,6 @@ def _backward_blend_impl(settings, band, st: _ForwardState, tensors, alpha, grad
                          grad2d_out: Optional[torch.Tensor] = None):
     """Stage 1: returns (grad2d[P,12], dL_dsemantics[P,S]) — the per-rank partial sums under tile-row sharding.
     grad2d_out: write the sums there instead of a fresh tensor (peer-mapped workspace of the Gaussian-sharded mode)."""
-    L = _capi.lib()
     means3D = tensors["means3D"]
     device, P = means3D.device, means3D.shape[0]
     S = int(tensors["semantics"].shape[1]) if tensors["semantics"] is not None else 0
@@ -332,13 +308,10 @@ def _backward_blend_impl(settings, band, st: _ForwardState, tensors, alpha, grad
     fr, keep = _make_frame(settings, P, M, S, device, band)
     grad2d = grad2d_out if grad2d_out is not None else torch.empty((P, 12), device=device, dtype=torch.float32)
     g_sem = torch.empty((P, S), device=device, dtype=torch.float32)
-    gc, gd, ga = _dev_f32(grad_color, device), _dev_f32(grad_depth, device), _dev_f32(grad_alpha, device)
-    gs = _dev_f32(grad_semantic, device) if S > 0 else None
-    with torch.cuda.device(device):
-        rc = L.sgr_backward_blend(C.byref(fr), st.num_instances, _ptr(tensors["semantics"]), _ptr(st.geom), _ptr(st.binning),
-                                  _ptr(st.img), _ptr(alpha), _ptr(gc), _ptr(gd), _ptr(ga), _ptr(gs), _ptr(grad2d), _ptr(g_sem),
-                                  _stream(device))
-    _capi.check(rc, "sgr_backward_blend")
+    gc, gd, ga = (_capi.f32(g, device, align16=True) for g in (grad_color, grad_depth, grad_alpha))
+    gs = _capi.f32(grad_semantic, device, align16=True) if S > 0 else None
+    _capi.call("sgr_backward_blend", device, C.byref(fr), st.num_instances, ptr(tensors["semantics"]), ptr(st.geom), ptr(st.binning),
+               ptr(st.img), ptr(alpha), ptr(gc), ptr(gd), ptr(ga), ptr(gs), ptr(grad2d), ptr(g_sem))
     del keep
     return grad2d, g_sem
 
@@ -347,7 +320,6 @@ def _backward_layer_blends(settings, st: _ForwardState, tensors, layers, layer_b
     """The layers' stage 1 (sgr_backward_blend_layer): returns (SgrLayerGrad table for _backward_geom_impl, gradient of each layer's
     means2D sink or None, tensors the table points into).  A layer with an empty range, or whose outputs got no upstream gradient,
     keeps a table row without grad2d and costs nothing."""
-    L = _capi.lib()
     means3D = tensors["means3D"]
     dev, P = means3D.device, int(means3D.shape[0])
     S = int(tensors["semantics"].shape[1]) if tensors["semantics"] is not None else 0
@@ -359,13 +331,11 @@ def _backward_layer_blends(settings, st: _ForwardState, tensors, layers, layer_b
         lg = _capi.SgrLayerGrad(b, e, None, None)
         sg = None
         if (gc is not None or gd is not None or ga is not None) and e > b:
-            gc, gd, ga = (_dev_f32(g, dev) for g in _image_grads(settings, dev, (gc, gd, ga), (3, 1, 1)))
+            gc, gd, ga = (_capi.f32(g, dev, align16=True) for g in _image_grads(settings, dev, (gc, gd, ga), (3, 1, 1)))
             g2 = torch.empty((e - b, 12), device=dev, dtype=torch.float32)
             lay = _capi.SgrLayer(b, e, layer_bgs[k].data_ptr())
-            with torch.cuda.device(dev):
-                rc = L.sgr_backward_blend_layer(C.byref(fr), C.byref(lay), _ptr(st.geom), _ptr(layer_states[k]), _ptr(layer_alphas[k]),
-                                                _ptr(gc), _ptr(gd), _ptr(ga), _ptr(g2), _stream(dev))
-            _capi.check(rc, "sgr_backward_blend_layer")
+            _capi.call("sgr_backward_blend_layer", dev, C.byref(fr), C.byref(lay), ptr(st.geom), ptr(layer_states[k]), ptr(layer_alphas[k]),
+                       ptr(gc), ptr(gd), ptr(ga), ptr(g2))
             lg.grad2d = g2.data_ptr()
             keep_alive += [gc, gd, ga, g2]
             if sink is not None and sink_wanted[k]:
@@ -381,7 +351,6 @@ def _backward_geom_impl(settings, band, st: _ForwardState, tensors, radii, grad2
     """Stage 2: per-Gaussian chain rule.  Outputs are torch.empty — the kernel writes every element.  `layers`: the SgrLayerGrad
     table of _backward_layer_blends; the rows of its live layers are merged into grad2d (sgr_backward_geom_layered), while the
     main means2D gradient stays that of the main images."""
-    L = _capi.lib()
     means3D = tensors["means3D"]
     device, P = means3D.device, means3D.shape[0]
     S = int(tensors["semantics"].shape[1]) if tensors["semantics"] is not None else 0
@@ -390,17 +359,14 @@ def _backward_geom_impl(settings, band, st: _ForwardState, tensors, radii, grad2
     fr, keep = _make_frame(settings, P, M, S, device, band)
     grads = _geom_grad_buffers(tensors, P, device)
     live = [lg for lg in layers or () if lg.grad2d]
-    inputs = (C.byref(fr), _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(scales), _ptr(rots), _ptr(cov), _ptr(radii), _ptr(st.geom),
-              _ptr(grad2d))
-    with torch.cuda.device(device):
-        if not live:
-            rc = L.sgr_backward_geom(*inputs, *map(_ptr, grads), _stream(device))
-        else:
-            lo, hi = min(lg.begin for lg in live), max(lg.end for lg in live)
-            scratch = torch.empty((3 * (hi - lo),), device=device, dtype=torch.float32)
-            table = (_capi.SgrLayerGrad * len(layers))(*layers)
-            rc = L.sgr_backward_geom_layered(*inputs, table, len(layers), _ptr(scratch), *map(_ptr, grads), _stream(device))
-    _capi.check(rc, "sgr_backward_geom_layered" if live else "sgr_backward_geom")
+    inputs = (C.byref(fr), ptr(means3D), ptr(sh), ptr(colors), ptr(scales), ptr(rots), ptr(cov), ptr(radii), ptr(st.geom), ptr(grad2d))
+    if not live:
+        _capi.call("sgr_backward_geom", device, *inputs, *map(ptr, grads))
+    else:
+        lo, hi = min(lg.begin for lg in live), max(lg.end for lg in live)
+        scratch = torch.empty((3 * (hi - lo),), device=device, dtype=torch.float32)
+        table = (_capi.SgrLayerGrad * len(layers))(*layers)
+        _capi.call("sgr_backward_geom_layered", device, *inputs, table, len(layers), ptr(scratch), *map(ptr, grads))
     del keep
     return grads
 
@@ -423,7 +389,6 @@ def _forward_or_dump(means3D, sh, colors_precomp, semantics, opacities, scales, 
 def _forward_layers(settings, st: _ForwardState, tensors, P: int, device, layers):
     """Renders every layer from the tile lists of the main forward in `st` (sgr_forward_layer).  Returns (bg tensor per layer, layer
     state per layer, [color, depth, alpha] of every layer in one flat list); an empty range needs no state."""
-    L = _capi.lib()
     H, W = int(settings.image_height), int(settings.image_width)
     M = int(tensors["sh"].shape[1]) if tensors is not None and tensors["sh"] is not None else 0
     S = int(tensors["semantics"].shape[1]) if tensors is not None and tensors["semantics"] is not None else 0
@@ -431,18 +396,16 @@ def _forward_layers(settings, st: _ForwardState, tensors, P: int, device, layers
     f32 = dict(device=device, dtype=torch.float32)
     bgs, states, outs = [], [], []
     for b, e, bg, _ in layers:
-        bg = _dev_f32(bg, device)
+        bg = _capi.f32(bg, device, align16=True)
         c, d, a = torch.empty((3, H, W), **f32), torch.empty((1, H, W), **f32), torch.empty((1, H, W), **f32)
         lay = _capi.SgrLayer(b, e, bg.data_ptr())
         ls, nbytes = None, 0
         if e > b:
             nb = C.c_size_t(0)
-            _capi.check(L.sgr_layer_state_sizes(C.byref(fr), st.num_instances, C.byref(nb)), "sgr_layer_state_sizes")
+            _capi.call("sgr_layer_state_sizes", None, C.byref(fr), st.num_instances, C.byref(nb))
             ls, nbytes = torch.empty((nb.value,), device=device, dtype=torch.uint8), nb.value
-        with torch.cuda.device(device):
-            rc = L.sgr_forward_layer(C.byref(fr), C.byref(lay), st.num_instances, _ptr(st.geom), _ptr(st.binning), _ptr(st.img), _ptr(ls),
-                                     nbytes, _ptr(c), _ptr(d), _ptr(a), _stream(device))
-        _capi.check(rc, "sgr_forward_layer")
+        _capi.call("sgr_forward_layer", device, C.byref(fr), C.byref(lay), st.num_instances, ptr(st.geom), ptr(st.binning), ptr(st.img),
+                   ptr(ls), nbytes, ptr(c), ptr(d), ptr(a))
         bgs.append(bg)
         states.append(ls)
         outs += [c, d, a]
@@ -570,20 +533,17 @@ class GaussianRasterizer(nn.Module):
             self.capacity.check(wait=True)
 
     def markVisible(self, positions):
-        L = _capi.lib()
         s = self.raster_settings
         with torch.no_grad():
             if not positions.is_cuda:
                 raise _capi.SgrError("markVisible needs a CUDA tensor")
             dev = positions.device
-            pos = _dev_f32(positions, dev)
+            pos = _capi.f32(positions, dev, align16=True)
             P = pos.shape[0]
             visible = torch.zeros((P,), device=dev, dtype=torch.bool)
             if P:
-                view, proj = _dev_f32(s.viewmatrix, dev), _dev_f32(s.projmatrix, dev)
-                with torch.cuda.device(dev):
-                    rc = L.sgr_mark_visible(P, _ptr(pos), _ptr(view), _ptr(proj), C.c_void_p(visible.data_ptr()), _stream(dev))
-                _capi.check(rc, "sgr_mark_visible")
+                view, proj = _capi.f32(s.viewmatrix, dev, align16=True), _capi.f32(s.projmatrix, dev, align16=True)
+                _capi.call("sgr_mark_visible", dev, P, ptr(pos), ptr(view), ptr(proj), C.c_void_p(visible.data_ptr()))
         return visible
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
@@ -615,7 +575,6 @@ class GaussianRasterizer(nn.Module):
         return tuple(out[:5]) + (tuple(tuple(out[5 + 3 * k: 8 + 3 * k]) for k in range(len(layers))),)
 
     def visible_filter(self, means3D, scales=None, rotations=None, cov3D_precomp=None) -> Tuple[torch.Tensor, torch.Tensor]:
-        L = _capi.lib()
         s = self.raster_settings
         with torch.no_grad():
             if means3D.dim() != 2 or means3D.shape[1] != 3:
@@ -627,15 +586,13 @@ class GaussianRasterizer(nn.Module):
             radii = torch.zeros((P,), device=dev, dtype=torch.int32)
             means2D = torch.zeros((P, 2), device=dev, dtype=torch.float32)
             if P:
-                m = _dev_f32(means3D, dev)
+                m = _capi.f32(means3D, dev, align16=True)
                 sc, ro, cv = _none_if_empty(scales), _none_if_empty(rotations), _none_if_empty(cov3D_precomp)
-                sc = _dev_f32(sc, dev) if sc is not None else None
-                ro = _dev_f32(ro, dev) if ro is not None else None
-                cv = _dev_f32(cv, dev) if cv is not None else None
+                sc = _capi.f32(sc, dev, align16=True) if sc is not None else None
+                ro = _capi.f32(ro, dev, align16=True) if ro is not None else None
+                cv = _capi.f32(cv, dev, align16=True) if cv is not None else None
                 fr, keep = _make_frame(s, P, 0, 0, dev, None)
-                with torch.cuda.device(dev):
-                    rc = L.sgr_visible_filter(C.byref(fr), _ptr(m), _ptr(sc), _ptr(ro), _ptr(cv), _ptr(radii), _ptr(means2D), _stream(dev))
-                _capi.check(rc, "sgr_visible_filter")
+                _capi.call("sgr_visible_filter", dev, C.byref(fr), ptr(m), ptr(sc), ptr(ro), ptr(cv), ptr(radii), ptr(means2D))
                 del keep
         return radii, means2D
 
@@ -646,13 +603,11 @@ def distCUDA2(points: torch.Tensor) -> torch.Tensor:
     if not points.is_cuda:
         raise _capi.SgrError("distCUDA2 needs a CUDA tensor")
     dev = points.device
-    pts = _dev_f32(points, dev)
+    pts = _capi.f32(points, dev, align16=True)
     P = pts.shape[0]
     out = torch.zeros((P,), device=dev, dtype=torch.float32)
     if P:
         nbytes = L.sgr_knn_scratch_bytes(P)
         scratch = torch.empty((nbytes,), device=dev, dtype=torch.uint8)
-        with torch.cuda.device(dev):
-            rc = L.sgr_knn_mean_dist2(P, _ptr(pts), _ptr(out), _ptr(scratch), nbytes, _stream(dev))
-        _capi.check(rc, "sgr_knn_mean_dist2")
+        _capi.call("sgr_knn_mean_dist2", dev, P, ptr(pts), ptr(out), ptr(scratch), nbytes)
     return out

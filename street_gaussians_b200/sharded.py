@@ -31,9 +31,10 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from . import _capi
+from ._capi import ptr
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, InstanceCapacity, TileRowBand, _copy_status, _ForwardState,
-                         _backward_blend_impl, _backward_geom_impl, _dev_f32, _fit_grads, _fp32_inputs, _geom_grad_buffers, _image_grads,
-                         _input_shapes, _make_frame, _ptr, _reference_inputs, _stream)
+                         _backward_blend_impl, _backward_geom_impl, _fit_grads, _fp32_inputs, _geom_grad_buffers, _image_grads,
+                         _input_shapes, _make_frame, _reference_inputs)
 
 
 def cyclic_band(image_height: int, rank: int, world: int) -> TileRowBand:
@@ -115,7 +116,6 @@ _local_tensors = _fp32_inputs  # step 0: the local Gaussians as the kernels read
 def project_records(tensors, settings: GaussianRasterizationSettings, chunk: int):
     """Step 1 (sgr_project): records[chunk,12] float32 view + radii[chunk] int32 of the local Gaussians; slots past
     P_local are padding (radii == 0)."""
-    L = _capi.lib()
     means3D = tensors["means3D"]
     device, P = means3D.device, int(means3D.shape[0])
     if P > chunk:
@@ -124,11 +124,8 @@ def project_records(tensors, settings: GaussianRasterizationSettings, chunk: int
     radii = (torch.empty if P == chunk else torch.zeros)((chunk,), device=device, dtype=torch.int32)
     M = int(tensors["sh"].shape[1]) if tensors["sh"] is not None else 0
     fr, keep = _make_frame(settings, P, M, 0, device, None)
-    with torch.cuda.device(device):
-        rc = L.sgr_project(C.byref(fr), _ptr(means3D), _ptr(tensors["sh"]), _ptr(tensors["colors_precomp"]), _ptr(tensors["opacities"]),
-                           _ptr(tensors["scales"]), _ptr(tensors["rotations"]), _ptr(tensors["cov3Ds_precomp"]), _ptr(radii), _ptr(rec),
-                           _stream(device))
-    _capi.check(rc, "sgr_project")
+    _capi.call("sgr_project", device, C.byref(fr), ptr(means3D), ptr(tensors["sh"]), ptr(tensors["colors_precomp"]), ptr(tensors["opacities"]),
+               ptr(tensors["scales"]), ptr(tensors["rotations"]), ptr(tensors["cov3Ds_precomp"]), ptr(radii), ptr(rec))
     del keep
     return rec, radii
 
@@ -136,10 +133,9 @@ def project_records(tensors, settings: GaussianRasterizationSettings, chunk: int
 def alloc_gathered(settings: GaussianRasterizationSettings, P_total: int, S: int, device):
     """Forward state for P_total gathered Gaussians.  Returns (state, records view [P_total,12] float32 into state.geom —
     the all-gather target —, geom_bytes, img_bytes)."""
-    L = _capi.lib()
     fr, keep = _make_frame(settings, P_total, 0, S, device, None)
     gb, ib = C.c_size_t(0), C.c_size_t(0)
-    _capi.check(L.sgr_state_sizes(C.byref(fr), C.byref(gb), C.byref(ib)), "sgr_state_sizes")
+    _capi.call("sgr_state_sizes", None, C.byref(fr), C.byref(gb), C.byref(ib))
     st = _ForwardState()
     st.geom = torch.empty((gb.value,), device=device, dtype=torch.uint8)
     st.img = torch.empty((ib.value,), device=device, dtype=torch.uint8)
@@ -176,18 +172,15 @@ def forward_records(settings: GaussianRasterizationSettings, band: Optional[Tile
 
     cb = _capi.ALLOC_FN() if bounded else _capi.ALLOC_FN(_alloc)
     bin_ptr, n_inst = C.c_void_p(), C.c_int64(0)
-    with torch.cuda.device(device):
-        rc = L.sgr_forward_records(C.byref(fr), _ptr(radii_all), _ptr(semantics_all), _ptr(color), _ptr(depth), _ptr(alpha), _ptr(semantic),
-                                   _ptr(st.geom), gb, _ptr(st.img), ib, cb, None, C.byref(bin_ptr), C.byref(n_inst),
-                                   _ptr(st.binning) if bounded else None, nbytes, cap, _stream(device))
-        _capi.check(rc, "sgr_forward_records")
-        if bounded:
-            capacity.record_status(fr, st.geom, device)
-            st.num_instances = cap
-        else:
-            st.num_instances = int(n_inst.value)
-            if capacity is not None:
-                capacity.observe(st.num_instances)
+    _capi.call("sgr_forward_records", device, C.byref(fr), ptr(radii_all), ptr(semantics_all), ptr(color), ptr(depth), ptr(alpha), ptr(semantic),
+               ptr(st.geom), gb, ptr(st.img), ib, cb, None, C.byref(bin_ptr), C.byref(n_inst), ptr(st.binning) if bounded else None, nbytes, cap)
+    if bounded:
+        capacity.record_status(fr, st.geom, device)
+        st.num_instances = cap
+    else:
+        st.num_instances = int(n_inst.value)
+        if capacity is not None:
+            capacity.observe(st.num_instances)
     del keep
     return color, depth, alpha, semantic
 
@@ -258,10 +251,9 @@ class PeerWorkspace:
     @staticmethod
     def layout(settings, P_total: int, device):
         """(geom_bytes, img_bytes, offset of radii_all, offset of grad2d, offset of the barrier pad, total bytes) of the per-rank buffer."""
-        L = _capi.lib()
         fr, keep = _make_frame(settings, P_total, 0, 0, device, None)
         gb, ib = C.c_size_t(0), C.c_size_t(0)
-        _capi.check(L.sgr_state_sizes(C.byref(fr), C.byref(gb), C.byref(ib)), "sgr_state_sizes")
+        _capi.call("sgr_state_sizes", None, C.byref(fr), C.byref(gb), C.byref(ib))
         del keep
         off_radii = _align(gb.value)
         off_grad = _align(off_radii + 4 * P_total)
@@ -303,25 +295,19 @@ class PeerWorkspace:
 
 def scatter_records(settings, ws: PeerWorkspace, rec_local, radii_local, P_local: int):
     """Step 2 over peer memory (sgr_scatter_records).  The caller issues ws.barrier() afterwards."""
-    L = _capi.lib()
     device = rec_local.device
     fr, keep = _make_frame(settings, P_local, 0, 0, device, None)
-    with torch.cuda.device(device):
-        rc = L.sgr_scatter_records(C.byref(fr), C.byref(ws.peers), _ptr(rec_local), _ptr(radii_local), _stream(device))
-    _capi.check(rc, "sgr_scatter_records")
+    _capi.call("sgr_scatter_records", device, C.byref(fr), C.byref(ws.peers), ptr(rec_local), ptr(radii_local))
     del keep
 
 
 def gather_grad2d(settings, ws: PeerWorkspace, rec_local, radii_local, P_local: int):
     """Step 4 over peer memory (sgr_gather_grad2d): summed grad2d rows [chunk,12] of the local Gaussians.  The caller has
     issued ws.barrier() after every rank's backward_blend_records(grad2d_out=ws.grad2d)."""
-    L = _capi.lib()
     device = rec_local.device
     out = torch.empty((ws.chunk, 12), device=device, dtype=torch.float32)
     fr, keep = _make_frame(settings, P_local, 0, 0, device, None)
-    with torch.cuda.device(device):
-        rc = L.sgr_gather_grad2d(C.byref(fr), C.byref(ws.peers), _ptr(rec_local), _ptr(radii_local), _ptr(out), _stream(device))
-    _capi.check(rc, "sgr_gather_grad2d")
+    _capi.call("sgr_gather_grad2d", device, C.byref(fr), C.byref(ws.peers), ptr(rec_local), ptr(radii_local), ptr(out))
     del keep
     return out
 
@@ -446,17 +432,14 @@ def sharded_forward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, ca
     pre = 1 if ws.fwd_pending else 0
     ws.next_epochs(1 + pre)  # host-side tally only: the epochs themselves are counted on the device (barrier_epoch = 0)
     epoch = 0
-    with torch.cuda.device(device):
-        rc = L.sgr_sharded_forward(C.byref(fr), C.byref(ws.peers), _ptr(tensors["means3D"]), _ptr(tensors["sh"]), _ptr(tensors["colors_precomp"]),
-                                   _ptr(tensors["opacities"]), _ptr(tensors["scales"]), _ptr(tensors["rotations"]), _ptr(tensors["cov3Ds_precomp"]),
-                                   _ptr(color), _ptr(depth), _ptr(alpha), _ptr(bufs["radii"]), _ptr(bufs["rec"]), ws.geom_bytes,
-                                   _ptr(bufs["img"]), ws.img_bytes, _ptr(bufs["binning"]), nbytes, capacity, gaussian_capacity, epoch, pre,
-                                   _stream(device))
-        _capi.check(rc, "sgr_sharded_forward")
-        if status_word is not None:  # the status of the gathered frame (P_total slots)
-            frt, keep2 = _make_frame(settings, ws.P_total, 0, 0, device, band)
-            _copy_status(frt, ws.geom, status_word, device)
-            del keep2
+    _capi.call("sgr_sharded_forward", device, C.byref(fr), C.byref(ws.peers), ptr(tensors["means3D"]), ptr(tensors["sh"]),
+               ptr(tensors["colors_precomp"]), ptr(tensors["opacities"]), ptr(tensors["scales"]), ptr(tensors["rotations"]),
+               ptr(tensors["cov3Ds_precomp"]), ptr(color), ptr(depth), ptr(alpha), ptr(bufs["radii"]), ptr(bufs["rec"]), ws.geom_bytes,
+               ptr(bufs["img"]), ws.img_bytes, ptr(bufs["binning"]), nbytes, capacity, gaussian_capacity, epoch, pre)
+    if status_word is not None:  # the status of the gathered frame (P_total slots)
+        frt, keep2 = _make_frame(settings, ws.P_total, 0, 0, device, band)
+        _copy_status(frt, ws.geom, status_word, device)
+        del keep2
     del keep
     ws.fwd_pending = True
     return color, depth, alpha, bufs
@@ -464,7 +447,6 @@ def sharded_forward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, ca
 
 def sharded_backward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, capacity: int, alpha, gc, gd, ga):
     """One sgr_sharded_backward call on the current stream.  Returns the 8 gradients in _backward_geom_impl's order."""
-    L = _capi.lib()
     dev = alpha.device
     sh, colors, scales, rots, cov = (tensors[k] for k in ("sh", "colors_precomp", "scales", "rotations", "cov3Ds_precomp"))
     M = int(sh.shape[1]) if sh is not None else 0
@@ -473,12 +455,9 @@ def sharded_backward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, c
     fr, keep = _make_frame(settings, P, M, 0, dev, band)
     ws.next_epochs(1)
     epoch = 0  # device-side count
-    with torch.cuda.device(dev):
-        rc = L.sgr_sharded_backward(C.byref(fr), C.byref(ws.peers), capacity, _ptr(tensors["means3D"]), _ptr(sh), _ptr(colors), _ptr(scales),
-                                    _ptr(rots), _ptr(cov), _ptr(bufs["radii"]), _ptr(bufs["rec"]), _ptr(bufs["img"]), _ptr(bufs["binning"]),
-                                    _ptr(alpha), _ptr(gc), _ptr(gd), _ptr(ga), _ptr(g_means3D), _ptr(g_means2D), _ptr(g_sh), _ptr(g_colors),
-                                    _ptr(g_opac), _ptr(g_scales), _ptr(g_rots), _ptr(g_cov), epoch, _stream(dev))
-    _capi.check(rc, "sgr_sharded_backward")
+    _capi.call("sgr_sharded_backward", dev, C.byref(fr), C.byref(ws.peers), capacity, ptr(tensors["means3D"]), ptr(sh), ptr(colors), ptr(scales),
+               ptr(rots), ptr(cov), ptr(bufs["radii"]), ptr(bufs["rec"]), ptr(bufs["img"]), ptr(bufs["binning"]), ptr(alpha), ptr(gc), ptr(gd),
+               ptr(ga), ptr(g_means3D), ptr(g_means2D), ptr(g_sh), ptr(g_colors), ptr(g_opac), ptr(g_scales), ptr(g_rots), ptr(g_cov), epoch)
     del keep
     ws.fwd_pending = False  # every rank passed the backward barrier after its blend_bwd: the records may be overwritten
     return g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rots, g_cov
@@ -516,7 +495,7 @@ def _fused_backward(ctx, grad_color, grad_depth, grad_alpha):
     (alpha,) = ctx.saved_tensors
     settings, owner, ws, P, tensors, shapes = ctx.settings, ctx.owner, ctx.ws, ctx.P, ctx.tensors, ctx.shapes
     dev = alpha.device
-    gc, gd, ga = (_dev_f32(g, dev) for g in _image_grads(settings, dev, (grad_color, grad_depth, grad_alpha), (3, 1, 1)))
+    gc, gd, ga = (_capi.f32(g, dev, align16=True) for g in _image_grads(settings, dev, (grad_color, grad_depth, grad_alpha), (3, 1, 1)))
     g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rots, g_cov = sharded_backward_raw(settings, owner.band, ws, tensors, P,
                                                                                                    ctx.capacity, alpha, gc, gd, ga)
     ws.in_flight = False

@@ -17,7 +17,7 @@ from typing import Optional
 import torch
 
 from . import _capi
-from .rasterizer import _ptr, _stream
+from ._capi import ptr
 
 
 def _check(rgb, acc, cube_map, K, w2c, sky_mask):
@@ -53,7 +53,6 @@ class _SkyComposite(torch.autograd.Function):
     @staticmethod
     def forward(ctx, rgb, acc, cube_map, K, w2c, sky_mask, perturb: bool, fill: float):
         H, W, R = _check(rgb, acc, cube_map, K, w2c, sky_mask)
-        L = _capi.lib()
         dev = rgb.device
         rgb_c, acc_c, cube = rgb.contiguous(), acc.contiguous(), cube_map.contiguous()
         Kc, Tc = K.contiguous(), w2c.contiguous()
@@ -65,17 +64,14 @@ class _SkyComposite(torch.autograd.Function):
         else:
             jx = jy = None
         out = torch.empty_like(rgb_c)
-        with torch.cuda.device(dev):
-            rc = L.sgr_sky_composite_forward(H, W, R, mode, float(fill), _ptr(rgb_c), _ptr(acc_c), _ptr(mask), _ptr(cube), _ptr(Kc), _ptr(Tc),
-                                             _ptr(jx), _ptr(jy), _ptr(out), _stream(dev))
-        _capi.check(rc, "sgr_sky_composite_forward")
+        _capi.call("sgr_sky_composite_forward", dev, H, W, R, mode, float(fill), ptr(rgb_c), ptr(acc_c), ptr(mask), ptr(cube), ptr(Kc), ptr(Tc),
+                   ptr(jx), ptr(jy), ptr(out))
         ctx.save_for_backward(acc_c, cube, Kc, Tc, mask, jx, jy)
         ctx.args = (H, W, R, mode, float(fill))
         return out
 
     @staticmethod
     def backward(ctx, g_out):
-        L = _capi.lib()
         acc, cube, Kc, Tc, mask, jx, jy = ctx.saved_tensors
         H, W, R, mode, fill = ctx.args
         dev = acc.device
@@ -83,10 +79,8 @@ class _SkyComposite(torch.autograd.Function):
         need_rgb, need_acc, need_cube = ctx.needs_input_grad[:3]
         g_acc = torch.empty_like(acc) if need_acc else None
         g_cube = torch.zeros_like(cube) if need_cube else None
-        with torch.cuda.device(dev):
-            rc = L.sgr_sky_composite_backward(H, W, R, mode, fill, _ptr(acc), _ptr(mask), _ptr(cube), _ptr(Kc), _ptr(Tc), _ptr(jx), _ptr(jy),
-                                              _ptr(g), _ptr(g_acc), _ptr(g_cube), _stream(dev))
-        _capi.check(rc, "sgr_sky_composite_backward")
+        _capi.call("sgr_sky_composite_backward", dev, H, W, R, mode, fill, ptr(acc), ptr(mask), ptr(cube), ptr(Kc), ptr(Tc), ptr(jx), ptr(jy),
+                   ptr(g), ptr(g_acc), ptr(g_cube))
         return (g_out if need_rgb else None), g_acc, g_cube, None, None, None, None, None
 
 

@@ -28,7 +28,7 @@ from typing import Iterable, Sequence
 import torch
 
 from . import _capi
-from .rasterizer import _ptr, _stream
+from ._capi import ptr
 
 
 def _attr(model, name):
@@ -36,7 +36,6 @@ def _attr(model, name):
 
 
 def add_densification_stats(models: Sequence, radii: torch.Tensor, viewspace_point_grad: torch.Tensor) -> None:
-    L = _capi.lib()
     if not radii.is_cuda:
         raise _capi.SgrError("add_densification_stats needs CUDA tensors (there is no CPU fallback)")
     dev = radii.device
@@ -58,11 +57,8 @@ def add_densification_stats(models: Sequence, radii: torch.Tensor, viewspace_poi
     if radii.numel() != start or viewspace_point_grad.shape != (start, 3):
         raise ValueError(f"radii must be [{start}] and the viewspace gradient [{start}, 3] for these models")
     r = radii if (radii.dtype == torch.int32 and radii.is_contiguous()) else radii.to(torch.int32).contiguous()
-    g = viewspace_point_grad if (viewspace_point_grad.dtype == torch.float32 and viewspace_point_grad.is_contiguous()) \
-        else viewspace_point_grad.to(torch.float32).contiguous()
-    with torch.cuda.device(dev):
-        rc = L.sgr_densify_stats(segs, n, _ptr(r), _ptr(g), _stream(dev))
-    _capi.check(rc, "sgr_densify_stats")
+    g = _capi.f32(viewspace_point_grad)
+    _capi.call("sgr_densify_stats", dev, segs, n, ptr(r), ptr(g))
 
 
 def _advance_state(st, p):
@@ -84,7 +80,6 @@ class FusedAdam(torch.optim.Optimizer):
     @torch.no_grad()
     def step(self, closure=None):
         loss = closure() if closure is not None else None
-        L = _capi.lib()
         buckets = {}  # (device, betas, eps) -> [(param, group)]
         for group in self.param_groups:
             for p in group["params"]:
@@ -100,14 +95,12 @@ class FusedAdam(torch.optim.Optimizer):
             keep = []
             for k, (p, group) in enumerate(items):
                 st = _advance_state(self.state[p], p)
-                g = p.grad if (p.grad.dtype == torch.float32 and p.grad.is_contiguous()) else p.grad.to(torch.float32).contiguous()
+                g = _capi.f32(p.grad)
                 keep.append(g)
                 t = tab[k]
                 t.param, t.grad, t.exp_avg, t.exp_avg_sq = p.data_ptr(), g.data_ptr(), st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr()
                 t.numel, t.lr, t.step = p.numel(), float(group["lr"]), st["step"]
-            with torch.cuda.device(dev):
-                rc = L.sgr_adam_step(tab, len(items), float(betas[0]), float(betas[1]), eps, _stream(dev))
-            _capi.check(rc, "sgr_adam_step")
+            _capi.call("sgr_adam_step", dev, tab, len(items), float(betas[0]), float(betas[1]), eps)
             del keep
         return loss
 
@@ -252,10 +245,8 @@ def _densify(models, max_grad, min_opacity, prune_big_points, optimizer=None, gr
     nbytes = L.sgr_densify_scratch_bytes(nm, P)
     scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     result = (C.c_int64 * (nm * _capi.DENSIFY_RESULT))()
-    npp = _ptr(noise) if noise is not None else None
-    with torch.cuda.device(dev):
-        rc = L.sgr_densify_plan(segs, nm, C.c_uint64(seed), npp, scratch.data_ptr(), nbytes, result, _stream(dev))
-    _capi.check(rc, "sgr_densify_plan")
+    npp = ptr(noise) if noise is not None else None
+    _capi.call("sgr_densify_plan", dev, segs, nm, C.c_uint64(seed), npp, scratch.data_ptr(), nbytes, result)
     outs = (_capi.SgrDensifyOutput * nm)()
     new = []
     for k, (params, moments, widths) in enumerate(infos):
@@ -278,9 +269,7 @@ def _densify(models, max_grad, min_opacity, prune_big_points, optimizer=None, gr
         if n_new:
             o.max_radii2D, o.xyz_gradient_accum, o.denom = (t.data_ptr() for t in stats)
         new.append((np_, nmom, stats))
-    with torch.cuda.device(dev):
-        rc = L.sgr_densify_apply(segs, outs, nm, C.c_uint64(seed), npp, scratch.data_ptr(), nbytes, _stream(dev))
-    _capi.check(rc, "sgr_densify_apply")
+    _capi.call("sgr_densify_apply", dev, segs, outs, nm, C.c_uint64(seed), npp, scratch.data_ptr(), nbytes)
     scalars = []
     for k, m in enumerate(models):
         params, moments, _ = infos[k]
@@ -340,7 +329,6 @@ def reset_opacity(models: Sequence, optimizer=None) -> None:
     """GaussianModel.reset_opacity (lib/models/gaussian_model.py:410-414) for every model in one kernel:
     _opacity = inverse_sigmoid(min(sigmoid(_opacity), 0.01)) and the opacity's Adam moments zeroed, in place (the parameter
     objects stay the same, so the optimizer needs no update)."""
-    L = _capi.lib()
     models = list(models)
     if not models:
         return
@@ -358,9 +346,7 @@ def reset_opacity(models: Sequence, optimizer=None) -> None:
                 for t in mv:
                     _check_tensor(t, dev, f"model {k}: Adam state of _opacity")
                 segs[k].exp_avg[3], segs[k].exp_avg_sq[3] = mv[0].data_ptr(), mv[1].data_ptr()
-    with torch.cuda.device(dev):
-        rc = L.sgr_reset_opacity(segs, len(models), _stream(dev))
-    _capi.check(rc, "sgr_reset_opacity")
+    _capi.call("sgr_reset_opacity", dev, segs, len(models))
 
 
 # ---- visibility-masked Adam ----
@@ -444,7 +430,6 @@ class SparseAdam(torch.optim.Optimizer):
                 buckets.setdefault(key, []).append((k, a, p, lr, w))
         if not buckets:
             return loss
-        L = _capi.lib()
         r = radii.contiguous()
         for (betas, eps), items in buckets.items():
             # per model: param, grad, exp_avg, exp_avg_sq, width, lr, step of its 7 tensors, written into the ctypes record at once
@@ -459,7 +444,7 @@ class SparseAdam(torch.optim.Optimizer):
                     f = fields[k] = [[None] * 7, [None] * 7, [None] * 7, [None] * 7, [0] * 7, [0.0] * 7, [0] * 7]
                 f[4][a], f[5][a], f[6][a] = w, lr, st["step"]
                 if p.numel():
-                    g = p.grad if (p.grad.dtype == torch.float32 and p.grad.is_contiguous()) else p.grad.to(torch.float32).contiguous()
+                    g = _capi.f32(p.grad)
                     keep.append(g)
                     f[0][a], f[1][a], f[2][a], f[3][a] = p.data_ptr(), g.data_ptr(), st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr()
             segs = (_capi.SgrSparseAdamSegment * len(models))()
@@ -471,8 +456,6 @@ class SparseAdam(torch.optim.Optimizer):
                 f = fields[k]
                 if f is not None:
                     s.param[:], s.grad[:], s.exp_avg[:], s.exp_avg_sq[:], s.width[:], s.lr[:], s.step[:] = f
-            with torch.cuda.device(dev):
-                rc = L.sgr_sparse_adam_step(segs, len(models), _ptr(r), float(betas[0]), float(betas[1]), eps, _stream(dev))
-            _capi.check(rc, "sgr_sparse_adam_step")
+            _capi.call("sgr_sparse_adam_step", dev, segs, len(models), ptr(r), float(betas[0]), float(betas[1]), eps)
             del keep
         return loss

@@ -15,7 +15,7 @@ import torch
 import loss64_case as LC
 from oracle import step64 as S64
 from street_gaussians_b200 import _capi, losses
-from street_gaussians_b200.rasterizer import _ptr, _stream
+from street_gaussians_b200._capi import ptr, stream
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -39,8 +39,8 @@ def lidar_direct(c, with_grads):
     scalars = torch.empty(4, device=DEV)
     nbytes = int(L.sgr_lidar_depth_loss_scratch_bytes(N))
     scratch = torch.empty(nbytes, device=DEV, dtype=torch.uint8)
-    rc = L.sgr_lidar_depth_loss(N, _ptr(d), _ptr(a), _ptr(l), _ptr(m), C.c_double(c["keep"]), C.c_float(c["weight"]), _ptr(gd), _ptr(ga),
-                                _ptr(scalars), _ptr(scratch), nbytes, _stream(torch.device(DEV)))
+    rc = L.sgr_lidar_depth_loss(N, ptr(d), ptr(a), ptr(l), ptr(m), C.c_double(c["keep"]), C.c_float(c["weight"]), ptr(gd), ptr(ga),
+                                ptr(scalars), ptr(scratch), nbytes, stream(torch.device(DEV)))
     _capi.check(rc, "sgr_lidar_depth_loss")
     torch.cuda.synchronize()
     return scalars.cpu().numpy()

@@ -13,7 +13,7 @@ import compose_case as CC
 import street_gaussians_b200 as sgb
 from oracle import step64 as S64
 from street_gaussians_b200 import _capi, losses, training
-from street_gaussians_b200.rasterizer import _ptr, _stream
+from street_gaussians_b200._capi import ptr, stream
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -173,9 +173,9 @@ def test_compose_backward_c_abi_unposed_rows_are_zero(actors):
     dposes = torch.full((nseg, 8), float("nan"), device=DEV)
     scratch = torch.empty(nseg, 16, device=DEV)
     L = _capi.lib()
-    p = lambda t: _ptr(t) if t.numel() else None
-    rc = L.sgr_compose_backward(segs, gtab, nseg, M, _ptr(pose_tab), _ptr(idft_tab), None, None, p(up["xyz"]), p(up["rotation"]),
-                                p(up["scaling"]), p(up["opacity"]), p(up["features"]), _ptr(dposes), _ptr(scratch), _stream(torch.device(DEV)))
+    p = lambda t: ptr(t) if t.numel() else None
+    rc = L.sgr_compose_backward(segs, gtab, nseg, M, ptr(pose_tab), ptr(idft_tab), None, None, p(up["xyz"]), p(up["rotation"]),
+                                p(up["scaling"]), p(up["opacity"]), p(up["features"]), ptr(dposes), ptr(scratch), stream(torch.device(DEV)))
     _capi.check(rc, "sgr_compose_backward")
     d = dposes.cpu()
     assert torch.equal(d[0], torch.zeros(8)), d[0]
@@ -231,8 +231,8 @@ def capi_image_loss(img, gt, mask, w_l1, w_ssim):
     scalars = torch.empty(4, device=DEV)
     nb = int(L.sgr_image_loss_scratch_bytes(Cn, H, W))
     scratch = torch.empty(nb, device=DEV, dtype=torch.uint8)
-    rc = L.sgr_image_loss(Cn, H, W, _ptr(x), _ptr(y), _ptr(m), float(w_l1), float(w_ssim), _ptr(grad), _ptr(scalars), _ptr(scratch), nb,
-                          _stream(torch.device(DEV)))
+    rc = L.sgr_image_loss(Cn, H, W, ptr(x), ptr(y), ptr(m), float(w_l1), float(w_ssim), ptr(grad), ptr(scalars), ptr(scratch), nb,
+                          stream(torch.device(DEV)))
     _capi.check(rc, "sgr_image_loss")
     return grad, scalars.cpu()
 
@@ -394,7 +394,7 @@ def test_sgr_adam_step_direct():
         t = tab[k]
         t.param, t.grad, t.exp_avg, t.exp_avg_sq = ps[k].data_ptr(), gs[k].data_ptr(), ms[k].data_ptr(), vs[k].data_ptr()
         t.numel, t.lr, t.step = shapes[k], lrs[k], steps[k]
-    rc = _capi.lib().sgr_adam_step(tab, n, 0.9, 0.999, 1e-15, _stream(torch.device(DEV)))
+    rc = _capi.lib().sgr_adam_step(tab, n, 0.9, 0.999, 1e-15, stream(torch.device(DEV)))
     _capi.check(rc, "sgr_adam_step")
     torch.cuda.synchronize()
     worst = {}

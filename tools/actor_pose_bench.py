@@ -135,7 +135,7 @@ def host_split(fused, ids, t, ego, w, iters=200):
     """Median host time (no synchronise) of the pieces of one fused forward + backward: the whole forward call, the whole backward
     call, and inside the forward the conversion of the table arguments and the bare ctypes call of sgr_actor_pose_forward."""
     from street_gaussians_b200 import _capi
-    from street_gaussians_b200.rasterizer import _ptr, _stream
+    from street_gaussians_b200._capi import ptr, stream
     L = _capi.lib()
     slots = (ctypes.c_int32 * len(ids))(*[fused._slot[i] for i in ids])
     poses = torch.empty((len(ids), 7), device=DEV)
@@ -149,8 +149,8 @@ def host_split(fused, ids, t, ego, w, iters=200):
         t2 = time.perf_counter()
         args = fused._table_args()
         t3 = time.perf_counter()
-        rc = L.sgr_actor_pose_forward(*args, len(ids), slots, t, 0, 0, _ptr(ego), _ptr(fused.opt_trans), _ptr(fused.opt_rots), 0, 1.0, 1,
-                                      _ptr(poses), None, _stream(ego.device))
+        rc = L.sgr_actor_pose_forward(*args, len(ids), slots, t, 0, 0, ptr(ego), ptr(fused.opt_trans), ptr(fused.opt_rots), 0, 1.0, 1,
+                                      ptr(poses), None, stream(ego.device))
         t4 = time.perf_counter()
         assert rc == 0
         for k, d in zip(parts, (t1 - t0, t2 - t1, t3 - t2, t4 - t3)):
