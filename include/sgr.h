@@ -491,6 +491,71 @@ size_t sgr_lidar_depth_loss_scratch_bytes(int64_t N);
 int sgr_lidar_depth_loss(int64_t N, const float *depth, const float *acc, const float *lidar_depth, const uint8_t *mask, double keep,
                          float weight, float *dL_ddepth, float *dL_dacc, float *scalars, void *scratch, size_t scratch_bytes, void *stream);
 
+/* ---- The same four losses on a tile-row band (multi-GPU: each rank holds the rendered rows of its band, DESIGN.md §8) ----
+ * The band is row_begin / row_end / row_step as in SgrFrame (16-pixel tile rows r with row_begin <= r < row_end, (r - row_begin) %
+ * row_step == 0; row_begin == row_end is an empty band).  The rendered inputs (image, acc, depth) are [.., H, W] frames of which the
+ * band's rows are read (and, for the image, the halo rows); gt, the masks and lidar_depth are whole frames.  Each loss runs in stages
+ * with a collective of the caller in between: kernels -> SUM of the partial buffers over the ranks -> kernels.  Every rank then holds
+ * the value of the whole frame, and the gradient rows of its band equal those of the single-GPU call bit for bit; the calls write only
+ * the band's rows of the gradients (the caller zeroes the rest).
+ *
+ * Halo: the photometric loss reads the image rows within 10 px of the band.  A rank sends, for each of its tile rows whose neighbour
+ * is owned by another rank, 10 rows to that owner: SEND_UP the first rows of the tile row (to the owner of the tile row above),
+ * SEND_DOWN its last rows (to the owner of the row below).  It receives RECV_UP, the 10 rows above (the SEND_DOWN of the rank above),
+ * and RECV_DOWN, the 10 rows below (the SEND_UP of the rank below); rows past H are dropped.  A buffer is [C][rows][W] fp32, rows =
+ * sgr_band_halo_rows(...) (-1 for a bad band or side).  An empty band sends and receives nothing. */
+#define SGR_HALO_SEND_UP 0
+#define SGR_HALO_SEND_DOWN 1
+#define SGR_HALO_RECV_UP 2
+#define SGR_HALO_RECV_DOWN 3
+int64_t sgr_band_halo_rows(int32_t H, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t side);
+int sgr_band_halo_pack(int32_t C, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t side, const float *image,
+                       float *buffer, void *stream);
+int sgr_band_halo_unpack(int32_t C, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t side,
+                         const float *buffer, float *image, void *stream);
+/* Photometric loss (sgr_image_loss) on a band, image holding the band's rows and its halo.  partials (device, 3 doubles): {sum of the SSIM
+ * map, sum of |image - gt| over the masked elements, number of masked pixels} over the band's pixels; stats zeroes and fills them, the
+ * caller sums them over the ranks, grad reads the sums.  scratch: sgr_image_loss_scratch_bytes(C, H, W), the same buffer in both calls.
+ * scalars: as sgr_image_loss's, of the whole frame. */
+int sgr_band_image_loss_stats(int32_t C, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *image,
+                              const float *gt, const uint8_t *mask, double *partials, void *scratch, size_t scratch_bytes, void *stream);
+int sgr_band_image_loss_grad(int32_t C, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *image,
+                             const float *gt, const uint8_t *mask, float w_l1, float w_ssim, const double *partials, float *dL_dimage,
+                             float *scalars, void *scratch, size_t scratch_bytes, void *stream);
+/* Sky and object-accumulation losses on a band: the band's dL_dacc rows (weight / (H W) times the derivative; or NULL) and
+ * partial[0] = the sum of the per-pixel losses over the band (device double, zeroed by the call).  After the caller's sum,
+ * sgr_band_acc_loss_value writes {weight * mean, mean} with mean = sum / N, N = H W. */
+int sgr_band_sky_loss(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *acc, const uint8_t *sky_mask,
+                      float weight, float *dL_dacc, double *partial, void *stream);
+int sgr_band_obj_acc_loss(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *acc, const uint8_t *obj_bound,
+                          float weight, float *dL_dacc, double *partial, void *stream);
+int sgr_band_acc_loss_value(int64_t N, float weight, const double *sum, float *scalars, void *stream);
+/* LiDAR depth loss on a band: the radix select of sgr_lidar_depth_loss with every histogram summed over the ranks.
+ *   keys                      the band's keys, n and the level-0 histogram into *state (zeroed first);  caller sums words
+ *                             [0, SGR_LIDAR_LEVEL0_WORDS) of *state: n, the select fields (still zero) and hist[0];
+ *   select level 1, 2         select on the summed level l - 1, the band's level-l histogram;  caller sums hist[l];
+ *   select level 3            select on the summed level 2 (k, t and the ties to take are now the same on every rank), then
+ *                             sums[0] = sum of the errors < t and sums[1 + r] = number of errors == t in tile row r, over the band
+ *                             (device doubles [1 + ceil(H / 16)], zeroed by the call);  caller sums `sums`;
+ *   grad                      the band's gradient rows (either may be NULL) and scalars {weight * mean, mean, n, k} of the frame.
+ * The ties taken are those of lowest flat index over the whole frame: a rank's come after the summed ties of the tile rows above.
+ * scratch: sgr_band_lidar_scratch_bytes(H, W), the same buffer in every stage.  H W < 2^31. */
+#define SGR_LIDAR_BINS 2048
+typedef struct SgrLidarState {
+	uint32_t n, k, prefix, rank; /* valid pixels; int(keep n); the selected digits, in the end t; rank of t among them, in the end the ties taken */
+	double sum_lt;               /* used by sgr_lidar_depth_loss only */
+	uint32_t hist[3][SGR_LIDAR_BINS];
+} SgrLidarState;
+#define SGR_LIDAR_LEVEL0_WORDS (6 + SGR_LIDAR_BINS)
+size_t sgr_band_lidar_scratch_bytes(int32_t H, int32_t W);
+int sgr_band_lidar_keys(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *depth, const float *acc,
+                        const float *lidar_depth, const uint8_t *mask, SgrLidarState *state, void *scratch, size_t scratch_bytes, void *stream);
+int sgr_band_lidar_select(int32_t level, double keep, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step,
+                          SgrLidarState *state, double *sums, void *scratch, size_t scratch_bytes, void *stream);
+int sgr_band_lidar_grad(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *depth, const float *acc,
+                        const float *lidar_depth, float weight, const SgrLidarState *state, const double *sums, float *dL_ddepth,
+                        float *dL_dacc, float *scalars, void *scratch, size_t scratch_bytes, void *stream);
+
 /* ---- Post-backward bookkeeping of a training iteration (SURVEY.md §8 row f3) ----
  * Densification statistics of StreetGaussianModel.set_max_radii2D + add_densification_stats
  * (lib/models/street_gaussian_model.py:551-571), all sub-models in one pass over the composed index space: for every Gaussian

@@ -27,7 +27,9 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_state_s
            "sgr_color_correct_backward", "sgr_color_correction_reg", "sgr_sky_composite_forward", "sgr_sky_composite_backward",
            "sgr_actor_pose_forward", "sgr_actor_pose_scratch_bytes", "sgr_actor_pose_backward", "sgr_gaussian_normals_forward",
            "sgr_gaussian_normals_backward", "sgr_compose_semantics_forward", "sgr_compose_semantics_backward", "sgr_finish_features_forward",
-           "sgr_finish_features_backward"]
+           "sgr_finish_features_backward", "sgr_band_halo_rows", "sgr_band_halo_pack", "sgr_band_halo_unpack", "sgr_band_image_loss_stats",
+           "sgr_band_image_loss_grad", "sgr_band_sky_loss", "sgr_band_obj_acc_loss", "sgr_band_acc_loss_value", "sgr_band_lidar_scratch_bytes",
+           "sgr_band_lidar_keys", "sgr_band_lidar_select", "sgr_band_lidar_grad"]
 
 SKY_MASK_ACC, SKY_MASK_GIVEN = 0, 1
 SEMANTIC_LOGITS, SEMANTIC_PROBABILITIES = 0, 1
@@ -106,6 +108,16 @@ class SgrLayer(C.Structure):
 
 class SgrLayerGrad(C.Structure):
     _fields_ = [("begin", C.c_int32), ("end", C.c_int32), ("grad2d", C.c_void_p), ("dL_dmeans2D", C.c_void_p)]
+
+
+HALO_SEND_UP, HALO_SEND_DOWN, HALO_RECV_UP, HALO_RECV_DOWN = 0, 1, 2, 3
+LIDAR_BINS = 2048
+LIDAR_LEVEL0_WORDS = 6 + LIDAR_BINS
+
+
+class SgrLidarState(C.Structure):
+    _fields_ = [("n", C.c_uint32), ("k", C.c_uint32), ("prefix", C.c_uint32), ("rank", C.c_uint32), ("sum_lt", C.c_double),
+                ("hist", (C.c_uint32 * LIDAR_BINS) * 3)]
 
 
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
@@ -222,6 +234,30 @@ def lib():
     L.sgr_lidar_depth_loss_scratch_bytes.argtypes = [C.c_int64]
     L.sgr_lidar_depth_loss.restype = C.c_int
     L.sgr_lidar_depth_loss.argtypes = [C.c_int64, vp, vp, vp, vp, C.c_double, C.c_float, vp, vp, vp, vp, C.c_size_t, vp]
+    band = [C.c_int32] * 3
+    L.sgr_band_halo_rows.restype = C.c_int64
+    L.sgr_band_halo_rows.argtypes = [C.c_int32] + band + [C.c_int32]
+    L.sgr_band_halo_pack.restype = C.c_int
+    L.sgr_band_halo_pack.argtypes = [C.c_int32] * 3 + band + [C.c_int32, vp, vp, vp]
+    L.sgr_band_halo_unpack.restype = C.c_int
+    L.sgr_band_halo_unpack.argtypes = [C.c_int32] * 3 + band + [C.c_int32, vp, vp, vp]
+    L.sgr_band_image_loss_stats.restype = C.c_int
+    L.sgr_band_image_loss_stats.argtypes = [C.c_int32] * 3 + band + [vp, vp, vp, vp, vp, C.c_size_t, vp]
+    L.sgr_band_image_loss_grad.restype = C.c_int
+    L.sgr_band_image_loss_grad.argtypes = [C.c_int32] * 3 + band + [vp, vp, vp, C.c_float, C.c_float, vp, vp, vp, vp, C.c_size_t, vp]
+    for name in ("sgr_band_sky_loss", "sgr_band_obj_acc_loss"):
+        getattr(L, name).restype = C.c_int
+        getattr(L, name).argtypes = [C.c_int32] * 2 + band + [vp, vp, C.c_float, vp, vp, vp]
+    L.sgr_band_acc_loss_value.restype = C.c_int
+    L.sgr_band_acc_loss_value.argtypes = [C.c_int64, C.c_float, vp, vp, vp]
+    L.sgr_band_lidar_scratch_bytes.restype = C.c_size_t
+    L.sgr_band_lidar_scratch_bytes.argtypes = [C.c_int32] * 2
+    L.sgr_band_lidar_keys.restype = C.c_int
+    L.sgr_band_lidar_keys.argtypes = [C.c_int32] * 2 + band + [vp] * 5 + [vp, C.c_size_t, vp]
+    L.sgr_band_lidar_select.restype = C.c_int
+    L.sgr_band_lidar_select.argtypes = [C.c_int32, C.c_double] + [C.c_int32] * 2 + band + [vp, vp, vp, C.c_size_t, vp]
+    L.sgr_band_lidar_grad.restype = C.c_int
+    L.sgr_band_lidar_grad.argtypes = [C.c_int32] * 2 + band + [vp] * 3 + [C.c_float] + [vp] * 5 + [vp, C.c_size_t, vp]
     L.sgr_densify_stats.restype = C.c_int
     L.sgr_densify_stats.argtypes = [C.POINTER(SgrStatSegment), C.c_int32, vp, vp, vp]
     L.sgr_adam_step.restype = C.c_int

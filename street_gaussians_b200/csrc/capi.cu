@@ -1128,6 +1128,165 @@ int sgr_lidar_depth_loss(int64_t N, const float *depth, const float *acc, const 
 	return SGR_OK;
 }
 
+// ---- the losses on a tile-row band ----
+static int loss_band(const char *fn, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, Band *band) {
+	if (H <= 0 || W <= 0 || (int64_t)H * W >= ((int64_t)1 << 31)) return fail(SGR_EINVAL, "%s: bad image size H=%d W=%d", fn, H, W);
+	const int rows = (H + 15) / 16;
+	if (row_step <= 0 || row_begin < 0 || row_end > rows || row_begin > row_end)
+		return fail(SGR_EINVAL, "%s: bad tile-row band [%d,%d) step %d for %d tile rows", fn, row_begin, row_end, row_step, rows);
+	*band = Band{row_begin, row_end, row_step};
+	return SGR_OK;
+}
+
+int64_t sgr_band_halo_rows(int32_t H, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t side) {
+	Band band;
+	if (loss_band("sgr_band_halo_rows", H, 1, row_begin, row_end, row_step, &band) != SGR_OK) return -1;
+	if (side < SGR_HALO_SEND_UP || side > SGR_HALO_RECV_DOWN) return -1;
+	return halo_rows(H, halo_strips(H, band, side));
+}
+
+static int halo_copy(const char *fn, bool pack, int32_t C, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t side,
+                     float *image, float *buffer, void *stream) {
+	Band band;
+	if (int rc = loss_band(fn, H, W, row_begin, row_end, row_step, &band)) return rc;
+	if (C <= 0) return fail(SGR_EINVAL, "%s: bad channel count %d", fn, C);
+	const bool ok = pack ? (side == SGR_HALO_SEND_UP || side == SGR_HALO_SEND_DOWN) : (side == SGR_HALO_RECV_UP || side == SGR_HALO_RECV_DOWN);
+	if (!ok) return fail(SGR_EINVAL, "%s: side %d is not a %s side", fn, side, pack ? "send" : "receive");
+	if (halo_rows(H, halo_strips(H, band, side)) > 0 && (!image || !buffer)) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_halo_copy(pack, C, H, W, band, side, image, buffer, st), fn);
+	return SGR_OK;
+}
+
+int sgr_band_halo_pack(int32_t C, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t side, const float *image,
+                       float *buffer, void *stream) {
+	return halo_copy("sgr_band_halo_pack", true, C, H, W, row_begin, row_end, row_step, side, const_cast<float *>(image), buffer, stream);
+}
+
+int sgr_band_halo_unpack(int32_t C, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t side,
+                         const float *buffer, float *image, void *stream) {
+	return halo_copy("sgr_band_halo_unpack", false, C, H, W, row_begin, row_end, row_step, side, image, const_cast<float *>(buffer), stream);
+}
+
+static int band_image_loss_check(const char *fn, int32_t C, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step,
+                                 const float *image, const float *gt, const double *partials, void *scratch, size_t scratch_bytes, Band *band) {
+	if (int rc = loss_band(fn, H, W, row_begin, row_end, row_step, band)) return rc;
+	if (C <= 0) return fail(SGR_EINVAL, "%s: bad channel count %d", fn, C);
+	if (!image || !gt || !partials) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	if (!scratch || scratch_bytes < image_loss_scratch_bytes(C, H, W))
+		return fail(SGR_ENOMEM, "%s: scratch too small: %zu < %zu", fn, scratch_bytes, image_loss_scratch_bytes(C, H, W));
+	return SGR_OK;
+}
+
+int sgr_band_image_loss_stats(int32_t C, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *image,
+                              const float *gt, const uint8_t *mask, double *partials, void *scratch, size_t scratch_bytes, void *stream) {
+	Band band;
+	if (int rc = band_image_loss_check("sgr_band_image_loss_stats", C, H, W, row_begin, row_end, row_step, image, gt, partials, scratch, scratch_bytes,
+	                                   &band))
+		return rc;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_image_loss_stats(C, H, W, band, image, gt, mask, partials, scratch, st), "band_image_loss_stats");
+	return SGR_OK;
+}
+
+int sgr_band_image_loss_grad(int32_t C, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *image,
+                             const float *gt, const uint8_t *mask, float w_l1, float w_ssim, const double *partials, float *dL_dimage,
+                             float *scalars, void *scratch, size_t scratch_bytes, void *stream) {
+	Band band;
+	if (int rc = band_image_loss_check("sgr_band_image_loss_grad", C, H, W, row_begin, row_end, row_step, image, gt, partials, scratch, scratch_bytes,
+	                                   &band))
+		return rc;
+	if (!scalars) return fail(SGR_EINVAL, "NULL pointer passed to sgr_band_image_loss_grad");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_image_loss_grad(C, H, W, band, image, gt, mask, partials, w_l1, w_ssim, dL_dimage, scalars, scratch, st), "band_image_loss_grad");
+	return SGR_OK;
+}
+
+static int band_acc_loss(const char *fn, int form, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *acc,
+                         const uint8_t *flag, float weight, float *dL_dacc, double *partial, void *stream) {
+	Band band;
+	if (int rc = loss_band(fn, H, W, row_begin, row_end, row_step, &band)) return rc;
+	if (!acc || !flag || !partial) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_acc_loss_band(form, H, W, band, acc, flag, weight, dL_dacc, partial, st), fn);
+	return SGR_OK;
+}
+
+int sgr_band_sky_loss(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *acc, const uint8_t *sky_mask,
+                      float weight, float *dL_dacc, double *partial, void *stream) {
+	return band_acc_loss("sgr_band_sky_loss", 0, H, W, row_begin, row_end, row_step, acc, sky_mask, weight, dL_dacc, partial, stream);
+}
+
+int sgr_band_obj_acc_loss(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *acc, const uint8_t *obj_bound,
+                          float weight, float *dL_dacc, double *partial, void *stream) {
+	return band_acc_loss("sgr_band_obj_acc_loss", 1, H, W, row_begin, row_end, row_step, acc, obj_bound, weight, dL_dacc, partial, stream);
+}
+
+int sgr_band_acc_loss_value(int64_t N, float weight, const double *sum, float *scalars, void *stream) {
+	if (N <= 0) return fail(SGR_EINVAL, "N must be positive");
+	if (!sum || !scalars) return fail(SGR_EINVAL, "NULL pointer passed to sgr_band_acc_loss_value");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_acc_loss_value((size_t)N, weight, sum, scalars, st), "band_acc_loss_value");
+	return SGR_OK;
+}
+
+size_t sgr_band_lidar_scratch_bytes(int32_t H, int32_t W) {
+	return (H > 0 && W > 0 && (int64_t)H * W < ((int64_t)1 << 31)) ? lidar_band_scratch_bytes(H, W) : 0;
+}
+
+static int band_lidar_check(const char *fn, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const void *state,
+                            void *scratch, size_t scratch_bytes, Band *band) {
+	if (int rc = loss_band(fn, H, W, row_begin, row_end, row_step, band)) return rc;
+	if (!state) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	if (!scratch || scratch_bytes < lidar_band_scratch_bytes(H, W))
+		return fail(SGR_ENOMEM, "%s: scratch too small: %zu < %zu", fn, scratch_bytes, lidar_band_scratch_bytes(H, W));
+	return SGR_OK;
+}
+
+int sgr_band_lidar_keys(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *depth, const float *acc,
+                        const float *lidar_depth, const uint8_t *mask, SgrLidarState *state, void *scratch, size_t scratch_bytes, void *stream) {
+	const char *fn = "sgr_band_lidar_keys";
+	Band band;
+	if (int rc = band_lidar_check(fn, H, W, row_begin, row_end, row_step, state, scratch, scratch_bytes, &band)) return rc;
+	if (!depth || !acc || !lidar_depth) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_lidar_band_keys(H, W, band, depth, acc, lidar_depth, mask, state, scratch, st), fn);
+	return SGR_OK;
+}
+
+int sgr_band_lidar_select(int32_t level, double keep, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step,
+                          SgrLidarState *state, double *sums, void *scratch, size_t scratch_bytes, void *stream) {
+	const char *fn = "sgr_band_lidar_select";
+	Band band;
+	if (int rc = band_lidar_check(fn, H, W, row_begin, row_end, row_step, state, scratch, scratch_bytes, &band)) return rc;
+	if (level < 1 || level > 3) return fail(SGR_EINVAL, "%s: level must be 1, 2 or 3, got %d", fn, level);
+	if (!(keep > 0.0 && keep <= 1.0)) return fail(SGR_EINVAL, "keep must be in (0, 1], got %g", keep);
+	if (level == 3 && !sums) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_lidar_band_select(level, keep, H, W, band, state, sums, scratch, st), fn);
+	return SGR_OK;
+}
+
+int sgr_band_lidar_grad(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *depth, const float *acc,
+                        const float *lidar_depth, float weight, const SgrLidarState *state, const double *sums, float *dL_ddepth,
+                        float *dL_dacc, float *scalars, void *scratch, size_t scratch_bytes, void *stream) {
+	const char *fn = "sgr_band_lidar_grad";
+	Band band;
+	if (int rc = band_lidar_check(fn, H, W, row_begin, row_end, row_step, state, scratch, scratch_bytes, &band)) return rc;
+	if (!depth || !acc || !lidar_depth || !sums || !scalars) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_lidar_band_grad(H, W, band, depth, acc, lidar_depth, weight, state, sums, dL_ddepth, dL_dacc, scalars, scratch, st), fn);
+	return SGR_OK;
+}
+
 int sgr_densify_stats(const SgrStatSegment *segments, int32_t num_segments, const int32_t *radii, const float *means2D_grad, void *stream) {
 	if (!segments || num_segments <= 0) return fail(SGR_EINVAL, "segment table is empty");
 	int64_t at = 0;

@@ -416,6 +416,28 @@ cudaError_t launch_obj_acc_loss(size_t N, const float *accm, const uint8_t *obj_
 size_t lidar_depth_loss_scratch_bytes(size_t N);
 cudaError_t launch_lidar_depth_loss(size_t N, const float *depth, const float *acc, const float *lidar, const uint8_t *mask, double keep, float weight,
                                     float *dL_ddepth, float *dL_dacc, float *scalars, void *scratch, cudaStream_t st);
+// the losses on a tile-row band (losses.cu)
+constexpr int kBandHalo = 10;  // image rows past a band's edge the photometric loss reads: 5 for the SSIM window, 5 for its derivative maps
+struct HaloStrips {
+	int first, count, step, offset;
+};
+HaloStrips halo_strips(int H, Band band, int side);
+int64_t halo_rows(int H, const HaloStrips &h);
+cudaError_t launch_halo_copy(bool pack, int C, int H, int W, Band band, int side, float *image, float *buf, cudaStream_t st);
+cudaError_t launch_image_loss_stats(int C, int H, int W, Band band, const float *img, const float *gt, const uint8_t *mask, double *acc,
+                                    void *scratch, cudaStream_t st);
+cudaError_t launch_image_loss_grad(int C, int H, int W, Band band, const float *img, const float *gt, const uint8_t *mask, const double *acc,
+                                   float w_l1, float w_ssim, float *grad, float *scalars, void *scratch, cudaStream_t st);
+cudaError_t launch_acc_loss_band(int form, int H, int W, Band band, const float *accm, const uint8_t *flag, float weight, float *grad, double *sum,
+                                 cudaStream_t st);
+cudaError_t launch_acc_loss_value(size_t N, float weight, const double *sum, float *scalars, cudaStream_t st);
+size_t lidar_band_scratch_bytes(int H, int W);
+cudaError_t launch_lidar_band_keys(int H, int W, Band band, const float *depth, const float *acc, const float *lidar, const uint8_t *mask,
+                                   SgrLidarState *s, void *scratch, cudaStream_t st);
+cudaError_t launch_lidar_band_select(int level, double keep, int H, int W, Band band, SgrLidarState *s, double *sums, void *scratch, cudaStream_t st);
+cudaError_t launch_lidar_band_grad(int H, int W, Band band, const float *depth, const float *acc, const float *lidar, float weight,
+                                   const SgrLidarState *s, const double *sums, float *dL_ddepth, float *dL_dacc, float *scalars, void *scratch,
+                                   cudaStream_t st);
 cudaError_t launch_densify_stats(const SgrStatSegment *segs, int nseg, const int32_t *radii, const float *grad2d, cudaStream_t st);
 cudaError_t launch_adam(const SgrAdamTensor *ts, int n_tensors, double beta1, double beta2, double eps, cudaStream_t st);
 cudaError_t launch_sparse_adam(const SgrSparseAdamSegment *segs, int nseg, const int32_t *radii, double beta1, double beta2, double eps,

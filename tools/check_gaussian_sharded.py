@@ -101,6 +101,50 @@ def run_case(rank, world, dev, S, P, W, H, bounded, exchange="nccl"):
     return worst, floor
 
 
+def run_losses(rank, world, dev, W=1280, H=720):
+    """Loss leg: each rank's band losses (band_losses.py) on its banded render against the single-GPU losses of the gathered frame."""
+    from street_gaussians_b200 import band_losses, losses
+    scene = synthetic.make_scene(P=60_001, width=W, height=H, sh_degree=3, seed=78, pose=True)
+    st = util.settings_from(sgb, scene["cam"], dev)
+    rast = GaussianShardedRasterizer(st)
+    P = scene["means3D"].shape[0]
+    chunk = (P + world - 1) // world
+    lo, hi = min(P, rank * chunk), min(P, (rank + 1) * chunk)
+    with torch.no_grad():
+        got = rast(means3D=scene["means3D"][lo:hi].to(dev), means2D=None, opacities=scene["opacities"][lo:hi].to(dev),
+                   shs=scene["shs"][lo:hi].to(dev), scales=scene["scales"][lo:hi].to(dev), rotations=scene["rotations"][lo:hi].to(dev))
+    color, depth, acc = got[0], got[2], got[3]
+    full = [t.clone() for t in (color, depth, acc)]
+    for t in full:
+        if world > 1:
+            dist.all_reduce(t)
+    g = torch.Generator(device=dev).manual_seed(5)  # the data inputs are the same whole frames on every rank
+    gt = torch.rand(3, H, W, device=dev, generator=g)
+    mask = torch.rand(1, H, W, device=dev, generator=g) > 0.1
+    sky = torch.rand(1, H, W, device=dev, generator=g) > 0.5
+    lidar = full[1] * (1 + 0.05 * torch.randn(1, H, W, device=dev, generator=g)) * (torch.rand(1, H, W, device=dev, generator=g) > 0.5)
+    rows = band_of_rows(H, rank, world).to(dev)
+    band = rast.band if rast.band is not None else sgb.TileRowBand(0, (H + 15) // 16, 1)
+
+    def grads(fn, *xs):
+        xs = [x.detach().clone().requires_grad_(True) for x in xs]
+        v = fn(*xs)
+        v.backward()
+        return v.detach(), [x.grad for x in xs]
+
+    checks = (("photometric", lambda x, b=None, gr=None: losses.photometric_loss(x, gt, mask, band=b, group=gr), (0,)),
+              ("sky", lambda a, b=None, gr=None: losses.sky_loss(a, sky, band=b, group=gr), (2,)),
+              ("lidar", lambda d, a, b=None, gr=None: losses.lidar_depth_loss(d, a, lidar, mask, band=b, group=gr), (1, 2)))
+    for name, fn, which in checks:
+        v_ref, g_ref = grads(fn, *(full[i] for i in which))
+        v, g_band = grads(lambda *xs: fn(*xs, b=band, gr=None), *((color, depth, acc)[i] for i in which))
+        a, b = float(v), float(v_ref)
+        assert (a != a and b != b) or abs(a - b) <= 4e-6 * abs(b), (name, a, b)
+        for x, y in zip(g_band, g_ref):
+            assert torch.equal(x[:, rows].contiguous().view(torch.int32), y[:, rows].contiguous().view(torch.int32)), f"{name}: gradient rows differ"
+            assert not bool(x[:, ~rows].any()), f"{name}: foreign gradient rows not zero"
+
+
 def main():
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -115,6 +159,8 @@ def main():
             worst, floor = run_case(rank, world, dev, S, P, W, H, bounded, exchange)
             print(f"[rank {rank}/{world}] exchange={exchange} S={S} P={P} {W}x{H} bounded={bounded}: images bit-equal, worst grad rel err {worst:.2e} "
                   f"(single-GPU run-to-run floor {floor:.2e})", flush=True)
+        run_losses(rank, world, dev)
+        print(f"[rank {rank}/{world}] band losses: the frame's values, gradient rows bit-equal to the single-GPU losses", flush=True)
     except AssertionError as e:
         ok = False
         print(f"[rank {rank}] FAILED: {e!r}", flush=True)
