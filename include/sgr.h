@@ -210,17 +210,23 @@ int sgr_backward_geom_layered(const SgrFrame *frame, const float *means3D, const
  * "variant A": every rank owns P/N Gaussians AND a tile-row band) --------------------------------------------------
  * The forward of DGR/cuda_rasterizer/rasterizer_impl.cu:197-343 is split at the point where the per-Gaussian work
  * (FORWARD::preprocess, forward.cu:155-256) hands fixed-size screen-space records to the per-tile work:
- *   1. sgr_project          on the rank's own Gaussians -> records[P_local] (sgr_record_bytes() each) + radii[P_local]
- *   2. caller all-gathers records and radii (NCCL) into the first P_total*sgr_record_bytes() bytes of a geom_state
+ *   1. sgr_project          on the rank's own Gaussians -> a geom_state for P_local (sgr_state_sizes bytes, NOT P_local *
+ *                           sgr_record_bytes()): records[P_local] at its head, the colour Jacobian further in + radii[P_local]
+ *   2. caller all-gathers the records (the first P_local*sgr_record_bytes() bytes of that state, padded to chunk) and radii
+ *      (NCCL) into the first P_total*sgr_record_bytes() bytes of a geom_state
  *      sized for P_total, and a radii[P_total] array; padding slots must carry radii == 0
  *   3. sgr_forward_records  bins / sorts / blends the rank's tile-row band from the gathered records
  *   4. sgr_backward_blend   (frame.P = P_total) -> partial grad2d[P_total,12]; caller reduce-scatters it
- *   5. sgr_backward_geom    with frame.P = P_local, geom_state = the rank's own records, grad2d = its reduced slice.
+ *   5. sgr_backward_geom    with frame.P = P_local, geom_state = the state step 1 wrote, unchanged (it reads the colour Jacobian
+ *                           there), grad2d = its reduced slice.
  * Results are bit-identical to the single-GPU path for the forward images and agree to float summation order in the
  * gradients (tests/test_parity_gpu.py::test_gaussian_sharded_*). */
 size_t sgr_record_bytes(void);
 /* Step 1.  frame.P = number of local Gaussians; the tile-row band of `frame` is ignored.  Same input rules as
- * sgr_forward.  Writes records[P] (only slots with radii > 0 are meaningful) and radii[P] (all). */
+ * sgr_forward.  `records` must be a geom state for frame.P: at least the geom_bytes sgr_state_sizes reports for this frame.  The
+ * call writes records[P] at its head (only slots with radii > 0 are meaningful), and with shs the SH colour's direction Jacobian
+ * (48 B per visible Gaussian) BEYOND the first P*sgr_record_bytes() bytes, where sgr_backward_geom (step 5) reads it; and
+ * radii[P] (all).  A buffer of only P*sgr_record_bytes() bytes is too small. */
 int sgr_project(const SgrFrame *frame, const float *means3D, const float *shs, const float *colors_precomp,
                 const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
                 int32_t *radii, void *records, void *stream);

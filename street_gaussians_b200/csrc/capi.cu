@@ -56,6 +56,7 @@ GeomView carve_geom(void *base, int P) {
 	g.offsets = take<uint32_t>(p, n);
 	g.big_list = take<uint32_t>(p, n);
 	g.big_count = take<uint32_t>(p, 64);
+	g.jac = take<float4>(p, 3 * n);
 	g.ckey = take<uint32_t>(p, n);
 	g.cval = take<uint32_t>(p, n);
 	g.temp_bytes = memo_bytes((int64_t)P, [](int64_t n) { return geom_temp_bytes((int)n); });
@@ -326,8 +327,9 @@ int sgr_project(const SgrFrame *frame, const float *means3D, const float *shs, c
 	if (!f.view || !f.proj || !f.campos) return fail(SGR_EINVAL, "camera pointer (viewmatrix/projmatrix/campos) is NULL");
 	if (!means3D || !opacities || !radii || !records) return fail(SGR_EINVAL, "means3D / opacities / radii / records is NULL");
 	if ((rc = check_gaussian_inputs(f, shs, colors_precomp, scales, rotations, cov3D_precomp)) != SGR_OK) return rc;
-	SGR_TRY(launch_project(f, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, radii,
-	                       reinterpret_cast<GaussRec *>(records), st),
+	// `records` is the head of a geom state for frame.P: the records go there, the colour Jacobian that sgr_backward_geom reads after them
+	const GeomView g = carve_geom(records, f.P);
+	SGR_TRY(launch_project(f, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, radii, g.rec, g.jac, st),
 	        "project");
 	return SGR_OK;
 }
@@ -452,7 +454,7 @@ int sgr_sharded_forward(const SgrFrame *frame, const SgrPeers *peers, const floa
 	// (g.depth_key of this rank = the destination masks of its own Gaussians, kept for the backward; g.iota of rank d = the run-length
 	// table the owners fill — same offset inside every rank's geom state)
 	SGR_TRY(launch_project_scatter(fl, pt, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, radii_local,
-	                               reinterpret_cast<GaussRec *>(records_local), g.depth_key,
+	                               reinterpret_cast<GaussRec *>(records_local), g.jac, g.depth_key,
 	                               (size_t)(reinterpret_cast<char *>(g.iota) - reinterpret_cast<char *>(geom_state)), st),
 	        "project+scatter");
 	if (ft.P == 0) return SGR_OK;
@@ -492,7 +494,7 @@ int sgr_sharded_backward(const SgrFrame *frame, const SgrPeers *peers, int64_t c
 		SGR_TRY(launch_blend_bwd(ft, g, b, img, nullptr, out_alpha, dL_dcolor, dL_ddepth, dL_dalpha, nullptr, grad2d, nullptr, st, true), "blend_bwd");
 	SGR_TRY(launch_peer_barrier(pt, barrier_epoch, ft.P > 0 ? g.big_count : nullptr, st), "barrier");
 	SGR_TRY(launch_preprocess_bwd(fl, &pt, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii_local,
-	                              reinterpret_cast<const GaussRec *>(records_local), reinterpret_cast<const float *>(g.depth_key), dL_dmeans3D,
+	                              g.jac, reinterpret_cast<const float *>(g.depth_key), dL_dmeans3D,
 	                              dL_dmeans2D, shs ? dL_dsh : nullptr, dL_dcolors_precomp, dL_dopacity, cov3D_precomp ? nullptr : dL_dscales,
 	                              cov3D_precomp ? nullptr : dL_drotations, dL_dcov3D, st),
 	        "preprocess_bwd+gather");
@@ -578,7 +580,7 @@ static int backward_geom(const char *fn, const SgrFrame *frame, const float *mea
 		SGR_TRY(launch_layer_stash(grad2d, lo, hi, scratch, false, nullptr, st), "layer stash");
 		SGR_TRY(launch_layer_merge(grad2d, layers, num_layers, st), "layer merge");
 	}
-	SGR_TRY(launch_preprocess_bwd(f, nullptr, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii, g.rec, grad2d, dL_dmeans3D,
+	SGR_TRY(launch_preprocess_bwd(f, nullptr, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii, g.jac, grad2d, dL_dmeans3D,
 	                              dL_dmeans2D, shs ? dL_dsh : nullptr, dL_dcolors_precomp, dL_dopacity,
 	                              cov3D_precomp ? nullptr : dL_dscales, cov3D_precomp ? nullptr : dL_drotations, dL_dcov3D, st),
 	        "preprocess_bwd");

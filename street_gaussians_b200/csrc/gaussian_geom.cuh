@@ -18,6 +18,89 @@ static __device__ __constant__ float kC2[5] = {1.0925484305920792f, -1.092548430
 static __device__ __constant__ float kC3[7] = {-0.5900435899266435f, 2.890611442640554f, -0.4570457994644658f, 0.3731763325901154f,
                                                -0.4570457994644658f, 1.445305721320277f, -0.5900435899266435f};
 
+// Real SH basis B_k of the unit view direction (x, y, z) for k < (deg + 1)^2, 0 beyond (reference forward.cu:20-71).
+__device__ __forceinline__ void sh_basis(int deg, float x, float y, float z, float (&B)[16]) {
+#pragma unroll
+	for (int k = 0; k < 16; k++) B[k] = 0.f;
+	B[0] = kC0;
+	if (deg > 0) {
+		B[1] = -kC1 * y; B[2] = kC1 * z; B[3] = -kC1 * x;
+		if (deg > 1) {
+			const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
+			B[4] = kC2[0] * xy; B[5] = kC2[1] * yz; B[6] = kC2[2] * (2.f * zz - xx - yy); B[7] = kC2[3] * xz; B[8] = kC2[4] * (xx - yy);
+			if (deg > 2) {
+				B[9] = kC3[0] * y * (3.f * xx - yy); B[10] = kC3[1] * xy * z; B[11] = kC3[2] * y * (4.f * zz - xx - yy);
+				B[12] = kC3[3] * z * (2.f * zz - 3.f * xx - 3.f * yy); B[13] = kC3[4] * x * (4.f * zz - xx - yy); B[14] = kC3[5] * z * (xx - yy);
+				B[15] = kC3[6] * x * (xx - 3.f * yy);
+			}
+		}
+	}
+}
+
+// Colour Jacobian of one coefficient row c (coefficient-major, RGB innermost) at the unit direction: J[3 a + ch] = d colour_ch /
+// d dir_a for a = x, y, z — the reference's per-channel dRGBdx / dRGBdy / dRGBdz sums (backward.cu:20-139).  It does not depend on
+// the upstream gradient, so the forward evaluates it while it holds the row, and the backward never reads the coefficients.
+__device__ __forceinline__ void sh_color_jacobian(int deg, float x, float y, float z, const float *c, float (&J)[9]) {
+#pragma unroll
+	for (int ch = 0; ch < 3; ch++) {
+#define SHC(k) c[(k) * 3 + ch]
+		float dx = 0.f, dy = 0.f, dz = 0.f;
+		if (deg > 0) {
+			dx = -kC1 * SHC(3); dy = -kC1 * SHC(1); dz = kC1 * SHC(2);
+			if (deg > 1) {
+				const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
+				dx += kC2[0] * y * SHC(4) + kC2[2] * 2.f * -x * SHC(6) + kC2[3] * z * SHC(7) + kC2[4] * 2.f * x * SHC(8);
+				dy += kC2[0] * x * SHC(4) + kC2[1] * z * SHC(5) + kC2[2] * 2.f * -y * SHC(6) + kC2[4] * 2.f * -y * SHC(8);
+				dz += kC2[1] * y * SHC(5) + kC2[2] * 2.f * 2.f * z * SHC(6) + kC2[3] * x * SHC(7);
+				if (deg > 2) {
+					dx += (kC3[0] * SHC(9) * 3.f * 2.f * xy + kC3[1] * SHC(10) * yz + kC3[2] * SHC(11) * -2.f * xy +
+					       kC3[3] * SHC(12) * -3.f * 2.f * xz + kC3[4] * SHC(13) * (-3.f * xx + 4.f * zz - yy) +
+					       kC3[5] * SHC(14) * 2.f * xz + kC3[6] * SHC(15) * 3.f * (xx - yy));
+					dy += (kC3[0] * SHC(9) * 3.f * (xx - yy) + kC3[1] * SHC(10) * xz + kC3[2] * SHC(11) * (-3.f * yy + 4.f * zz - xx) +
+					       kC3[3] * SHC(12) * -3.f * 2.f * yz + kC3[4] * SHC(13) * -2.f * xy + kC3[5] * SHC(14) * -2.f * yz +
+					       kC3[6] * SHC(15) * -3.f * 2.f * xy);
+					dz += (kC3[1] * SHC(10) * xy + kC3[2] * SHC(11) * 4.f * 2.f * yz + kC3[3] * SHC(12) * 3.f * (2.f * zz - xx - yy) +
+					       kC3[4] * SHC(13) * 4.f * 2.f * xz + kC3[5] * SHC(14) * (xx - yy));
+				}
+			}
+		}
+#undef SHC
+		J[ch] = dx; J[3 + ch] = dy; J[6 + ch] = dz;
+	}
+}
+
+// The colour Jacobian as the forward stores it, three float4 per Gaussian: {J0 J1 J2 J3} {J4 J5 J6 J7} {J8, clamp bits, 0, 0}.
+// The clamp bits (bit ch: colour channel ch was clamped at 0, so no gradient flows through it) travel with it, so the backward reads
+// nothing of the 48-B blend record.
+__device__ __forceinline__ void store_color_jac(float4 *dst, const float (&J)[9], uint32_t clamp_bits) {
+	dst[0] = make_float4(J[0], J[1], J[2], J[3]);
+	dst[1] = make_float4(J[4], J[5], J[6], J[7]);
+	dst[2] = make_float4(J[8], __uint_as_float(clamp_bits), 0.f, 0.f);
+}
+struct ColorJac {
+	float4 a, b, c;
+};
+__device__ __forceinline__ ColorJac load_color_jac(const float4 *__restrict__ src) {
+	return ColorJac{__ldg(src), __ldg(src + 1), __ldg(src + 2)};
+}
+// dL/dRGB with the clamped channels zeroed
+__device__ __forceinline__ void masked_drgb(const ColorJac &cj, float r, float g, float b, float (&dRGB)[3]) {
+	const uint32_t clamp_bits = __float_as_uint(cj.c.y);
+	dRGB[0] = (clamp_bits & 1u) ? 0.f : r;
+	dRGB[1] = (clamp_bits & 2u) ? 0.f : g;
+	dRGB[2] = (clamp_bits & 4u) ? 0.f : b;
+}
+// dL/d(unit direction) = J^T dL/dRGB, summed over the channels in the reference's order
+__device__ __forceinline__ float3 color_jac_dir_grad(const ColorJac &cj, const float (&dRGB)[3]) {
+	const float J[9] = {cj.a.x, cj.a.y, cj.a.z, cj.a.w, cj.b.x, cj.b.y, cj.b.z, cj.b.w, cj.c.x};
+	float3 d = make_float3(0.f, 0.f, 0.f);
+#pragma unroll
+	for (int ch = 0; ch < 3; ch++) {
+		d.x += J[ch] * dRGB[ch]; d.y += J[3 + ch] * dRGB[ch]; d.z += J[6 + ch] * dRGB[ch];
+	}
+	return d;
+}
+
 // The per-Gaussian shape inputs.  The forward loads them at the TOP of its kernel together with the position and the opacity: the
 // round-1 kernel loaded them where they were used (after the near cull, inside the projection), which serialised three DRAM round
 // trips per thread (the profiler's source view put most long-scoreboard stalls on exactly these loads).

@@ -8,13 +8,16 @@
 //     reference's 304 B/Gaussian of torch::zeros (rasterize_points.cu:166-176) disappears;
 //   * dL/dmean3D is accumulated in registers across the three contributions and stored once (the reference does
 //     one store + two read-modify-writes + one more inside the SH routine).
-//   * SH coefficients in / SH gradients out are staged through shared memory per warp: the 32 Gaussians of a warp own
-//     one contiguous 32 x M x 3 float block of `shs` / `dL_dsh`, which the warp moves with fully coalesced 16-B accesses
-//     (rows padded to 49 floats in smem so the per-thread row walks are bank-conflict free).  The direct per-thread
-//     version (48 strided scalar loads + 48 strided scalar stores per Gaussian) wastes most of each memory transaction.
+//   * the SH coefficients are NOT read: dL/dsh = B_k(dir) dL/dRGB needs only the view direction, and dL/ddir = J^T dL/dRGB takes
+//     the colour Jacobian J (3 x 3, with the clamp bits) that the forward stored while it held the coefficient row — 48 B per
+//     visible Gaussian instead of the 12 M-byte row plus a sector of the blend record;
+//   * SH gradients out are staged through shared memory per warp: the 32 Gaussians of a warp own one contiguous 32 x M x 3
+//     float block of `dL_dsh`, which leaves with fully coalesced 16-B stores (rows padded to 49 floats in smem so the per-thread
+//     row writes are bank-conflict free).  Direct per-thread stores (48 strided scalar stores per Gaussian) waste most of each
+//     memory transaction.
 // Formulas and evaluation order follow the reference so gradients agree to fp32 rounding.  The geometry (covariances, EWA
-// Jacobian, projective divide, depth, scale / rotation) is gaussian_geom.cuh's, the same functions the forward calls; the two
-// kernels below differ in how they load their inputs, the gather, their SH backward loop and their stores.
+// Jacobian, projective divide, depth, scale / rotation) and the SH basis and colour Jacobian are gaussian_geom.cuh's, the same
+// functions the forward calls; the two kernels below differ in how they load their inputs, the gather and their stores.
 #include <cstdlib>
 
 #include "gaussian_geom.cuh"
@@ -83,7 +86,7 @@ template <bool STAGED, bool GATHER = false>
 __global__ void __launch_bounds__(256) preprocess_bwd_kernel(
     const FrameDev f, const PeerTable pt, const float *__restrict__ means3D, const float *__restrict__ shs, const float *__restrict__ colors_precomp,
     const float *__restrict__ scales, const float *__restrict__ rotations, const float *__restrict__ cov3D_precomp,
-    const int32_t *__restrict__ radii, const GaussRec *__restrict__ rec, const float *__restrict__ grad2d,
+    const int32_t *__restrict__ radii, const float4 *__restrict__ jac, const float *__restrict__ grad2d,
     float *__restrict__ dL_dmeans3D, float *__restrict__ dL_dmeans2D, float *__restrict__ dL_dsh, float *__restrict__ dL_dcolors,
     float *__restrict__ dL_dopacity, float *__restrict__ dL_dscales, float *__restrict__ dL_drot, float *__restrict__ dL_dcov3D) {
 	extern __shared__ float s_sh[];  // [warps][32][kShRow] when STAGED
@@ -94,33 +97,6 @@ __global__ void __launch_bounds__(256) preprocess_bwd_kernel(
 	const int nsh = f.M * 3;
 	const bool visible = in_range && radii[idx] > 0;
 	float *srow = STAGED ? (s_sh + ((size_t)warp * 32 + lane) * kShRow) : nullptr;
-
-	if (STAGED && shs != nullptr) {
-		// coalesced stage-in of this warp's 32 x nsh block (visible rows only)
-		const unsigned vis_mask = __ballot_sync(0xffffffffu, visible);
-		const size_t g0 = (size_t)(blockIdx.x * blockDim.x + warp * 32);
-		const int rows = (int)min((size_t)32, g0 < (size_t)f.P ? (size_t)f.P - g0 : (size_t)0);
-		float *wbase = s_sh + (size_t)warp * 32 * kShRow;
-		if ((nsh & 3) == 0) {
-			const float4 *src = reinterpret_cast<const float4 *>(shs + g0 * nsh);
-			const int n4 = rows * nsh / 4;
-			for (int e = lane; e < n4; e += 32) {
-				const int row = (4 * e) / nsh, col = (4 * e) - row * nsh;
-				if ((vis_mask >> row) & 1u) {
-					const float4 v = __ldg(src + e);
-					float *d = wbase + row * kShRow + col;
-					d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
-				}
-			}
-		} else {
-			const float *src = shs + g0 * nsh;
-			for (int e = lane; e < rows * nsh; e += 32) {
-				const int row = e / nsh, col = e - row * nsh;
-				if ((vis_mask >> row) & 1u) wbase[row * kShRow + col] = __ldg(src + e);
-			}
-		}
-		__syncwarp();
-	}
 
 	float4 g0v = make_float4(0.f, 0.f, 0.f, 0.f), g1v = g0v, g2v = g0v;
 	if (GATHER) {  // (`grad2d` carries the destination masks the forward stored)
@@ -181,66 +157,25 @@ __global__ void __launch_bounds__(256) preprocess_bwd_kernel(
 	add_to(dmean, mean2d_bwd(mean, proj, g0.x, g0.y));
 	add_to(dmean, depth_bwd(mean, view, g2.z));
 
-	// ---- SH backward (reference backward.cu:20-139) ----
+	// ---- SH backward (reference backward.cu:20-139) from the direction basis and the forward's colour Jacobian ----
 	if (shs != nullptr) {
-		const float *sh = STAGED ? srow : shs + i * nsh;
 		float *dsh = STAGED ? srow : dL_dsh + i * nsh;
-		const uint32_t clamp_bits = __float_as_uint(rec[idx].q2.w) & 7u;  // (the fused forward keeps the radius in the upper bits)
+		const ColorJac cj = load_color_jac(jac + 3 * i);
 		const float3 campos = make_float3(f.campos[0], f.campos[1], f.campos[2]);
 		const float3 dir_orig = make_float3(mean.x - campos.x, mean.y - campos.y, mean.z - campos.z);
 		const float len = sqrtf(dir_orig.x * dir_orig.x + dir_orig.y * dir_orig.y + dir_orig.z * dir_orig.z);
 		const float x = dir_orig.x / len, y = dir_orig.y / len, z = dir_orig.z / len;
-		float dRGB[3] = {g1.w, g2.x, g2.y};
-		dRGB[0] *= (clamp_bits & 1u) ? 0 : 1;
-		dRGB[1] *= (clamp_bits & 2u) ? 0 : 1;
-		dRGB[2] *= (clamp_bits & 4u) ? 0 : 1;
-		const int deg = f.D;
-		const int ncoef = min(f.M, (deg + 1) * (deg + 1));
-		float ddir[3] = {0.f, 0.f, 0.f};
-		// coefficients beyond the active degree receive zero gradient
-		for (int k = ncoef * 3; k < nsh; k++) dsh[k] = 0.f;
+		float dRGB[3];
+		masked_drgb(cj, g1.w, g2.x, g2.y, dRGB);
+		const int ncoef = min(f.M, (f.D + 1) * (f.D + 1));
+		float B[16];
+		sh_basis(f.D, x, y, z, B);
+		// coefficients beyond the active degree receive +0 gradient
 #pragma unroll
-		for (int ch = 0; ch < 3; ch++) {
-			// all coefficients of this channel are read before any gradient is written: sh and dsh may alias (staged rows)
-			float cf[16];
-#pragma unroll
-			for (int k = 0; k < 16; k++) cf[k] = k < ncoef ? sh[k * 3 + ch] : 0.f;
-#define SHC(k) cf[k]
-#define DSH(k) dsh[(k) * 3 + ch]
-			const float g = dRGB[ch];
-			float dx = 0.f, dy = 0.f, dz = 0.f;
-			DSH(0) = kC0 * g;
-			if (deg > 0 && ncoef >= 4) {
-				DSH(1) = (-kC1 * y) * g; DSH(2) = (kC1 * z) * g; DSH(3) = (-kC1 * x) * g;
-				dx = -kC1 * SHC(3); dy = -kC1 * SHC(1); dz = kC1 * SHC(2);
-				if (deg > 1 && ncoef >= 9) {
-					const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-					DSH(4) = (kC2[0] * xy) * g; DSH(5) = (kC2[1] * yz) * g; DSH(6) = (kC2[2] * (2.f * zz - xx - yy)) * g;
-					DSH(7) = (kC2[3] * xz) * g; DSH(8) = (kC2[4] * (xx - yy)) * g;
-					dx += kC2[0] * y * SHC(4) + kC2[2] * 2.f * -x * SHC(6) + kC2[3] * z * SHC(7) + kC2[4] * 2.f * x * SHC(8);
-					dy += kC2[0] * x * SHC(4) + kC2[1] * z * SHC(5) + kC2[2] * 2.f * -y * SHC(6) + kC2[4] * 2.f * -y * SHC(8);
-					dz += kC2[1] * y * SHC(5) + kC2[2] * 2.f * 2.f * z * SHC(6) + kC2[3] * x * SHC(7);
-					if (deg > 2 && ncoef >= 16) {
-						DSH(9) = (kC3[0] * y * (3.f * xx - yy)) * g; DSH(10) = (kC3[1] * xy * z) * g;
-						DSH(11) = (kC3[2] * y * (4.f * zz - xx - yy)) * g; DSH(12) = (kC3[3] * z * (2.f * zz - 3.f * xx - 3.f * yy)) * g;
-						DSH(13) = (kC3[4] * x * (4.f * zz - xx - yy)) * g; DSH(14) = (kC3[5] * z * (xx - yy)) * g;
-						DSH(15) = (kC3[6] * x * (xx - 3.f * yy)) * g;
-						dx += (kC3[0] * SHC(9) * 3.f * 2.f * xy + kC3[1] * SHC(10) * yz + kC3[2] * SHC(11) * -2.f * xy +
-						       kC3[3] * SHC(12) * -3.f * 2.f * xz + kC3[4] * SHC(13) * (-3.f * xx + 4.f * zz - yy) +
-						       kC3[5] * SHC(14) * 2.f * xz + kC3[6] * SHC(15) * 3.f * (xx - yy));
-						dy += (kC3[0] * SHC(9) * 3.f * (xx - yy) + kC3[1] * SHC(10) * xz + kC3[2] * SHC(11) * (-3.f * yy + 4.f * zz - xx) +
-						       kC3[3] * SHC(12) * -3.f * 2.f * yz + kC3[4] * SHC(13) * -2.f * xy + kC3[5] * SHC(14) * -2.f * yz +
-						       kC3[6] * SHC(15) * -3.f * 2.f * xy);
-						dz += (kC3[1] * SHC(10) * xy + kC3[2] * SHC(11) * 4.f * 2.f * yz + kC3[3] * SHC(12) * 3.f * (2.f * zz - xx - yy) +
-						       kC3[4] * SHC(13) * 4.f * 2.f * xz + kC3[5] * SHC(14) * (xx - yy));
-					}
-				}
-			}
-#undef SHC
-#undef DSH
-			ddir[0] += dx * g; ddir[1] += dy * g; ddir[2] += dz * g;
-		}
-		add_to(dmean, dnormvdv(dir_orig, make_float3(ddir[0], ddir[1], ddir[2])));
+		for (int e = 0; e < 48; e++)
+			if (e < nsh) dsh[e] = e / 3 < ncoef ? B[e / 3] * dRGB[e % 3] : 0.f;
+		for (int e = 48; e < nsh; e++) dsh[e] = 0.f;
+		add_to(dmean, dnormvdv(dir_orig, color_jac_dir_grad(cj, dRGB)));
 	}
 	dL_dmeans3D[3 * i] = dmean.x; dL_dmeans3D[3 * i + 1] = dmean.y; dL_dmeans3D[3 * i + 2] = dmean.z;
 
@@ -279,23 +214,17 @@ __global__ void __launch_bounds__(256) preprocess_bwd_kernel(
 
 // ---------------------------------------------------------------------------------------------------------------------------------
 // TMA variant (rows of 12*M bytes with M in {4, 8, 12, 16}, 16-B aligned: SH degree 1 and 3).  Same geometry functions as the kernel
-// above; what changes is how the two big streams of this kernel — the SH coefficients in (12M B per Gaussian) and their gradients out
-// (12M B) — move:
-//   * at the very top every lane issues ONE cp.async.bulk of its coefficient row into a padded shared-memory row (stride
-//     kBwdStride floats = 208 B: 16-B aligned for TMA / LDS.128, and 13 x 16 B so the 8 lanes of a quarter-warp hit 8 distinct
-//     16-B bank groups); one mbarrier per warp counts the bytes.  The round-1 kernel staged the block with a per-lane loop of
-//     "load 16 B, store to shared" — one DRAM round trip per iteration, 12 iterations; the profiler's source view put a large share of
-//     the warp stalls on those two STS, and the padded-row scalar stores caused bank conflicts;
-//   * every other per-Gaussian input (radius, the 12 screen-space sums, position, scale, rotation, clamp bits) is requested before
-//     any arithmetic, so the whole kernel waits for DRAM once;
-//   * the SH backward runs IN PLACE on the row with LDS.128 / STS.128 (coefficient e = 3k + ch of float4 j = e / 4 is read, its
-//     contribution to d colour / d direction accumulated, and its gradient basis_k * dL/dRGB[ch] written back to the same slot);
-//   * each lane then issues ONE cp.async.bulk shared -> global of its gradient row (zeros for culled Gaussians).
+// above; what changes is how the biggest stream of this kernel — the SH gradients out (12M B per Gaussian) — leaves, and the load order:
+//   * every per-Gaussian input (radius, the 12 screen-space sums, position, scale, rotation, and for visible Gaussians the colour
+//     Jacobian) is requested before any arithmetic, so the kernel waits for DRAM about once;
+//   * each lane writes its gradient row basis_k * dL/dRGB[ch] with STS.128 into a padded shared-memory row (stride kBwdStride floats
+//     = 208 B: 16-B aligned for the bulk copy, and 13 x 16 B so the 8 lanes of a quarter-warp hit 8 distinct 16-B bank groups) and
+//     issues ONE cp.async.bulk shared -> global of it (zeros for culled Gaussians).
 template <bool GATHER>
 __global__ void __launch_bounds__(256, 3) preprocess_bwd_tma_kernel(
-    const FrameDev f, const PeerTable pt, const float *__restrict__ means3D, const float *__restrict__ shs, const float *__restrict__ scales,
+    const FrameDev f, const PeerTable pt, const float *__restrict__ means3D, const float *__restrict__ scales,
     const float *__restrict__ rotations, const float *__restrict__ cov3D_precomp, const int32_t *__restrict__ radii,
-    const GaussRec *__restrict__ rec, const float *__restrict__ grad2d, float *__restrict__ dL_dmeans3D, float *__restrict__ dL_dmeans2D,
+    const float4 *__restrict__ jac, const float *__restrict__ grad2d, float *__restrict__ dL_dmeans3D, float *__restrict__ dL_dmeans2D,
     float *__restrict__ dL_dsh, float *__restrict__ dL_dopacity, float *__restrict__ dL_dscales, float *__restrict__ dL_drot,
     float *__restrict__ dL_dcov3D) {
 	extern __shared__ __align__(16) unsigned char s_stage[];
@@ -306,28 +235,15 @@ __global__ void __launch_bounds__(256, 3) preprocess_bwd_tma_kernel(
 	const size_t i = (size_t)idx;
 	const int nsh = f.M * 3;
 	const uint32_t row_bytes = (uint32_t)nsh * 4u;
-	const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(s_stage);
-	const uint32_t row = sbase + (uint32_t)((warp * 32 + lane) * kBwdStride) * 4u;
-	const uint32_t bar = sbase + (uint32_t)(8 * 32 * kBwdStride) * 4u + (uint32_t)warp * 8u;
-	const int first = blockIdx.x * blockDim.x + warp * 32;
-	const int rows = min(32, f.P - first);
-	if (rows > 0) {
-		if (lane == 0) {
-			mbar_init(bar, 1);
-			fence_proxy_async();
-		}
-		__syncwarp();
-		if (in_range) bulk_g2s(row, shs + i * nsh, row_bytes, bar);
-		if (lane == 0) mbar_expect_tx(bar, row_bytes * (uint32_t)rows);
-	}
-	// ---- every small input up front ----
+	const uint32_t row = (uint32_t)__cvta_generic_to_shared(s_stage) + (uint32_t)((warp * 32 + lane) * kBwdStride) * 4u;
+	// ---- every input up front ----
 	int radius = 0;
 	float4 g0v = make_float4(0.f, 0.f, 0.f, 0.f), g1v = g0v, g2v = g0v;
 	float3 mean = make_float3(0.f, 0.f, 0.f);
 	float3 sc = make_float3(0.f, 0.f, 0.f);
 	float4 q = make_float4(1.f, 0.f, 0.f, 0.f);
 	float c6[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-	uint32_t clamp_bits = 0u;
+	ColorJac cj = {g0v, g0v, g0v};
 	if (in_range) {
 		radius = radii[idx];
 		mean = make_float3(means3D[3 * i], means3D[3 * i + 1], means3D[3 * i + 2]);
@@ -338,12 +254,13 @@ __global__ void __launch_bounds__(256, 3) preprocess_bwd_tma_kernel(
 			q = *reinterpret_cast<const float4 *>(rotations + 4 * i);
 			sc = make_float3(scales[3 * i], scales[3 * i + 1], scales[3 * i + 2]);
 		}
-		clamp_bits = __float_as_uint(rec[idx].q2.w) & 7u;  // (the fused forward keeps the radius in the upper bits)
 		if (!GATHER) {
 			g0v = reinterpret_cast<const float4 *>(grad2d)[3 * i];      // mean2D.x, .y, .z(abs), conic.xx
 			g1v = reinterpret_cast<const float4 *>(grad2d)[3 * i + 1];  // conic.xy, conic.yy, opacity, color.r
 			g2v = reinterpret_cast<const float4 *>(grad2d)[3 * i + 2];  // color.g, color.b, depth, pad
 		}
+		// (the forward writes it for visible Gaussians only; the gather keeps it out of its registers)
+		if (!GATHER && radius > 0) cj = load_color_jac(jac + 3 * i);
 	}
 	if (threadIdx.x < 16) s_cam[threadIdx.x] = f.view[threadIdx.x];
 	else if (threadIdx.x < 32) s_cam[threadIdx.x] = f.proj[threadIdx.x - 16];
@@ -356,17 +273,24 @@ __global__ void __launch_bounds__(256, 3) preprocess_bwd_tma_kernel(
 		__shared__ float4 s_g[3 * kRunBlock];
 		const uint32_t mask = visible ? reinterpret_cast<const uint32_t *>(grad2d)[idx] : 0u;
 		gather_runs(pt, mask, rs, s_g, g0v, g1v, g2v);
+		if (visible) cj = load_color_jac(jac + 3 * i);
 	}
 	const float4 g0 = g0v, g1 = g1v, g2 = g2v;
 	if (in_range) {
 		dL_dmeans2D[3 * i] = g0.x; dL_dmeans2D[3 * i + 1] = g0.y; dL_dmeans2D[3 * i + 2] = g0.z;
 		dL_dopacity[i] = g1.z;
 	}
+	// the colour terms first: 6 live floats instead of the 12 of the Jacobian through the geometry below
+	float dRGB[3] = {0.f, 0.f, 0.f};
+	float3 ddir = make_float3(0.f, 0.f, 0.f);
+	if (visible) {
+		masked_drgb(cj, g1.w, g2.x, g2.y, dRGB);
+		ddir = color_jac_dir_grad(cj, dRGB);
+	}
 	float3 dmean = make_float3(0.f, 0.f, 0.f);
 	float dcov[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
 	float3 dscale = make_float3(0.f, 0.f, 0.f);
 	float4 dq = make_float4(0.f, 0.f, 0.f, 0.f);
-	float dRGB[3] = {0.f, 0.f, 0.f};
 	float3 dir_orig = make_float3(0.f, 0.f, 1.f);
 	if (visible) {
 		float3 s_mod = make_float3(f.mod * sc.x, f.mod * sc.y, f.mod * sc.z);
@@ -381,9 +305,6 @@ __global__ void __launch_bounds__(256, 3) preprocess_bwd_tma_kernel(
 		add_to(dmean, mean2d_bwd(mean, proj, g0.x, g0.y));
 		add_to(dmean, depth_bwd(mean, view, g2.z));
 		if (cov3D_precomp == nullptr) cov3d_bwd(s_mod, q, R, dcov, dscale, dq);
-		dRGB[0] = (clamp_bits & 1u) ? 0.f : g1.w;
-		dRGB[1] = (clamp_bits & 2u) ? 0.f : g2.x;
-		dRGB[2] = (clamp_bits & 4u) ? 0.f : g2.y;
 		dir_orig = make_float3(mean.x - s_cam[32], mean.y - s_cam[33], mean.z - s_cam[34]);
 	}
 	if (in_range) {
@@ -394,65 +315,27 @@ __global__ void __launch_bounds__(256, 3) preprocess_bwd_tma_kernel(
 			for (int k = 0; k < 6; k++) dL_dcov3D[6 * i + k] = dcov[k];
 		}
 	}
-	// ---- SH backward in place on the staged row (reference backward.cu:20-139) ----
-	if (rows > 0) mbar_wait(bar, 0);  // the warp's rows have landed; nobody may touch (or abandon) the stage before this
+	// ---- SH backward (reference backward.cu:20-139) into the staged row ----
 	if (in_range) {
 		const float len = sqrtf(dir_orig.x * dir_orig.x + dir_orig.y * dir_orig.y + dir_orig.z * dir_orig.z);
 		const float x = dir_orig.x / len, y = dir_orig.y / len, z = dir_orig.z / len;
-		const int deg = f.D;
-		const int ncoef = visible ? min(f.M, (deg + 1) * (deg + 1)) : 0;  // culled: every gradient 0
-		// basis_k and its partial derivatives w.r.t. the unit direction; coefficients beyond the active degree get zeros
-		float B[16], Bx[16], By[16], Bz[16];
-#pragma unroll
-		for (int k = 0; k < 16; k++) { B[k] = 0.f; Bx[k] = 0.f; By[k] = 0.f; Bz[k] = 0.f; }
-		const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-		if (ncoef >= 1) B[0] = kC0;
-		if (deg > 0 && ncoef >= 4) {
-			B[1] = -kC1 * y; B[2] = kC1 * z; B[3] = -kC1 * x;
-			By[1] = -kC1; Bz[2] = kC1; Bx[3] = -kC1;
-		}
-		if (deg > 1 && ncoef >= 9) {
-			B[4] = kC2[0] * xy; B[5] = kC2[1] * yz; B[6] = kC2[2] * (2.f * zz - xx - yy); B[7] = kC2[3] * xz; B[8] = kC2[4] * (xx - yy);
-			Bx[4] = kC2[0] * y; By[4] = kC2[0] * x;
-			By[5] = kC2[1] * z; Bz[5] = kC2[1] * y;
-			Bx[6] = kC2[2] * 2.f * -x; By[6] = kC2[2] * 2.f * -y; Bz[6] = kC2[2] * 2.f * 2.f * z;
-			Bx[7] = kC2[3] * z; Bz[7] = kC2[3] * x;
-			Bx[8] = kC2[4] * 2.f * x; By[8] = kC2[4] * 2.f * -y;
-		}
-		if (deg > 2 && ncoef >= 16) {
-			B[9] = kC3[0] * y * (3.f * xx - yy); B[10] = kC3[1] * xy * z; B[11] = kC3[2] * y * (4.f * zz - xx - yy);
-			B[12] = kC3[3] * z * (2.f * zz - 3.f * xx - 3.f * yy); B[13] = kC3[4] * x * (4.f * zz - xx - yy); B[14] = kC3[5] * z * (xx - yy);
-			B[15] = kC3[6] * x * (xx - 3.f * yy);
-			Bx[9] = kC3[0] * 3.f * 2.f * xy; By[9] = kC3[0] * 3.f * (xx - yy);
-			Bx[10] = kC3[1] * yz; By[10] = kC3[1] * xz; Bz[10] = kC3[1] * xy;
-			Bx[11] = kC3[2] * -2.f * xy; By[11] = kC3[2] * (-3.f * yy + 4.f * zz - xx); Bz[11] = kC3[2] * 4.f * 2.f * yz;
-			Bx[12] = kC3[3] * -3.f * 2.f * xz; By[12] = kC3[3] * -3.f * 2.f * yz; Bz[12] = kC3[3] * 3.f * (2.f * zz - xx - yy);
-			Bx[13] = kC3[4] * (-3.f * xx + 4.f * zz - yy); By[13] = kC3[4] * -2.f * xy; Bz[13] = kC3[4] * 4.f * 2.f * xz;
-			Bx[14] = kC3[5] * 2.f * xz; By[14] = kC3[5] * -2.f * yz; Bz[14] = kC3[5] * (xx - yy);
-			Bx[15] = kC3[6] * 3.f * (xx - yy); By[15] = kC3[6] * -3.f * 2.f * xy;
-		}
-		float ddx = 0.f, ddy = 0.f, ddz = 0.f;
+		const int ncoef = visible ? min(f.M, (f.D + 1) * (f.D + 1)) : 0;  // culled: every gradient 0
+		float B[16];
+		sh_basis(f.D, x, y, z, B);
 #pragma unroll
 		for (int j = 0; j < 12; j++) {
 			if (4 * j < nsh) {
-				float4 v;
-				asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(row + 16u * j));
-				const float cv[4] = {v.x, v.y, v.z, v.w};
 				float o[4];
 #pragma unroll
 				for (int tt = 0; tt < 4; tt++) {
 					const int e = 4 * j + tt, k = e / 3, ch = e % 3;  // compile-time after unrolling
-					// coefficients beyond the active degree are never read (a NaN or Inf stored there must not reach dL/dmean3D)
-					// and get +0 (B[k] = 0 times a negative dL/dRGB would store -0)
-					const bool active = k < ncoef;
-					const float cg = active ? cv[tt] * dRGB[ch] : 0.f;
-					ddx += Bx[k] * cg; ddy += By[k] * cg; ddz += Bz[k] * cg;
-					o[tt] = active ? B[k] * dRGB[ch] : 0.f;
+					// coefficients beyond the active degree get +0 (B[k] = 0 times a negative dL/dRGB would store -0)
+					o[tt] = k < ncoef ? B[k] * dRGB[ch] : 0.f;
 				}
 				asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(row + 16u * j), "f"(o[0]), "f"(o[1]), "f"(o[2]), "f"(o[3]) : "memory");
 			}
 		}
-		if (visible) add_to(dmean, dnormvdv(dir_orig, make_float3(ddx, ddy, ddz)));
+		if (visible) add_to(dmean, dnormvdv(dir_orig, ddir));
 		dL_dmeans3D[3 * i] = dmean.x; dL_dmeans3D[3 * i + 1] = dmean.y; dL_dmeans3D[3 * i + 2] = dmean.z;
 		// this lane's gradient row leaves through the async proxy
 		fence_proxy_async();
@@ -468,11 +351,11 @@ static bool bwd_rows_fit_tma(const FrameDev &f, const float *shs, const float *d
 	return shs != nullptr && dL_dsh != nullptr && f.M > 0 && f.M <= 16 && (f.M * 12) % 16 == 0 && (reinterpret_cast<uintptr_t>(shs) & 15u) == 0 &&
 	       (reinterpret_cast<uintptr_t>(dL_dsh) & 15u) == 0;
 }
-constexpr size_t kBwdStageBytes = (size_t)8 * 32 * kBwdStride * sizeof(float) + 8 * sizeof(uint64_t);
+constexpr size_t kBwdStageBytes = (size_t)8 * 32 * kBwdStride * sizeof(float);
 
 cudaError_t launch_preprocess_bwd(const FrameDev &f, const PeerTable *pt, const float *means3D, const float *shs, const float *colors_precomp,
                                   const float *scales, const float *rotations, const float *cov3D_precomp, const int32_t *radii,
-                                  const GaussRec *rec, const float *grad2d, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh,
+                                  const float4 *jac, const float *grad2d, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh,
                                   float *dL_dcolors, float *dL_dopacity, float *dL_dscales, float *dL_drot, float *dL_dcov3D, cudaStream_t st) {
 	if (f.P == 0) return cudaSuccess;
 	const bool gather = pt != nullptr;  // pt == nullptr: the local path, grad2d holds this process's screen-space sums
@@ -484,7 +367,7 @@ cudaError_t launch_preprocess_bwd(const FrameDev &f, const PeerTable *pt, const 
 		const auto kernel = gather ? preprocess_bwd_tma_kernel<true> : preprocess_bwd_tma_kernel<false>;
 		if ((e = ensure_dynamic_smem(kernel, (int)kBwdStageBytes, configured[gather])) != cudaSuccess) return e;
 		count_launch();
-		kernel<<<grid, 256, kBwdStageBytes, st>>>(f, peers, means3D, shs, scales, rotations, cov3D_precomp, radii, rec, grad2d, dL_dmeans3D,
+		kernel<<<grid, 256, kBwdStageBytes, st>>>(f, peers, means3D, scales, rotations, cov3D_precomp, radii, jac, grad2d, dL_dmeans3D,
 		                                          dL_dmeans2D, dL_dsh, dL_dopacity, dL_dscales, dL_drot, dL_dcov3D);
 		return cudaGetLastError();
 	}
@@ -497,7 +380,7 @@ cudaError_t launch_preprocess_bwd(const FrameDev &f, const PeerTable *pt, const 
 		if ((e = ensure_dynamic_smem(kernel, (int)smem, configured[gather])) != cudaSuccess) return e;
 	}
 	count_launch();
-	kernel<<<grid, 256, smem, st>>>(f, peers, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii, rec, grad2d, dL_dmeans3D,
+	kernel<<<grid, 256, smem, st>>>(f, peers, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii, jac, grad2d, dL_dmeans3D,
 	                                dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drot, dL_dcov3D);
 	return cudaGetLastError();
 }

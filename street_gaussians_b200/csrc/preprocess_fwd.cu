@@ -9,7 +9,8 @@
 // recomputes it), (3) tiles_touched counts only the tiles of the 3-sigma rectangle that can actually receive a
 // contribution (exact opacity-aware row-span cull, tile_visit.cuh) and that lie in this process's tile-row band,
 // (4) large rectangles are counted warp-cooperatively instead of by one thread, (5) a 32-bit depth key per Gaussian
-// feeds the depth pre-sort of binning.cu.  The per-Gaussian geometry it shares with the backward is in gaussian_geom.cuh.
+// feeds the depth pre-sort of binning.cu, (6) the SH colour's 3 x 3 direction Jacobian (+ clamp bits) is stored for the backward,
+// which then never reads the coefficient rows.  The per-Gaussian geometry it shares with the backward is in gaussian_geom.cuh.
 #include "gaussian_geom.cuh"
 #include "tile_visit.cuh"
 
@@ -85,10 +86,8 @@ __device__ __forceinline__ void load_sh_global(float *c, const float *__restrict
 	}
 }
 
-__device__ __forceinline__ float3 sh_eval(int deg, const float3 p, const float3 campos, const float *c, uint32_t &clamp_bits) {
-	float3 d = make_float3(p.x - campos.x, p.y - campos.y, p.z - campos.z);
-	const float len = sqrtf(d.x * d.x + d.y * d.y + d.z * d.z);
-	const float x = d.x / len, y = d.y / len, z = d.z / len;
+// (x, y, z) = the unit view direction (mean - campos) / |mean - campos|
+__device__ __forceinline__ float3 sh_eval(int deg, const float x, const float y, const float z, const float *c, uint32_t &clamp_bits) {
 	float res[3];
 #pragma unroll
 	for (int ch = 0; ch < 3; ch++) {
@@ -126,7 +125,7 @@ __global__ void __launch_bounds__(256) preprocess_fwd_kernel(const FrameDev f, c
                                                              const float *__restrict__ opacities, const float *__restrict__ scales,
                                                              const float *__restrict__ rotations, const float *__restrict__ cov3D_precomp,
                                                              int32_t *__restrict__ radii, GaussRec *__restrict__ rec,
-                                                             uint32_t *__restrict__ tiles_touched, uint32_t *__restrict__ depth_key,
+                                                             float4 *__restrict__ jac, uint32_t *__restrict__ tiles_touched, uint32_t *__restrict__ depth_key,
                                                              uint32_t *__restrict__ iota, const size_t cnt_offset = 0) {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	const bool in_range = idx < f.P;
@@ -162,7 +161,15 @@ __global__ void __launch_bounds__(256) preprocess_fwd_kernel(const FrameDev f, c
 				float c[48];
 				const int n = min(f.M, (f.D + 1) * (f.D + 1)) * 3;
 				load_sh_global(c, shs + (size_t)idx * f.M * 3, f.M, n);
-				rgb = sh_eval(f.D, p, campos, c, clamp_bits);
+				const float3 d = make_float3(p.x - campos.x, p.y - campos.y, p.z - campos.z);
+				const float len = sqrtf(d.x * d.x + d.y * d.y + d.z * d.z);
+				const float x = d.x / len, y = d.y / len, z = d.z / len;
+				rgb = sh_eval(f.D, x, y, z, c, clamp_bits);
+				// the colour's direction Jacobian for the backward, taken while the row is in registers: the backward then reads 48 B
+				// per Gaussian instead of the 12 M-byte row
+				float J[9];
+				sh_color_jacobian(f.D, x, y, z, c, J);
+				store_color_jac(jac + 3 * (size_t)idx, J, clamp_bits);
 			} else {
 				rgb = make_float3(colors_precomp[3 * (size_t)idx], colors_precomp[3 * (size_t)idx + 1], colors_precomp[3 * (size_t)idx + 2]);
 			}
@@ -261,27 +268,27 @@ cudaError_t launch_preprocess_fwd(const FrameDev &f, const float *means3D, const
 	if (f.P == 0) return cudaSuccess;
 	count_launch();
 	preprocess_fwd_kernel<true><<<(f.P + 255) / 256, 256, 0, st>>>(f, PeerTable{}, means3D, shs, colors_precomp, opacities, scales, rotations,
-	                                                                  cov3D_precomp, radii, g.rec, g.tiles_touched, g.depth_key, g.iota);
+	                                                                  cov3D_precomp, radii, g.rec, g.jac, g.tiles_touched, g.depth_key, g.iota);
 	return cudaGetLastError();
 }
 cudaError_t launch_project(const FrameDev &f, const float *means3D, const float *shs, const float *colors_precomp,
                            const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
-                           int32_t *radii, GaussRec *rec, cudaStream_t st) {
+                           int32_t *radii, GaussRec *rec, float4 *jac, cudaStream_t st) {
 	if (f.P == 0) return cudaSuccess;
 	count_launch();
 	preprocess_fwd_kernel<false><<<(f.P + 255) / 256, 256, 0, st>>>(f, PeerTable{}, means3D, shs, colors_precomp, opacities, scales, rotations,
-	                                                                   cov3D_precomp, radii, rec, nullptr, nullptr, nullptr);
+	                                                                   cov3D_precomp, radii, rec, jac, nullptr, nullptr, nullptr);
 	return cudaGetLastError();
 }
 cudaError_t launch_project_scatter(const FrameDev &f, const PeerTable &pt, const float *means3D, const float *shs,
                                    const float *colors_precomp, const float *opacities, const float *scales, const float *rotations,
-                                   const float *cov3D_precomp, int32_t *radii_local, GaussRec *rec_local, uint32_t *masks_local,
-                                   size_t cnt_offset, cudaStream_t st) {
+                                   const float *cov3D_precomp, int32_t *radii_local, GaussRec *rec_local, float4 *jac_local,
+                                   uint32_t *masks_local, size_t cnt_offset, cudaStream_t st) {
 	if (pt.chunk == 0) return cudaSuccess;
 	count_launch();
 	const unsigned nblk = (unsigned)((pt.chunk + kRunBlock - 1) / kRunBlock);
 	preprocess_fwd_kernel<false, true><<<nblk, 256, 0, st>>>(f, pt, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-	                                                         radii_local, rec_local, nullptr, masks_local, nullptr, cnt_offset);
+	                                                         radii_local, rec_local, jac_local, nullptr, masks_local, nullptr, cnt_offset);
 	return cudaGetLastError();
 }
 cudaError_t launch_filter(const FrameDev &f, const float *means3D, const float *scales, const float *rotations,

@@ -43,6 +43,7 @@ struct GeomView {
 	uint32_t *big_count;      // status words, zeroed per forward: [0] number of entries in big_list (device counter)
 	                          // [1] instance count R, [2] overflow bits (1 = instance capacity, 2 = Gaussian capacity of the compacted
 	                          // depth order), [3] instances actually emitted (bounded mode), [4] Gaussians with instances (compacted mode)
+	float4 *jac;              // per Gaussian with SH colour: 3 float4, d colour / d view direction + clamp bits (gaussian_geom.cuh)
 	uint32_t *ckey, *cval;    // compacted depth-sort input (keys / Gaussian indices), Gaussian-sharded forward only
 	void *temp;               // cub temp storage: max(scan, depth sort)
 	size_t temp_bytes;
@@ -242,7 +243,7 @@ cudaError_t launch_preprocess_fwd(const FrameDev &f, const float *means3D, const
 // records + radii only (no tile counts): step 1 of the Gaussian-sharded forward
 cudaError_t launch_project(const FrameDev &f, const float *means3D, const float *shs, const float *colors_precomp,
                            const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
-                           int32_t *radii, GaussRec *rec, cudaStream_t st);
+                           int32_t *radii, GaussRec *rec, float4 *jac, cudaStream_t st);
 cudaError_t launch_filter(const FrameDev &f, const float *means3D, const float *scales, const float *rotations,
                           const float *cov3D_precomp, int32_t *radii, float *means2D, cudaStream_t st);
 cudaError_t launch_mark_visible(int P, const float *means3D, const float *view, uint8_t *present, cudaStream_t st);
@@ -325,8 +326,8 @@ cudaError_t launch_peer_barrier(const PeerTable &pt, uint32_t epoch, uint32_t *s
 // sgr_project fused with sgr_scatter_records: one pass over the rank's chunk (f.P local Gaussians, pt.chunk slots)
 cudaError_t launch_project_scatter(const FrameDev &f, const PeerTable &pt, const float *means3D, const float *shs,
                                    const float *colors_precomp, const float *opacities, const float *scales, const float *rotations,
-                                   const float *cov3D_precomp, int32_t *radii_local, GaussRec *rec_local, uint32_t *masks_local,
-                                   size_t cnt_offset, cudaStream_t st);
+                                   const float *cov3D_precomp, int32_t *radii_local, GaussRec *rec_local, float4 *jac_local,
+                                   uint32_t *masks_local, size_t cnt_offset, cudaStream_t st);
 cudaError_t launch_scatter_records(const FrameDev &f, const PeerTable &pt, const GaussRec *rec, const int32_t *radii, cudaStream_t st);
 cudaError_t launch_gather_grad2d(const FrameDev &f, const PeerTable &pt, const GaussRec *rec, const int32_t *radii, float *out,
                                  cudaStream_t st);
@@ -351,7 +352,7 @@ cudaError_t launch_blend_bwd2(const FrameDev &f, GeomView g, BinView b, ImgView 
 // and grad2d carries instead the destination masks (u32[f.P]) the forward stored.
 cudaError_t launch_preprocess_bwd(const FrameDev &f, const PeerTable *pt, const float *means3D, const float *shs, const float *colors_precomp,
                                   const float *scales, const float *rotations, const float *cov3D_precomp, const int32_t *radii,
-                                  const GaussRec *rec, const float *grad2d, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh,
+                                  const float4 *jac, const float *grad2d, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh,
                                   float *dL_dcolors, float *dL_dopacity, float *dL_dscales, float *dL_drot, float *dL_dcov3D, cudaStream_t st);
 // render layers (layers.cu)
 cudaError_t launch_layer_lists(const FrameDev &f, ImgView main_img, BinView main_bin, int begin, int end, ImgView layer_img, uint32_t *layer_list,

@@ -115,17 +115,22 @@ _local_tensors = _fp32_inputs  # step 0: the local Gaussians as the kernels read
 
 def project_records(tensors, settings: GaussianRasterizationSettings, chunk: int):
     """Step 1 (sgr_project): records[chunk,12] float32 view + radii[chunk] int32 of the local Gaussians; slots past
-    P_local are padding (radii == 0)."""
+    P_local are padding (radii == 0).  The records are the head of a whole geom state for P_local (sgr_state_sizes bytes,
+    132 B per Gaussian + cub temp), which also holds the colour Jacobian that backward_geom_local reads, so the state stays
+    alive with the records until the backward; the rows of padding slots may overlap that Jacobian (they are never read)."""
     means3D = tensors["means3D"]
     device, P = means3D.device, int(means3D.shape[0])
     if P > chunk:
         raise _capi.SgrError(f"{P} local Gaussians do not fit the per-rank chunk of {chunk}; call repartition()")
-    rec = torch.empty((chunk, REC_FLOATS), device=device, dtype=torch.float32)
-    radii = (torch.empty if P == chunk else torch.zeros)((chunk,), device=device, dtype=torch.int32)
     M = int(tensors["sh"].shape[1]) if tensors["sh"] is not None else 0
     fr, keep = _make_frame(settings, P, M, 0, device, None)
+    gb = C.c_size_t(0)
+    _capi.call("sgr_state_sizes", None, C.byref(fr), C.byref(gb), None)
+    state = torch.empty((max(gb.value, chunk * REC_FLOATS * 4),), device=device, dtype=torch.uint8)
+    rec = state[: chunk * REC_FLOATS * 4].view(torch.float32).view(chunk, REC_FLOATS)
+    radii = (torch.empty if P == chunk else torch.zeros)((chunk,), device=device, dtype=torch.int32)
     _capi.call("sgr_project", device, C.byref(fr), ptr(means3D), ptr(tensors["sh"]), ptr(tensors["colors_precomp"]), ptr(tensors["opacities"]),
-               ptr(tensors["scales"]), ptr(tensors["rotations"]), ptr(tensors["cov3Ds_precomp"]), ptr(radii), ptr(rec))
+               ptr(tensors["scales"]), ptr(tensors["rotations"]), ptr(tensors["cov3Ds_precomp"]), ptr(radii), ptr(state))
     del keep
     return rec, radii
 
@@ -196,7 +201,7 @@ def backward_geom_local(settings, tensors, rec_local, radii_local, grad2d_local)
     """Step 5: chain rule for the local Gaussians from their own records and their reduced grad2d rows."""
     P = int(tensors["means3D"].shape[0])
     st = _ForwardState()
-    st.geom = rec_local  # sgr_backward_geom reads only the record array, which sits at offset 0 of a geom_state
+    st.geom = rec_local  # the head of project_records' geom state: sgr_backward_geom reads the colour Jacobian sgr_project left there
     local = dict(tensors)
     local["semantics"] = None
     return _backward_geom_impl(settings, None, st, local, radii_local[:P], grad2d_local[:P].contiguous())
