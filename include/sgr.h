@@ -84,6 +84,19 @@ const char *sgr_last_error(void);
  * included).  Diagnostic only — bench.py reports the delta over its timed region as `gpu_launches`.  No reference counterpart. */
 uint64_t sgr_launch_count(void);
 
+/* Saturation split of sgr_forward / sgr_forward_bounded (whole-image frames of at most 16384 tiles without semantic channels; other
+ * forwards bin in one pass).  The Gaussians whose depth-order instance offsets stay within a budget of B instances are binned and
+ * blended first; the farther ones are then binned only into the tiles where some pixel has not saturated (T >= 1e-4), so their
+ * instances behind saturated pixels are never emitted.  Images, radii, n_contrib and the tile lists the backward reads do not depend
+ * on B; the instances emitted (status word 3) do.  Per calling thread, like sgr_last_error: sgr_set_near_budget sets B for the
+ * forwards the thread enqueues from then on and returns the previous setting.  SGR_NEAR_BUDGET_AUTO (any negative value) is the
+ * library's rule, a fixed fraction of the frame's instance count; a budget of at least the instance count (SGR_NEAR_BUDGET_ALL)
+ * is the one-pass binning, whose tile lists hold every instance — sgr_forward_layer needs those.  A bounded frame overflows only when
+ * the instances it emits exceed the capacity; it then keeps the Gaussians whose whole instance counts fit, as the one-pass binning. */
+#define SGR_NEAR_BUDGET_AUTO (-1)
+#define SGR_NEAR_BUDGET_ALL INT64_MAX
+int64_t sgr_set_near_budget(int64_t budget);
+
 /* Sizes (bytes) of the caller-owned forward state.  geom: per-Gaussian records (reference GeometryState,
  * DGR/cuda_rasterizer/rasterizer_impl.h:21-37); img: per-pixel / per-tile state (ImageState, :46-52).
  * binning (BinningState, :54-64) depends on the instance count R and is requested through sgr_alloc_fn;
@@ -181,7 +194,8 @@ typedef struct SgrLayer {
  * whose sgr_backward_* calls take num_instances: the instance count of sgr_forward, or the capacity of sgr_forward_bounded. */
 int sgr_layer_state_sizes(const SgrFrame *frame, int64_t num_instances, size_t *layer_bytes);
 /* Renders `layer` from the state a whole-image sgr_forward / sgr_forward_bounded left in geom / binning / img state (frame == that
- * call's frame, num_instances == the value its backward takes).  out_color[3,H,W], out_depth[1,H,W], out_alpha[1,H,W]: every pixel
+ * call's frame, num_instances == the value its backward takes).  That call must have binned every instance: enqueue it with
+ * sgr_set_near_budget(SGR_NEAR_BUDGET_ALL).  out_color[3,H,W], out_depth[1,H,W], out_alpha[1,H,W]: every pixel
  * written.  With an empty range no state is read (geom / binning / img state may be NULL). */
 int sgr_forward_layer(const SgrFrame *frame, const SgrLayer *layer, int64_t num_instances, const void *geom_state, const void *binning_state,
                       const void *img_state, void *layer_state, size_t layer_bytes, float *out_color, float *out_depth, float *out_alpha,

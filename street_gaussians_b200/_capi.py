@@ -4,6 +4,7 @@ missing or does not export the ABI, importing / calling raises — it never rout
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import os
 from typing import Optional
@@ -14,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libsgr.so")
 ABI_VERSION = 7
 
-SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_state_sizes", "sgr_binning_bytes", "sgr_forward", "sgr_forward_bounded",
+SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_set_near_budget", "sgr_state_sizes", "sgr_binning_bytes", "sgr_forward", "sgr_forward_bounded",
            "sgr_forward_status", "sgr_forward_status_async", "sgr_backward_blend",
            "sgr_backward_geom", "sgr_backward", "sgr_mark_visible", "sgr_visible_filter", "sgr_knn_scratch_bytes",
            "sgr_knn_mean_dist2", "sgr_record_bytes", "sgr_project", "sgr_forward_records",
@@ -296,6 +297,23 @@ def lib():
     L.sgr_knn_mean_dist2.argtypes = [C.c_int32, vp, vp, vp, C.c_size_t, vp]
     _lib = L
     return L
+
+
+# sgr_set_near_budget: the library's rule / every instance in one binning pass (the full tile lists render layers are compacted from)
+NEAR_BUDGET_AUTO, NEAR_BUDGET_ALL = -1, (1 << 63) - 1
+
+
+@contextlib.contextmanager
+def near_budget(budget: int):
+    """The forwards this thread enqueues inside the block use `budget` as the near budget of the saturation split (include/sgr.h,
+    sgr_set_near_budget); the previous setting is restored on exit.  Their results do not depend on it."""
+    fn = (_lib or lib()).sgr_set_near_budget
+    fn.restype, fn.argtypes = C.c_int64, [C.c_int64]
+    prev = fn(int(budget))
+    try:
+        yield
+    finally:
+        fn(prev)
 
 
 def check(rc: int, what: str) -> None:

@@ -49,6 +49,9 @@ size_t geom_temp_bytes(int P) {
 	size_t c = 0;
 	CountIter it(cub::CountingInputIterator<int>(0), GatherCount{nullptr, nullptr, nullptr});
 	cub::DeviceScan::InclusiveSum(nullptr, a, it, (uint32_t *)nullptr, n);
+	size_t d = 0;  // the far pass of the saturation split scans a plain count array
+	cub::DeviceScan::InclusiveSum(nullptr, d, (const uint32_t *)nullptr, (uint32_t *)nullptr, n);
+	a = a > d ? a : d;
 	cub::DeviceRadixSort::SortPairs(nullptr, b, (uint32_t *)nullptr, (uint32_t *)nullptr, (uint32_t *)nullptr, (uint32_t *)nullptr, n);
 	cub::DeviceSelect::If(nullptr, c, cub::CountingInputIterator<int>(0), (uint32_t *)nullptr, (uint32_t *)nullptr, n, WasDelivered{nullptr});
 	a = a > b ? a : b;
@@ -238,12 +241,17 @@ constexpr uint32_t kEmitStage = 512;  // instances staged per warp (2 x 2 KB of 
 
 // thread t handles the t-th Gaussian in depth order.  KeyT = uint16_t whenever the image has at most 65,536 tiles (up to
 // 4096 x 4096 px): the tile sort then moves 6 instead of 8 bytes per pair per pass.
-template <typename KeyT>
+// Saturation split (launch_near_binning / launch_far_binning): the near pass passes dev_cap -> its end of the emitted sequence, so
+// only the Gaussians before the split emit; the far pass passes its own offsets, dev_cap -> the end of the emitted sequence,
+// dev_floor -> the near pass's end (the Gaussians before the split then have empty ranges there) and the KeepUnsaturated predicate.
+template <typename KeyT, typename Keep = KeepAll>
 __global__ void __launch_bounds__(256) emit_pairs_kernel(const FrameDev f, const GaussRec *__restrict__ rec, const int32_t *__restrict__ radii,
                                                         const uint32_t *__restrict__ /*tiles_touched*/, const uint32_t *__restrict__ perm,
                                                         const uint32_t *__restrict__ offsets, KeyT *__restrict__ keys,
                                                         uint32_t *__restrict__ vals, uint32_t *__restrict__ big_list,
-                                                        uint32_t *__restrict__ big_count, const uint32_t cap, const int n_order) {
+                                                        uint32_t *__restrict__ big_count, uint32_t cap, const int n_order,
+                                                        const uint32_t *__restrict__ dev_cap = nullptr,
+                                                        const uint32_t *__restrict__ dev_floor = nullptr, const Keep keep = Keep()) {
 	__shared__ KeyT s_keys[8][kEmitStage];
 	__shared__ uint32_t s_vals[8][kEmitStage];
 	const int warp = threadIdx.x >> 5;
@@ -257,6 +265,12 @@ __global__ void __launch_bounds__(256) emit_pairs_kernel(const FrameDev f, const
 	uint32_t end = offsets[tc];
 	uint32_t off = tc == 0 ? 0u : offsets[tc - 1];
 	if (t >= n_order) off = end;
+	if (dev_cap) cap = min(cap, *dev_cap);
+	if (dev_floor) {
+		const uint32_t fl = *dev_floor;
+		off = max(off, fl);
+		end = max(end, fl);
+	}
 	// bounded mode: a Gaussian whose range does not fit the caller's capacity emits nothing.  BOTH ends are clamped so that
 	// warp_first / warp_last (taken from lanes 0 / 31 below) never address past `cap`, even when every lane of the warp
 	// overflows: the staged flush then covers at most [warp_first, cap), and pad_keys_kernel rewrites [emitted, cap).
@@ -277,17 +291,17 @@ __global__ void __launch_bounds__(256) emit_pairs_kernel(const FrameDev f, const
 	const uint32_t warp_last = __shfl_sync(0xffffffffu, end, 31);
 	const uint32_t warp_total = warp_last >= warp_first ? warp_last - warp_first : 0xffffffffu;  // (overflow tail: no staging)
 	uint32_t count;
-	visit_tiles<true, KeyT>(active, x0, y0, x1, y1, cp, f.band, f.gx, gidx, off, keys, vals, count, s_keys[warp], s_vals[warp], kEmitStage,
-	                  warp_first, warp_total, big_list, big_count, (uint32_t)t);
+	visit_tiles<true, KeyT, Keep>(active, x0, y0, x1, y1, cp, f.band, f.gx, gidx, off, keys, vals, count, s_keys[warp], s_vals[warp],
+	                              kEmitStage, warp_first, warp_total, big_list, big_count, (uint32_t)t, keep);
 }
 
 // One warp per deferred (large-rectangle) Gaussian, grid-strided over the device-side list: no host round trip for the count.
-template <typename KeyT>
+template <typename KeyT, typename Keep = KeepAll>
 __global__ void __launch_bounds__(256) emit_big_kernel(const FrameDev f, const GaussRec *__restrict__ rec, const int32_t *__restrict__ radii,
                                                       const uint32_t *__restrict__ perm, const uint32_t *__restrict__ offsets,
                                                       KeyT *__restrict__ keys, uint32_t *__restrict__ vals,
                                                       const uint32_t *__restrict__ big_list, const uint32_t *__restrict__ big_count,
-                                                      const uint32_t cap) {
+                                                      const uint32_t cap, const Keep keep = Keep()) {
 	const uint32_t n = *big_count;
 	const uint32_t nwarps = gridDim.x * 8u;
 	const int lane = threadIdx.x & 31;
@@ -302,7 +316,8 @@ __global__ void __launch_bounds__(256) emit_big_kernel(const FrameDev f, const G
 		if (offsets[t] > cap) continue;  // bounded mode overflow (never deferred in practice: emit_pairs already skipped it)
 		// lane 0 carries the Gaussian through the cooperative path of visit_tiles (all other lanes inactive)
 		uint32_t count;
-		visit_tiles<true, KeyT>(lane == 0, x0, y0, x1, y1, cp, f.band, f.gx, gidx, off, keys, vals, count);
+		visit_tiles<true, KeyT, Keep>(lane == 0, x0, y0, x1, y1, cp, f.band, f.gx, gidx, off, keys, vals, count, nullptr, nullptr, 0u, 0u, 0u,
+		                              nullptr, nullptr, 0u, keep);
 	}
 }
 
@@ -344,16 +359,22 @@ __global__ void __launch_bounds__(256) tile_ranges_kernel(int64_t L, const KeyT 
 	}
 }
 
+// number of leading depth-order slots whose inclusive offset is <= limit (offsets ascend)
+__device__ __forceinline__ int slots_within(const uint32_t *__restrict__ offsets, int n, uint32_t limit) {
+	int lo = 0, hi = n;  // first index with offsets[i] > limit
+	while (lo < hi) {
+		const int mid = (lo + hi) >> 1;
+		if (offsets[mid] > limit) hi = mid; else lo = mid + 1;
+	}
+	return lo;
+}
+
 // status words: [1] = R (true instance count), [2] = overflow flag, [3] = instances actually emitted (<= cap)
 __global__ void count_status_kernel(const uint32_t *__restrict__ offsets, int P, uint32_t cap, uint32_t *__restrict__ status) {
 	const uint32_t R = offsets[P - 1];
 	uint32_t emitted = R;
 	if (R > cap) {  // largest scanned offset that still fits: Gaussians are emitted in depth order, the tail is dropped
-		int lo = 0, hi = P;  // first index with offsets[i] > cap
-		while (lo < hi) {
-			const int mid = (lo + hi) >> 1;
-			if (offsets[mid] > cap) hi = mid; else lo = mid + 1;
-		}
+		const int lo = slots_within(offsets, P, cap);
 		emitted = lo == 0 ? 0u : offsets[lo - 1];
 	}
 	status[1] = R;
@@ -726,6 +747,141 @@ cudaError_t launch_binning(const FrameDev &f, GeomView g, const int32_t *radii, 
 		tile_ranges_kernel<uint32_t><<<(unsigned)((R + 256 * kRangeKeysPerThread - 1) / (256 * kRangeKeysPerThread)), 256, 0, st>>>(R, b.keys_out, img.ranges, (uint32_t)ntile);
 	}
 	return cudaGetLastError();
+}
+
+// ---- saturation split: near pass, blend, far pass (include/sgr.h sgr_set_near_budget, DESIGN.md §7) ----
+// Most instances of a frame lie behind the point where every pixel of their tile has saturated (T < 1e-4): the blend never reads
+// them.  The split emits and buckets the nearest Gaussians first (those whose depth-order offsets stay within the budget B), blends
+// those lists (blend_fwd.cu, kBlendNear), and emits the remaining Gaussians only into the tiles that pass left unsaturated.  The
+// emitted sequence is near ++ far, both in depth order, so one stable bucketing of [0, E) gives every unsaturated tile exactly the
+// list of the unsplit binning and every saturated tile its near part; kBlendResume finishes the unsaturated tiles from the stored
+// per-pixel state.  Images, n_contrib and tile_max_contrib do not depend on B.
+
+// one thread: the split.  fit = Gaussians whose whole instance counts fit the capacity (all unless the bounded mode can overflow);
+// B = the budget (budget < 0: R / kNearBudgetDivisor), clamped to what fits; K = Gaussians whose inclusive offset is <= B.  The near
+// block's word 3 = its end in the emitted sequence, as the bucketing reads it.  Words 2 and 3 are settled by split_total_kernel.
+__global__ void split_status_kernel(const uint32_t *__restrict__ offsets, int n, uint32_t cap, long long budget, uint32_t *__restrict__ status) {
+	const uint32_t R = offsets[n - 1];
+	const int fit = R > cap ? slots_within(offsets, n, cap) : n;
+	const uint32_t fit_end = fit == 0 ? 0u : offsets[fit - 1];
+	uint32_t B = budget < 0 ? R / kNearBudgetDivisor : (uint32_t)min(budget, 0xffffffffll);
+	B = min(B, fit_end);
+	const int K = slots_within(offsets, fit, B);
+	status[1] = R;
+	status[kStatusNear] = 0u;
+	status[kStatusNear + 3] = K == 0 ? 0u : offsets[K - 1];
+	status[kStatusSplitK] = (uint32_t)K;
+	status[kStatusSplitFit] = (uint32_t)fit;
+}
+
+// thread t = t-th Gaussian in depth order: its instance count in the emitted sequence.  Near Gaussians keep their scanned count;
+// a far one counts the tiles of its rectangle that the near blend left unsaturated, by the code emit_pairs / emit_big run.
+__global__ void __launch_bounds__(256) far_count_kernel(const FrameDev f, const GaussRec *__restrict__ rec, const int32_t *__restrict__ radii,
+                                                       const uint32_t *__restrict__ perm, const uint32_t *__restrict__ offsets,
+                                                       const uint32_t *__restrict__ status, const int n_order,
+                                                       const KeepUnsaturated keep, uint32_t *__restrict__ cnt) {
+	const int t = blockIdx.x * blockDim.x + threadIdx.x;
+	const int K = (int)status[kStatusSplitK];
+	bool active = false;
+	int x0 = 0, y0 = 0, x1 = 0, y1 = 0;
+	CullParams cp = {};
+	uint32_t c = 0u;
+	if (t < n_order) {
+		const uint32_t off = t == 0 ? 0u : offsets[t - 1], end = offsets[t];
+		if (t < K) {
+			c = end - off;
+		} else if (end > off) {
+			const uint32_t gidx = perm[t];
+			const float4 q0 = rec[gidx].q0, q1 = rec[gidx].q1;
+			tile_rect(q0.x, q0.y, radii[gidx], f.gx, f.gy, x0, y0, x1, y1);
+			cp = make_cull(q0.x, q0.y, q0.z, q0.w, q1.x, q1.y);
+			active = true;
+		}
+	}
+	uint32_t count = 0u;
+	visit_tiles<false, uint16_t, KeepUnsaturated>(active, x0, y0, x1, y1, cp, f.band, f.gx, 0u, 0u, nullptr, nullptr, count, nullptr, nullptr,
+	                                              0u, 0u, 0u, nullptr, nullptr, 0u, keep);
+	if (t < n_order) cnt[t] = active ? count : c;
+}
+
+// one warp per tile row, after the near blend: prefix[ty * (gx + 1) + tx] = unsaturated tiles (top bit of tile_max_contrib) before
+// column tx, for KeepUnsaturated.  prefix lives in the img ranges, which are free from the near blend until the final bucketing.
+__global__ void __launch_bounds__(32) unsat_prefix_kernel(const uint32_t *__restrict__ tile_word, const int gx, uint32_t *__restrict__ prefix) {
+	const int ty = blockIdx.x, lane = threadIdx.x;
+	uint32_t *row = prefix + (size_t)ty * (gx + 1);
+	uint32_t carry = 0u;
+	for (int t0 = 0; t0 < gx; t0 += 32) {
+		const int tx = t0 + lane;
+		const bool u = tx < gx && (tile_word[(size_t)ty * gx + tx] >> 31) != 0u;
+		const unsigned m = __ballot_sync(0xffffffffu, u);
+		if (tx < gx) row[tx] = carry + (uint32_t)__popc(m & ((1u << lane) - 1u));
+		carry += (uint32_t)__popc(m);
+	}
+	if (lane == 0) row[gx] = carry;
+}
+
+// one thread, after the scan of far_count_kernel's counts: E = the instances emitted.  A bounded frame overflows only if the emitted
+// sequence exceeds the capacity; it then keeps the Gaussians whose whole instance counts fit (split_status_kernel's `fit`), as the
+// one-pass binning does, so that an overflowing frame is the same whatever the budget.  The far emission reads E as its cap.
+__global__ void split_total_kernel(const uint32_t *__restrict__ offsets, int n, uint32_t cap, uint32_t *__restrict__ status) {
+	const uint32_t total = offsets[n - 1];
+	if (total <= cap) {
+		status[3] = total;
+	} else {
+		const int fit = (int)status[kStatusSplitFit];
+		status[3] = fit == 0 ? 0u : offsets[fit - 1];
+		status[2] |= 1u;
+	}
+}
+
+bool split_applies(const FrameDev &f) {
+	return f.S == 0 && f.band.begin == 0 && f.band.end == f.gy && f.band.step == 1 && f.gx * f.gy <= kBucketMaxTiles &&
+	       (uint32_t)f.P <= kPackMask + 1u;
+}
+
+// near pass: split, emit the Gaussians before it into [0, E_near), bucket them into vals_out / ranges.  slots = binning capacity.
+cudaError_t launch_near_binning(const FrameDev &f, GeomView g, const int32_t *radii, BinView b, ImgView img, int64_t slots, cudaStream_t st,
+                                int64_t cap, int n_order, int64_t budget) {
+	const uint32_t cap32 = cap >= 0 ? (uint32_t)cap : 0xffffffffu;
+	uint32_t *near = g.big_count + kStatusNear;
+	uint16_t *kin = reinterpret_cast<uint16_t *>(b.keys_in);
+	count_launch(3);
+	split_status_kernel<<<1, 1, 0, st>>>(g.offsets, n_order, cap32, (long long)budget, g.big_count);
+	emit_pairs_kernel<uint16_t><<<(unsigned)((n_order + 255) / 256), 256, 0, st>>>(f, g.rec, radii, g.tiles_touched, g.perm, g.offsets, kin,
+	                                                                               b.vals_in, g.big_list, near, cap32, n_order, near + 3);
+	emit_big_kernel<uint16_t><<<kNumSMs * 4, 256, 0, st>>>(f, g.rec, radii, g.perm, g.offsets, kin, b.vals_in, g.big_list, near, cap32);
+	cudaError_t e = cudaGetLastError();
+	if (e != cudaSuccess) return e;
+	return launch_bucketing(b, img, near, f.gx * f.gy, slots, st);
+}
+
+// far pass, after the near blend marked the unsaturated tiles: count, scan (into g.ckey; g.iota holds the counts — both are dead
+// after the depth sort of this forward), emit behind the near instances, and bucket the whole emitted sequence.
+cudaError_t launch_far_binning(const FrameDev &f, GeomView g, const int32_t *radii, BinView b, ImgView img, int64_t slots, cudaStream_t st,
+                               int64_t cap, int n_order) {
+	const uint32_t cap32 = cap >= 0 ? (uint32_t)cap : 0xffffffffu;
+	const unsigned nblk = (unsigned)((n_order + 255) / 256);
+	uint32_t *prefix = reinterpret_cast<uint32_t *>(img.ranges);  // (gx + 1) gy <= 2 (ntile + 1) words
+	const KeepUnsaturated keep{prefix, f.gx + 1};
+	uint32_t *far_offsets = g.ckey;
+	uint16_t *kin = reinterpret_cast<uint16_t *>(b.keys_in);
+	count_launch(2);
+	unsat_prefix_kernel<<<f.gy, 32, 0, st>>>(img.tile_max_contrib, f.gx, prefix);
+	far_count_kernel<<<nblk, 256, 0, st>>>(f, g.rec, radii, g.perm, g.offsets, g.big_count, n_order, keep, g.iota);
+	cudaError_t e = cudaGetLastError();
+	if (e != cudaSuccess) return e;
+	size_t bytes = g.temp_bytes;
+	if ((e = cub::DeviceScan::InclusiveSum(g.temp, bytes, g.iota, far_offsets, n_order, st)) != cudaSuccess) return e;
+	if ((e = cudaMemsetAsync(g.big_count, 0, sizeof(uint32_t), st)) != cudaSuccess) return e;
+	count_launch(3);
+	split_total_kernel<<<1, 1, 0, st>>>(far_offsets, n_order, cap32, g.big_count);
+	emit_pairs_kernel<uint16_t, KeepUnsaturated><<<nblk, 256, 0, st>>>(f, g.rec, radii, g.tiles_touched, g.perm, far_offsets, kin, b.vals_in,
+	                                                                   g.big_list, g.big_count, cap32, n_order, g.big_count + 3,
+	                                                                   g.big_count + kStatusNear + 3, keep);
+	emit_big_kernel<uint16_t, KeepUnsaturated><<<kNumSMs * 4, 256, 0, st>>>(f, g.rec, radii, g.perm, far_offsets, kin, b.vals_in, g.big_list,
+	                                                                        g.big_count, cap32, keep);
+	if ((e = cudaGetLastError()) != cudaSuccess) return e;
+	return launch_bucketing(b, img, g.big_count, f.gx * f.gy, slots, st);
 }
 
 }  // namespace sgr

@@ -15,6 +15,11 @@
 //     expf for pairs that cannot reach alpha >= 1/255;
 //   * semantics are accumulated in registers and written once (the reference does a global read-modify-write per
 //     contribution, forward.cu:442-444).
+// Saturation split (binning.cu): PASS = kBlendNear blends the near lists; a tile whose inside pixels all saturated is final, any
+// other one parks its per-pixel state (C and weight / depth sums in the output images, last contributor in n_contrib, T with the
+// `done` bit as its sign in blend_T) and marks itself by the top bit of tile_max_contrib over its near count.  PASS = kBlendResume
+// runs on those tiles only, over the final list from that position on.  The state round-trips bit for bit and the per-pixel loop
+// does not depend on where batches start, so every output equals the one-pass blend's.
 #include "sgr_common.cuh"
 
 namespace sgr {
@@ -31,13 +36,15 @@ __device__ __forceinline__ void sts128(uint32_t addr, float4 v) {
 	asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
 
-template <int SCH>
+template <int SCH, int PASS = kBlendFull>
 __global__ void __launch_bounds__(256) blend_fwd_kernel(const FrameDev f, const uint2 *__restrict__ ranges,
                                                         const uint32_t *__restrict__ point_list, const GaussRec *__restrict__ rec,
                                                         const float *__restrict__ semantics, uint32_t *__restrict__ n_contrib,
                                                         uint32_t *__restrict__ tile_max_contrib, float *__restrict__ out_color,
                                                         float *__restrict__ out_depth, float *__restrict__ out_alpha,
-                                                        float *__restrict__ out_sem, const int sem_ch0, const int sem_only) {
+                                                        float *__restrict__ out_sem, const int sem_ch0, const int sem_only,
+                                                        float *__restrict__ blend_T) {
+	static_assert(PASS == kBlendFull || SCH == 0, "the split passes carry no semantic channels");
 	__shared__ __align__(16) unsigned char s_rec[2][kFwdBatch * kRecBytes];  // 2 x 12 KB: GaussRec per list slot
 	__shared__ uint32_t s_id[SCH > 0 ? 2 : 1][SCH > 0 ? kFwdBatch : 1];
 	__shared__ uint32_t s_max;
@@ -52,8 +59,14 @@ __global__ void __launch_bounds__(256) blend_fwd_kernel(const FrameDev f, const 
 	const size_t pix_id = (size_t)f.W * py + px;
 	const float2 pixf = make_float2((float)px, (float)py);
 
+	uint32_t start = 0u;  // first list position blended here (kBlendResume: the tile's near count)
+	if (PASS == kBlendResume) {
+		const uint32_t w = tile_max_contrib[tile];
+		if (!(w >> 31)) return;  // saturated in the near pass: its outputs are final
+		start = w & 0x7fffffffu;
+	}
 	const uint2 range = ranges[tile];
-	const int n = (int)(range.y - range.x);
+	const int n = (int)(range.y - range.x - start);
 	const int nb = (n + kFwdBatch - 1) / kFwdBatch;
 	if (tid == 0) s_max = 0;
 	__syncthreads();
@@ -68,13 +81,22 @@ __global__ void __launch_bounds__(256) blend_fwd_kernel(const FrameDev f, const 
 	for (int c = 0; c < (SCH > 0 ? SCH : 1); c++) sem[c] = 0.f;
 	const int nsem = SCH > 0 ? min(SCH, f.S - sem_ch0) : 0;
 	uint32_t last_contributor = 0;
+	if (PASS == kBlendResume && inside) {
+		const uint32_t tb = __float_as_uint(blend_T[pix_id]);
+		done = (tb >> 31) != 0u;
+		T = __uint_as_float(tb & 0x7fffffffu);
+		C0 = out_color[pix_id]; C1 = out_color[HW + pix_id]; C2 = out_color[2 * HW + pix_id];
+		weight = out_alpha[pix_id];
+		Dacc = out_depth[pix_id];
+		last_contributor = n_contrib[pix_id];
+	}
 
 	float4 r0 = make_float4(0, 0, 0, 0), r1 = r0, r2 = r0;
 	uint32_t rid = 0;
 	auto fetch = [&](int b) {
 		const int k = b * kFwdBatch + tid;
 		if (k < n) {
-			rid = point_list[range.x + k];
+			rid = point_list[range.x + start + k];
 			const GaussRec *p = rec + rid;
 			r0 = p->q0; r1 = p->q1; r2 = p->q2;
 		}
@@ -126,10 +148,23 @@ __global__ void __launch_bounds__(256) blend_fwd_kernel(const FrameDev f, const 
 			T = test_T;
 			a_last = a;
 		}
-		if (a_last != 0xffffffffu) last_contributor = (uint32_t)(b * kFwdBatch) + (a_last - a0) / kRecBytes + 1u;
+		if (a_last != 0xffffffffu) last_contributor = start + (uint32_t)(b * kFwdBatch) + (a_last - a0) / kRecBytes + 1u;
 		if (b + 1 < nb) stash((b + 1) & 1);
 	}
 
+	if (PASS == kBlendNear && __syncthreads_count(done) != SGR_TILE_PIX) {  // unsaturated: park the state for kBlendResume
+		if (inside) {
+			n_contrib[pix_id] = last_contributor;
+			out_color[pix_id] = C0;
+			out_color[HW + pix_id] = C1;
+			out_color[2 * HW + pix_id] = C2;
+			out_alpha[pix_id] = weight;
+			out_depth[pix_id] = Dacc;
+			blend_T[pix_id] = __uint_as_float(__float_as_uint(T) | (done ? 0x80000000u : 0u));
+		}
+		if (tid == 0) tile_max_contrib[tile] = 0x80000000u | (uint32_t)n;
+		return;
+	}
 	if (inside) {
 		if (!sem_only) {
 			n_contrib[pix_id] = last_contributor;
@@ -155,14 +190,24 @@ __global__ void __launch_bounds__(256) blend_fwd_kernel(const FrameDev f, const 
 }
 
 cudaError_t launch_blend_fwd(const FrameDev &f, GeomView g, BinView b, ImgView img, const float *semantics, float *out_color,
-                             float *out_depth, float *out_alpha, float *out_sem, cudaStream_t st) {
+                             float *out_depth, float *out_alpha, float *out_sem, cudaStream_t st, BlendPass pass) {
 	const int rows = band_rows(f.band);
 	if (rows <= 0 || f.gx <= 0) return cudaSuccess;
 	const dim3 grid(f.gx, rows);
 	count_launch();
+	if (pass != kBlendFull && f.S > 0) return cudaErrorInvalidValue;
+	if (pass == kBlendNear || pass == kBlendResume) {
+		if (pass == kBlendNear)
+			blend_fwd_kernel<0, kBlendNear><<<grid, 256, 0, st>>>(f, img.ranges, b.vals_out, g.rec, nullptr, img.n_contrib, img.tile_max_contrib,
+			                                                      out_color, out_depth, out_alpha, nullptr, 0, 0, img.blend_T);
+		else
+			blend_fwd_kernel<0, kBlendResume><<<grid, 256, 0, st>>>(f, img.ranges, b.vals_out, g.rec, nullptr, img.n_contrib, img.tile_max_contrib,
+			                                                        out_color, out_depth, out_alpha, nullptr, 0, 0, img.blend_T);
+		return cudaGetLastError();
+	}
 #define SGR_LAUNCH_FWD(SCH, ch0, only)                                                                                        \
 	blend_fwd_kernel<SCH><<<grid, 256, 0, st>>>(f, img.ranges, b.vals_out, g.rec, semantics, img.n_contrib,                     \
-	                                            img.tile_max_contrib, out_color, out_depth, out_alpha, out_sem, ch0, only)
+	                                            img.tile_max_contrib, out_color, out_depth, out_alpha, out_sem, ch0, only, nullptr)
 	if (f.S <= 0)
 		SGR_LAUNCH_FWD(0, 0, 0);
 	else if (f.S <= 4)

@@ -12,6 +12,7 @@
 namespace sgr {
 
 static thread_local char g_err[512] = "";
+static thread_local int64_t g_near_budget = SGR_NEAR_BUDGET_AUTO;  // sgr_set_near_budget
 std::atomic<uint64_t> g_kernel_launches{0};
 
 // cub's temp-storage size queries (two per carve_geom, two per carve_bin) walk cub's dispatch layer every time; every C-ABI
@@ -64,13 +65,15 @@ GeomView carve_geom(void *base, int P) {
 	g.total_bytes = (size_t)(p - reinterpret_cast<char *>(base));
 	return g;
 }
-ImgView carve_img(void *base, int W, int H) {
+// blend_state: the per-pixel T of the saturation split (forward img states; a layer's img has none)
+ImgView carve_img(void *base, int W, int H, bool blend_state) {
 	ImgView v;
 	char *p = reinterpret_cast<char *>(base);
 	const size_t gx = (W + SGR_TILE - 1) / SGR_TILE, gy = (H + SGR_TILE - 1) / SGR_TILE;
 	v.ranges = take<uint2>(p, gx * gy + 1);
 	v.tile_max_contrib = take<uint32_t>(p, gx * gy + 1);
 	v.n_contrib = take<uint32_t>(p, (size_t)W * H + 1);
+	v.blend_T = blend_state ? take<float>(p, (size_t)W * H) : nullptr;
 	v.total_bytes = (size_t)(p - reinterpret_cast<char *>(base));
 	return v;
 }
@@ -207,6 +210,11 @@ using namespace sgr;
 extern "C" {
 
 int sgr_abi_version(void) { return SGR_ABI_VERSION; }
+int64_t sgr_set_near_budget(int64_t budget) {
+	const int64_t prev = g_near_budget;
+	g_near_budget = budget < 0 ? SGR_NEAR_BUDGET_AUTO : budget;
+	return prev;
+}
 uint64_t sgr_launch_count(void) { return g_kernel_launches.load(std::memory_order_relaxed); }
 const char *sgr_last_error(void) { return g_err; }
 
@@ -288,6 +296,17 @@ static int forward_impl(const SgrFrame *frame, const float *means3D, const float
 		if (binning_state) *binning_state = bin;
 	}
 	if (num_instances) *num_instances = R;
+	// Saturation split (binning.cu): whole-image frames that bucket and carry no semantic channels; a budget that covers every
+	// instance the binning can hold is the one-pass binning.  The records path is the tile-row-sharded mode and keeps the latter.
+	const int64_t budget = g_near_budget;
+	if (!from_records && f.P > 0 && R > 0 && split_applies(f) && (budget < 0 || budget < R)) {
+		const int64_t cap = bounded ? capacity : -1;
+		SGR_TRY(launch_near_binning(f, g, radii, b, img, R, st, cap, n_order, budget), "near binning");
+		SGR_TRY(launch_blend_fwd(f, g, b, img, nullptr, out_color, out_depth, out_alpha, nullptr, st, kBlendNear), "near blend_fwd");
+		SGR_TRY(launch_far_binning(f, g, radii, b, img, R, st, cap, n_order), "far binning");
+		SGR_TRY(launch_blend_fwd(f, g, b, img, nullptr, out_color, out_depth, out_alpha, nullptr, st, kBlendResume), "resume blend_fwd");
+		return SGR_OK;
+	}
 	SGR_TRY(launch_binning(f, g, radii, b, img, R, st, bounded ? capacity : -1, n_order), "binning");
 	SGR_TRY(launch_blend_fwd(f, g, b, img, semantics, out_color, out_depth, out_alpha, out_semantic, st), "blend_fwd");
 	return SGR_OK;
@@ -623,7 +642,7 @@ struct LayerView {
 };
 static LayerView carve_layer(void *base, int W, int H, int64_t R) {
 	LayerView v;
-	v.img = carve_img(base, W, H);
+	v.img = carve_img(base, W, H, false);
 	char *p = reinterpret_cast<char *>(base) + v.img.total_bytes;
 	v.list = take<uint32_t>(p, R > 0 ? (size_t)R : 1);
 	v.total_bytes = (size_t)(p - reinterpret_cast<char *>(base));

@@ -4,7 +4,7 @@
 //   geom state   : GaussRec[P] (48 B packed record, 3 x float4 — one 16-B aligned gather of 3 vectors per splat
 //                  instance in the blend passes), then tiles_touched / depth_key / iota / depth_sorted / perm / offsets
 //                  (u32[P] each) and cub temp storage.
-//   img state    : ranges uint2[Ntile], n_contrib u32[H*W], block-max n_contrib u32[Ntile]
+//   img state    : ranges uint2[Ntile], n_contrib u32[H*W], block-max n_contrib u32[Ntile], blend state f32[H*W] (saturation split)
 //   binning state: keys_in u32[R], keys_out u32[R] (tile ids), vals_in u32[R], vals_out u32[R] (= tile-ordered,
 //                  depth-sorted point list), sort temp, tile-bucketing scratch
 #pragma once
@@ -43,8 +43,10 @@ struct GeomView {
 	uint32_t *big_count;      // status words, zeroed per forward: [0] number of entries in big_list (device counter)
 	                          // [1] instance count R, [2] overflow bits (1 = instance capacity, 2 = Gaussian capacity of the compacted
 	                          // depth order), [3] instances actually emitted (bounded mode), [4] Gaussians with instances (compacted mode)
+	                          // [8..13] saturation split (kStatusNear ...)
 	float4 *jac;              // per Gaussian with SH colour: 3 float4, d colour / d view direction + clamp bits (gaussian_geom.cuh)
-	uint32_t *ckey, *cval;    // compacted depth-sort input (keys / Gaussian indices), Gaussian-sharded forward only
+	uint32_t *ckey, *cval;    // compacted depth-sort input (keys / Gaussian indices), Gaussian-sharded forward only; the saturation
+	                          // split's far offsets live in ckey (and its far counts in iota, dead after the depth sort)
 	void *temp;               // cub temp storage: max(scan, depth sort)
 	size_t temp_bytes;
 	size_t total_bytes;
@@ -53,8 +55,17 @@ struct ImgView {
 	uint2 *ranges;
 	uint32_t *n_contrib;
 	uint32_t *tile_max_contrib;
+	float *blend_T;  // saturation split: T of each pixel of an unsaturated tile between the near blend and its resumption (sign = done)
 	size_t total_bytes;
 };
+
+// Saturation split (binning.cu launch_near_binning / launch_far_binning, blend_fwd.cu kBlendNear / kBlendResume): status words
+// kStatusNear.. = the near pass's block as the emission and bucketing read it ([+0] its big-list counter, [+3] its end E_near in the
+// emitted sequence); kStatusSplitK = Gaussians of the near pass (depth order), kStatusSplitFit = Gaussians that fit the capacity.
+constexpr int kStatusNear = 8, kStatusSplitK = 12, kStatusSplitFit = 13;
+// the near budget when the caller sets none: R / kNearBudgetDivisor instances (DESIGN.md §7, sweep on config C)
+constexpr uint32_t kNearBudgetDivisor = 8;
+enum BlendPass { kBlendFull = 0, kBlendNear = 1, kBlendResume = 2 };
 struct BinView {
 	uint32_t *keys_in, *keys_out;  // tile ids
 	uint32_t *vals_in, *vals_out;  // Gaussian indices; vals_out is the tile-ordered, depth-sorted point list
@@ -226,7 +237,7 @@ __device__ __forceinline__ CullParams make_cull(float mx, float my, float a, flo
 }
 // state carving (host) — implemented in capi.cu
 GeomView carve_geom(void *base, int P);
-ImgView carve_img(void *base, int W, int H);
+ImgView carve_img(void *base, int W, int H, bool blend_state = true);
 BinView carve_bin(void *base, int64_t R);
 
 // kernel launchers (host) — one per translation unit
@@ -340,8 +351,16 @@ size_t bucket_scratch_bytes(int64_t R);
 // slots and the true count lives in g.big_count[1..3].
 cudaError_t launch_binning(const FrameDev &f, GeomView g, const int32_t *radii, BinView b, ImgView img, int64_t R,
                            cudaStream_t st, int64_t cap = -1, int n_order = -1);
+// saturation split: whether a forward of this frame can take it (whole image, tile bucketing, no semantic channels), then its passes.
+// near: split + near emission + bucketing; far (after launch_blend_fwd kBlendNear): far count / emission + the final bucketing.
+bool split_applies(const FrameDev &f);
+cudaError_t launch_near_binning(const FrameDev &f, GeomView g, const int32_t *radii, BinView b, ImgView img, int64_t slots, cudaStream_t st,
+                                int64_t cap, int n_order, int64_t budget);
+cudaError_t launch_far_binning(const FrameDev &f, GeomView g, const int32_t *radii, BinView b, ImgView img, int64_t slots, cudaStream_t st,
+                               int64_t cap, int n_order);
+// pass != kBlendFull needs f.S == 0
 cudaError_t launch_blend_fwd(const FrameDev &f, GeomView g, BinView b, ImgView img, const float *semantics, float *out_color,
-                             float *out_depth, float *out_alpha, float *out_sem, cudaStream_t st);
+                             float *out_depth, float *out_alpha, float *out_sem, cudaStream_t st, BlendPass pass = kBlendFull);
 cudaError_t launch_blend_bwd(const FrameDev &f, GeomView g, BinView b, ImgView img, const float *semantics,
                              const float *out_alpha, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
                              const float *dL_dsem, float *grad2d, float *dL_dsemantics, cudaStream_t st, bool grad2d_zeroed = false);

@@ -88,13 +88,33 @@ __device__ __forceinline__ void row_span(const CullParams cp, const EllipseAux e
 	if (xe < xb) xe = xb;
 }
 
-template <bool EMIT, typename KeyT = uint32_t>
+// Tile predicates of visit_tiles: which of the culled tiles are counted / emitted.  span(ty, xb, xe) = kept tiles among columns
+// [xb, xe) of tile row ty, tile(ty, tx) = whether one is kept.
+struct KeepAll {  // every tile (one binning pass per frame)
+	static constexpr bool kAll = true;
+	__device__ __forceinline__ uint32_t span(int, int xb, int xe) const { return (uint32_t)(xe - xb); }
+	__device__ __forceinline__ bool tile(int, int) const { return true; }
+};
+// Far pass of the saturation split (binning.cu): only the tiles the near pass left unsaturated.  prefix[ty * (gx + 1) + tx] = number
+// of unsaturated tiles before column tx of row ty (unsat_prefix_kernel), so a row span costs two loads, as KeepAll's costs none.
+struct KeepUnsaturated {
+	static constexpr bool kAll = false;
+	const uint32_t *prefix;
+	int stride;  // gx + 1
+	__device__ __forceinline__ uint32_t span(int ty, int xb, int xe) const {
+		const uint32_t *row = prefix + (size_t)ty * stride;
+		return xe > xb ? row[xe] - row[xb] : 0u;
+	}
+	__device__ __forceinline__ bool tile(int ty, int tx) const { return span(ty, tx, tx + 1) != 0u; }
+};
+
+template <bool EMIT, typename KeyT = uint32_t, typename Keep = KeepAll>
 __device__ __forceinline__ void visit_tiles(bool active, int x0, int y0, int x1, int y1, const CullParams cp, const Band band,
                                             int gx, uint32_t gauss_idx, uint32_t offset, KeyT *__restrict__ keys,
                                             uint32_t *__restrict__ vals, uint32_t &count, KeyT *stage_keys = nullptr,
                                             uint32_t *stage_vals = nullptr, uint32_t stage_cap = 0, uint32_t warp_first = 0,
                                             uint32_t warp_total = 0, uint32_t *big_list = nullptr, uint32_t *big_count = nullptr,
-                                            uint32_t big_tag = 0) {
+                                            uint32_t big_tag = 0, const Keep keep = Keep()) {
 	const unsigned full = 0xffffffffu;
 	const int lane = threadIdx.x & 31;
 	if (active) {
@@ -134,21 +154,24 @@ __device__ __forceinline__ void visit_tiles(bool active, int x0, int y0, int x1,
 			int xb, xe;
 			row_span(cp, ea, ty, x0, x1, xb, xe);
 			if (EMIT) {
+				if (!Keep::kAll && keep.span(ty, xb, xe) == 0u) continue;
 				if (staged) {
 					for (int tx = xb; tx < xe; tx++) {
+						if (!Keep::kAll && !keep.tile(ty, tx)) continue;
 						stage_keys[off - warp_first] = (KeyT)(ty * gx + tx);
 						stage_vals[off - warp_first] = gauss_idx;
 						off++;
 					}
 				} else {
 					for (int tx = xb; tx < xe; tx++) {
+						if (!Keep::kAll && !keep.tile(ty, tx)) continue;
 						keys[off] = (KeyT)(ty * gx + tx);
 						vals[off] = gauss_idx;
 						off++;
 					}
 				}
 			} else {
-				off += (uint32_t)(xe - xb);
+				off += keep.span(ty, xb, xe);
 			}
 		}
 		count = off - offset;
@@ -177,7 +200,7 @@ __device__ __forceinline__ void visit_tiles(bool active, int x0, int y0, int x1,
 			const int ty = r0 + lane;
 			int xb = 0, xe = 0;
 			if (ty < sy1 && band_owns(band, ty)) row_span(c2, ea2, ty, sx0, sx1, xb, xe);
-			const uint32_t n = (uint32_t)(xe - xb);
+			const uint32_t n = keep.span(ty, xb, xe);
 			uint32_t incl = n;  // inclusive warp scan of the per-row counts
 #pragma unroll
 			for (int o = 1; o < 32; o <<= 1) {
@@ -190,9 +213,24 @@ __device__ __forceinline__ void visit_tiles(bool active, int x0, int y0, int x1,
 					const int rxb = __shfl_sync(full, xb, r), rxe = __shfl_sync(full, xe, r);
 					const uint32_t rbase = base + __shfl_sync(full, incl - n, r);
 					const uint32_t tile0 = (uint32_t)((r0 + r) * gx);
-					for (int tx = rxb + lane; tx < rxe; tx += 32) {
-						keys[rbase + (uint32_t)(tx - rxb)] = (KeyT)(tile0 + (uint32_t)tx);
-						vals[rbase + (uint32_t)(tx - rxb)] = sidx;
+					if (Keep::kAll) {
+						for (int tx = rxb + lane; tx < rxe; tx += 32) {
+							keys[rbase + (uint32_t)(tx - rxb)] = (KeyT)(tile0 + (uint32_t)tx);
+							vals[rbase + (uint32_t)(tx - rxb)] = sidx;
+						}
+					} else {  // kept tiles of the row, compacted in ascending column order
+						uint32_t pos = rbase;
+						for (int t0 = rxb; t0 < rxe; t0 += 32) {
+							const int tx = t0 + lane;
+							const bool k = tx < rxe && keep.tile(r0 + r, tx);
+							const unsigned m = __ballot_sync(full, k);
+							if (k) {
+								const uint32_t q = pos + (uint32_t)__popc(m & ((1u << lane) - 1u));
+								keys[q] = (KeyT)(tile0 + (uint32_t)tx);
+								vals[q] = sidx;
+							}
+							pos += (uint32_t)__popc(m);
+						}
 					}
 				}
 			}

@@ -14,6 +14,7 @@ All arithmetic happens in libsgr.so (hand-written CUDA, sm_90a) through include/
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 from typing import NamedTuple, Optional, Tuple
 
@@ -422,8 +423,10 @@ class _RasterizeGaussians(torch.autograd.Function):
                 raster_settings, band=None, grad_reduce=None, capacity=None, layers=(), *sinks):
         # with layers an output without upstream gradient arrives as None, so a layer without one costs nothing in backward
         ctx.set_materialize_grads(not layers)
-        color, radii, depth, alpha, semantic, st, tensors = _forward_or_dump(means3D, sh, colors_precomp, semantics, opacities, scales,
-                                                                             rotations, cov3Ds_precomp, raster_settings, band, capacity)
+        # the layers are compacted out of the main call's tile lists: those must hold every instance (one binning pass)
+        with _capi.near_budget(_capi.NEAR_BUDGET_ALL) if layers else contextlib.nullcontext():
+            color, radii, depth, alpha, semantic, st, tensors = _forward_or_dump(means3D, sh, colors_precomp, semantics, opacities, scales,
+                                                                                 rotations, cov3Ds_precomp, raster_settings, band, capacity)
         bgs, states, layer_outs = (_forward_layers(raster_settings, st, tensors, int(means3D.shape[0]), means3D.device, layers)
                                    if layers else ((), (), []))
         ctx.raster_settings, ctx.band, ctx.state, ctx.grad_reduce = raster_settings, band, st, grad_reduce
