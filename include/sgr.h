@@ -576,6 +576,31 @@ int sgr_band_lidar_grad(int32_t H, int32_t W, int32_t row_begin, int32_t row_end
                         const float *lidar_depth, float weight, const SgrLidarState *state, const double *sums, float *dL_ddepth,
                         float *dL_dacc, float *scalars, void *scratch, size_t scratch_bytes, void *stream);
 
+/* ---- The sky composite and the colour correction on a tile-row band (the stages between the rasterizer and the losses) ----
+ * The band and the buffers as in the band losses above: every image argument is a whole [.., H, W] frame of which only the band's pixels
+ * are read and written (the caller zeroes the other rows where it needs zeros); sky_mask and the jitters are whole frames.  Each pixel is
+ * indexed by its global row and column, so the band's rows of every output equal those of the whole-frame call bit for bit.  Grid sizes
+ * depend on H, W (and R) and the band only; nothing is read back to the host.
+ * Sky: the arguments of sgr_sky_composite_forward / _backward.  dL_dcube is ADDED to and receives this band's partial sum; the caller
+ * sums it over the ranks (its texels' float atomics make it equal to the whole-frame dL_dcube up to their order).
+ * Colour correction: the backward writes the band's dL_dimage rows (may be NULL) and partials[12] (device doubles, row-major like the
+ * affine) = the band's sums dL_dout_i [image_j, 1], accumulated in double in a fixed order.  The caller sums partials over the ranks,
+ * then sgr_band_color_correct_affine_grad rounds the sums to the fp32 dL_daffine[3,4].  scratch: sgr_band_color_correct_scratch_bytes(H, W)
+ * bytes (0 for a bad size).  H W < 2^31. */
+int sgr_band_sky_composite_forward(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t R, int32_t mode, float fill,
+                                   const float *rgb, const float *acc, const uint8_t *sky_mask, const float *cube_map, const float *K,
+                                   const float *w2c, const float *jitter_x, const float *jitter_y, float *rgb_out, void *stream);
+int sgr_band_sky_composite_backward(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t R, int32_t mode, float fill,
+                                    const float *acc, const uint8_t *sky_mask, const float *cube_map, const float *K, const float *w2c,
+                                    const float *jitter_x, const float *jitter_y, const float *dL_dout, float *dL_dacc, float *dL_dcube,
+                                    void *stream);
+int sgr_band_color_correct_forward(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *image, const float *affine,
+                                   float *out, void *stream);
+size_t sgr_band_color_correct_scratch_bytes(int32_t H, int32_t W);
+int sgr_band_color_correct_backward(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *image, const float *affine,
+                                    const float *dL_dout, float *dL_dimage, double *partials, void *scratch, size_t scratch_bytes, void *stream);
+int sgr_band_color_correct_affine_grad(const double *sums, float *dL_daffine, void *stream);
+
 /* ---- Post-backward bookkeeping of a training iteration (SURVEY.md §8 row f3) ----
  * Densification statistics of StreetGaussianModel.set_max_radii2D + add_densification_stats
  * (lib/models/street_gaussian_model.py:551-571), all sub-models in one pass over the composed index space: for every Gaussian

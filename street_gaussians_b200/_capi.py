@@ -30,7 +30,9 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_set_nea
            "sgr_gaussian_normals_backward", "sgr_compose_semantics_forward", "sgr_compose_semantics_backward", "sgr_finish_features_forward",
            "sgr_finish_features_backward", "sgr_band_halo_rows", "sgr_band_halo_pack", "sgr_band_halo_unpack", "sgr_band_image_loss_stats",
            "sgr_band_image_loss_grad", "sgr_band_sky_loss", "sgr_band_obj_acc_loss", "sgr_band_acc_loss_value", "sgr_band_lidar_scratch_bytes",
-           "sgr_band_lidar_keys", "sgr_band_lidar_select", "sgr_band_lidar_grad"]
+           "sgr_band_lidar_keys", "sgr_band_lidar_select", "sgr_band_lidar_grad", "sgr_band_sky_composite_forward",
+           "sgr_band_sky_composite_backward", "sgr_band_color_correct_forward", "sgr_band_color_correct_scratch_bytes",
+           "sgr_band_color_correct_backward", "sgr_band_color_correct_affine_grad"]
 
 SKY_MASK_ACC, SKY_MASK_GIVEN = 0, 1
 SEMANTIC_LOGITS, SEMANTIC_PROBABILITIES = 0, 1
@@ -259,6 +261,18 @@ def lib():
     L.sgr_band_lidar_select.argtypes = [C.c_int32, C.c_double] + [C.c_int32] * 2 + band + [vp, vp, vp, C.c_size_t, vp]
     L.sgr_band_lidar_grad.restype = C.c_int
     L.sgr_band_lidar_grad.argtypes = [C.c_int32] * 2 + band + [vp] * 3 + [C.c_float] + [vp] * 5 + [vp, C.c_size_t, vp]
+    L.sgr_band_sky_composite_forward.restype = C.c_int
+    L.sgr_band_sky_composite_forward.argtypes = [C.c_int32] * 2 + band + [C.c_int32] * 2 + [C.c_float] + [vp] * 10
+    L.sgr_band_sky_composite_backward.restype = C.c_int
+    L.sgr_band_sky_composite_backward.argtypes = [C.c_int32] * 2 + band + [C.c_int32] * 2 + [C.c_float] + [vp] * 11
+    L.sgr_band_color_correct_forward.restype = C.c_int
+    L.sgr_band_color_correct_forward.argtypes = [C.c_int32] * 2 + band + [vp] * 4
+    L.sgr_band_color_correct_scratch_bytes.restype = C.c_size_t
+    L.sgr_band_color_correct_scratch_bytes.argtypes = [C.c_int32] * 2
+    L.sgr_band_color_correct_backward.restype = C.c_int
+    L.sgr_band_color_correct_backward.argtypes = [C.c_int32] * 2 + band + [vp] * 6 + [C.c_size_t, vp]
+    L.sgr_band_color_correct_affine_grad.restype = C.c_int
+    L.sgr_band_color_correct_affine_grad.argtypes = [vp] * 3
     L.sgr_densify_stats.restype = C.c_int
     L.sgr_densify_stats.argtypes = [C.POINTER(SgrStatSegment), C.c_int32, vp, vp, vp]
     L.sgr_adam_step.restype = C.c_int

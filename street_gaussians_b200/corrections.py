@@ -7,6 +7,10 @@ sgr_color_correct_forward / sgr_color_correct_backward / sgr_color_correction_re
 `affine` is the [3, 4] matrix ColorCorrection.get_affine_trans(camera) returns, in its embedding or its MLP mode (the MLP stays the
 caller's torch module; its output is differentiable like any other tensor).  The background pose correction is not here: pass its
 two rows to `compose(..., pose_correction=...)`.  CUDA tensors only: there is no CPU fallback.
+
+color_correct's band= / group= (keyword-only, as in losses.py): the image holds the rendered rows of this rank's TileRowBand
+(sharded.py); the band's rows are corrected (sgr_band_color_correct_*), and the backward all-reduces the band's 12 fp64 sums of
+dL/daffine over `group` before rounding them, so every rank's affine gradient is the whole frame's.
 """
 from __future__ import annotations
 
@@ -35,17 +39,25 @@ def _affine(a: torch.Tensor, what: str, dev) -> torch.Tensor:
 
 class _ColorCorrect(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, image, affine):
+    def forward(ctx, image, affine, band, group):
         _check_cuda(image, "image")
         img = _capi.f32(image)
         if img.dim() != 3 or img.shape[0] != 3:
             raise ValueError(f"image must be [3, H, W], got {tuple(image.shape)}")
         A = _affine(affine, "affine", img.device)
         H, W = int(img.shape[1]), int(img.shape[2])
-        out = torch.empty_like(img)
-        _capi.call("sgr_color_correct_forward", img.device, H, W, ptr(img), ptr(A), ptr(out))
+        if band is None:
+            rows = None
+            out = torch.empty_like(img)
+            _capi.call("sgr_color_correct_forward", img.device, H, W, ptr(img), ptr(A), ptr(out))
+        else:
+            from .band_losses import check_band
+            rows = check_band(band, H)
+            out = torch.zeros_like(img)
+            _capi.call("sgr_band_color_correct_forward", img.device, H, W, *rows, ptr(img), ptr(A), ptr(out))
         ctx.save_for_backward(img, A)
         ctx.dtypes = (image.dtype, affine.dtype)
+        ctx.band, ctx.group = rows, group
         return out
 
     @staticmethod
@@ -56,17 +68,38 @@ class _ColorCorrect(torch.autograd.Function):
         H, W = int(img.shape[1]), int(img.shape[2])
         _check_cuda(g_out, "dL/dout")
         g = _capi.f32(g_out)
-        g_img = torch.empty_like(img) if ctx.needs_input_grad[0] else None
         g_A = torch.empty((3, 4), device=dev, dtype=torch.float32)
-        nbytes = int(L.sgr_color_correct_scratch_bytes(H, W))
-        scratch = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-        _capi.call("sgr_color_correct_backward", dev, H, W, ptr(img), ptr(A), ptr(g), ptr(g_img), ptr(g_A), ptr(scratch), nbytes)
-        return (g_img.to(ctx.dtypes[0]) if g_img is not None else None), (g_A.to(ctx.dtypes[1]) if ctx.needs_input_grad[1] else None)
+        if ctx.band is None:
+            g_img = torch.empty_like(img) if ctx.needs_input_grad[0] else None
+            nbytes = int(L.sgr_color_correct_scratch_bytes(H, W))
+            scratch = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+            _capi.call("sgr_color_correct_backward", dev, H, W, ptr(img), ptr(A), ptr(g), ptr(g_img), ptr(g_A), ptr(scratch), nbytes)
+        else:
+            from .band_losses import all_reduce_sum
+            g_img = torch.zeros_like(img) if ctx.needs_input_grad[0] else None
+            sums = torch.empty(12, device=dev, dtype=torch.float64)
+            nbytes = int(L.sgr_band_color_correct_scratch_bytes(H, W))
+            scratch = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+            _capi.call("sgr_band_color_correct_backward", dev, H, W, *ctx.band, ptr(img), ptr(A), ptr(g), ptr(g_img), ptr(sums), ptr(scratch), nbytes)
+            if ctx.needs_input_grad[1]:  # COLLECTIVE: the band's 12 sums -> the frame's, rounded once to fp32
+                all_reduce_sum(sums, ctx.group)
+                _capi.call("sgr_band_color_correct_affine_grad", dev, ptr(sums), ptr(g_A))
+        return ((g_img.to(ctx.dtypes[0]) if g_img is not None else None), (g_A.to(ctx.dtypes[1]) if ctx.needs_input_grad[1] else None), None,
+                None)
 
 
-def color_correct(image: torch.Tensor, affine: torch.Tensor) -> torch.Tensor:
-    """einsum('ij,jhw->ihw', affine[:3, :3], image) + affine[:3, 3, None, None] for image [3, H, W]; differentiable in both."""
-    return _ColorCorrect.apply(image, affine)
+def color_correct(image: torch.Tensor, affine: torch.Tensor, *, band=None, group=None) -> torch.Tensor:
+    """einsum('ij,jhw->ihw', affine[:3, :3], image) + affine[:3, 3, None, None] for image [3, H, W]; differentiable in both.
+
+    band= / group=: image holds the rendered rows of this rank's TileRowBand (sharded.py).  The output and dL/dimage have the band's
+    rows, zeros elsewhere, equal bit for bit to the whole-frame call's rows.  COLLECTIVE in the backward: the 12 fp64 sums of
+    dL/daffine are all-reduced over `group` (every rank must run its backward), then rounded once, so dL/daffine is the frame's on
+    every rank and does not depend on how the rows are split (it may differ from the whole-frame call's fp32-accumulated sums by
+    their rounding).  An affine from the MLP mode works unchanged: its gradient flows back into the module as usual."""
+    if band is not None:  # a bad band fails before anything else
+        from .band_losses import check_band
+        check_band(band, int(image.shape[-2]))
+    return _ColorCorrect.apply(image, affine, band, group)
 
 
 class _Reg(torch.autograd.Function):

@@ -1308,6 +1308,78 @@ int sgr_band_lidar_grad(int32_t H, int32_t W, int32_t row_begin, int32_t row_end
 	return SGR_OK;
 }
 
+// ---- the sky composite and the colour correction on a tile-row band ----
+int sgr_band_sky_composite_forward(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t R, int32_t mode, float fill,
+                                   const float *rgb, const float *acc, const uint8_t *sky_mask, const float *cube_map, const float *K,
+                                   const float *w2c, const float *jitter_x, const float *jitter_y, float *rgb_out, void *stream) {
+	const char *fn = "sgr_band_sky_composite_forward";
+	Band band;
+	if (int rc = loss_band(fn, H, W, row_begin, row_end, row_step, &band)) return rc;
+	if (int rc = sky_check(fn, H, W, R, mode, sky_mask)) return rc;
+	if (!rgb || !acc || !cube_map || !K || !w2c || !rgb_out) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	if (!jitter_x != !jitter_y) return fail(SGR_EINVAL, "%s: give both jitters or neither", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_sky_composite_fwd(H, W, band, R, mode, fill, rgb, acc, sky_mask, cube_map, K, w2c, jitter_x, jitter_y, rgb_out, st), fn);
+	return SGR_OK;
+}
+
+int sgr_band_sky_composite_backward(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t R, int32_t mode, float fill,
+                                    const float *acc, const uint8_t *sky_mask, const float *cube_map, const float *K, const float *w2c,
+                                    const float *jitter_x, const float *jitter_y, const float *dL_dout, float *dL_dacc, float *dL_dcube,
+                                    void *stream) {
+	const char *fn = "sgr_band_sky_composite_backward";
+	Band band;
+	if (int rc = loss_band(fn, H, W, row_begin, row_end, row_step, &band)) return rc;
+	if (int rc = sky_check(fn, H, W, R, mode, sky_mask)) return rc;
+	if (!acc || !cube_map || !K || !w2c || !dL_dout) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	if (!jitter_x != !jitter_y) return fail(SGR_EINVAL, "%s: give both jitters or neither", fn);
+	if (!dL_dacc && !dL_dcube) return SGR_OK;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_sky_composite_bwd(H, W, band, R, mode, fill, acc, sky_mask, cube_map, K, w2c, jitter_x, jitter_y, dL_dout, dL_dacc, dL_dcube, st),
+	        fn);
+	return SGR_OK;
+}
+
+int sgr_band_color_correct_forward(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *image, const float *affine,
+                                   float *out, void *stream) {
+	const char *fn = "sgr_band_color_correct_forward";
+	Band band;
+	if (int rc = loss_band(fn, H, W, row_begin, row_end, row_step, &band)) return rc;
+	if (!image || !affine || !out) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_color_correct_fwd(H, W, band, image, affine, out, st), fn);
+	return SGR_OK;
+}
+
+size_t sgr_band_color_correct_scratch_bytes(int32_t H, int32_t W) {
+	return (H > 0 && W > 0 && (int64_t)H * W < ((int64_t)1 << 31)) ? color_correct_band_scratch_bytes(H, W) : 0;
+}
+
+int sgr_band_color_correct_backward(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *image, const float *affine,
+                                    const float *dL_dout, float *dL_dimage, double *partials, void *scratch, size_t scratch_bytes, void *stream) {
+	const char *fn = "sgr_band_color_correct_backward";
+	Band band;
+	if (int rc = loss_band(fn, H, W, row_begin, row_end, row_step, &band)) return rc;
+	if (!image || !affine || !dL_dout || !partials) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	if (!scratch || scratch_bytes < color_correct_band_scratch_bytes(H, W))
+		return fail(SGR_ENOMEM, "%s: scratch too small: %zu < %zu", fn, scratch_bytes, color_correct_band_scratch_bytes(H, W));
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_color_correct_bwd(H, W, band, image, affine, dL_dout, dL_dimage, partials, scratch, st), fn);
+	return SGR_OK;
+}
+
+int sgr_band_color_correct_affine_grad(const double *sums, float *dL_daffine, void *stream) {
+	if (!sums || !dL_daffine) return fail(SGR_EINVAL, "NULL pointer passed to sgr_band_color_correct_affine_grad");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_color_correct_affine_grad(sums, dL_daffine, st), "band_color_correct_affine_grad");
+	return SGR_OK;
+}
+
 int sgr_densify_stats(const SgrStatSegment *segments, int32_t num_segments, const int32_t *radii, const float *means2D_grad, void *stream) {
 	if (!segments || num_segments <= 0) return fail(SGR_EINVAL, "segment table is empty");
 	int64_t at = 0;

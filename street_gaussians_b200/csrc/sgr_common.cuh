@@ -171,6 +171,13 @@ __host__ __device__ __forceinline__ bool band_owns(const Band b, int row) {
 }
 // dense index of an owned row within the band (used to launch one CTA per owned tile)
 __host__ __device__ __forceinline__ int band_rows(const Band b) { return b.end > b.begin ? (b.end - b.begin + b.step - 1) / b.step : 0; }
+// Item t of the band's pixels in a [H, W] plane, the band_rows(b) * strip items of its tile rows in order (strip = the items of one
+// 16-row tile row): its index in the frame.  Items of the last tile row past the image's last row map to indices >= H W.
+constexpr int kBandTileRows = 16;
+__host__ __device__ __forceinline__ int64_t band_pixel(const int64_t t, const Band b, const int64_t strip) {
+	const int64_t k = t / strip;
+	return (int64_t)(b.begin + (int)k * b.step) * strip + (t - k * strip);
+}
 
 // ---- TMA bulk copies (cp.async.bulk, 1-D) + mbarrier: the Hopper (sm_90) way to move a contiguous row block between HBM and
 // shared memory without a register round trip.  SASS: UBLKCP (copy), SYNCS.ARRIVE.TRANS64 (expect_tx), SYNCS.PHASECHK (try_wait).
@@ -390,12 +397,24 @@ cudaError_t launch_color_correct_fwd(int64_t N, const float *image, const float 
 size_t color_correct_scratch_bytes(int64_t N);
 cudaError_t launch_color_correct_bwd(int64_t N, const float *image, const float *affine, const float *g_out, float *g_image, float *g_affine,
                                      void *scratch, cudaStream_t st);
+// the same on a tile-row band: the band's rows of out / g_image, and the band's 12 sums g_i [x_j, 1] accumulated in double into sums[12]
+cudaError_t launch_color_correct_fwd(int H, int W, Band band, const float *image, const float *affine, float *out, cudaStream_t st);
+size_t color_correct_band_scratch_bytes(int H, int W);
+cudaError_t launch_color_correct_bwd(int H, int W, Band band, const float *image, const float *affine, const float *g_out, float *g_image,
+                                     double *sums, void *scratch, cudaStream_t st);
+cudaError_t launch_color_correct_affine_grad(const double *sums, float *g_affine, cudaStream_t st);
 cudaError_t launch_color_correction_reg(const float *affine, const float *affine_sky, float weight, float *value, float *g_affine,
                                         float *g_affine_sky, cudaStream_t st);
 cudaError_t launch_sky_composite_fwd(int H, int W, int R, int mode, float fill, const float *rgb, const float *acc, const uint8_t *mask,
                                      const float *cube, const float *K, const float *w2c, const float *jx, const float *jy, float *out,
                                      cudaStream_t st);
 cudaError_t launch_sky_composite_bwd(int H, int W, int R, int mode, float fill, const float *acc, const uint8_t *mask, const float *cube,
+                                     const float *K, const float *w2c, const float *jx, const float *jy, const float *gout, float *gacc,
+                                     float *gcube, cudaStream_t st);
+cudaError_t launch_sky_composite_fwd(int H, int W, Band band, int R, int mode, float fill, const float *rgb, const float *acc, const uint8_t *mask,
+                                     const float *cube, const float *K, const float *w2c, const float *jx, const float *jy, float *out,
+                                     cudaStream_t st);
+cudaError_t launch_sky_composite_bwd(int H, int W, Band band, int R, int mode, float fill, const float *acc, const uint8_t *mask, const float *cube,
                                      const float *K, const float *w2c, const float *jx, const float *jy, const float *gout, float *gacc,
                                      float *gcube, cudaStream_t st);
 // tracked actor poses (actor_pose.cu): the device-resident track table and one call's camera

@@ -5,7 +5,8 @@
 // (training with a sky mask: the mask or rows 0-49; otherwise 1 - acc > 1e-3), the cube lookup dr.texture(linear, cube) restates
 // (face of the largest component, face coordinates inverting cube_to_dir, sky_cubemap.py:154-161, bilinear over four taps with edge
 // and corner wrap), the clamp to [0, 1] and rgb + sky (1 - acc).  The backward recomputes the ray and the taps from the saved jitter.
-// Nothing depends on how many pixels are sky: grids depend on H x W only and nothing is read back to the host.
+// Nothing depends on how many pixels are sky: grids depend on H x W only and nothing is read back to the host.  The band forms run the
+// same kernels over the pixels of a tile-row band only (multi-GPU, DESIGN.md §8): grids depend on H x W and the band.
 #include "sgr_common.cuh"
 
 namespace sgr {
@@ -155,14 +156,20 @@ __device__ __forceinline__ bool sky_pixel(const SkyCam &cam, const int64_t pix, 
 	return __fsub_rn(1.f, accv) > 1e-3f;
 }
 
-__global__ void __launch_bounds__(kSkyThreads) sky_composite_fwd_kernel(const int64_t N, const int W, const int R, const int mode, const float fill,
+// Work item t of M: pixel t of the frame (M = N), or with kBand pixel t of the band's tile rows (M = band_rows * 16 W, band_pixel).
+// Every pixel is indexed by its global (i, j): the ray and the rows-0-49 rule depend on the row in the frame.
+template <bool kBand>
+__global__ void __launch_bounds__(kSkyThreads) sky_composite_fwd_kernel(const int64_t N, const int64_t M, const Band band, const int W, const int R,
+                                                                        const int mode, const float fill,
                                                                         const float *__restrict__ rgb, const float *__restrict__ acc,
                                                                         const uint8_t *__restrict__ mask, const float *__restrict__ cube,
                                                                         const float *__restrict__ K, const float *__restrict__ w2c,
                                                                         const float *__restrict__ jx, const float *__restrict__ jy,
                                                                         float *__restrict__ out) {
-	const int64_t pix = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-	if (pix >= N) return;
+	const int64_t item = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (item >= M) return;
+	const int64_t pix = kBand ? band_pixel(item, band, (int64_t)kBandTileRows * W) : item;
+	if (kBand && pix >= N) return;
 	const SkyCam cam = sky_camera(K, w2c);
 	const float accv = __ldg(acc + pix);
 	float d[3], sky[3] = {fill, fill, fill};
@@ -198,15 +205,18 @@ __device__ __forceinline__ void sky_scatter(const int idx, float g0, float g1, f
 }
 
 // dL/dacc = -sum_c sky_c g_c; dL/dcube: each tap's weight times g (1 - acc) where 0 <= s <= 1, a corner tap's weight shared by thirds
-// among the three taps that exist.  dL/drgb is dL/dout itself.  Every lane of a warp reaches sky_scatter (idx = -1 past the image).
-__global__ void __launch_bounds__(kSkyThreads) sky_composite_bwd_kernel(const int64_t N, const int W, const int R, const int mode, const float fill,
+// among the three taps that exist.  dL/drgb is dL/dout itself.  Every lane of a warp reaches sky_scatter (idx = -1 past the image or the band).
+template <bool kBand>
+__global__ void __launch_bounds__(kSkyThreads) sky_composite_bwd_kernel(const int64_t N, const int64_t M, const Band band, const int W, const int R,
+                                                                        const int mode, const float fill,
                                                                         const float *__restrict__ acc, const uint8_t *__restrict__ mask,
                                                                         const float *__restrict__ cube, const float *__restrict__ K,
                                                                         const float *__restrict__ w2c, const float *__restrict__ jx,
                                                                         const float *__restrict__ jy, const float *__restrict__ gout,
                                                                         float *__restrict__ gacc, float *__restrict__ gcube) {
-	const int64_t pix = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-	const bool live = pix < N;
+	const int64_t item = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	const int64_t pix = kBand ? band_pixel(item, band, (int64_t)kBandTileRows * W) : item;
+	const bool live = item < M && pix < N;
 	const SkyCam cam = sky_camera(K, w2c);
 	const float accv = live ? __ldg(acc + pix) : 1.f;
 	float d[3] = {1.f, 0.f, 0.f};
@@ -252,7 +262,8 @@ cudaError_t launch_sky_composite_fwd(int H, int W, int R, int mode, float fill, 
                                      cudaStream_t st) {
 	const int64_t N = (int64_t)H * W;
 	count_launch();
-	sky_composite_fwd_kernel<<<sky_blocks(N), kSkyThreads, 0, st>>>(N, W, R, mode, fill, rgb, acc, mask, cube, K, w2c, jx, jy, out);
+	sky_composite_fwd_kernel<false><<<sky_blocks(N), kSkyThreads, 0, st>>>(N, N, Band{0, 1, 1}, W, R, mode, fill, rgb, acc, mask, cube, K, w2c, jx,
+	                                                                       jy, out);
 	return cudaGetLastError();
 }
 
@@ -261,7 +272,30 @@ cudaError_t launch_sky_composite_bwd(int H, int W, int R, int mode, float fill, 
                                      float *gcube, cudaStream_t st) {
 	const int64_t N = (int64_t)H * W;
 	count_launch();
-	sky_composite_bwd_kernel<<<sky_blocks(N), kSkyThreads, 0, st>>>(N, W, R, mode, fill, acc, mask, cube, K, w2c, jx, jy, gout, gacc, gcube);
+	sky_composite_bwd_kernel<false><<<sky_blocks(N), kSkyThreads, 0, st>>>(N, N, Band{0, 1, 1}, W, R, mode, fill, acc, mask, cube, K, w2c, jx, jy,
+	                                                                       gout, gacc, gcube);
+	return cudaGetLastError();
+}
+
+// The band's forms: one thread per pixel of the band's tile rows (an empty band launches nothing).
+cudaError_t launch_sky_composite_fwd(int H, int W, Band band, int R, int mode, float fill, const float *rgb, const float *acc, const uint8_t *mask,
+                                     const float *cube, const float *K, const float *w2c, const float *jx, const float *jy, float *out,
+                                     cudaStream_t st) {
+	const int64_t N = (int64_t)H * W, M = (int64_t)band_rows(band) * kBandTileRows * W;
+	if (M == 0) return cudaSuccess;
+	count_launch();
+	sky_composite_fwd_kernel<true><<<sky_blocks(M), kSkyThreads, 0, st>>>(N, M, band, W, R, mode, fill, rgb, acc, mask, cube, K, w2c, jx, jy, out);
+	return cudaGetLastError();
+}
+
+cudaError_t launch_sky_composite_bwd(int H, int W, Band band, int R, int mode, float fill, const float *acc, const uint8_t *mask, const float *cube,
+                                     const float *K, const float *w2c, const float *jx, const float *jy, const float *gout, float *gacc,
+                                     float *gcube, cudaStream_t st) {
+	const int64_t N = (int64_t)H * W, M = (int64_t)band_rows(band) * kBandTileRows * W;
+	if (M == 0) return cudaSuccess;
+	count_launch();
+	sky_composite_bwd_kernel<true><<<sky_blocks(M), kSkyThreads, 0, st>>>(N, M, band, W, R, mode, fill, acc, mask, cube, K, w2c, jx, jy, gout, gacc,
+	                                                                      gcube);
 	return cudaGetLastError();
 }
 

@@ -9,6 +9,10 @@ with the guidance mask) the cube is sampled where the mask is set and on rows 0-
 mask is only read: the reference sets its rows 0-49 in place, which the sky loss then sees, so a caller who wants that loss input
 sets those rows itself.  `perturb` jitters each pixel's sample point as get_rays_torch(perturb=True) does, with two torch.rand(H, W)
 draws on the current CUDA generator.  CUDA tensors only: there is no CPU fallback.
+
+band= / group= (keyword-only, as in losses.py): rgb and acc hold the rendered rows of this rank's TileRowBand (sharded.py); the
+composite runs on the band's pixels only (sgr_band_sky_composite_*), the output is zero outside the band, and the backward gives
+dL/dacc on the band's rows and all-reduces the cube map's gradient over `group`, so every rank's cube_map.grad is the whole frame's.
 """
 from __future__ import annotations
 
@@ -49,10 +53,19 @@ def _check(rgb, acc, cube_map, K, w2c, sky_mask):
     return H, W, int(cube_map.shape[1])
 
 
+def _band_rows(band, H: int):
+    """(begin, end, step) of the band, or None for the whole frame."""
+    if band is None:
+        return None
+    from .band_losses import check_band
+    return check_band(band, H)
+
+
 class _SkyComposite(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, rgb, acc, cube_map, K, w2c, sky_mask, perturb: bool, fill: float):
+    def forward(ctx, rgb, acc, cube_map, K, w2c, sky_mask, perturb: bool, fill: float, band, group):
         H, W, R = _check(rgb, acc, cube_map, K, w2c, sky_mask)
+        rows = _band_rows(band, H)
         dev = rgb.device
         rgb_c, acc_c, cube = rgb.contiguous(), acc.contiguous(), cube_map.contiguous()
         Kc, Tc = K.contiguous(), w2c.contiguous()
@@ -63,11 +76,17 @@ class _SkyComposite(torch.autograd.Function):
             jy = torch.rand(H, W, device=dev)
         else:
             jx = jy = None
-        out = torch.empty_like(rgb_c)
-        _capi.call("sgr_sky_composite_forward", dev, H, W, R, mode, float(fill), ptr(rgb_c), ptr(acc_c), ptr(mask), ptr(cube), ptr(Kc), ptr(Tc),
-                   ptr(jx), ptr(jy), ptr(out))
+        if rows is None:
+            out = torch.empty_like(rgb_c)
+            _capi.call("sgr_sky_composite_forward", dev, H, W, R, mode, float(fill), ptr(rgb_c), ptr(acc_c), ptr(mask), ptr(cube), ptr(Kc),
+                       ptr(Tc), ptr(jx), ptr(jy), ptr(out))
+        else:
+            out = torch.zeros_like(rgb_c)
+            _capi.call("sgr_band_sky_composite_forward", dev, H, W, *rows, R, mode, float(fill), ptr(rgb_c), ptr(acc_c), ptr(mask), ptr(cube),
+                       ptr(Kc), ptr(Tc), ptr(jx), ptr(jy), ptr(out))
         ctx.save_for_backward(acc_c, cube, Kc, Tc, mask, jx, jy)
         ctx.args = (H, W, R, mode, float(fill))
+        ctx.band, ctx.group = rows, group
         return out
 
     @staticmethod
@@ -77,16 +96,32 @@ class _SkyComposite(torch.autograd.Function):
         dev = acc.device
         g = g_out.contiguous()
         need_rgb, need_acc, need_cube = ctx.needs_input_grad[:3]
-        g_acc = torch.empty_like(acc) if need_acc else None
         g_cube = torch.zeros_like(cube) if need_cube else None
-        _capi.call("sgr_sky_composite_backward", dev, H, W, R, mode, fill, ptr(acc), ptr(mask), ptr(cube), ptr(Kc), ptr(Tc), ptr(jx), ptr(jy),
-                   ptr(g), ptr(g_acc), ptr(g_cube))
-        return (g_out if need_rgb else None), g_acc, g_cube, None, None, None, None, None
+        if ctx.band is None:
+            g_acc = torch.empty_like(acc) if need_acc else None
+            _capi.call("sgr_sky_composite_backward", dev, H, W, R, mode, fill, ptr(acc), ptr(mask), ptr(cube), ptr(Kc), ptr(Tc), ptr(jx),
+                       ptr(jy), ptr(g), ptr(g_acc), ptr(g_cube))
+        else:
+            g_acc = torch.zeros_like(acc) if need_acc else None
+            _capi.call("sgr_band_sky_composite_backward", dev, H, W, *ctx.band, R, mode, fill, ptr(acc), ptr(mask), ptr(cube), ptr(Kc), ptr(Tc),
+                       ptr(jx), ptr(jy), ptr(g), ptr(g_acc), ptr(g_cube))
+            if need_cube:  # COLLECTIVE: this band's partial dL/dcube -> the whole frame's, on every rank
+                from .band_losses import all_reduce_sum
+                all_reduce_sum(g_cube, ctx.group)
+        return (g_out if need_rgb else None), g_acc, g_cube, None, None, None, None, None, None, None
 
 
 def sky_composite(rgb: torch.Tensor, acc: torch.Tensor, cube_map: torch.Tensor, K: torch.Tensor, w2c: torch.Tensor, *,
-                  sky_mask: Optional[torch.Tensor] = None, perturb: bool = False, white_background: bool = True) -> torch.Tensor:
+                  sky_mask: Optional[torch.Tensor] = None, perturb: bool = False, white_background: bool = True, band=None,
+                  group=None) -> torch.Tensor:
     """rgb [3, H, W] + sky * (1 - acc [1, H, W]) with the sky sampled from cube_map [6, R, R, 3] along the rays of K [3, 3] and
     w2c [4, 4], clamped to [0, 1]; pixels the mask rule leaves out take 1 (white_background) or 0.  Differentiable in rgb, acc and
-    cube_map.  sky_mask: bool [1, H, W] or [H, W] (training with the guidance mask), None for the acc rule.  All fp32 CUDA tensors."""
-    return _SkyComposite.apply(rgb, acc, cube_map, K, w2c, sky_mask, bool(perturb), 1.0 if white_background else 0.0)
+    cube_map.  sky_mask: bool [1, H, W] or [H, W] (training with the guidance mask), None for the acc rule.  All fp32 CUDA tensors.
+
+    band= / group=: rgb and acc hold the rendered rows of this rank's TileRowBand (sharded.py); sky_mask is the whole frame's.  The
+    output has the band's rows, zeros elsewhere, equal bit for bit to the whole-frame call's rows; dL/dacc covers the band's rows.
+    COLLECTIVE in the backward: the cube map's gradient is all-reduced over `group` (every rank must run its backward).  perturb=True
+    draws the same full-frame [H, W] jitter pair, in the same order, as the whole-frame call, so a rank's rows equal the single-GPU
+    call's whenever the ranks' CUDA generators are in the same state."""
+    _band_rows(band, int(rgb.shape[-2]))  # a bad band fails before anything else
+    return _SkyComposite.apply(rgb, acc, cube_map, K, w2c, sky_mask, bool(perturb), 1.0 if white_background else 0.0, band, group)

@@ -9,6 +9,10 @@ foreign rows zero, and the gradients of the rank's own Gaussians equal up to flo
 between ANY two runs (float atomics), so the run-to-run difference of the single-GPU rasterizer is measured beside it
 and printed as `floor`; the bound asserted is GRAD_TOL = 5e-4 of max|ref| per tensor — half the 1e-3 parity bar the
 single-GPU path is held to against the reference.
+
+Two further legs run each rank's band stages against the single-GPU calls on the gathered frame: the training losses (band_losses.py),
+and the sky composite and colour correction with band= / group= (their parameter gradients all-reduced).  Neither leg has been run on
+several H100s yet; the single-GPU emulations of tests/test_band_losses_gpu.py and tests/test_band_image_gpu.py cover their kernels.
 """
 import os
 import sys
@@ -145,6 +149,56 @@ def run_losses(rank, world, dev, W=1280, H=720):
             assert not bool(x[:, ~rows].any()), f"{name}: foreign gradient rows not zero"
 
 
+def run_image_stages(rank, world, dev, W=1280, H=720, R=256):
+    """Sky and colour-correction leg: sky_composite and color_correct with band= / group= on each rank's banded render against the
+    whole-frame calls on the gathered frame.  Output and image-gradient rows bit-equal, foreign rows zero; the all-reduced cube gradient
+    equal to the whole-frame one up to the order of its float atomics (1e-5 of max|ref|), and the all-reduced affine gradient within one
+    fp32 ulp of its fp64 sum."""
+    from street_gaussians_b200 import corrections
+    scene = synthetic.make_scene(P=60_001, width=W, height=H, sh_degree=3, seed=79, pose=True)
+    st = util.settings_from(sgb, scene["cam"], dev)
+    rast = GaussianShardedRasterizer(st)
+    P = scene["means3D"].shape[0]
+    chunk = (P + world - 1) // world
+    lo, hi = min(P, rank * chunk), min(P, (rank + 1) * chunk)
+    with torch.no_grad():
+        got = rast(means3D=scene["means3D"][lo:hi].to(dev), means2D=None, opacities=scene["opacities"][lo:hi].to(dev),
+                   shs=scene["shs"][lo:hi].to(dev), scales=scene["scales"][lo:hi].to(dev), rotations=scene["rotations"][lo:hi].to(dev))
+    color, acc = got[0], got[3]
+    full = [t.clone() for t in (color, acc)]
+    for t in full:
+        if world > 1:
+            dist.all_reduce(t)
+    g = torch.Generator(device=dev).manual_seed(6)  # the same whole-frame inputs on every rank
+    cube = torch.rand(6, R, R, 3, device=dev, generator=g)
+    affine = torch.eye(4, device=dev)[:3] + 0.05 * torch.randn(3, 4, device=dev, generator=g)
+    sky_mask = torch.rand(1, H, W, device=dev, generator=g) > 0.5
+    up = torch.randn(3, H, W, device=dev, generator=g)
+    f = W / (2 * float(st.tanfovx))
+    K = torch.tensor([[f, 0.0, W / 2], [0.0, f, H / 2], [0.0, 0.0, 1.0]], device=dev)
+    w2c = st.viewmatrix.T.contiguous()
+    rows = band_of_rows(H, rank, world).to(dev)
+    band = rast.band if rast.band is not None else sgb.TileRowBand(0, (H + 15) // 16, 1)
+
+    def step(rgb, a, b):
+        xs = [t.detach().clone().requires_grad_(True) for t in (rgb, a, cube, affine)]
+        out = sgb.sky_composite(xs[0], xs[1], xs[2], K, w2c, sky_mask=sky_mask, band=b)
+        col = corrections.color_correct(out, xs[3], band=b)
+        col.backward(torch.where(rows.view(1, -1, 1), up, torch.zeros_like(up)) if b is not None else up)
+        return [col.detach()] + [x.grad for x in xs]
+
+    ref = step(full[0], full[1], None)
+    got = step(color, acc, band)
+    bits = lambda x: x.contiguous().view(torch.int32)
+    for name, x, y in (("rgb_out", got[0], ref[0]), ("dL/drgb", got[1], ref[1]), ("dL/dacc", got[2], ref[2])):
+        assert torch.equal(bits(x[:, rows]), bits(y[:, rows])), f"{name}: band rows differ"
+        assert not bool(x[:, ~rows].any()), f"{name}: foreign rows not zero"
+    assert float((got[3] - ref[3]).abs().max()) <= 1e-5 * float(ref[3].abs().max()), "dL/dcube"
+    x64 = torch.cat([sgb.sky_composite(*full, cube, K, w2c, sky_mask=sky_mask).detach().reshape(3, -1), torch.ones(1, H * W, device=dev)]).double()
+    exact = (up.reshape(3, -1).double() @ x64.T).cpu().numpy()
+    assert (np.abs(got[4].cpu().double().numpy() - exact) <= np.spacing(np.abs(exact).astype(np.float32))).all(), "dL/daffine"
+
+
 def main():
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -161,6 +215,9 @@ def main():
                   f"(single-GPU run-to-run floor {floor:.2e})", flush=True)
         run_losses(rank, world, dev)
         print(f"[rank {rank}/{world}] band losses: the frame's values, gradient rows bit-equal to the single-GPU losses", flush=True)
+        run_image_stages(rank, world, dev)
+        print(f"[rank {rank}/{world}] band sky and colour correction: rows bit-equal to the single-GPU calls, parameter gradients the frame's",
+              flush=True)
     except AssertionError as e:
         ok = False
         print(f"[rank {rank}] FAILED: {e!r}", flush=True)
