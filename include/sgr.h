@@ -601,6 +601,52 @@ int sgr_band_color_correct_backward(int32_t H, int32_t W, int32_t row_begin, int
                                     const float *dL_dout, float *dL_dimage, double *partials, void *scratch, size_t scratch_bytes, void *stream);
 int sgr_band_color_correct_affine_grad(const double *sums, float *dL_daffine, void *stream);
 
+/* ---- Evaluation metrics: masked L1, PSNR and SSIM of rendered views, value only ----
+ * Replaces the scoring of training_report (train.py:274-303: l1_loss and psnr of the clamped render, lib/utils/loss_utils.py:21-37,
+ * 61-78) and of metrics.py:76-81 (ssim and psnr of the saved 8-bit PNGs).  Per view, over C channels of H x W:
+ *   abs_diff, sq_diff   sum of |x - y| and (x - y)^2 over the masked elements (C x the pixels whose mask byte is non-zero; every
+ *                       pixel when mask is NULL), the difference formed in fp64;
+ *   masked              the number of masked elements (an integer, exact below 2^53);
+ *   ssim                sum of the SSIM map over all C H W elements: the reference's ssim / _ssim (11x11 Gaussian window, sigma 1.5,
+ *                       zero padding, C1 = 0.01^2, C2 = 0.03^2, sigma = E[x^2] - mu^2) in fp32, the arithmetic of sgr_image_loss;
+ *   elements            C H W (of the band, for the band call).
+ * flags (per call):
+ *   SGR_EVAL_CLAMP        image and gt clamped to [0, 1] first (training_report); NaN stays NaN;
+ *   SGR_EVAL_QUANT8       then the round trip of the PNGs metrics.py reads: torchvision.utils.save_image stores
+ *                         uint8(clamp(255 x + 0.5, 0, 255)) (255 x and + 0.5 each rounded in fp32: the nearest level, halves up) and
+ *                         to_tensor reads it back as / 255 in fp32 (needs CLAMP);
+ *   SGR_EVAL_SSIM_MASKED  SSIM of the images zeroed outside the mask, as ssim(mask=) does; without it SSIM runs on the unmasked images;
+ *   SGR_EVAL_NO_SSIM      the SSIM map is not formed (the L1 / PSNR sums only): ssim and elements get nothing added.
+ * sgr_eval_metrics_accumulate scores V views (image, gt: [V][C][H][W] fp32 device; mask: uint8 [V][H][W] device or NULL) and ADDS view
+ * v's sums to sums[v] (device; the caller zeroes a fresh slot).  No float atomics: each 16 x 16 tile's partial sums are formed in a
+ * fixed order and the tiles summed in a fixed order in fp64, so identical calls give identical bits and V views in one call give the
+ * bits of V calls of one view.  Nothing is read back to the host; the grids depend on V, C, H, W (and the band) only.
+ * scratch: sgr_eval_metrics_scratch_bytes(V, C, H, W) bytes (0 for bad sizes).  V C <= 65535, H W < 2^31.
+ *
+ * sgr_band_eval_metrics_accumulate: the same sums over the pixels of a tile-row band (as for the band losses above), image holding the
+ * band's rows and the rows within 5 px of them (the photometric loss's halo, sgr_band_halo_pack / _unpack, carries them); gt and mask
+ * are whole frames.  A tile gives the partials of the whole-frame call's block for that tile, so the sums over the ranks equal the
+ * whole-frame sums up to the fp64 regrouping of the tile partials: |difference| <= 2 (T - 1) 2^-53 sum |partials| for T tiles.
+ *
+ * sgr_eval_metrics_finish: out[V + 1][4] fp32 device: out[v] = {psnr, ssim, l1, n} with mse = sq_diff / masked,
+ * psnr = 20 log10(1 / sqrt(mse)), ssim = ssim / elements, l1 = abs_diff / masked, n = masked; out[V] = {the means over the views of
+ * the fp32 psnr, ssim and l1 values (summed in fp64), V}.  The reference's edge results are kept: mse = 0 gives psnr = +inf, and an
+ * empty mask gives NaN psnr and l1 (0 / 0), which make their means NaN as well.  A view scored only with SGR_EVAL_NO_SSIM has ssim NaN. */
+#define SGR_EVAL_CLAMP 1
+#define SGR_EVAL_QUANT8 2
+#define SGR_EVAL_SSIM_MASKED 4
+#define SGR_EVAL_NO_SSIM 8
+typedef struct SgrEvalSums {
+	double abs_diff, sq_diff, ssim, masked, elements;
+} SgrEvalSums;
+size_t sgr_eval_metrics_scratch_bytes(int32_t V, int32_t C, int32_t H, int32_t W);
+int sgr_eval_metrics_accumulate(int32_t V, int32_t C, int32_t H, int32_t W, int32_t flags, const float *image, const float *gt,
+                                const uint8_t *mask, SgrEvalSums *sums, void *scratch, size_t scratch_bytes, void *stream);
+int sgr_band_eval_metrics_accumulate(int32_t V, int32_t C, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step,
+                                     int32_t flags, const float *image, const float *gt, const uint8_t *mask, SgrEvalSums *sums,
+                                     void *scratch, size_t scratch_bytes, void *stream);
+int sgr_eval_metrics_finish(int32_t V, const SgrEvalSums *sums, float *out, void *stream);
+
 /* ---- Post-backward bookkeeping of a training iteration (SURVEY.md §8 row f3) ----
  * Densification statistics of StreetGaussianModel.set_max_radii2D + add_densification_stats
  * (lib/models/street_gaussian_model.py:551-571), all sub-models in one pass over the composed index space: for every Gaussian

@@ -18,10 +18,11 @@ from .corrections import color_correct, color_correction_reg_loss  # noqa: E402,
 from .sky import sky_composite  # noqa: E402,F401
 from .actor_pose import ActorPose  # noqa: E402,F401
 from .features import compose_semantics, finish_features, gaussian_normals  # noqa: E402,F401
-from . import band_losses, corrections, features, losses, sky, training  # noqa: E402,F401
+from .metrics import ViewMetrics  # noqa: E402,F401
+from . import band_losses, corrections, features, losses, metrics, sky, training  # noqa: E402,F401
 
 __all__ = ["compose", "ActorPose", "color_correct", "color_correction_reg_loss", "sky_composite", "gaussian_normals", "compose_semantics",
-           "finish_features", "GaussianRasterizationSettings", "GaussianRasterizer", "TileRowBand", "InstanceCapacity", "RenderLayer", "rasterize_gaussians", "distCUDA2",
+           "finish_features", "ViewMetrics", "GaussianRasterizationSettings", "GaussianRasterizer", "TileRowBand", "InstanceCapacity", "RenderLayer", "rasterize_gaussians", "distCUDA2",
            "install_shims"]
 
 _SHIMS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "shims")

@@ -32,7 +32,8 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_set_nea
            "sgr_band_image_loss_grad", "sgr_band_sky_loss", "sgr_band_obj_acc_loss", "sgr_band_acc_loss_value", "sgr_band_lidar_scratch_bytes",
            "sgr_band_lidar_keys", "sgr_band_lidar_select", "sgr_band_lidar_grad", "sgr_band_sky_composite_forward",
            "sgr_band_sky_composite_backward", "sgr_band_color_correct_forward", "sgr_band_color_correct_scratch_bytes",
-           "sgr_band_color_correct_backward", "sgr_band_color_correct_affine_grad"]
+           "sgr_band_color_correct_backward", "sgr_band_color_correct_affine_grad", "sgr_eval_metrics_scratch_bytes",
+           "sgr_eval_metrics_accumulate", "sgr_band_eval_metrics_accumulate", "sgr_eval_metrics_finish"]
 
 SKY_MASK_ACC, SKY_MASK_GIVEN = 0, 1
 SEMANTIC_LOGITS, SEMANTIC_PROBABILITIES = 0, 1
@@ -121,6 +122,10 @@ LIDAR_LEVEL0_WORDS = 6 + LIDAR_BINS
 class SgrLidarState(C.Structure):
     _fields_ = [("n", C.c_uint32), ("k", C.c_uint32), ("prefix", C.c_uint32), ("rank", C.c_uint32), ("sum_lt", C.c_double),
                 ("hist", (C.c_uint32 * LIDAR_BINS) * 3)]
+
+
+EVAL_CLAMP, EVAL_QUANT8, EVAL_SSIM_MASKED, EVAL_NO_SSIM = 1, 2, 4, 8
+EVAL_SUMS = 5  # doubles of an SgrEvalSums: abs_diff, sq_diff, ssim, masked, elements
 
 
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
@@ -273,6 +278,14 @@ def lib():
     L.sgr_band_color_correct_backward.argtypes = [C.c_int32] * 2 + band + [vp] * 6 + [C.c_size_t, vp]
     L.sgr_band_color_correct_affine_grad.restype = C.c_int
     L.sgr_band_color_correct_affine_grad.argtypes = [vp] * 3
+    L.sgr_eval_metrics_scratch_bytes.restype = C.c_size_t
+    L.sgr_eval_metrics_scratch_bytes.argtypes = [C.c_int32] * 4
+    L.sgr_eval_metrics_accumulate.restype = C.c_int
+    L.sgr_eval_metrics_accumulate.argtypes = [C.c_int32] * 5 + [vp] * 4 + [vp, C.c_size_t, vp]
+    L.sgr_band_eval_metrics_accumulate.restype = C.c_int
+    L.sgr_band_eval_metrics_accumulate.argtypes = [C.c_int32] * 4 + band + [C.c_int32] + [vp] * 4 + [vp, C.c_size_t, vp]
+    L.sgr_eval_metrics_finish.restype = C.c_int
+    L.sgr_eval_metrics_finish.argtypes = [C.c_int32, vp, vp, vp]
     L.sgr_densify_stats.restype = C.c_int
     L.sgr_densify_stats.argtypes = [C.POINTER(SgrStatSegment), C.c_int32, vp, vp, vp]
     L.sgr_adam_step.restype = C.c_int

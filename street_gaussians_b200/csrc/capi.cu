@@ -1380,6 +1380,61 @@ int sgr_band_color_correct_affine_grad(const double *sums, float *dL_daffine, vo
 	return SGR_OK;
 }
 
+// ---- evaluation metrics ----
+static bool eval_sizes_ok(int32_t V, int32_t C, int32_t H, int32_t W) {
+	if (V <= 0 || C <= 0 || H <= 0 || W <= 0 || (int64_t)H * W >= ((int64_t)1 << 31)) return false;
+	// one grid z per (view, channel), one grid y per tile row; the tile partials of a view are counted in 32 bits
+	const int64_t rows = ((int64_t)H + 15) / 16, cols = ((int64_t)W + 15) / 16;
+	return (int64_t)V * C <= 65535 && rows <= 65535 && (int64_t)C * rows * cols < ((int64_t)1 << 31);
+}
+
+size_t sgr_eval_metrics_scratch_bytes(int32_t V, int32_t C, int32_t H, int32_t W) {
+	return eval_sizes_ok(V, C, H, W) ? eval_metrics_scratch_bytes(V, C, H, W) : 0;
+}
+
+static int eval_accumulate(const char *fn, int32_t V, int32_t C, int32_t H, int32_t W, bool whole, int32_t row_begin, int32_t row_end,
+                           int32_t row_step, int32_t flags, const float *image, const float *gt, const uint8_t *mask, SgrEvalSums *sums,
+                           void *scratch, size_t scratch_bytes, void *stream) {
+	if (!eval_sizes_ok(V, C, H, W)) return fail(SGR_EINVAL, "%s: bad sizes V=%d C=%d H=%d W=%d", fn, V, C, H, W);
+	Band band;
+	if (whole) {
+		band = Band{0, (int)(((int64_t)H + 15) / 16), 1};
+	} else if (int rc = loss_band(fn, H, W, row_begin, row_end, row_step, &band)) {
+		return rc;
+	}
+	const int32_t known = SGR_EVAL_CLAMP | SGR_EVAL_QUANT8 | SGR_EVAL_SSIM_MASKED | SGR_EVAL_NO_SSIM;
+	if ((flags & ~known) != 0 || ((flags & SGR_EVAL_QUANT8) && !(flags & SGR_EVAL_CLAMP)))
+		return fail(SGR_EINVAL, "%s: bad flags %d (SGR_EVAL_QUANT8 needs SGR_EVAL_CLAMP)", fn, flags);
+	if (!image || !gt || !sums) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	if (!scratch || scratch_bytes < eval_metrics_scratch_bytes(V, C, H, W))
+		return fail(SGR_ENOMEM, "%s: scratch too small: %zu < %zu", fn, scratch_bytes, eval_metrics_scratch_bytes(V, C, H, W));
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_eval_metrics(V, C, H, W, band, flags, image, gt, mask, sums, scratch, st), fn);
+	return SGR_OK;
+}
+
+int sgr_band_eval_metrics_accumulate(int32_t V, int32_t C, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step,
+                                     int32_t flags, const float *image, const float *gt, const uint8_t *mask, SgrEvalSums *sums,
+                                     void *scratch, size_t scratch_bytes, void *stream) {
+	return eval_accumulate("sgr_band_eval_metrics_accumulate", V, C, H, W, false, row_begin, row_end, row_step, flags, image, gt, mask, sums,
+	                       scratch, scratch_bytes, stream);
+}
+
+int sgr_eval_metrics_accumulate(int32_t V, int32_t C, int32_t H, int32_t W, int32_t flags, const float *image, const float *gt,
+                                const uint8_t *mask, SgrEvalSums *sums, void *scratch, size_t scratch_bytes, void *stream) {
+	return eval_accumulate("sgr_eval_metrics_accumulate", V, C, H, W, true, 0, 0, 1, flags, image, gt, mask, sums, scratch, scratch_bytes, stream);
+}
+
+int sgr_eval_metrics_finish(int32_t V, const SgrEvalSums *sums, float *out, void *stream) {
+	if (V <= 0) return fail(SGR_EINVAL, "sgr_eval_metrics_finish: V must be positive, got %d", V);
+	if (!sums || !out) return fail(SGR_EINVAL, "NULL pointer passed to sgr_eval_metrics_finish");
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_eval_metrics_finish(V, sums, out, st), "eval_metrics_finish");
+	return SGR_OK;
+}
+
 int sgr_densify_stats(const SgrStatSegment *segments, int32_t num_segments, const int32_t *radii, const float *means2D_grad, void *stream) {
 	if (!segments || num_segments <= 0) return fail(SGR_EINVAL, "segment table is empty");
 	int64_t at = 0;

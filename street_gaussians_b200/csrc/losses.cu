@@ -12,11 +12,11 @@
 //            block (0,0,0) also finalises the scalars.
 // Semantics follow the reference exactly: with a mask both images are ZEROED outside it before SSIM (loss_utils.py:95-97) and
 // the SSIM mean runs over all pixels, while L1 averages over the masked pixels only (:31-35).
-#include "sgr_common.cuh"
+#include "ssim_tile.cuh"
 
 namespace sgr {
 
-constexpr int kWin = 11, kHalo = 5, kTileL = 16, kExt = kTileL + 2 * kHalo;  // 26
+constexpr int kWin = kSsimWin, kHalo = kSsimHalo, kTileL = kSsimTile, kExt = kSsimExt;  // 26
 
 // The tiles ssim_stats_kernel covers for a band: its own tile rows and the neighbours above and below them.  With step <= 2 they form
 // one run of tile rows; otherwise block row y is neighbour y % 3 - 1 of the (y / 3)-th owned tile row, -1 when that lies outside
@@ -34,9 +34,6 @@ __device__ __forceinline__ int stats_tile(const Band b, int y, int rows) {
 	return t >= 0 && t < rows ? t : -1;
 }
 
-struct GaussWin {
-	float w[kWin];
-};
 // loss_utils.py:84-86: exp(-(x - 5)^2 / (2 * 1.5^2)) normalised (float32, like torch.Tensor([...]) / sum).  The sum is the fp32
 // rounding of the exact sum, as torch's sum gives for these 11 values; a sequential fp32 sum is one ulp low and would move 9 of the
 // 11 weights by one ulp.
@@ -82,34 +79,15 @@ __global__ void __launch_bounds__(256) ssim_stats_kernel(const int C, const int 
 		sy[r][q] = b;
 	}
 	__syncthreads();
-	// horizontal pass: 26 rows x 16 columns x 5 quantities
-	for (int e = threadIdx.x; e < kExt * kTileL; e += 256) {
-		const int r = e / kTileL, q = e - r * kTileL;
-		float m1 = 0.f, m2 = 0.f, s11 = 0.f, s22 = 0.f, s12 = 0.f;
-#pragma unroll
-		for (int k = 0; k < kWin; k++) {
-			const float a = sx[r][q + k], b = sy[r][q + k], w = win.w[k];
-			m1 += w * a; m2 += w * b; s11 += w * a * a; s22 += w * b * b; s12 += w * a * b;
-		}
-		h[0][r][q] = m1; h[1][r][q] = m2; h[2][r][q] = s11; h[3][r][q] = s22; h[4][r][q] = s12;
-	}
+	ssim_tile_horizontal(sx, sy, h, win);
 	__syncthreads();
 	const int px = blockIdx.x * kTileL + tx, py = tile_y * kTileL + ty;
 	float v_ssim = 0.f, v_l1 = 0.f, v_cnt = 0.f;
 	if (px < W && py < H && needed) {
-		float m1 = 0.f, m2 = 0.f, s11 = 0.f, s22 = 0.f, s12 = 0.f;
-#pragma unroll
-		for (int k = 0; k < kWin; k++) {
-			const float w = win.w[k];
-			m1 += w * h[0][ty + k][tx]; m2 += w * h[1][ty + k][tx]; s11 += w * h[2][ty + k][tx]; s22 += w * h[3][ty + k][tx];
-			s12 += w * h[4][ty + k][tx];
-		}
-		const float C1 = 0.01f * 0.01f, C2 = 0.03f * 0.03f;
-		const float mu1_sq = m1 * m1, mu2_sq = m2 * m2, mu12 = m1 * m2;
-		const float sig1 = s11 - mu1_sq, sig2 = s22 - mu2_sq, sig12 = s12 - mu12;
-		const float A1 = 2.f * mu12 + C1, A2 = 2.f * sig12 + C2, B1 = mu1_sq + mu2_sq + C1, B2 = sig1 + sig2 + C2;
-		const float inv = 1.0f / (B1 * B2);
-		const float S = A1 * A2 * inv;
+		const SsimSums q = ssim_tile_vertical(h, win, tx, ty);
+		const float m1 = q.m1, m2 = q.m2;
+		const SsimTerms t = ssim_terms(q);
+		const float A1 = t.A1, A2 = t.A2, B1 = t.B1, B2 = t.B2, inv = t.inv, S = t.S;
 		v_ssim = owned ? S : 0.f;
 		const size_t o = (size_t)c * plane + (size_t)py * W + px;
 		// S = A1 A2 / (B1 B2);  dA1/dmu1 = 2 mu2, dA2/dmu1 = -2 mu2, dB1/dmu1 = 2 mu1, dB2/dmu1 = -2 mu1, dB2/ds11 = 1, dA2/ds12 = 2
@@ -263,7 +241,7 @@ __global__ void acc_loss_finalize_kernel(const size_t N, const float weight, con
 
 size_t image_loss_scratch_bytes(int C, int H, int W) { return align_up((size_t)3 * C * H * W * sizeof(float)) + 256; }
 
-static const GaussWin &window() {
+const GaussWin &ssim_window() {
 	static const GaussWin win = make_window();
 	return win;
 }
@@ -277,7 +255,7 @@ cudaError_t launch_image_loss_stats(int C, int H, int W, Band band, const float 
 	const unsigned tiles = stats_tiles(band, (H + kTileL - 1) / kTileL);
 	if (tiles == 0) return cudaSuccess;
 	count_launch(1);
-	ssim_stats_kernel<<<dim3((W + kTileL - 1) / kTileL, tiles, C), 256, 0, st>>>(C, H, W, band, window(), img, gt, mask, d_mu, d_xx, d_xy, acc);
+	ssim_stats_kernel<<<dim3((W + kTileL - 1) / kTileL, tiles, C), 256, 0, st>>>(C, H, W, band, ssim_window(), img, gt, mask, d_mu, d_xx, d_xy, acc);
 	return cudaGetLastError();
 }
 
@@ -288,7 +266,7 @@ cudaError_t launch_image_loss_grad(int C, int H, int W, Band band, const float *
 	const unsigned rows = band_rows(band);
 	count_launch(1);
 	ssim_grad_kernel<<<grad && rows ? dim3((W + kTileL - 1) / kTileL, rows, C) : dim3(1, 1, 1), 256, 0, st>>>(
-	    C, H, W, band, window(), img, gt, mask, d_mu, d_xx, d_xy, acc, w_l1, w_ssim, grad, scalars);
+	    C, H, W, band, ssim_window(), img, gt, mask, d_mu, d_xx, d_xy, acc, w_l1, w_ssim, grad, scalars);
 	return cudaGetLastError();
 }
 

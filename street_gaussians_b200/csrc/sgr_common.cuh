@@ -446,6 +446,12 @@ cudaError_t launch_compose_semantics_bwd(int n_bg, int K, int mode, const float 
 cudaError_t launch_finish_features_fwd(int S, int H, int W, int nc, int mode, const float *in, float *nout, float *sout, cudaStream_t st);
 cudaError_t launch_finish_features_bwd(int S, int H, int W, int nc, int mode, const float *in, const float *gn, const float *gs, float *gin,
                                        cudaStream_t st);
+// the 11-tap SSIM window of loss_utils.py (losses.cu), shared by the image loss and the evaluation metrics
+constexpr int kSsimWin = 11;
+struct GaussWin {
+	float w[kSsimWin];
+};
+const GaussWin &ssim_window();
 size_t image_loss_scratch_bytes(int C, int H, int W);
 cudaError_t launch_image_loss(int C, int H, int W, const float *img, const float *gt, const uint8_t *mask, float w_l1, float w_ssim, float *grad,
                               float *scalars, void *scratch, cudaStream_t st);
@@ -477,6 +483,11 @@ cudaError_t launch_lidar_band_select(int level, double keep, int H, int W, Band 
 cudaError_t launch_lidar_band_grad(int H, int W, Band band, const float *depth, const float *acc, const float *lidar, float weight,
                                    const SgrLidarState *s, const double *sums, float *dL_ddepth, float *dL_dacc, float *scalars, void *scratch,
                                    cudaStream_t st);
+// evaluation metrics (metrics.cu)
+size_t eval_metrics_scratch_bytes(int V, int C, int H, int W);
+cudaError_t launch_eval_metrics(int V, int C, int H, int W, Band band, int flags, const float *img, const float *gt, const uint8_t *mask,
+                                SgrEvalSums *sums, void *scratch, cudaStream_t st);
+cudaError_t launch_eval_metrics_finish(int V, const SgrEvalSums *sums, float *out, cudaStream_t st);
 cudaError_t launch_densify_stats(const SgrStatSegment *segs, int nseg, const int32_t *radii, const float *grad2d, cudaStream_t st);
 cudaError_t launch_adam(const SgrAdamTensor *ts, int n_tensors, double beta1, double beta2, double eps, cudaStream_t st);
 cudaError_t launch_sparse_adam(const SgrSparseAdamSegment *segs, int nseg, const int32_t *radii, double beta1, double beta2, double eps,
