@@ -404,11 +404,10 @@ static int bits_for(uint32_t n) {  // smallest b with (1 << b) >= n, i.e. enough
 // stable bucketing by tile id gives exactly the list the tile radix sort gives, over E instead of the whole capacity and without
 // padding.  A single ranked scatter straight into the ~10^4 tile buckets writes isolated words (a partition holds ~3 instances of
 // a tile); on config C it took 0.40 ms on an H100, more than the radix sort it replaces.  Two passes over 128 buckets write runs.
-//   1. bucket_count<TILES>:  [0, E) is cut into partitions of kBucketPart instances; CTA p counts its partition's tile ids in a
-//                            shared-memory histogram, writes row p of the (partition x tile) matrix and of the (partition x low
-//                            digit) matrix;
-//   2. bucket_columns:       per column, the total over the partitions (the tile totals -> ranges[t].y; the digit totals), and
-//                            for the digit matrices the exclusive prefix over the partitions, in place;
+//   1. bucket_count<TILES>:  [0, E) is cut into partitions of bucket_part(E) instances; CTA p counts its partition's tile ids in a
+//                            shared-memory histogram, adds its non-zero bins into the tile totals (ranges[t].y, zeroed first) and
+//                            writes row p of the (partition x low digit) matrix;
+//   2. bucket_columns:       per digit, the total over the partitions and the exclusive prefix over the partitions, in place;
 //   3. bucket_ranges:        one CTA scans the tile totals into `ranges` ((0, 0) for a tile without instances);
 //   4. bucket_pass<false>:   CTA p walks its partition in rounds; a stable match-based block rank of the round on the low digit
 //                            gives every instance its position among equal digits, added to the digit's running cursor in shared
@@ -416,33 +415,54 @@ static int bits_for(uint32_t n) {  // smallest b with (1 << b) >= n, i.e. enough
 //                            intermediate array (frames of at most 2^25 Gaussians; larger ones take the radix sort);
 //   5. bucket_count<false>, bucket_columns, bucket_pass<true>: the same on the high digit of the intermediate array, writing the
 //                            Gaussian indices into vals_out.
-// Positions come from ranks and prefix sums only, never from the order of atomics.  E is read on the device (status[3]) and the
-// grids are sized from the capacity, so the bounded mode stays free of host synchronisation.
-constexpr uint32_t kBucketPart = 32768;  // instances per partition (whole rounds)
+// Positions come from ranks and prefix sums only, never from the order of atomics (the tile totals are integer sums, which do not
+// depend on it).  E is read on the device (status[3]) and the grids are sized for the most partitions any E up to the capacity
+// can give, so the bounded mode stays free of host synchronisation.
 constexpr int kBucketThreads = 512;  // histogram CTAs
 constexpr int kPassThreads = 256;    // rank-and-scatter CTAs: 72 registers, 3 CTAs per SM
 constexpr int kDigitBits = 7, kDigits = 1 << kDigitBits;
 constexpr int kPassItems = 8;
 constexpr uint32_t kPassRound = kPassThreads * kPassItems;
-static_assert(kBucketPart % kPassRound == 0, "partitions are whole rounds");
+// Partition size: about E / kBucketTargetParts instances in whole rounds, at least one round and at most kBucketMaxPart.  With a
+// fixed 32768 a frame of 1.4 M instances (config C's saturation split) had 43 partitions for 132 SMs, each walking 16 rounds behind
+// three barriers per round; the target was chosen by a sweep on config C (DESIGN.md §7).  SGR_BUCKET_TARGET_PARTS exists for that
+// sweep (tools/saturation_split_ab.py --sweep-parts builds one library per value).
+#ifndef SGR_BUCKET_TARGET_PARTS
+#define SGR_BUCKET_TARGET_PARTS 396
+#endif
+constexpr uint32_t kBucketTargetParts = SGR_BUCKET_TARGET_PARTS;
+constexpr uint32_t kBucketMaxPart = 32768;
+static_assert(kBucketTargetParts > 0 && kBucketMaxPart % kPassRound == 0, "partitions are whole rounds");
+static_assert(kBucketThreads % kDigits == 0, "a histogram thread's tiles share one low digit");
+__host__ __device__ __forceinline__ uint32_t bucket_part(uint32_t E) {
+	const uint32_t per = E / kBucketTargetParts + (E % kBucketTargetParts != 0u);
+	const uint32_t whole = (per + kPassRound - 1u) / kPassRound * kPassRound;
+	return min(max(whole, kPassRound), kBucketMaxPart);
+}
+// Partitions of any E <= slots: bucket_part(E) >= ceil(E / kBucketTargetParts) unless capped, so at most kBucketTargetParts of them, or
+// ceil(slots / kBucketMaxPart) when capped; and never more than ceil(slots / kPassRound).  CTAs past the last partition return.
+static unsigned bucket_grid(int64_t slots) {
+	const int64_t n = slots > 0 ? slots : 1;
+	const int64_t most = std::max<int64_t>(kBucketTargetParts, (n + kBucketMaxPart - 1) / kBucketMaxPart);
+	return (unsigned)std::min<int64_t>(most, (n + kPassRound - 1) / kPassRound);
+}
 static_assert(kBucketMaxTiles <= (1 << (2 * kDigitBits)), "two digits cover every tile id of a bucketed frame");
 constexpr uint32_t kNoGaussian = 0xffffffffu;  // value of the slots of the last round past E
 // the intermediate words carry the high digit in their top 7 bits, so a bucketed frame has at most 2^25 Gaussians
 constexpr int kPackShift = 32 - kDigitBits;
 constexpr uint32_t kPackMask = (1u << kPackShift) - 1u;
 
-// the bucketing scratch behind the cub temp of the binning state (carve_bin): the count matrices and the digit totals.  Sized for
-// kBucketMaxTiles tiles, so that it does not depend on the frame.
+// the bucketing scratch behind the cub temp of the binning state (carve_bin): the two (partition x digit) count matrices and the
+// digit totals.
 struct BucketScratch {
-	uint32_t *tile_counts, *digit_counts[2], *digit_totals[2];
+	uint32_t *digit_counts[2], *digit_totals[2];
 	size_t bytes;
 };
 static BucketScratch carve_bucket(void *base, int64_t slots) {
 	BucketScratch s;
 	char *p = reinterpret_cast<char *>(base);
-	const size_t n = slots > 0 ? (size_t)slots : 1, nparts = (n + kBucketPart - 1) / kBucketPart;
+	const size_t nparts = bucket_grid(slots);
 	auto take = [&](size_t bytes) { char *r = p; p += align_up(bytes); return r; };
-	s.tile_counts = reinterpret_cast<uint32_t *>(take(nparts * kBucketMaxTiles * sizeof(uint32_t)));
 	for (int i = 0; i < 2; i++) s.digit_counts[i] = reinterpret_cast<uint32_t *>(take(nparts * kDigits * sizeof(uint32_t)));
 	for (int i = 0; i < 2; i++) s.digit_totals[i] = reinterpret_cast<uint32_t *>(take(kDigits * sizeof(uint32_t)));
 	s.bytes = (size_t)(p - reinterpret_cast<char *>(base));
@@ -450,17 +470,20 @@ static BucketScratch carve_bucket(void *base, int64_t slots) {
 }
 size_t bucket_scratch_bytes(int64_t slots) { return carve_bucket(nullptr, slots).bytes; }
 
+// TILES: tile_totals[2 t] += this partition's instances of tile t (ranges[t].y, zeroed by the caller)
 template <bool TILES>
 __global__ void __launch_bounds__(kBucketThreads) bucket_count_kernel(const uint16_t *__restrict__ keys, const uint32_t *__restrict__ status,
-                                                                    const uint32_t ntile, uint32_t *__restrict__ tile_counts,
+                                                                    const uint32_t ntile, uint32_t *__restrict__ tile_totals,
                                                                     uint32_t *__restrict__ digit_counts) {
 	extern __shared__ uint32_t s_hist[];  // TILES: per tile id of keys_in; else per high digit of the intermediate words
-	const uint32_t E = status[3];
-	const uint32_t begin = blockIdx.x * kBucketPart;
+	__shared__ uint32_t s_digit[kDigits];
+	const uint32_t E = status[3], part = bucket_part(E);
+	const uint32_t begin = blockIdx.x * part;
 	if (begin >= E) return;  // (rows past the last partition are never read)
-	const uint32_t end = min(begin + kBucketPart, E);
+	const uint32_t end = min(begin + part, E);
 	const uint32_t nbin = TILES ? ntile : (uint32_t)kDigits;
 	for (uint32_t t = threadIdx.x; t < nbin; t += kBucketThreads) s_hist[t] = 0u;
+	if (TILES && threadIdx.x < kDigits) s_digit[threadIdx.x] = 0u;
 	__syncthreads();
 	if (!TILES) {
 		const uint32_t *words = reinterpret_cast<const uint32_t *>(keys);
@@ -488,45 +511,44 @@ __global__ void __launch_bounds__(kBucketThreads) bucket_count_kernel(const uint
 	__syncthreads();
 	uint32_t *drow = digit_counts + (size_t)blockIdx.x * kDigits;
 	if (TILES) {
-		uint32_t *row = tile_counts + (size_t)blockIdx.x * ntile;
-		for (uint32_t t = threadIdx.x; t < ntile; t += kBucketThreads) row[t] = s_hist[t];
-		for (uint32_t d = threadIdx.x; d < (uint32_t)kDigits; d += kBucketThreads) {  // low digit = tile id mod 128
-			uint32_t sum = 0u;
-			for (uint32_t t = d; t < ntile; t += kDigits) sum += s_hist[t];
-			drow[d] = sum;
+		// thread i visits the tiles i + 512 k, which all have the low digit (tile id mod 128) i mod 128
+		uint32_t dsum = 0u;
+		for (uint32_t t = threadIdx.x; t < ntile; t += kBucketThreads) {
+			const uint32_t c = s_hist[t];
+			if (c) atomicAdd(&tile_totals[2 * (size_t)t], c);
+			dsum += c;
 		}
+		atomicAdd(&s_digit[threadIdx.x & (kDigits - 1)], dsum);
+		__syncthreads();
+		if (threadIdx.x < kDigits) drow[threadIdx.x] = s_digit[threadIdx.x];
 	} else {
 		for (uint32_t d = threadIdx.x; d < (uint32_t)kDigits; d += kBucketThreads) drow[d] = s_hist[d];
 	}
 }
 
-// 32 columns per CTA (one per lane: coalesced rows), the partitions split into 32 contiguous slices (one per warp).  Each warp sums
-// its slice and the slice totals are scanned across the warps in shared memory: totals[c * stride] = the column total and, with
-// `prefix`, the slice is rewritten as the exclusive prefix over the partitions.
+// The (partition x digit) matrix: 32 digits per CTA (one per lane: coalesced rows), the partitions split into 32 contiguous slices
+// (one per warp).  Each warp sums its slice and the slice totals are scanned across the warps in shared memory: totals[d] = the
+// digit's total, and the slice is rewritten as the exclusive prefix over the partitions.
 __global__ void __launch_bounds__(1024) bucket_columns_kernel(uint32_t *__restrict__ counts, const uint32_t *__restrict__ status,
-                                                             const uint32_t ncol, uint32_t *__restrict__ totals, const uint32_t stride,
-                                                             const bool prefix) {
+                                                             uint32_t *__restrict__ totals) {
 	__shared__ uint32_t s_tot[32][33];
-	const uint32_t nparts = (status[3] + kBucketPart - 1) / kBucketPart;
+	const uint32_t E = status[3], part = bucket_part(E);
+	const uint32_t nparts = E / part + (E % part != 0u);
 	const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
 	const uint32_t c = blockIdx.x * 32u + lane;
 	const uint32_t per = (nparts + 31u) / 32u;
 	const uint32_t p0 = min(w * per, nparts), p1 = min(p0 + per, nparts);
 	uint32_t sum = 0u;
-	if (c < ncol) {
 #pragma unroll 4
-		for (uint32_t p = p0; p < p1; p++) sum += counts[(size_t)p * ncol + c];
-	}
+	for (uint32_t p = p0; p < p1; p++) sum += counts[(size_t)p * kDigits + c];
 	s_tot[w][lane] = sum;
 	__syncthreads();
 	uint32_t run = 0u;
 	for (uint32_t v = 0; v < w; v++) run += s_tot[v][lane];
-	if (c >= ncol) return;
-	if (w == 31u) totals[(size_t)c * stride] = run + sum;
-	if (!prefix) return;
+	if (w == 31u) totals[c] = run + sum;
 	for (uint32_t p = p0; p < p1; p++) {
-		const uint32_t x = counts[(size_t)p * ncol + c];
-		counts[(size_t)p * ncol + c] = run;
+		const uint32_t x = counts[(size_t)p * kDigits + c];
+		counts[(size_t)p * kDigits + c] = run;
 		run += x;
 	}
 }
@@ -598,10 +620,10 @@ __global__ void __launch_bounds__(kPassThreads) bucket_pass_kernel(const uint16_
 	__shared__ uint16_t s_keys[kPassRound];
 	__shared__ uint32_t s_cursor[kDigits];  // per digit: output position of the first instance of this round
 	__shared__ uint32_t s_pref[kDigits];    // per digit: its first position in the round's digit order
-	const uint32_t E = status[3];
-	const uint32_t begin = blockIdx.x * kBucketPart;
+	const uint32_t E = status[3], part = bucket_part(E);
+	const uint32_t begin = blockIdx.x * part;
 	if (begin >= E) return;
-	const uint32_t end = min(begin + kBucketPart, E);
+	const uint32_t end = min(begin + part, E);
 	const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
 	if (threadIdx.x < 32) {  // digit starts (exclusive scan of the totals, 4 digits per lane) + this partition's prefix
 		const uint4 t4 = reinterpret_cast<const uint4 *>(totals)[lane];
@@ -674,20 +696,20 @@ static cudaError_t launch_bucketing(const BinView &b, ImgView img, const uint32_
 	cudaError_t e;
 	if ((e = ensure_dynamic_smem(bucket_count_kernel<true>, kBucketMaxTiles * sizeof(uint32_t), smem_count)) != cudaSuccess) return e;
 	const BucketScratch sc = carve_bucket(b.bucket, slots);
-	const unsigned nparts = (unsigned)((slots + kBucketPart - 1) / kBucketPart);
+	const unsigned nparts = bucket_grid(slots);
 	const uint16_t *keys = reinterpret_cast<const uint16_t *>(b.keys_in);
-	count_launch(8);
-	bucket_count_kernel<true><<<nparts, kBucketThreads, (size_t)ntile * sizeof(uint32_t), st>>>(keys, status, (uint32_t)ntile, sc.tile_counts,
-	                                                                                          sc.digit_counts[0]);
-	bucket_columns_kernel<<<(unsigned)((ntile + 31) / 32), 1024, 0, st>>>(sc.tile_counts, status, (uint32_t)ntile,
-	                                                                      reinterpret_cast<uint32_t *>(img.ranges) + 1, 2u, false);
+	// the tile totals accumulate in ranges[t].y (the far pass kept its unsaturated-tile table there until now)
+	if ((e = cudaMemsetAsync(img.ranges, 0, (size_t)ntile * sizeof(uint2), st)) != cudaSuccess) return e;
+	count_launch(7);
+	bucket_count_kernel<true><<<nparts, kBucketThreads, (size_t)ntile * sizeof(uint32_t), st>>>(
+		keys, status, (uint32_t)ntile, reinterpret_cast<uint32_t *>(img.ranges) + 1, sc.digit_counts[0]);
 	bucket_ranges_kernel<<<1, 1024, 0, st>>>(img.ranges, (uint32_t)ntile);
-	bucket_columns_kernel<<<kDigits / 32, 1024, 0, st>>>(sc.digit_counts[0], status, kDigits, sc.digit_totals[0], 1u, true);
+	bucket_columns_kernel<<<kDigits / 32, 1024, 0, st>>>(sc.digit_counts[0], status, sc.digit_totals[0]);
 	uint32_t *mid = b.keys_out;
 	bucket_pass_kernel<false><<<nparts, kPassThreads, 0, st>>>(keys, b.vals_in, status, sc.digit_counts[0], sc.digit_totals[0], mid);
 	bucket_count_kernel<false><<<nparts, kBucketThreads, kDigits * sizeof(uint32_t), st>>>(reinterpret_cast<const uint16_t *>(mid), status,
 	                                                                                     0u, nullptr, sc.digit_counts[1]);
-	bucket_columns_kernel<<<kDigits / 32, 1024, 0, st>>>(sc.digit_counts[1], status, kDigits, sc.digit_totals[1], 1u, true);
+	bucket_columns_kernel<<<kDigits / 32, 1024, 0, st>>>(sc.digit_counts[1], status, sc.digit_totals[1]);
 	bucket_pass_kernel<true><<<nparts, kPassThreads, 0, st>>>(nullptr, mid, status, sc.digit_counts[1], sc.digit_totals[1], b.vals_out);
 	return cudaGetLastError();
 }
@@ -775,7 +797,9 @@ __global__ void split_status_kernel(const uint32_t *__restrict__ offsets, int n,
 }
 
 // thread t = t-th Gaussian in depth order: its instance count in the emitted sequence.  Near Gaussians keep their scanned count;
-// a far one counts the tiles of its rectangle that the near blend left unsaturated, by the code emit_pairs / emit_big run.
+// a far one counts the tiles of its rectangle that the near blend left unsaturated, by the code emit_pairs / emit_big run.  Every
+// row span of that walk lies inside the rectangle, so a rectangle without an unsaturated tile (four table loads) counts 0 without it:
+// on config C almost every tile saturates in the near slab, and most far Gaussians stop there.
 __global__ void __launch_bounds__(256) far_count_kernel(const FrameDev f, const GaussRec *__restrict__ rec, const int32_t *__restrict__ radii,
                                                        const uint32_t *__restrict__ perm, const uint32_t *__restrict__ offsets,
                                                        const uint32_t *__restrict__ status, const int n_order,
@@ -792,10 +816,13 @@ __global__ void __launch_bounds__(256) far_count_kernel(const FrameDev f, const 
 			c = end - off;
 		} else if (end > off) {
 			const uint32_t gidx = perm[t];
-			const float4 q0 = rec[gidx].q0, q1 = rec[gidx].q1;
+			const float4 q0 = rec[gidx].q0;
 			tile_rect(q0.x, q0.y, radii[gidx], f.gx, f.gy, x0, y0, x1, y1);
-			cp = make_cull(q0.x, q0.y, q0.z, q0.w, q1.x, q1.y);
-			active = true;
+			if (x1 > x0 && y1 > y0 && keep.rect(y0, y1, x0, x1) != 0u) {
+				const float4 q1 = rec[gidx].q1;
+				cp = make_cull(q0.x, q0.y, q0.z, q0.w, q1.x, q1.y);
+				active = true;
+			}
 		}
 	}
 	uint32_t count = 0u;
@@ -804,20 +831,40 @@ __global__ void __launch_bounds__(256) far_count_kernel(const FrameDev f, const 
 	if (t < n_order) cnt[t] = active ? count : c;
 }
 
-// one warp per tile row, after the near blend: prefix[ty * (gx + 1) + tx] = unsaturated tiles (top bit of tile_max_contrib) before
-// column tx, for KeepUnsaturated.  prefix lives in the img ranges, which are free from the near blend until the final bucketing.
-__global__ void __launch_bounds__(32) unsat_prefix_kernel(const uint32_t *__restrict__ tile_word, const int gx, uint32_t *__restrict__ prefix) {
-	const int ty = blockIdx.x, lane = threadIdx.x;
-	uint32_t *row = prefix + (size_t)ty * (gx + 1);
-	uint32_t carry = 0u;
-	for (int t0 = 0; t0 < gx; t0 += 32) {
-		const int tx = t0 + lane;
-		const bool u = tx < gx && (tile_word[(size_t)ty * gx + tx] >> 31) != 0u;
-		const unsigned m = __ballot_sync(0xffffffffu, u);
-		if (tx < gx) row[tx] = carry + (uint32_t)__popc(m & ((1u << lane) - 1u));
-		carry += (uint32_t)__popc(m);
+// one CTA, after the near blend: the table of KeepUnsaturated, sat[y * (gx + 1) + x] = unsaturated tiles (top bit of
+// tile_max_contrib) in rows < y and columns < x.  The warps prefix the tile rows, then the threads the columns.  sat lives in the img
+// ranges, which are free from the near blend until the final bucketing: (gx + 1)(gy + 1) <= 2 gx gy + 2 words.
+constexpr int kSatBatch = 16;  // rows loaded ahead by each column thread
+__global__ void __launch_bounds__(1024) unsat_prefix_kernel(const uint32_t *__restrict__ tile_word, const int gx, const int gy, uint32_t *sat) {
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	const int stride = gx + 1;
+	for (int x = threadIdx.x; x < stride; x += blockDim.x) sat[x] = 0u;
+	for (int ty = warp; ty < gy; ty += 32) {
+		uint32_t *row = sat + (size_t)(ty + 1) * stride;
+		if (lane == 0) row[0] = 0u;
+		uint32_t carry = 0u;
+		for (int t0 = 0; t0 < gx; t0 += 32) {
+			const int tx = t0 + lane;
+			const bool u = tx < gx && (tile_word[(size_t)ty * gx + tx] >> 31) != 0u;
+			const unsigned m = __ballot_sync(0xffffffffu, u);
+			if (tx < gx) row[tx + 1] = carry + (uint32_t)__popc(m & (0xffffffffu >> (31 - lane)));
+			carry += (uint32_t)__popc(m);
+		}
 	}
-	if (lane == 0) row[gx] = carry;
+	__syncthreads();  // (also orders the rows' global stores before the column pass reads them)
+	for (int x = threadIdx.x; x < stride; x += blockDim.x) {
+		uint32_t run = 0u;
+		for (int y0 = 1; y0 <= gy; y0 += kSatBatch) {
+			uint32_t v[kSatBatch];
+#pragma unroll
+			for (int j = 0; j < kSatBatch; j++) v[j] = y0 + j <= gy ? sat[(size_t)(y0 + j) * stride + x] : 0u;
+#pragma unroll
+			for (int j = 0; j < kSatBatch; j++) {
+				run += v[j];
+				if (y0 + j <= gy) sat[(size_t)(y0 + j) * stride + x] = run;
+			}
+		}
+	}
 }
 
 // one thread, after the scan of far_count_kernel's counts: E = the instances emitted.  A bounded frame overflows only if the emitted
@@ -861,12 +908,12 @@ cudaError_t launch_far_binning(const FrameDev &f, GeomView g, const int32_t *rad
                                int64_t cap, int n_order) {
 	const uint32_t cap32 = cap >= 0 ? (uint32_t)cap : 0xffffffffu;
 	const unsigned nblk = (unsigned)((n_order + 255) / 256);
-	uint32_t *prefix = reinterpret_cast<uint32_t *>(img.ranges);  // (gx + 1) gy <= 2 (ntile + 1) words
-	const KeepUnsaturated keep{prefix, f.gx + 1};
+	uint32_t *sat = reinterpret_cast<uint32_t *>(img.ranges);  // (gx + 1)(gy + 1) <= 2 (ntile + 1) words
+	const KeepUnsaturated keep{sat, f.gx + 1};
 	uint32_t *far_offsets = g.ckey;
 	uint16_t *kin = reinterpret_cast<uint16_t *>(b.keys_in);
 	count_launch(2);
-	unsat_prefix_kernel<<<f.gy, 32, 0, st>>>(img.tile_max_contrib, f.gx, prefix);
+	unsat_prefix_kernel<<<1, 1024, 0, st>>>(img.tile_max_contrib, f.gx, f.gy, sat);
 	far_count_kernel<<<nblk, 256, 0, st>>>(f, g.rec, radii, g.perm, g.offsets, g.big_count, n_order, keep, g.iota);
 	cudaError_t e = cudaGetLastError();
 	if (e != cudaSuccess) return e;

@@ -95,17 +95,20 @@ struct KeepAll {  // every tile (one binning pass per frame)
 	__device__ __forceinline__ uint32_t span(int, int xb, int xe) const { return (uint32_t)(xe - xb); }
 	__device__ __forceinline__ bool tile(int, int) const { return true; }
 };
-// Far pass of the saturation split (binning.cu): only the tiles the near pass left unsaturated.  prefix[ty * (gx + 1) + tx] = number
-// of unsaturated tiles before column tx of row ty (unsat_prefix_kernel), so a row span costs two loads, as KeepAll's costs none.
+// Far pass of the saturation split (binning.cu): only the tiles the near pass left unsaturated.  sat[y * (gx + 1) + x] = number of
+// unsaturated tiles in rows < y and columns < x (unsat_prefix_kernel), so any rectangle of tiles, a row span included, costs four
+// loads.
 struct KeepUnsaturated {
 	static constexpr bool kAll = false;
-	const uint32_t *prefix;
+	const uint32_t *sat;
 	int stride;  // gx + 1
-	__device__ __forceinline__ uint32_t span(int ty, int xb, int xe) const {
-		const uint32_t *row = prefix + (size_t)ty * stride;
-		return xe > xb ? row[xe] - row[xb] : 0u;
+	// unsaturated tiles in rows [y0, y1) x columns [x0, x1) (y0 <= y1, x0 <= x1)
+	__device__ __forceinline__ uint32_t rect(int y0, int y1, int x0, int x1) const {
+		const uint32_t *a = sat + (size_t)y0 * stride, *b = sat + (size_t)y1 * stride;
+		return (b[x1] - b[x0]) - (a[x1] - a[x0]);
 	}
-	__device__ __forceinline__ bool tile(int ty, int tx) const { return span(ty, tx, tx + 1) != 0u; }
+	__device__ __forceinline__ uint32_t span(int ty, int xb, int xe) const { return xe > xb ? rect(ty, ty + 1, xb, xe) : 0u; }
+	__device__ __forceinline__ bool tile(int ty, int tx) const { return rect(ty, ty + 1, tx, tx + 1) != 0u; }
 };
 
 template <bool EMIT, typename KeyT = uint32_t, typename Keep = KeepAll>

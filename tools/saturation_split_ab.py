@@ -9,14 +9,19 @@ current.  For each build, per round and alternating:
   * in a separate profiled run, the device time per step of every kernel from torch.profiler.
 The two builds' outputs of one step are compared first (images and radii bit-equal, largest gradient differences), and the
 instances each build emits (status word 3) are read from an exact-mode forward.  --sweep also times the new build at the budgets
-R / d for each d given (the rule of the library is R / 8).
+R / d for each d given (the rule of the library is R / 8).  --sweep-parts builds one more library per value n, with the bucketing's
+partition target (csrc/binning.cu kBucketTargetParts) set to n, and times and profiles each next to parent and new.
 Prints one JSON line with the GPU name and its enforced power limit.
 
-python tools/saturation_split_ab.py --parent PATH/libsgr.so [--new PATH/libsgr.so] [--rounds 3] [--steps 50] [--sweep 16 8 4 2]"""
+python tools/saturation_split_ab.py --parent PATH/libsgr.so [--new PATH/libsgr.so] [--rounds 3] [--steps 50] [--sweep 16 8 4 2]
+                                    [--sweep-parts 132 264 396 528]"""
 import argparse
 import json
 import os
+import subprocess
 import sys
+import tempfile
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
@@ -42,20 +47,47 @@ def load(path, symbols):
         _capi.SYMBOLS = saved
 
 
+def build_target_parts(values, out_dir):
+    """One libsgr.so per partition target: binning.cu recompiled with SGR_BUCKET_TARGET_PARTS=n, linked with the objects build()
+    left in the package's _obj/."""
+    from street_gaussians_b200 import build as B
+    nvcc = B._nvcc()
+    others = [os.path.join(B.OBJ, s + ".o") for s in B.SOURCES if s != "binning.cu"]
+    missing = [o for o in others if not os.path.exists(o)]
+    if values and missing:
+        raise SystemExit(f"--sweep-parts links the objects of the package build; missing: {missing}")
+
+    def one(n):
+        obj, lib = os.path.join(out_dir, f"binning_{n}.o"), os.path.join(out_dir, f"libsgr_parts{n}.so")
+        subprocess.run([nvcc, "-c", os.path.join(B.CSRC, "binning.cu"), "-o", obj, f"-DSGR_BUCKET_TARGET_PARTS={n}"] + B.NVCC_FLAGS,
+                       check=True)
+        subprocess.run([nvcc, "-shared", "-o", lib, obj] + others + ["-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC"],
+                       check=True)
+        return lib
+
+    with ThreadPoolExecutor(max_workers=max(1, len(values))) as ex:
+        return dict(zip(values, ex.map(one, values)))
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--parent", required=True, help="libsgr.so of the build to compare against (without the split)")
+    ap.add_argument("--parent", required=True, help="libsgr.so of the build to compare against")
     ap.add_argument("--new", default=_capi.LIB_PATH)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--profile-steps", type=int, default=10)
     ap.add_argument("--sweep", type=int, nargs="*", default=[], help="divisors d: also time the new build at budget R / d")
+    ap.add_argument("--sweep-parts", type=int, nargs="*", default=[],
+                    help="partition targets n: also time and profile the new sources built with SGR_BUCKET_TARGET_PARTS=n")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         print(json.dumps({"error": "no CUDA device"}))
         return 1
     old_symbols = [s for s in _capi.SYMBOLS if s != "sgr_set_near_budget"]
     libs = {"parent": load(os.path.abspath(args.parent), old_symbols), "new": load(os.path.abspath(args.new), _capi.SYMBOLS)}
+    tmp = tempfile.TemporaryDirectory(prefix="sgr_parts_")
+    for n, path in build_target_parts(args.sweep_parts, tmp.name).items():
+        libs[f"parts={n}"] = load(path, _capi.SYMBOLS)
 
     scene = synthetic.make_config("C", seed=0)
     cam = scene["cam"]
@@ -67,7 +99,7 @@ def main():
         image_height=cam["image_height"], image_width=cam["image_width"], tanfovx=cam["tanfovx"], tanfovy=cam["tanfovy"],
         bg=cam["bg"].to(DEV), scale_modifier=cam["scale_modifier"], viewmatrix=cam["viewmatrix"].to(DEV),
         projmatrix=cam["projmatrix"].to(DEV), sh_degree=cam["sh_degree"], campos=cam["campos"].to(DEV), prefiltered=False, debug=False)
-    variants = {"parent": ("parent", None), "new": ("new", None)}
+    variants = {name: (name, None) for name in libs}
     rast = {k: sgb.GaussianRasterizer(settings, capacity=sgb.InstanceCapacity()) for k in variants}
 
     def emitted(name):
@@ -138,8 +170,8 @@ def main():
             torch.cuda.synchronize()
             step_ms[name].append(e0.elapsed_time(e1) / args.steps)
 
-    # ---- kernel times (profiled separately), alternating: parent and new only ----
-    kern_us = {k: {} for k in ("parent", "new")}
+    # ---- kernel times (profiled separately), alternating: each library at its own budget rule ----
+    kern_us = {k: {} for k in libs}
     for _ in range(args.rounds):
         for name in kern_us:
             step(name)
@@ -154,7 +186,7 @@ def main():
     table = {}
     for name in kern_us:
         for k, v in kern_us[name].items():
-            table.setdefault(k, {"parent": 0.0, "new": 0.0})[name] = round(float(np.median(v)), 1)
+            table.setdefault(k, {n: 0.0 for n in kern_us})[name] = round(float(np.median(v)), 1)
     table = dict(sorted(table.items(), key=lambda kv: -max(kv[1].values())))
 
     _, E_new = emitted("new")
