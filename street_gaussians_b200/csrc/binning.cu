@@ -16,7 +16,6 @@
 #include <cub/block/block_scan.cuh>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
-#include <cub/device/device_select.cuh>
 #include <cub/iterator/counting_input_iterator.cuh>
 #include <cub/iterator/transform_input_iterator.cuh>
 
@@ -33,10 +32,6 @@ struct GatherCount {
 		return depth_sorted[t] == 0xffffffffu ? 0u : tiles_touched[perm[t]];
 	}
 };
-struct WasDelivered {  // (predicate of the round-2 second-cut stream compaction; only sizes the temp storage now — the run tables replaced it)
-	const int32_t *radii;
-	__host__ __device__ __forceinline__ bool operator()(int i) const { return radii[i] > 0; }
-};
 using CountIter = cub::TransformInputIterator<uint32_t, GatherCount, cub::CountingInputIterator<int>>;
 
 // Frames of up to this many tiles bucket their instances by tile (launch_bucketing below): the per-tile histogram and cursors
@@ -46,16 +41,13 @@ constexpr int kBucketMaxTiles = 16384;
 size_t geom_temp_bytes(int P) {
 	const int n = P > 0 ? P : 1;
 	size_t a = 0, b = 0;
-	size_t c = 0;
 	CountIter it(cub::CountingInputIterator<int>(0), GatherCount{nullptr, nullptr, nullptr});
 	cub::DeviceScan::InclusiveSum(nullptr, a, it, (uint32_t *)nullptr, n);
 	size_t d = 0;  // the far pass of the saturation split scans a plain count array
 	cub::DeviceScan::InclusiveSum(nullptr, d, (const uint32_t *)nullptr, (uint32_t *)nullptr, n);
 	a = a > d ? a : d;
 	cub::DeviceRadixSort::SortPairs(nullptr, b, (uint32_t *)nullptr, (uint32_t *)nullptr, (uint32_t *)nullptr, (uint32_t *)nullptr, n);
-	cub::DeviceSelect::If(nullptr, c, cub::CountingInputIterator<int>(0), (uint32_t *)nullptr, (uint32_t *)nullptr, n, WasDelivered{nullptr});
-	a = a > b ? a : b;
-	return a > c ? a : c;
+	return a > b ? a : b;
 }
 size_t sort_temp_bytes(int64_t R) {
 	size_t a = 0, b = 0;
@@ -65,9 +57,29 @@ size_t sort_temp_bytes(int64_t R) {
 	return a > b ? a : b;
 }
 
+// A Gaussian's footprint on the tile grid, from its record and radius: the 3-sigma tile rectangle [x0, x1) x [y0, y1) and the
+// parameters of the exact cull.  The default (empty) footprint is what a thread without a Gaussian hands to visit_tiles.
+struct Footprint {
+	int x0 = 0, y0 = 0, x1 = 0, y1 = 0;
+	CullParams cp = {};
+};
+__device__ __forceinline__ Footprint rec_footprint(const FrameDev &f, const GaussRec &rec, int radius) {
+	const float4 q0 = rec.q0, q1 = rec.q1;
+	Footprint fp;
+	tile_rect(q0.x, q0.y, radius, f.gx, f.gy, fp.x0, fp.y0, fp.x1, fp.y1);
+	fp.cp = make_cull(q0.x, q0.y, q0.z, q0.w, q1.x, q1.y);
+	return fp;
+}
+// clears row i of a grad2d[P, 12] (nullable)
+__device__ __forceinline__ void zero_grad2d_row(float4 *__restrict__ rows, size_t i) {
+	if (!rows) return;
+	const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+	rows[3 * i] = z; rows[3 * i + 1] = z; rows[3 * i + 2] = z;
+}
+
 // Gaussian-sharded mode (include/sgr.h, sgr_forward_records): the records were projected on other ranks and gathered, so
 // the tail of preprocess_fwd_kernel — instance count against THIS rank's tile-row band, depth sort key, identity
-// permutation — runs here from the 48-B record + radius.  Same tile_rect / make_cull / visit_tiles as the emission
+// permutation — runs here from the 48-B record + radius.  Same rec_footprint / visit_tiles as the emission
 // kernels below, so counts and emitted ranges agree by construction.
 // zero_rows (nullable): this rank's partial grad2d[P,12].  The rows of the Gaussians delivered to this rank (radius != 0 <=>
 // rectangle meets the band) are the only ones its blend_bwd can touch and the only ones their owners read back, so they are
@@ -79,25 +91,19 @@ __global__ void __launch_bounds__(256) count_tiles_kernel(const FrameDev f, cons
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	const bool in_range = idx < f.P;
 	bool ok = false;
-	int x0 = 0, y0 = 0, x1 = 0, y1 = 0;
-	CullParams cp = {};
+	Footprint fp;
 	float depth = 0.f;
 	if (in_range) {
 		const int r = radii[idx];
 		if (r > 0) {
-			const float4 q0 = rec[idx].q0, q1 = rec[idx].q1;
-			tile_rect(q0.x, q0.y, r, f.gx, f.gy, x0, y0, x1, y1);
-			cp = make_cull(q0.x, q0.y, q0.z, q0.w, q1.x, q1.y);
-			depth = q1.w;
+			fp = rec_footprint(f, rec[idx], r);
+			depth = rec[idx].q1.w;
 			ok = true;
-			if (zero_rows) {
-				const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-				zero_rows[3 * (size_t)idx] = z; zero_rows[3 * (size_t)idx + 1] = z; zero_rows[3 * (size_t)idx + 2] = z;
-			}
+			zero_grad2d_row(zero_rows, idx);
 		}
 	}
 	uint32_t count = 0;
-	visit_tiles<false, uint32_t>(ok, x0, y0, x1, y1, cp, f.band, f.gx, 0u, 0u, nullptr, nullptr, count);
+	visit_tiles<false, uint32_t>(ok, fp.x0, fp.y0, fp.x1, fp.y1, fp.cp, f.band, f.gx, 0u, 0u, nullptr, nullptr, count);
 	if (in_range) {
 		tiles_touched[idx] = count;
 		depth_key[idx] = count > 0 ? __float_as_uint(depth) : 0xffffffffu;
@@ -112,17 +118,23 @@ cudaError_t launch_count_tiles(const FrameDev &f, GeomView g, const int32_t *rad
 	return cudaGetLastError();
 }
 
+// n (depth key, Gaussian) pairs sorted into g.depth_sorted / g.perm, then the inclusive scan of the Gaussians' instance counts
+// (g.tiles_touched) in that order into g.offsets
+static cudaError_t sort_and_scan_depth(GeomView g, const uint32_t *keys, const uint32_t *vals, int n, cudaStream_t st) {
+	size_t bytes = g.temp_bytes;
+	cudaError_t e = cub::DeviceRadixSort::SortPairs(g.temp, bytes, keys, g.depth_sorted, vals, g.perm, n, 0, 32, st);
+	if (e != cudaSuccess) return e;
+	CountIter it(cub::CountingInputIterator<int>(0), GatherCount{g.tiles_touched, g.perm, g.depth_sorted});
+	bytes = g.temp_bytes;
+	return cub::DeviceScan::InclusiveSum(g.temp, bytes, it, g.offsets, n, st);
+}
+
 // depth order of the Gaussians + inclusive scan of their instance counts in that order (uncompacted: all f.P Gaussians take part,
 // those without instances carry the key 0xFFFFFFFF and sort to the end).  tiles_touched / depth_key / iota come from
 // preprocess_fwd_kernel<COUNT> or count_tiles_kernel.
 cudaError_t launch_depth_order(const FrameDev &f, GeomView g, cudaStream_t st) {
 	if (f.P == 0) return cudaSuccess;
-	size_t bytes = g.temp_bytes;
-	cudaError_t e = cub::DeviceRadixSort::SortPairs(g.temp, bytes, g.depth_key, g.depth_sorted, g.iota, g.perm, f.P, 0, 32, st);
-	if (e != cudaSuccess) return e;
-	CountIter it(cub::CountingInputIterator<int>(0), GatherCount{g.tiles_touched, g.perm, g.depth_sorted});
-	bytes = g.temp_bytes;
-	return cub::DeviceScan::InclusiveSum(g.temp, bytes, it, g.offsets, f.P, st);
+	return sort_and_scan_depth(g, g.depth_key, g.iota, f.P, st);
 }
 
 // ---- fused Gaussian-sharded forward: the delivered runs (sgr_common.cuh "block-run exchange") -> compact depth-sort input ----
@@ -178,8 +190,7 @@ __global__ void __launch_bounds__(256) count_runs_kernel(const FrameDev f, const
 	if (j == 0 && n_act > cap_v) atomicOr(&status[2], 2u);
 	const bool live = j < n_act && j < cap_v;
 	bool ok = false;
-	int x0 = 0, y0 = 0, x1 = 0, y1 = 0;
-	CullParams cp = {};
+	Footprint fp;
 	float depth = 0.f;
 	uint32_t gidx = 0u;
 	if (live) {
@@ -190,20 +201,15 @@ __global__ void __launch_bounds__(256) count_runs_kernel(const FrameDev f, const
 		}
 		const uint32_t s = lo / nblk, b = lo - s * nblk;
 		gidx = (uint32_t)((long long)s * chunk + (long long)b * kRunBlock) + (j - pre[lo]);
-		const float4 q0 = rec[gidx].q0, q1 = rec[gidx].q1;
 		const int r = packed_radius(rec[gidx].q2.w);
 		radii[gidx] = r;  // emit_pairs / emit_big read the radius from here
-		tile_rect(q0.x, q0.y, r, f.gx, f.gy, x0, y0, x1, y1);
-		cp = make_cull(q0.x, q0.y, q0.z, q0.w, q1.x, q1.y);
-		depth = q1.w;
+		fp = rec_footprint(f, rec[gidx], r);
+		depth = rec[gidx].q1.w;
 		ok = true;
-		if (zero_rows) {
-			const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-			zero_rows[3 * (size_t)gidx] = z; zero_rows[3 * (size_t)gidx + 1] = z; zero_rows[3 * (size_t)gidx + 2] = z;
-		}
+		zero_grad2d_row(zero_rows, gidx);
 	}
 	uint32_t count = 0;
-	visit_tiles<false, uint32_t>(ok, x0, y0, x1, y1, cp, f.band, f.gx, 0u, 0u, nullptr, nullptr, count);
+	visit_tiles<false, uint32_t>(ok, fp.x0, fp.y0, fp.x1, fp.y1, fp.cp, f.band, f.gx, 0u, 0u, nullptr, nullptr, count);
 	if (j < cap_v) {
 		ckey[j] = (live && count > 0u) ? __float_as_uint(depth) : 0xffffffffu;
 		cval[j] = gidx;
@@ -228,13 +234,8 @@ cudaError_t launch_count_and_order_runs(const FrameDev &f, GeomView g, int32_t *
 	                                                               g.ckey, g.cval, reinterpret_cast<float4 *>(zero_rows));
 	cudaError_t e = cudaGetLastError();
 	if (e != cudaSuccess) return e;
-	size_t bytes = g.temp_bytes;
-	e = cub::DeviceRadixSort::SortPairs(g.temp, bytes, g.ckey, g.depth_sorted, g.cval, g.perm, n, 0, 32, st);
-	if (e != cudaSuccess) return e;
 	if (n_order) *n_order = n;
-	CountIter it(cub::CountingInputIterator<int>(0), GatherCount{g.tiles_touched, g.perm, g.depth_sorted});
-	bytes = g.temp_bytes;
-	return cub::DeviceScan::InclusiveSum(g.temp, bytes, it, g.offsets, n, st);
+	return sort_and_scan_depth(g, g.ckey, g.cval, n, st);
 }
 
 constexpr uint32_t kEmitStage = 512;  // instances staged per warp (2 x 2 KB of shared memory per warp)
@@ -246,8 +247,7 @@ constexpr uint32_t kEmitStage = 512;  // instances staged per warp (2 x 2 KB of 
 // dev_floor -> the near pass's end (the Gaussians before the split then have empty ranges there) and the KeepUnsaturated predicate.
 template <typename KeyT, typename Keep = KeepAll>
 __global__ void __launch_bounds__(256) emit_pairs_kernel(const FrameDev f, const GaussRec *__restrict__ rec, const int32_t *__restrict__ radii,
-                                                        const uint32_t *__restrict__ /*tiles_touched*/, const uint32_t *__restrict__ perm,
-                                                        const uint32_t *__restrict__ offsets, KeyT *__restrict__ keys,
+                                                        const uint32_t *__restrict__ perm, const uint32_t *__restrict__ offsets, KeyT *__restrict__ keys,
                                                         uint32_t *__restrict__ vals, uint32_t *__restrict__ big_list,
                                                         uint32_t *__restrict__ big_count, uint32_t cap, const int n_order,
                                                         const uint32_t *__restrict__ dev_cap = nullptr,
@@ -257,8 +257,7 @@ __global__ void __launch_bounds__(256) emit_pairs_kernel(const FrameDev f, const
 	const int warp = threadIdx.x >> 5;
 	const int t = blockIdx.x * blockDim.x + threadIdx.x;
 	bool active = false;
-	int x0 = 0, y0 = 0, x1 = 0, y1 = 0;
-	CullParams cp = {};
+	Footprint fp;
 	uint32_t gidx = 0;
 	// [off, end) = this Gaussian's output range (offsets = inclusive scan in depth order); lanes past P get an empty range
 	const int tc = min(t, n_order - 1);  // n_order = depth-order slots: f.P, or the Gaussian capacity of the compacted mode
@@ -281,9 +280,7 @@ __global__ void __launch_bounds__(256) emit_pairs_kernel(const FrameDev f, const
 	if (t < n_order) {
 		if (end > off) {
 			gidx = perm[t];  // (padding slots of the compacted order have end == off and a meaningless perm)
-			const float4 q0 = rec[gidx].q0, q1 = rec[gidx].q1;
-			tile_rect(q0.x, q0.y, radii[gidx], f.gx, f.gy, x0, y0, x1, y1);
-			cp = make_cull(q0.x, q0.y, q0.z, q0.w, q1.x, q1.y);
+			fp = rec_footprint(f, rec[gidx], radii[gidx]);
 			active = true;
 		}
 	}
@@ -291,7 +288,7 @@ __global__ void __launch_bounds__(256) emit_pairs_kernel(const FrameDev f, const
 	const uint32_t warp_last = __shfl_sync(0xffffffffu, end, 31);
 	const uint32_t warp_total = warp_last >= warp_first ? warp_last - warp_first : 0xffffffffu;  // (overflow tail: no staging)
 	uint32_t count;
-	visit_tiles<true, KeyT, Keep>(active, x0, y0, x1, y1, cp, f.band, f.gx, gidx, off, keys, vals, count, s_keys[warp], s_vals[warp],
+	visit_tiles<true, KeyT, Keep>(active, fp.x0, fp.y0, fp.x1, fp.y1, fp.cp, f.band, f.gx, gidx, off, keys, vals, count, s_keys[warp], s_vals[warp],
 	                              kEmitStage, warp_first, warp_total, big_list, big_count, (uint32_t)t, keep);
 }
 
@@ -308,17 +305,29 @@ __global__ void __launch_bounds__(256) emit_big_kernel(const FrameDev f, const G
 	for (uint32_t i = blockIdx.x * 8u + (threadIdx.x >> 5); i < n; i += nwarps) {
 		const uint32_t t = big_list[i];
 		const uint32_t gidx = perm[t];
-		const float4 q0 = rec[gidx].q0, q1 = rec[gidx].q1;
-		int x0, y0, x1, y1;
-		tile_rect(q0.x, q0.y, radii[gidx], f.gx, f.gy, x0, y0, x1, y1);
-		const CullParams cp = make_cull(q0.x, q0.y, q0.z, q0.w, q1.x, q1.y);
+		const Footprint fp = rec_footprint(f, rec[gidx], radii[gidx]);
 		const uint32_t off = t == 0 ? 0u : offsets[t - 1];
 		if (offsets[t] > cap) continue;  // bounded mode overflow (never deferred in practice: emit_pairs already skipped it)
 		// lane 0 carries the Gaussian through the cooperative path of visit_tiles (all other lanes inactive)
 		uint32_t count;
-		visit_tiles<true, KeyT, Keep>(lane == 0, x0, y0, x1, y1, cp, f.band, f.gx, gidx, off, keys, vals, count, nullptr, nullptr, 0u, 0u, 0u,
+		visit_tiles<true, KeyT, Keep>(lane == 0, fp.x0, fp.y0, fp.x1, fp.y1, fp.cp, f.band, f.gx, gidx, off, keys, vals, count, nullptr, nullptr, 0u, 0u, 0u,
 		                              nullptr, nullptr, 0u, keep);
 	}
+}
+
+// the emission of one pass: the instances of depth-order slot t go to [offsets[t - 1], offsets[t]) of (b.keys_in, b.vals_in);
+// status = the status block whose word 0 counts the deferred Gaussians.  dev_cap, dev_floor, keep: see emit_pairs_kernel.
+template <typename KeyT, typename Keep = KeepAll>
+static cudaError_t launch_emit(const FrameDev &f, GeomView g, const int32_t *radii, const BinView &b, const uint32_t *offsets, uint32_t *status,
+                               uint32_t cap32, int n_order, cudaStream_t st, const uint32_t *dev_cap = nullptr,
+                               const uint32_t *dev_floor = nullptr, const Keep keep = Keep()) {
+	KeyT *keys = reinterpret_cast<KeyT *>(b.keys_in);
+	count_launch(2);
+	emit_pairs_kernel<KeyT, Keep><<<(unsigned)((n_order + 255) / 256), 256, 0, st>>>(f, g.rec, radii, g.perm, offsets, keys, b.vals_in,
+	                                                                               g.big_list, status, cap32, n_order, dev_cap, dev_floor, keep);
+	// persistent-style grid for the deferred large rectangles
+	emit_big_kernel<KeyT, Keep><<<kNumSMs * 4, 256, 0, st>>>(f, g.rec, radii, g.perm, offsets, keys, b.vals_in, g.big_list, status, cap32, keep);
+	return cudaGetLastError();
 }
 
 // One thread per sorted instance: a tile's range starts / ends where the tile id changes
@@ -399,6 +408,27 @@ static int bits_for(uint32_t n) {  // smallest b with (1 << b) >= n, i.e. enough
 	return b > 0 ? b : 1;
 }
 
+// the per-tile lists of a frame that does not bucket: a stable radix sort of the R emitted slots by tile id, then the ranges.  The
+// bounded mode (R = its capacity) first pads [emitted, R) with the largest key, so every sort bit of KeyT takes part; the exact mode
+// sorts on the bits the tile ids use.
+template <typename KeyT>
+static cudaError_t launch_tile_sort(const BinView &b, ImgView img, const uint32_t *status, int ntile, int64_t R, bool bounded, cudaStream_t st) {
+	KeyT *kin = reinterpret_cast<KeyT *>(b.keys_in), *kout = reinterpret_cast<KeyT *>(b.keys_out);
+	cudaError_t e;
+	if (bounded) {
+		count_launch();
+		pad_keys_kernel<KeyT><<<(unsigned)std::min<int64_t>(R / 256 + 1, kNumSMs * 8), 256, 0, st>>>(kin, b.vals_in, (uint32_t)R, status);
+		if ((e = cudaGetLastError()) != cudaSuccess) return e;
+	}
+	const int sort_bits = bounded ? 8 * (int)sizeof(KeyT) : bits_for(ntile);
+	size_t bytes = b.sort_temp_bytes;
+	if ((e = cub::DeviceRadixSort::SortPairs(b.sort_temp, bytes, kin, kout, b.vals_in, b.vals_out, R, 0, sort_bits, st)) != cudaSuccess) return e;
+	count_launch();
+	tile_ranges_kernel<KeyT><<<(unsigned)((R + 256 * kRangeKeysPerThread - 1) / (256 * kRangeKeysPerThread)), 256, 0, st>>>(R, kout, img.ranges,
+	                                                                                                                  (uint32_t)ntile);
+	return cudaGetLastError();
+}
+
 // ---- tile bucketing: the per-tile lists as a stable LSD radix sort of the EMITTED instances [0, E) on two 7-bit digits ----
 // Emission already writes the instances in their final within-tile order (ascending depth bits, ties by ascending index), so a
 // stable bucketing by tile id gives exactly the list the tile radix sort gives, over E instead of the whole capacity and without
@@ -451,6 +481,8 @@ constexpr uint32_t kNoGaussian = 0xffffffffu;  // value of the slots of the last
 // the intermediate words carry the high digit in their top 7 bits, so a bucketed frame has at most 2^25 Gaussians
 constexpr int kPackShift = 32 - kDigitBits;
 constexpr uint32_t kPackMask = (1u << kPackShift) - 1u;
+// whether a frame's instances are bucketed (16-bit tile ids) rather than taking the tile radix sort
+static bool bucketable(const FrameDev &f) { return f.gx * f.gy <= kBucketMaxTiles && (uint32_t)f.P <= kPackMask + 1u; }
 
 // the bucketing scratch behind the cub temp of the binning state (carve_bin): the two (partition x digit) count matrices and the
 // digit totals.
@@ -728,47 +760,14 @@ cudaError_t launch_binning(const FrameDev &f, GeomView g, const int32_t *radii, 
 	if ((e = cudaGetLastError()) != cudaSuccess) return e;
 	if (bounded) R = cap;  // every pass below runs over the caller's capacity; the padding carries the largest key
 	if (R == 0) return cudaSuccess;
-	size_t bytes = b.sort_temp_bytes;
-	const unsigned nblk = (unsigned)((n_order + 255) / 256);
-	const unsigned nbig_blk = kNumSMs * 4;  // persistent-style grid for the deferred large rectangles
 	if ((e = cudaMemsetAsync(g.big_count, 0, sizeof(uint32_t), st)) != cudaSuccess) return e;
-	const unsigned npad_blk = bounded ? (unsigned)(cap / 256 + 1 < kNumSMs * 8 ? cap / 256 + 1 : kNumSMs * 8) : 0u;
-	const int sort_bits = bounded ? (ntile <= 65535 ? 16 : 32) : bits_for(ntile);
-	if (ntile <= kBucketMaxTiles && (uint32_t)f.P <= kPackMask + 1u) {  // tile bucketing of the emitted instances (16-bit tile ids)
-		uint16_t *kin = reinterpret_cast<uint16_t *>(b.keys_in);
-		count_launch();
-		emit_pairs_kernel<uint16_t><<<nblk, 256, 0, st>>>(f, g.rec, radii, g.tiles_touched, g.perm, g.offsets, kin, b.vals_in, g.big_list, g.big_count, cap32, n_order);
-		count_launch();
-		emit_big_kernel<uint16_t><<<nbig_blk, 256, 0, st>>>(f, g.rec, radii, g.perm, g.offsets, kin, b.vals_in, g.big_list, g.big_count, cap32);
-		if ((e = cudaGetLastError()) != cudaSuccess) return e;
-		return launch_bucketing(b, img, g.big_count, ntile, R, st);
-	} else if (ntile <= 65535 || (!bounded && ntile <= 65536)) {  // 16-bit tile ids (the key arrays are allocated for 32-bit ids either way)
-		uint16_t *kin = reinterpret_cast<uint16_t *>(b.keys_in), *kout = reinterpret_cast<uint16_t *>(b.keys_out);
-		count_launch();
-		emit_pairs_kernel<uint16_t><<<nblk, 256, 0, st>>>(f, g.rec, radii, g.tiles_touched, g.perm, g.offsets, kin, b.vals_in, g.big_list, g.big_count, cap32, n_order);
-		count_launch();
-		emit_big_kernel<uint16_t><<<nbig_blk, 256, 0, st>>>(f, g.rec, radii, g.perm, g.offsets, kin, b.vals_in, g.big_list, g.big_count, cap32);
-		if (bounded) count_launch();
-		if (bounded) pad_keys_kernel<uint16_t><<<npad_blk, 256, 0, st>>>(kin, b.vals_in, cap32, g.big_count);
-		if ((e = cudaGetLastError()) != cudaSuccess) return e;
-		e = cub::DeviceRadixSort::SortPairs(b.sort_temp, bytes, kin, kout, b.vals_in, b.vals_out, R, 0, sort_bits, st);
-		if (e != cudaSuccess) return e;
-		count_launch();
-		tile_ranges_kernel<uint16_t><<<(unsigned)((R + 256 * kRangeKeysPerThread - 1) / (256 * kRangeKeysPerThread)), 256, 0, st>>>(R, kout, img.ranges, (uint32_t)ntile);
-	} else {
-		count_launch();
-		emit_pairs_kernel<uint32_t><<<nblk, 256, 0, st>>>(f, g.rec, radii, g.tiles_touched, g.perm, g.offsets, b.keys_in, b.vals_in, g.big_list, g.big_count, cap32, n_order);
-		count_launch();
-		emit_big_kernel<uint32_t><<<nbig_blk, 256, 0, st>>>(f, g.rec, radii, g.perm, g.offsets, b.keys_in, b.vals_in, g.big_list, g.big_count, cap32);
-		if (bounded) count_launch();
-		if (bounded) pad_keys_kernel<uint32_t><<<npad_blk, 256, 0, st>>>(b.keys_in, b.vals_in, cap32, g.big_count);
-		if ((e = cudaGetLastError()) != cudaSuccess) return e;
-		e = cub::DeviceRadixSort::SortPairs(b.sort_temp, bytes, b.keys_in, b.keys_out, b.vals_in, b.vals_out, R, 0, sort_bits, st);
-		if (e != cudaSuccess) return e;
-		count_launch();
-		tile_ranges_kernel<uint32_t><<<(unsigned)((R + 256 * kRangeKeysPerThread - 1) / (256 * kRangeKeysPerThread)), 256, 0, st>>>(R, b.keys_out, img.ranges, (uint32_t)ntile);
+	if (ntile <= 65535 || (!bounded && ntile <= 65536)) {  // 16-bit tile ids (the key arrays are allocated for 32-bit ids either way)
+		if ((e = launch_emit<uint16_t>(f, g, radii, b, g.offsets, g.big_count, cap32, n_order, st)) != cudaSuccess) return e;
+		if (bucketable(f)) return launch_bucketing(b, img, g.big_count, ntile, R, st);
+		return launch_tile_sort<uint16_t>(b, img, g.big_count, ntile, R, bounded, st);
 	}
-	return cudaGetLastError();
+	if ((e = launch_emit<uint32_t>(f, g, radii, b, g.offsets, g.big_count, cap32, n_order, st)) != cudaSuccess) return e;
+	return launch_tile_sort<uint32_t>(b, img, g.big_count, ntile, R, bounded, st);
 }
 
 // ---- saturation split: near pass, blend, far pass (include/sgr.h sgr_set_near_budget, DESIGN.md §7) ----
@@ -881,9 +880,9 @@ __global__ void split_total_kernel(const uint32_t *__restrict__ offsets, int n, 
 	}
 }
 
-bool split_applies(const FrameDev &f) {
-	return f.S == 0 && f.band.begin == 0 && f.band.end == f.gy && f.band.step == 1 && f.gx * f.gy <= kBucketMaxTiles &&
-	       (uint32_t)f.P <= kPackMask + 1u;
+bool split_applies(const FrameDev &f, int64_t R, int64_t budget, bool from_records) {
+	const bool whole_image = f.band.begin == 0 && f.band.end == f.gy && f.band.step == 1;
+	return !from_records && f.P > 0 && R > 0 && (budget < 0 || budget < R) && f.S == 0 && whole_image && bucketable(f);
 }
 
 // near pass: split, emit the Gaussians before it into [0, E_near), bucket them into vals_out / ranges.  slots = binning capacity.
@@ -891,13 +890,9 @@ cudaError_t launch_near_binning(const FrameDev &f, GeomView g, const int32_t *ra
                                 int64_t cap, int n_order, int64_t budget) {
 	const uint32_t cap32 = cap >= 0 ? (uint32_t)cap : 0xffffffffu;
 	uint32_t *near = g.big_count + kStatusNear;
-	uint16_t *kin = reinterpret_cast<uint16_t *>(b.keys_in);
-	count_launch(3);
+	count_launch();
 	split_status_kernel<<<1, 1, 0, st>>>(g.offsets, n_order, cap32, (long long)budget, g.big_count);
-	emit_pairs_kernel<uint16_t><<<(unsigned)((n_order + 255) / 256), 256, 0, st>>>(f, g.rec, radii, g.tiles_touched, g.perm, g.offsets, kin,
-	                                                                               b.vals_in, g.big_list, near, cap32, n_order, near + 3);
-	emit_big_kernel<uint16_t><<<kNumSMs * 4, 256, 0, st>>>(f, g.rec, radii, g.perm, g.offsets, kin, b.vals_in, g.big_list, near, cap32);
-	cudaError_t e = cudaGetLastError();
+	cudaError_t e = launch_emit<uint16_t>(f, g, radii, b, g.offsets, near, cap32, n_order, st, near + 3);
 	if (e != cudaSuccess) return e;
 	return launch_bucketing(b, img, near, f.gx * f.gy, slots, st);
 }
@@ -911,7 +906,6 @@ cudaError_t launch_far_binning(const FrameDev &f, GeomView g, const int32_t *rad
 	uint32_t *sat = reinterpret_cast<uint32_t *>(img.ranges);  // (gx + 1)(gy + 1) <= 2 (ntile + 1) words
 	const KeepUnsaturated keep{sat, f.gx + 1};
 	uint32_t *far_offsets = g.ckey;
-	uint16_t *kin = reinterpret_cast<uint16_t *>(b.keys_in);
 	count_launch(2);
 	unsat_prefix_kernel<<<1, 1024, 0, st>>>(img.tile_max_contrib, f.gx, f.gy, sat);
 	far_count_kernel<<<nblk, 256, 0, st>>>(f, g.rec, radii, g.perm, g.offsets, g.big_count, n_order, keep, g.iota);
@@ -920,14 +914,11 @@ cudaError_t launch_far_binning(const FrameDev &f, GeomView g, const int32_t *rad
 	size_t bytes = g.temp_bytes;
 	if ((e = cub::DeviceScan::InclusiveSum(g.temp, bytes, g.iota, far_offsets, n_order, st)) != cudaSuccess) return e;
 	if ((e = cudaMemsetAsync(g.big_count, 0, sizeof(uint32_t), st)) != cudaSuccess) return e;
-	count_launch(3);
+	count_launch();
 	split_total_kernel<<<1, 1, 0, st>>>(far_offsets, n_order, cap32, g.big_count);
-	emit_pairs_kernel<uint16_t, KeepUnsaturated><<<nblk, 256, 0, st>>>(f, g.rec, radii, g.tiles_touched, g.perm, far_offsets, kin, b.vals_in,
-	                                                                   g.big_list, g.big_count, cap32, n_order, g.big_count + 3,
-	                                                                   g.big_count + kStatusNear + 3, keep);
-	emit_big_kernel<uint16_t, KeepUnsaturated><<<kNumSMs * 4, 256, 0, st>>>(f, g.rec, radii, g.perm, far_offsets, kin, b.vals_in, g.big_list,
-	                                                                        g.big_count, cap32, keep);
-	if ((e = cudaGetLastError()) != cudaSuccess) return e;
+	if ((e = launch_emit<uint16_t>(f, g, radii, b, far_offsets, g.big_count, cap32, n_order, st, g.big_count + 3, g.big_count + kStatusNear + 3,
+	                               keep)) != cudaSuccess)
+		return e;
 	return launch_bucketing(b, img, g.big_count, f.gx * f.gy, slots, st);
 }
 

@@ -296,10 +296,8 @@ static int forward_impl(const SgrFrame *frame, const float *means3D, const float
 		if (binning_state) *binning_state = bin;
 	}
 	if (num_instances) *num_instances = R;
-	// Saturation split (binning.cu): whole-image frames that bucket and carry no semantic channels; a budget that covers every
-	// instance the binning can hold is the one-pass binning.  The records path is the tile-row-sharded mode and keeps the latter.
 	const int64_t budget = g_near_budget;
-	if (!from_records && f.P > 0 && R > 0 && split_applies(f) && (budget < 0 || budget < R)) {
+	if (split_applies(f, R, budget, from_records)) {
 		const int64_t cap = bounded ? capacity : -1;
 		SGR_TRY(launch_near_binning(f, g, radii, b, img, R, st, cap, n_order, budget), "near binning");
 		SGR_TRY(launch_blend_fwd(f, g, b, img, nullptr, out_color, out_depth, out_alpha, nullptr, st, kBlendNear), "near blend_fwd");

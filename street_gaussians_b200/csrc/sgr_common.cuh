@@ -358,9 +358,12 @@ size_t bucket_scratch_bytes(int64_t R);
 // slots and the true count lives in g.big_count[1..3].
 cudaError_t launch_binning(const FrameDev &f, GeomView g, const int32_t *radii, BinView b, ImgView img, int64_t R,
                            cudaStream_t st, int64_t cap = -1, int n_order = -1);
-// saturation split: whether a forward of this frame can take it (whole image, tile bucketing, no semantic channels), then its passes.
+// saturation split: whether a forward of this frame takes it, then its passes.  It applies to a whole-image frame that buckets, has
+// no semantic channels and R > 0 instances, projected by this process (the records of the Gaussian-sharded mode keep the one-pass
+// binning), with a near budget below R (budget < 0: automatic; a budget that covers every instance the binning can hold is the
+// one-pass binning).
 // near: split + near emission + bucketing; far (after launch_blend_fwd kBlendNear): far count / emission + the final bucketing.
-bool split_applies(const FrameDev &f);
+bool split_applies(const FrameDev &f, int64_t R, int64_t budget, bool from_records);
 cudaError_t launch_near_binning(const FrameDev &f, GeomView g, const int32_t *radii, BinView b, ImgView img, int64_t slots, cudaStream_t st,
                                 int64_t cap, int n_order, int64_t budget);
 cudaError_t launch_far_binning(const FrameDev &f, GeomView g, const int32_t *radii, BinView b, ImgView img, int64_t slots, cudaStream_t st,

@@ -1,8 +1,8 @@
 """The per-tile lists against a torch restatement of the bucketing, from the library's own emitted sequence: vals_out[:E] must be
 vals_in[:E] stably sorted by keys_in[:E], and ranges[t] = (start, start + count) from bincount / cumsum, (0, 0) for a tile without
 instances.  E = status word 3 (the instances actually emitted; R in exact mode).  Covers the tile-bucketing path (frames of at most
-16384 tiles) at its partition edges (32768 instances) and the tile radix sort of larger frames.  tools/ab_binning.py compares the
-lists, images and gradients of two builds of the library frame by frame, layered renders included."""
+16384 tiles) at multiples of its largest partition (32768 instances) and the tile radix sort of larger frames.  tools/ab_binning.py
+compares the lists, images and gradients of two builds of the library frame by frame, layered renders included."""
 import pytest
 import torch
 
@@ -13,7 +13,7 @@ from street_gaussians_b200 import synthetic
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-K = 32768           # instances per bucketing partition (csrc/binning.cu kBucketPart)
+K = 32768           # largest bucketing partition (csrc/binning.cu kBucketMaxPart; a frame's partitions hold bucket_part(E) instances)
 MAX_TILES = 16384   # largest frame that buckets (csrc/binning.cu kBucketMaxTiles)
 
 

@@ -81,7 +81,9 @@ def main():
     scenes = [(c, synthetic.make_config(c, seed=0)) for c in args.configs.split(",") if c]
     scenes += [("small_sh3", synthetic.make_scene(P=3000, width=208, height=120, sh_degree=3, seed=7, pose=True, scale_med=0.08)),
                ("60k_720p", synthetic.make_scene(P=60_000, width=1280, height=720, sh_degree=1, seed=3, pose=True)),
-               ("smoke_A", synthetic.smoke_script_scene(10000, 256, 256, seed=0))]
+               ("smoke_A", synthetic.smoke_script_scene(10000, 256, 256, seed=0)),
+               # 313 x 250 tiles: the tile radix sort on 32-bit tile ids
+               ("5000x4000", synthetic.make_scene(P=200_000, width=5000, height=4000, sh_degree=0, seed=2, scale_med=0.02))]
     bad = 0
     for name, sc in scenes:
         rows = (sc["cam"]["image_height"] + 15) // 16
