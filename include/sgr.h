@@ -273,6 +273,9 @@ typedef struct SgrPeers {
 	const float *grad2d[SGR_MAX_PEERS]; /* rank p's partial grad2d[world*chunk,12] (output of its sgr_backward_blend) */
 	uint32_t *flags[SGR_MAX_PEERS];     /* rank p's barrier pad: uint32[SGR_MAX_PEERS], zero-initialised once by the caller and mapped
 	                                       into every rank like the arrays above.  Only needed by sgr_peer_barrier / sgr_sharded_*. */
+	float *sem[SGR_MAX_PEERS];          /* feature channels of the fused step (sgr_sharded_*_features only; may be NULL otherwise):  */
+	float *gsem[SGR_MAX_PEERS];         /* rank p's sem[world*chunk, S] (delivered semantics) and gsem[world*chunk, S] (its partial
+	                                       dL/dsemantics), rows by slot like records and grad2d, mapped into every rank */
 } SgrPeers;
 int sgr_scatter_records(const SgrFrame *frame, const SgrPeers *peers, const void *records_local, const int32_t *radii_local,
                         void *stream);
@@ -323,6 +326,26 @@ int sgr_sharded_backward(const SgrFrame *frame, const SgrPeers *peers, int64_t c
                          const float *out_alpha, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
                          float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors_precomp, float *dL_dopacity,
                          float *dL_dscales, float *dL_drotations, float *dL_dcov3D, uint32_t barrier_epoch, void *stream);
+/* The same two calls with feature channels: frame->S in [1, SGR_MAX_SEMANTIC_BWD] and peers->sem / peers->gsem set for every rank.
+ * Forward: semantics [frame.P, S] (this rank's own rows) travel with the records — the same block runs, the same slots, in rank d's
+ * sem section — and the blend reads them by slot; out_semantic [S, H, W] receives the band's rows (the caller zeroes the others).
+ * Backward: the blend writes this band's partial dL/dsemantics rows by slot into the rank's gsem section (which it zeroes first);
+ * after the barrier each rank fetches its own Gaussians' rows from the ranks that rendered them, as the same runs, and adds them in
+ * ascending rank order into dL_dsemantics [frame.P, S].  No NCCL, no host read-back; the arguments before them are those of
+ * sgr_sharded_forward / sgr_sharded_backward. */
+int sgr_sharded_forward_features(const SgrFrame *frame, const SgrPeers *peers, const float *means3D, const float *shs, const float *colors_precomp,
+                                 const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
+                                 float *out_color, float *out_depth, float *out_alpha, int32_t *radii_local, void *records_local,
+                                 size_t geom_bytes, void *img_state, size_t img_bytes, void *binning_state, size_t binning_bytes,
+                                 int64_t capacity, int64_t gaussian_capacity, uint32_t barrier_epoch, int32_t pre_barrier,
+                                 const float *semantics, float *out_semantic, void *stream);
+int sgr_sharded_backward_features(const SgrFrame *frame, const SgrPeers *peers, int64_t capacity, const float *means3D, const float *shs,
+                                  const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                                  const int32_t *radii_local, const void *records_local, const void *img_state, const void *binning_state,
+                                  const float *out_alpha, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                                  float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors_precomp, float *dL_dopacity,
+                                  float *dL_dscales, float *dL_drotations, float *dL_dcov3D, uint32_t barrier_epoch,
+                                  const float *dL_dsemantic, float *dL_dsemantics, void *stream);
 
 /* ---- Scene-graph composer (SURVEY.md §8 row f1; no native counterpart in the reference, which composes with ~40 PyTorch kernels) ----
  * One call builds the rasterizer's inputs from the raw parameters of every sub-model of the scene graph, as
@@ -600,6 +623,16 @@ size_t sgr_band_color_correct_scratch_bytes(int32_t H, int32_t W);
 int sgr_band_color_correct_backward(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *image, const float *affine,
                                     const float *dL_dout, float *dL_dimage, double *partials, void *scratch, size_t scratch_bytes, void *stream);
 int sgr_band_color_correct_affine_grad(const double *sums, float *dL_daffine, void *stream);
+/* The feature maps' finishing (sgr_finish_features_forward / _backward) on a tile-row band: the whole-frame calls' arguments plus the
+ * band.  rendered, normals, semantic, dL_dnormals, dL_dsemantic and dL_drendered are whole [C, H, W] frames; only the band's pixels are
+ * read and written (the caller zeroes the other rows where it needs zeros), each at its frame index, so the band's rows equal the
+ * whole-frame call's bit for bit.  The operation is per pixel: no partial sums, nothing for the ranks to exchange.  An empty band
+ * launches nothing.  H W < 2^31. */
+int sgr_band_finish_features_forward(int32_t S, int32_t H, int32_t W, int32_t normal_channels, int32_t mode, int32_t row_begin, int32_t row_end,
+                                     int32_t row_step, const float *rendered, float *normals, float *semantic, void *stream);
+int sgr_band_finish_features_backward(int32_t S, int32_t H, int32_t W, int32_t normal_channels, int32_t mode, int32_t row_begin, int32_t row_end,
+                                      int32_t row_step, const float *rendered, const float *dL_dnormals, const float *dL_dsemantic,
+                                      float *dL_drendered, void *stream);
 
 /* ---- Evaluation metrics: masked L1, PSNR and SSIM of rendered views, value only ----
  * Replaces the scoring of training_report (train.py:274-303: l1_loss and psnr of the clamped render, lib/utils/loss_utils.py:21-37,

@@ -20,6 +20,7 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_set_nea
            "sgr_backward_geom", "sgr_backward", "sgr_mark_visible", "sgr_visible_filter", "sgr_knn_scratch_bytes",
            "sgr_knn_mean_dist2", "sgr_record_bytes", "sgr_project", "sgr_forward_records",
            "sgr_scatter_records", "sgr_gather_grad2d", "sgr_peer_barrier", "sgr_sharded_forward", "sgr_sharded_backward",
+           "sgr_sharded_forward_features", "sgr_sharded_backward_features",
            "sgr_compose_forward", "sgr_compose_backward", "sgr_image_loss_scratch_bytes", "sgr_image_loss", "sgr_sky_loss",
            "sgr_obj_acc_loss", "sgr_lidar_depth_loss_scratch_bytes", "sgr_lidar_depth_loss", "sgr_densify_stats", "sgr_adam_step",
            "sgr_densify_scratch_bytes", "sgr_densify_plan", "sgr_densify_apply", "sgr_reset_opacity", "sgr_sparse_adam_step",
@@ -32,11 +33,13 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_set_nea
            "sgr_band_image_loss_grad", "sgr_band_sky_loss", "sgr_band_obj_acc_loss", "sgr_band_acc_loss_value", "sgr_band_lidar_scratch_bytes",
            "sgr_band_lidar_keys", "sgr_band_lidar_select", "sgr_band_lidar_grad", "sgr_band_sky_composite_forward",
            "sgr_band_sky_composite_backward", "sgr_band_color_correct_forward", "sgr_band_color_correct_scratch_bytes",
-           "sgr_band_color_correct_backward", "sgr_band_color_correct_affine_grad", "sgr_eval_metrics_scratch_bytes",
+           "sgr_band_color_correct_backward", "sgr_band_color_correct_affine_grad", "sgr_band_finish_features_forward",
+           "sgr_band_finish_features_backward", "sgr_eval_metrics_scratch_bytes",
            "sgr_eval_metrics_accumulate", "sgr_band_eval_metrics_accumulate", "sgr_eval_metrics_finish"]
 
 SKY_MASK_ACC, SKY_MASK_GIVEN = 0, 1
 SEMANTIC_LOGITS, SEMANTIC_PROBABILITIES = 0, 1
+MAX_SEMANTIC_BWD = 32  # SGR_MAX_SEMANTIC_BWD: feature channels a backward (and the fused Gaussian-sharded step) takes
 
 
 class SgrFrame(C.Structure):
@@ -51,7 +54,8 @@ MAX_PEERS = 16
 
 class SgrPeers(C.Structure):
     _fields_ = [("world", C.c_int32), ("rank", C.c_int32), ("chunk", C.c_int64), ("records", C.c_void_p * MAX_PEERS),
-                ("radii", C.c_void_p * MAX_PEERS), ("grad2d", C.c_void_p * MAX_PEERS), ("flags", C.c_void_p * MAX_PEERS)]
+                ("radii", C.c_void_p * MAX_PEERS), ("grad2d", C.c_void_p * MAX_PEERS), ("flags", C.c_void_p * MAX_PEERS),
+                ("sem", C.c_void_p * MAX_PEERS), ("gsem", C.c_void_p * MAX_PEERS)]
 
 
 MAX_FOURIER = 8
@@ -189,6 +193,10 @@ def lib():
                                                                                                 C.c_int32, vp]
     L.sgr_sharded_backward.restype = C.c_int
     L.sgr_sharded_backward.argtypes = [C.POINTER(SgrFrame), C.POINTER(SgrPeers), C.c_int64] + [vp] * 6 + [vp] * 4 + [vp] * 4 + [vp] * 8 + [C.c_uint32, vp]
+    L.sgr_sharded_forward_features.restype = C.c_int
+    L.sgr_sharded_forward_features.argtypes = L.sgr_sharded_forward.argtypes[:-1] + [vp, vp, vp]
+    L.sgr_sharded_backward_features.restype = C.c_int
+    L.sgr_sharded_backward_features.argtypes = L.sgr_sharded_backward.argtypes[:-1] + [vp, vp, vp]
     L.sgr_compose_forward.restype = C.c_int
     L.sgr_compose_forward.argtypes = [C.POINTER(SgrSegment), C.c_int32, C.c_int32] + [vp] * 10
     L.sgr_compose_backward.restype = C.c_int
@@ -278,6 +286,10 @@ def lib():
     L.sgr_band_color_correct_backward.argtypes = [C.c_int32] * 2 + band + [vp] * 6 + [C.c_size_t, vp]
     L.sgr_band_color_correct_affine_grad.restype = C.c_int
     L.sgr_band_color_correct_affine_grad.argtypes = [vp] * 3
+    L.sgr_band_finish_features_forward.restype = C.c_int
+    L.sgr_band_finish_features_forward.argtypes = [C.c_int32] * 5 + band + [vp] * 4
+    L.sgr_band_finish_features_backward.restype = C.c_int
+    L.sgr_band_finish_features_backward.argtypes = [C.c_int32] * 5 + band + [vp] * 5
     L.sgr_eval_metrics_scratch_bytes.restype = C.c_size_t
     L.sgr_eval_metrics_scratch_bytes.argtypes = [C.c_int32] * 4
     L.sgr_eval_metrics_accumulate.restype = C.c_int

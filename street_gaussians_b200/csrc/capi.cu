@@ -421,11 +421,22 @@ int sgr_peer_barrier(const SgrPeers *peers, uint32_t epoch, void *stream) {
 }
 
 // FrameDev of the gathered problem (all world*chunk slots) seen through this rank's band
-static int make_total_frame(const SgrFrame *frame, const SgrPeers *peers, FrameDev &fl, FrameDev &ft, PeerTable &pt, bool need_grad) {
+static int make_total_frame(const SgrFrame *frame, const SgrPeers *peers, FrameDev &fl, FrameDev &ft, PeerTable &pt, bool need_grad,
+                            SemPeers *sp = nullptr) {
 	int rc = make_frame(frame, fl);
 	if (rc) return rc;
 	if ((rc = make_peers(peers, fl, need_grad, pt)) != SGR_OK) return rc;
-	if (fl.S != 0) return fail(SGR_EUNSUPPORTED, "the fused Gaussian-sharded step supports S == 0 only (use the staged calls for feature channels)");
+	if (!sp && fl.S != 0)
+		return fail(SGR_EUNSUPPORTED, "sgr_sharded_forward / _backward take S == 0 only (feature channels: sgr_sharded_*_features)");
+	if (sp) {
+		if (fl.S < 1 || fl.S > SGR_MAX_SEMANTIC_BWD)
+			return fail(SGR_EUNSUPPORTED, "the fused step carries 1 to %d feature channels, got S = %d", SGR_MAX_SEMANTIC_BWD, fl.S);
+		for (int p = 0; p < pt.world; p++) {
+			if (!peers->sem[p] || (need_grad && !peers->gsem[p])) return fail(SGR_EINVAL, "peer table entry %d has no feature section", p);
+			sp->sem[p] = peers->sem[p];
+			sp->gsem[p] = peers->gsem[p];
+		}
+	}
 	for (int p = 0; p < pt.world; p++)
 		if (pt.world > 1 && !pt.flags[p]) return fail(SGR_EINVAL, "peer table entry %d has no barrier pad", p);
 	// a rank past the last tile row (more ranks than tile rows) owns no row: its cyclic band is empty (cyclic_band passes [0, 0)), it
@@ -439,15 +450,18 @@ static int make_total_frame(const SgrFrame *frame, const SgrPeers *peers, FrameD
 	return SGR_OK;
 }
 
-int sgr_sharded_forward(const SgrFrame *frame, const SgrPeers *peers, const float *means3D, const float *shs, const float *colors_precomp,
-                        const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp, float *out_color,
-                        float *out_depth, float *out_alpha, int32_t *radii_local, void *records_local, size_t geom_bytes, void *img_state,
-                        size_t img_bytes, void *binning_state, size_t binning_bytes, int64_t capacity, int64_t gaussian_capacity,
-                        uint32_t barrier_epoch, int32_t pre_barrier, void *stream) {
+// sp != nullptr: the feature form (sgr_sharded_forward_features)
+static int sharded_forward(const SgrFrame *frame, const SgrPeers *peers, const float *means3D, const float *shs, const float *colors_precomp,
+                           const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp, float *out_color,
+                           float *out_depth, float *out_alpha, int32_t *radii_local, void *records_local, size_t geom_bytes, void *img_state,
+                           size_t img_bytes, void *binning_state, size_t binning_bytes, int64_t capacity, int64_t gaussian_capacity,
+                           uint32_t barrier_epoch, int32_t pre_barrier, SemPeers *sp, const float *semantics, float *out_semantic,
+                           void *stream) {
 	FrameDev fl, ft;
 	PeerTable pt = {};
-	int rc = make_total_frame(frame, peers, fl, ft, pt, false);
+	int rc = make_total_frame(frame, peers, fl, ft, pt, false, sp);
 	if (rc) return rc;
+	if (sp && (!out_semantic || (fl.P > 0 && !semantics))) return fail(SGR_EINVAL, "semantics / out_semantic is NULL");
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 	const bool debug = frame->debug != 0;
 	if (capacity < 0 || capacity > 0x7fffffffLL) return fail(SGR_EINVAL, "capacity must be in [0, 2^31)");
@@ -474,6 +488,7 @@ int sgr_sharded_forward(const SgrFrame *frame, const SgrPeers *peers, const floa
 	                               reinterpret_cast<GaussRec *>(records_local), g.jac, g.depth_key,
 	                               (size_t)(reinterpret_cast<char *>(g.iota) - reinterpret_cast<char *>(geom_state)), st),
 	        "project+scatter");
+	if (sp) SGR_TRY(launch_scatter_semantics(pt, *sp, fl.P, fl.S, g.depth_key, semantics, st), "scatter semantics");
 	if (ft.P == 0) return SGR_OK;
 	SGR_TRY(cudaMemsetAsync(g.big_count, 0, 64 * sizeof(uint32_t), st), "status reset");
 	SGR_TRY(launch_peer_barrier(pt, barrier_epoch, g.big_count, st), "barrier");
@@ -482,7 +497,69 @@ int sgr_sharded_forward(const SgrFrame *frame, const SgrPeers *peers, const floa
 	        "count + depth_order");
 	const BinView b = capacity > 0 ? carve_bin(binning_state, capacity) : carve_bin(nullptr, 0);
 	SGR_TRY(launch_binning(ft, g, pt.radii[pt.rank], b, img, capacity, st, capacity, n_order), "binning");
-	SGR_TRY(launch_blend_fwd(ft, g, b, img, nullptr, out_color, out_depth, out_alpha, nullptr, st), "blend_fwd");
+	SGR_TRY(launch_blend_fwd(ft, g, b, img, sp ? sp->sem[pt.rank] : nullptr, out_color, out_depth, out_alpha, sp ? out_semantic : nullptr, st),
+	        "blend_fwd");
+	return SGR_OK;
+}
+
+int sgr_sharded_forward(const SgrFrame *frame, const SgrPeers *peers, const float *means3D, const float *shs, const float *colors_precomp,
+                        const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp, float *out_color,
+                        float *out_depth, float *out_alpha, int32_t *radii_local, void *records_local, size_t geom_bytes, void *img_state,
+                        size_t img_bytes, void *binning_state, size_t binning_bytes, int64_t capacity, int64_t gaussian_capacity,
+                        uint32_t barrier_epoch, int32_t pre_barrier, void *stream) {
+	return sharded_forward(frame, peers, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, out_color, out_depth, out_alpha,
+	                       radii_local, records_local, geom_bytes, img_state, img_bytes, binning_state, binning_bytes, capacity, gaussian_capacity,
+	                       barrier_epoch, pre_barrier, nullptr, nullptr, nullptr, stream);
+}
+
+int sgr_sharded_forward_features(const SgrFrame *frame, const SgrPeers *peers, const float *means3D, const float *shs, const float *colors_precomp,
+                                 const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp,
+                                 float *out_color, float *out_depth, float *out_alpha, int32_t *radii_local, void *records_local,
+                                 size_t geom_bytes, void *img_state, size_t img_bytes, void *binning_state, size_t binning_bytes,
+                                 int64_t capacity, int64_t gaussian_capacity, uint32_t barrier_epoch, int32_t pre_barrier,
+                                 const float *semantics, float *out_semantic, void *stream) {
+	SemPeers sp = {};
+	return sharded_forward(frame, peers, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, out_color, out_depth, out_alpha,
+	                       radii_local, records_local, geom_bytes, img_state, img_bytes, binning_state, binning_bytes, capacity, gaussian_capacity,
+	                       barrier_epoch, pre_barrier, &sp, semantics, out_semantic, stream);
+}
+
+static int sharded_backward(const SgrFrame *frame, const SgrPeers *peers, int64_t capacity, const float *means3D, const float *shs,
+                            const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                            const int32_t *radii_local, const void *records_local, const void *img_state, const void *binning_state,
+                            const float *out_alpha, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                            float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors_precomp, float *dL_dopacity,
+                            float *dL_dscales, float *dL_drotations, float *dL_dcov3D, uint32_t barrier_epoch, SemPeers *sp,
+                            const float *dL_dsemantic, float *dL_dsemantics, void *stream) {
+	FrameDev fl, ft;
+	PeerTable pt = {};
+	int rc = make_total_frame(frame, peers, fl, ft, pt, true, sp);
+	if (rc) return rc;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = frame->debug != 0;
+	if (!img_state || !out_alpha || !dL_dcolor || !dL_ddepth || !dL_dalpha) return fail(SGR_EINVAL, "NULL pointer passed to sgr_sharded_backward");
+	if (sp && (!dL_dsemantic || (fl.P > 0 && !dL_dsemantics))) return fail(SGR_EINVAL, "dL_dsemantic / dL_dsemantics is NULL");
+	if (capacity > 0 && !binning_state) return fail(SGR_EINVAL, "capacity > 0 but binning_state is NULL");
+	if (fl.P > 0 && (rc = check_geom_grads("sgr_sharded_backward", fl, means3D && radii_local && records_local, shs, scales, rotations, cov3D_precomp,
+	                                       dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dopacity, dL_dscales, dL_drotations)) != SGR_OK)
+		return rc;
+	const GeomView g = carve_geom(pt.rec[pt.rank], ft.P);
+	const ImgView img = carve_img(const_cast<void *>(img_state), ft.W, ft.H);
+	const BinView b = carve_bin(const_cast<void *>(binning_state), capacity);
+	float *grad2d = const_cast<float *>(pt.grad2d[pt.rank]);
+	// (S > 0: the blend backward zeroes grad2d and gsem of every slot first; that is after the forward barrier, which a peer passes only
+	// after the gather of its previous backward, the last reader of both)
+	if (ft.P > 0)
+		SGR_TRY(launch_blend_bwd(ft, g, b, img, sp ? sp->sem[pt.rank] : nullptr, out_alpha, dL_dcolor, dL_ddepth, dL_dalpha, sp ? dL_dsemantic : nullptr,
+		                         grad2d, sp ? sp->gsem[pt.rank] : nullptr, st, true),
+		        "blend_bwd");
+	SGR_TRY(launch_peer_barrier(pt, barrier_epoch, ft.P > 0 ? g.big_count : nullptr, st), "barrier");
+	SGR_TRY(launch_preprocess_bwd(fl, &pt, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii_local,
+	                              g.jac, reinterpret_cast<const float *>(g.depth_key), dL_dmeans3D,
+	                              dL_dmeans2D, shs ? dL_dsh : nullptr, dL_dcolors_precomp, dL_dopacity, cov3D_precomp ? nullptr : dL_dscales,
+	                              cov3D_precomp ? nullptr : dL_drotations, dL_dcov3D, st),
+	        "preprocess_bwd+gather");
+	if (sp) SGR_TRY(launch_gather_semantics(pt, *sp, fl.P, fl.S, g.depth_key, dL_dsemantics, st), "gather semantics");
 	return SGR_OK;
 }
 
@@ -492,30 +569,22 @@ int sgr_sharded_backward(const SgrFrame *frame, const SgrPeers *peers, int64_t c
                          const float *out_alpha, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
                          float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors_precomp, float *dL_dopacity,
                          float *dL_dscales, float *dL_drotations, float *dL_dcov3D, uint32_t barrier_epoch, void *stream) {
-	FrameDev fl, ft;
-	PeerTable pt = {};
-	int rc = make_total_frame(frame, peers, fl, ft, pt, true);
-	if (rc) return rc;
-	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-	const bool debug = frame->debug != 0;
-	if (!img_state || !out_alpha || !dL_dcolor || !dL_ddepth || !dL_dalpha) return fail(SGR_EINVAL, "NULL pointer passed to sgr_sharded_backward");
-	if (capacity > 0 && !binning_state) return fail(SGR_EINVAL, "capacity > 0 but binning_state is NULL");
-	if (fl.P > 0 && (rc = check_geom_grads("sgr_sharded_backward", fl, means3D && radii_local && records_local, shs, scales, rotations, cov3D_precomp,
-	                                       dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dopacity, dL_dscales, dL_drotations)) != SGR_OK)
-		return rc;
-	const GeomView g = carve_geom(pt.rec[pt.rank], ft.P);
-	const ImgView img = carve_img(const_cast<void *>(img_state), ft.W, ft.H);
-	const BinView b = carve_bin(const_cast<void *>(binning_state), capacity);
-	float *grad2d = const_cast<float *>(pt.grad2d[pt.rank]);
-	if (ft.P > 0)
-		SGR_TRY(launch_blend_bwd(ft, g, b, img, nullptr, out_alpha, dL_dcolor, dL_ddepth, dL_dalpha, nullptr, grad2d, nullptr, st, true), "blend_bwd");
-	SGR_TRY(launch_peer_barrier(pt, barrier_epoch, ft.P > 0 ? g.big_count : nullptr, st), "barrier");
-	SGR_TRY(launch_preprocess_bwd(fl, &pt, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii_local,
-	                              g.jac, reinterpret_cast<const float *>(g.depth_key), dL_dmeans3D,
-	                              dL_dmeans2D, shs ? dL_dsh : nullptr, dL_dcolors_precomp, dL_dopacity, cov3D_precomp ? nullptr : dL_dscales,
-	                              cov3D_precomp ? nullptr : dL_drotations, dL_dcov3D, st),
-	        "preprocess_bwd+gather");
-	return SGR_OK;
+	return sharded_backward(frame, peers, capacity, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii_local, records_local,
+	                        img_state, binning_state, out_alpha, dL_dcolor, dL_ddepth, dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors_precomp,
+	                        dL_dopacity, dL_dscales, dL_drotations, dL_dcov3D, barrier_epoch, nullptr, nullptr, nullptr, stream);
+}
+
+int sgr_sharded_backward_features(const SgrFrame *frame, const SgrPeers *peers, int64_t capacity, const float *means3D, const float *shs,
+                                  const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                                  const int32_t *radii_local, const void *records_local, const void *img_state, const void *binning_state,
+                                  const float *out_alpha, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                                  float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors_precomp, float *dL_dopacity,
+                                  float *dL_dscales, float *dL_drotations, float *dL_dcov3D, uint32_t barrier_epoch,
+                                  const float *dL_dsemantic, float *dL_dsemantics, void *stream) {
+	SemPeers sp = {};
+	return sharded_backward(frame, peers, capacity, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii_local, records_local,
+	                        img_state, binning_state, out_alpha, dL_dcolor, dL_ddepth, dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors_precomp,
+	                        dL_dopacity, dL_dscales, dL_drotations, dL_dcov3D, barrier_epoch, &sp, dL_dsemantic, dL_dsemantics, stream);
 }
 
 int sgr_forward_status_async(const SgrFrame *frame, const void *geom_state, uint32_t *host_status, void *stream) {
@@ -1375,6 +1444,34 @@ int sgr_band_color_correct_affine_grad(const double *sums, float *dL_daffine, vo
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 	const bool debug = false;
 	SGR_TRY(launch_color_correct_affine_grad(sums, dL_daffine, st), "band_color_correct_affine_grad");
+	return SGR_OK;
+}
+
+// ---- the feature maps' finishing on a tile-row band ----
+int sgr_band_finish_features_forward(int32_t S, int32_t H, int32_t W, int32_t normal_channels, int32_t mode, int32_t row_begin, int32_t row_end,
+                                     int32_t row_step, const float *rendered, float *normals, float *semantic, void *stream) {
+	const char *fn = "sgr_band_finish_features_forward";
+	if (int rc = finish_check(fn, S, H, W, normal_channels, mode)) return rc;
+	Band band;
+	if (int rc = loss_band(fn, H, W, row_begin, row_end, row_step, &band)) return rc;
+	if (!rendered || (normal_channels > 0 && !normals) || (S > normal_channels && !semantic)) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_finish_features_fwd(S, H, W, band, normal_channels, mode, rendered, normals, semantic, st), fn);
+	return SGR_OK;
+}
+
+int sgr_band_finish_features_backward(int32_t S, int32_t H, int32_t W, int32_t normal_channels, int32_t mode, int32_t row_begin, int32_t row_end,
+                                      int32_t row_step, const float *rendered, const float *dL_dnormals, const float *dL_dsemantic,
+                                      float *dL_drendered, void *stream) {
+	const char *fn = "sgr_band_finish_features_backward";
+	if (int rc = finish_check(fn, S, H, W, normal_channels, mode)) return rc;
+	Band band;
+	if (int rc = loss_band(fn, H, W, row_begin, row_end, row_step, &band)) return rc;
+	if (!rendered || !dL_drendered) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_finish_features_bwd(S, H, W, band, normal_channels, mode, rendered, dL_dnormals, dL_dsemantic, dL_drendered, st), fn);
 	return SGR_OK;
 }
 

@@ -262,11 +262,18 @@ constexpr float kProbEps = 1e-8f;     // street_gaussian_renderer.py:261-262
 // One thread per pixel.  Channels [0, nc) are the normals (nc = 3) or absent (nc = 0); channels [nc, S) the semantics.
 //   normals:  x / max(|x|, eps)
 //   semantic: 'probabilities'  log(x / (sum_c x_c + 1e-8) + 1e-8);  'logits'  x
+// Work item t is pixel t of the frame, or with kBand pixel band_pixel(t) of the band's M = band_rows * 16 W pixels (those past the
+// image's last row do nothing).  Either way a pixel keeps its frame index p, so a band's rows equal the whole frame's bit for bit.
+// The whole-frame instantiation ignores the trailing band arguments, so its instructions do not depend on them.
+template <bool kBand>
 __global__ void __launch_bounds__(kFeatThreads) finish_features_fwd_kernel(const int64_t N, const int S, const int nc, const int mode,
                                                                            const float *__restrict__ in, float *__restrict__ nout,
-                                                                           float *__restrict__ sout) {
-	const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-	if (p >= N) return;
+                                                                           float *__restrict__ sout, const int64_t M, const Band band,
+                                                                           const int64_t strip) {
+	const int64_t item = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (item >= (kBand ? M : N)) return;
+	const int64_t p = kBand ? band_pixel(item, band, strip) : item;
+	if (kBand && p >= N) return;
 	if (nc == 3) {
 		const float x0 = __ldg(in + p), x1 = __ldg(in + N + p), x2 = __ldg(in + 2 * N + p);
 		const float d = fmaxf(__fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(x0, x0), __fmul_rn(x1, x1)), __fmul_rn(x2, x2))), kNormalEps);
@@ -288,11 +295,16 @@ __global__ void __launch_bounds__(kFeatThreads) finish_features_fwd_kernel(const
 
 // Fused backward of both.  normals: dL/dx = g / d - [|x| >= eps] (g . x) / d^2 x / |x| (the clamp passes no gradient below eps).
 // 'probabilities': with t = sum x + 1e-8, p = x / t, h = g / (p + 1e-8): dL/dx = (h - sum_c h_c p_c) / t.  A NULL gradient is 0.
+// The pixels as in the forward.
+template <bool kBand>
 __global__ void __launch_bounds__(kFeatThreads) finish_features_bwd_kernel(const int64_t N, const int S, const int nc, const int mode,
                                                                            const float *__restrict__ in, const float *__restrict__ gn,
-                                                                           const float *__restrict__ gs, float *__restrict__ gin) {
-	const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-	if (p >= N) return;
+                                                                           const float *__restrict__ gs, float *__restrict__ gin,
+                                                                           const int64_t M, const Band band, const int64_t strip) {
+	const int64_t item = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (item >= (kBand ? M : N)) return;
+	const int64_t p = kBand ? band_pixel(item, band, strip) : item;
+	if (kBand && p >= N) return;
 	if (nc == 3) {
 		if (gn) {
 			const float x0 = __ldg(in + p), x1 = __ldg(in + N + p), x2 = __ldg(in + 2 * N + p);
@@ -336,7 +348,7 @@ __global__ void __launch_bounds__(kFeatThreads) finish_features_bwd_kernel(const
 cudaError_t launch_finish_features_fwd(int S, int H, int W, int nc, int mode, const float *in, float *nout, float *sout, cudaStream_t st) {
 	const int64_t N = (int64_t)H * W;
 	count_launch();
-	finish_features_fwd_kernel<<<feat_blocks(N), kFeatThreads, 0, st>>>(N, S, nc, mode, in, nout, sout);
+	finish_features_fwd_kernel<false><<<feat_blocks(N), kFeatThreads, 0, st>>>(N, S, nc, mode, in, nout, sout, N, Band{0, 1, 1}, 1);
 	return cudaGetLastError();
 }
 
@@ -344,7 +356,26 @@ cudaError_t launch_finish_features_bwd(int S, int H, int W, int nc, int mode, co
                                        cudaStream_t st) {
 	const int64_t N = (int64_t)H * W;
 	count_launch();
-	finish_features_bwd_kernel<<<feat_blocks(N), kFeatThreads, 0, st>>>(N, S, nc, mode, in, gn, gs, gin);
+	finish_features_bwd_kernel<false><<<feat_blocks(N), kFeatThreads, 0, st>>>(N, S, nc, mode, in, gn, gs, gin, N, Band{0, 1, 1}, 1);
+	return cudaGetLastError();
+}
+
+// The band's pixels: band_rows(band) tile rows of 16 W pixels each; an empty band launches nothing.  The grid depends on the band and
+// the image size only.
+cudaError_t launch_finish_features_fwd(int S, int H, int W, Band band, int nc, int mode, const float *in, float *nout, float *sout, cudaStream_t st) {
+	const int64_t N = (int64_t)H * W, strip = (int64_t)kBandTileRows * W, M = band_rows(band) * strip;
+	if (M == 0) return cudaSuccess;
+	count_launch();
+	finish_features_fwd_kernel<true><<<feat_blocks(M), kFeatThreads, 0, st>>>(N, S, nc, mode, in, nout, sout, M, band, strip);
+	return cudaGetLastError();
+}
+
+cudaError_t launch_finish_features_bwd(int S, int H, int W, Band band, int nc, int mode, const float *in, const float *gn, const float *gs,
+                                       float *gin, cudaStream_t st) {
+	const int64_t N = (int64_t)H * W, strip = (int64_t)kBandTileRows * W, M = band_rows(band) * strip;
+	if (M == 0) return cudaSuccess;
+	count_launch();
+	finish_features_bwd_kernel<true><<<feat_blocks(M), kFeatThreads, 0, st>>>(N, S, nc, mode, in, gn, gs, gin, M, band, strip);
 	return cudaGetLastError();
 }
 

@@ -64,6 +64,76 @@ __global__ void __launch_bounds__(256) gather_grad2d_kernel(const FrameDev f, co
 	dst[0] = a; dst[1] = b; dst[2] = c;
 }
 
+// ---- feature channels of the fused step (sgr_sharded_forward_features / sgr_sharded_backward_features) ----
+// The S floats of each Gaussian travel like its record: the Gaussians of one block of kRunBlock own slots that rank d needs form ONE
+// contiguous run of rows in the block's slots of rank d's `sem` section, in ascending Gaussian order, into the same slots as the records
+// preprocess_fwd_kernel<false, SCATTER> sent.  The runs are re-derived from the destination masks that kernel stored (the same
+// block_run_ranks over the same masks), so records and rows agree slot for slot.  A run's rows are consecutive in the destination, so a
+// block writes each run as one stream of consecutive floats (whole 128-B lines).
+__global__ void __launch_bounds__(kRunBlock) scatter_semantics_kernel(const int P, const int S, const PeerTable pt, const SemPeers sp,
+                                                                     const uint32_t *__restrict__ masks, const float *__restrict__ sem) {
+	__shared__ RunScratch rs;
+	__shared__ uint8_t s_src[kRunBlock * kMaxPeers];
+	const long long idx = (long long)blockIdx.x * kRunBlock + threadIdx.x;
+	const uint32_t mask = idx < P ? masks[idx] : 0u;
+	block_run_ranks(rs, mask, pt.world);
+	for (int d = 0; d < pt.world; d++) {
+		const uint32_t r = run_rank(rs, mask, d);
+		if ((mask >> d) & 1u) s_src[rs.cpre[d] + r] = (uint8_t)threadIdx.x;
+	}
+	__syncthreads();
+	const uint32_t total = rs.cpre[pt.world];
+	const size_t slot0 = (size_t)pt.rank * (size_t)pt.chunk + (size_t)blockIdx.x * kRunBlock;
+	const float *src = sem + (size_t)blockIdx.x * kRunBlock * (size_t)S;
+	for (uint32_t e = threadIdx.x; e < total * (uint32_t)S; e += kRunBlock) {
+		const uint32_t pos = e / (uint32_t)S, c = e - pos * (uint32_t)S;
+		const int d = run_dest(rs, pos, pt.world);
+		sp.sem[d][(slot0 + (pos - rs.cpre[d])) * (size_t)S + c] = src[(size_t)s_src[pos] * S + c];
+	}
+}
+
+// dL/dsemantics of the own Gaussians: the partial rows the ranks' blend backward left in their `gsem` sections, fetched as the same runs
+// and added in ascending rank order (from 0, one fp32 add per rank that rendered the Gaussian); a Gaussian no rank received gets 0.
+__global__ void __launch_bounds__(kRunBlock) gather_semantics_kernel(const int P, const int S, const PeerTable pt, const SemPeers sp,
+                                                                    const uint32_t *__restrict__ masks, float *__restrict__ out) {
+	__shared__ RunScratch rs;
+	__shared__ uint8_t s_pos[kMaxPeers][kRunBlock];  // thread t's position in destination d's run (where bit d of its mask is set)
+	__shared__ uint32_t s_mask[kRunBlock];
+	const long long first = (long long)blockIdx.x * kRunBlock;
+	const uint32_t mask = first + threadIdx.x < P ? masks[first + threadIdx.x] : 0u;
+	block_run_ranks(rs, mask, pt.world);
+	for (int d = 0; d < pt.world; d++) {
+		const uint32_t r = run_rank(rs, mask, d);
+		s_pos[d][threadIdx.x] = (uint8_t)r;
+	}
+	s_mask[threadIdx.x] = mask;
+	__syncthreads();
+	const int n = (int)min((long long)kRunBlock, (long long)P - first);
+	const size_t slot0 = (size_t)pt.rank * (size_t)pt.chunk + (size_t)first;
+	for (int e = threadIdx.x; e < n * S; e += kRunBlock) {
+		const int t = e / S, c = e - t * S;
+		const uint32_t m = s_mask[t];
+		float v = 0.f;
+		for (int d = 0; d < pt.world; d++)
+			if ((m >> d) & 1u) v += sp.gsem[d][(slot0 + s_pos[d][t]) * (size_t)S + c];
+		out[(size_t)first * S + e] = v;
+	}
+}
+
+cudaError_t launch_scatter_semantics(const PeerTable &pt, const SemPeers &sp, int P, int S, const uint32_t *masks, const float *sem, cudaStream_t st) {
+	if (P == 0) return cudaSuccess;
+	count_launch();
+	scatter_semantics_kernel<<<(unsigned)((P + kRunBlock - 1) / kRunBlock), kRunBlock, 0, st>>>(P, S, pt, sp, masks, sem);
+	return cudaGetLastError();
+}
+
+cudaError_t launch_gather_semantics(const PeerTable &pt, const SemPeers &sp, int P, int S, const uint32_t *masks, float *out, cudaStream_t st) {
+	if (P == 0) return cudaSuccess;
+	count_launch();
+	gather_semantics_kernel<<<(unsigned)((P + kRunBlock - 1) / kRunBlock), kRunBlock, 0, st>>>(P, S, pt, sp, masks, out);
+	return cudaGetLastError();
+}
+
 // Cross-rank barrier on the caller's stream: thread p announces this rank's arrival in rank p's pad (a release store at system
 // scope, after a system-scope fence that orders this rank's earlier peer stores — issued by previous kernels of the stream —
 // before it) and then waits until rank p has announced itself in this rank's pad.  Epochs increase by one per barrier and every

@@ -342,6 +342,13 @@ __device__ __forceinline__ int run_dest(const RunScratch &rs, uint32_t pos, int 
 }
 cudaError_t launch_peer_barrier(const PeerTable &pt, uint32_t epoch, uint32_t *status, cudaStream_t st);
 // sgr_project fused with sgr_scatter_records: one pass over the rank's chunk (f.P local Gaussians, pt.chunk slots)
+// The feature sections of the fused step's peer workspace: sem[P_total, S] and gsem[P_total, S] of every rank, rows by slot.
+struct SemPeers {
+	float *sem[kMaxPeers];
+	float *gsem[kMaxPeers];
+};
+cudaError_t launch_scatter_semantics(const PeerTable &pt, const SemPeers &sp, int P, int S, const uint32_t *masks, const float *sem, cudaStream_t st);
+cudaError_t launch_gather_semantics(const PeerTable &pt, const SemPeers &sp, int P, int S, const uint32_t *masks, float *out, cudaStream_t st);
 cudaError_t launch_project_scatter(const FrameDev &f, const PeerTable &pt, const float *means3D, const float *shs,
                                    const float *colors_precomp, const float *opacities, const float *scales, const float *rotations,
                                    const float *cov3D_precomp, int32_t *radii_local, GaussRec *rec_local, float4 *jac_local,
@@ -449,6 +456,10 @@ cudaError_t launch_compose_semantics_bwd(int n_bg, int K, int mode, const float 
 cudaError_t launch_finish_features_fwd(int S, int H, int W, int nc, int mode, const float *in, float *nout, float *sout, cudaStream_t st);
 cudaError_t launch_finish_features_bwd(int S, int H, int W, int nc, int mode, const float *in, const float *gn, const float *gs, float *gin,
                                        cudaStream_t st);
+// the same on the pixels of a tile-row band only (multi-GPU)
+cudaError_t launch_finish_features_fwd(int S, int H, int W, Band band, int nc, int mode, const float *in, float *nout, float *sout, cudaStream_t st);
+cudaError_t launch_finish_features_bwd(int S, int H, int W, Band band, int nc, int mode, const float *in, const float *gn, const float *gs,
+                                       float *gin, cudaStream_t st);
 // the 11-tap SSIM window of loss_utils.py (losses.cu), shared by the image loss and the evaluation metrics
 constexpr int kSsimWin = 11;
 struct GaussWin {

@@ -8,7 +8,8 @@ over the sgr_gaussian_normals_*, sgr_compose_semantics_* and sgr_finish_features
     compose_semantics(models, class_labels, mode)                 -> semantics [P, K]
         StreetGaussianModel.get_semantic (street_gaussian_model.py:417-431) over the [background, actor_0, ...] list compose takes.
     finish_features(rendered, normal_channels, semantic_mode)    -> (normals [3, H, W] or None, semantic [K, H, W] or None)
-        the split, F.normalize and the probabilities' log of render_kernel (street_gaussian_renderer.py:245-264).
+        the split, F.normalize and the probabilities' log of render_kernel (street_gaussian_renderer.py:245-264); with band= on the
+        rows of a rank's TileRowBand only (sgr_band_finish_features_*).
 
 The feature tensor the rasterizer takes is torch.cat([normals, semantics], -1) ([P, 3 + K]; training needs 3 + K <= 32).  CUDA tensors
 only: there is no CPU fallback.
@@ -140,41 +141,57 @@ def compose_semantics(models: Sequence, class_labels: Sequence[int] = (), mode: 
 
 class _FinishFeatures(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, rendered, nc: int, mode: int):
+    def forward(ctx, rendered, nc: int, mode: int, rows: Optional[Tuple[int, int, int]]):
         ctx.set_materialize_grads(False)
         S, H, W = (int(v) for v in rendered.shape)
         dev = rendered.device
         x = rendered.contiguous()
-        normals = torch.empty((nc, H, W), device=dev, dtype=torch.float32)
-        semantic = torch.empty((S - nc, H, W), device=dev, dtype=torch.float32)
-        _capi.call("sgr_finish_features_forward", dev, S, H, W, nc, mode, ptr(x), ptr(normals), ptr(semantic))
+        new = torch.empty if rows is None else torch.zeros  # a band writes its rows only
+        normals = new((nc, H, W), device=dev, dtype=torch.float32)
+        semantic = new((S - nc, H, W), device=dev, dtype=torch.float32)
+        if rows is None:
+            _capi.call("sgr_finish_features_forward", dev, S, H, W, nc, mode, ptr(x), ptr(normals), ptr(semantic))
+        else:
+            _capi.call("sgr_band_finish_features_forward", dev, S, H, W, nc, mode, *rows, ptr(x), ptr(normals), ptr(semantic))
         ctx.save_for_backward(x)
-        ctx.args = (S, H, W, nc, mode)
+        ctx.args = (S, H, W, nc, mode, rows)
         return normals, semantic
 
     @staticmethod
     def backward(ctx, g_normals, g_semantic):
         (x,) = ctx.saved_tensors
-        S, H, W, nc, mode = ctx.args
+        S, H, W, nc, mode, rows = ctx.args
         dev = x.device
         gn = g_normals.contiguous() if g_normals is not None else None
         gs = g_semantic.contiguous() if g_semantic is not None else None
-        g = torch.empty_like(x)
-        _capi.call("sgr_finish_features_backward", dev, S, H, W, nc, mode, ptr(x), ptr(gn), ptr(gs), ptr(g))
-        return g, None, None
+        if rows is None:
+            g = torch.empty_like(x)
+            _capi.call("sgr_finish_features_backward", dev, S, H, W, nc, mode, ptr(x), ptr(gn), ptr(gs), ptr(g))
+        else:
+            g = torch.zeros_like(x)
+            _capi.call("sgr_band_finish_features_backward", dev, S, H, W, nc, mode, *rows, ptr(x), ptr(gn), ptr(gs), ptr(g))
+        return g, None, None, None
 
 
-def finish_features(rendered: torch.Tensor, normal_channels: int, semantic_mode: str = "logits"
+def finish_features(rendered: torch.Tensor, normal_channels: int, semantic_mode: str = "logits", *, band=None
                     ) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
     """rendered [S, H, W] (the rasterizer's feature image: normal_channels = 3 normal channels first, or 0, then the semantics)
     -> (normals [3, H, W] = per-pixel F.normalize, or None; semantic [S - normal_channels, H, W], or None): the semantic channels
-    as they are ('logits') or log(x / (sum_c x + 1e-8) + 1e-8) ('probabilities').  Differentiable in `rendered`."""
+    as they are ('logits') or log(x / (sum_c x + 1e-8) + 1e-8) ('probabilities').  Differentiable in `rendered`.
+
+    band= (keyword-only, a TileRowBand of sharded.py): rendered holds the rendered rows of this rank's band, as a sharded rasterizer
+    returns them.  The outputs and dL/drendered have the band's rows, zeros elsewhere, equal bit for bit to the whole-frame call's
+    rows.  The operation is per pixel, so no collective is needed and the ranks' results summed are the whole frame's."""
     nc = int(normal_channels)
     if nc not in (0, 3):
         raise ValueError(f"normal_channels must be 0 or 3, got {normal_channels}")
     m = _mode(semantic_mode)
     if rendered.dim() != 3 or rendered.shape[0] < max(nc, 1) or rendered.shape[1] < 1 or rendered.shape[2] < 1:
         raise ValueError(f"rendered must be [S, H, W] with S >= max(normal_channels, 1), got {tuple(rendered.shape)}")
+    rows = None
+    if band is not None:  # a bad band fails before anything is launched
+        from .band_losses import check_band
+        rows = check_band(band, int(rendered.shape[1]))
     _cuda_f32("finish_features", dict(rendered=rendered))
-    normals, semantic = _FinishFeatures.apply(rendered, nc, m)
+    normals, semantic = _FinishFeatures.apply(rendered, nc, m, rows)
     return (normals if nc else None), (semantic if semantic.shape[0] else None)

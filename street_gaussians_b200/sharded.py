@@ -219,11 +219,14 @@ class PeerWorkspace:
     over NVLink).  `emulate(...)` builds `world` ordinary buffers on ONE device that point at each other, so the exchange
     kernels can be tested without a second GPU."""
 
-    def __init__(self, settings, chunk: int, world: int, rank: int, device, group=None, _buffers=None):
+    def __init__(self, settings, chunk: int, world: int, rank: int, device, group=None, _buffers=None, S: int = 0):
         self.chunk, self.world, self.rank, self.P_total = int(chunk), int(world), int(rank), int(chunk) * int(world)
+        self.S = int(S)
         if world > _capi.MAX_PEERS:
             raise _capi.SgrError(f"peer exchange supports at most {_capi.MAX_PEERS} ranks, got {world}")
-        self.geom_bytes, self.img_bytes, self.off_radii, self.off_grad, self.off_flags, self.total = self.layout(settings, self.P_total, device)
+        self.geom_bytes, self.img_bytes, self.off_radii, self.off_grad, self.off_flags, self.total = self.layout(settings, self.P_total, device,
+                                                                                                                 self.S)
+        self.off_sem, self.off_gsem = self.feature_offsets(self.off_grad, self.P_total, self.S)
         self.hdl = None
         self.in_flight = False  # a differentiable forward has used the buffers and its backward has not run yet
         self.epoch = 0          # epoch of the last sgr_peer_barrier issued on this workspace (every rank counts alike)
@@ -252,26 +255,39 @@ class PeerWorkspace:
             self.peers.radii[p] = ptrs[p] + self.off_radii
             self.peers.grad2d[p] = ptrs[p] + self.off_grad
             self.peers.flags[p] = ptrs[p] + self.off_flags
+            if self.S:
+                self.peers.sem[p] = ptrs[p] + self.off_sem
+                self.peers.gsem[p] = ptrs[p] + self.off_gsem
+        nsem = self.P_total * self.S
+        self.sem = self.buf[self.off_sem: self.off_sem + 4 * nsem].view(torch.float32).view(self.P_total, self.S)
+        self.gsem = self.buf[self.off_gsem: self.off_gsem + 4 * nsem].view(torch.float32).view(self.P_total, self.S)
 
     @staticmethod
-    def layout(settings, P_total: int, device):
-        """(geom_bytes, img_bytes, offset of radii_all, offset of grad2d, offset of the barrier pad, total bytes) of the per-rank buffer."""
+    def feature_offsets(off_grad: int, P_total: int, S: int):
+        """Offsets of the feature sections sem and gsem ([P_total, S] fp32 each, rows by slot), between grad2d and the barrier pad."""
+        off_sem = _align(off_grad + 48 * P_total)
+        return off_sem, _align(off_sem + 4 * P_total * S)
+
+    @staticmethod
+    def layout(settings, P_total: int, device, S: int = 0):
+        """(geom_bytes, img_bytes, offset of radii_all, offset of grad2d, offset of the barrier pad, total bytes) of the per-rank buffer.
+        With S feature channels the sections sem and gsem (feature_offsets) sit before the pad; S = 0 leaves them empty."""
         fr, keep = _make_frame(settings, P_total, 0, 0, device, None)
         gb, ib = C.c_size_t(0), C.c_size_t(0)
         _capi.call("sgr_state_sizes", None, C.byref(fr), C.byref(gb), C.byref(ib))
         del keep
         off_radii = _align(gb.value)
         off_grad = _align(off_radii + 4 * P_total)
-        off_flags = _align(off_grad + 48 * P_total)
+        off_flags = _align(PeerWorkspace.feature_offsets(off_grad, P_total, S)[1] + 4 * P_total * S)
         return gb.value, ib.value, off_radii, off_grad, off_flags, off_flags + 256
 
     @classmethod
-    def emulate(cls, settings, chunk: int, world: int, device):
+    def emulate(cls, settings, chunk: int, world: int, device, S: int = 0):
         """`world` workspaces on ONE device whose peer tables point at each other (tests; world == 1 module path)."""
-        total = cls.layout(settings, int(chunk) * int(world), device)[5]
+        total = cls.layout(settings, int(chunk) * int(world), device, S)[-1]
         bufs = [torch.empty(total, dtype=torch.uint8, device=device) for _ in range(world)]
         ptrs = [b.data_ptr() for b in bufs]
-        return [cls(settings, chunk, world, r, device, _buffers=(bufs[r], ptrs)) for r in range(world)]
+        return [cls(settings, chunk, world, r, device, _buffers=(bufs[r], ptrs), S=S) for r in range(world)]
 
     def barrier(self):
         """Device-side barrier of the STAGED path (torch symmetric memory's signal pad)."""
@@ -334,10 +350,12 @@ class _GaussianShardedRasterize(torch.autograd.Function):
         world, chunk, group = owner.world, owner.chunk_for(P), owner.group
         S = int(tensors["semantics"].shape[1]) if tensors["semantics"] is not None else 0
         P_total = chunk * world
-        ws = owner.workspace(device) if owner.exchange == "p2p" else None
-        sem_all = None
         cap = owner.capacity
-        if ws is not None and owner.fused and S == 0 and cap is not None and cap.capacity is not None:
+        # feature channels ride the fused step up to the blend backward's limit; more take the staged path (forward only)
+        fused = owner.exchange == "p2p" and owner.fused and S <= _capi.MAX_SEMANTIC_BWD and cap is not None and cap.capacity is not None
+        ws = owner.workspace(device, S if fused else 0) if owner.exchange == "p2p" else None
+        sem_all = None
+        if fused:
             return _fused_forward(ctx, tensors, settings, owner, ws, P, chunk, differentiable,
                                   (means3D, means2D, sh, colors_precomp, semantics, opacities, scales, rotations, cov3Ds_precomp))
         rec, radii = project_records(tensors, settings, chunk)
@@ -385,7 +403,7 @@ class _GaussianShardedRasterize(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha, grad_semantic):
         if getattr(ctx, "fused", False):
-            return _fused_backward(ctx, grad_color, grad_depth, grad_alpha)
+            return _fused_backward(ctx, grad_color, grad_depth, grad_alpha, grad_semantic)
         rec, radii, alpha = ctx.saved_tensors
         settings, owner, st, tensors, shapes = ctx.settings, ctx.owner, ctx.state, ctx.tensors, ctx.shapes
         dev = alpha.device
@@ -422,9 +440,11 @@ class _GaussianShardedRasterize(torch.autograd.Function):
                                    g_cov)) + (None, None, None)
 
 
-def sharded_forward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, capacity: int, gaussian_capacity: int, status_word=None):
+def sharded_forward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, capacity: int, gaussian_capacity: int, status_word=None,
+                        semantics=None):
     """One sgr_sharded_forward call on the current stream (used by the autograd path and, with emulated workspaces on
-    separate streams, by the single-GPU tests).  Returns (color, depth, alpha, step buffers)."""
+    separate streams, by the single-GPU tests).  Returns (color, depth, alpha, step buffers).  semantics [P, S] (this rank's rows,
+    S = ws.S): sgr_sharded_forward_features, and the banded feature image [S, H, W] is returned as a fifth value."""
     L = _capi.lib()
     device = tensors["means3D"].device
     H, W = int(settings.image_height), int(settings.image_width)
@@ -433,39 +453,56 @@ def sharded_forward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, ca
     z = lambda c: torch.zeros((c, H, W), device=device, dtype=torch.float32)  # foreign rows stay zero
     color, depth, alpha = z(3), z(1), z(1)  # (separate tensors: autograd outputs that are views of one base cannot be modified in place)
     M = int(tensors["sh"].shape[1]) if tensors["sh"] is not None else 0
-    fr, keep = _make_frame(settings, P, M, 0, device, band)
+    S = 0 if semantics is None else int(semantics.shape[1])
+    if S != ws.S:
+        raise ValueError(f"the workspace carries {ws.S} feature channels, the call {S}")
+    fr, keep = _make_frame(settings, P, M, S, device, band)
     pre = 1 if ws.fwd_pending else 0
     ws.next_epochs(1 + pre)  # host-side tally only: the epochs themselves are counted on the device (barrier_epoch = 0)
     epoch = 0
-    _capi.call("sgr_sharded_forward", device, C.byref(fr), C.byref(ws.peers), ptr(tensors["means3D"]), ptr(tensors["sh"]),
-               ptr(tensors["colors_precomp"]), ptr(tensors["opacities"]), ptr(tensors["scales"]), ptr(tensors["rotations"]),
-               ptr(tensors["cov3Ds_precomp"]), ptr(color), ptr(depth), ptr(alpha), ptr(bufs["radii"]), ptr(bufs["rec"]), ws.geom_bytes,
-               ptr(bufs["img"]), ws.img_bytes, ptr(bufs["binning"]), nbytes, capacity, gaussian_capacity, epoch, pre)
+    args = (C.byref(fr), C.byref(ws.peers), ptr(tensors["means3D"]), ptr(tensors["sh"]), ptr(tensors["colors_precomp"]), ptr(tensors["opacities"]),
+            ptr(tensors["scales"]), ptr(tensors["rotations"]), ptr(tensors["cov3Ds_precomp"]), ptr(color), ptr(depth), ptr(alpha), ptr(bufs["radii"]),
+            ptr(bufs["rec"]), ws.geom_bytes, ptr(bufs["img"]), ws.img_bytes, ptr(bufs["binning"]), nbytes, capacity, gaussian_capacity, epoch, pre)
+    if S:
+        sem_in = _capi.f32(semantics, device)
+        semantic = z(S)
+        _capi.call("sgr_sharded_forward_features", device, *args, ptr(sem_in), ptr(semantic))
+    else:
+        _capi.call("sgr_sharded_forward", device, *args)
     if status_word is not None:  # the status of the gathered frame (P_total slots)
         frt, keep2 = _make_frame(settings, ws.P_total, 0, 0, device, band)
         _copy_status(frt, ws.geom, status_word, device)
         del keep2
     del keep
     ws.fwd_pending = True
-    return color, depth, alpha, bufs
+    return (color, depth, alpha, bufs, semantic) if S else (color, depth, alpha, bufs)
 
 
-def sharded_backward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, capacity: int, alpha, gc, gd, ga):
-    """One sgr_sharded_backward call on the current stream.  Returns the 8 gradients in _backward_geom_impl's order."""
+def sharded_backward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, capacity: int, alpha, gc, gd, ga, gs=None):
+    """One sgr_sharded_backward call on the current stream.  Returns the 8 gradients in _backward_geom_impl's order.  gs [S, H, W]
+    (the feature image's upstream gradient, after a forward with semantics): sgr_sharded_backward_features, and dL/dsemantics [P, S]
+    of this rank's own Gaussians is returned as a ninth value."""
     dev = alpha.device
     sh, colors, scales, rots, cov = (tensors[k] for k in ("sh", "colors_precomp", "scales", "rotations", "cov3Ds_precomp"))
     M = int(sh.shape[1]) if sh is not None else 0
     g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rots, g_cov = _geom_grad_buffers(tensors, P, dev)
     bufs = ws.step_buffers(0)
-    fr, keep = _make_frame(settings, P, M, 0, dev, band)
+    S = 0 if gs is None else ws.S
+    fr, keep = _make_frame(settings, P, M, S, dev, band)
     ws.next_epochs(1)
     epoch = 0  # device-side count
-    _capi.call("sgr_sharded_backward", dev, C.byref(fr), C.byref(ws.peers), capacity, ptr(tensors["means3D"]), ptr(sh), ptr(colors), ptr(scales),
-               ptr(rots), ptr(cov), ptr(bufs["radii"]), ptr(bufs["rec"]), ptr(bufs["img"]), ptr(bufs["binning"]), ptr(alpha), ptr(gc), ptr(gd),
-               ptr(ga), ptr(g_means3D), ptr(g_means2D), ptr(g_sh), ptr(g_colors), ptr(g_opac), ptr(g_scales), ptr(g_rots), ptr(g_cov), epoch)
+    args = (C.byref(fr), C.byref(ws.peers), capacity, ptr(tensors["means3D"]), ptr(sh), ptr(colors), ptr(scales), ptr(rots), ptr(cov),
+            ptr(bufs["radii"]), ptr(bufs["rec"]), ptr(bufs["img"]), ptr(bufs["binning"]), ptr(alpha), ptr(gc), ptr(gd), ptr(ga), ptr(g_means3D),
+            ptr(g_means2D), ptr(g_sh), ptr(g_colors), ptr(g_opac), ptr(g_scales), ptr(g_rots), ptr(g_cov), epoch)
+    if S:
+        g_sem = torch.empty((P, S), device=dev, dtype=torch.float32)
+        _capi.call("sgr_sharded_backward_features", dev, *args, ptr(_capi.f32(gs, dev)), ptr(g_sem))
+    else:
+        _capi.call("sgr_sharded_backward", dev, *args)
     del keep
     ws.fwd_pending = False  # every rank passed the backward barrier after its blend_bwd: the records may be overwritten
-    return g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rots, g_cov
+    grads = (g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rots, g_cov)
+    return grads + (g_sem,) if S else grads
 
 
 def _fused_forward(ctx, tensors, settings, owner, ws: "PeerWorkspace", P: int, chunk: int, differentiable: bool, inputs):
@@ -481,7 +518,10 @@ def _fused_forward(ctx, tensors, settings, owner, ws: "PeerWorkspace", P: int, c
     capacity = int(cap.capacity)
     # depth-order slots: learnt from the previous frames (status word 4); the first fused frame compacts into all slots
     gcap = int(cap.gaussian_capacity) if cap.gaussian_capacity is not None else ws.P_total
-    color, depth, alpha, bufs = sharded_forward_raw(settings, owner.band, ws, tensors, P, capacity, gcap)
+    S = ws.S
+    out = sharded_forward_raw(settings, owner.band, ws, tensors, P, capacity, gcap, semantics=tensors["semantics"] if S else None)
+    color, depth, alpha, bufs = out[:4]
+    semantic = out[4] if S else torch.zeros((0, H, W), device=device, dtype=torch.float32)
     if not cap.frozen:  # the status of the gathered frame (P_total slots)
         frt, keep = _make_frame(settings, ws.P_total, 0, 0, device, owner.band)
         cap.record_status(frt, ws.geom, device)
@@ -492,19 +532,22 @@ def _fused_forward(ctx, tensors, settings, owner, ws: "PeerWorkspace", P: int, c
     ctx.save_for_backward(alpha)
     radii_out = bufs["radii"][:P]
     ctx.mark_non_differentiable(radii_out)
-    return color, radii_out, depth, alpha, torch.zeros((0, H, W), device=device, dtype=torch.float32)
+    return color, radii_out, depth, alpha, semantic
 
 
-def _fused_backward(ctx, grad_color, grad_depth, grad_alpha):
+def _fused_backward(ctx, grad_color, grad_depth, grad_alpha, grad_semantic):
     """sgr_sharded_backward: blend_bwd, barrier, chain rule with the peer gather folded in — ONE C-ABI call."""
     (alpha,) = ctx.saved_tensors
     settings, owner, ws, P, tensors, shapes = ctx.settings, ctx.owner, ctx.ws, ctx.P, ctx.tensors, ctx.shapes
     dev = alpha.device
-    gc, gd, ga = (_capi.f32(g, dev, align16=True) for g in _image_grads(settings, dev, (grad_color, grad_depth, grad_alpha), (3, 1, 1)))
-    g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rots, g_cov = sharded_backward_raw(settings, owner.band, ws, tensors, P,
-                                                                                                   ctx.capacity, alpha, gc, gd, ga)
+    S = ws.S
+    gc, gd, ga, gs = (_capi.f32(g, dev, align16=True) if g is not None else None
+                      for g in _image_grads(settings, dev, (grad_color, grad_depth, grad_alpha, grad_semantic), (3, 1, 1, S)))
+    out = sharded_backward_raw(settings, owner.band, ws, tensors, P, ctx.capacity, alpha, gc, gd, ga, gs if S else None)
+    g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rots, g_cov = out[:8]
+    g_sem = out[8] if S else None
     ws.in_flight = False
-    return _fit_grads(shapes, (g_means3D, g_means2D, g_sh, g_colors, None, g_opac, g_scales, g_rots, g_cov)) + (None, None, None)
+    return _fit_grads(shapes, (g_means3D, g_means2D, g_sh, g_colors, g_sem, g_opac, g_scales, g_rots, g_cov)) + (None, None, None)
 
 
 class GaussianShardedRasterizer(nn.Module):
@@ -526,7 +569,7 @@ class GaussianShardedRasterizer(nn.Module):
         if exchange == "p2p" and layout != "cyclic":
             raise ValueError("the peer-memory exchange needs the cyclic tile-row layout")
         self.exchange, self._ws = exchange, None
-        # exchange="p2p" with a capacity object (sync-free binning) and no feature channels runs the whole forward / backward as
+        # exchange="p2p" with a capacity object (sync-free binning) and at most 32 feature channels runs the whole forward / backward as
         # ONE C-ABI call each (sgr_sharded_forward / sgr_sharded_backward) once the capacity is known; fused=False keeps the
         # staged calls (one per step of include/sgr.h's list)
         self.fused = bool(fused)
@@ -542,13 +585,14 @@ class GaussianShardedRasterizer(nn.Module):
         self.chunk = chunk_size(P_local, self.group)
         return self.chunk
 
-    def workspace(self, device) -> "PeerWorkspace":
-        """COLLECTIVE on first use and after repartition(): allocate + rendezvous the peer-mapped buffer."""
-        if self._ws is None or self._ws.chunk != self.chunk:
+    def workspace(self, device, S: int = 0) -> "PeerWorkspace":
+        """COLLECTIVE on first use, after repartition() and when the number of feature channels the fused step carries changes:
+        allocate + rendezvous the peer-mapped buffer (keyed on (chunk, S))."""
+        if self._ws is None or self._ws.chunk != self.chunk or self._ws.S != S:
             if self.world > 1:
-                self._ws = PeerWorkspace(self.raster_settings, self.chunk, self.world, self.rank, device, self.group)
+                self._ws = PeerWorkspace(self.raster_settings, self.chunk, self.world, self.rank, device, self.group, S=S)
             else:
-                self._ws = PeerWorkspace.emulate(self.raster_settings, self.chunk, 1, device)[0]
+                self._ws = PeerWorkspace.emulate(self.raster_settings, self.chunk, 1, device, S)[0]
         return self._ws
 
     def release_workspace(self):

@@ -4,15 +4,19 @@
         tools/check_gaussian_sharded.py
 
 Every rank renders the WHOLE scene with GaussianRasterizer (the checker) and its own share with
-GaussianShardedRasterizer (NCCL all-gather of records / reduce-scatter of grad2d).  Own image rows must be bit-identical,
+GaussianShardedRasterizer (NCCL all-gather of records / reduce-scatter of grad2d; with the argument p2p the peer-memory exchange,
+whose bounded passes run the fused step, feature channels (S = 3 + 4) included; that case has run at world 1 only, not on several
+H100s).  Own image rows must be bit-identical,
 foreign rows zero, and the gradients of the rank's own Gaussians equal up to float summation order.  That order differs
 between ANY two runs (float atomics), so the run-to-run difference of the single-GPU rasterizer is measured beside it
 and printed as `floor`; the bound asserted is GRAD_TOL = 5e-4 of max|ref| per tensor — half the 1e-3 parity bar the
 single-GPU path is held to against the reference.
 
-Two further legs run each rank's band stages against the single-GPU calls on the gathered frame: the training losses (band_losses.py),
-and the sky composite and colour correction with band= / group= (their parameter gradients all-reduced).  Neither leg has been run on
-several H100s yet; the single-GPU emulations of tests/test_band_losses_gpu.py and tests/test_band_image_gpu.py cover their kernels.
+Three further legs run each rank's band stages against the single-GPU calls on the gathered frame: the training losses (band_losses.py),
+the sky composite and colour correction with band= / group= (their parameter gradients all-reduced), and the feature maps' finishing
+(finish_features(band=)) on an S = 3 + 4 render (normals and semantics).  None of these legs has been run on several H100s yet; the
+single-GPU emulations of tests/test_band_losses_gpu.py, tests/test_band_image_gpu.py and tests/test_band_features_gpu.py cover their
+kernels.
 """
 import os
 import sys
@@ -199,6 +203,45 @@ def run_image_stages(rank, world, dev, W=1280, H=720, R=256):
     assert (np.abs(got[4].cpu().double().numpy() - exact) <= np.spacing(np.abs(exact).astype(np.float32))).all(), "dL/daffine"
 
 
+def run_features(rank, world, dev, W=1280, H=720, K=4):
+    """Feature leg: the sharded rasterizer with feature channels (3 normal channels, then K semantic ones) and finish_features(band=) on
+    each rank's banded feature image, in both semantic modes, against finish_features on the gathered frame.  Output and dL/drendered rows
+    bit-equal, foreign rows zero (the finishing is per pixel: no collective)."""
+    from street_gaussians_b200 import features
+    scene = synthetic.make_scene(P=60_001, width=W, height=H, sh_degree=3, seed=80, pose=True, semantics=3 + K)
+    st = util.settings_from(sgb, scene["cam"], dev)
+    rast = GaussianShardedRasterizer(st)
+    P = scene["means3D"].shape[0]
+    chunk = (P + world - 1) // world
+    lo, hi = min(P, rank * chunk), min(P, (rank + 1) * chunk)
+    sem = scene["semantics"].abs()  # accumulated probabilities are non-negative
+    with torch.no_grad():
+        got = rast(means3D=scene["means3D"][lo:hi].to(dev), means2D=None, opacities=scene["opacities"][lo:hi].to(dev),
+                   shs=scene["shs"][lo:hi].to(dev), scales=scene["scales"][lo:hi].to(dev), rotations=scene["rotations"][lo:hi].to(dev),
+                   semantics=sem[lo:hi].to(dev))
+    feat = got[4]
+    full = feat.clone()
+    if world > 1:
+        dist.all_reduce(full)
+    g = torch.Generator(device=dev).manual_seed(7)
+    gn, gs = torch.randn(3, H, W, device=dev, generator=g), torch.randn(K, H, W, device=dev, generator=g)
+    rows = band_of_rows(H, rank, world).to(dev)
+    band = rast.band if rast.band is not None else sgb.TileRowBand(0, (H + 15) // 16, 1)
+    bits = lambda x: x.contiguous().view(torch.int32)
+
+    def step(x, mode, b):
+        x = x.detach().clone().requires_grad_(True)
+        n, s = features.finish_features(x, 3, mode, band=b)
+        torch.autograd.backward([n, s], [gn, gs])
+        return n.detach(), s.detach(), x.grad
+
+    for mode in ("logits", "probabilities"):
+        ref, out = step(full, mode, None), step(feat, mode, band)
+        for name, x, y in zip(("normals", "semantic", "dL/drendered"), out, ref):
+            assert torch.equal(bits(x[:, rows]), bits(y[:, rows])), f"{mode} {name}: band rows differ"
+            assert not bool(x[:, ~rows].any()), f"{mode} {name}: foreign rows not zero"
+
+
 def main():
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -209,7 +252,10 @@ def main():
     ok = True
     try:
         exchange = sys.argv[1] if len(sys.argv) > 1 else "nccl"
-        for S, P, W, H, bounded in ((0, 200_003, 1280, 720, False), (2, 60_001, 800, 608, False), (0, 200_003, 1280, 720, True)):
+        # the last case carries feature channels through the bounded path: with exchange=p2p its passes 2-4 are the fused step with
+        # semantics (sgr_sharded_*_features, no NCCL), with exchange=nccl the staged one
+        for S, P, W, H, bounded in ((0, 200_003, 1280, 720, False), (2, 60_001, 800, 608, False), (0, 200_003, 1280, 720, True),
+                                    (3 + 4, 60_001, 800, 608, True)):
             worst, floor = run_case(rank, world, dev, S, P, W, H, bounded, exchange)
             print(f"[rank {rank}/{world}] exchange={exchange} S={S} P={P} {W}x{H} bounded={bounded}: images bit-equal, worst grad rel err {worst:.2e} "
                   f"(single-GPU run-to-run floor {floor:.2e})", flush=True)
@@ -218,6 +264,8 @@ def main():
         run_image_stages(rank, world, dev)
         print(f"[rank {rank}/{world}] band sky and colour correction: rows bit-equal to the single-GPU calls, parameter gradients the frame's",
               flush=True)
+        run_features(rank, world, dev)
+        print(f"[rank {rank}/{world}] band feature finishing: rows bit-equal to the single-GPU calls", flush=True)
     except AssertionError as e:
         ok = False
         print(f"[rank {rank}] FAILED: {e!r}", flush=True)
