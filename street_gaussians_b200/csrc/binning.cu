@@ -245,6 +245,7 @@ constexpr uint32_t kEmitStage = 512;  // instances staged per warp (2 x 2 KB of 
 // Saturation split (launch_near_binning / launch_far_binning): the near pass passes dev_cap -> its end of the emitted sequence, so
 // only the Gaussians before the split emit; the far pass passes its own offsets, dev_cap -> the end of the emitted sequence,
 // dev_floor -> the near pass's end (the Gaussians before the split then have empty ranges there) and the KeepUnsaturated predicate.
+// A pass whose device-side cap does not exceed its floor (0 without one) has nothing to emit: the whole grid returns.
 template <typename KeyT, typename Keep = KeepAll>
 __global__ void __launch_bounds__(256) emit_pairs_kernel(const FrameDev f, const GaussRec *__restrict__ rec, const int32_t *__restrict__ radii,
                                                         const uint32_t *__restrict__ perm, const uint32_t *__restrict__ offsets, KeyT *__restrict__ keys,
@@ -252,6 +253,7 @@ __global__ void __launch_bounds__(256) emit_pairs_kernel(const FrameDev f, const
                                                         uint32_t *__restrict__ big_count, uint32_t cap, const int n_order,
                                                         const uint32_t *__restrict__ dev_cap = nullptr,
                                                         const uint32_t *__restrict__ dev_floor = nullptr, const Keep keep = Keep()) {
+	if (dev_cap && *dev_cap <= (dev_floor ? *dev_floor : 0u)) return;
 	__shared__ KeyT s_keys[8][kEmitStage];
 	__shared__ uint32_t s_vals[8][kEmitStage];
 	const int warp = threadIdx.x >> 5;
@@ -446,7 +448,7 @@ static cudaError_t launch_tile_sort(const BinView &b, ImgView img, const uint32_
 //   5. bucket_count<false>, bucket_columns, bucket_pass<true>: the same on the high digit of the intermediate array, writing the
 //                            Gaussian indices into vals_out.
 // Positions come from ranks and prefix sums only, never from the order of atomics (the tile totals are integer sums, which do not
-// depend on it).  E is read on the device (status[3]) and the grids are sized for the most partitions any E up to the capacity
+// depend on it).  E is read on the device (*n_inst: status word 3, or the far pass's count) and the grids are sized for the most partitions any E up to the capacity
 // can give, so the bounded mode stays free of host synchronisation.
 constexpr int kBucketThreads = 512;  // histogram CTAs
 constexpr int kPassThreads = 256;    // rank-and-scatter CTAs: 72 registers, 3 CTAs per SM
@@ -502,17 +504,32 @@ static BucketScratch carve_bucket(void *base, int64_t slots) {
 }
 size_t bucket_scratch_bytes(int64_t slots) { return carve_bucket(nullptr, slots).bytes; }
 
+// The slots [first, last) a bucketing pass covers (first = 0 unless the far pass of the saturation split buckets its instances
+// behind the near ones).  Its partitions of bucket_part(last - base) slots start at base = first rounded down to a multiple of 8, so
+// that the 16-B loads of 8 tile ids stay aligned; the slots before `first` take no part.  last - base <= the capacity, so the
+// grids of bucket_grid(capacity) CTAs cover every partition.
+struct BucketSpan {
+	uint32_t first, base, end, part;
+	__device__ __forceinline__ BucketSpan(const uint32_t *first_p, const uint32_t *last_p) {
+		first = first_p ? *first_p : 0u;
+		base = first & ~7u;
+		end = *last_p;
+		part = bucket_part(end - base);
+	}
+	__device__ __forceinline__ uint32_t parts() const { return (end - base) / part + ((end - base) % part != 0u); }
+};
+
 // TILES: tile_totals[2 t] += this partition's instances of tile t (ranges[t].y, zeroed by the caller)
 template <bool TILES>
-__global__ void __launch_bounds__(kBucketThreads) bucket_count_kernel(const uint16_t *__restrict__ keys, const uint32_t *__restrict__ status,
-                                                                    const uint32_t ntile, uint32_t *__restrict__ tile_totals,
-                                                                    uint32_t *__restrict__ digit_counts) {
+__global__ void __launch_bounds__(kBucketThreads) bucket_count_kernel(const uint16_t *__restrict__ keys, const uint32_t *__restrict__ first_p,
+                                                                    const uint32_t *__restrict__ last_p, const uint32_t ntile,
+                                                                    uint32_t *__restrict__ tile_totals, uint32_t *__restrict__ digit_counts) {
 	extern __shared__ uint32_t s_hist[];  // TILES: per tile id of keys_in; else per high digit of the intermediate words
 	__shared__ uint32_t s_digit[kDigits];
-	const uint32_t E = status[3], part = bucket_part(E);
-	const uint32_t begin = blockIdx.x * part;
-	if (begin >= E) return;  // (rows past the last partition are never read)
-	const uint32_t end = min(begin + part, E);
+	const BucketSpan sp(first_p, last_p);
+	const uint32_t begin = sp.base + blockIdx.x * sp.part;
+	if (begin >= sp.end) return;  // (rows past the last partition are never read)
+	const uint32_t end = min(begin + sp.part, sp.end), first = sp.first;
 	const uint32_t nbin = TILES ? ntile : (uint32_t)kDigits;
 	for (uint32_t t = threadIdx.x; t < nbin; t += kBucketThreads) s_hist[t] = 0u;
 	if (TILES && threadIdx.x < kDigits) s_digit[threadIdx.x] = 0u;
@@ -520,24 +537,24 @@ __global__ void __launch_bounds__(kBucketThreads) bucket_count_kernel(const uint
 	if (!TILES) {
 		const uint32_t *words = reinterpret_cast<const uint32_t *>(keys);
 		for (uint32_t i = begin + threadIdx.x * 4u; i < end; i += kBucketThreads * 4u) {
-			if (i + 4u <= end) {
+			if (i >= first && i + 4u <= end) {
 				const uint4 v = *reinterpret_cast<const uint4 *>(words + i);
 				atomicAdd(&s_hist[v.x >> kPackShift], 1u); atomicAdd(&s_hist[v.y >> kPackShift], 1u);
 				atomicAdd(&s_hist[v.z >> kPackShift], 1u); atomicAdd(&s_hist[v.w >> kPackShift], 1u);
 			} else {
-				for (uint32_t j = i; j < end; j++) atomicAdd(&s_hist[words[j] >> kPackShift], 1u);
+				for (uint32_t j = max(i, first); j < min(i + 4u, end); j++) atomicAdd(&s_hist[words[j] >> kPackShift], 1u);
 			}
 		}
 	} else
 	for (uint32_t i = begin + threadIdx.x * 8u; i < end; i += kBucketThreads * 8u) {
-		if (i + 8u <= end) {  // begin is a multiple of 8 and keys is 256-B aligned: one 16-B load of 8 tile ids
+		if (i >= first && i + 8u <= end) {  // begin is a multiple of 8 and keys is 256-B aligned: one 16-B load of 8 tile ids
 			const uint4 v = *reinterpret_cast<const uint4 *>(keys + i);
 			atomicAdd(&s_hist[v.x & 0xffffu], 1u); atomicAdd(&s_hist[v.x >> 16], 1u);
 			atomicAdd(&s_hist[v.y & 0xffffu], 1u); atomicAdd(&s_hist[v.y >> 16], 1u);
 			atomicAdd(&s_hist[v.z & 0xffffu], 1u); atomicAdd(&s_hist[v.z >> 16], 1u);
 			atomicAdd(&s_hist[v.w & 0xffffu], 1u); atomicAdd(&s_hist[v.w >> 16], 1u);
 		} else {
-			for (uint32_t j = i; j < end; j++) atomicAdd(&s_hist[keys[j]], 1u);
+			for (uint32_t j = max(i, first); j < min(i + 8u, end); j++) atomicAdd(&s_hist[keys[j]], 1u);
 		}
 	}
 	__syncthreads();
@@ -561,11 +578,10 @@ __global__ void __launch_bounds__(kBucketThreads) bucket_count_kernel(const uint
 // The (partition x digit) matrix: 32 digits per CTA (one per lane: coalesced rows), the partitions split into 32 contiguous slices
 // (one per warp).  Each warp sums its slice and the slice totals are scanned across the warps in shared memory: totals[d] = the
 // digit's total, and the slice is rewritten as the exclusive prefix over the partitions.
-__global__ void __launch_bounds__(1024) bucket_columns_kernel(uint32_t *__restrict__ counts, const uint32_t *__restrict__ status,
-                                                             uint32_t *__restrict__ totals) {
+__global__ void __launch_bounds__(1024) bucket_columns_kernel(uint32_t *__restrict__ counts, const uint32_t *__restrict__ first_p,
+                                                             const uint32_t *__restrict__ last_p, uint32_t *__restrict__ totals) {
 	__shared__ uint32_t s_tot[32][33];
-	const uint32_t E = status[3], part = bucket_part(E);
-	const uint32_t nparts = E / part + (E % part != 0u);
+	const uint32_t nparts = BucketSpan(first_p, last_p).parts();
 	const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
 	const uint32_t c = blockIdx.x * 32u + lane;
 	const uint32_t per = (nparts + 31u) / 32u;
@@ -585,10 +601,12 @@ __global__ void __launch_bounds__(1024) bucket_columns_kernel(uint32_t *__restri
 	}
 }
 
-// one CTA: ranges[t] = (start, start + total) from the exclusive scan of the tile totals in ranges[t].y, (0, 0) for a tile without
-// instances.  Warp w owns tiles [512 w, 512 w + 512), read and written 32 consecutive tiles at a time.
+// one CTA of 1024 threads: out[t] = (start, start + total(t)) from the exclusive scan of the tile totals, (0, 0) for a tile without
+// instances.  Warp w owns tiles [512 w, 512 w + 512), read and written 32 consecutive tiles at a time; every total is read before
+// any range is written, so `out` may be where the totals come from.
 constexpr int kRangesPerLane = kBucketMaxTiles / (32 * 32);
-__global__ void __launch_bounds__(1024) bucket_ranges_kernel(uint2 *__restrict__ ranges, const uint32_t ntile) {
+template <typename Total>
+__device__ __forceinline__ void scan_tile_ranges(const Total total, uint2 *out, const uint32_t ntile) {
 	__shared__ uint32_t s_warp[32];
 	const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
 	const uint32_t seg = w * 32u * kRangesPerLane;
@@ -596,7 +614,7 @@ __global__ void __launch_bounds__(1024) bucket_ranges_kernel(uint2 *__restrict__
 #pragma unroll
 	for (int j = 0; j < kRangesPerLane; j++) {
 		const uint32_t t = seg + j * 32u + lane;
-		tot[j] = t < ntile ? ranges[t].y : 0u;
+		tot[j] = t < ntile ? total(t) : 0u;
 	}
 	uint32_t carry = 0u;
 #pragma unroll
@@ -627,8 +645,16 @@ __global__ void __launch_bounds__(1024) bucket_ranges_kernel(uint2 *__restrict__
 #pragma unroll
 	for (int j = 0; j < kRangesPerLane; j++) {
 		const uint32_t t = seg + j * 32u + lane;
-		if (t < ntile) ranges[t] = tot[j] ? make_uint2(base + excl[j], base + excl[j] + tot[j]) : make_uint2(0u, 0u);
+		if (t < ntile) out[t] = tot[j] ? make_uint2(base + excl[j], base + excl[j] + tot[j]) : make_uint2(0u, 0u);
 	}
+}
+// ranges[t] = its range, from the tile totals the histogram pass accumulated in ranges[t].y
+struct BucketTotal {
+	const uint2 *ranges;
+	__device__ __forceinline__ uint32_t operator()(uint32_t t) const { return ranges[t].y; }
+};
+__global__ void __launch_bounds__(1024) bucket_ranges_kernel(uint2 *ranges, const uint32_t ntile) {
+	scan_tile_ranges(BucketTotal{ranges}, ranges, ntile);
 }
 
 struct TileDigit {
@@ -643,7 +669,8 @@ struct TileDigit {
 // counts, so the ranks are stable; the round is then staged in shared memory in digit order and written out in runs.
 template <bool HIGH>
 __global__ void __launch_bounds__(kPassThreads) bucket_pass_kernel(const uint16_t *__restrict__ keys, const uint32_t *__restrict__ vals,
-                                                                   const uint32_t *__restrict__ status, const uint32_t *__restrict__ prefix,
+                                                                   const uint32_t *__restrict__ first_p, const uint32_t *__restrict__ last_p,
+                                                                   const uint32_t *__restrict__ prefix,
                                                                    const uint32_t *__restrict__ totals, uint32_t *__restrict__ out) {
 	constexpr int kShift = HIGH ? kDigitBits : 0;
 	using Rank = cub::BlockRadixRankMatch<kPassThreads, kDigitBits, false>;
@@ -652,10 +679,13 @@ __global__ void __launch_bounds__(kPassThreads) bucket_pass_kernel(const uint16_
 	__shared__ uint16_t s_keys[kPassRound];
 	__shared__ uint32_t s_cursor[kDigits];  // per digit: output position of the first instance of this round
 	__shared__ uint32_t s_pref[kDigits];    // per digit: its first position in the round's digit order
-	const uint32_t E = status[3], part = bucket_part(E);
-	const uint32_t begin = blockIdx.x * part;
-	if (begin >= E) return;
-	const uint32_t end = min(begin + part, E);
+	// The rounds start at the partition's first slot in [first, last): a slot loaded but not bucketed still takes a rank among its
+	// digit and moves that digit's cursor, which is harmless only behind the last instance.
+	const BucketSpan sp(HIGH ? nullptr : first_p, last_p);  // (the intermediate words start at 0)
+	const uint32_t part_begin = sp.base + blockIdx.x * sp.part;
+	const uint32_t begin = max(part_begin, sp.first);
+	if (begin >= sp.end) return;
+	const uint32_t end = min(part_begin + sp.part, sp.end);
 	const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
 	if (threadIdx.x < 32) {  // digit starts (exclusive scan of the totals, 4 digits per lane) + this partition's prefix
 		const uint4 t4 = reinterpret_cast<const uint4 *>(totals)[lane];
@@ -680,7 +710,7 @@ __global__ void __launch_bounds__(kPassThreads) bucket_pass_kernel(const uint16_
 #pragma unroll
 		for (int j = 0; j < kPassItems; j++) {
 			const uint32_t i = base + warp * (32u * kPassItems) + j * 32u + lane;
-			const bool in = i < end;  // slots past E: the largest digit, behind every real instance of it, written nowhere
+			const bool in = i < end;  // slots past the end: the largest digit, behind every real instance of it, written nowhere
 			if (HIGH) {
 				const uint32_t x = in ? vals[i] : 0u;
 				k[j] = in ? (x >> kPackShift) << kDigitBits : 0xffffu;
@@ -721,28 +751,30 @@ __global__ void __launch_bounds__(kPassThreads) bucket_pass_kernel(const uint16_
 	}
 }
 
-// 16-bit tile ids, at most kBucketMaxTiles tiles and 2^25 Gaussians.  The intermediate words live in keys_out, the count matrices
-// and totals in the bucketing scratch.
-static cudaError_t launch_bucketing(const BinView &b, ImgView img, const uint32_t *status, int ntile, int64_t slots, cudaStream_t st) {
+// 16-bit tile ids, at most kBucketMaxTiles tiles and 2^25 Gaussians.  Buckets the instances [*first, *last) of (b.keys_in, b.vals_in)
+// (first = nullptr: from 0) into b.vals_out[0, *last - *first) and `ranges`; n_mid = the number of instances, *last - *first, on the
+// device.  The intermediate words live in keys_out, the count matrices and totals in the bucketing scratch.
+static cudaError_t launch_bucketing(const BinView &b, uint2 *ranges, const uint32_t *first, const uint32_t *last, const uint32_t *n_mid,
+                                   int ntile, int64_t slots, cudaStream_t st) {
 	static std::atomic<uint64_t> smem_count{0};
 	cudaError_t e;
 	if ((e = ensure_dynamic_smem(bucket_count_kernel<true>, kBucketMaxTiles * sizeof(uint32_t), smem_count)) != cudaSuccess) return e;
 	const BucketScratch sc = carve_bucket(b.bucket, slots);
 	const unsigned nparts = bucket_grid(slots);
 	const uint16_t *keys = reinterpret_cast<const uint16_t *>(b.keys_in);
-	// the tile totals accumulate in ranges[t].y (the far pass kept its unsaturated-tile table there until now)
-	if ((e = cudaMemsetAsync(img.ranges, 0, (size_t)ntile * sizeof(uint2), st)) != cudaSuccess) return e;
+	// the tile totals accumulate in ranges[t].y
+	if ((e = cudaMemsetAsync(ranges, 0, (size_t)ntile * sizeof(uint2), st)) != cudaSuccess) return e;
 	count_launch(7);
 	bucket_count_kernel<true><<<nparts, kBucketThreads, (size_t)ntile * sizeof(uint32_t), st>>>(
-		keys, status, (uint32_t)ntile, reinterpret_cast<uint32_t *>(img.ranges) + 1, sc.digit_counts[0]);
-	bucket_ranges_kernel<<<1, 1024, 0, st>>>(img.ranges, (uint32_t)ntile);
-	bucket_columns_kernel<<<kDigits / 32, 1024, 0, st>>>(sc.digit_counts[0], status, sc.digit_totals[0]);
+		keys, first, last, (uint32_t)ntile, reinterpret_cast<uint32_t *>(ranges) + 1, sc.digit_counts[0]);
+	bucket_ranges_kernel<<<1, 1024, 0, st>>>(ranges, (uint32_t)ntile);
+	bucket_columns_kernel<<<kDigits / 32, 1024, 0, st>>>(sc.digit_counts[0], first, last, sc.digit_totals[0]);
 	uint32_t *mid = b.keys_out;
-	bucket_pass_kernel<false><<<nparts, kPassThreads, 0, st>>>(keys, b.vals_in, status, sc.digit_counts[0], sc.digit_totals[0], mid);
-	bucket_count_kernel<false><<<nparts, kBucketThreads, kDigits * sizeof(uint32_t), st>>>(reinterpret_cast<const uint16_t *>(mid), status,
-	                                                                                     0u, nullptr, sc.digit_counts[1]);
-	bucket_columns_kernel<<<kDigits / 32, 1024, 0, st>>>(sc.digit_counts[1], status, sc.digit_totals[1]);
-	bucket_pass_kernel<true><<<nparts, kPassThreads, 0, st>>>(nullptr, mid, status, sc.digit_counts[1], sc.digit_totals[1], b.vals_out);
+	bucket_pass_kernel<false><<<nparts, kPassThreads, 0, st>>>(keys, b.vals_in, first, last, sc.digit_counts[0], sc.digit_totals[0], mid);
+	bucket_count_kernel<false><<<nparts, kBucketThreads, kDigits * sizeof(uint32_t), st>>>(reinterpret_cast<const uint16_t *>(mid), nullptr,
+	                                                                                     n_mid, 0u, nullptr, sc.digit_counts[1]);
+	bucket_columns_kernel<<<kDigits / 32, 1024, 0, st>>>(sc.digit_counts[1], nullptr, n_mid, sc.digit_totals[1]);
+	bucket_pass_kernel<true><<<nparts, kPassThreads, 0, st>>>(nullptr, mid, nullptr, n_mid, sc.digit_counts[1], sc.digit_totals[1], b.vals_out);
 	return cudaGetLastError();
 }
 
@@ -763,7 +795,7 @@ cudaError_t launch_binning(const FrameDev &f, GeomView g, const int32_t *radii, 
 	if ((e = cudaMemsetAsync(g.big_count, 0, sizeof(uint32_t), st)) != cudaSuccess) return e;
 	if (ntile <= 65535 || (!bounded && ntile <= 65536)) {  // 16-bit tile ids (the key arrays are allocated for 32-bit ids either way)
 		if ((e = launch_emit<uint16_t>(f, g, radii, b, g.offsets, g.big_count, cap32, n_order, st)) != cudaSuccess) return e;
-		if (bucketable(f)) return launch_bucketing(b, img, g.big_count, ntile, R, st);
+		if (bucketable(f)) return launch_bucketing(b, img.ranges, nullptr, g.big_count + 3, g.big_count + 3, ntile, R, st);
 		return launch_tile_sort<uint16_t>(b, img, g.big_count, ntile, R, bounded, st);
 	}
 	if ((e = launch_emit<uint32_t>(f, g, radii, b, g.offsets, g.big_count, cap32, n_order, st)) != cudaSuccess) return e;
@@ -774,9 +806,13 @@ cudaError_t launch_binning(const FrameDev &f, GeomView g, const int32_t *radii, 
 // Most instances of a frame lie behind the point where every pixel of their tile has saturated (T < 1e-4): the blend never reads
 // them.  The split emits and buckets the nearest Gaussians first (those whose depth-order offsets stay within the budget B), blends
 // those lists (blend_fwd.cu, kBlendNear), and emits the remaining Gaussians only into the tiles that pass left unsaturated.  The
-// emitted sequence is near ++ far, both in depth order, so one stable bucketing of [0, E) gives every unsaturated tile exactly the
-// list of the unsplit binning and every saturated tile its near part; kBlendResume finishes the unsaturated tiles from the stored
-// per-pixel state.  Images, n_contrib and tile_max_contrib do not depend on B.
+// emitted sequence is near ++ far, both in depth order, and the bucketing is stable, so a tile's list is its near list followed by
+// its far list: the far pass buckets the far instances alone and splices each tile's two lists.  Every unsaturated tile then has
+// exactly the list of the unsplit binning and every saturated tile its near part; kBlendResume finishes the unsaturated tiles from
+// the stored per-pixel state.  Images, n_contrib and tile_max_contrib do not depend on B.
+// Buffers: the emitted sequence is [0, E) of (keys_in, vals_in), as in the unsplit binning.  The near lists are bucketed through
+// vals_out into keys_out (split_near_lists), the far lists through vals_out into sort_temp (a bucketed frame never sorts, and
+// carve_bin sizes it for that), and the splice writes vals_out.
 
 // one thread: the split.  fit = Gaussians whose whole instance counts fit the capacity (all unless the bounded mode can overflow);
 // B = the budget (budget < 0: R / kNearBudgetDivisor), clamped to what fits; K = Gaussians whose inclusive offset is <= B.  The near
@@ -798,13 +834,15 @@ __global__ void split_status_kernel(const uint32_t *__restrict__ offsets, int n,
 // thread t = t-th Gaussian in depth order: its instance count in the emitted sequence.  Near Gaussians keep their scanned count;
 // a far one counts the tiles of its rectangle that the near blend left unsaturated, by the code emit_pairs / emit_big run.  Every
 // row span of that walk lies inside the rectangle, so a rectangle without an unsaturated tile (four table loads) counts 0 without it:
-// on config C almost every tile saturates in the near slab, and most far Gaussians stop there.
+// on config C almost every tile saturates in the near slab, and most far Gaussians stop there.  When no tile is left unsaturated
+// (the table's last entry is 0), no far Gaussian is gathered at all.
 __global__ void __launch_bounds__(256) far_count_kernel(const FrameDev f, const GaussRec *__restrict__ rec, const int32_t *__restrict__ radii,
                                                        const uint32_t *__restrict__ perm, const uint32_t *__restrict__ offsets,
                                                        const uint32_t *__restrict__ status, const int n_order,
                                                        const KeepUnsaturated keep, uint32_t *__restrict__ cnt) {
 	const int t = blockIdx.x * blockDim.x + threadIdx.x;
 	const int K = (int)status[kStatusSplitK];
+	const bool any = keep.sat[(size_t)f.gy * keep.stride + f.gx] != 0u;
 	bool active = false;
 	int x0 = 0, y0 = 0, x1 = 0, y1 = 0;
 	CullParams cp = {};
@@ -813,7 +851,7 @@ __global__ void __launch_bounds__(256) far_count_kernel(const FrameDev f, const 
 		const uint32_t off = t == 0 ? 0u : offsets[t - 1], end = offsets[t];
 		if (t < K) {
 			c = end - off;
-		} else if (end > off) {
+		} else if (any && end > off) {
 			const uint32_t gidx = perm[t];
 			const float4 q0 = rec[gidx].q0;
 			tile_rect(q0.x, q0.y, radii[gidx], f.gx, f.gy, x0, y0, x1, y1);
@@ -832,7 +870,7 @@ __global__ void __launch_bounds__(256) far_count_kernel(const FrameDev f, const 
 
 // one CTA, after the near blend: the table of KeepUnsaturated, sat[y * (gx + 1) + x] = unsaturated tiles (top bit of
 // tile_max_contrib) in rows < y and columns < x.  The warps prefix the tile rows, then the threads the columns.  sat lives in the img
-// ranges, which are free from the near blend until the final bucketing: (gx + 1)(gy + 1) <= 2 gx gy + 2 words.
+// state's split table: (gx + 1)(gy + 1) <= 2 gx gy + 2 words.
 constexpr int kSatBatch = 16;  // rows loaded ahead by each column thread
 __global__ void __launch_bounds__(1024) unsat_prefix_kernel(const uint32_t *__restrict__ tile_word, const int gx, const int gy, uint32_t *sat) {
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -866,18 +904,48 @@ __global__ void __launch_bounds__(1024) unsat_prefix_kernel(const uint32_t *__re
 	}
 }
 
-// one thread, after the scan of far_count_kernel's counts: E = the instances emitted.  A bounded frame overflows only if the emitted
-// sequence exceeds the capacity; it then keeps the Gaussians whose whole instance counts fit (split_status_kernel's `fit`), as the
-// one-pass binning does, so that an overflowing frame is the same whatever the budget.  The far emission reads E as its cap.
+// one thread, after the scan of far_count_kernel's counts: E = the instances emitted, E_far = E - E_near.  A bounded frame overflows
+// only if the emitted sequence exceeds the capacity; it then keeps the Gaussians whose whole instance counts fit (split_status_kernel's
+// `fit`), as the one-pass binning does, so that an overflowing frame is the same whatever the budget.  The far emission reads E as its
+// cap; the far bucketing covers [E_near, E) and its second digit pass the E_far words of the first.
 __global__ void split_total_kernel(const uint32_t *__restrict__ offsets, int n, uint32_t cap, uint32_t *__restrict__ status) {
 	const uint32_t total = offsets[n - 1];
-	if (total <= cap) {
-		status[3] = total;
-	} else {
+	uint32_t E = total;
+	if (total > cap) {
 		const int fit = (int)status[kStatusSplitFit];
-		status[3] = fit == 0 ? 0u : offsets[fit - 1];
+		E = fit == 0 ? 0u : offsets[fit - 1];
 		status[2] |= 1u;
 	}
+	status[3] = E;
+	status[kStatusFarEnd] = E - status[kStatusNear + 3];
+}
+
+// a tile's spliced list: its near list followed by its far list
+struct SplicedTotal {
+	const uint2 *near, *far;
+	__device__ __forceinline__ uint32_t operator()(uint32_t t) const {
+		const uint2 a = near[t], b = far[t];
+		return (a.y - a.x) + (b.y - b.x);
+	}
+};
+__global__ void __launch_bounds__(1024) splice_ranges_kernel(const uint2 *__restrict__ near, const uint2 *__restrict__ far, uint2 *__restrict__ out,
+                                                            const uint32_t ntile) {
+	scan_tile_ranges(SplicedTotal{near, far}, out, ntile);
+}
+// one warp per tile: its near list, then its far list, copied to the spliced range; the spliced range then replaces the near one
+constexpr int kSpliceWarps = 8;
+__global__ void __launch_bounds__(32 * kSpliceWarps) splice_lists_kernel(uint2 *ranges, const uint2 *__restrict__ far_ranges,
+                                                                         const uint2 *__restrict__ spliced, const uint32_t *__restrict__ near_lists,
+                                                                         const uint32_t *__restrict__ far_lists, uint32_t *__restrict__ out,
+                                                                         const uint32_t ntile) {
+	const uint32_t t = blockIdx.x * kSpliceWarps + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
+	if (t >= ntile) return;
+	const uint2 nr = ranges[t], fr = far_ranges[t], sr = spliced[t];
+	const uint32_t nn = nr.y - nr.x, nf = fr.y - fr.x;
+	for (uint32_t i = lane; i < nn; i += 32u) out[sr.x + i] = near_lists[nr.x + i];
+	for (uint32_t i = lane; i < nf; i += 32u) out[sr.x + nn + i] = far_lists[fr.x + i];
+	__syncwarp();  // (every lane has read ranges[t])
+	if (lane == 0) ranges[t] = sr;
 }
 
 bool split_applies(const FrameDev &f, int64_t R, int64_t budget, bool from_records) {
@@ -885,7 +953,8 @@ bool split_applies(const FrameDev &f, int64_t R, int64_t budget, bool from_recor
 	return !from_records && f.P > 0 && R > 0 && (budget < 0 || budget < R) && f.S == 0 && whole_image && bucketable(f);
 }
 
-// near pass: split, emit the Gaussians before it into [0, E_near), bucket them into vals_out / ranges.  slots = binning capacity.
+// near pass: split, emit the Gaussians before it into [0, E_near), bucket them into keys_out (split_near_lists) / ranges.
+// slots = binning capacity.
 cudaError_t launch_near_binning(const FrameDev &f, GeomView g, const int32_t *radii, BinView b, ImgView img, int64_t slots, cudaStream_t st,
                                 int64_t cap, int n_order, int64_t budget) {
 	const uint32_t cap32 = cap >= 0 ? (uint32_t)cap : 0xffffffffu;
@@ -894,32 +963,43 @@ cudaError_t launch_near_binning(const FrameDev &f, GeomView g, const int32_t *ra
 	split_status_kernel<<<1, 1, 0, st>>>(g.offsets, n_order, cap32, (long long)budget, g.big_count);
 	cudaError_t e = launch_emit<uint16_t>(f, g, radii, b, g.offsets, near, cap32, n_order, st, near + 3);
 	if (e != cudaSuccess) return e;
-	return launch_bucketing(b, img, near, f.gx * f.gy, slots, st);
+	BinView nb = split_near_lists(b);
+	nb.keys_out = b.vals_out;  // (the intermediate words)
+	return launch_bucketing(nb, img.ranges, nullptr, near + 3, near + 3, f.gx * f.gy, slots, st);
 }
 
 // far pass, after the near blend marked the unsaturated tiles: count, scan (into g.ckey; g.iota holds the counts — both are dead
-// after the depth sort of this forward), emit behind the near instances, and bucket the whole emitted sequence.
+// after the depth sort of this forward), emit behind the near instances, bucket [E_near, E) alone into sort_temp / img.far_ranges,
+// and splice the near and far lists into vals_out / ranges.
 cudaError_t launch_far_binning(const FrameDev &f, GeomView g, const int32_t *radii, BinView b, ImgView img, int64_t slots, cudaStream_t st,
                                int64_t cap, int n_order) {
 	const uint32_t cap32 = cap >= 0 ? (uint32_t)cap : 0xffffffffu;
+	const int ntile = f.gx * f.gy;
 	const unsigned nblk = (unsigned)((n_order + 255) / 256);
-	uint32_t *sat = reinterpret_cast<uint32_t *>(img.ranges);  // (gx + 1)(gy + 1) <= 2 (ntile + 1) words
+	uint32_t *sat = reinterpret_cast<uint32_t *>(img.split);  // (gx + 1)(gy + 1) <= 2 (ntile + 1) words
 	const KeepUnsaturated keep{sat, f.gx + 1};
 	uint32_t *far_offsets = g.ckey;
+	uint32_t *status = g.big_count, *near_end = g.big_count + kStatusNear + 3;
 	count_launch(2);
 	unsat_prefix_kernel<<<1, 1024, 0, st>>>(img.tile_max_contrib, f.gx, f.gy, sat);
-	far_count_kernel<<<nblk, 256, 0, st>>>(f, g.rec, radii, g.perm, g.offsets, g.big_count, n_order, keep, g.iota);
+	far_count_kernel<<<nblk, 256, 0, st>>>(f, g.rec, radii, g.perm, g.offsets, status, n_order, keep, g.iota);
 	cudaError_t e = cudaGetLastError();
 	if (e != cudaSuccess) return e;
 	size_t bytes = g.temp_bytes;
 	if ((e = cub::DeviceScan::InclusiveSum(g.temp, bytes, g.iota, far_offsets, n_order, st)) != cudaSuccess) return e;
-	if ((e = cudaMemsetAsync(g.big_count, 0, sizeof(uint32_t), st)) != cudaSuccess) return e;
+	if ((e = cudaMemsetAsync(status, 0, sizeof(uint32_t), st)) != cudaSuccess) return e;
 	count_launch();
-	split_total_kernel<<<1, 1, 0, st>>>(far_offsets, n_order, cap32, g.big_count);
-	if ((e = launch_emit<uint16_t>(f, g, radii, b, far_offsets, g.big_count, cap32, n_order, st, g.big_count + 3, g.big_count + kStatusNear + 3,
-	                               keep)) != cudaSuccess)
-		return e;
-	return launch_bucketing(b, img, g.big_count, f.gx * f.gy, slots, st);
+	split_total_kernel<<<1, 1, 0, st>>>(far_offsets, n_order, cap32, status);
+	if ((e = launch_emit<uint16_t>(f, g, radii, b, far_offsets, status, cap32, n_order, st, status + 3, near_end, keep)) != cudaSuccess) return e;
+	BinView fb = b;
+	fb.keys_out = b.vals_out;  // (the intermediate words)
+	fb.vals_out = reinterpret_cast<uint32_t *>(b.sort_temp);
+	if ((e = launch_bucketing(fb, img.far_ranges, near_end, status + 3, status + kStatusFarEnd, ntile, slots, st)) != cudaSuccess) return e;
+	count_launch(2);
+	splice_ranges_kernel<<<1, 1024, 0, st>>>(img.ranges, img.far_ranges, img.split, (uint32_t)ntile);
+	splice_lists_kernel<<<(unsigned)((ntile + kSpliceWarps - 1) / kSpliceWarps), 32 * kSpliceWarps, 0, st>>>(
+		img.ranges, img.far_ranges, img.split, split_near_lists(b).vals_out, fb.vals_out, b.vals_out, (uint32_t)ntile);
+	return cudaGetLastError();
 }
 
 }  // namespace sgr

@@ -74,6 +74,8 @@ ImgView carve_img(void *base, int W, int H, bool blend_state) {
 	v.tile_max_contrib = take<uint32_t>(p, gx * gy + 1);
 	v.n_contrib = take<uint32_t>(p, (size_t)W * H + 1);
 	v.blend_T = blend_state ? take<float>(p, (size_t)W * H) : nullptr;
+	v.far_ranges = blend_state ? take<uint2>(p, gx * gy + 1) : nullptr;
+	v.split = blend_state ? take<uint2>(p, gx * gy + 1) : nullptr;
 	v.total_bytes = (size_t)(p - reinterpret_cast<char *>(base));
 	return v;
 }
@@ -85,7 +87,7 @@ BinView carve_bin(void *base, int64_t R) {
 	b.keys_out = take<uint32_t>(p, n);
 	b.vals_in = take<uint32_t>(p, n);
 	b.vals_out = take<uint32_t>(p, n);
-	b.sort_temp_bytes = memo_bytes(R, [](int64_t n) { return sort_temp_bytes(n); });
+	b.sort_temp_bytes = std::max(memo_bytes(R, [](int64_t n) { return sort_temp_bytes(n); }), n * sizeof(uint32_t));
 	b.sort_temp = take<char>(p, b.sort_temp_bytes);
 	b.bucket_bytes = bucket_scratch_bytes(R);
 	b.bucket = take<char>(p, b.bucket_bytes);
@@ -300,7 +302,8 @@ static int forward_impl(const SgrFrame *frame, const float *means3D, const float
 	if (split_applies(f, R, budget, from_records)) {
 		const int64_t cap = bounded ? capacity : -1;
 		SGR_TRY(launch_near_binning(f, g, radii, b, img, R, st, cap, n_order, budget), "near binning");
-		SGR_TRY(launch_blend_fwd(f, g, b, img, nullptr, out_color, out_depth, out_alpha, nullptr, st, kBlendNear), "near blend_fwd");
+		SGR_TRY(launch_blend_fwd(f, g, split_near_lists(b), img, nullptr, out_color, out_depth, out_alpha, nullptr, st, kBlendNear),
+		        "near blend_fwd");
 		SGR_TRY(launch_far_binning(f, g, radii, b, img, R, st, cap, n_order), "far binning");
 		SGR_TRY(launch_blend_fwd(f, g, b, img, nullptr, out_color, out_depth, out_alpha, nullptr, st, kBlendResume), "resume blend_fwd");
 		return SGR_OK;

@@ -4,7 +4,8 @@
 //   geom state   : GaussRec[P] (48 B packed record, 3 x float4 — one 16-B aligned gather of 3 vectors per splat
 //                  instance in the blend passes), then tiles_touched / depth_key / iota / depth_sorted / perm / offsets
 //                  (u32[P] each) and cub temp storage.
-//   img state    : ranges uint2[Ntile], n_contrib u32[H*W], block-max n_contrib u32[Ntile], blend state f32[H*W] (saturation split)
+//   img state    : ranges uint2[Ntile], n_contrib u32[H*W], block-max n_contrib u32[Ntile], blend state f32[H*W], far ranges and
+//                  split table uint2[Ntile] each (saturation split)
 //   binning state: keys_in u32[R], keys_out u32[R] (tile ids), vals_in u32[R], vals_out u32[R] (= tile-ordered,
 //                  depth-sorted point list), sort temp, tile-bucketing scratch
 #pragma once
@@ -43,7 +44,7 @@ struct GeomView {
 	uint32_t *big_count;      // status words, zeroed per forward: [0] number of entries in big_list (device counter)
 	                          // [1] instance count R, [2] overflow bits (1 = instance capacity, 2 = Gaussian capacity of the compacted
 	                          // depth order), [3] instances actually emitted (bounded mode), [4] Gaussians with instances (compacted mode)
-	                          // [8..13] saturation split (kStatusNear ...)
+	                          // [8..14] saturation split (kStatusNear ...)
 	float4 *jac;              // per Gaussian with SH colour: 3 float4, d colour / d view direction + clamp bits (gaussian_geom.cuh)
 	uint32_t *ckey, *cval;    // compacted depth-sort input (keys / Gaussian indices), Gaussian-sharded forward only; the saturation
 	                          // split's far offsets live in ckey (and its far counts in iota, dead after the depth sort)
@@ -56,25 +57,35 @@ struct ImgView {
 	uint32_t *n_contrib;
 	uint32_t *tile_max_contrib;
 	float *blend_T;  // saturation split: T of each pixel of an unsaturated tile between the near blend and its resumption (sign = done)
+	// saturation split (forward img states only, like blend_T; ntile + 1 entries each): far_ranges = the per-tile ranges of the far
+	// lists; split = the unsaturated-tile table of the far pass (KeepUnsaturated), then the spliced ranges until they replace `ranges`
+	uint2 *far_ranges, *split;
 	size_t total_bytes;
 };
 
 // Saturation split (binning.cu launch_near_binning / launch_far_binning, blend_fwd.cu kBlendNear / kBlendResume): status words
 // kStatusNear.. = the near pass's block as the emission and bucketing read it ([+0] its big-list counter, [+3] its end E_near in the
-// emitted sequence); kStatusSplitK = Gaussians of the near pass (depth order), kStatusSplitFit = Gaussians that fit the capacity.
-constexpr int kStatusNear = 8, kStatusSplitK = 12, kStatusSplitFit = 13;
+// emitted sequence); kStatusSplitK = Gaussians of the near pass (depth order), kStatusSplitFit = Gaussians that fit the capacity;
+// kStatusFarEnd = instances the far pass emitted (the emitted sequence is E_near + that).
+constexpr int kStatusNear = 8, kStatusSplitK = 12, kStatusSplitFit = 13, kStatusFarEnd = 14;
 // the near budget when the caller sets none: R / kNearBudgetDivisor instances (DESIGN.md §7, sweep on config C)
 constexpr uint32_t kNearBudgetDivisor = 8;
 enum BlendPass { kBlendFull = 0, kBlendNear = 1, kBlendResume = 2 };
 struct BinView {
 	uint32_t *keys_in, *keys_out;  // tile ids
 	uint32_t *vals_in, *vals_out;  // Gaussian indices; vals_out is the tile-ordered, depth-sorted point list
-	void *sort_temp;
+	void *sort_temp;  // cub temp of the tile radix sort; in a bucketed frame the far lists of the saturation split (>= 4 B per slot)
 	size_t sort_temp_bytes;
 	void *bucket;  // tile-bucketing scratch (binning.cu carve_bucket): count matrices, digit totals
 	size_t bucket_bytes;
 	size_t total_bytes;
 };
+// The near pass of the saturation split leaves its per-tile lists in keys_out (vals_out receives the spliced lists of the far pass):
+// the view the near blend reads them through.
+static inline BinView split_near_lists(BinView b) {
+	b.vals_out = b.keys_out;
+	return b;
+}
 
 static inline size_t align_up(size_t v, size_t a = SGR_ALIGN) { return (v + a - 1) / a * a; }
 
