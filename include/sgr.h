@@ -104,6 +104,29 @@ int64_t sgr_set_near_budget(int64_t budget);
 int sgr_state_sizes(const SgrFrame *frame, size_t *geom_bytes, size_t *img_bytes);
 size_t sgr_binning_bytes(int64_t num_instances);
 
+/* Byte offsets of the sections of the three forward states, as the library carves them for `frame` and a binning state of
+ * num_instances slots (sgr_forward's instance count, or the capacity of a bounded forward: bounded != 0).  Every section starts
+ * 256-byte aligned; geom_bytes / img_bytes / binning_bytes are what sgr_state_sizes and sgr_binning_bytes report.  key_bytes is the
+ * width of the tile ids in keys_in (2 or 4).  Diagnostic only, like sgr_launch_count: it lets tests and tools read a state without
+ * restating its layout (DESIGN.md §3 gives each section's contents).  No reference counterpart. */
+typedef struct SgrStateLayout {
+	size_t rec, tiles_touched, depth_key, iota, depth_sorted, perm, offsets, big_list, status, jac, ckey, cval, geom_bytes;
+	size_t ranges, tile_max_contrib, n_contrib, blend_T, far_ranges, split, img_bytes;
+	size_t keys_in, keys_out, vals_in, vals_out, sort_temp, bucket, binning_bytes;
+	int32_t key_bytes;
+} SgrStateLayout;
+int sgr_state_layout(const SgrFrame *frame, int64_t num_instances, int32_t bounded, SgrStateLayout *out);
+/* Indices of the u32[64] status words (section `status` of the geom state; zeroed by every forward, words 1-8 are what
+ * sgr_forward_status_async copies). */
+#define SGR_STATUS_INSTANCES 1    /* instance count R of the frame */
+#define SGR_STATUS_OVERFLOW 2     /* overflow bits, as sgr_forward_status reports them */
+#define SGR_STATUS_EMITTED 3      /* instances emitted E: the emitted sequence is [0, E) of keys_in / vals_in */
+#define SGR_STATUS_NEAR 8         /* saturation split: the near pass's block of four words, laid out like words 0-3 */
+#define SGR_STATUS_NEAR_END (SGR_STATUS_NEAR + 3)  /* end E_near of the near pass in the emitted sequence */
+#define SGR_STATUS_SPLIT_K 12     /* Gaussians of the near pass, in depth order */
+#define SGR_STATUS_SPLIT_FIT 13   /* Gaussians whose whole instance counts fit the capacity */
+#define SGR_STATUS_FAR_END 14     /* instances the far pass emitted (E = E_near + this) */
+
 /* Forward rasterisation.  Replaces RasterizeGaussiansCUDA -> CudaRasterizer::Rasterizer::forward
  * (DGR/rasterize_points.cu:35-124, DGR/cuda_rasterizer/rasterizer_impl.cu:197-343; pybind name
  * `rasterize_gaussians`, DGR/ext.cpp:16).

@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libsgr.so")
 ABI_VERSION = 7
 
-SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_set_near_budget", "sgr_state_sizes", "sgr_binning_bytes", "sgr_forward", "sgr_forward_bounded",
+SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_set_near_budget", "sgr_state_sizes", "sgr_binning_bytes", "sgr_state_layout", "sgr_forward", "sgr_forward_bounded",
            "sgr_forward_status", "sgr_forward_status_async", "sgr_backward_blend",
            "sgr_backward_geom", "sgr_backward", "sgr_mark_visible", "sgr_visible_filter", "sgr_knn_scratch_bytes",
            "sgr_knn_mean_dist2", "sgr_record_bytes", "sgr_project", "sgr_forward_records",
@@ -47,6 +47,22 @@ class SgrFrame(C.Structure):
                 ("tan_fovx", C.c_float), ("tan_fovy", C.c_float), ("scale_modifier", C.c_float), ("prefiltered", C.c_int32),
                 ("debug", C.c_int32), ("row_begin", C.c_int32), ("row_end", C.c_int32), ("row_step", C.c_int32),
                 ("bg", C.c_void_p), ("viewmatrix", C.c_void_p), ("projmatrix", C.c_void_p), ("campos", C.c_void_p)]
+
+
+# sgr_state_layout: the byte offset of each section of the geom, img and binning states, in carve order, and each state's size
+GEOM_SECTIONS = ("rec", "tiles_touched", "depth_key", "iota", "depth_sorted", "perm", "offsets", "big_list", "status", "jac", "ckey", "cval")
+IMG_SECTIONS = ("ranges", "tile_max_contrib", "n_contrib", "blend_T", "far_ranges", "split")
+BIN_SECTIONS = ("keys_in", "keys_out", "vals_in", "vals_out", "sort_temp", "bucket")
+
+
+class SgrStateLayout(C.Structure):
+    _fields_ = ([(k, C.c_size_t) for k in GEOM_SECTIONS + ("geom_bytes",) + IMG_SECTIONS + ("img_bytes",) + BIN_SECTIONS + ("binning_bytes",)]
+                + [("key_bytes", C.c_int32)])
+
+
+# indices of the status words (SGR_STATUS_*, include/sgr.h)
+STATUS_INSTANCES, STATUS_OVERFLOW, STATUS_EMITTED = 1, 2, 3
+STATUS_NEAR, STATUS_NEAR_END, STATUS_SPLIT_K, STATUS_SPLIT_FIT, STATUS_FAR_END = 8, 11, 12, 13, 14
 
 
 MAX_PEERS = 16
@@ -163,6 +179,8 @@ def lib():
     L.sgr_state_sizes.argtypes = [C.POINTER(SgrFrame), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
     L.sgr_binning_bytes.restype = C.c_size_t
     L.sgr_binning_bytes.argtypes = [C.c_int64]
+    L.sgr_state_layout.restype = C.c_int
+    L.sgr_state_layout.argtypes = [C.POINTER(SgrFrame), C.c_int64, C.c_int32, C.POINTER(SgrStateLayout)]
     vp = C.c_void_p
     L.sgr_forward.restype = C.c_int
     L.sgr_forward.argtypes = [C.POINTER(SgrFrame)] + [vp] * 8 + [vp] * 5 + [vp, C.c_size_t, vp, C.c_size_t, ALLOC_FN, vp,
@@ -375,7 +393,7 @@ def stream(device) -> C.c_void_p:
 def call(name: str, device, *args) -> None:
     """Call the entry `name` with `args` and raise SgrError if it fails.  With a `device`, the call runs with that device current
     (work the library enqueues and the ALLOC_FN callbacks it makes target it) and gets the device's current stream as its last
-    argument.  device=None is for the entries that take no stream (sgr_state_sizes, sgr_layer_state_sizes)."""
+    argument.  device=None is for the entries that take no stream (sgr_state_sizes, sgr_state_layout, sgr_layer_state_sizes)."""
     fn = getattr(_lib or lib(), name)
     if device is None:
         rc = fn(*args)

@@ -793,7 +793,7 @@ cudaError_t launch_binning(const FrameDev &f, GeomView g, const int32_t *radii, 
 	if (bounded) R = cap;  // every pass below runs over the caller's capacity; the padding carries the largest key
 	if (R == 0) return cudaSuccess;
 	if ((e = cudaMemsetAsync(g.big_count, 0, sizeof(uint32_t), st)) != cudaSuccess) return e;
-	if (ntile <= 65535 || (!bounded && ntile <= 65536)) {  // 16-bit tile ids (the key arrays are allocated for 32-bit ids either way)
+	if (tile_key_bytes(ntile, bounded) == 2) {
 		if ((e = launch_emit<uint16_t>(f, g, radii, b, g.offsets, g.big_count, cap32, n_order, st)) != cudaSuccess) return e;
 		if (bucketable(f)) return launch_bucketing(b, img.ranges, nullptr, g.big_count + 3, g.big_count + 3, ntile, R, st);
 		return launch_tile_sort<uint16_t>(b, img, g.big_count, ntile, R, bounded, st);

@@ -231,6 +231,28 @@ int sgr_state_sizes(const SgrFrame *frame, size_t *geom_bytes, size_t *img_bytes
 
 size_t sgr_binning_bytes(int64_t R) { return carve_bin(nullptr, R).total_bytes; }
 
+int sgr_state_layout(const SgrFrame *frame, int64_t num_instances, int32_t bounded, SgrStateLayout *out) {
+	FrameDev f;
+	int rc = make_frame(frame, f);
+	if (rc) return rc;
+	if (!out || num_instances < 0) return fail(SGR_EINVAL, "out is NULL or num_instances %lld < 0", (long long)num_instances);
+	// carved from a null base, every section pointer is its byte offset
+	const GeomView g = carve_geom(nullptr, f.P);
+	const ImgView v = carve_img(nullptr, f.W, f.H);
+	const BinView b = carve_bin(nullptr, num_instances);
+	const auto at = [](const void *p) { return (size_t)reinterpret_cast<uintptr_t>(p); };
+	SgrStateLayout &l = *out;
+	l.rec = at(g.rec); l.tiles_touched = at(g.tiles_touched); l.depth_key = at(g.depth_key); l.iota = at(g.iota);
+	l.depth_sorted = at(g.depth_sorted); l.perm = at(g.perm); l.offsets = at(g.offsets); l.big_list = at(g.big_list);
+	l.status = at(g.big_count); l.jac = at(g.jac); l.ckey = at(g.ckey); l.cval = at(g.cval); l.geom_bytes = g.total_bytes;
+	l.ranges = at(v.ranges); l.tile_max_contrib = at(v.tile_max_contrib); l.n_contrib = at(v.n_contrib); l.blend_T = at(v.blend_T);
+	l.far_ranges = at(v.far_ranges); l.split = at(v.split); l.img_bytes = v.total_bytes;
+	l.keys_in = at(b.keys_in); l.keys_out = at(b.keys_out); l.vals_in = at(b.vals_in); l.vals_out = at(b.vals_out);
+	l.sort_temp = at(b.sort_temp); l.bucket = at(b.bucket); l.binning_bytes = b.total_bytes;
+	l.key_bytes = tile_key_bytes(f.gx * f.gy, bounded != 0);
+	return SGR_OK;
+}
+
 // shared body of sgr_forward (exact: reads the instance count back, asks the caller's allocator) and sgr_forward_bounded
 // (no host synchronisation: caller-sized binning state, count stays on the device)
 static int forward_impl(const SgrFrame *frame, const float *means3D, const float *shs, const float *colors_precomp,

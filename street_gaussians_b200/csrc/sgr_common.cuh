@@ -1,13 +1,7 @@
 // sgr_common.cuh — shared device helpers, state layout and the exact tile-cull test.
 //
-// Data layout in HBM (all caller-owned, see include/sgr.h):
-//   geom state   : GaussRec[P] (48 B packed record, 3 x float4 — one 16-B aligned gather of 3 vectors per splat
-//                  instance in the blend passes), then tiles_touched / depth_key / iota / depth_sorted / perm / offsets
-//                  (u32[P] each) and cub temp storage.
-//   img state    : ranges uint2[Ntile], n_contrib u32[H*W], block-max n_contrib u32[Ntile], blend state f32[H*W], far ranges and
-//                  split table uint2[Ntile] each (saturation split)
-//   binning state: keys_in u32[R], keys_out u32[R] (tile ids), vals_in u32[R], vals_out u32[R] (= tile-ordered,
-//                  depth-sorted point list), sort temp, tile-bucketing scratch
+// The caller-owned states (include/sgr.h) are carved by carve_geom / carve_img / carve_bin (capi.cu) into the views below;
+// sgr_state_layout reports the carved offsets.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -44,7 +38,7 @@ struct GeomView {
 	uint32_t *big_count;      // status words, zeroed per forward: [0] number of entries in big_list (device counter)
 	                          // [1] instance count R, [2] overflow bits (1 = instance capacity, 2 = Gaussian capacity of the compacted
 	                          // depth order), [3] instances actually emitted (bounded mode), [4] Gaussians with instances (compacted mode)
-	                          // [8..14] saturation split (kStatusNear ...)
+	                          // [8..14] saturation split (kStatusNear ...); include/sgr.h names them SGR_STATUS_*
 	float4 *jac;              // per Gaussian with SH colour: 3 float4, d colour / d view direction + clamp bits (gaussian_geom.cuh)
 	uint32_t *ckey, *cval;    // compacted depth-sort input (keys / Gaussian indices), Gaussian-sharded forward only; the saturation
 	                          // split's far offsets live in ckey (and its far counts in iota, dead after the depth sort)
@@ -67,7 +61,8 @@ struct ImgView {
 // kStatusNear.. = the near pass's block as the emission and bucketing read it ([+0] its big-list counter, [+3] its end E_near in the
 // emitted sequence); kStatusSplitK = Gaussians of the near pass (depth order), kStatusSplitFit = Gaussians that fit the capacity;
 // kStatusFarEnd = instances the far pass emitted (the emitted sequence is E_near + that).
-constexpr int kStatusNear = 8, kStatusSplitK = 12, kStatusSplitFit = 13, kStatusFarEnd = 14;
+constexpr int kStatusNear = SGR_STATUS_NEAR, kStatusSplitK = SGR_STATUS_SPLIT_K, kStatusSplitFit = SGR_STATUS_SPLIT_FIT,
+              kStatusFarEnd = SGR_STATUS_FAR_END;
 // the near budget when the caller sets none: R / kNearBudgetDivisor instances (DESIGN.md §7, sweep on config C)
 constexpr uint32_t kNearBudgetDivisor = 8;
 enum BlendPass { kBlendFull = 0, kBlendNear = 1, kBlendResume = 2 };
@@ -88,6 +83,9 @@ static inline BinView split_near_lists(BinView b) {
 }
 
 static inline size_t align_up(size_t v, size_t a = SGR_ALIGN) { return (v + a - 1) / a * a; }
+// Bytes per tile id in keys_in: 16-bit ids whenever every tile id fits below the bounded mode's padding key 0xFFFF (or, in the exact
+// mode, which pads nothing, fits at all); the key arrays are allocated for 32-bit ids either way.
+static inline int tile_key_bytes(int ntile, bool bounded) { return ntile <= 65535 || (!bounded && ntile <= 65536) ? 2 : 4; }
 
 // Number of kernels of THIS library enqueued so far by the process (cub's internal kernels are not counted); read through
 // sgr_launch_count() — bench.py reports the delta over its timed region as `gpu_launches`.

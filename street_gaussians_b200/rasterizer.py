@@ -16,6 +16,7 @@ from __future__ import annotations
 
 import contextlib
 import ctypes as C
+import math
 from typing import NamedTuple, Optional, Tuple
 
 import torch
@@ -78,8 +79,40 @@ def _dump(path: str, args) -> None:
 
 
 class _ForwardState:
-    """Caller-owned forward->backward state (the reference keeps geomBuffer/binningBuffer/imgBuffer byte tensors)."""
-    __slots__ = ("geom", "img", "binning", "num_instances")
+    """Caller-owned forward->backward state (the reference keeps geomBuffer/binningBuffer/imgBuffer byte tensors).  `bounded`: the
+    binning state holds `num_instances` slots of a bounded forward (its capacity) rather than the exact instance count."""
+    __slots__ = ("geom", "img", "binning", "num_instances", "bounded")
+
+
+def state_views(settings: GaussianRasterizationSettings, state: _ForwardState, P: int) -> dict:
+    """Named views into the byte tensors of a forward's state (P Gaussians), at the offsets sgr_state_layout reports.  For tests and
+    tools; the forward and backward never call it.  The u32 sections are int32 views: rec [P, 12] f32; the per-Gaussian sections
+    tiles_touched ... cval [P]; status [64] (_capi.STATUS_*); ranges [ntile, 2]; tile_max_contrib [ntile]; n_contrib [H, W]; keys_in
+    [R] as int16 or int32 (the tile-id width of the frame), keys_out, vals_in, vals_out [R], with R = state.num_instances.  The
+    binning views are absent when the forward allocated no binning state."""
+    fr, keep = _make_frame(settings, P, 0, 0, None, None)
+    lay = _capi.SgrStateLayout()
+    _capi.call("sgr_state_layout", None, C.byref(fr), state.num_instances, int(state.bounded), C.byref(lay))
+    del keep
+    H, W = int(settings.image_height), int(settings.image_width)
+    ntile = ((W + 15) // 16) * ((H + 15) // 16)
+
+    def view(buf, off, dtype, *shape):
+        return buf[off:off + dtype.itemsize * math.prod(shape)].view(dtype).reshape(shape)
+
+    i32 = torch.int32
+    v = dict(rec=view(state.geom, lay.rec, torch.float32, P, 12), status=view(state.geom, lay.status, i32, 64),
+             ranges=view(state.img, lay.ranges, i32, ntile, 2), tile_max_contrib=view(state.img, lay.tile_max_contrib, i32, ntile),
+             n_contrib=view(state.img, lay.n_contrib, i32, H, W))
+    for k in _capi.GEOM_SECTIONS:
+        if k not in ("rec", "status", "jac"):
+            v[k] = view(state.geom, getattr(lay, k), i32, P)
+    if state.binning is not None:
+        R = state.num_instances
+        v["keys_in"] = view(state.binning, lay.keys_in, torch.int16 if lay.key_bytes == 2 else i32, R)
+        for k in ("keys_out", "vals_in", "vals_out"):
+            v[k] = view(state.binning, getattr(lay, k), i32, R)
+    return v
 
 
 def _reference_inputs(means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, semantics):
@@ -247,6 +280,7 @@ def _forward_impl(means3D, sh, colors_precomp, semantics, opacities, scales, rot
     st = _ForwardState()
     st.num_instances = 0
     st.binning = None
+    st.bounded = False
     if P == 0:  # the reference short-circuits and returns zero-filled images (DGR/rasterize_points.cu:86)
         st.geom = st.img = None
         z = lambda c: torch.zeros((c, H, W), **f32)
@@ -277,7 +311,7 @@ def _forward_impl(means3D, sh, colors_precomp, semantics, opacities, scales, rot
                    ptr(st.img), ib.value, ptr(st.binning), nbytes, cap)
         if not capacity.frozen:
             capacity.record_status(fr, st.geom, device)
-        st.num_instances = cap
+        st.num_instances, st.bounded = cap, True
         del keep
         return color, radii, depth, alpha, semantic, st, tensors
 

@@ -179,6 +179,7 @@ def forward_records(settings: GaussianRasterizationSettings, band: Optional[Tile
     bin_ptr, n_inst = C.c_void_p(), C.c_int64(0)
     _capi.call("sgr_forward_records", device, C.byref(fr), ptr(radii_all), ptr(semantics_all), ptr(color), ptr(depth), ptr(alpha), ptr(semantic),
                ptr(st.geom), gb, ptr(st.img), ib, cb, None, C.byref(bin_ptr), C.byref(n_inst), ptr(st.binning) if bounded else None, nbytes, cap)
+    st.bounded = bounded
     if bounded:
         capacity.record_status(fr, st.geom, device)
         st.num_instances = cap

@@ -210,13 +210,15 @@ def test_header_compiles_as_c_and_struct_layouts_match_ctypes(tmp_path):
     field offsets as its C struct — the boundary a cgo / JNI / ctypes binding would be written against."""
     import subprocess
     src = tmp_path / "layout.c"
-    structs = ["SgrFrame", "SgrPeers", "SgrSegment", "SgrSegmentGrads", "SgrStatSegment", "SgrAdamTensor"]
+    structs = ["SgrFrame", "SgrPeers", "SgrSegment", "SgrSegmentGrads", "SgrStatSegment", "SgrAdamTensor", "SgrStateLayout"]
+    status = ["INSTANCES", "OVERFLOW", "EMITTED", "NEAR", "NEAR_END", "SPLIT_K", "SPLIT_FIT", "FAR_END"]
     body = ['#include <stdio.h>', '#include <stddef.h>', '#include "sgr.h"', 'int main(void) {']
     for name in structs:
         body.append(f'  printf("{name} %zu\\n", sizeof({name}));')
         body += [f'  printf("{name}.{f[0]} %zu\\n", offsetof({name}, {f[0]}));' for f in getattr(_capi, name)._fields_]
     body += ['  printf("SGR_MAX_PEERS %d\\n", SGR_MAX_PEERS);', '  printf("SGR_ABI_VERSION %d\\n", SGR_ABI_VERSION);',
-             '  printf("SGR_MAX_FOURIER %d\\n", SGR_MAX_FOURIER);', '  return 0;', '}']
+             '  printf("SGR_MAX_FOURIER %d\\n", SGR_MAX_FOURIER);']
+    body += [f'  printf("SGR_STATUS_{w} %d\\n", SGR_STATUS_{w});' for w in status] + ['  return 0;', '}']
     src.write_text("\n".join(body))
     exe = tmp_path / "layout"
     subprocess.run(["/usr/bin/gcc", "-std=c99", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
@@ -228,6 +230,8 @@ def test_header_compiles_as_c_and_struct_layouts_match_ctypes(tmp_path):
             assert int(out[f"{name}.{f[0]}"]) == getattr(ct, f[0]).offset, (name, f[0])
     assert int(out["SGR_MAX_PEERS"]) == _capi.MAX_PEERS and int(out["SGR_ABI_VERSION"]) == _capi.ABI_VERSION
     assert int(out["SGR_MAX_FOURIER"]) == _capi.MAX_FOURIER
+    for w in status:
+        assert int(out[f"SGR_STATUS_{w}"]) == getattr(_capi, f"STATUS_{w}"), w
 
 
 def test_gaussian_sharded_entry_points_validate_before_touching_cuda():

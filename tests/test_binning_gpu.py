@@ -10,15 +10,12 @@ import util
 import street_gaussians_b200 as sgb
 from street_gaussians_b200 import rasterizer as R
 from street_gaussians_b200 import synthetic
+from street_gaussians_b200._capi import STATUS_EMITTED
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 K = 32768           # largest bucketing partition (csrc/binning.cu kBucketMaxPart; a frame's partitions hold bucket_part(E) instances)
 MAX_TILES = 16384   # largest frame that buckets (csrc/binning.cu kBucketMaxTiles)
-
-
-def _align(n):
-    return (n + 255) // 256 * 256
 
 
 def bin_lists(scene, band=None, capacity=None):
@@ -31,23 +28,14 @@ def bin_lists(scene, band=None, capacity=None):
                               dv("rotations"), dv("cov3D_precomp"), st, band, capacity)
     fst = out[5]
     torch.cuda.synchronize()
-    W, H = cam["image_width"], cam["image_height"]
-    ntile = ((W + 15) // 16) * ((H + 15) // 16)
-    n = max(P, 1)
-    status = fst.geom[_align(48 * n) + 7 * _align(4 * n):][:64].view(torch.int32)
-    E = int(status[3])
-    ranges = fst.img[:8 * ntile].view(torch.int32).reshape(ntile, 2).long()
-    cap = fst.num_instances
-    b = _align(4 * max(cap, 1))
-    if cap == 0:
+    v = R.state_views(st, fst, P)
+    E = int(v["status"][STATUS_EMITTED])
+    ranges, ntile = v["ranges"].long(), v["ranges"].shape[0]
+    if fst.num_instances == 0:
         empty = torch.zeros(0, dtype=torch.long, device=DEV)
         return dict(E=E, ntile=ntile, keys=empty, vals=empty, out=empty, ranges=ranges)
-    kdt = torch.int16 if ntile <= 65535 or (capacity is None and ntile <= 65536) else torch.int32
-    ksz = 2 if kdt == torch.int16 else 4
-    keys = fst.binning[:ksz * E].view(kdt).long() & (0xFFFF if ksz == 2 else 0xFFFFFFFF)
-    vals = fst.binning[2 * b:2 * b + 4 * E].view(torch.int32).long()
-    lst = fst.binning[3 * b:3 * b + 4 * E].view(torch.int32).long()
-    return dict(E=E, ntile=ntile, keys=keys, vals=vals, out=lst, ranges=ranges)
+    keys = v["keys_in"][:E].long() & (0xFFFF if v["keys_in"].dtype == torch.int16 else 0xFFFFFFFF)
+    return dict(E=E, ntile=ntile, keys=keys, vals=v["vals_in"][:E].long(), out=v["vals_out"][:E].long(), ranges=ranges)
 
 
 def check_lists(d, expect_E=None):

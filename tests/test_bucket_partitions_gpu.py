@@ -15,6 +15,7 @@ import street_gaussians_b200 as sgb
 from street_gaussians_b200 import _capi
 from street_gaussians_b200 import rasterizer as R
 from street_gaussians_b200 import synthetic
+from street_gaussians_b200._capi import STATUS_EMITTED, STATUS_INSTANCES, STATUS_NEAR_END, STATUS_SPLIT_K
 import util
 from test_binning_gpu import bin_lists, capacity_of, check_lists, single_tile_scene
 from test_saturation_split_gpu import render, scene_of, splats
@@ -25,7 +26,6 @@ ALL, AUTO = _capi.NEAR_BUDGET_ALL, _capi.NEAR_BUDGET_AUTO
 TARGET_PARTS = 396   # csrc/binning.cu kBucketTargetParts
 ROUND = 2048         # kPassRound
 MAX_PART = 32768     # kBucketMaxPart
-NEAR_END, SPLIT_K = 8 + 3, 12  # status words (csrc/sgr_common.cuh kStatusNear + 3, kStatusSplitK)
 
 
 def part_size(E):
@@ -113,7 +113,7 @@ def test_split_frame(B):
     d = lists(sc, B)
     check_lists(d, expect_E=n)
     full, got = render(sc, ALL, backward=False), render(sc, B, backward=False)
-    assert int(got["status"][NEAR_END]) == B and int(got["status"][3]) == n
+    assert int(got["status"][STATUS_NEAR_END]) == B and int(got["status"][STATUS_EMITTED]) == n
     for k in ("color", "depth", "alpha", "radii", "n_contrib", "tile_max"):
         assert torch.equal(full[k], got[k]), k
     assert part_size(n) == 2 * ROUND and part_size(B) == (2 * ROUND if B > TARGET_PARTS * ROUND else ROUND)
@@ -133,10 +133,6 @@ def test_cyclic_band(E):
 
 # ---- far count ----
 
-def _align(n):
-    return (n + 255) // 256 * 256
-
-
 def split_state(scene, budget):
     """Forward at `budget`: status words, depth order (perm), counts per depth slot (iota), emitted sequence and lists."""
     cam = scene["cam"]
@@ -147,17 +143,11 @@ def split_state(scene, budget):
         out = R._forward_impl(dv("means3D"), dv("shs"), None, None, dv("opacities"), dv("scales"), dv("rotations"), None, st, None, None)
     fst = out[5]
     torch.cuda.synchronize()
-    W, H = cam["image_width"], cam["image_height"]
-    ntile = ((W + 15) // 16) * ((H + 15) // 16)
-    base, u = _align(48 * P), _align(4 * P)
-    sec = lambda i: fst.geom[base + i * u:base + i * u + 4 * P].view(torch.int32).long()
-    status = fst.geom[base + 7 * u:][:64].view(torch.int32).long().cpu()
-    E = int(status[3])
-    b = _align(4 * fst.num_instances)
-    return dict(status=status, iota=sec(2), perm=sec(4), ntile=ntile, E=E,
-                keys=fst.binning[:2 * E].view(torch.int16).long() & 0xFFFF, vals=fst.binning[2 * b:2 * b + 4 * E].view(torch.int32).long(),
-                out=fst.binning[3 * b:3 * b + 4 * E].view(torch.int32).long(),
-                ranges=fst.img[:8 * ntile].view(torch.int32).reshape(ntile, 2).long())
+    v = R.state_views(st, fst, P)
+    status = v["status"].long().cpu()
+    E = int(status[STATUS_EMITTED])
+    return dict(status=status, iota=v["iota"].long(), perm=v["perm"].long(), ntile=v["ranges"].shape[0], E=E,
+                keys=v["keys_in"][:E].long() & 0xFFFF, vals=v["vals_in"][:E].long(), out=v["vals_out"][:E].long(), ranges=v["ranges"].long())
 
 
 def check_far_counts(scene, budget):
@@ -166,7 +156,7 @@ def check_far_counts(scene, budget):
     check_lists(full)
     check_lists(split)
     P, ntile = scene["means3D"].shape[0], full["ntile"]
-    K = int(split["status"][SPLIT_K])
+    K = int(split["status"][STATUS_SPLIT_K])
     slot = torch.empty(P, dtype=torch.long, device=DEV)
     slot[split["perm"]] = torch.arange(P, device=DEV)
     far_pair = slot[full["vals"]] >= K
@@ -217,7 +207,7 @@ def test_far_count_holes_at_corners_and_edge():
               (W / 2, H / 2, 60.0)]             # a large rectangle around the middle, far from every hole
     sc, n_wall_gauss, n_bg = holed_wall_scene(W, H, holes, probes)
     B = int(render(scene_of(sc["cam"], *[{k: sc[k][:n_wall_gauss] for k in ("means3D", "scales", "rotations", "opacities", "shs")}]),
-                   ALL, backward=False)["status"][1])
+                   ALL, backward=False)["status"][STATUS_INSTANCES])
     unsat, walk = check_far_counts(sc, B)
     for tx, ty in holes:
         assert bool(unsat[ty * gx + tx]), (tx, ty)

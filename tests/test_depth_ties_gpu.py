@@ -26,20 +26,16 @@ from oracle import raster64 as R64
 import street_gaussians_b200 as sgb
 from street_gaussians_b200 import _capi, synthetic, training
 from street_gaussians_b200 import rasterizer as R
+from street_gaussians_b200._capi import STATUS_EMITTED, STATUS_INSTANCES, STATUS_NEAR_END, STATUS_OVERFLOW, STATUS_SPLIT_K
 from test_bucket_partitions_gpu import part_size, split_state
 from test_saturation_split_gpu import assert_same, render
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 ALL, AUTO = _capi.NEAR_BUDGET_ALL, _capi.NEAR_BUDGET_AUTO
-NEAR_END, SPLIT_K = 8 + 3, 12  # status words (csrc/sgr_common.cuh kStatusNear + 3, kStatusSplitK)
 MAX_BUCKET_TILES = 16384       # csrc/binning.cu kBucketMaxTiles
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "live", "ties.npz")
 REPORT = {}
-
-
-def _align(n):
-    return (n + 255) // 256 * 256
 
 
 def frame_lists(scene, band=None, capacity=None, budget=ALL):
@@ -54,16 +50,12 @@ def frame_lists(scene, band=None, capacity=None, budget=ALL):
                               None, st, band, capacity)
     fst = out[5]
     torch.cuda.synchronize()
-    W, H = cam["image_width"], cam["image_height"]
-    ntile = ((W + 15) // 16) * ((H + 15) // 16)
-    status = fst.geom[_align(48 * P) + 7 * _align(4 * P):][:64].view(torch.int32).long().cpu()
-    E = int(status[3])
-    b = _align(4 * max(fst.num_instances, 1))
-    lst = fst.binning[3 * b:3 * b + 4 * E].view(torch.int32).long()
-    rec = fst.geom[:48 * P].view(torch.float32).reshape(P, 12)
-    bits = rec[:, 7].contiguous().view(torch.int32).long()
-    ranges = fst.img[:8 * ntile].view(torch.int32).reshape(ntile, 2).long()
-    return dict(list=lst, ranges=ranges, status=status, E=E, bits=bits, radii=out[1], ntile=ntile)
+    v = R.state_views(st, fst, P)
+    status = v["status"].long().cpu()
+    E = int(status[STATUS_EMITTED])
+    bits = v["rec"][:, 7].contiguous().view(torch.int32).long()
+    return dict(list=v["vals_out"][:E].long(), ranges=v["ranges"].long(), status=status, E=E, bits=bits, radii=out[1],
+                ntile=v["ranges"].shape[0])
 
 
 def check_order(d):
@@ -108,9 +100,9 @@ def _path(d, ntile_cond, split=False):
     st = d["status"]
     assert ntile_cond(d["ntile"]), d["ntile"]
     if split:
-        assert int(st[NEAR_END]) < int(st[1]), "the split took effect: the near pass holds part of the frame"
+        assert int(st[STATUS_NEAR_END]) < int(st[STATUS_INSTANCES]), "the split took effect: the near pass holds part of the frame"
     else:
-        assert int(st[3]) == int(st[1]), "one pass: every instance emitted"
+        assert int(st[STATUS_EMITTED]) == int(st[STATUS_INSTANCES]), "one pass: every instance emitted"
 
 
 MODES = ["bucketed", "sort16", "sort32", "band", "bounded", "split"]
@@ -142,7 +134,7 @@ def test_list_order(mode, cases, wide):
         for sc in [c["scene"] for c in cases.values()] + [quantized_scene(1920, 1280)]:
             R_ = frame_lists(sc)["E"]
             d = frame_lists(sc, capacity=sgb.InstanceCapacity(initial=R_ + 100))
-            assert int(d["status"][2]) == 0 and d["E"] == R_
+            assert int(d["status"][STATUS_OVERFLOW]) == 0 and d["E"] == R_
             scenes.append(check_order(d))
     elif mode == "split":
         for sc in [cases["groups"]["scene"], cases["stack"]["scene"], quantized_scene(1920, 1280)]:
@@ -217,7 +209,7 @@ def test_per_element_band_bounded_split(cases):
     T64.check("ties_bounded", sc, capacity=R.InstanceCapacity(initial=R_ + 64), max_removed=0.0)
     for budget in (AUTO, R_ // 3):
         with _capi.near_budget(budget):
-            assert int(frame_lists(sc, budget=budget)["status"][NEAR_END]) < R_
+            assert int(frame_lists(sc, budget=budget)["status"][STATUS_NEAR_END]) < R_
             T64.check(f"ties_split{budget}", sc, max_removed=0.0)
 
 
@@ -230,7 +222,7 @@ def test_every_split_of_a_tied_stack(cases):
     sc = c["scene"]
     P = sc["means3D"].shape[0]
     full = render(sc, ALL)
-    Rn = int(full["status"][1])
+    Rn = int(full["status"][STATUS_INSTANCES])
     # depth-order slot of every Gaussian: (depth, index) order; all of the stack is visible
     z = sc["means3D"][:, 2].double()
     slot = torch.empty(P, dtype=torch.long)
@@ -241,12 +233,12 @@ def test_every_split_of_a_tied_stack(cases):
     for b in range(Rn + 1):
         got = render(sc, b)
         assert_same(full, got, what=f"B={b}")
-        K = int(got["status"][SPLIT_K])
+        K = int(got["status"][STATUS_SPLIT_K])
         if not any(lo < K < hi for lo, hi in spans):
             continue
         inside.append(b)
         s = split_state(sc, b)
-        assert int(s["status"][SPLIT_K]) == K
+        assert int(s["status"][STATUS_SPLIT_K]) == K
         assert torch.equal(s["perm"][:K].cpu().sort().values, torch.nonzero(slot < K).reshape(-1).sort().values)
         ln = s["ranges"][:, 1] - s["ranges"][:, 0]
         tile = torch.repeat_interleave(torch.arange(s["ntile"], device=DEV), ln)

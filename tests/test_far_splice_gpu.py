@@ -10,12 +10,12 @@ import pytest
 import torch
 
 from street_gaussians_b200 import _capi, synthetic
+from street_gaussians_b200._capi import STATUS_EMITTED, STATUS_FAR_END, STATUS_INSTANCES, STATUS_NEAR_END, STATUS_OVERFLOW
 from test_binning_gpu import bin_lists, capacity_of, check_lists, single_tile_scene
 from test_saturation_split_gpu import assert_same, render, scene_of, splats, wall_scene
 
 pytestmark = pytest.mark.gpu
 ALL, AUTO = _capi.NEAR_BUDGET_ALL, _capi.NEAR_BUDGET_AUTO
-NEAR_END, FAR_END = 8 + 3, 14  # status words (csrc/sgr_common.cuh kStatusNear + 3, kStatusFarEnd)
 
 
 def split_lists(scene, budget, capacity=None):
@@ -31,9 +31,9 @@ def status(scene, budget, capacity=None):
 
 def test_empty_far_slab():
     sc, walls = wall_scene(640, 480)
-    R_wall = int(status(walls, ALL)[1])
+    R_wall = int(status(walls, ALL)[STATUS_INSTANCES])
     st = status(sc, R_wall)
-    assert int(st[NEAR_END]) == R_wall and int(st[3]) == R_wall and int(st[FAR_END]) == 0
+    assert int(st[STATUS_NEAR_END]) == R_wall and int(st[STATUS_EMITTED]) == R_wall and int(st[STATUS_FAR_END]) == 0
     d = split_lists(sc, R_wall)
     assert d["E"] == R_wall
     assert_same(render(sc, ALL), render(sc, R_wall), what="empty far slab")
@@ -42,7 +42,7 @@ def test_empty_far_slab():
 def test_whole_sequence_far():
     sc, _ = wall_scene(640, 480, seed=1, layers=2)
     st = status(sc, 0)
-    assert int(st[NEAR_END]) == 0 and int(st[FAR_END]) == int(st[3]) == int(st[1])
+    assert int(st[STATUS_NEAR_END]) == 0 and int(st[STATUS_FAR_END]) == int(st[STATUS_EMITTED]) == int(st[STATUS_INSTANCES])
     split_lists(sc, 0)
     assert_same(render(sc, ALL), render(sc, 0), what="B = 0")
 
@@ -59,13 +59,13 @@ def test_far_only_tiles():
     bg = splats(cam, torch.rand(n, generator=gen) * W, torch.rand(n, generator=gen) * H, 5 + 40 * torch.rand(n, generator=gen),
                 1 + 6 * torch.rand(n, generator=gen), 0.3 + 0.6 * torch.rand(n, generator=gen), 50)
     sc, wall_sc = scene_of(cam, *walls, bg), scene_of(cam, *walls)
-    R_wall = int(status(wall_sc, ALL)[1])
+    R_wall = int(status(wall_sc, ALL)[STATUS_INSTANCES])
     full = render(sc, ALL)
     for b in (R_wall, R_wall + 1, AUTO):
         d = split_lists(sc, b)
         assert_same(full, render(sc, b), what=f"B={b}")
     st = status(sc, R_wall)
-    assert int(st[NEAR_END]) == R_wall and int(st[FAR_END]) > 0
+    assert int(st[STATUS_NEAR_END]) == R_wall and int(st[STATUS_FAR_END]) > 0
     d = split_lists(sc, R_wall)
     near_tiles = torch.bincount(d["keys"][:R_wall], minlength=d["ntile"]) > 0
     far_tiles = torch.bincount(d["keys"][R_wall:], minlength=d["ntile"]) > 0
@@ -82,7 +82,7 @@ def test_near_end_at_every_alignment():
     full = render(sc, ALL)
     for b in range(4096, 4096 + 9):
         st = status(sc, b)
-        assert int(st[NEAR_END]) == b and int(st[3]) == n
+        assert int(st[STATUS_NEAR_END]) == b and int(st[STATUS_EMITTED]) == n
         split_lists(sc, b)
         assert_same(full, render(sc, b), what=f"B={b}")
 
@@ -92,15 +92,15 @@ def test_overflow_inside_the_far_slab():
     one-pass binning with that capacity does."""
     sc = synthetic.make_config("B", seed=2)
     st = status(sc, AUTO)
-    E_near, E = int(st[NEAR_END]), int(st[3])
+    E_near, E = int(st[STATUS_NEAR_END]), int(st[STATUS_EMITTED])
     assert E > E_near + 16
     far_emitted = False
     for cap in (E_near + 1, (E_near + E) // 2, E - 1):
         split = render(sc, AUTO, capacity=cap)
         s = split["status"]
-        assert int(s[2]) & 1 and int(s[3]) <= cap
-        assert int(s[FAR_END]) == int(s[3]) - int(s[NEAR_END])
-        far_emitted |= int(s[FAR_END]) > 0
+        assert int(s[STATUS_OVERFLOW]) & 1 and int(s[STATUS_EMITTED]) <= cap
+        assert int(s[STATUS_FAR_END]) == int(s[STATUS_EMITTED]) - int(s[STATUS_NEAR_END])
+        far_emitted |= int(s[STATUS_FAR_END]) > 0
         split_lists(sc, AUTO, capacity=cap)
         assert_same(render(sc, ALL, capacity=cap), split, what=f"cap={cap}")
     assert far_emitted
@@ -109,8 +109,8 @@ def test_overflow_inside_the_far_slab():
 def test_many_far_partitions():
     """Config C at a small budget: the far slab spans several partitions of the bucketing."""
     sc = synthetic.make_config("C", seed=0)
-    R_ = int(status(sc, ALL)[1])
+    R_ = int(status(sc, ALL)[STATUS_INSTANCES])
     b = R_ // 64
     st = status(sc, b)
-    assert int(st[FAR_END]) > 4 * 2048
+    assert int(st[STATUS_FAR_END]) > 4 * 2048
     split_lists(sc, b)

@@ -263,7 +263,7 @@ def test_geometry_bitwise_vs_reference():
                                                            scene["opacities"].to(dev), scene["scales"].to(dev), scene["rotations"].to(dev),
                                                            None, mst, None)
     torch.cuda.synchronize()
-    rec = fst.geom[:P * 48].cpu().numpy().view(np.float32).reshape(P, 12)
+    rec = R.state_views(mst, fst, P)["rec"].cpu().numpy()
     ref_radii = z["ref_radii"]  # (GeometryState.internal_radii is unused when the caller passes a radii tensor)
     assert (rad.cpu().numpy() == ref_radii).all()
     assert (ref_radii > 0).sum() > 50_000

@@ -27,10 +27,6 @@ DEV = "cuda"
 REPORT = {}
 
 
-def _align(n):
-    return (n + 255) // 256 * 256
-
-
 def run_kernels(scene, band=None, capacity=None, backward=True):
     """Forward + backward stage 1 through the library; returns the images, grad2d and the kernel's own records / lists."""
     cam = scene["cam"]
@@ -48,19 +44,10 @@ def run_kernels(scene, band=None, capacity=None, backward=True):
             g2d, gsem = R._backward_blend_impl(st, band, fst, tens, alp, scene["grad_color"].to(DEV), scene["grad_depth"].to(DEV),
                                                scene["grad_alpha"].to(DEV), gs)
     torch.cuda.synchronize()
-    W, H = cam["image_width"], cam["image_height"]
-    ntile = ((W + 15) // 16) * ((H + 15) // 16)
-    rec = fst.geom[:P * 48].view(torch.float32).reshape(P, 12).clone()
-    img = fst.img
-    o = 0
-    ranges = img[o:o + 8 * ntile].view(torch.int32).reshape(ntile, 2).clone(); o += _align(8 * (ntile + 1))
-    o += _align(4 * (ntile + 1))
-    n_contrib = img[o:o + 4 * W * H].view(torch.int32).reshape(H, W).clone()
-    R_ = fst.num_instances
-    b = _align(4 * max(R_, 1))
-    vals_out = fst.binning[3 * b:3 * b + 4 * R_].view(torch.int32).clone() if R_ else torch.zeros(0, dtype=torch.int32, device=DEV)
-    return dict(color=col, depth=dep, alpha=alp, semantic=sem, radii=rad, grad2d=g2d, gsem=gsem, rec=rec, ranges=ranges,
-                n_contrib=n_contrib, list=vals_out, state=fst, tensors=tens, settings=st)
+    v = R.state_views(st, fst, P)
+    vals_out = v["vals_out"].clone() if fst.num_instances else torch.zeros(0, dtype=torch.int32, device=DEV)
+    return dict(color=col, depth=dep, alpha=alp, semantic=sem, radii=rad, grad2d=g2d, gsem=gsem, rec=v["rec"].clone(), ranges=v["ranges"].clone(),
+                n_contrib=v["n_contrib"].clone(), list=vals_out, state=fst, tensors=tens, settings=st)
 
 
 def check(name, scene, band=None, capacity=None, delta=R64.margins.__defaults__[0], backward=True, max_removed=0.1, kept=None):

@@ -12,15 +12,11 @@ import street_gaussians_b200 as sgb
 from street_gaussians_b200 import _capi
 from street_gaussians_b200 import rasterizer as R
 from street_gaussians_b200 import synthetic
+from street_gaussians_b200._capi import STATUS_EMITTED, STATUS_INSTANCES, STATUS_NEAR_END, STATUS_OVERFLOW
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 ALL, AUTO = _capi.NEAR_BUDGET_ALL, _capi.NEAR_BUDGET_AUTO
-NEAR_END = 8 + 3  # status word: end of the near pass in the emitted sequence (csrc/sgr_common.cuh, kStatusNear + 3)
-
-
-def _align(n):
-    return (n + 255) // 256 * 256
 
 
 def render(scene, budget, capacity=None, backward=True):
@@ -31,18 +27,13 @@ def render(scene, budget, capacity=None, backward=True):
     dv = lambda k: scene[k].to(DEV) if scene.get(k) is not None else None
     P = scene["means3D"].shape[0]
     W, H = cam["image_width"], cam["image_height"]
-    ntile = ((W + 15) // 16) * ((H + 15) // 16)
     cap = sgb.InstanceCapacity(initial=capacity) if capacity else None
     with torch.no_grad(), _capi.near_budget(budget):
         color, radii, depth, alpha, _, fst, tensors = R._forward_impl(dv("means3D"), dv("shs"), None, None, dv("opacities"), dv("scales"),
                                                                       dv("rotations"), None, st, None, cap)
-    out = dict(color=color, depth=depth, alpha=alpha, radii=radii)
-    img = fst.img
-    o = _align(8 * (ntile + 1))
-    out["tile_max"] = img[o:o + 4 * ntile].view(torch.int32).clone()
-    o += _align(4 * (ntile + 1))
-    out["n_contrib"] = img[o:o + 4 * W * H].view(torch.int32).clone()
-    out["status"] = fst.geom[_align(48 * P) + 7 * _align(4 * P):][:64].view(torch.int32).cpu()  # 16 status words
+    v = R.state_views(st, fst, P)
+    out = dict(color=color, depth=depth, alpha=alpha, radii=radii, tile_max=v["tile_max_contrib"].clone(), n_contrib=v["n_contrib"].clone(),
+               status=v["status"].cpu())
     if backward:
         gen = torch.Generator().manual_seed(7)
         g = lambda c: (torch.randn(c, H, W, generator=gen) / (H * W)).to(DEV)
@@ -102,14 +93,14 @@ def config_c():
 def test_config_C(config_c):
     full = render(config_c, ALL)
     noise = float((render(config_c, ALL)["grad2d"] - full["grad2d"]).abs().max())
-    Rn = int(full["status"][1])
-    assert int(full["status"][3]) == Rn
+    Rn = int(full["status"][STATUS_INSTANCES])
+    assert int(full["status"][STATUS_EMITTED]) == Rn
     for b in (AUTO, 0, Rn // 64, Rn // 4, Rn - 1):
         got = render(config_c, b)
         assert_same(full, got, noise, f"B={b}")
-        assert int(got["status"][1]) == Rn
+        assert int(got["status"][STATUS_INSTANCES]) == Rn
     auto = render(config_c, AUTO, backward=False)
-    assert int(auto["status"][3]) < Rn // 2  # most instances lie behind saturated pixels
+    assert int(auto["status"][STATUS_EMITTED]) < Rn // 2  # most instances lie behind saturated pixels
 
 
 def test_no_tile_saturates():
@@ -119,21 +110,21 @@ def test_no_tile_saturates():
     sc = scene_of(cam, splats(cam, torch.rand(n, generator=gen) * 640, torch.rand(n, generator=gen) * 480, 3 + 30 * torch.rand(n, generator=gen),
                               2 + 6 * torch.rand(n, generator=gen), 0.05))
     full = render(sc, ALL)
-    for b in (AUTO, 0, 1, int(full["status"][1]) // 3):
+    for b in (AUTO, 0, 1, int(full["status"][STATUS_INSTANCES]) // 3):
         got = render(sc, b)
         assert_same(full, got, what=f"B={b}")
-        assert int(got["status"][3]) == int(full["status"][1])  # nothing saturates, so every instance is emitted
+        assert int(got["status"][STATUS_EMITTED]) == int(full["status"][STATUS_INSTANCES])  # nothing saturates, so every instance is emitted
 
 
 def test_every_tile_saturates_in_the_near_slab():
     sc, walls = wall_scene(640, 480)
-    R_wall = int(render(walls, ALL, backward=False)["status"][1])
+    R_wall = int(render(walls, ALL, backward=False)["status"][STATUS_INSTANCES])
     full = render(sc, ALL)
-    assert int(full["status"][1]) > R_wall
+    assert int(full["status"][STATUS_INSTANCES]) > R_wall
     got = render(sc, R_wall)
     assert_same(full, got, what="B = the walls' instances")
     st = got["status"]
-    assert int(st[NEAR_END]) == R_wall and int(st[3]) == R_wall  # the far pass found no unsaturated tile
+    assert int(st[STATUS_NEAR_END]) == R_wall and int(st[STATUS_EMITTED]) == R_wall  # the far pass found no unsaturated tile
     for b in (AUTO, 0, R_wall // 2, R_wall + 1):
         assert_same(full, render(sc, b), what=f"B={b}")
 
@@ -145,14 +136,14 @@ def test_every_split_of_a_stack():
     n = 10
     sc = scene_of(cam, splats(cam, torch.full((n,), 31.5), torch.full((n,), 23.5), 1.0 + torch.arange(n), 400.0, 0.8))
     full = render(sc, ALL)
-    Rn = int(full["status"][1])
+    Rn = int(full["status"][STATUS_INSTANCES])
     assert Rn == n * 12
     saturated_in_near = 0
     for b in range(Rn + 1):
         got = render(sc, b)
         assert_same(full, got, what=f"B={b}")
         st = got["status"]
-        if int(st[NEAR_END]) < Rn and int(st[3]) == int(st[NEAR_END]):  # every tile saturated inside the near slab
+        if int(st[STATUS_NEAR_END]) < Rn and int(st[STATUS_EMITTED]) == int(st[STATUS_NEAR_END]):  # every tile saturated inside the near slab
             saturated_in_near += 1
     assert saturated_in_near > 0
 
@@ -160,11 +151,11 @@ def test_every_split_of_a_stack():
 def test_partial_edge_tiles():
     sc, _ = wall_scene(1000, 700, seed=3, layers=2)
     full = render(sc, ALL)
-    for b in (AUTO, 0, int(full["status"][1]) // 5):
+    for b in (AUTO, 0, int(full["status"][STATUS_INSTANCES]) // 5):
         got = render(sc, b)
         assert_same(full, got, what=f"B={b}")
         if b != 0:  # (with B = 0 nothing is blended before the far pass, so every instance is emitted)
-            assert int(got["status"][3]) < int(full["status"][1])
+            assert int(got["status"][STATUS_EMITTED]) < int(full["status"][STATUS_INSTANCES])
 
 
 def test_bounded_overflow():
@@ -172,20 +163,20 @@ def test_bounded_overflow():
     counts fit, as the one-pass binning does, whatever the budget; a capacity between the split's emission and R renders it whole."""
     sc = synthetic.make_config("B", seed=1)
     exact = render(sc, ALL, backward=False)
-    Rn = int(exact["status"][1])
-    emitted = {b: int(render(sc, b, backward=False)["status"][3]) for b in (AUTO, 0, Rn // 50)}
+    Rn = int(exact["status"][STATUS_INSTANCES])
+    emitted = {b: int(render(sc, b, backward=False)["status"][STATUS_EMITTED]) for b in (AUTO, 0, Rn // 50)}
     cap = min(emitted.values()) // 2 + 3
     full = render(sc, ALL, capacity=cap)
-    assert int(full["status"][2]) & 1 and int(full["status"][3]) <= cap
+    assert int(full["status"][STATUS_OVERFLOW]) & 1 and int(full["status"][STATUS_EMITTED]) <= cap
     for b in emitted:
         got = render(sc, b, capacity=cap)
         assert_same(full, got, what=f"B={b}")
-        assert int(got["status"][1]) == Rn and int(got["status"][2]) & 1 and int(got["status"][3]) <= int(full["status"][3])
+        assert int(got["status"][STATUS_INSTANCES]) == Rn and int(got["status"][STATUS_OVERFLOW]) & 1 and int(got["status"][STATUS_EMITTED]) <= int(full["status"][STATUS_EMITTED])
     cap = emitted[AUTO] + 1000
     assert cap < Rn
     got = render(sc, AUTO, capacity=cap, backward=False)
     assert_same(exact, got, what="capacity between E and R")
-    assert int(got["status"][2]) == 0 and int(got["status"][3]) == emitted[AUTO]
+    assert int(got["status"][STATUS_OVERFLOW]) == 0 and int(got["status"][STATUS_EMITTED]) == emitted[AUTO]
 
 
 def test_more_tiles_than_bucketing_keeps_one_pass():
@@ -193,7 +184,7 @@ def test_more_tiles_than_bucketing_keeps_one_pass():
     full = render(sc, ALL)
     got = render(sc, 0)
     assert_same(full, got, what="2064 x 2048")
-    assert int(got["status"][3]) == int(got["status"][1])
+    assert int(got["status"][STATUS_EMITTED]) == int(got["status"][STATUS_INSTANCES])
 
 
 def test_layers_keep_one_pass():

@@ -19,10 +19,6 @@ from street_gaussians_b200 import rasterizer as R  # noqa: E402
 DEV = "cuda"
 
 
-def _align(n):
-    return (n + 255) // 256 * 256
-
-
 def use(lib):
     _capi._lib = None
     _capi.LIB_PATH = os.path.abspath(lib)
@@ -43,14 +39,11 @@ def frame(scene, band, capacity):
         g2d, _ = R._backward_blend_impl(st, band, fst, tens, alp, scene["grad_color"].to(DEV), scene["grad_depth"].to(DEV),
                                         scene["grad_alpha"].to(DEV), torch.zeros(0, H, W, device=DEV))
     torch.cuda.synchronize()
-    ntile = ((W + 15) // 16) * ((H + 15) // 16)
-    n = max(P, 1)
-    status = fst.geom[_align(48 * n) + 7 * _align(4 * n):][:32].view(torch.int32).clone()
-    E = int(status[3])
-    b = _align(4 * max(fst.num_instances, 1))
-    lst = fst.binning[3 * b:3 * b + 4 * E].view(torch.int32).clone() if E else torch.zeros(0, dtype=torch.int32, device=DEV)
-    return dict(status=status[:5], ranges=fst.img[:8 * ntile].view(torch.int32).clone(), list=lst, color=col, depth=dep, alpha=alp,
-                radii=rad, grad2d=g2d), E
+    v = R.state_views(st, fst, P)
+    E = int(v["status"][_capi.STATUS_EMITTED])
+    lst = v["vals_out"][:E].clone() if E else torch.zeros(0, dtype=torch.int32, device=DEV)
+    return dict(status=v["status"][:5].clone(), ranges=v["ranges"].clone(), list=lst, color=col, depth=dep, alpha=alp, radii=rad,
+                grad2d=g2d), E
 
 
 def layered(scene):
@@ -106,7 +99,7 @@ def main():
                 note = f" (grad2d differs by float-atomic order: max rel {rel:.2e})"
                 if rel > 1e-5:
                     diff.append("grad2d")
-            print(f"{name:10s} {label:9s} E={int(a['status'][3]) if 'status' in a else '-':>9} {'OK' if not diff else 'DIFF ' + ','.join(map(str, diff))}{note}",
+            print(f"{name:10s} {label:9s} E={int(a['status'][_capi.STATUS_EMITTED]) if 'status' in a else '-':>9} {'OK' if not diff else 'DIFF ' + ','.join(map(str, diff))}{note}",
                   flush=True)
             bad += bool(diff)
         del res

@@ -109,8 +109,8 @@ def main():
             out = R._forward_impl(params["means3D"], params["shs"], None, None, params["opacities"], params["scales"], params["rotations"],
                                   None, settings, None)
         torch.cuda.synchronize()
-        st = out[5].geom[(48 * P + 255) // 256 * 256 + 7 * ((4 * P + 255) // 256 * 256):][:16].view(torch.int32).tolist()  # status words 0..3
-        return st[1], st[3]
+        st = R.state_views(settings, out[5], P)["status"].tolist()
+        return st[_capi.STATUS_INSTANCES], st[_capi.STATUS_EMITTED]
 
     R_total, E_parent = emitted("parent")
     for d in args.sweep:
