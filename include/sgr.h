@@ -760,7 +760,7 @@ typedef struct SgrDensifySegment {
 	int32_t semantic_width;  /* floats per row of _semantic      (0 -> param NULL)              */
 	int32_t grad_col;        /* column of xyz_gradient_accum: 0, or 1 with densify_grad_abs      */
 	int32_t prune_big;
-	int32_t reserved;
+	int32_t moments;         /* bit a: tensor a carries Adam moments in the rebalance row format (read by sgr_rebalance_* only) */
 	float *param[SGR_DENSIFY_TENSORS];       /* device, rows of width 3, dc, rest, 1, 3, 4, semantic */
 	float *exp_avg[SGR_DENSIFY_TENSORS];     /* NULL (both moments) when the tensor has no optimizer state */
 	float *exp_avg_sq[SGR_DENSIFY_TENSORS];
@@ -789,6 +789,43 @@ int sgr_densify_apply(const SgrDensifySegment *segments, const SgrDensifyOutput 
 /* GaussianModel.reset_opacity (lib/models/gaussian_model.py:410-414) in place: _opacity = inverse_sigmoid(min(sigmoid(_opacity), 0.01))
  * and the opacity tensor's exp_avg / exp_avg_sq (when non-NULL) zeroed.  Reads count, param[3], exp_avg[3], exp_avg_sq[3] only. */
 int sgr_reset_opacity(const SgrDensifySegment *segments, int32_t num_segments, void *stream);
+
+/* ---- Rebalancing Gaussian ownership across ranks (Gaussian-sharded training; no reference counterpart) ----
+ * Moves row ranges of every sub-model between ranks together with their Adam moments and densification statistics.  The row
+ * format of a segment's tensors, in this order:
+ *   param[0..6] (widths 3, dc, rest, 1, 3, 4, semantic; a zero width is skipped), exp_avg[0..6] then exp_avg_sq[0..6] of the
+ *   tensors whose bit is set in `moments`, then max_radii2D (1), xyz_gradient_accum (2), denom (1);
+ * one range's block holds its `rows` rows tensor after tensor (each tensor's rows contiguous, so every copy is one flat span), i.e.
+ * rows x sgr_rebalance_row_floats(segment) floats.  A buffer holds the blocks of the ranges that name it, in table order, from
+ * float 0.  Segments: SgrDensifySegment with count, the widths, `moments` and, for count > 0, the pointers of every tensor carried
+ * (exp_avg[a] / exp_avg_sq[a] non-NULL exactly where bit a of `moments` is set); kind and the thresholds are not read.  Ranges,
+ * segments, buffers and buffer_floats are HOST arrays; the buffers and tensors are device memory.  Each call is ONE kernel that
+ * copies every span (none when no range has rows), after one host-to-device copy of its span table into `scratch`.  Traffic: 2 x 4 B
+ * per float moved (a read and a write). */
+typedef struct SgrRebalanceRange {
+	int32_t segment;   /* index into the segment table                                                        */
+	int32_t buffer;    /* index into the buffer table; sgr_rebalance_splice only: -1 = the segment's old tensors */
+	int32_t src_row;   /* first row read from the segment's old tensors (pack, and splice with buffer -1)      */
+	int32_t dst_row;   /* first row written into the new tensors (splice; not read by pack)                    */
+	int32_t rows;
+	int32_t reserved;
+} SgrRebalanceRange;
+/* Floats per row of `segment` in a buffer; -1 (and sgr_last_error) for bad widths or moment bits. */
+int64_t sgr_rebalance_row_floats(const SgrDensifySegment *segment);
+/* Device scratch for the span table of a call with num_ranges ranges. */
+size_t sgr_rebalance_scratch_bytes(int32_t num_ranges);
+/* Copy rows [src_row, src_row + rows) of every tensor of ranges[i].segment into the block of range i in buffers[ranges[i].buffer].
+ * Every range must lie inside its segment's rows and every buffer must hold its blocks (buffer_floats[b] floats). */
+int sgr_rebalance_pack(const SgrDensifySegment *segments, int32_t num_segments, const SgrRebalanceRange *ranges, int32_t num_ranges,
+                       float *const *buffers, const int64_t *buffer_floats, int32_t num_buffers, void *scratch, size_t scratch_bytes,
+                       void *stream);
+/* Write the new tensors outputs[k] (count = the segment's new row count; pointers as sgr_densify_apply's outputs, with moments
+ * exactly where bit a of segments[k].moments is set): range i fills new rows [dst_row, dst_row + rows) of its segment from its block
+ * in buffers[buffer], or with buffer -1 from the segment's old rows [src_row, src_row + rows).  The ranges of each segment must cover
+ * its new rows exactly once.  The caller orders them [received from lower ranks | kept | received from higher ranks]. */
+int sgr_rebalance_splice(const SgrDensifySegment *segments, const SgrDensifyOutput *outputs, int32_t num_segments, const SgrRebalanceRange *ranges,
+                         int32_t num_ranges, const float *const *buffers, const int64_t *buffer_floats, int32_t num_buffers, void *scratch,
+                         size_t scratch_bytes, void *stream);
 
 /* ---- Visibility-masked ("sparse") Adam: an OPT-IN deviation from the reference (no counterpart there) ----
  * One Adam step that updates only the rows of the Gaussians this frame rendered.  Segments are the sub-models in composition order

@@ -23,7 +23,8 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_set_nea
            "sgr_sharded_forward_features", "sgr_sharded_backward_features",
            "sgr_compose_forward", "sgr_compose_backward", "sgr_image_loss_scratch_bytes", "sgr_image_loss", "sgr_sky_loss",
            "sgr_obj_acc_loss", "sgr_lidar_depth_loss_scratch_bytes", "sgr_lidar_depth_loss", "sgr_densify_stats", "sgr_adam_step",
-           "sgr_densify_scratch_bytes", "sgr_densify_plan", "sgr_densify_apply", "sgr_reset_opacity", "sgr_sparse_adam_step",
+           "sgr_densify_scratch_bytes", "sgr_densify_plan", "sgr_densify_apply", "sgr_reset_opacity", "sgr_rebalance_row_floats",
+           "sgr_rebalance_scratch_bytes", "sgr_rebalance_pack", "sgr_rebalance_splice", "sgr_sparse_adam_step",
            "sgr_layer_state_sizes", "sgr_forward_layer", "sgr_backward_blend_layer", "sgr_backward_geom_layered",
            "sgr_compose_forward_corrected", "sgr_compose_backward_corrected", "sgr_color_correct_forward", "sgr_color_correct_scratch_bytes",
            "sgr_color_correct_backward", "sgr_color_correction_reg", "sgr_sky_composite_forward", "sgr_sky_composite_backward",
@@ -105,7 +106,7 @@ DENSIFY_BACKGROUND, DENSIFY_ACTOR = 0, 1
 
 class SgrDensifySegment(C.Structure):
     _fields_ = [("kind", C.c_int32), ("count", C.c_int32), ("dc_width", C.c_int32), ("rest_width", C.c_int32), ("semantic_width", C.c_int32),
-                ("grad_col", C.c_int32), ("prune_big", C.c_int32), ("reserved", C.c_int32), ("param", C.c_void_p * DENSIFY_TENSORS),
+                ("grad_col", C.c_int32), ("prune_big", C.c_int32), ("moments", C.c_int32), ("param", C.c_void_p * DENSIFY_TENSORS),
                 ("exp_avg", C.c_void_p * DENSIFY_TENSORS), ("exp_avg_sq", C.c_void_p * DENSIFY_TENSORS), ("max_radii2D", C.c_void_p),
                 ("xyz_gradient_accum", C.c_void_p), ("denom", C.c_void_p), ("grad_threshold", C.c_float), ("dense_threshold", C.c_float),
                 ("big_threshold", C.c_float), ("min_opacity", C.c_float), ("sphere_center", C.c_float * 3), ("sphere_diameter", C.c_float),
@@ -115,6 +116,11 @@ class SgrDensifySegment(C.Structure):
 class SgrDensifyOutput(C.Structure):
     _fields_ = [("count", C.c_int32), ("reserved", C.c_int32), ("param", C.c_void_p * DENSIFY_TENSORS), ("exp_avg", C.c_void_p * DENSIFY_TENSORS),
                 ("exp_avg_sq", C.c_void_p * DENSIFY_TENSORS), ("max_radii2D", C.c_void_p), ("xyz_gradient_accum", C.c_void_p), ("denom", C.c_void_p)]
+
+
+class SgrRebalanceRange(C.Structure):
+    _fields_ = [("segment", C.c_int32), ("buffer", C.c_int32), ("src_row", C.c_int32), ("dst_row", C.c_int32), ("rows", C.c_int32),
+                ("reserved", C.c_int32)]
 
 
 SPARSE_ADAM_MAX_WIDTH = 8388607   # floats per row
@@ -328,6 +334,15 @@ def lib():
     L.sgr_densify_apply.argtypes = [C.POINTER(SgrDensifySegment), C.POINTER(SgrDensifyOutput), C.c_int32, C.c_uint64, vp, vp, C.c_size_t, vp]
     L.sgr_reset_opacity.restype = C.c_int
     L.sgr_reset_opacity.argtypes = [C.POINTER(SgrDensifySegment), C.c_int32, vp]
+    L.sgr_rebalance_row_floats.restype = C.c_int64
+    L.sgr_rebalance_row_floats.argtypes = [C.POINTER(SgrDensifySegment)]
+    L.sgr_rebalance_scratch_bytes.restype = C.c_size_t
+    L.sgr_rebalance_scratch_bytes.argtypes = [C.c_int32]
+    rebalance_tables = [C.POINTER(SgrRebalanceRange), C.c_int32, C.POINTER(vp), C.POINTER(C.c_int64), C.c_int32, vp, C.c_size_t, vp]
+    L.sgr_rebalance_pack.restype = C.c_int
+    L.sgr_rebalance_pack.argtypes = [C.POINTER(SgrDensifySegment), C.c_int32] + rebalance_tables
+    L.sgr_rebalance_splice.restype = C.c_int
+    L.sgr_rebalance_splice.argtypes = [C.POINTER(SgrDensifySegment), C.POINTER(SgrDensifyOutput), C.c_int32] + rebalance_tables
     L.sgr_sparse_adam_step.restype = C.c_int
     L.sgr_sparse_adam_step.argtypes = [C.POINTER(SgrSparseAdamSegment), C.c_int32, vp, C.c_double, C.c_double, C.c_double, vp]
     L.sgr_layer_state_sizes.restype = C.c_int

@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "libsgr.so")
-SOURCES = ["capi.cu", "preprocess_fwd.cu", "binning.cu", "blend_fwd.cu", "blend_bwd.cu", "blend_bwd2.cu", "preprocess_bwd.cu", "knn.cu", "peer_exchange.cu", "compose.cu", "corrections.cu", "losses.cu", "optim.cu", "densify.cu", "layers.cu", "sky.cu", "actor_pose.cu", "features.cu", "metrics.cu"]
+SOURCES = ["capi.cu", "preprocess_fwd.cu", "binning.cu", "blend_fwd.cu", "blend_bwd.cu", "blend_bwd2.cu", "preprocess_bwd.cu", "knn.cu", "peer_exchange.cu", "compose.cu", "corrections.cu", "losses.cu", "optim.cu", "densify.cu", "rebalance.cu", "layers.cu", "sky.cu", "actor_pose.cu", "features.cu", "metrics.cu"]
 HEADERS = ["sgr_common.cuh", "ssim_tile.cuh", "gaussian_geom.cuh", "tile_visit.cuh", os.path.join("..", "..", "include", "sgr.h")]
 # no --use_fast_math: parity with the reference needs IEEE division/sqrt and the accurate expf (DGR/setup.py:30 has none either)
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",

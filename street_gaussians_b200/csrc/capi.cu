@@ -1,5 +1,6 @@
 // capi.cu — the extern "C" surface of libsgr.so (include/sgr.h): argument validation, state carving, launch order.
 // Host-side only; every device kernel lives in its own translation unit.
+#include <algorithm>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -1684,6 +1685,189 @@ int sgr_reset_opacity(const SgrDensifySegment *segments, int32_t num_segments, v
 	const bool debug = false;
 	SGR_TRY(launch_reset_opacity(segments, num_segments, st), "reset_opacity");
 	return SGR_OK;
+}
+
+// ---- rebalancing: the row format of include/sgr.h as (pointer, floats per row) per tensor, and the span tables of pack / splice ----
+constexpr int kRebalanceTensors = 3 * SGR_DENSIFY_TENSORS + 3;
+
+static int rebalance_format_ok(const SgrDensifySegment &s, int k) {
+	if (s.count < 0 || s.dc_width <= 0 || s.rest_width < 0 || s.semantic_width < 0)
+		return fail(SGR_EINVAL, "segment %d: bad count %d or row widths dc=%d rest=%d semantic=%d", k, s.count, s.dc_width, s.rest_width,
+		            s.semantic_width);
+	for (int a = 0; a < 32; a++)
+		if (((s.moments >> a) & 1) && (a >= SGR_DENSIFY_TENSORS || densify_width(s, a) == 0))
+			return fail(SGR_EINVAL, "segment %d: moment bit %d names no tensor with a nonzero width", k, a);
+	return SGR_OK;
+}
+
+// fills ptr[] / width[] in the row format's order from the given pointer arrays; returns the number of tensors carried
+static int rebalance_tensors(const SgrDensifySegment &s, float *const *param, float *const *m, float *const *v, float *mr, float *ga, float *dn,
+                             float *ptr[kRebalanceTensors], int width[kRebalanceTensors]) {
+	int n = 0;
+	for (int a = 0; a < SGR_DENSIFY_TENSORS; a++)
+		if (densify_width(s, a) > 0) { ptr[n] = param[a]; width[n++] = densify_width(s, a); }
+	for (int j = 0; j < 2; j++)
+		for (int a = 0; a < SGR_DENSIFY_TENSORS; a++)
+			if ((s.moments >> a) & 1) { ptr[n] = (j ? v : m)[a]; width[n++] = densify_width(s, a); }
+	ptr[n] = mr; width[n++] = 1;
+	ptr[n] = ga; width[n++] = 2;
+	ptr[n] = dn; width[n++] = 1;
+	return n;
+}
+
+static int64_t rebalance_row_floats(const SgrDensifySegment &s) {
+	float *ptr[kRebalanceTensors];
+	int width[kRebalanceTensors];
+	const int n = rebalance_tensors(s, s.param, s.exp_avg, s.exp_avg_sq, s.max_radii2D, s.xyz_gradient_accum, s.denom, ptr, width);
+	int64_t f = 0;
+	for (int t = 0; t < n; t++) f += width[t];
+	return f;
+}
+
+// segments carrying rows must give every tensor of the format (and no moment the format does not carry)
+static int check_rebalance_segments(const char *fn, const SgrDensifySegment *segments, int32_t num_segments) {
+	if (!segments || num_segments <= 0) return fail(SGR_EINVAL, "%s: segment table is empty", fn);
+	for (int k = 0; k < num_segments; k++) {
+		const SgrDensifySegment &s = segments[k];
+		int rc = rebalance_format_ok(s, k);
+		if (rc) return rc;
+		if (s.count == 0) continue;
+		for (int a = 0; a < SGR_DENSIFY_TENSORS; a++) {
+			const bool has = densify_width(s, a) > 0, mom = (s.moments >> a) & 1;
+			if (has != (s.param[a] != nullptr)) return fail(SGR_EINVAL, "%s: segment %d: %s is %s", fn, k, kDensifyTensor[a], has ? "NULL" : "given for a zero row width");
+			if (mom != (s.exp_avg[a] != nullptr) || mom != (s.exp_avg_sq[a] != nullptr))
+				return fail(SGR_EINVAL, "%s: segment %d: the Adam moments of %s must be given exactly where its moment bit is set", fn, k, kDensifyTensor[a]);
+		}
+		if (!s.max_radii2D || !s.xyz_gradient_accum || !s.denom) return fail(SGR_EINVAL, "%s: segment %d has a NULL statistics array", fn, k);
+	}
+	return SGR_OK;
+}
+
+// checks the ranges against the segments and buffers and appends one span per tensor of each range with rows (pack: rows -> buffer;
+// splice: buffer or old rows -> new rows of outs[k])
+static int rebalance_spans(const char *fn, const SgrDensifySegment *segments, const SgrDensifyOutput *outs, int32_t num_segments,
+                           const SgrRebalanceRange *ranges, int32_t num_ranges, float *const *buffers, const int64_t *buffer_floats,
+                           int32_t num_buffers, std::vector<RebalanceSpan> &spans) {
+	if (num_ranges < 0 || (num_ranges > 0 && !ranges)) return fail(SGR_EINVAL, "%s: bad range table", fn);
+	if (num_buffers < 0 || (num_buffers > 0 && (!buffers || !buffer_floats))) return fail(SGR_EINVAL, "%s: bad buffer table", fn);
+	std::vector<int64_t> used(num_buffers, 0);
+	const bool splice = outs != nullptr;
+	for (int i = 0; i < num_ranges; i++) {
+		const SgrRebalanceRange &r = ranges[i];
+		if (r.segment < 0 || r.segment >= num_segments) return fail(SGR_EINVAL, "%s: range %d names segment %d of %d", fn, i, r.segment, num_segments);
+		if (r.buffer < (splice ? -1 : 0) || r.buffer >= num_buffers) return fail(SGR_EINVAL, "%s: range %d names buffer %d of %d", fn, i, r.buffer, num_buffers);
+		const SgrDensifySegment &s = segments[r.segment];
+		const bool from_old = !splice || r.buffer < 0;
+		if (r.rows < 0 || (from_old && (r.src_row < 0 || (int64_t)r.src_row + r.rows > s.count)))
+			return fail(SGR_EINVAL, "%s: range %d reads rows [%d, %lld) of segment %d, which has %d", fn, i, r.src_row, (long long)r.src_row + r.rows,
+			            r.segment, s.count);
+		if (splice && (r.dst_row < 0 || (int64_t)r.dst_row + r.rows > outs[r.segment].count))
+			return fail(SGR_EINVAL, "%s: range %d writes rows [%d, %lld) of output %d, which has %d", fn, i, r.dst_row, (long long)r.dst_row + r.rows,
+			            r.segment, outs[r.segment].count);
+		const int64_t block = (int64_t)r.rows * rebalance_row_floats(s);
+		int64_t at = 0;
+		if (r.buffer >= 0) {
+			at = used[r.buffer];
+			used[r.buffer] += block;
+			if (used[r.buffer] > buffer_floats[r.buffer])
+				return fail(SGR_ENOMEM, "%s: buffer %d holds %lld floats, its blocks need %lld or more", fn, r.buffer, (long long)buffer_floats[r.buffer],
+				            (long long)used[r.buffer]);
+			if (!buffers[r.buffer] && block > 0) return fail(SGR_EINVAL, "%s: buffer %d is NULL", fn, r.buffer);
+		}
+		if (r.rows == 0) continue;
+		float *src[kRebalanceTensors], *dst[kRebalanceTensors];
+		int width[kRebalanceTensors];
+		const int nt = rebalance_tensors(s, s.param, s.exp_avg, s.exp_avg_sq, s.max_radii2D, s.xyz_gradient_accum, s.denom, src, width);
+		if (splice) {
+			const SgrDensifyOutput &o = outs[r.segment];
+			rebalance_tensors(s, o.param, o.exp_avg, o.exp_avg_sq, o.max_radii2D, o.xyz_gradient_accum, o.denom, dst, width);
+		}
+		float *buf = r.buffer >= 0 ? buffers[r.buffer] + at : nullptr;
+		for (int t = 0; t < nt; t++) {
+			const int64_t n = (int64_t)r.rows * width[t];
+			float *old_rows = from_old ? src[t] + (int64_t)r.src_row * width[t] : nullptr;
+			if (!splice) spans.push_back(RebalanceSpan{old_rows, buf, n});
+			else spans.push_back(RebalanceSpan{from_old ? old_rows : buf, dst[t] + (int64_t)r.dst_row * width[t], n});
+			if (buf) buf += n;
+		}
+	}
+	return SGR_OK;
+}
+
+int64_t sgr_rebalance_row_floats(const SgrDensifySegment *segment) {
+	if (!segment) {
+		fail(SGR_EINVAL, "segment is NULL");
+		return -1;
+	}
+	if (rebalance_format_ok(*segment, 0)) return -1;
+	return rebalance_row_floats(*segment);
+}
+
+size_t sgr_rebalance_scratch_bytes(int32_t num_ranges) {
+	return num_ranges >= 0 ? rebalance_scratch_bytes((long long)num_ranges * kRebalanceTensors) : 0;
+}
+
+static int rebalance_copy(const char *fn, const std::vector<RebalanceSpan> &spans, int32_t num_ranges, void *scratch, size_t scratch_bytes,
+                          void *stream) {
+	const size_t need = rebalance_scratch_bytes((long long)num_ranges * kRebalanceTensors);
+	if (!spans.empty() && (!scratch || scratch_bytes < need)) return fail(SGR_ENOMEM, "%s: scratch too small: %zu < %zu", fn, scratch_bytes, need);
+	if (rebalance_blocks(spans.data(), (int)spans.size()) > 0x7fffffffLL) return fail(SGR_EUNSUPPORTED, "%s: more than 2^31-1 blocks of floats to copy", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_rebalance_copy(spans.data(), (int)spans.size(), scratch, st), fn);
+	return SGR_OK;
+}
+
+int sgr_rebalance_pack(const SgrDensifySegment *segments, int32_t num_segments, const SgrRebalanceRange *ranges, int32_t num_ranges,
+                       float *const *buffers, const int64_t *buffer_floats, int32_t num_buffers, void *scratch, size_t scratch_bytes,
+                       void *stream) {
+	const char *fn = "sgr_rebalance_pack";
+	int rc = check_rebalance_segments(fn, segments, num_segments);
+	if (rc) return rc;
+	std::vector<RebalanceSpan> spans;
+	if ((rc = rebalance_spans(fn, segments, nullptr, num_segments, ranges, num_ranges, buffers, buffer_floats, num_buffers, spans))) return rc;
+	return rebalance_copy(fn, spans, num_ranges, scratch, scratch_bytes, stream);
+}
+
+int sgr_rebalance_splice(const SgrDensifySegment *segments, const SgrDensifyOutput *outputs, int32_t num_segments, const SgrRebalanceRange *ranges,
+                         int32_t num_ranges, const float *const *buffers, const int64_t *buffer_floats, int32_t num_buffers, void *scratch,
+                         size_t scratch_bytes, void *stream) {
+	const char *fn = "sgr_rebalance_splice";
+	int rc = check_rebalance_segments(fn, segments, num_segments);
+	if (rc) return rc;
+	if (!outputs) return fail(SGR_EINVAL, "%s: output table is NULL", fn);
+	for (int k = 0; k < num_segments; k++) {
+		const SgrDensifySegment &s = segments[k];
+		const SgrDensifyOutput &o = outputs[k];
+		if (o.count < 0) return fail(SGR_EINVAL, "%s: output %d: count %d", fn, k, o.count);
+		if (o.count == 0) continue;
+		for (int a = 0; a < SGR_DENSIFY_TENSORS; a++) {
+			const bool has = densify_width(s, a) > 0, mom = (s.moments >> a) & 1;
+			if (has != (o.param[a] != nullptr)) return fail(SGR_EINVAL, "%s: output %d: %s is %s", fn, k, kDensifyTensor[a], has ? "NULL" : "given for a zero row width");
+			if (mom != (o.exp_avg[a] != nullptr) || mom != (o.exp_avg_sq[a] != nullptr))
+				return fail(SGR_EINVAL, "%s: output %d: the Adam moments of %s must be given exactly where its moment bit is set", fn, k, kDensifyTensor[a]);
+		}
+		if (!o.max_radii2D || !o.xyz_gradient_accum || !o.denom) return fail(SGR_EINVAL, "%s: output %d has a NULL statistics array", fn, k);
+	}
+	std::vector<RebalanceSpan> spans;
+	if ((rc = rebalance_spans(fn, segments, outputs, num_segments, ranges, num_ranges, const_cast<float *const *>(buffers), buffer_floats, num_buffers,
+	                          spans)))
+		return rc;
+	// every new row written exactly once: per segment, the ranges sorted by dst_row must tile [0, count)
+	std::vector<std::pair<int64_t, int32_t>> cover;  // (segment << 32 | dst_row, rows)
+	for (int i = 0; i < num_ranges; i++)
+		if (ranges[i].rows > 0) cover.push_back({((int64_t)ranges[i].segment << 32) | (uint32_t)ranges[i].dst_row, ranges[i].rows});
+	std::sort(cover.begin(), cover.end());
+	size_t c = 0;
+	for (int k = 0; k < num_segments; k++) {
+		int64_t at = 0;
+		for (; c < cover.size() && (cover[c].first >> 32) == k; c++) {
+			if ((cover[c].first & 0xffffffffLL) != at) return fail(SGR_EINVAL, "%s: output %d: rows from %lld on are not written exactly once", fn, k, (long long)at);
+			at += cover[c].second;
+		}
+		if (at != outputs[k].count) return fail(SGR_EINVAL, "%s: output %d: the ranges write %lld of its %d rows", fn, k, (long long)at, outputs[k].count);
+	}
+	return rebalance_copy(fn, spans, num_ranges, scratch, scratch_bytes, stream);
 }
 
 int sgr_sparse_adam_step(const SgrSparseAdamSegment *segments, int32_t num_segments, const int32_t *radii, double beta1, double beta2,

@@ -521,6 +521,15 @@ cudaError_t launch_densify_plan(const SgrDensifySegment *segs, int nseg, unsigne
 cudaError_t launch_densify_apply(const SgrDensifySegment *segs, const SgrDensifyOutput *outs, int nseg, unsigned long long seed, const float *draws,
                                  void *scratch, cudaStream_t st);
 cudaError_t launch_reset_opacity(const SgrDensifySegment *segs, int nseg, cudaStream_t st);
+// rebalancing (rebalance.cu): one flat copy of n floats
+struct RebalanceSpan {
+	const float *src;
+	float *dst;
+	long long n;
+};
+size_t rebalance_scratch_bytes(long long nspans);
+long long rebalance_blocks(const RebalanceSpan *spans, int nspans);
+cudaError_t launch_rebalance_copy(const RebalanceSpan *spans, int nspans, void *scratch, cudaStream_t st);
 size_t knn_scratch_bytes(int P);
 cudaError_t launch_knn(int P, const float *points, float *out, void *scratch, size_t scratch_bytes, cudaStream_t st);
 

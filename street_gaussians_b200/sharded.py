@@ -24,7 +24,7 @@ fwd/bwd were about a third of the step) and the 2x91 MB all-reduce becomes a 91 
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional
+from typing import List, NamedTuple, Optional, Sequence
 
 import torch
 import torch.distributed as dist
@@ -32,6 +32,7 @@ import torch.nn as nn
 
 from . import _capi
 from ._capi import ptr
+from .training import PARAM_NAMES, _attr, _install, _param_slots, _segment, _stat_segment
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, InstanceCapacity, TileRowBand, _copy_status, _ForwardState,
                          _backward_blend_impl, _backward_geom_impl, _fit_grads, _fp32_inputs, _geom_grad_buffers, _image_grads,
                          _input_shapes, _make_frame, _reference_inputs)
@@ -581,9 +582,10 @@ class GaussianShardedRasterizer(nn.Module):
         self.band = mk(raster_settings.image_height, self.rank, self.world) if self.world > 1 else None
         self.chunk = int(chunk) if chunk else None
 
-    def repartition(self, P_local: int) -> int:
-        """COLLECTIVE: agree on the per-rank slot count after the local Gaussian count changed (densify / prune)."""
-        self.chunk = chunk_size(P_local, self.group)
+    def repartition(self, P_local: int, chunk: Optional[int] = None) -> int:
+        """COLLECTIVE: agree on the per-rank slot count after the local Gaussian count changed (densify / prune).  A caller that
+        already knows every rank's count (rebalance) passes their maximum as `chunk`, and then no collective is taken."""
+        self.chunk = int(chunk) if chunk is not None else chunk_size(P_local, self.group)
         return self.chunk
 
     def workspace(self, device, S: int = 0) -> "PeerWorkspace":
@@ -620,3 +622,209 @@ class GaussianShardedRasterizer(nn.Module):
         args = (means3D, means2D, shs, colors_precomp, semantics, opacities, scales, rotations, cov3D_precomp)
         differentiable = torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in args)
         return _GaussianShardedRasterize.apply(*args, self.raster_settings, self, differentiable)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Rebalancing Gaussian ownership after densification (DESIGN.md §8)
+# ---------------------------------------------------------------------------------------------------------------------
+class RebalanceMove(NamedTuple):
+    """Rows [src_row_begin, src_row_end) of sub-model `model` on rank `src` become rows [dst_row_begin, ...) of that sub-model on
+    rank `dst`.  In RebalancePlan.kept, src == dst: the rows a rank keeps, and where they land in its new tensors."""
+    src: int
+    dst: int
+    model: int
+    src_row_begin: int
+    src_row_end: int
+    dst_row_begin: int
+
+
+class RebalancePlan(NamedTuple):
+    moves: List[RebalanceMove]  # by model, then source rank, then destination rank
+    kept: List[RebalanceMove]
+    counts: List[List[int]]     # the new counts[world][n_models]
+
+
+def rebalance_plan(counts: Sequence[Sequence[int]]) -> RebalancePlan:
+    """Host-only plan of rebalance(): counts[r][m] rows of sub-model m on rank r (composition order), split as GaussianShardedRasterizer
+    requires: the rank-major concatenation of the ranks' rows is the model-major global array.  Rank r ends up owning the global rows
+    [B_r, B_{r+1}), B the even split (the first P_total % world ranks get one row more), and every row keeps its global position; a
+    row moves only when its new owner is another rank, possibly past its neighbours."""
+    counts = [[int(c) for c in row] for row in counts]
+    world = len(counts)
+    if world == 0:
+        raise ValueError("counts: no ranks")
+    nm = len(counts[0])
+    if any(len(row) != nm for row in counts) or any(c < 0 for row in counts for c in row):
+        raise ValueError(f"counts must be [world][n_models] non-negative integers, got {counts}")
+    last = -1  # highest model a lower rank holds rows of: no later rank may hold rows of a model before it
+    for r, row in enumerate(counts):
+        held = [m for m, c in enumerate(row) if c]
+        if held and held[0] < last:
+            raise ValueError(f"rank {r} holds rows of model {held[0]} but a lower rank holds rows of model {last}: the ranks' rows are not "
+                             "the rank-major split of the model-major global array")
+        last = held[-1] if held else last
+    base, extra = divmod(sum(map(sum, counts)), world)
+    B = [r * base + min(r, extra) for r in range(world + 1)]
+    new = [[0] * nm for _ in range(world)]
+    moves, kept = [], []
+    g0 = 0
+    for m in range(nm):
+        g1 = g0 + sum(row[m] for row in counts)
+        nb = [max(B[d], g0) for d in range(world)]  # model m's new global range on rank d
+        ne = [min(B[d + 1], g1) for d in range(world)]
+        for d in range(world):
+            new[d][m] = max(0, ne[d] - nb[d])
+        a = g0
+        for s in range(world):
+            b = a + counts[s][m]
+            for d in range(world):
+                lo, hi = max(a, nb[d]), min(b, ne[d])
+                if lo < hi:
+                    (kept if d == s else moves).append(RebalanceMove(s, d, m, lo - a, hi - a, lo - nb[d]))
+            a = b
+        g0 = g1
+    return RebalancePlan(moves, kept, new)
+
+
+class ProcessGroupTransport:
+    """rebalance()'s two exchanges over torch.distributed (NCCL or gloo): an all_gather of a small int64 table and the packed row
+    buffers.  Tests substitute an object with the same four members that exchanges between emulated ranks."""
+
+    def __init__(self, group=None):
+        self.group = group
+        self.world = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
+        self.rank = dist.get_rank(group) if self.world > 1 else 0
+
+    def all_gather(self, t: torch.Tensor) -> List[torch.Tensor]:
+        """Every rank's `t` (a CPU tensor), as CPU tensors in rank order."""
+        if self.world == 1:
+            return [t]
+        dev = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend(self.group) == "nccl" else torch.device("cpu")
+        out = [torch.empty_like(t, device=dev) for _ in range(self.world)]
+        dist.all_gather(out, t.to(dev), group=self.group)
+        return list(torch.stack(out).cpu())
+
+    def exchange(self, sends: dict, recvs: dict) -> None:
+        """sends[dst] goes to rank dst and recvs[src] is filled from rank src, one batch_isend_irecv for all pairs."""
+        peer = (lambda r: r) if self.group is None else (lambda r: dist.get_global_rank(self.group, r))
+        ops = [dist.P2POp(dist.isend, b, peer(d), self.group) for d, b in sends.items()]
+        ops += [dist.P2POp(dist.irecv, b, peer(s), self.group) for s, b in recvs.items()]
+        if ops:
+            for req in dist.batch_isend_irecv(ops):
+                req.wait()
+
+
+def _rebalance_tables(L, ranges, buffers, dev):
+    rt = (_capi.SgrRebalanceRange * max(1, len(ranges)))()
+    for i, (seg, buf, src_row, dst_row, rows) in enumerate(ranges):
+        rt[i].segment, rt[i].buffer, rt[i].src_row, rt[i].dst_row, rt[i].rows = seg, buf, src_row, dst_row, rows
+    nb = len(buffers)
+    bp = (C.c_void_p * max(1, nb))(*[b.data_ptr() for b in buffers])
+    bf = (C.c_int64 * max(1, nb))(*[b.numel() for b in buffers])
+    scratch = torch.empty((int(L.sgr_rebalance_scratch_bytes(len(ranges))),), dtype=torch.uint8, device=dev)
+    return (rt, len(ranges), bp, bf, nb, ptr(scratch), scratch.numel()), scratch
+
+
+def rebalance(models: Sequence, optimizer=None, group: Optional[dist.ProcessGroup] = None, rasterizer: Optional["GaussianShardedRasterizer"] = None,
+              transport=None) -> int:
+    """COLLECTIVE: even out the ranks' Gaussian counts after densify_and_prune, moving rows between ranks together with their Adam
+    moments and densification statistics.  Returns the new local Gaussian count.
+
+    models: this rank's sub-models in composition order (background, then actors; the attributes densify_and_prune reads: the seven
+      parameters and max_radii2D, xyz_gradient_accum, denom), the same list on every rank; a sub-model may have 0 local rows.  The
+      ranks' rows must form the split GaussianShardedRasterizer documents (rebalance_plan).  Afterwards rank r owns the global rows
+      [B_r, B_{r+1}) of the even split and every row keeps its global position, so the Gaussian-sharded render is the same.
+    optimizer: one optimizer or a list (as for densify_and_prune).  Parameters are replaced by new nn.Parameters in their groups, found
+      by identity, and their state moves to the new key with the moments of the rows they now hold; step is unchanged and must be equal
+      on every rank (ValueError otherwise, on every rank).
+    rasterizer: its repartition() is called with the new counts' maximum (no further collective).
+    transport: see ProcessGroupTransport; default ProcessGroupTransport(group).
+
+    Communication: one all_gather of a [n_models, 11] int64 table (counts, row widths, Adam steps), the only host read, and, when some
+    row moves, one batch_isend_irecv of one packed buffer per (source, destination) pair.  The rows are packed by one
+    sgr_rebalance_pack launch and the new tensors written by one sgr_rebalance_splice launch; when no row moves (world 1, or ranks
+    already balanced) nothing is launched."""
+    tr = transport if transport is not None else ProcessGroupTransport(group)
+    world, rank = int(tr.world), int(tr.rank)
+    models = list(models)
+    nm = len(models)
+    if nm == 0:
+        raise ValueError("rebalance needs the sub-models (background, then actors)")
+    L = _capi.lib()
+    dev = _attr(models[0], "_xyz").device
+    slots = _param_slots(optimizer)
+    segs = (_capi.SgrDensifySegment * nm)()
+    infos = []
+    meta = torch.full((nm, 4 + _capi.DENSIFY_TENSORS), -1, dtype=torch.int64)
+    for k, m in enumerate(models):
+        seg, params, moments, widths = _segment(m, k, optimizer, slots, dev)
+        _stat_segment(seg, m, k, dev)
+        meta[k, :4] = torch.tensor([seg.count, seg.dc_width, seg.rest_width, seg.semantic_width])
+        for a, p in enumerate(params):
+            if moments[a] is not None:
+                opt = slots[id(p)][0]
+                meta[k, 4 + a] = int(opt.state[p]["step"])
+                if widths[a]:
+                    seg.moments |= 1 << a
+        segs[k] = seg
+        infos.append((params, moments))
+    table = torch.stack(tr.all_gather(meta)).tolist()  # [world][nm][11]
+    for k in range(nm):
+        for r in range(world):
+            if table[r][k][1:4] != table[0][k][1:4]:
+                raise ValueError(f"model {k}: rows of {table[0][k][1:4]} (dc, rest, semantic floats) on rank 0, {table[r][k][1:4]} on rank {r}")
+            for a in range(_capi.DENSIFY_TENSORS):
+                if table[r][k][4 + a] != table[0][k][4 + a]:
+                    st = lambda v: "no Adam state" if v < 0 else f"Adam step {v}"
+                    raise ValueError(f"model {k}: {PARAM_NAMES[a]} has {st(table[0][k][4 + a])} on rank 0 and {st(table[r][k][4 + a])} on rank {r}; "
+                                     "rebalance needs the same optimizer state on every rank")
+    plan = rebalance_plan([[row[0] for row in table[r]] for r in range(world)])
+    P_new = sum(plan.counts[rank])
+    if rasterizer is not None:
+        rasterizer.repartition(P_new, chunk=max(sum(c) for c in plan.counts))
+    if not plan.moves:
+        return P_new
+    rf = [int(L.sgr_rebalance_row_floats(C.byref(segs[k]))) for k in range(nm)]
+    # pack: one buffer per destination, its blocks in plan order (the receiver lists them in the same order)
+    sends = [mv for mv in plan.moves if mv.src == rank]
+    recvs = [mv for mv in plan.moves if mv.dst == rank]
+    dsts = sorted({mv.dst for mv in sends})
+    srcs = sorted({mv.src for mv in recvs})
+    floats = lambda mvs, peer, side: sum((mv.src_row_end - mv.src_row_begin) * rf[mv.model] for mv in mvs if getattr(mv, side) == peer)
+    send_bufs = [torch.empty((floats(sends, d, "dst"),), dtype=torch.float32, device=dev) for d in dsts]
+    recv_bufs = [torch.empty((floats(recvs, s, "src"),), dtype=torch.float32, device=dev) for s in srcs]
+    if sends:
+        args, scratch = _rebalance_tables(L, [(mv.model, dsts.index(mv.dst), mv.src_row_begin, 0, mv.src_row_end - mv.src_row_begin)
+                                              for mv in sends], send_bufs, dev)
+        _capi.call("sgr_rebalance_pack", dev, segs, nm, *args)
+    tr.exchange(dict(zip(dsts, send_bufs)), dict(zip(srcs, recv_bufs)))
+    # splice: per model [received from lower ranks | kept | received from higher ranks]
+    ranges = [(mv.model, srcs.index(mv.src), 0, mv.dst_row_begin, mv.src_row_end - mv.src_row_begin) for mv in recvs]
+    ranges += [(mv.model, -1, mv.src_row_begin, mv.dst_row_begin, mv.src_row_end - mv.src_row_begin) for mv in plan.kept if mv.src == rank]
+    ranges.sort(key=lambda t: (t[0], t[3]))
+    outs = (_capi.SgrDensifyOutput * nm)()
+    new = []
+    for k, (params, moments) in enumerate(infos):
+        n_new = plan.counts[rank][k]
+        o = outs[k]
+        o.count = n_new
+        nps, nmom = [], []
+        for a, p in enumerate(params):
+            t = torch.empty((n_new,) + tuple(p.shape[1:]), dtype=torch.float32, device=dev)
+            mv = None if moments[a] is None else (torch.empty_like(t), torch.empty_like(t))
+            if n_new and t.numel():
+                o.param[a] = t.data_ptr()
+                if mv is not None:
+                    o.exp_avg[a], o.exp_avg_sq[a] = mv[0].data_ptr(), mv[1].data_ptr()
+            nps.append(t)
+            nmom.append(mv)
+        stats = (torch.empty(n_new, device=dev), torch.empty(n_new, 2, device=dev), torch.empty(n_new, 1, device=dev))
+        if n_new:
+            o.max_radii2D, o.xyz_gradient_accum, o.denom = (t.data_ptr() for t in stats)
+        new.append((nps, nmom, stats))
+    if ranges:
+        args, scratch = _rebalance_tables(L, ranges, recv_bufs, dev)
+        _capi.call("sgr_rebalance_splice", dev, segs, outs, nm, *args)
+    for k, m in enumerate(models):
+        _install(m, infos[k][0], *new[k], slots)
+    return P_new

@@ -107,6 +107,7 @@ class FusedAdam(torch.optim.Optimizer):
 
 # ---- densification ----
 PARAM_NAMES = ("_xyz", "_features_dc", "_features_rest", "_opacity", "_scaling", "_rotation", "_semantic")
+STAT_NAMES = ("max_radii2D", "xyz_gradient_accum", "denom")
 SCALAR_NAMES = ("points_total", "points_clone", "points_split", "points_below_min_opacity", "points_big_ws", "points_pruned")
 
 
@@ -192,6 +193,37 @@ def _segment(model, k, optimizer, slots, dev):
     return seg, params, moments, widths
 
 
+def _stat_segment(seg, model, k, dev):
+    """Check the model's densification statistics against seg.count rows and point the segment at them."""
+    n = seg.count
+    stats = [_attr(model, s) for s in STAT_NAMES]
+    for t, w in zip(stats, (1, 2, 1)):
+        _check_tensor(t, dev, f"model {k}: densification statistics")
+        if t.numel() != w * n:
+            raise ValueError(f"model {k}: max_radii2D must be [{n}], xyz_gradient_accum [{n}, 2] and denom [{n}, 1]")
+    if n:
+        seg.max_radii2D, seg.xyz_gradient_accum, seg.denom = (t.data_ptr() for t in stats)
+
+
+def _install(model, params, new_params, new_moments, new_stats, slots):
+    """Replace the model's parameters `params` by new nn.Parameters over `new_params` (same requires_grad), in their optimizer groups
+    too (found by identity): each optimizer state moves to the new key with its step unchanged and the new moments (None: the state
+    is kept as it is).  The statistics become `new_stats`."""
+    for a, (old, t) in enumerate(zip(params, new_params)):
+        p = torch.nn.Parameter(t, requires_grad=old.requires_grad)
+        if id(old) in slots:
+            opt, g, j = slots[id(old)]
+            g["params"][j] = p
+            st = opt.state.pop(old, None)
+            if st is not None:
+                if new_moments[a] is not None:
+                    st["exp_avg"], st["exp_avg_sq"] = new_moments[a]
+                opt.state[p] = st
+        _set(model, PARAM_NAMES[a], p)
+    for name, t in zip(STAT_NAMES, new_stats):
+        _set(model, name, t)
+
+
 def _densify(models, max_grad, min_opacity, prune_big_points, optimizer=None, grad_abs=False, seed=None, noise=None, keep_masks=False):
     L = _capi.lib()
     models = list(models)
@@ -205,14 +237,7 @@ def _densify(models, max_grad, min_opacity, prune_big_points, optimizer=None, gr
     infos = []
     for k, m in enumerate(models):
         seg, params, moments, widths = _segment(m, k, optimizer, slots, dev)
-        n = seg.count
-        stats = [_attr(m, s) for s in ("max_radii2D", "xyz_gradient_accum", "denom")]
-        for t, w in zip(stats, (1, 2, 1)):
-            _check_tensor(t, dev, f"model {k}: densification statistics")
-            if t.numel() != w * n:
-                raise ValueError(f"model {k}: max_radii2D must be [{n}], xyz_gradient_accum [{n}, 2] and denom [{n}, 1]")
-        if n:
-            seg.max_radii2D, seg.xyz_gradient_accum, seg.denom = (t.data_ptr() for t in stats)
+        _stat_segment(seg, m, k, dev)
         if _has(m, "scene_radius"):       # GaussianModelBkgd (gaussian_model_bkgd.py:21-23, 86-98)
             seg.kind, extent = _capi.DENSIFY_BACKGROUND, _attr(m, "scene_radius")
             c = torch.as_tensor(_attr(m, "sphere_center"), dtype=torch.float32).detach().cpu().reshape(-1)
@@ -272,21 +297,7 @@ def _densify(models, max_grad, min_opacity, prune_big_points, optimizer=None, gr
     _capi.call("sgr_densify_apply", dev, segs, outs, nm, C.c_uint64(seed), npp, scratch.data_ptr(), nbytes)
     scalars = []
     for k, m in enumerate(models):
-        params, moments, _ = infos[k]
-        np_, nmom, stats = new[k]
-        for a, (old, t) in enumerate(zip(params, np_)):
-            p = torch.nn.Parameter(t, requires_grad=old.requires_grad)
-            if id(old) in slots:
-                opt, g, j = slots[id(old)]
-                g["params"][j] = p
-                st = opt.state.pop(old, None)
-                if st is not None:
-                    if nmom[a] is not None:
-                        st["exp_avg"], st["exp_avg_sq"] = nmom[a]
-                    opt.state[p] = st
-            _set(m, PARAM_NAMES[a], p)
-        for name, t in zip(("max_radii2D", "xyz_gradient_accum", "denom"), stats):
-            _set(m, name, t)
+        _install(m, infos[k][0], *new[k], slots)
         r = result[k * _capi.DENSIFY_RESULT:(k + 1) * _capi.DENSIFY_RESULT]
         d = dict(zip(SCALAR_NAMES, (int(v) for v in r[1:7])))
         if not prune_big_points:

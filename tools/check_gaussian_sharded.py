@@ -17,6 +17,9 @@ the sky composite and colour correction with band= / group= (their parameter gra
 (finish_features(band=)) on an S = 3 + 4 render (normals and semantics).  None of these legs has been run on several H100s yet; the
 single-GPU emulations of tests/test_band_losses_gpu.py, tests/test_band_image_gpu.py and tests/test_band_features_gpu.py cover their
 kernels.
+
+With the argument `rebalance` only the rebalance leg runs (run_rebalance): sharded.rebalance over NCCL on an uneven split, against the
+global arrays each rank restates.  It has run at world 1 only, not on several H100s; tests/test_rebalance_gpu.py emulates 2 to 8 ranks.
 """
 import os
 import sys
@@ -242,6 +245,122 @@ def run_features(rank, world, dev, W=1280, H=720, K=4):
             assert not bool(x[:, ~rows].any()), f"{mode} {name}: foreign rows not zero"
 
 
+def run_rebalance(rank, world, dev, W=640, H=400):
+    """Rebalance leg (argument `rebalance`): every rank builds the same with_raw scene, owns an uneven share of it (rank r weighted r + 1,
+    the last rank three times more), steps FusedAdam three times on it and calls sharded.rebalance (NCCL all_gather and batch_isend_irecv).
+    Each rank restates the global arrays and their Adam steps on its own GPU (the update is elementwise), so afterwards its new rows of
+    every parameter, both moments and the statistics must be the even split's slice of them, bit for bit; one more step too.  The
+    Gaussian-sharded render before and after has the single-GPU render's own rows bit for bit; densify_and_prune runs on the result."""
+    import types
+    from street_gaussians_b200 import sharded, training
+    names, stats = training.PARAM_NAMES, training.STAT_NAMES
+    scene = synthetic.make_scene(P=200_000, width=W, height=H, sh_degree=3, seed=81, n_vehicles=4, per_vehicle=20_000, with_raw=True,
+                                 scale_med=0.02)
+    raw = scene["raw"]
+    poses, idft = raw["poses"].to(dev), raw["idft"].to(dev)
+    g = torch.Generator().manual_seed(9)
+    glob = []
+    for r in raw["models"]:
+        n = r["xyz"].shape[0]
+        m = {"_" + a: v.to(dev).contiguous() for a, v in r.items()}
+        m["_semantic"] = torch.rand(n, 2, generator=g).to(dev)
+        m["max_radii2D"], m["xyz_gradient_accum"], m["denom"] = (torch.rand(n, generator=g).to(dev), torch.rand(n, 2, generator=g).to(dev),
+                                                                 torch.rand(n, 1, generator=g).to(dev) + 1)
+        glob.append(m)
+    counts = [m["_xyz"].shape[0] for m in glob]
+    P = sum(counts)
+    w = [r + 1 for r in range(world)]
+    w[-1] *= 3
+    B = [P * sum(w[:r]) // sum(w) for r in range(world + 1)]
+    G = [sum(counts[:k]) for k in range(len(glob) + 1)]
+    rows = lambda Bs: [(max(Bs[rank], G[k]) - G[k], max(max(Bs[rank], G[k]), min(Bs[rank + 1], G[k + 1])) - G[k]) for k in range(len(glob))]
+    grads = [[torch.randn(m[a].shape, generator=g).to(dev) * 1e-2 for a in names] for m in glob]
+
+    def model(k, m, lo, hi):
+        o = types.SimpleNamespace(**{a: torch.nn.Parameter(m[a][lo:hi].clone()) for a in names}, **{s: m[s][lo:hi].clone() for s in stats},
+                                  percent_dense=0.01, percent_big_ws=0.1)
+        if k == 0:
+            o.scene_radius, o.sphere_center, o.sphere_radius = torch.tensor([20.0]), torch.zeros(3), torch.tensor([40.0])
+        else:
+            o.extent, o.min_xyz, o.max_xyz = torch.tensor([3.0]), torch.tensor([-3.0, -1.5, -1.5]), torch.tensor([3.0, 1.5, 1.5])
+        return o
+
+    def adam(objs):
+        return training.FusedAdam([{"params": [getattr(o, a)], "lr": 1e-3 * (1 + i)} for o in objs for i, a in enumerate(names)], eps=1e-15)
+
+    def step(objs, opt, rr, scale):
+        for k, o in enumerate(objs):
+            for a, gk in zip(names, grads[k]):
+                getattr(o, a).grad = gk[rr[k][0]:rr[k][1]] * scale
+        opt.step()
+
+    full = [model(k, m, 0, counts[k]) for k, m in enumerate(glob)]
+    mine = [model(k, m, *rows(B)[k]) for k, m in enumerate(glob)]
+    fopt, opt = adam(full), adam(mine)
+    for it in range(3):
+        step(full, fopt, [(0, n) for n in counts], 1 + it)
+        step(mine, opt, rows(B), 1 + it)
+    st = util.settings_from(sgb, scene["cam"], dev)
+    img_rows = band_of_rows(H, rank, world).to(dev)
+    with torch.no_grad():
+        xyz, rot, scale, opac, sh = sgb.compose(full, poses, idft)
+        ref = sgb.GaussianRasterizer(st)(means3D=xyz, means2D=None, opacities=opac, shs=sh, scales=scale, rotations=rot)
+    rast = GaussianShardedRasterizer(st)
+
+    def render_own_rows(tag):
+        with torch.no_grad():
+            xyz, rot, scale, opac, sh = sgb.compose(mine, poses, idft)
+            got = rast(means3D=xyz, means2D=None, opacities=opac, shs=sh, scales=scale, rotations=rot)
+        for a, b, name in ((got[0], ref[0], "color"), (got[2], ref[2], "depth"), (got[3], ref[3], "alpha")):
+            assert torch.equal(a[:, img_rows], b[:, img_rows]), f"rebalance {tag}: {name} own rows differ"
+
+    render_own_rows("before")
+    P_new = sharded.rebalance(mine, opt, rasterizer=rast)
+    base, extra = divmod(P, world)
+    Bn = [r * base + min(r, extra) for r in range(world + 1)]
+    assert P_new == Bn[rank + 1] - Bn[rank] and rast.chunk == base + (extra > 0), (P_new, rast.chunk)
+    bits = lambda t: t.detach().contiguous().view(torch.int32)
+    for k, (o, f) in enumerate(zip(mine, full)):
+        lo, hi = rows(Bn)[k]
+        for a in names:
+            p, q = getattr(o, a), getattr(f, a)
+            assert torch.equal(bits(p), bits(q[lo:hi])), (k, a)
+            assert any(p is x for grp in opt.param_groups for x in grp["params"]) and opt.state[p]["step"] == 3
+            for mk in ("exp_avg", "exp_avg_sq"):
+                assert torch.equal(bits(opt.state[p][mk]), bits(fopt.state[q][mk][lo:hi])), (k, a, mk)
+        for s in stats:
+            assert torch.equal(bits(getattr(o, s)), bits(getattr(f, s)[lo:hi])), (k, s)
+    step(full, fopt, [(0, n) for n in counts], 7)
+    step(mine, opt, rows(Bn), 7)
+    for k, (o, f) in enumerate(zip(mine, full)):
+        lo, hi = rows(Bn)[k]
+        for a in names:
+            assert torch.equal(bits(getattr(o, a)), bits(getattr(f, a)[lo:hi])), ("step after rebalance", k, a)
+    with torch.no_grad():  # the render of the stepped arrays, before the comparison render
+        xyz, rot, scale, opac, sh = sgb.compose(full, poses, idft)
+        ref = sgb.GaussianRasterizer(st)(means3D=xyz, means2D=None, opacities=opac, shs=sh, scales=scale, rotations=rot)
+    render_own_rows("after")
+    training.densify_and_prune(mine, 1e-7, 0.005, True, opt, seed=rank)
+    return P_new
+
+
+def run_all(rank, world, dev, exchange):
+    # the last case carries feature channels through the bounded path: with exchange=p2p its passes 2-4 are the fused step with
+    # semantics (sgr_sharded_*_features, no NCCL), with exchange=nccl the staged one
+    for S, P, W, H, bounded in ((0, 200_003, 1280, 720, False), (2, 60_001, 800, 608, False), (0, 200_003, 1280, 720, True),
+                                (3 + 4, 60_001, 800, 608, True)):
+        worst, floor = run_case(rank, world, dev, S, P, W, H, bounded, exchange)
+        print(f"[rank {rank}/{world}] exchange={exchange} S={S} P={P} {W}x{H} bounded={bounded}: images bit-equal, worst grad rel err {worst:.2e} "
+              f"(single-GPU run-to-run floor {floor:.2e})", flush=True)
+    run_losses(rank, world, dev)
+    print(f"[rank {rank}/{world}] band losses: the frame's values, gradient rows bit-equal to the single-GPU losses", flush=True)
+    run_image_stages(rank, world, dev)
+    print(f"[rank {rank}/{world}] band sky and colour correction: rows bit-equal to the single-GPU calls, parameter gradients the frame's",
+          flush=True)
+    run_features(rank, world, dev)
+    print(f"[rank {rank}/{world}] band feature finishing: rows bit-equal to the single-GPU calls", flush=True)
+
+
 def main():
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -251,21 +370,13 @@ def main():
         dist.init_process_group("nccl", device_id=dev)
     ok = True
     try:
-        exchange = sys.argv[1] if len(sys.argv) > 1 else "nccl"
-        # the last case carries feature channels through the bounded path: with exchange=p2p its passes 2-4 are the fused step with
-        # semantics (sgr_sharded_*_features, no NCCL), with exchange=nccl the staged one
-        for S, P, W, H, bounded in ((0, 200_003, 1280, 720, False), (2, 60_001, 800, 608, False), (0, 200_003, 1280, 720, True),
-                                    (3 + 4, 60_001, 800, 608, True)):
-            worst, floor = run_case(rank, world, dev, S, P, W, H, bounded, exchange)
-            print(f"[rank {rank}/{world}] exchange={exchange} S={S} P={P} {W}x{H} bounded={bounded}: images bit-equal, worst grad rel err {worst:.2e} "
-                  f"(single-GPU run-to-run floor {floor:.2e})", flush=True)
-        run_losses(rank, world, dev)
-        print(f"[rank {rank}/{world}] band losses: the frame's values, gradient rows bit-equal to the single-GPU losses", flush=True)
-        run_image_stages(rank, world, dev)
-        print(f"[rank {rank}/{world}] band sky and colour correction: rows bit-equal to the single-GPU calls, parameter gradients the frame's",
-              flush=True)
-        run_features(rank, world, dev)
-        print(f"[rank {rank}/{world}] band feature finishing: rows bit-equal to the single-GPU calls", flush=True)
+        mode = sys.argv[1] if len(sys.argv) > 1 else "nccl"
+        if mode == "rebalance":
+            P_new = run_rebalance(rank, world, dev)
+            print(f"[rank {rank}/{world}] rebalance: {P_new} Gaussians, rows / moments / statistics the even split's slice bit for bit, "
+                  "own image rows bit-equal before and after", flush=True)
+        else:
+            run_all(rank, world, dev, mode)
     except AssertionError as e:
         ok = False
         print(f"[rank {rank}] FAILED: {e!r}", flush=True)
