@@ -299,6 +299,8 @@ typedef struct SgrPeers {
 	float *sem[SGR_MAX_PEERS];          /* feature channels of the fused step (sgr_sharded_*_features only; may be NULL otherwise):  */
 	float *gsem[SGR_MAX_PEERS];         /* rank p's sem[world*chunk, S] (delivered semantics) and gsem[world*chunk, S] (its partial
 	                                       dL/dsemantics), rows by slot like records and grad2d, mapped into every rank */
+	float *pose_acc[SGR_MAX_PEERS];     /* rank p's composer accumulator section: SGR_POSE_ACC_ROWS rows of 16 floats, mapped into every
+	                                       rank (sgr_compose_pose_reduce_peers only; may be NULL otherwise) */
 } SgrPeers;
 int sgr_scatter_records(const SgrFrame *frame, const SgrPeers *peers, const void *records_local, const int32_t *radii_local,
                         void *stream);
@@ -423,6 +425,36 @@ int sgr_compose_backward_corrected(const SgrSegment *segments, const SgrSegmentG
                                    const float *bkgd_correction, const float *dL_dmeans3D, const float *dL_drotations, const float *dL_dscales,
                                    const float *dL_dopacities, const float *dL_dshs, float *dposes, float *dcorrection, float *pose_scratch,
                                    void *stream);
+/* The composer under Gaussian sharding: each rank composes its own rows of every sub-model (a segment may have count 0) with the
+ * replicated poses and correction, so its backward sees one share of the frame's pose and correction terms.  The backward above is
+ * split in two around a sum over the ranks:
+ *   sgr_compose_backward_rows : the per-row gradients exactly as sgr_compose_backward (bkgd_correction NULL) or
+ *                               sgr_compose_backward_corrected write them, and this rank's accumulator rows
+ *                               pose_acc[sgr_compose_pose_rows(num_segments, bkgd_correction != NULL), 16] (device, fully written): per
+ *                               segment (then one row for the correction) the 16 sums sum g_xyz (x) x_local (9), the rotation path (4),
+ *                               sum g_xyz (3) of its rows.
+ *   sgr_compose_pose_finalize : dposes[num_segments, 8] and, with bkgd_correction, dcorrection[8] from accumulator rows that already
+ *                               hold the frame's sums.  The map is linear in the rows with coefficients from poses / bkgd_correction
+ *                               only, so finalizing summed rows equals finalizing the rows of the whole frame up to the order of the
+ *                               fp32 additions (which the single-GPU call takes from its atomics).
+ *   sgr_compose_pose_reduce_peers : pose_acc on entry holds this rank's rows, on return the frame's sums, added from 0 in ascending rank
+ *                               order from every rank's peers->pose_acc section (so every rank computes the same bytes), and dposes /
+ *                               dcorrection are finalized from them.  Per group of SGR_POSE_ACC_ROWS rows: the rank's rows are copied
+ *                               into its section, device barrier, sum, device barrier (no rank overwrites its section while a peer may
+ *                               still read it).  The barriers take the device-side count of sgr_peer_barrier (the fused step's pad).
+ *                               No NCCL, no host read-back; every rank must make the call with the same segment table.
+ * pose_acc_bytes: the size of pose_acc (SGR_ENOMEM below 64 bytes per row).  Arguments are checked before anything is enqueued. */
+#define SGR_POSE_ACC_ROWS 256
+int32_t sgr_compose_pose_rows(int32_t num_segments, int32_t corrected);
+int sgr_compose_backward_rows(const SgrSegment *segments, const SgrSegmentGrads *grads, int32_t num_segments, int32_t M, const float *poses,
+                              const float *idft, const uint8_t *flip, const float *flip_quat, const float *bkgd_correction,
+                              const float *dL_dmeans3D, const float *dL_drotations, const float *dL_dscales, const float *dL_dopacities,
+                              const float *dL_dshs, float *pose_acc, size_t pose_acc_bytes, void *stream);
+int sgr_compose_pose_finalize(const SgrSegment *segments, int32_t num_segments, const float *poses, const float *bkgd_correction,
+                              const float *pose_acc, size_t pose_acc_bytes, float *dposes, float *dcorrection, void *stream);
+int sgr_compose_pose_reduce_peers(const SgrPeers *peers, const SgrSegment *segments, int32_t num_segments, const float *poses,
+                                  const float *bkgd_correction, float *pose_acc, size_t pose_acc_bytes, float *dposes, float *dcorrection,
+                                  void *stream);
 
 /* ---- Colour correction (lib/models/color_correction.py:129-140, cfg.model.use_color_correction) ----
  * out[i] = A[i,0] image[0] + A[i,1] image[1] + A[i,2] image[2] + A[i,3] per pixel: the products in einsum's order, then the bias.

@@ -26,7 +26,8 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_set_nea
            "sgr_densify_scratch_bytes", "sgr_densify_plan", "sgr_densify_apply", "sgr_reset_opacity", "sgr_rebalance_row_floats",
            "sgr_rebalance_scratch_bytes", "sgr_rebalance_pack", "sgr_rebalance_splice", "sgr_sparse_adam_step",
            "sgr_layer_state_sizes", "sgr_forward_layer", "sgr_backward_blend_layer", "sgr_backward_geom_layered",
-           "sgr_compose_forward_corrected", "sgr_compose_backward_corrected", "sgr_color_correct_forward", "sgr_color_correct_scratch_bytes",
+           "sgr_compose_forward_corrected", "sgr_compose_backward_corrected", "sgr_compose_pose_rows", "sgr_compose_backward_rows",
+           "sgr_compose_pose_finalize", "sgr_compose_pose_reduce_peers", "sgr_color_correct_forward", "sgr_color_correct_scratch_bytes",
            "sgr_color_correct_backward", "sgr_color_correction_reg", "sgr_sky_composite_forward", "sgr_sky_composite_backward",
            "sgr_actor_pose_forward", "sgr_actor_pose_scratch_bytes", "sgr_actor_pose_backward", "sgr_gaussian_normals_forward",
            "sgr_gaussian_normals_backward", "sgr_compose_semantics_forward", "sgr_compose_semantics_backward", "sgr_finish_features_forward",
@@ -72,7 +73,10 @@ MAX_PEERS = 16
 class SgrPeers(C.Structure):
     _fields_ = [("world", C.c_int32), ("rank", C.c_int32), ("chunk", C.c_int64), ("records", C.c_void_p * MAX_PEERS),
                 ("radii", C.c_void_p * MAX_PEERS), ("grad2d", C.c_void_p * MAX_PEERS), ("flags", C.c_void_p * MAX_PEERS),
-                ("sem", C.c_void_p * MAX_PEERS), ("gsem", C.c_void_p * MAX_PEERS)]
+                ("sem", C.c_void_p * MAX_PEERS), ("gsem", C.c_void_p * MAX_PEERS), ("pose_acc", C.c_void_p * MAX_PEERS)]
+
+
+POSE_ACC_ROWS = 256  # SGR_POSE_ACC_ROWS: rows of 16 floats in a rank's composer accumulator section
 
 
 MAX_FOURIER = 8
@@ -229,6 +233,14 @@ def lib():
     L.sgr_compose_forward_corrected.argtypes = [C.POINTER(SgrSegment), C.c_int32, C.c_int32] + [vp] * 11
     L.sgr_compose_backward_corrected.restype = C.c_int
     L.sgr_compose_backward_corrected.argtypes = [C.POINTER(SgrSegment), C.POINTER(SgrSegmentGrads), C.c_int32, C.c_int32] + [vp] * 14
+    L.sgr_compose_pose_rows.restype = C.c_int32
+    L.sgr_compose_pose_rows.argtypes = [C.c_int32, C.c_int32]
+    L.sgr_compose_backward_rows.restype = C.c_int
+    L.sgr_compose_backward_rows.argtypes = [C.POINTER(SgrSegment), C.POINTER(SgrSegmentGrads), C.c_int32, C.c_int32] + [vp] * 11 + [C.c_size_t, vp]
+    L.sgr_compose_pose_finalize.restype = C.c_int
+    L.sgr_compose_pose_finalize.argtypes = [C.POINTER(SgrSegment), C.c_int32] + [vp] * 3 + [C.c_size_t, vp, vp, vp]
+    L.sgr_compose_pose_reduce_peers.restype = C.c_int
+    L.sgr_compose_pose_reduce_peers.argtypes = [C.POINTER(SgrPeers), C.POINTER(SgrSegment), C.c_int32] + [vp] * 3 + [C.c_size_t, vp, vp, vp]
     L.sgr_color_correct_forward.restype = C.c_int
     L.sgr_color_correct_forward.argtypes = [C.c_int32, C.c_int32, vp, vp, vp, vp]
     L.sgr_color_correct_scratch_bytes.restype = C.c_size_t

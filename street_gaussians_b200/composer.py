@@ -37,7 +37,7 @@ def _raw(model, key):
 
 class _Compose(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, poses, idft, flip, flip_quat, corr_rot, corr_trans, n_models, *raw):
+    def forward(ctx, poses, idft, flip, flip_quat, corr_rot, corr_trans, n_models, reduce, *raw):
         if not raw[0].is_cuda:
             raise _capi.SgrError("street_gaussians_b200 composer needs CUDA tensors (there is no CPU fallback)")
         dev = raw[0].device
@@ -86,7 +86,7 @@ class _Compose(torch.autograd.Function):
         ctx.pose_shape = None if poses is None else (tuple(poses.shape), poses.dtype, poses.device)
         ctx.corr_meta = None if corr is None else ((tuple(corr_rot.shape), corr_rot.dtype, corr_rot.device),
                                                    (tuple(corr_trans.shape), corr_trans.dtype, corr_trans.device))
-        ctx.corr = corr
+        ctx.corr, ctx.reduce = corr, reduce
         ctx.save_for_backward(pose_tab, idft_tab, *raw)
         return xyz, rot, scale, opac, sh
 
@@ -105,13 +105,16 @@ class _Compose(torch.autograd.Function):
             g.xyz, g.rotation, g.scaling, g.opacity, g.features_dc, g.features_rest = (t.data_ptr() if t.numel() else None for t in grads[6 * k: 6 * k + 6])
         dposes = torch.empty((nseg, 8), device=dev, dtype=torch.float32)
         corr = ctx.corr
-        if corr is None:
+        dcorr = None if corr is None else torch.empty((8,), device=dev, dtype=torch.float32)
+        if ctx.reduce is not None:
+            _backward_rows_reduced(ctx.reduce, dev, ctx.segs, gtab, nseg, M, pose_tab, idft_tab, ctx.flip_full, ctx.flip_quat, corr,
+                                   (g_xyz, g_rot, g_scale, g_opac, g_sh), dposes, dcorr)
+        elif corr is None:
             scratch = torch.empty((nseg, 16), device=dev, dtype=torch.float32)
             _capi.call("sgr_compose_backward", dev, ctx.segs, gtab, nseg, M, ptr(pose_tab), ptr(idft_tab), ptr(ctx.flip_full), ptr(ctx.flip_quat),
                        ptr(g_xyz), ptr(g_rot), ptr(g_scale), ptr(g_opac), ptr(g_sh), ptr(dposes), ptr(scratch))
         else:
             scratch = torch.empty((nseg + 1, 16), device=dev, dtype=torch.float32)
-            dcorr = torch.empty((8,), device=dev, dtype=torch.float32)
             _capi.call("sgr_compose_backward_corrected", dev, ctx.segs, gtab, nseg, M, ptr(pose_tab), ptr(idft_tab), ptr(ctx.flip_full),
                        ptr(ctx.flip_quat), ptr(corr), ptr(g_xyz), ptr(g_rot), ptr(g_scale), ptr(g_opac), ptr(g_sh), ptr(dposes), ptr(dcorr),
                        ptr(scratch))
@@ -122,14 +125,54 @@ class _Compose(torch.autograd.Function):
         if corr is not None:
             (rs, rd, rdev), (ts, td, tdev) = ctx.corr_meta
             g_crot, g_ctrans = dcorr[:4].to(device=rdev, dtype=rd).reshape(rs), dcorr[4:7].to(device=tdev, dtype=td).reshape(ts)
-        return (g_poses, None, None, None, g_crot, g_ctrans, None) + tuple(grads)
+        return (g_poses, None, None, None, g_crot, g_ctrans, None, None) + tuple(grads)
+
+
+def _backward_rows_reduced(reduce, dev, segs, gtab, nseg, M, pose_tab, idft_tab, flip_full, flip_quat, corr, upstream, dposes, dcorr):
+    """The backward of one rank's rows under Gaussian sharding: its per-row gradients and accumulator rows, the rows summed over the
+    ranks (COLLECTIVE), then dposes / dcorr finalized from the frame's sums, the same bytes on every rank."""
+    L = _capi.lib()
+    acc = torch.empty((int(L.sgr_compose_pose_rows(nseg, int(corr is not None))), 16), device=dev, dtype=torch.float32)
+    _capi.call("sgr_compose_backward_rows", dev, segs, gtab, nseg, M, ptr(pose_tab), ptr(idft_tab), ptr(flip_full), ptr(flip_quat), ptr(corr),
+               *(ptr(g) for g in upstream), ptr(acc), acc.numel() * 4)
+    kind, arg = reduce
+    if kind == "p2p":  # over the rasterizer's peer workspace: stage, barrier, sum in rank order, barrier per group of rows, then finalize
+        ws = arg.pose_workspace()
+        ws.next_epochs(2 * ((acc.shape[0] + _capi.POSE_ACC_ROWS - 1) // _capi.POSE_ACC_ROWS))
+        _capi.call("sgr_compose_pose_reduce_peers", dev, C.byref(ws.peers), segs, nseg, ptr(pose_tab), ptr(corr), ptr(acc), acc.numel() * 4,
+                   ptr(dposes), ptr(dcorr))
+    else:
+        from .band_losses import all_reduce_sum
+        all_reduce_sum(acc, arg)
+        _capi.call("sgr_compose_pose_finalize", dev, segs, nseg, ptr(pose_tab), ptr(corr), ptr(acc), acc.numel() * 4, ptr(dposes), ptr(dcorr))
+
+
+def _reduction(group, rasterizer):
+    """(kind, what) of the sum over the ranks, or None for the single-GPU call."""
+    if rasterizer is None and group is None:
+        return None
+    if rasterizer is not None:
+        if group is not None and group is not rasterizer.group:
+            raise ValueError("compose: group= differs from the rasterizer's group")
+        if rasterizer.exchange == "p2p":
+            return ("p2p", rasterizer)
+        group = rasterizer.group
+    return ("nccl", group)
 
 
 def compose(models: Sequence, poses: Optional[torch.Tensor] = None, idft: Optional[torch.Tensor] = None,
             flip: Optional[torch.Tensor] = None, flip_quat: Optional[torch.Tensor] = None, *,
-            pose_correction: Optional[Tuple[torch.Tensor, torch.Tensor]] = None):
+            pose_correction: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, group=None, rasterizer=None):
     """-> (means3D[P,3], rotations[P,4], scales[P,3], opacities[P,1], shs[P,M,3]) of background + actors, differentiable.
-    pose_correction = (rot [4], trans [3]) moves the background by the learned per-image correction; gradients return to both."""
+    pose_correction = (rot [4], trans [3]) moves the background by the learned per-image correction; gradients return to both.
+
+    group= / rasterizer= (Gaussian sharding, sharded.GaussianShardedRasterizer): `models` hold this rank's rows of every sub-model (any
+    of them may have 0 rows, as sharded.rebalance can leave them) while poses, idft and pose_correction are the frame's, the same on every
+    rank.  The composed rows are the single-GPU call's rows bit for bit.  COLLECTIVE in the backward: the per-segment pose and correction
+    sums of every rank's rows are added before they become dL/dposes and dL/dcorrection, so those are the frame's gradients and the same
+    bytes on every rank (up to the order of fp32 additions, they are the single-GPU call's), and replicated pose parameters step alike.
+    rasterizer= with exchange="p2p" sums over its peer workspace, in ascending rank order, with device-side barriers and no NCCL call;
+    otherwise (exchange="nccl", or group= alone) one all_reduce over the group.  None for both keeps the single-GPU call."""
     raw = [_raw(m, k) for m in models for k in RAW_KEYS]
     n_act = len(models) - 1
     if n_act > 0:
@@ -144,4 +187,4 @@ def compose(models: Sequence, poses: Optional[torch.Tensor] = None, idft: Option
         corr_rot, corr_trans = pose_correction
         if corr_rot.numel() != 4 or corr_trans.numel() != 3:
             raise ValueError("pose_correction must be (rot [4] = qw, qx, qy, qz; trans [3])")
-    return _Compose.apply(poses, idft, flip, flip_quat, corr_rot, corr_trans, len(models), *raw)
+    return _Compose.apply(poses, idft, flip, flip_quat, corr_rot, corr_trans, len(models), _reduction(group, rasterizer), *raw)

@@ -943,6 +943,83 @@ int sgr_compose_backward_corrected(const SgrSegment *segments, const SgrSegmentG
 	                             dL_dmeans3D, dL_drotations, dL_dscales, dL_dopacities, dL_dshs, dposes, dcorrection, pose_scratch, stream);
 }
 
+int32_t sgr_compose_pose_rows(int32_t num_segments, int32_t corrected) { return num_segments > 0 ? num_segments + (corrected ? 1 : 0) : 0; }
+
+static int check_pose_acc_bytes(const char *fn, int32_t num_segments, const float *bkgd_correction, size_t bytes) {
+	const size_t need = (size_t)sgr_compose_pose_rows(num_segments, bkgd_correction != nullptr) * 16 * sizeof(float);
+	if (bytes < need) return fail(SGR_ENOMEM, "%s: pose_acc holds %zu bytes, %zu needed", fn, bytes, need);
+	return SGR_OK;
+}
+
+int sgr_compose_backward_rows(const SgrSegment *segments, const SgrSegmentGrads *grads, int32_t num_segments, int32_t M, const float *poses,
+                              const float *idft, const uint8_t *flip, const float *flip_quat, const float *bkgd_correction,
+                              const float *dL_dmeans3D, const float *dL_drotations, const float *dL_dscales, const float *dL_dopacities,
+                              const float *dL_dshs, float *pose_acc, size_t pose_acc_bytes, void *stream) {
+	int64_t P = 0;
+	int rc = check_segments(segments, num_segments, M, P);
+	if (rc) return rc;
+	if (!grads || !pose_acc || !poses || !idft) return fail(SGR_EINVAL, "NULL pointer passed to sgr_compose_backward_rows");
+	if (P > 0 && (!dL_dmeans3D || !dL_drotations || !dL_dscales || !dL_dopacities || !dL_dshs)) return fail(SGR_EINVAL, "NULL upstream gradient");
+	if (flip && !flip_quat) return fail(SGR_EINVAL, "flip mask given without flip_quat");
+	for (int k = 0; k < num_segments; k++) {
+		const SgrSegmentGrads &g = grads[k];
+		if (segments[k].count > 0 && (!g.xyz || !g.rotation || !g.scaling || !g.opacity || !g.features_dc || (M > 1 && !g.features_rest)))
+			return fail(SGR_EINVAL, "segment %d has a NULL gradient array", k);
+	}
+	if ((rc = check_pose_acc_bytes("sgr_compose_backward_rows", num_segments, bkgd_correction, pose_acc_bytes)) != SGR_OK) return rc;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_compose_bwd_rows(segments, grads, num_segments, M, poses, idft, flip, flip_quat, dL_dmeans3D, dL_drotations, dL_dscales,
+	                                dL_dopacities, dL_dshs, pose_acc, bkgd_correction, st),
+	        "compose_bwd_rows");
+	return SGR_OK;
+}
+
+// what the finalize reads: the posed flags of the segments and, with a correction, somewhere to put its gradient
+static int check_pose_finalize(const char *fn, const SgrSegment *segments, int32_t num_segments, const float *poses, const float *bkgd_correction,
+                               const float *pose_acc, size_t pose_acc_bytes, const float *dposes, const float *dcorrection) {
+	if (!segments || num_segments <= 0) return fail(SGR_EINVAL, "segment table is empty");
+	if (!poses || !pose_acc || !dposes) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	if (bkgd_correction && !dcorrection) return fail(SGR_EINVAL, "%s: bkgd_correction given without dcorrection", fn);
+	if (!bkgd_correction && dcorrection) return fail(SGR_EINVAL, "%s: dcorrection given without bkgd_correction", fn);
+	return check_pose_acc_bytes(fn, num_segments, bkgd_correction, pose_acc_bytes);
+}
+
+int sgr_compose_pose_finalize(const SgrSegment *segments, int32_t num_segments, const float *poses, const float *bkgd_correction,
+                              const float *pose_acc, size_t pose_acc_bytes, float *dposes, float *dcorrection, void *stream) {
+	int rc = check_pose_finalize("sgr_compose_pose_finalize", segments, num_segments, poses, bkgd_correction, pose_acc, pose_acc_bytes, dposes,
+	                             dcorrection);
+	if (rc) return rc;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_compose_pose_finalize(segments, num_segments, poses, pose_acc, dposes, bkgd_correction, dcorrection, st), "compose_pose_finalize");
+	return SGR_OK;
+}
+
+int sgr_compose_pose_reduce_peers(const SgrPeers *peers, const SgrSegment *segments, int32_t num_segments, const float *poses,
+                                  const float *bkgd_correction, float *pose_acc, size_t pose_acc_bytes, float *dposes, float *dcorrection,
+                                  void *stream) {
+	if (!peers) return fail(SGR_EINVAL, "peers is NULL");
+	int rc = check_pose_finalize("sgr_compose_pose_reduce_peers", segments, num_segments, poses, bkgd_correction, pose_acc, pose_acc_bytes, dposes,
+	                             dcorrection);
+	if (rc) return rc;
+	FrameDev f = {};
+	PeerTable pt = {};
+	if ((rc = make_peers(peers, f, false, pt)) != SGR_OK) return rc;
+	PoseAccPeers pp = {};
+	pp.world = pt.world;
+	for (int p = 0; p < pt.world; p++) {
+		if (!peers->pose_acc[p]) return fail(SGR_EINVAL, "peer table entry %d has no composer accumulator section", p);
+		if (pt.world > 1 && !pt.flags[p]) return fail(SGR_EINVAL, "peer table entry %d has no barrier pad", p);
+		pp.sec[p] = peers->pose_acc[p];
+	}
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_compose_pose_reduce(pt, pp, pose_acc, sgr_compose_pose_rows(num_segments, bkgd_correction != nullptr), st), "compose_pose_reduce");
+	SGR_TRY(launch_compose_pose_finalize(segments, num_segments, poses, pose_acc, dposes, bkgd_correction, dcorrection, st), "compose_pose_finalize");
+	return SGR_OK;
+}
+
 int sgr_color_correct_forward(int32_t H, int32_t W, const float *image, const float *affine, float *out, void *stream) {
 	if (H <= 0 || W <= 0) return fail(SGR_EINVAL, "bad image size H=%d W=%d", H, W);
 	if (!image || !affine || !out) return fail(SGR_EINVAL, "NULL pointer passed to sgr_color_correct_forward");

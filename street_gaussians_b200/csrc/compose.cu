@@ -450,10 +450,11 @@ cudaError_t launch_compose_fwd(const SgrSegment *segs, int nseg, int M, const fl
 	return cudaGetLastError();
 }
 
-cudaError_t launch_compose_bwd(const SgrSegment *segs, const SgrSegmentGrads *grads, int nseg, int M, const float *poses, const float *idft,
-                               const uint8_t *flip, const float *flip_quat, const float *g_xyz, const float *g_rot, const float *g_scale,
-                               const float *g_opac, const float *g_sh, float *acc, float *dposes, const float *corr, float *dcorr,
-                               cudaStream_t st) {
+// The backward without the finalize: the per-row gradients and the accumulator rows acc[nseg (+1 with a correction), 16].
+cudaError_t launch_compose_bwd_rows(const SgrSegment *segs, const SgrSegmentGrads *grads, int nseg, int M, const float *poses,
+                                    const float *idft, const uint8_t *flip, const float *flip_quat, const float *g_xyz, const float *g_rot,
+                                    const float *g_scale, const float *g_opac, const float *g_sh, float *acc, const float *corr,
+                                    cudaStream_t st) {
 	// with a correction, acc has one more row (index nseg) for the sums of the unposed rows
 	cudaError_t e = cudaMemsetAsync(acc, 0, (size_t)(nseg + (corr ? 1 : 0)) * 16 * sizeof(float), st);
 	if (e != cudaSuccess) return e;
@@ -476,6 +477,12 @@ cudaError_t launch_compose_bwd(const SgrSegment *segs, const SgrSegmentGrads *gr
 			compose_bwd_kernel<false><<<(count + 255) / 256, 256, 0, st>>>(t, gt, M, poses, idft, flip, flip_quat, g_xyz, g_rot, g_scale, g_opac,
 			                                                                g_sh, acc, nullptr, 0);
 	}
+	return cudaGetLastError();
+}
+
+// acc (the frame's sums) -> dposes (+ dcorr)
+cudaError_t launch_compose_pose_finalize(const SgrSegment *segs, int nseg, const float *poses, const float *acc, float *dposes,
+                                         const float *corr, float *dcorr, cudaStream_t st) {
 	for (int first = 0; first < nseg; first += kMaxSeg) {
 		const int n = nseg - first < kMaxSeg ? nseg - first : kMaxSeg;
 		unsigned posed = 0;
@@ -486,6 +493,45 @@ cudaError_t launch_compose_bwd(const SgrSegment *segs, const SgrSegmentGrads *gr
 			                                                              first + n == nseg ? dcorr : nullptr, nseg);
 		else
 			compose_pose_finalize_kernel<false><<<1, kMaxSeg, 0, st>>>(first, n, posed, poses, acc, dposes, nullptr, nullptr, 0);
+	}
+	return cudaGetLastError();
+}
+
+cudaError_t launch_compose_bwd(const SgrSegment *segs, const SgrSegmentGrads *grads, int nseg, int M, const float *poses, const float *idft,
+                               const uint8_t *flip, const float *flip_quat, const float *g_xyz, const float *g_rot, const float *g_scale,
+                               const float *g_opac, const float *g_sh, float *acc, float *dposes, const float *corr, float *dcorr,
+                               cudaStream_t st) {
+	cudaError_t e = launch_compose_bwd_rows(segs, grads, nseg, M, poses, idft, flip, flip_quat, g_xyz, g_rot, g_scale, g_opac, g_sh, acc, corr, st);
+	if (e != cudaSuccess) return e;
+	return launch_compose_pose_finalize(segs, nseg, poses, acc, dposes, corr, dcorr, st);
+}
+
+// ---- the accumulator rows summed over the ranks of a Gaussian-sharded step (sgr_compose_pose_reduce_peers) ----
+// One group of at most SGR_POSE_ACC_ROWS rows: stage this rank's rows into its own section; after the barrier every rank adds the
+// sections from 0 in ascending rank order, so all ranks compute the same bytes.
+__global__ void __launch_bounds__(256) pose_acc_stage_kernel(const float *__restrict__ src, float *__restrict__ dst, const int n) {
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < n) dst[i] = src[i];
+}
+__global__ void __launch_bounds__(256) pose_acc_sum_kernel(const PoseAccPeers pp, const int n, float *__restrict__ out) {
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	float v = 0.f;
+	for (int p = 0; p < pp.world; p++) v += pp.sec[p][i];
+	out[i] = v;
+}
+
+cudaError_t launch_compose_pose_reduce(const PeerTable &pt, const PoseAccPeers &pp, float *acc, int rows, cudaStream_t st) {
+	for (int r0 = 0; r0 < rows; r0 += SGR_POSE_ACC_ROWS) {
+		const int n = 16 * (rows - r0 < SGR_POSE_ACC_ROWS ? rows - r0 : SGR_POSE_ACC_ROWS);
+		float *mine = acc + (size_t)r0 * 16;
+		count_launch();
+		pose_acc_stage_kernel<<<(n + 255) / 256, 256, 0, st>>>(mine, pp.sec[pt.rank], n);
+		cudaError_t e = launch_peer_barrier(pt, 0u, nullptr, st);
+		if (e != cudaSuccess) return e;
+		count_launch();
+		pose_acc_sum_kernel<<<(n + 255) / 256, 256, 0, st>>>(pp, n, mine);
+		if ((e = launch_peer_barrier(pt, 0u, nullptr, st)) != cudaSuccess) return e;
 	}
 	return cudaGetLastError();
 }

@@ -412,6 +412,18 @@ cudaError_t launch_compose_bwd(const SgrSegment *segs, const SgrSegmentGrads *gr
                                const uint8_t *flip, const float *flip_quat, const float *g_xyz, const float *g_rot, const float *g_scale,
                                const float *g_opac, const float *g_sh, float *acc, float *dposes, const float *corr, float *dcorr,
                                cudaStream_t st);
+cudaError_t launch_compose_bwd_rows(const SgrSegment *segs, const SgrSegmentGrads *grads, int nseg, int M, const float *poses,
+                                    const float *idft, const uint8_t *flip, const float *flip_quat, const float *g_xyz, const float *g_rot,
+                                    const float *g_scale, const float *g_opac, const float *g_sh, float *acc, const float *corr,
+                                    cudaStream_t st);
+cudaError_t launch_compose_pose_finalize(const SgrSegment *segs, int nseg, const float *poses, const float *acc, float *dposes,
+                                         const float *corr, float *dcorr, cudaStream_t st);
+// every rank's composer accumulator section (SgrPeers.pose_acc): SGR_POSE_ACC_ROWS rows of 16 floats
+struct PoseAccPeers {
+	int world;
+	float *sec[kMaxPeers];
+};
+cudaError_t launch_compose_pose_reduce(const PeerTable &pt, const PoseAccPeers &pp, float *acc, int rows, cudaStream_t st);
 cudaError_t launch_color_correct_fwd(int64_t N, const float *image, const float *affine, float *out, cudaStream_t st);
 size_t color_correct_scratch_bytes(int64_t N);
 cudaError_t launch_color_correct_bwd(int64_t N, const float *image, const float *affine, const float *g_out, float *g_image, float *g_affine,

@@ -214,7 +214,8 @@ def _align(n: int, a: int = 256) -> int:
 
 
 class PeerWorkspace:
-    """Per-rank buffer [geom_state | radii_all | grad2d] that every rank of the group can address (include/sgr.h, SgrPeers).
+    """Per-rank buffer [geom_state | radii_all | grad2d | sem | gsem | pose_acc | barrier pad] that every rank of the group can address
+    (include/sgr.h, SgrPeers).
 
     Real multi-GPU: ONE torch symmetric-memory allocation per rank (CUDA VMM mapped into every process; NVLink loads and
     stores), rendezvous'ed once; `barrier()` is the device-side signal-pad barrier of that allocation (a few microseconds
@@ -229,6 +230,7 @@ class PeerWorkspace:
         self.geom_bytes, self.img_bytes, self.off_radii, self.off_grad, self.off_flags, self.total = self.layout(settings, self.P_total, device,
                                                                                                                  self.S)
         self.off_sem, self.off_gsem = self.feature_offsets(self.off_grad, self.P_total, self.S)
+        self.off_pose = self.pose_offset(self.off_grad, self.P_total, self.S)
         self.hdl = None
         self.in_flight = False  # a differentiable forward has used the buffers and its backward has not run yet
         self.epoch = 0          # epoch of the last sgr_peer_barrier issued on this workspace (every rank counts alike)
@@ -260,6 +262,7 @@ class PeerWorkspace:
             if self.S:
                 self.peers.sem[p] = ptrs[p] + self.off_sem
                 self.peers.gsem[p] = ptrs[p] + self.off_gsem
+            self.peers.pose_acc[p] = ptrs[p] + self.off_pose
         nsem = self.P_total * self.S
         self.sem = self.buf[self.off_sem: self.off_sem + 4 * nsem].view(torch.float32).view(self.P_total, self.S)
         self.gsem = self.buf[self.off_gsem: self.off_gsem + 4 * nsem].view(torch.float32).view(self.P_total, self.S)
@@ -271,16 +274,23 @@ class PeerWorkspace:
         return off_sem, _align(off_sem + 4 * P_total * S)
 
     @staticmethod
+    def pose_offset(off_grad: int, P_total: int, S: int) -> int:
+        """Offset of the composer's accumulator section (_capi.POSE_ACC_ROWS rows of 16 fp32, composer.compose's reduction over the
+        ranks), after the feature sections and before the barrier pad."""
+        return _align(PeerWorkspace.feature_offsets(off_grad, P_total, S)[1] + 4 * P_total * S)
+
+    @staticmethod
     def layout(settings, P_total: int, device, S: int = 0):
         """(geom_bytes, img_bytes, offset of radii_all, offset of grad2d, offset of the barrier pad, total bytes) of the per-rank buffer.
-        With S feature channels the sections sem and gsem (feature_offsets) sit before the pad; S = 0 leaves them empty."""
+        With S feature channels the sections sem and gsem (feature_offsets) sit before the pad; S = 0 leaves them empty.  The composer's
+        accumulator section (pose_offset) follows them."""
         fr, keep = _make_frame(settings, P_total, 0, 0, device, None)
         gb, ib = C.c_size_t(0), C.c_size_t(0)
         _capi.call("sgr_state_sizes", None, C.byref(fr), C.byref(gb), C.byref(ib))
         del keep
         off_radii = _align(gb.value)
         off_grad = _align(off_radii + 4 * P_total)
-        off_flags = _align(PeerWorkspace.feature_offsets(off_grad, P_total, S)[1] + 4 * P_total * S)
+        off_flags = _align(PeerWorkspace.pose_offset(off_grad, P_total, S) + 64 * _capi.POSE_ACC_ROWS)
         return gb.value, ib.value, off_radii, off_grad, off_flags, off_flags + 256
 
     @classmethod
@@ -596,6 +606,14 @@ class GaussianShardedRasterizer(nn.Module):
                 self._ws = PeerWorkspace(self.raster_settings, self.chunk, self.world, self.rank, device, self.group, S=S)
             else:
                 self._ws = PeerWorkspace.emulate(self.raster_settings, self.chunk, 1, device, S)[0]
+        return self._ws
+
+    def pose_workspace(self) -> "PeerWorkspace":
+        """The peer workspace composer.compose(rasterizer=self) sums its accumulator rows through (exchange="p2p"): the one this
+        module's forward set up, so the composer's reduction takes no collective of its own."""
+        if self._ws is None:
+            raise _capi.SgrError("compose(rasterizer=...) with exchange='p2p' sums over the rasterizer's peer workspace: run the "
+                                 "rasterizer's forward before the composer's backward")
         return self._ws
 
     def release_workspace(self):

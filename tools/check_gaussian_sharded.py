@@ -20,6 +20,10 @@ kernels.
 
 With the argument `rebalance` only the rebalance leg runs (run_rebalance): sharded.rebalance over NCCL on an uneven split, against the
 global arrays each rank restates.  It has run at world 1 only, not on several H100s; tests/test_rebalance_gpu.py emulates 2 to 8 ranks.
+
+With the argument `compose` (NCCL all_reduce of the accumulator rows) or `compose-p2p` (the rasterizer's peer workspace) only the composer
+leg runs (run_compose): compose(..., group= / rasterizer=) on each rank's rows of a config-C-like scene, before and after the rebalanced
+split.  It has run at world 1 only, not on several H100s; tests/test_sharded_compose_gpu.py emulates 2 to 8 ranks on one GPU.
 """
 import os
 import sys
@@ -37,6 +41,7 @@ import util  # noqa: E402
 
 KEYS = ("means3D", "shs", "opacities", "scales", "rotations")
 GRAD_TOL = 5e-4
+POSE_TOL = 1e-4  # composer pose / correction gradients: sums of ~5e5 fp32 terms, added in another order than the single-GPU atomics
 
 
 def run_case(rank, world, dev, S, P, W, H, bounded, exchange="nccl"):
@@ -344,6 +349,66 @@ def run_rebalance(rank, world, dev, W=640, H=400):
     return P_new
 
 
+def run_compose(rank, world, dev, exchange, n_bg=400_000, actors=(20_000, 0, 7_000, 35_000, 1_000, 12_000, 3, 50_000)):
+    """compose(..., rasterizer=) on this rank's rows of a config-C-like scene (background, 8 tracked actors, flip mask, pose correction)
+    against compose() of the whole scene: own composed rows and raw gradient rows bit-equal, dL/dposes and dL/dcorrection the same bytes on
+    every rank and within POSE_TOL of max|ref| of the single-GPU call (whose float atomics order its sums differently)."""
+    import compose_case as CC
+    from street_gaussians_b200.sharded import rebalance_plan
+    names = ("xyz", "rotation", "scaling", "opacity", "features")
+    models = [{k: v.to(dev) for k, v in m.items()} for m in CC.make_case(5, n_bg, list(actors), 16, 5)]
+    g = torch.Generator().manual_seed(6)
+    poses, idft = torch.randn(len(actors), 7, generator=g).to(dev), torch.randn(len(actors), 5, generator=g).to(dev)
+    flip, fq = (torch.rand(sum(actors), generator=g) < 0.5).to(dev), torch.tensor([0.0, 0.0, 1.0, 0.0], device=dev)
+    corr = ((torch.tensor([1.0, 0, 0, 0]) + 0.1 * torch.randn(4, generator=g)).to(dev), torch.randn(3, generator=g).to(dev))
+    P = n_bg + sum(actors)
+    up = {k: v.to(dev) for k, v in CC.upstream(7, P, 16).items()}
+    starts = np.concatenate([[0], np.cumsum([int(m["xyz"].shape[0]) for m in models])])
+
+    def run(mods, fl, upr, **kw):
+        mods = [{k: v.detach().clone().requires_grad_(True) for k, v in m.items()} for m in mods]
+        dp, cr, ct = poses.clone().requires_grad_(True), corr[0].clone().requires_grad_(True), corr[1].clone().requires_grad_(True)
+        out = sgb.compose(mods, dp, idft, fl, fq, pose_correction=(cr, ct), **kw)
+        torch.autograd.backward(list(out), [upr[k] for k in names])
+        return [o.detach() for o in out], [{k: m[k].grad for k in m} for m in mods], dp.grad, torch.cat([cr.grad, ct.grad])
+
+    ref_out, ref_raw, ref_dp, ref_dc = run(models, flip, up)
+    uneven = [P * r * (r + 1) // (world * (world + 1)) for r in range(world + 1)]
+    counts = [[max(0, min(uneven[r + 1], starts[m + 1]) - max(uneven[r], starts[m])) for m in range(len(models))] for r in range(world)]
+    even = [0]
+    for row in rebalance_plan(counts).counts:
+        even.append(even[-1] + sum(row))
+    for tag, B in (("uneven", uneven), ("rebalanced", even)):
+        lo, hi = B[rank], B[rank + 1]
+        mine, fl = [], []
+        for m, mod in enumerate(models):
+            a, b = max(lo, starts[m]) - starts[m], max(lo, min(hi, starts[m + 1])) - starts[m]
+            a, b = min(a, b), b
+            mine.append({k: v[a:b] for k, v in mod.items()})
+            if m:
+                fl.append(flip[starts[m] - n_bg + a: starts[m] - n_bg + b])
+        st = util.settings_from(sgb, synthetic.make_scene(P=8, width=64, height=48, sh_degree=0, seed=1)["cam"], dev)
+        rast = GaussianShardedRasterizer(st, exchange=exchange)
+        if exchange == "p2p":  # COLLECTIVE: the workspace a forward of the rasterizer would have set up
+            rast.repartition(hi - lo)
+            rast.workspace(dev)
+        out, raw, dp, dc = run(mine, torch.cat(fl), {k: v[lo:hi] for k, v in up.items()}, rasterizer=rast)
+        for k, a, b in zip(names, out, ref_out):
+            assert torch.equal(a, b[lo:hi]), (tag, k)
+        for m, (a, b) in enumerate(zip(raw, ref_raw)):
+            s0, s1 = max(lo, starts[m]) - starts[m], max(lo, min(hi, starts[m + 1])) - starts[m]
+            for k in a:
+                assert torch.equal(a[k], b[k][min(s0, s1):s1]), (tag, m, k)
+        both = torch.cat([dp.reshape(-1), dc])
+        if world > 1:
+            alls = [torch.empty_like(both) for _ in range(world)]
+            dist.all_gather(alls, both)
+            assert all(torch.equal(a, both) for a in alls), (tag, "pose gradients differ across ranks")
+        for a, b in ((dp, ref_dp), (dc, ref_dc)):
+            assert float((a - b).abs().max()) <= POSE_TOL * float(b.abs().max()), (tag, float((a - b).abs().max()), float(b.abs().max()))
+    return P
+
+
 def run_all(rank, world, dev, exchange):
     # the last case carries feature channels through the bounded path: with exchange=p2p its passes 2-4 are the fused step with
     # semantics (sgr_sharded_*_features, no NCCL), with exchange=nccl the staged one
@@ -371,7 +436,11 @@ def main():
     ok = True
     try:
         mode = sys.argv[1] if len(sys.argv) > 1 else "nccl"
-        if mode == "rebalance":
+        if mode in ("compose", "compose-p2p"):
+            P = run_compose(rank, world, dev, "p2p" if mode == "compose-p2p" else "nccl")
+            print(f"[rank {rank}/{world}] compose ({mode}): {P} Gaussians, own rows bit-equal, dL/dposes and dL/dcorrection the same bytes on "
+                  "every rank and the frame's", flush=True)
+        elif mode == "rebalance":
             P_new = run_rebalance(rank, world, dev)
             print(f"[rank {rank}/{world}] rebalance: {P_new} Gaussians, rows / moments / statistics the even split's slice bit for bit, "
                   "own image rows bit-equal before and after", flush=True)
