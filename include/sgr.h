@@ -301,6 +301,9 @@ typedef struct SgrPeers {
 	                                       dL/dsemantics), rows by slot like records and grad2d, mapped into every rank */
 	float *pose_acc[SGR_MAX_PEERS];     /* rank p's composer accumulator section: SGR_POSE_ACC_ROWS rows of 16 floats, mapped into every
 	                                       rank (sgr_compose_pose_reduce_peers only; may be NULL otherwise) */
+	void *loss[SGR_MAX_PEERS];          /* rank p's loss section: loss_bytes bytes, mapped into every rank (sgr_band_halo_exchange_peers /
+	                                       sgr_band_peer_sum only; may be NULL otherwise) */
+	size_t loss_bytes;                  /* size of every rank's loss section (sgr_band_peer_bytes) */
 } SgrPeers;
 int sgr_scatter_records(const SgrFrame *frame, const SgrPeers *peers, const void *records_local, const int32_t *radii_local,
                         void *stream);
@@ -653,6 +656,30 @@ int sgr_band_lidar_select(int32_t level, double keep, int32_t H, int32_t W, int3
 int sgr_band_lidar_grad(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *depth, const float *acc,
                         const float *lidar_depth, float weight, const SgrLidarState *state, const double *sums, float *dL_ddepth,
                         float *dL_dacc, float *scalars, void *scratch, size_t scratch_bytes, void *stream);
+/* The band losses' two exchanges over peer memory (the Gaussian-sharded step's SgrPeers, its loss sections and its barrier pad): no NCCL,
+ * no host read-back.  Every rank of `peers` makes the same sequence of calls with the same C, H, W (and the same type and count).
+ *   sgr_band_halo_exchange_peers : this rank's SEND_UP and SEND_DOWN messages of `image` (sgr_band_halo_pack's [C][rows][W] layout) go
+ *                           into its own loss section (SEND_UP at offset 0, SEND_DOWN at half the section's halo part), device barrier,
+ *                           then RECV_UP is read from the SEND_DOWN message in the section of rank (rank - 1) % world and RECV_DOWN from
+ *                           the SEND_UP message of rank (rank + 1) % world (the neighbours of cyclic and contiguous bands) and written
+ *                           into `out` with sgr_band_halo_unpack's mapping, device barrier.  Only the RECV rows of `out` are written;
+ *                           `out` may be `image`.  An empty band, or world 1, sends and receives nothing but takes both barriers.
+ *   sgr_band_peer_sum      : out[i] = sum over ranks p = 0, 1, .., world - 1 (in that order, from 0) of rank p's local[i]: the local
+ *                           array is copied into the rank's loss section, device barrier, every rank adds the sections, device
+ *                           barrier.  Every rank computes the same bytes; int32 sums are exact (two's complement), fp64 ones take
+ *                           that fixed order.  `out` may be `local`.  count == 0 takes the barriers only.
+ * The barriers are sgr_peer_barrier's with the device-side count (epoch 0): two per call, as sgr_compose_pose_reduce_peers takes them.  The
+ * second keeps a rank from overwriting its section while a peer may still read it, so the calls may follow each other on a stream.
+ * sgr_band_peer_bytes(C, H, W): the loss section both need: the largest pair of halo messages of any band of an image of H rows (two
+ * slots of C x 10 ceil(ceil(H / 16) / 2) x W floats) and the largest array the band losses sum (SGR_LIDAR_LEVEL0_WORDS int32, one
+ * level of SGR_LIDAR_BINS, 1 + ceil(H / 16) doubles, 5 doubles); 0 for bad sizes.  peers->loss_bytes below it: SGR_ENOMEM.  Arguments
+ * are checked before anything is enqueued. */
+#define SGR_PEER_SUM_INT32 0
+#define SGR_PEER_SUM_FLOAT64 1
+size_t sgr_band_peer_bytes(int32_t C, int32_t H, int32_t W);
+int sgr_band_halo_exchange_peers(const SgrPeers *peers, int32_t C, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step,
+                                 const float *image, float *out, void *stream);
+int sgr_band_peer_sum(const SgrPeers *peers, int32_t type, int64_t count, const void *local, void *out, void *stream);
 
 /* ---- The sky composite and the colour correction on a tile-row band (the stages between the rasterizer and the losses) ----
  * The band and the buffers as in the band losses above: every image argument is a whole [.., H, W] frame of which only the band's pixels

@@ -33,7 +33,8 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_set_nea
            "sgr_gaussian_normals_backward", "sgr_compose_semantics_forward", "sgr_compose_semantics_backward", "sgr_finish_features_forward",
            "sgr_finish_features_backward", "sgr_band_halo_rows", "sgr_band_halo_pack", "sgr_band_halo_unpack", "sgr_band_image_loss_stats",
            "sgr_band_image_loss_grad", "sgr_band_sky_loss", "sgr_band_obj_acc_loss", "sgr_band_acc_loss_value", "sgr_band_lidar_scratch_bytes",
-           "sgr_band_lidar_keys", "sgr_band_lidar_select", "sgr_band_lidar_grad", "sgr_band_sky_composite_forward",
+           "sgr_band_lidar_keys", "sgr_band_lidar_select", "sgr_band_lidar_grad", "sgr_band_peer_bytes", "sgr_band_halo_exchange_peers",
+           "sgr_band_peer_sum", "sgr_band_sky_composite_forward",
            "sgr_band_sky_composite_backward", "sgr_band_color_correct_forward", "sgr_band_color_correct_scratch_bytes",
            "sgr_band_color_correct_backward", "sgr_band_color_correct_affine_grad", "sgr_band_finish_features_forward",
            "sgr_band_finish_features_backward", "sgr_eval_metrics_scratch_bytes",
@@ -73,7 +74,8 @@ MAX_PEERS = 16
 class SgrPeers(C.Structure):
     _fields_ = [("world", C.c_int32), ("rank", C.c_int32), ("chunk", C.c_int64), ("records", C.c_void_p * MAX_PEERS),
                 ("radii", C.c_void_p * MAX_PEERS), ("grad2d", C.c_void_p * MAX_PEERS), ("flags", C.c_void_p * MAX_PEERS),
-                ("sem", C.c_void_p * MAX_PEERS), ("gsem", C.c_void_p * MAX_PEERS), ("pose_acc", C.c_void_p * MAX_PEERS)]
+                ("sem", C.c_void_p * MAX_PEERS), ("gsem", C.c_void_p * MAX_PEERS), ("pose_acc", C.c_void_p * MAX_PEERS),
+                ("loss", C.c_void_p * MAX_PEERS), ("loss_bytes", C.c_size_t)]
 
 
 POSE_ACC_ROWS = 256  # SGR_POSE_ACC_ROWS: rows of 16 floats in a rank's composer accumulator section
@@ -147,6 +149,7 @@ class SgrLayerGrad(C.Structure):
 HALO_SEND_UP, HALO_SEND_DOWN, HALO_RECV_UP, HALO_RECV_DOWN = 0, 1, 2, 3
 LIDAR_BINS = 2048
 LIDAR_LEVEL0_WORDS = 6 + LIDAR_BINS
+PEER_SUM_INT32, PEER_SUM_FLOAT64 = 0, 1  # element types of sgr_band_peer_sum
 
 
 class SgrLidarState(C.Structure):
@@ -310,6 +313,12 @@ def lib():
     L.sgr_band_lidar_select.argtypes = [C.c_int32, C.c_double] + [C.c_int32] * 2 + band + [vp, vp, vp, C.c_size_t, vp]
     L.sgr_band_lidar_grad.restype = C.c_int
     L.sgr_band_lidar_grad.argtypes = [C.c_int32] * 2 + band + [vp] * 3 + [C.c_float] + [vp] * 5 + [vp, C.c_size_t, vp]
+    L.sgr_band_peer_bytes.restype = C.c_size_t
+    L.sgr_band_peer_bytes.argtypes = [C.c_int32] * 3
+    L.sgr_band_halo_exchange_peers.restype = C.c_int
+    L.sgr_band_halo_exchange_peers.argtypes = [C.POINTER(SgrPeers)] + [C.c_int32] * 3 + band + [vp, vp, vp]
+    L.sgr_band_peer_sum.restype = C.c_int
+    L.sgr_band_peer_sum.argtypes = [C.POINTER(SgrPeers), C.c_int32, C.c_int64, vp, vp, vp]
     L.sgr_band_sky_composite_forward.restype = C.c_int
     L.sgr_band_sky_composite_forward.argtypes = [C.c_int32] * 2 + band + [C.c_int32] * 2 + [C.c_float] + [vp] * 10
     L.sgr_band_sky_composite_backward.restype = C.c_int

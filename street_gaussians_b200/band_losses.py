@@ -15,6 +15,12 @@ its band, bit-identical to the single-GPU call's:
 The low-level steps below are one C-ABI call each; the tests drive them directly to emulate N ranks on one GPU.  `frame_losses` is the
 autograd entry that runs the photometric, sky and object-accumulation losses of one frame with ONE all-reduce of their partial sums
 (the reference adds them); `losses.py`'s functions take the same `band=` / `group=` keywords.
+
+Two transports carry the halo and the sums; the stages, their order and the autograd functions are the same for both.  With band= /
+group= (or rasterizer= of a GaussianShardedRasterizer with exchange="nccl") they are NCCL's batch_isend_irecv and all_reduce.  With
+rasterizer= of one with exchange="p2p" they are the library's peer-memory calls over the loss section of the workspace that rasterizer's
+forward set up (sgr_band_halo_exchange_peers, sgr_band_peer_sum): device-side barriers, no NCCL call, no host read-back; the fp64 sums add
+the ranks in ascending order, so every rank holds the same bytes.
 """
 from __future__ import annotations
 
@@ -153,6 +159,63 @@ def all_reduce_sum(t: torch.Tensor, group=None) -> torch.Tensor:
     return t
 
 
+def peer_exchange_halo(ws, image: torch.Tensor, band) -> torch.Tensor:
+    """exchange_halo over the loss section of a peer workspace (sgr_band_halo_exchange_peers; COLLECTIVE over the workspace's ranks, on
+    the device): a copy of `image` [C, H, W] with the halo rows filled in.  C must fit the section (3 for sharded.PeerWorkspace)."""
+    out = _capi.f32(image).clone()
+    Cn, H, W = (int(v) for v in out.shape)
+    b, e, s = check_band(band, H)
+    ws.next_epochs(2)
+    _capi.call("sgr_band_halo_exchange_peers", out.device, C.byref(ws.peers), Cn, H, W, b, e, s, ptr(out), ptr(out))
+    return out
+
+
+def peer_sum(ws, t: torch.Tensor) -> torch.Tensor:
+    """all_reduce_sum over the loss section of a peer workspace (sgr_band_peer_sum; COLLECTIVE over the workspace's ranks, on the
+    device): in place, the ranks added from 0 in ascending order.  `t` is a contiguous int32 or float64 tensor."""
+    kinds = {torch.int32: _capi.PEER_SUM_INT32, torch.float64: _capi.PEER_SUM_FLOAT64}
+    if t.dtype not in kinds or not t.is_contiguous():
+        raise ValueError(f"peer_sum takes a contiguous int32 or float64 tensor, got {t.dtype}")
+    ws.next_epochs(2)
+    _capi.call("sgr_band_peer_sum", t.device, C.byref(ws.peers), kinds[t.dtype], t.numel(), ptr(t), ptr(t))
+    return t
+
+
+class Transport:
+    """How a band loss moves its halo and sums its partials: over `group` with NCCL (ws None) or over the loss section of the peer
+    workspace `ws`."""
+
+    def __init__(self, group=None, ws=None):
+        self.group, self.ws = group, ws
+
+    @property
+    def kind(self) -> str:
+        return "nccl" if self.ws is None else "p2p"
+
+    def halo(self, image: torch.Tensor, band) -> torch.Tensor:
+        return exchange_halo(image, band, self.group) if self.ws is None else peer_exchange_halo(self.ws, image, band)
+
+    def sum(self, t: torch.Tensor) -> torch.Tensor:
+        return all_reduce_sum(t, self.group) if self.ws is None else peer_sum(self.ws, t)
+
+
+def resolve(band, group, rasterizer, image_height: int):
+    """(band, Transport) of a band loss call.  Without `rasterizer`, band= / group= as given (NCCL over `group`).  With one (a
+    sharded.GaussianShardedRasterizer), its band (the whole image at world 1, where it has none) and, with exchange="p2p", the loss
+    section of the workspace its forward set up, else NCCL over its group; a band= or group= that differs from the rasterizer's raises
+    ValueError."""
+    if rasterizer is None:
+        return band, Transport(group)
+    if group is not None and group is not rasterizer.group:
+        raise ValueError("the band losses: group= differs from the rasterizer's group")
+    own = rasterizer.band if rasterizer.band is not None else TileRowBand(0, (int(image_height) + 15) // 16, 1)
+    if band is not None and tuple(int(v) for v in band) != tuple(int(v) for v in own):
+        raise ValueError(f"the band losses: band= {tuple(band)} differs from the rasterizer's band {tuple(own)}")
+    if rasterizer.exchange == "p2p":
+        return own, Transport(ws=rasterizer.loss_workspace())
+    return own, Transport(rasterizer.group)
+
+
 # ---- photometric loss ----------------------------------------------------------------------------------------------------------
 def _mask_u8(mask, n: int, device, what: str):
     if mask is None:
@@ -272,13 +335,13 @@ class _FrameLosses(torch.autograd.Function):
     """Photometric, sky and object-accumulation losses of one frame on a band, with one all-reduce of their partial sums."""
     @staticmethod
     def forward(ctx, image, acc, acc_obj, spec):
-        band, group = spec["band"], spec["group"]
+        band, xfer = spec["band"], spec["transport"]
         out = []
         dev = next(t for t in (image, acc, acc_obj) if t is not None).device
         partials = torch.empty(5, device=dev, dtype=torch.float64)  # {SSIM, L1, mask count} {sky} {obj}
         grads = [None, None, None]
         if image is not None:
-            img = exchange_halo(image, band, group)
+            img = xfer.halo(image, band)
             g = _capi.f32(spec["gt"].detach(), dev)
             if img.dim() != 3 or img.shape != g.shape:
                 raise ValueError(f"image / gt must both be [C, H, W], got {tuple(image.shape)} and {tuple(spec['gt'].shape)}")
@@ -292,7 +355,7 @@ class _FrameLosses(torch.autograd.Function):
             m = _mask_u8(spec[key], a.numel(), dev, key)
             grads[1 + i], _ = acc_loss_band(entry, a, m, spec["weights"][1 + i], band, t.requires_grad, partials[3 + i:4 + i])
             accs.append((i, a))
-        all_reduce_sum(partials, group)
+        xfer.sum(partials)
         if image is not None:
             grads[0], scalars = image_loss_grad(img, g, m_img, band, spec["w_l1"], spec["w_ssim"], partials[0:3], scratch, image.requires_grad)
             out.append(scalars[0])
@@ -318,14 +381,18 @@ class _FrameLosses(torch.autograd.Function):
         return res[0], res[1], res[2], None
 
 
-def _frame(image, gt, mask, w_l1: float, w_ssim: float, acc, sky_mask, sky_weight: float, acc_obj, obj_bound, obj_weight: float, band, group):
+def _frame(image, gt, mask, w_l1: float, w_ssim: float, acc, sky_mask, sky_weight: float, acc_obj, obj_bound, obj_weight: float, band, group,
+           rasterizer=None):
     """Values of the present losses, in the order image, acc, acc_obj; the image's is w_l1 * L1 + w_ssim * SSIM."""
-    if band is None:
+    if band is None and rasterizer is None:
         raise ValueError("the band losses need the rank's band")
     if image is None and acc is None and acc_obj is None:
         raise ValueError("frame_losses needs at least one of image, acc and acc_obj")
     H = int((image if image is not None else acc if acc is not None else acc_obj).shape[-2])
+    band, xfer = resolve(band, group, rasterizer, H)
     check_band(band, H)
+    if xfer.kind == "p2p" and image is not None and (image.dim() != 3 or int(image.shape[0]) != 3):
+        raise ValueError(f"the peer-memory halo carries 3-channel images, got an image of shape {tuple(image.shape)}")
     if image is not None and gt is None:
         raise ValueError("the photometric loss needs gt")
     if acc is not None and sky_mask is None:
@@ -333,19 +400,22 @@ def _frame(image, gt, mask, w_l1: float, w_ssim: float, acc, sky_mask, sky_weigh
     if acc_obj is not None and obj_bound is None:
         raise ValueError("the object-accumulation loss needs obj_bound")
     _check_cuda(image, gt, acc, acc_obj)
-    spec = dict(band=band, group=group, gt=gt, mask=mask, sky_mask=sky_mask, obj_bound=obj_bound, w_l1=w_l1, w_ssim=w_ssim,
+    spec = dict(band=band, transport=xfer, gt=gt, mask=mask, sky_mask=sky_mask, obj_bound=obj_bound, w_l1=w_l1, w_ssim=w_ssim,
                 weights=(None, sky_weight, obj_weight))
     return list(_FrameLosses.apply(image, acc, acc_obj, spec))
 
 
 def frame_losses(image=None, gt=None, mask=None, lambda_l1: float = 1.0, lambda_dssim: float = 0.2, acc=None, sky_mask=None,
-                 sky_weight: float = 1.0, acc_obj=None, obj_bound=None, obj_weight: float = 1.0, *, band: TileRowBand, group=None):
+                 sky_weight: float = 1.0, acc_obj=None, obj_bound=None, obj_weight: float = 1.0, *, band: Optional[TileRowBand] = None,
+                 group=None, rasterizer=None):
     """COLLECTIVE over `group`: the photometric loss of `image` (train.py:101-104), the sky loss of `acc` (:107-113) and the
     object-accumulation loss of `acc_obj` (:114-122) of one frame, each rank holding the rendered rows of its `band`; any of the three
     may be left out.  One halo exchange and ONE all-reduce of the five partial sums.  Returns {"photometric", "sky", "obj_acc"} (the
-    present ones) as the frame's values on every rank; their gradients reach the band's rows."""
+    present ones) as the frame's values on every rank; their gradients reach the band's rows.
+    rasterizer= (the GaussianShardedRasterizer that rendered the rows): its band, and with exchange="p2p" the halo and the sum over its
+    peer workspace (resolve); the image must then have 3 channels."""
     vals = _frame(image, gt, mask, (1.0 - lambda_dssim) * lambda_l1, -lambda_dssim, acc, sky_mask, sky_weight, acc_obj, obj_bound, obj_weight,
-                  band, group)
+                  band, group, rasterizer)
     out = {}
     if image is not None:
         out["photometric"] = vals.pop(0) + lambda_dssim
@@ -358,7 +428,7 @@ def frame_losses(image=None, gt=None, mask=None, lambda_l1: float = 1.0, lambda_
 
 class _LidarDepthLossBand(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, depth, acc, lidar_depth, mask, weight: float, keep: float, band, group):
+    def forward(ctx, depth, acc, lidar_depth, mask, weight: float, keep: float, band, xfer):
         _check_cuda(depth, acc, lidar_depth)
         d, a = _capi.f32(depth), _capi.f32(acc)
         dev = d.device
@@ -372,11 +442,11 @@ class _LidarDepthLossBand(torch.autograd.Function):
         m = _mask_u8(mask, H * W, dev, "mask")
         state, scratch = lidar_keys(d, a, ld, m, band)
         for level in (1, 2):
-            all_reduce_sum(lidar_level_words(state, level - 1), group)
+            xfer.sum(lidar_level_words(state, level - 1))
             lidar_select(level, keep, H, W, band, state, scratch)
-        all_reduce_sum(lidar_level_words(state, 2), group)
+        xfer.sum(lidar_level_words(state, 2))
         sums = lidar_select(3, keep, H, W, band, state, scratch)
-        all_reduce_sum(sums, group)
+        xfer.sum(sums)
         gd, ga, scalars = lidar_grad(d, a, ld, weight, band, state, sums, scratch, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
         ctx.save_for_backward(gd, ga)
         ctx.dtypes = (depth.dtype, acc.dtype)
@@ -389,10 +459,13 @@ class _LidarDepthLossBand(torch.autograd.Function):
                 None, None, None, None, None, None)
 
 
-def lidar_depth_loss(depth, acc, lidar_depth, mask=None, weight: float = 1.0, keep: float = 0.95, *, band: TileRowBand, group=None):
+def lidar_depth_loss(depth, acc, lidar_depth, mask=None, weight: float = 1.0, keep: float = 0.95, *, band: Optional[TileRowBand] = None,
+                     group=None, rasterizer=None):
     """COLLECTIVE over `group` (four small all-reduces): losses.lidar_depth_loss of the frame, each rank holding the rendered rows of
-    its `band` of depth and acc; lidar_depth and mask are whole frames.  The selected pixels are the single-GPU call's."""
+    its `band` of depth and acc; lidar_depth and mask are whole frames.  The selected pixels are the single-GPU call's.  rasterizer= as
+    frame_losses' (with exchange="p2p" the four sums go over its peer workspace)."""
     if not (0.0 < float(keep) <= 1.0):
         raise ValueError(f"keep must be in (0, 1], got {keep}")
+    band, xfer = resolve(band, group, rasterizer, int(depth.shape[-2]))
     check_band(band, int(depth.shape[-2]))
-    return _LidarDepthLossBand.apply(depth, acc, lidar_depth, mask, weight, keep, band, group)
+    return _LidarDepthLossBand.apply(depth, acc, lidar_depth, mask, weight, keep, band, xfer)

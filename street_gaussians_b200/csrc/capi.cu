@@ -1478,6 +1478,60 @@ int sgr_band_lidar_grad(int32_t H, int32_t W, int32_t row_begin, int32_t row_end
 	return SGR_OK;
 }
 
+// ---- the band losses' exchanges over peer memory ----
+size_t sgr_band_peer_bytes(int32_t C, int32_t H, int32_t W) {
+	if (C <= 0 || H <= 0 || W <= 0 || (int64_t)H * W >= ((int64_t)1 << 31)) return 0;
+	return band_peer_bytes(C, H, W);
+}
+
+// the peer table of the loss sections: world, rank and barrier pads, and every rank's section of at least `need` bytes
+static int loss_peers(const char *fn, const SgrPeers *peers, size_t need, PeerTable &pt, LossPeers &lp) {
+	if (!peers) return fail(SGR_EINVAL, "%s: peers is NULL", fn);
+	if (peers->world < 1 || peers->world > SGR_MAX_PEERS || peers->rank < 0 || peers->rank >= peers->world)
+		return fail(SGR_EINVAL, "%s: bad peer table: world=%d rank=%d (at most %d ranks)", fn, peers->world, peers->rank, SGR_MAX_PEERS);
+	pt.world = lp.world = peers->world;
+	pt.rank = peers->rank;
+	for (int p = 0; p < peers->world; p++) {
+		if (!peers->loss[p]) return fail(SGR_EINVAL, "%s: peer table entry %d has no loss section", fn, p);
+		if (peers->world > 1 && !peers->flags[p]) return fail(SGR_EINVAL, "%s: peer table entry %d has no barrier pad", fn, p);
+		lp.sec[p] = reinterpret_cast<char *>(peers->loss[p]);
+		pt.flags[p] = peers->flags[p];
+	}
+	if (peers->loss_bytes < need) return fail(SGR_ENOMEM, "%s: the loss sections hold %zu bytes, %zu needed", fn, peers->loss_bytes, need);
+	return SGR_OK;
+}
+
+int sgr_band_halo_exchange_peers(const SgrPeers *peers, int32_t C, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step,
+                                 const float *image, float *out, void *stream) {
+	const char *fn = "sgr_band_halo_exchange_peers";
+	Band band;
+	if (int rc = loss_band(fn, H, W, row_begin, row_end, row_step, &band)) return rc;
+	if (C <= 0) return fail(SGR_EINVAL, "%s: bad channel count %d", fn, C);
+	if (!image || !out) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	PeerTable pt = {};
+	LossPeers lp = {};
+	if (int rc = loss_peers(fn, peers, band_peer_bytes(C, H, W), pt, lp)) return rc;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_band_halo_exchange(pt, lp, C, H, W, band, image, out, st), fn);
+	return SGR_OK;
+}
+
+int sgr_band_peer_sum(const SgrPeers *peers, int32_t type, int64_t count, const void *local, void *out, void *stream) {
+	const char *fn = "sgr_band_peer_sum";
+	if (type != SGR_PEER_SUM_INT32 && type != SGR_PEER_SUM_FLOAT64) return fail(SGR_EINVAL, "%s: unknown element type %d", fn, type);
+	if (count < 0) return fail(SGR_EINVAL, "%s: negative count %lld", fn, (long long)count);
+	if (count > 0 && (!local || !out)) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	const size_t elem = type == SGR_PEER_SUM_INT32 ? sizeof(int32_t) : sizeof(double);
+	PeerTable pt = {};
+	LossPeers lp = {};
+	if (int rc = loss_peers(fn, peers, (size_t)count * elem, pt, lp)) return rc;
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_band_peer_sum(pt, lp, type == SGR_PEER_SUM_FLOAT64, count, local, out, st), fn);
+	return SGR_OK;
+}
+
 // ---- the sky composite and the colour correction on a tile-row band ----
 int sgr_band_sky_composite_forward(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t R, int32_t mode, float fill,
                                    const float *rgb, const float *acc, const uint8_t *sky_mask, const float *cube_map, const float *K,

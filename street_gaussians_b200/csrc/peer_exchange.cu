@@ -179,6 +179,80 @@ cudaError_t launch_peer_barrier(const PeerTable &pt, uint32_t epoch, uint32_t *s
 	return cudaGetLastError();
 }
 
+// ---- the band losses' exchanges (sgr_band_halo_exchange_peers / sgr_band_peer_sum) ----
+// A rank's loss section is [SEND_UP slot | SEND_DOWN slot] for the halo and [count elements] for a sum; the two never overlap in time
+// because each call ends with a barrier after which no peer reads the section any more.  A slot holds the largest message of any band:
+// with step >= 2 a band owns at most ceil(rows / 2) tile rows, each sending at most one strip per side; with step 1 one strip per side.
+size_t band_halo_slot_bytes(int C, int H, int W) {
+	const size_t rows = (size_t)(H + 15) / 16;
+	const size_t bytes = (size_t)C * kBandHalo * ((rows + 1) / 2) * (size_t)W * sizeof(float);
+	return (bytes + 255) / 256 * 256;
+}
+size_t band_peer_bytes(int C, int H, int W) {
+	const size_t rows = (size_t)(H + 15) / 16;
+	size_t sums = (size_t)SGR_LIDAR_LEVEL0_WORDS * 4;  // the largest of the summed arrays: LiDAR level-0 words, a level's
+	if ((size_t)SGR_LIDAR_BINS * 4 > sums) sums = (size_t)SGR_LIDAR_BINS * 4;  // histogram, the level-3 sums, the frame losses' partials
+	if ((1 + rows) * 8 > sums) sums = (1 + rows) * 8;
+	if (5 * 8 > sums) sums = 5 * 8;
+	const size_t halo = 2 * band_halo_slot_bytes(C, H, W);
+	return ((halo > sums ? halo : sums) + 255) / 256 * 256;
+}
+
+cudaError_t launch_band_halo_exchange(const PeerTable &pt, const LossPeers &lp, int C, int H, int W, Band band, const float *image, float *out,
+                                      cudaStream_t st) {
+	const size_t slot = band_halo_slot_bytes(C, H, W);
+	const int up = (pt.rank + pt.world - 1) % pt.world, down = (pt.rank + 1) % pt.world;
+	float *img = const_cast<float *>(image);
+	cudaError_t e = cudaSuccess;
+	if (pt.world > 1) {  // publish: the rows the neighbours need, in sgr_band_halo_pack's layout (an empty band has no message)
+		if ((e = launch_halo_copy(true, C, H, W, band, SGR_HALO_SEND_UP, img, reinterpret_cast<float *>(lp.sec[pt.rank]), st)) != cudaSuccess) return e;
+		if ((e = launch_halo_copy(true, C, H, W, band, SGR_HALO_SEND_DOWN, img, reinterpret_cast<float *>(lp.sec[pt.rank] + slot), st)) != cudaSuccess)
+			return e;
+	}
+	if ((e = launch_peer_barrier(pt, 0u, nullptr, st)) != cudaSuccess) return e;
+	if (pt.world > 1) {  // pull: the upper neighbour's SEND_DOWN is this rank's RECV_UP, the lower one's SEND_UP its RECV_DOWN
+		if ((e = launch_halo_copy(false, C, H, W, band, SGR_HALO_RECV_UP, out, reinterpret_cast<float *>(lp.sec[up] + slot), st)) != cudaSuccess) return e;
+		if ((e = launch_halo_copy(false, C, H, W, band, SGR_HALO_RECV_DOWN, out, reinterpret_cast<float *>(lp.sec[down]), st)) != cudaSuccess) return e;
+	}
+	return launch_peer_barrier(pt, 0u, nullptr, st);
+}
+
+// T: uint32_t for the int32 sums (wrap-around adds are the two's-complement ones), double for fp64
+template <typename T>
+__global__ void __launch_bounds__(256) loss_stage_kernel(const T *__restrict__ src, T *__restrict__ dst, const long long n) {
+	const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < n) dst[i] = src[i];
+}
+template <typename T>
+__global__ void __launch_bounds__(256) loss_sum_kernel(const LossPeers lp, const long long n, T *__restrict__ out) {
+	const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	T v = T(0);
+	for (int p = 0; p < lp.world; p++) v += reinterpret_cast<const T *>(lp.sec[p])[i];
+	out[i] = v;
+}
+
+template <typename T>
+static cudaError_t peer_sum(const PeerTable &pt, const LossPeers &lp, long long n, const T *local, T *out, cudaStream_t st) {
+	const unsigned nblk = (unsigned)((n + 255) / 256);
+	if (n > 0) {
+		count_launch();
+		loss_stage_kernel<T><<<nblk, 256, 0, st>>>(local, reinterpret_cast<T *>(lp.sec[pt.rank]), n);
+	}
+	cudaError_t e = launch_peer_barrier(pt, 0u, nullptr, st);
+	if (e != cudaSuccess) return e;
+	if (n > 0) {
+		count_launch();
+		loss_sum_kernel<T><<<nblk, 256, 0, st>>>(lp, n, out);
+	}
+	return launch_peer_barrier(pt, 0u, nullptr, st);
+}
+
+cudaError_t launch_band_peer_sum(const PeerTable &pt, const LossPeers &lp, bool f64, long long count, const void *local, void *out, cudaStream_t st) {
+	if (f64) return peer_sum<double>(pt, lp, count, static_cast<const double *>(local), static_cast<double *>(out), st);
+	return peer_sum<uint32_t>(pt, lp, count, static_cast<const uint32_t *>(local), static_cast<uint32_t *>(out), st);
+}
+
 cudaError_t launch_scatter_records(const FrameDev &f, const PeerTable &pt, const GaussRec *rec, const int32_t *radii, cudaStream_t st) {
 	if (pt.chunk == 0) return cudaSuccess;
 	count_launch();

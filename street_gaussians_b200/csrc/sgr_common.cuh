@@ -504,6 +504,16 @@ struct HaloStrips {
 HaloStrips halo_strips(int H, Band band, int side);
 int64_t halo_rows(int H, const HaloStrips &h);
 cudaError_t launch_halo_copy(bool pack, int C, int H, int W, Band band, int side, float *image, float *buf, cudaStream_t st);
+// the band losses' exchanges over peer memory (peer_exchange.cu): every rank's loss section (SgrPeers.loss)
+struct LossPeers {
+	int world;
+	char *sec[kMaxPeers];
+};
+size_t band_halo_slot_bytes(int C, int H, int W);
+size_t band_peer_bytes(int C, int H, int W);
+cudaError_t launch_band_halo_exchange(const PeerTable &pt, const LossPeers &lp, int C, int H, int W, Band band, const float *image, float *out,
+                                      cudaStream_t st);
+cudaError_t launch_band_peer_sum(const PeerTable &pt, const LossPeers &lp, bool f64, long long count, const void *local, void *out, cudaStream_t st);
 cudaError_t launch_image_loss_stats(int C, int H, int W, Band band, const float *img, const float *gt, const uint8_t *mask, double *acc,
                                     void *scratch, cudaStream_t st);
 cudaError_t launch_image_loss_grad(int C, int H, int W, Band band, const float *img, const float *gt, const uint8_t *mask, const double *acc,

@@ -63,18 +63,20 @@ class _ImageLoss(torch.autograd.Function):
         return (grad * g_out).to(ctx.in_dtype), None, None, None, None, None
 
 
-def _band_image(image, gt, mask, w_l1: float, w_ssim: float, band, group):
+def _band_image(image, gt, mask, w_l1: float, w_ssim: float, band, group, rasterizer):
     from . import band_losses
-    return band_losses._frame(image, gt, mask, w_l1, w_ssim, None, None, 0.0, None, None, 0.0, band, group)[0]
+    return band_losses._frame(image, gt, mask, w_l1, w_ssim, None, None, 0.0, None, None, 0.0, band, group, rasterizer)[0]
 
 
-def l1_loss(network_output, gt, mask=None, *, band=None, group=None):
+def l1_loss(network_output, gt, mask=None, *, band=None, group=None, rasterizer=None):
     """mean |network_output - gt| over the masked pixels (all pixels without a mask); inputs [C, H, W], mask [1, H, W] bool.
 
     band= / group=: network_output holds the rendered rows of this rank's TileRowBand (sharded.py); COLLECTIVE over `group`, the value
-    is the whole frame's on every rank and the gradient covers the band's rows (band_losses.py)."""
-    if band is not None:
-        return _band_image(network_output, gt, mask, 1.0, 0.0, band, group)
+    is the whole frame's on every rank and the gradient covers the band's rows (band_losses.py).  rasterizer= (the
+    GaussianShardedRasterizer that rendered the rows): its band, and with exchange="p2p" the halo and the sums over its peer workspace
+    (band_losses.resolve)."""
+    if band is not None or rasterizer is not None:
+        return _band_image(network_output, gt, mask, 1.0, 0.0, band, group, rasterizer)
     return _ImageLoss.apply(network_output, gt, mask, 1.0, 0.0, 0)
 
 
@@ -86,21 +88,21 @@ def l2_loss(network_output, gt, mask=None):
     return ((a - b) ** 2).mean()
 
 
-def ssim(img1, img2, window_size=11, size_average=True, mask=None, *, band=None, group=None):
+def ssim(img1, img2, window_size=11, size_average=True, mask=None, *, band=None, group=None, rasterizer=None):
     """Mean SSIM with the reference's 11x11 / sigma 1.5 Gaussian window, zero padding and masking convention.  band= / group= as l1_loss's
-    (img1 is the rendered image: its halo rows come from the ranks owning them)."""
+    (img1 is the rendered image: its halo rows come from the ranks owning them); rasterizer= as l1_loss's."""
     if window_size != 11 or not size_average:
         raise _capi.SgrError("the fused SSIM implements the configuration the reference trains with: window_size=11, size_average=True")
-    if band is not None:
-        return _band_image(img1, img2, mask, 0.0, 1.0, band, group)
+    if band is not None or rasterizer is not None:
+        return _band_image(img1, img2, mask, 0.0, 1.0, band, group, rasterizer)
     return _ImageLoss.apply(img1, img2, mask, 0.0, 1.0, 0)
 
 
-def photometric_loss(image, gt, mask=None, lambda_l1: float = 1.0, lambda_dssim: float = 0.2, *, band=None, group=None):
+def photometric_loss(image, gt, mask=None, lambda_l1: float = 1.0, lambda_dssim: float = 0.2, *, band=None, group=None, rasterizer=None):
     """(1 - lambda_dssim) * lambda_l1 * L1 + lambda_dssim * (1 - SSIM)   (train.py:101-104), one fused evaluation.  band= / group= as
-    l1_loss's; band_losses.frame_losses evaluates it with the sky and object-accumulation losses under one all-reduce."""
-    if band is not None:
-        return _band_image(image, gt, mask, (1.0 - lambda_dssim) * lambda_l1, -lambda_dssim, band, group) + lambda_dssim
+    l1_loss's (and rasterizer=); band_losses.frame_losses evaluates it with the sky and object-accumulation losses under one all-reduce."""
+    if band is not None or rasterizer is not None:
+        return _band_image(image, gt, mask, (1.0 - lambda_dssim) * lambda_l1, -lambda_dssim, band, group, rasterizer) + lambda_dssim
     return _ImageLoss.apply(image, gt, mask, (1.0 - lambda_dssim) * lambda_l1, -lambda_dssim, 0) + lambda_dssim
 
 
@@ -131,22 +133,23 @@ class _AccLoss(torch.autograd.Function):
         return (grad * g_out).to(ctx.in_dtype), None, None, None
 
 
-def sky_loss(acc, sky_mask, weight: float = 1.0, *, band=None, group=None):
+def sky_loss(acc, sky_mask, weight: float = 1.0, *, band=None, group=None, rasterizer=None):
     """weight * mean( sky ? -log(1 - acc) : -log(acc) ) with acc clamped to [1e-6, 1 - 1e-6]   (train.py:107-113).  band= / group= as
-    l1_loss's, acc [1, H, W]."""
-    if band is not None:
+    l1_loss's (and rasterizer=), acc [1, H, W]."""
+    if band is not None or rasterizer is not None:
         from . import band_losses
-        return band_losses.frame_losses(acc=acc, sky_mask=sky_mask, sky_weight=weight, band=band, group=group)["sky"]
+        return band_losses.frame_losses(acc=acc, sky_mask=sky_mask, sky_weight=weight, band=band, group=group, rasterizer=rasterizer)["sky"]
     return _AccLoss.apply(acc, sky_mask, weight, "sgr_sky_loss")
 
 
-def obj_acc_loss(acc_obj, obj_bound, weight: float = 1.0, *, band=None, group=None):
+def obj_acc_loss(acc_obj, obj_bound, weight: float = 1.0, *, band=None, group=None, rasterizer=None):
     """weight * mean( obj_bound ? -(a log a + (1 - a) log(1 - a)) : -log(1 - a) ), a = acc_obj clamped to [1e-6, 1 - 1e-6]
     (train.py:114-122).  acc_obj is the accumulation of the objects-only render (render_object), [1, H, W]; obj_bound bool [1, H, W].
-    band= / group= as l1_loss's."""
-    if band is not None:
+    band= / group= / rasterizer= as l1_loss's."""
+    if band is not None or rasterizer is not None:
         from . import band_losses
-        return band_losses.frame_losses(acc_obj=acc_obj, obj_bound=obj_bound, obj_weight=weight, band=band, group=group)["obj_acc"]
+        return band_losses.frame_losses(acc_obj=acc_obj, obj_bound=obj_bound, obj_weight=weight, band=band, group=group,
+                                        rasterizer=rasterizer)["obj_acc"]
     return _AccLoss.apply(acc_obj, obj_bound, weight, "sgr_obj_acc_loss")
 
 
@@ -186,7 +189,8 @@ class _LidarDepthLoss(torch.autograd.Function):
         return gd, ga, None, None, None, None
 
 
-def lidar_depth_loss(depth, acc, lidar_depth, mask=None, weight: float = 1.0, keep: float = 0.95, *, band=None, group=None):
+def lidar_depth_loss(depth, acc, lidar_depth, mask=None, weight: float = 1.0, keep: float = 0.95, *, band=None, group=None,
+                     rasterizer=None):
     """weight * mean of the int(keep * n) smallest |depth / (acc + 1e-10) - lidar_depth| over the n pixels with lidar_depth > 0 and
     mask (train.py:124-132); depth, acc, lidar_depth [1, H, W], mask bool [1, H, W] or None.
 
@@ -196,8 +200,9 @@ def lidar_depth_loss(depth, acc, lidar_depth, mask=None, weight: float = 1.0, ke
     k == 0 (fewer than two valid pixels at keep = 0.95) the value is NaN and both gradients are zero, like the reference.
 
     band= / group=: depth and acc hold the rendered rows of this rank's TileRowBand; COLLECTIVE over `group` (four small all-reduces of
-    the select's histograms and sums), the selected pixels and the value are the whole frame's (band_losses.py)."""
-    if band is not None:
+    the select's histograms and sums), the selected pixels and the value are the whole frame's (band_losses.py).  rasterizer= as
+    l1_loss's: with exchange="p2p" the four sums go over its peer workspace."""
+    if band is not None or rasterizer is not None:
         from . import band_losses
-        return band_losses.lidar_depth_loss(depth, acc, lidar_depth, mask, weight, keep, band=band, group=group)
+        return band_losses.lidar_depth_loss(depth, acc, lidar_depth, mask, weight, keep, band=band, group=group, rasterizer=rasterizer)
     return _LidarDepthLoss.apply(depth, acc, lidar_depth, mask, weight, keep)

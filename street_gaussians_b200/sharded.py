@@ -214,8 +214,8 @@ def _align(n: int, a: int = 256) -> int:
 
 
 class PeerWorkspace:
-    """Per-rank buffer [geom_state | radii_all | grad2d | sem | gsem | pose_acc | barrier pad] that every rank of the group can address
-    (include/sgr.h, SgrPeers).
+    """Per-rank buffer [geom_state | radii_all | grad2d | sem | gsem | pose_acc | loss | barrier pad] that every rank of the group can
+    address (include/sgr.h, SgrPeers).
 
     Real multi-GPU: ONE torch symmetric-memory allocation per rank (CUDA VMM mapped into every process; NVLink loads and
     stores), rendezvous'ed once; `barrier()` is the device-side signal-pad barrier of that allocation (a few microseconds
@@ -231,6 +231,7 @@ class PeerWorkspace:
                                                                                                                  self.S)
         self.off_sem, self.off_gsem = self.feature_offsets(self.off_grad, self.P_total, self.S)
         self.off_pose = self.pose_offset(self.off_grad, self.P_total, self.S)
+        self.off_loss, self.loss_bytes = self.loss_offset(self.off_grad, self.P_total, self.S), self.loss_section_bytes(settings)
         self.hdl = None
         self.in_flight = False  # a differentiable forward has used the buffers and its backward has not run yet
         self.epoch = 0          # epoch of the last sgr_peer_barrier issued on this workspace (every rank counts alike)
@@ -263,6 +264,8 @@ class PeerWorkspace:
                 self.peers.sem[p] = ptrs[p] + self.off_sem
                 self.peers.gsem[p] = ptrs[p] + self.off_gsem
             self.peers.pose_acc[p] = ptrs[p] + self.off_pose
+            self.peers.loss[p] = ptrs[p] + self.off_loss
+        self.peers.loss_bytes = self.loss_bytes
         nsem = self.P_total * self.S
         self.sem = self.buf[self.off_sem: self.off_sem + 4 * nsem].view(torch.float32).view(self.P_total, self.S)
         self.gsem = self.buf[self.off_gsem: self.off_gsem + 4 * nsem].view(torch.float32).view(self.P_total, self.S)
@@ -280,17 +283,32 @@ class PeerWorkspace:
         return _align(PeerWorkspace.feature_offsets(off_grad, P_total, S)[1] + 4 * P_total * S)
 
     @staticmethod
+    def loss_offset(off_grad: int, P_total: int, S: int) -> int:
+        """Offset of the band losses' section (band_losses.py's peer-memory halo and sums), after the composer's accumulator section
+        and before the barrier pad."""
+        return _align(PeerWorkspace.pose_offset(off_grad, P_total, S) + 64 * _capi.POSE_ACC_ROWS)
+
+    @staticmethod
+    def loss_section_bytes(settings) -> int:
+        """Bytes of the band losses' section for the settings' image: sgr_band_peer_bytes of a 3-channel image (the largest pair of
+        halo messages any band sends, or the largest array the losses sum)."""
+        n = int(_capi.lib().sgr_band_peer_bytes(3, int(settings.image_height), int(settings.image_width)))
+        if n == 0:
+            raise _capi.SgrError(f"bad image size {settings.image_width}x{settings.image_height} for the band losses' section")
+        return n
+
+    @staticmethod
     def layout(settings, P_total: int, device, S: int = 0):
         """(geom_bytes, img_bytes, offset of radii_all, offset of grad2d, offset of the barrier pad, total bytes) of the per-rank buffer.
         With S feature channels the sections sem and gsem (feature_offsets) sit before the pad; S = 0 leaves them empty.  The composer's
-        accumulator section (pose_offset) follows them."""
+        accumulator section (pose_offset) follows them, then the band losses' section (loss_offset, loss_section_bytes)."""
         fr, keep = _make_frame(settings, P_total, 0, 0, device, None)
         gb, ib = C.c_size_t(0), C.c_size_t(0)
         _capi.call("sgr_state_sizes", None, C.byref(fr), C.byref(gb), C.byref(ib))
         del keep
         off_radii = _align(gb.value)
         off_grad = _align(off_radii + 4 * P_total)
-        off_flags = _align(PeerWorkspace.pose_offset(off_grad, P_total, S) + 64 * _capi.POSE_ACC_ROWS)
+        off_flags = _align(PeerWorkspace.loss_offset(off_grad, P_total, S) + PeerWorkspace.loss_section_bytes(settings))
         return gb.value, ib.value, off_radii, off_grad, off_flags, off_flags + 256
 
     @classmethod
@@ -614,6 +632,14 @@ class GaussianShardedRasterizer(nn.Module):
         if self._ws is None:
             raise _capi.SgrError("compose(rasterizer=...) with exchange='p2p' sums over the rasterizer's peer workspace: run the "
                                  "rasterizer's forward before the composer's backward")
+        return self._ws
+
+    def loss_workspace(self) -> "PeerWorkspace":
+        """The peer workspace the band losses (band_losses.frame_losses / lidar_depth_loss with rasterizer=self) exchange their halo and
+        partial sums through (exchange="p2p"): the one this module's forward set up, in its loss section."""
+        if self._ws is None:
+            raise _capi.SgrError("the band losses with rasterizer= and exchange='p2p' exchange over the rasterizer's peer workspace: run "
+                                 "the rasterizer's forward before the losses")
         return self._ws
 
     def release_workspace(self):

@@ -24,6 +24,11 @@ global arrays each rank restates.  It has run at world 1 only, not on several H1
 With the argument `compose` (NCCL all_reduce of the accumulator rows) or `compose-p2p` (the rasterizer's peer workspace) only the composer
 leg runs (run_compose): compose(..., group= / rasterizer=) on each rank's rows of a config-C-like scene, before and after the rebalanced
 split.  It has run at world 1 only, not on several H100s; tests/test_sharded_compose_gpu.py emulates 2 to 8 ranks on one GPU.
+
+With the argument `losses-p2p` only the loss leg runs, through the p2p rasterizer: frame_losses / the losses.py wrappers with rasterizer=,
+so the halo and the sums go over its peer workspace (sgr_band_halo_exchange_peers / sgr_band_peer_sum).  Each rank's values must be the
+same bytes on every rank and the whole frame's, and its gradient rows bit-equal to the single-GPU losses'.  It has run at world 1 only,
+not on several H100s; tests/test_band_losses_p2p_gpu.py emulates 2 to 8 ranks on one GPU.
 """
 import os
 import sys
@@ -117,12 +122,14 @@ def run_case(rank, world, dev, S, P, W, H, bounded, exchange="nccl"):
     return worst, floor
 
 
-def run_losses(rank, world, dev, W=1280, H=720):
-    """Loss leg: each rank's band losses (band_losses.py) on its banded render against the single-GPU losses of the gathered frame."""
+def run_losses(rank, world, dev, W=1280, H=720, exchange="nccl"):
+    """Loss leg: each rank's band losses (band_losses.py) on its banded render against the single-GPU losses of the gathered frame.
+    exchange="p2p": the losses take rasterizer= of the p2p rasterizer that rendered the rows (halo and sums over its peer workspace), and
+    the values must also be the same bytes on every rank."""
     from street_gaussians_b200 import band_losses, losses
     scene = synthetic.make_scene(P=60_001, width=W, height=H, sh_degree=3, seed=78, pose=True)
     st = util.settings_from(sgb, scene["cam"], dev)
-    rast = GaussianShardedRasterizer(st)
+    rast = GaussianShardedRasterizer(st, exchange=exchange)
     P = scene["means3D"].shape[0]
     chunk = (P + world - 1) // world
     lo, hi = min(P, rank * chunk), min(P, (rank + 1) * chunk)
@@ -148,12 +155,23 @@ def run_losses(rank, world, dev, W=1280, H=720):
         v.backward()
         return v.detach(), [x.grad for x in xs]
 
-    checks = (("photometric", lambda x, b=None, gr=None: losses.photometric_loss(x, gt, mask, band=b, group=gr), (0,)),
-              ("sky", lambda a, b=None, gr=None: losses.sky_loss(a, sky, band=b, group=gr), (2,)),
-              ("lidar", lambda d, a, b=None, gr=None: losses.lidar_depth_loss(d, a, lidar, mask, band=b, group=gr), (1, 2)))
+    obj = torch.rand(1, H, W, device=dev, generator=g) > 0.7
+    frame = lambda x, a, **kw: sum(band_losses.frame_losses(x, gt, mask, acc=a, sky_mask=sky, acc_obj=a, obj_bound=obj, **kw).values())
+    checks = (("photometric", lambda x, **kw: losses.photometric_loss(x, gt, mask, **kw), (0,)),
+              ("sky", lambda a, **kw: losses.sky_loss(a, sky, **kw), (2,)),
+              ("lidar", lambda d, a, **kw: losses.lidar_depth_loss(d, a, lidar, mask, **kw), (1, 2)),
+              ("frame", lambda x, a, **kw: frame(x, a, **kw) if kw else (losses.photometric_loss(x, gt, mask) + losses.sky_loss(a, sky) +
+                                                                         losses.obj_acc_loss(a, obj)), (0, 2)))
+    how = dict(rasterizer=rast) if exchange == "p2p" else dict(band=band, group=None)
     for name, fn, which in checks:
+        if name == "frame" and exchange != "p2p":
+            continue
         v_ref, g_ref = grads(fn, *(full[i] for i in which))
-        v, g_band = grads(lambda *xs: fn(*xs, b=band, gr=None), *((color, depth, acc)[i] for i in which))
+        v, g_band = grads(lambda *xs: fn(*xs, **how), *((color, depth, acc)[i] for i in which))
+        if exchange == "p2p" and world > 1:
+            alls = [torch.empty_like(v.reshape(1)) for _ in range(world)]
+            dist.all_gather(alls, v.reshape(1))
+            assert all(torch.equal(t, v.reshape(1)) for t in alls), f"{name}: values differ across ranks"
         a, b = float(v), float(v_ref)
         assert (a != a and b != b) or abs(a - b) <= 4e-6 * abs(b), (name, a, b)
         for x, y in zip(g_band, g_ref):
@@ -436,7 +454,11 @@ def main():
     ok = True
     try:
         mode = sys.argv[1] if len(sys.argv) > 1 else "nccl"
-        if mode in ("compose", "compose-p2p"):
+        if mode == "losses-p2p":
+            run_losses(rank, world, dev, exchange="p2p")
+            print(f"[rank {rank}/{world}] band losses over peer memory: the same values on every rank, the frame's, gradient rows bit-equal "
+                  "to the single-GPU losses", flush=True)
+        elif mode in ("compose", "compose-p2p"):
             P = run_compose(rank, world, dev, "p2p" if mode == "compose-p2p" else "nccl")
             print(f"[rank {rank}/{world}] compose ({mode}): {P} Gaussians, own rows bit-equal, dL/dposes and dL/dcorrection the same bytes on "
                   "every rank and the frame's", flush=True)
