@@ -375,6 +375,59 @@ int sgr_sharded_backward_features(const SgrFrame *frame, const SgrPeers *peers, 
                                   float *dL_dscales, float *dL_drotations, float *dL_dcov3D, uint32_t barrier_epoch,
                                   const float *dL_dsemantic, float *dL_dsemantics, void *stream);
 
+/* Render layers in the fused Gaussian-sharded step: row ranges of THIS rank's Gaussians rendered on this rank's band from the tile lists
+ * of the same call, as sgr_forward_layer does on one GPU.  The tile lists hold slots, which do not give back an owner's row, so layer
+ * membership travels with the record: the owner writes one byte per Gaussian (bit k = layer k) by the same block runs into the same
+ * slot of layer_peers->layer_mask[d], before the forward's barrier.  Each layer's lists are compacted out of the main lists by that bit, so a
+ * rank's layer image equals the band rows of one GPU's separate call on the rank-major concatenation of every rank's layer rows (a
+ * layer empty on this rank still shows the other ranks' rows; empty everywhere: colour bg, zero depth and alpha).  Every rank passes
+ * the same number of layers (at most SGR_MAX_SHARDED_LAYERS) with the same bg; S must be 0.
+ *   sgr_sharded_layer_state_sizes : bytes of ONE layer's caller-owned state (frame.P = local count, `capacity` as in sgr_sharded_forward):
+ *                                   its tile lists and contributor counts, and room for the backward's scratch rows (60 B per local
+ *                                   Gaussian, used in the first layer's state).  Kept from the forward to its backward.
+ *   sgr_sharded_forward_layers    : sgr_sharded_forward plus the layers' images: the band's rows are written, the others left alone.
+ *   sgr_sharded_backward_layers   : sgr_sharded_backward plus the layers' gradients.  Each layer with a gradient is blended backward by
+ *                                   slot into its part of this rank's layer_grad2d section (the rows of the slots delivered here are
+ *                                   zeroed first); after the backward's barrier each owner sums its rows of the main section and of every
+ *                                   layer's from the ranks that rendered them, in ascending rank order, as the same runs, and the chain
+ *                                   rule runs once on main + layers (as sgr_backward_geom_layered), while dL_dmeans2D gets the main sums
+ *                                   only and each layer's sink its own [0:3].  With no layer gradient the call is sgr_sharded_backward.
+ * layers: HOST table.  No NCCL, no host read-back, no extra barrier; grids depend on the tile count and chunk only, so the layered step
+ * captures in a CUDA graph.  Every argument is checked before anything is enqueued.
+ * Every rank must give the same layers an upstream gradient (or none): an owner gathers the layer rows of the other ranks only for the
+ * layers that have a gradient on its own call, so a layer with a gradient on one rank and none on another loses that rank's share. */
+#define SGR_MAX_SHARDED_LAYERS 2
+typedef struct SgrLayerPeers {        /* the layer sections of every rank of the SgrPeers table, mapped into every rank like its arrays */
+	int32_t layers;                     /* L: layers every rank's layer_grad2d section holds (SGR_EINVAL when num_layers > L)       */
+	int32_t reserved;
+	uint8_t *layer_mask[SGR_MAX_PEERS]; /* rank p's layer_mask[world*chunk]: bit k = layer k, rows by slot like the records           */
+	float *layer_grad2d[SGR_MAX_PEERS]; /* rank p's layer_grad2d[L, world*chunk, 12] (L >= num_layers): its partial layer rows by slot,
+	                                       layer k at k*world*chunk*12 floats                                                           */
+} SgrLayerPeers;
+typedef struct SgrShardedLayer {
+	int32_t begin, end;           /* 0 <= begin <= end <= frame.P (this rank's rows)                                          */
+	const float *bg;              /* [3] device                                                                                */
+	void *state;                  /* sgr_sharded_layer_state_sizes bytes, device                                               */
+	size_t state_bytes;
+	float *color, *depth, *alpha; /* [3,H,W], [1,H,W], [1,H,W] device: forward outputs (the backward reads alpha)              */
+	const float *dL_dcolor, *dL_ddepth, *dL_dalpha;  /* backward: upstream gradients of the three images, all NULL = none          */
+	float *dL_dmeans2D;           /* backward: [end-begin, 3] device or NULL: the layer's own screen-space gradient             */
+} SgrShardedLayer;
+int sgr_sharded_layer_state_sizes(const SgrFrame *frame, int64_t capacity, size_t *layer_bytes);
+int sgr_sharded_forward_layers(const SgrFrame *frame, const SgrPeers *peers, const float *means3D, const float *shs, const float *colors_precomp,
+                               const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp, float *out_color,
+                               float *out_depth, float *out_alpha, int32_t *radii_local, void *records_local, size_t geom_bytes, void *img_state,
+                               size_t img_bytes, void *binning_state, size_t binning_bytes, int64_t capacity, int64_t gaussian_capacity,
+                               uint32_t barrier_epoch, int32_t pre_barrier, const SgrLayerPeers *layer_peers, const SgrShardedLayer *layers,
+                               int32_t num_layers, void *stream);
+int sgr_sharded_backward_layers(const SgrFrame *frame, const SgrPeers *peers, int64_t capacity, const float *means3D, const float *shs,
+                                const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                                const int32_t *radii_local, const void *records_local, const void *img_state, const void *binning_state,
+                                const float *out_alpha, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                                float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors_precomp, float *dL_dopacity,
+                                float *dL_dscales, float *dL_drotations, float *dL_dcov3D, uint32_t barrier_epoch, const SgrLayerPeers *layer_peers,
+                                const SgrShardedLayer *layers, int32_t num_layers, void *stream);
+
 /* ---- Scene-graph composer (SURVEY.md §8 row f1; no native counterpart in the reference, which composes with ~40 PyTorch kernels) ----
  * One call builds the rasterizer's inputs from the raw parameters of every sub-model of the scene graph, as
  * StreetGaussianModel.get_xyz / get_rotation / get_scaling / get_opacity / get_features do

@@ -21,6 +21,7 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_set_nea
            "sgr_knn_mean_dist2", "sgr_record_bytes", "sgr_project", "sgr_forward_records",
            "sgr_scatter_records", "sgr_gather_grad2d", "sgr_peer_barrier", "sgr_sharded_forward", "sgr_sharded_backward",
            "sgr_sharded_forward_features", "sgr_sharded_backward_features",
+           "sgr_sharded_layer_state_sizes", "sgr_sharded_forward_layers", "sgr_sharded_backward_layers",
            "sgr_compose_forward", "sgr_compose_backward", "sgr_image_loss_scratch_bytes", "sgr_image_loss", "sgr_sky_loss",
            "sgr_obj_acc_loss", "sgr_lidar_depth_loss_scratch_bytes", "sgr_lidar_depth_loss", "sgr_densify_stats", "sgr_adam_step",
            "sgr_densify_scratch_bytes", "sgr_densify_plan", "sgr_densify_apply", "sgr_reset_opacity", "sgr_rebalance_row_floats",
@@ -142,6 +143,19 @@ class SgrLayer(C.Structure):
     _fields_ = [("begin", C.c_int32), ("end", C.c_int32), ("bg", C.c_void_p)]
 
 
+MAX_SHARDED_LAYERS = 2  # SGR_MAX_SHARDED_LAYERS: render layers of the fused Gaussian-sharded step
+
+
+class SgrLayerPeers(C.Structure):
+    _fields_ = [("layers", C.c_int32), ("reserved", C.c_int32), ("layer_mask", C.c_void_p * MAX_PEERS), ("layer_grad2d", C.c_void_p * MAX_PEERS)]
+
+
+class SgrShardedLayer(C.Structure):
+    _fields_ = [("begin", C.c_int32), ("end", C.c_int32), ("bg", C.c_void_p), ("state", C.c_void_p), ("state_bytes", C.c_size_t),
+                ("color", C.c_void_p), ("depth", C.c_void_p), ("alpha", C.c_void_p), ("dL_dcolor", C.c_void_p), ("dL_ddepth", C.c_void_p),
+                ("dL_dalpha", C.c_void_p), ("dL_dmeans2D", C.c_void_p)]
+
+
 class SgrLayerGrad(C.Structure):
     _fields_ = [("begin", C.c_int32), ("end", C.c_int32), ("grad2d", C.c_void_p), ("dL_dmeans2D", C.c_void_p)]
 
@@ -228,6 +242,12 @@ def lib():
     L.sgr_sharded_forward_features.argtypes = L.sgr_sharded_forward.argtypes[:-1] + [vp, vp, vp]
     L.sgr_sharded_backward_features.restype = C.c_int
     L.sgr_sharded_backward_features.argtypes = L.sgr_sharded_backward.argtypes[:-1] + [vp, vp, vp]
+    L.sgr_sharded_layer_state_sizes.restype = C.c_int
+    L.sgr_sharded_layer_state_sizes.argtypes = [C.POINTER(SgrFrame), C.c_int64, C.POINTER(C.c_size_t)]
+    L.sgr_sharded_forward_layers.restype = C.c_int
+    L.sgr_sharded_forward_layers.argtypes = L.sgr_sharded_forward.argtypes[:-1] + [C.POINTER(SgrLayerPeers), C.POINTER(SgrShardedLayer), C.c_int32, vp]
+    L.sgr_sharded_backward_layers.restype = C.c_int
+    L.sgr_sharded_backward_layers.argtypes = L.sgr_sharded_backward.argtypes[:-1] + [C.POINTER(SgrLayerPeers), C.POINTER(SgrShardedLayer), C.c_int32, vp]
     L.sgr_compose_forward.restype = C.c_int
     L.sgr_compose_forward.argtypes = [C.POINTER(SgrSegment), C.c_int32, C.c_int32] + [vp] * 10
     L.sgr_compose_backward.restype = C.c_int

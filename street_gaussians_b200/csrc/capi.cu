@@ -446,6 +446,74 @@ int sgr_peer_barrier(const SgrPeers *peers, uint32_t epoch, void *stream) {
 	return SGR_OK;
 }
 
+// layer state: the img-state layout (ranges, tile_max_contrib, n_contrib) of the layer, then its tile lists u32[num_instances]
+struct LayerView {
+	ImgView img;
+	uint32_t *list;
+	size_t total_bytes;
+};
+static LayerView carve_layer(void *base, int W, int H, int64_t R) {
+	LayerView v;
+	v.img = carve_img(base, W, H, false);
+	char *p = reinterpret_cast<char *>(base) + v.img.total_bytes;
+	v.list = take<uint32_t>(p, R > 0 ? (size_t)R : 1);
+	v.total_bytes = (size_t)(p - reinterpret_cast<char *>(base));
+	return v;
+}
+// a layer of the fused Gaussian-sharded step: carve_layer's lists for `capacity` instances, then the backward's scratch rows of the P local
+// Gaussians (the summed main + layer rows [P, 12] the chain rule reads, and [P, 3] for the dL/dmeans2D it writes from them)
+struct ShardedLayerView {
+	LayerView lv;
+	float *rows, *means2D;
+	size_t total_bytes;
+};
+static ShardedLayerView carve_sharded_layer(void *base, int W, int H, int64_t capacity, int P) {
+	ShardedLayerView v;
+	v.lv = carve_layer(base, W, H, capacity);
+	char *p = reinterpret_cast<char *>(base) + v.lv.total_bytes;
+	const size_t n = P > 0 ? (size_t)P : 1;
+	v.rows = take<float>(p, 12 * n);
+	v.means2D = take<float>(p, 3 * n);
+	v.total_bytes = (size_t)(p - reinterpret_cast<char *>(base));
+	return v;
+}
+
+// the layer table of sgr_sharded_forward_layers / sgr_sharded_backward_layers, checked before the main call's arguments
+static int check_sharded_layers(const char *fn, const SgrFrame *frame, const SgrShardedLayer *layers, int32_t n, int64_t capacity, bool backward) {
+	if (!frame) return fail(SGR_EINVAL, "frame is NULL");
+	if (!layers) return fail(SGR_EINVAL, "%s: layer table is NULL", fn);
+	if (n < 1 || n > SGR_MAX_SHARDED_LAYERS) return fail(SGR_EINVAL, "%s: %d layers (1 to %d)", fn, n, SGR_MAX_SHARDED_LAYERS);
+	if (frame->S != 0) return fail(SGR_EINVAL, "%s: layers take no feature channels (S = %d)", fn, frame->S);
+	if (frame->width <= 0 || frame->height <= 0 || frame->P < 0) return fail(SGR_EINVAL, "bad sizes P=%d W=%d H=%d", frame->P, frame->width, frame->height);
+	if (capacity < 0 || capacity > 0x7fffffffLL) return fail(SGR_EINVAL, "capacity must be in [0, 2^31)");
+	const size_t need = carve_sharded_layer(nullptr, frame->width, frame->height, capacity, frame->P).total_bytes;
+	for (int k = 0; k < n; k++) {
+		const SgrShardedLayer &l = layers[k];
+		if (l.begin < 0 || l.begin > l.end || l.end > frame->P)
+			return fail(SGR_EINVAL, "%s: bad layer %d range [%d, %d) for %d local Gaussians", fn, k, l.begin, l.end, frame->P);
+		if (!l.bg) return fail(SGR_EINVAL, "%s: layer %d bg is NULL", fn, k);
+		if (!l.state) return fail(SGR_EINVAL, "%s: layer %d state is NULL", fn, k);
+		if (l.state_bytes < need) return fail(SGR_ENOMEM, "%s: layer %d state too small: %zu < %zu", fn, k, l.state_bytes, need);
+		if (!l.alpha || (!backward && (!l.color || !l.depth))) return fail(SGR_EINVAL, "%s: layer %d image pointer is NULL", fn, k);
+		const int given = (l.dL_dcolor != nullptr) + (l.dL_ddepth != nullptr) + (l.dL_dalpha != nullptr);
+		if (backward && given != 0 && given != 3)
+			return fail(SGR_EINVAL, "%s: layer %d has %d of its 3 upstream gradients (all or none)", fn, k, given);
+	}
+	return SGR_OK;
+}
+// both directions use every section: the forward writes the masks and clears its own layer rows, the backward writes and reads the rows
+static int layer_peers(const SgrLayerPeers *peers, const PeerTable &pt, int nl) {
+	if (!peers) return fail(SGR_EINVAL, "layer_peers is NULL");
+	if (peers->layers < nl) return fail(SGR_EINVAL, "the layer sections hold %d layers, the call has %d", peers->layers, nl);
+	for (int p = 0; p < pt.world; p++)
+		if (!peers->layer_mask[p] || !peers->layer_grad2d[p]) return fail(SGR_EINVAL, "peer table entry %d has no layer section", p);
+	return SGR_OK;
+}
+// layer k's rows of rank p: its part of p's layer_grad2d section
+static float *layer_section(const SgrLayerPeers *peers, int p, int k, const FrameDev &ft) {
+	return peers->layer_grad2d[p] + (size_t)k * (size_t)ft.P * 12;
+}
+
 // FrameDev of the gathered problem (all world*chunk slots) seen through this rank's band
 static int make_total_frame(const SgrFrame *frame, const SgrPeers *peers, FrameDev &fl, FrameDev &ft, PeerTable &pt, bool need_grad,
                             SemPeers *sp = nullptr) {
@@ -482,11 +550,12 @@ static int sharded_forward(const SgrFrame *frame, const SgrPeers *peers, const f
                            float *out_depth, float *out_alpha, int32_t *radii_local, void *records_local, size_t geom_bytes, void *img_state,
                            size_t img_bytes, void *binning_state, size_t binning_bytes, int64_t capacity, int64_t gaussian_capacity,
                            uint32_t barrier_epoch, int32_t pre_barrier, SemPeers *sp, const float *semantics, float *out_semantic,
-                           void *stream) {
+                           void *stream, const SgrLayerPeers *lpeers = nullptr, const SgrShardedLayer *layers = nullptr, int nl = 0) {
 	FrameDev fl, ft;
 	PeerTable pt = {};
 	int rc = make_total_frame(frame, peers, fl, ft, pt, false, sp);
 	if (rc) return rc;
+	if (nl && (rc = layer_peers(lpeers, pt, nl)) != SGR_OK) return rc;
 	if (sp && (!out_semantic || (fl.P > 0 && !semantics))) return fail(SGR_EINVAL, "semantics / out_semantic is NULL");
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 	const bool debug = frame->debug != 0;
@@ -515,6 +584,13 @@ static int sharded_forward(const SgrFrame *frame, const SgrPeers *peers, const f
 	                               (size_t)(reinterpret_cast<char *>(g.iota) - reinterpret_cast<char *>(geom_state)), st),
 	        "project+scatter");
 	if (sp) SGR_TRY(launch_scatter_semantics(pt, *sp, fl.P, fl.S, g.depth_key, semantics, st), "scatter semantics");
+	LayerPeers lp = {};
+	if (nl) {  // layer membership travels with the records, before the barrier
+		for (int p = 0; p < pt.world; p++) lp.mask[p] = lpeers->layer_mask[p];
+		lp.n = nl;
+		for (int k = 0; k < nl; k++) { lp.begin[k] = layers[k].begin; lp.end[k] = layers[k].end; }
+		SGR_TRY(launch_scatter_layer_mask(pt, lp, fl.P, g.depth_key, st), "scatter layer mask");
+	}
 	if (ft.P == 0) return SGR_OK;
 	SGR_TRY(cudaMemsetAsync(g.big_count, 0, 64 * sizeof(uint32_t), st), "status reset");
 	SGR_TRY(launch_peer_barrier(pt, barrier_epoch, g.big_count, st), "barrier");
@@ -525,6 +601,21 @@ static int sharded_forward(const SgrFrame *frame, const SgrPeers *peers, const f
 	SGR_TRY(launch_binning(ft, g, pt.radii[pt.rank], b, img, capacity, st, capacity, n_order), "binning");
 	SGR_TRY(launch_blend_fwd(ft, g, b, img, sp ? sp->sem[pt.rank] : nullptr, out_color, out_depth, out_alpha, sp ? out_semantic : nullptr, st),
 	        "blend_fwd");
+	if (nl) {
+		LayerRows zr = {};
+		zr.n = nl;
+		for (int k = 0; k < nl; k++) zr.rows[k] = layer_section(lpeers, pt.rank, k, ft);
+		SGR_TRY(launch_layer_zero_rows(g, n_order, zr, st), "layer rows reset");
+		for (int k = 0; k < nl; k++) {
+			const LayerView lv = carve_sharded_layer(layers[k].state, ft.W, ft.H, capacity, fl.P).lv;
+			SGR_TRY(launch_layer_lists_masked(ft, img, b, lp.mask[pt.rank], k, lv.img, lv.list, st), "layer_lists");
+			BinView lb = b;
+			lb.vals_out = lv.list;
+			FrameDev fk = ft;
+			fk.bg = layers[k].bg;
+			SGR_TRY(launch_blend_fwd(fk, g, lb, lv.img, nullptr, layers[k].color, layers[k].depth, layers[k].alpha, nullptr, st), "layer blend_fwd");
+		}
+	}
 	return SGR_OK;
 }
 
@@ -556,11 +647,12 @@ static int sharded_backward(const SgrFrame *frame, const SgrPeers *peers, int64_
                             const float *out_alpha, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
                             float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors_precomp, float *dL_dopacity,
                             float *dL_dscales, float *dL_drotations, float *dL_dcov3D, uint32_t barrier_epoch, SemPeers *sp,
-                            const float *dL_dsemantic, float *dL_dsemantics, void *stream) {
+                            const float *dL_dsemantic, float *dL_dsemantics, void *stream, const SgrLayerPeers *lpeers = nullptr, const SgrShardedLayer *layers = nullptr, int nl = 0) {
 	FrameDev fl, ft;
 	PeerTable pt = {};
 	int rc = make_total_frame(frame, peers, fl, ft, pt, true, sp);
 	if (rc) return rc;
+	if (nl && (rc = layer_peers(lpeers, pt, nl)) != SGR_OK) return rc;
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 	const bool debug = frame->debug != 0;
 	if (!img_state || !out_alpha || !dL_dcolor || !dL_ddepth || !dL_dalpha) return fail(SGR_EINVAL, "NULL pointer passed to sgr_sharded_backward");
@@ -579,7 +671,37 @@ static int sharded_backward(const SgrFrame *frame, const SgrPeers *peers, int64_
 		SGR_TRY(launch_blend_bwd(ft, g, b, img, sp ? sp->sem[pt.rank] : nullptr, out_alpha, dL_dcolor, dL_ddepth, dL_dalpha, sp ? dL_dsemantic : nullptr,
 		                         grad2d, sp ? sp->gsem[pt.rank] : nullptr, st, true),
 		        "blend_bwd");
+	if (nl) {  // the live layers (this call takes them only when one has a gradient): blend backward by slot into the layer sections
+		for (int k = 0; k < nl && ft.P > 0; k++) {
+			if (!layers[k].dL_dcolor) continue;
+			const LayerView lv = carve_sharded_layer(layers[k].state, ft.W, ft.H, capacity, fl.P).lv;
+			BinView lb = b;
+			lb.vals_out = lv.list;
+			FrameDev fk = ft;  // (the background term of the blend's alpha gradient is the layer's)
+			fk.bg = layers[k].bg;
+			SGR_TRY(launch_blend_bwd2(fk, g, lb, lv.img, layers[k].alpha, layers[k].dL_dcolor, layers[k].dL_ddepth, layers[k].dL_dalpha,
+			                          layer_section(lpeers, pt.rank, k, ft), st, true),
+			        "layer blend_bwd");
+		}
+	}
 	SGR_TRY(launch_peer_barrier(pt, barrier_epoch, ft.P > 0 ? g.big_count : nullptr, st), "barrier");
+	if (nl) {  // owner side: main + live layer rows summed from the ranks, then the chain rule once on them
+		const ShardedLayerView sv = carve_sharded_layer(layers[0].state, ft.W, ft.H, capacity, fl.P);
+		LayerGatherTable t = {};
+		for (int k = 0; k < nl; k++) {
+			if (!layers[k].dL_dcolor || layers[k].end == layers[k].begin) continue;
+			t.begin[t.n] = layers[k].begin; t.end[t.n] = layers[k].end; t.sink[t.n] = layers[k].dL_dmeans2D;
+			t.sec[t.n] = pt;
+			for (int p = 0; p < pt.world; p++) t.sec[t.n].grad2d[p] = layer_section(lpeers, p, k, ft);
+			t.n++;
+		}
+		SGR_TRY(launch_layer_gather(fl.P, pt, t, radii_local, g.depth_key, sv.rows, dL_dmeans2D, st), "layer gather");
+		SGR_TRY(launch_preprocess_bwd(fl, nullptr, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii_local, g.jac, sv.rows,
+		                              dL_dmeans3D, sv.means2D, shs ? dL_dsh : nullptr, dL_dcolors_precomp, dL_dopacity,
+		                              cov3D_precomp ? nullptr : dL_dscales, cov3D_precomp ? nullptr : dL_drotations, dL_dcov3D, st),
+		        "preprocess_bwd");
+		return SGR_OK;
+	}
 	SGR_TRY(launch_preprocess_bwd(fl, &pt, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii_local,
 	                              g.jac, reinterpret_cast<const float *>(g.depth_key), dL_dmeans3D,
 	                              dL_dmeans2D, shs ? dL_dsh : nullptr, dL_dcolors_precomp, dL_dopacity, cov3D_precomp ? nullptr : dL_dscales,
@@ -611,6 +733,45 @@ int sgr_sharded_backward_features(const SgrFrame *frame, const SgrPeers *peers, 
 	return sharded_backward(frame, peers, capacity, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii_local, records_local,
 	                        img_state, binning_state, out_alpha, dL_dcolor, dL_ddepth, dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors_precomp,
 	                        dL_dopacity, dL_dscales, dL_drotations, dL_dcov3D, barrier_epoch, &sp, dL_dsemantic, dL_dsemantics, stream);
+}
+
+int sgr_sharded_layer_state_sizes(const SgrFrame *frame, int64_t capacity, size_t *layer_bytes) {
+	FrameDev f;
+	int rc = make_frame(frame, f);
+	if (rc) return rc;
+	if (capacity < 0 || capacity > 0x7fffffffLL) return fail(SGR_EINVAL, "capacity must be in [0, 2^31)");
+	if (layer_bytes) *layer_bytes = carve_sharded_layer(nullptr, f.W, f.H, capacity, f.P).total_bytes;
+	return SGR_OK;
+}
+
+int sgr_sharded_forward_layers(const SgrFrame *frame, const SgrPeers *peers, const float *means3D, const float *shs, const float *colors_precomp,
+                               const float *opacities, const float *scales, const float *rotations, const float *cov3D_precomp, float *out_color,
+                               float *out_depth, float *out_alpha, int32_t *radii_local, void *records_local, size_t geom_bytes, void *img_state,
+                               size_t img_bytes, void *binning_state, size_t binning_bytes, int64_t capacity, int64_t gaussian_capacity,
+                               uint32_t barrier_epoch, int32_t pre_barrier, const SgrLayerPeers *layer_peers, const SgrShardedLayer *layers,
+                               int32_t num_layers, void *stream) {
+	int rc = check_sharded_layers("sgr_sharded_forward_layers", frame, layers, num_layers, capacity, false);
+	if (rc) return rc;
+	return sharded_forward(frame, peers, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, out_color, out_depth, out_alpha,
+	                       radii_local, records_local, geom_bytes, img_state, img_bytes, binning_state, binning_bytes, capacity, gaussian_capacity,
+	                       barrier_epoch, pre_barrier, nullptr, nullptr, nullptr, stream, layer_peers, layers, num_layers);
+}
+
+int sgr_sharded_backward_layers(const SgrFrame *frame, const SgrPeers *peers, int64_t capacity, const float *means3D, const float *shs,
+                                const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                                const int32_t *radii_local, const void *records_local, const void *img_state, const void *binning_state,
+                                const float *out_alpha, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
+                                float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors_precomp, float *dL_dopacity,
+                                float *dL_dscales, float *dL_drotations, float *dL_dcov3D, uint32_t barrier_epoch, const SgrLayerPeers *layer_peers,
+                                const SgrShardedLayer *layers, int32_t num_layers, void *stream) {
+	int rc = check_sharded_layers("sgr_sharded_backward_layers", frame, layers, num_layers, capacity, true);
+	if (rc) return rc;
+	bool live = false;  // a layer whose images got no gradient costs nothing: without one this is sgr_sharded_backward
+	for (int k = 0; k < num_layers; k++) live = live || layers[k].dL_dcolor != nullptr;
+	return sharded_backward(frame, peers, capacity, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii_local, records_local,
+	                        img_state, binning_state, out_alpha, dL_dcolor, dL_ddepth, dL_dalpha, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors_precomp,
+	                        dL_dopacity, dL_dscales, dL_drotations, dL_dcov3D, barrier_epoch, nullptr, nullptr, nullptr, stream, layer_peers,
+	                        live ? layers : nullptr, live ? num_layers : 0);
 }
 
 int sgr_forward_status_async(const SgrFrame *frame, const void *geom_state, uint32_t *host_status, void *stream) {
@@ -727,20 +888,6 @@ int sgr_backward(const SgrFrame *frame, int64_t num_instances, const float *mean
 }
 
 // ---- render layers ----
-// layer state: the img-state layout (ranges, tile_max_contrib, n_contrib) of the layer, then its tile lists u32[num_instances]
-struct LayerView {
-	ImgView img;
-	uint32_t *list;
-	size_t total_bytes;
-};
-static LayerView carve_layer(void *base, int W, int H, int64_t R) {
-	LayerView v;
-	v.img = carve_img(base, W, H, false);
-	char *p = reinterpret_cast<char *>(base) + v.img.total_bytes;
-	v.list = take<uint32_t>(p, R > 0 ? (size_t)R : 1);
-	v.total_bytes = (size_t)(p - reinterpret_cast<char *>(base));
-	return v;
-}
 // the frame of a layer: the main call's, whole image, no feature channels, the layer's background
 static int make_layer_frame(const SgrFrame *frame, const SgrLayer *layer, FrameDev &f) {
 	int rc = make_frame(frame, f);

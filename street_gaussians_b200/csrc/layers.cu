@@ -19,21 +19,38 @@
 //   layer_merge_kernel    add every layer's rows into the main grad2d, write each layer's [0:3] to its dL/dmeans2D sink
 //   preprocess_bwd        unchanged
 //   layer_restore_kernel  dL/dmeans2D of the covered rows <- the stashed main sums (what preprocess_bwd writes from unmerged rows)
+//
+// The fused Gaussian-sharded step (sgr_sharded_*_layers) lists slots, not ids: the *_masked passes keep the slots whose delivered layer
+// byte has the layer's bit, layer_zero_rows_kernel clears the layer rows of the slots delivered to a rank, and layer_gather_kernel sums
+// an owner's main and layer rows from the ranks that rendered them before preprocess_bwd runs once on the sum.
 #include "sgr_common.cuh"
 
 namespace sgr {
 
 constexpr int kLayerThreads = 256;
 
-__global__ void __launch_bounds__(kLayerThreads) layer_count_kernel(const uint2 *__restrict__ ranges, const uint32_t *__restrict__ list,
-                                                                    const uint32_t begin, const uint32_t end, uint2 *__restrict__ out_ranges) {
+// which entries of the main list a layer keeps: one GPU, ids in [begin, end); the fused Gaussian-sharded step, slots whose delivered
+// layer byte has the layer's bit (the lists hold slots, which do not give back an owner's row)
+struct InRange {
+	uint32_t begin, end;
+	__device__ __forceinline__ bool operator()(uint32_t id) const { return id >= begin && id < end; }
+};
+struct MaskBit {
+	const uint8_t *mask;
+	uint32_t bit;
+	__device__ __forceinline__ bool operator()(uint32_t id) const { return (mask[id] >> bit) & 1u; }
+};
+
+template <typename Keep>
+__device__ __forceinline__ void layer_count(const uint2 *__restrict__ ranges, const uint32_t *__restrict__ list, const Keep keep,
+                                            uint2 *__restrict__ out_ranges) {
 	__shared__ uint32_t s_warp[kLayerThreads / 32];
 	const int tile = blockIdx.x;
 	const uint2 r = ranges[tile];
 	uint32_t n = 0;
 	for (uint32_t k = r.x + threadIdx.x; k < r.y; k += kLayerThreads) {
 		const uint32_t id = list[k];
-		n += (id >= begin && id < end) ? 1u : 0u;
+		n += keep(id) ? 1u : 0u;
 	}
 	n = __reduce_add_sync(0xffffffffu, n);
 	if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = n;
@@ -84,9 +101,9 @@ __global__ void __launch_bounds__(1024) layer_scan_kernel(uint2 *__restrict__ ra
 }
 
 // stable: within a chunk of 256 entries the output position is the number of matching entries before it (warp ballots + warp prefix)
-__global__ void __launch_bounds__(kLayerThreads) layer_compact_kernel(const uint2 *__restrict__ ranges, const uint32_t *__restrict__ list,
-                                                                      const uint32_t begin, const uint32_t end,
-                                                                      const uint2 *__restrict__ out_ranges, uint32_t *__restrict__ out_list) {
+template <typename Keep>
+__device__ __forceinline__ void layer_compact(const uint2 *__restrict__ ranges, const uint32_t *__restrict__ list, const Keep keep,
+                                              const uint2 *__restrict__ out_ranges, uint32_t *__restrict__ out_list) {
 	__shared__ uint32_t s_warp[kLayerThreads / 32];
 	const int tile = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const uint2 r = ranges[tile];
@@ -97,7 +114,7 @@ __global__ void __launch_bounds__(kLayerThreads) layer_compact_kernel(const uint
 		bool hit = false;
 		if (k < r.y) {
 			id = list[k];
-			hit = id >= begin && id < end;
+			hit = keep(id);
 		}
 		const unsigned b = __ballot_sync(0xffffffffu, hit);
 		if (lane == 0) s_warp[warp] = (uint32_t)__popc(b);
@@ -128,6 +145,26 @@ __global__ void __launch_bounds__(kLayerThreads) layer_fill_kernel(const size_t 
 	}
 }
 
+__global__ void __launch_bounds__(kLayerThreads) layer_count_kernel(const uint2 *__restrict__ ranges, const uint32_t *__restrict__ list,
+                                                                    const uint32_t begin, const uint32_t end, uint2 *__restrict__ out_ranges) {
+	layer_count(ranges, list, InRange{begin, end}, out_ranges);
+}
+__global__ void __launch_bounds__(kLayerThreads) layer_compact_kernel(const uint2 *__restrict__ ranges, const uint32_t *__restrict__ list,
+                                                                      const uint32_t begin, const uint32_t end,
+                                                                      const uint2 *__restrict__ out_ranges, uint32_t *__restrict__ out_list) {
+	layer_compact(ranges, list, InRange{begin, end}, out_ranges, out_list);
+}
+__global__ void __launch_bounds__(kLayerThreads) layer_count_masked_kernel(const uint2 *__restrict__ ranges, const uint32_t *__restrict__ list,
+                                                                           const uint8_t *__restrict__ mask, const uint32_t bit,
+                                                                           uint2 *__restrict__ out_ranges) {
+	layer_count(ranges, list, MaskBit{mask, bit}, out_ranges);
+}
+__global__ void __launch_bounds__(kLayerThreads) layer_compact_masked_kernel(const uint2 *__restrict__ ranges, const uint32_t *__restrict__ list,
+                                                                             const uint8_t *__restrict__ mask, const uint32_t bit,
+                                                                             const uint2 *__restrict__ out_ranges, uint32_t *__restrict__ out_list) {
+	layer_compact(ranges, list, MaskBit{mask, bit}, out_ranges, out_list);
+}
+
 cudaError_t launch_layer_lists(const FrameDev &f, ImgView main_img, BinView main_bin, int begin, int end, ImgView layer_img, uint32_t *layer_list,
                                cudaStream_t st) {
 	const int ntile = f.gx * f.gy;
@@ -137,6 +174,18 @@ cudaError_t launch_layer_lists(const FrameDev &f, ImgView main_img, BinView main
 	layer_scan_kernel<<<1, 1024, 0, st>>>(layer_img.ranges, (uint32_t)ntile);
 	layer_compact_kernel<<<ntile, kLayerThreads, 0, st>>>(main_img.ranges, main_bin.vals_out, (uint32_t)begin, (uint32_t)end, layer_img.ranges,
 	                                                      layer_list);
+	return cudaGetLastError();
+}
+// the same three passes keeping the slots whose delivered layer byte has bit `bit` (the fused Gaussian-sharded step)
+cudaError_t launch_layer_lists_masked(const FrameDev &f, ImgView main_img, BinView main_bin, const uint8_t *mask, int bit, ImgView layer_img,
+                                      uint32_t *layer_list, cudaStream_t st) {
+	const int ntile = f.gx * f.gy;
+	if (ntile <= 0) return cudaSuccess;
+	count_launch(3);
+	layer_count_masked_kernel<<<ntile, kLayerThreads, 0, st>>>(main_img.ranges, main_bin.vals_out, mask, (uint32_t)bit, layer_img.ranges);
+	layer_scan_kernel<<<1, 1024, 0, st>>>(layer_img.ranges, (uint32_t)ntile);
+	layer_compact_masked_kernel<<<ntile, kLayerThreads, 0, st>>>(main_img.ranges, main_bin.vals_out, mask, (uint32_t)bit, layer_img.ranges,
+	                                                             layer_list);
 	return cudaGetLastError();
 }
 
@@ -229,6 +278,79 @@ cudaError_t launch_layer_merge(float *grad2d, const SgrLayerGrad *layers, int n,
 		if (e != cudaSuccess) return e;
 	}
 	return cudaSuccess;
+}
+
+// ---- the fused Gaussian-sharded step (sgr_sharded_forward_layers / sgr_sharded_backward_layers) ----
+// The rows of a rank's layer sections that its owners read back are those of every slot delivered to the rank, but its layer blends
+// write only the slots of their lists.  So, like count_runs_kernel for the main rows, the forward clears the layer rows of the delivered
+// slots: thread j = j-th delivered Gaussian (cval, in ascending slot order), j < the delivered count on the device (status[4]) and the
+// depth-order slots n of the call.
+__global__ void __launch_bounds__(kLayerThreads) layer_zero_rows_kernel(const uint32_t *__restrict__ cval, const uint32_t *__restrict__ status,
+                                                                        const uint32_t n, const LayerRows t) {
+	const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+	if (j >= n || j >= status[4]) return;
+	const size_t g = cval[j];
+	const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+	for (int k = 0; k < kMaxShardedLayers; k++) {
+		if (k >= t.n) break;
+		float4 *row = reinterpret_cast<float4 *>(t.rows[k]) + 3 * g;
+		row[0] = z; row[1] = z; row[2] = z;
+	}
+}
+cudaError_t launch_layer_zero_rows(GeomView g, int n, const LayerRows &t, cudaStream_t st) {
+	if (n <= 0 || t.n == 0) return cudaSuccess;
+	count_launch();
+	layer_zero_rows_kernel<<<(unsigned)((n + kLayerThreads - 1) / kLayerThreads), kLayerThreads, 0, st>>>(g.cval, g.big_count, (uint32_t)n, t);
+	return cudaGetLastError();
+}
+
+// Owner side of the layered backward: every block fetches the rows of its 256 Gaussians from the ranks that rendered them, the main
+// section and then each live layer's (gather_runs: the same runs, ascending rank order, from 0), and writes
+//   out[i]         = main + every covering live layer in table order (what layer_merge_kernel makes of them on one GPU),
+//   dL_dmeans2D[i] = main[0:3]             (the densification statistics read the main sums only),
+//   sink_k[i - b]  = layer k's [0:3].
+// Rows of Gaussians without a destination are zero (their mask is 0).
+__global__ void __launch_bounds__(kRunBlock) layer_gather_kernel(const int P, const PeerTable pt, const LayerGatherTable t,
+                                                                 const int32_t *__restrict__ radii, const uint32_t *__restrict__ masks,
+                                                                 float *__restrict__ out, float *__restrict__ dL_dmeans2D) {
+	__shared__ RunScratch rs;
+	__shared__ float4 s_g[3 * kRunBlock];
+	const int idx = blockIdx.x * kRunBlock + threadIdx.x;
+	const bool in_range = idx < P;
+	const uint32_t mask = in_range && radii[idx] > 0 ? masks[idx] : 0u;
+	float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a, c = a;
+	gather_runs(pt, mask, rs, s_g, a, b, c);
+	if (in_range) {
+		dL_dmeans2D[3 * (size_t)idx] = a.x; dL_dmeans2D[3 * (size_t)idx + 1] = a.y; dL_dmeans2D[3 * (size_t)idx + 2] = a.z;
+	}
+#pragma unroll
+	for (int k = 0; k < kMaxShardedLayers; k++) {
+		if (k >= t.n) break;  // (uniform over the block: gather_runs is collective)
+		__syncthreads();      // the previous gather's last readers of rs are done
+		float4 x = make_float4(0.f, 0.f, 0.f, 0.f), y = x, z = x;
+		gather_runs(t.sec[k], mask, rs, s_g, x, y, z);
+		if (in_range && idx >= t.begin[k] && idx < t.end[k]) {
+			a.x += x.x; a.y += x.y; a.z += x.z; a.w += x.w;
+			b.x += y.x; b.y += y.y; b.z += y.z; b.w += y.w;
+			c.x += z.x; c.y += z.y; c.z += z.z; c.w += z.w;
+			if (t.sink[k]) {
+				const size_t r = (size_t)(idx - t.begin[k]);
+				t.sink[k][3 * r] = x.x; t.sink[k][3 * r + 1] = x.y; t.sink[k][3 * r + 2] = x.z;
+			}
+		}
+	}
+	if (in_range) {
+		float4 *dst = reinterpret_cast<float4 *>(out) + 3 * (size_t)idx;
+		dst[0] = a; dst[1] = b; dst[2] = c;
+	}
+}
+cudaError_t launch_layer_gather(int P, const PeerTable &pt, const LayerGatherTable &t, const int32_t *radii, const uint32_t *masks, float *out,
+                                float *dL_dmeans2D, cudaStream_t st) {
+	if (P == 0) return cudaSuccess;
+	count_launch();
+	layer_gather_kernel<<<(unsigned)((P + kRunBlock - 1) / kRunBlock), kRunBlock, 0, st>>>(P, pt, t, radii, masks, out, dL_dmeans2D);
+	return cudaGetLastError();
 }
 
 }  // namespace sgr

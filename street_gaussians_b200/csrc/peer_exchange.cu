@@ -120,6 +120,31 @@ __global__ void __launch_bounds__(kRunBlock) gather_semantics_kernel(const int P
 	}
 }
 
+// ---- render layers of the fused step (sgr_sharded_forward_layers) ----
+// One byte per Gaussian (bit k = the Gaussian lies in layer k's rows), delivered like its record: the same block runs, the same slots of
+// rank d's mask section.  The runs are re-derived from the destination masks preprocess_fwd_kernel<false, SCATTER> stored, as above.
+__global__ void __launch_bounds__(kRunBlock) scatter_layer_mask_kernel(const int P, const PeerTable pt, const LayerPeers lp,
+                                                                      const uint32_t *__restrict__ masks) {
+	__shared__ RunScratch rs;
+	const int idx = blockIdx.x * kRunBlock + threadIdx.x;
+	const uint32_t mask = idx < P ? masks[idx] : 0u;
+	uint32_t bits = 0u;
+	for (int k = 0; k < lp.n; k++) bits |= (idx >= lp.begin[k] && idx < lp.end[k]) ? 1u << k : 0u;
+	block_run_ranks(rs, mask, pt.world);
+	const size_t slot0 = (size_t)pt.rank * (size_t)pt.chunk + (size_t)blockIdx.x * kRunBlock;
+	for (int d = 0; d < pt.world; d++) {
+		const uint32_t r = run_rank(rs, mask, d);
+		if ((mask >> d) & 1u) lp.mask[d][slot0 + r] = (uint8_t)bits;
+	}
+}
+
+cudaError_t launch_scatter_layer_mask(const PeerTable &pt, const LayerPeers &lp, int P, const uint32_t *masks, cudaStream_t st) {
+	if (P == 0) return cudaSuccess;
+	count_launch();
+	scatter_layer_mask_kernel<<<(unsigned)((P + kRunBlock - 1) / kRunBlock), kRunBlock, 0, st>>>(P, pt, lp, masks);
+	return cudaGetLastError();
+}
+
 cudaError_t launch_scatter_semantics(const PeerTable &pt, const SemPeers &sp, int P, int S, const uint32_t *masks, const float *sem, cudaStream_t st) {
 	if (P == 0) return cudaSuccess;
 	count_launch();

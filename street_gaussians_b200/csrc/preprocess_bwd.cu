@@ -27,58 +27,6 @@ namespace sgr {
 constexpr int kShRow = 49;  // padded smem row (floats) for up to 16 x 3 SH coefficients
 constexpr int kBwdStride = 52;  // row stride (floats) of the TMA variant's stage: 208 B
 
-// Block-run gather (sgr_common.cuh): the rows this block's Gaussians accumulated on rank d are the first c(d) rows of the block's 256
-// slots in rank d's partial grad2d — one contiguous run per rank, fetched with lane-contiguous 16-B loads (whole 128-B lines over
-// NVLink) into shared memory, 256 rows per round; every thread then adds its own rows in ascending rank order.  Collective over the
-// block; `mask` must be the destination mask the forward stored for this thread's Gaussian (0 for none).
-__device__ __forceinline__ void gather_runs(const PeerTable &pt, const uint32_t mask, RunScratch &rs, float4 *s_g, float4 &g0v, float4 &g1v,
-                                            float4 &g2v) {
-	block_run_ranks(rs, mask, pt.world);
-	const uint32_t total = rs.cpre[pt.world];
-	const size_t slot0 = (size_t)pt.rank * (size_t)pt.chunk + (size_t)blockIdx.x * kRunBlock;
-	auto fetch = [&](uint32_t base, float4 (&v)[3]) {  // this thread's (up to) three 16-B pieces of the round that starts at `base`
-		const uint32_t n = base < total ? min((uint32_t)kRunBlock, total - base) : 0u;
-#pragma unroll
-		for (int k = 0; k < 3; k++) {
-			const uint32_t e = threadIdx.x + (uint32_t)k * kRunBlock;
-			if (e < 3u * n) {
-				const uint32_t pos = base + e / 3u, part = e % 3u;
-				const int d = run_dest(rs, pos, pt.world);
-				v[k] = reinterpret_cast<const float4 *>(pt.grad2d[d] + (slot0 + (pos - rs.cpre[d])) * 12)[part];
-			}
-		}
-	};
-	auto consume = [&](uint32_t base, const float4 (&v)[3]) {  // collective: publish the round, add the rows that fall into it
-		const uint32_t n = min((uint32_t)kRunBlock, total - base);
-#pragma unroll
-		for (int k = 0; k < 3; k++) {
-			const uint32_t e = threadIdx.x + (uint32_t)k * kRunBlock;
-			if (e < 3u * n) s_g[e] = v[k];
-		}
-		__syncthreads();
-		for (int d = 0; d < pt.world; d++) {
-			const uint32_t r = run_rank(rs, mask, d);
-			const uint32_t pos = rs.cpre[d] + r;
-			if (((mask >> d) & 1u) && pos >= base && pos < base + kRunBlock) {
-				const float4 a = s_g[(pos - base) * 3u], b = s_g[(pos - base) * 3u + 1u], c = s_g[(pos - base) * 3u + 2u];
-				g0v.x += a.x; g0v.y += a.y; g0v.z += a.z; g0v.w += a.w;
-				g1v.x += b.x; g1v.y += b.y; g1v.z += b.z; g1v.w += b.w;
-				g2v.x += c.x; g2v.y += c.y; g2v.z += c.z; g2v.w += c.w;
-			}
-		}
-		__syncthreads();
-	};
-	// rounds of 256 rows, two in flight: the loads of the second are requested before the first is waited for (the typical block has
-	// 1.2-1.4 rows per Gaussian, i.e. exactly two rounds, so one NVLink round trip replaces two)
-	for (uint32_t base = 0; base < total; base += 2u * kRunBlock) {
-		float4 va[3], vb[3];
-		fetch(base, va);
-		fetch(base + kRunBlock, vb);
-		consume(base, va);
-		if (base + kRunBlock < total) consume(base + kRunBlock, vb);
-	}
-}
-
 // GATHER = true (sgr_sharded_backward): grad2d is not a local array — the 12 sums of local Gaussian idx (global id
 // rank*chunk + idx) are read from the partial grad2d of every rank whose cyclic band its rectangle meets (NVLink peer loads)
 // and added in ascending rank order, exactly what sgr_gather_grad2d produced as a separate pass.

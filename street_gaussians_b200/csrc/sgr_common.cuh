@@ -349,6 +349,58 @@ __device__ __forceinline__ int run_dest(const RunScratch &rs, uint32_t pos, int 
 	while (d + 1 < world && pos >= rs.cpre[d + 1]) d++;
 	return d;
 }
+// Block-run gather: the rows this block's Gaussians accumulated on rank d are the first c(d) rows of the block's 256
+// slots in rank d's partial grad2d — one contiguous run per rank, fetched with lane-contiguous 16-B loads (whole 128-B lines over
+// NVLink) into shared memory, 256 rows per round; every thread then adds its own rows in ascending rank order.  Collective over the
+// block; `mask` must be the destination mask the forward stored for this thread's Gaussian (0 for none).
+__device__ __forceinline__ void gather_runs(const PeerTable &pt, const uint32_t mask, RunScratch &rs, float4 *s_g, float4 &g0v, float4 &g1v,
+                                            float4 &g2v) {
+	block_run_ranks(rs, mask, pt.world);
+	const uint32_t total = rs.cpre[pt.world];
+	const size_t slot0 = (size_t)pt.rank * (size_t)pt.chunk + (size_t)blockIdx.x * kRunBlock;
+	auto fetch = [&](uint32_t base, float4 (&v)[3]) {  // this thread's (up to) three 16-B pieces of the round that starts at `base`
+		const uint32_t n = base < total ? min((uint32_t)kRunBlock, total - base) : 0u;
+#pragma unroll
+		for (int k = 0; k < 3; k++) {
+			const uint32_t e = threadIdx.x + (uint32_t)k * kRunBlock;
+			if (e < 3u * n) {
+				const uint32_t pos = base + e / 3u, part = e % 3u;
+				const int d = run_dest(rs, pos, pt.world);
+				v[k] = reinterpret_cast<const float4 *>(pt.grad2d[d] + (slot0 + (pos - rs.cpre[d])) * 12)[part];
+			}
+		}
+	};
+	auto consume = [&](uint32_t base, const float4 (&v)[3]) {  // collective: publish the round, add the rows that fall into it
+		const uint32_t n = min((uint32_t)kRunBlock, total - base);
+#pragma unroll
+		for (int k = 0; k < 3; k++) {
+			const uint32_t e = threadIdx.x + (uint32_t)k * kRunBlock;
+			if (e < 3u * n) s_g[e] = v[k];
+		}
+		__syncthreads();
+		for (int d = 0; d < pt.world; d++) {
+			const uint32_t r = run_rank(rs, mask, d);
+			const uint32_t pos = rs.cpre[d] + r;
+			if (((mask >> d) & 1u) && pos >= base && pos < base + kRunBlock) {
+				const float4 a = s_g[(pos - base) * 3u], b = s_g[(pos - base) * 3u + 1u], c = s_g[(pos - base) * 3u + 2u];
+				g0v.x += a.x; g0v.y += a.y; g0v.z += a.z; g0v.w += a.w;
+				g1v.x += b.x; g1v.y += b.y; g1v.z += b.z; g1v.w += b.w;
+				g2v.x += c.x; g2v.y += c.y; g2v.z += c.z; g2v.w += c.w;
+			}
+		}
+		__syncthreads();
+	};
+	// rounds of 256 rows, two in flight: the loads of the second are requested before the first is waited for (the typical block has
+	// 1.2-1.4 rows per Gaussian, i.e. exactly two rounds, so one NVLink round trip replaces two)
+	for (uint32_t base = 0; base < total; base += 2u * kRunBlock) {
+		float4 va[3], vb[3];
+		fetch(base, va);
+		fetch(base + kRunBlock, vb);
+		consume(base, va);
+		if (base + kRunBlock < total) consume(base + kRunBlock, vb);
+	}
+}
+
 cudaError_t launch_peer_barrier(const PeerTable &pt, uint32_t epoch, uint32_t *status, cudaStream_t st);
 // sgr_project fused with sgr_scatter_records: one pass over the rank's chunk (f.P local Gaussians, pt.chunk slots)
 // The feature sections of the fused step's peer workspace: sem[P_total, S] and gsem[P_total, S] of every rank, rows by slot.
@@ -358,6 +410,28 @@ struct SemPeers {
 };
 cudaError_t launch_scatter_semantics(const PeerTable &pt, const SemPeers &sp, int P, int S, const uint32_t *masks, const float *sem, cudaStream_t st);
 cudaError_t launch_gather_semantics(const PeerTable &pt, const SemPeers &sp, int P, int S, const uint32_t *masks, float *out, cudaStream_t st);
+// Render layers of the fused step (sgr_sharded_*_layers): the layer sections of the peer workspace, layer_mask[P_total] (bit k = layer k,
+// rows by slot) and layer_grad2d[L, P_total, 12] of every rank; a layer's rows [begin, end) of the owner's Gaussians.
+constexpr int kMaxShardedLayers = SGR_MAX_SHARDED_LAYERS;
+struct LayerPeers {
+	uint8_t *mask[kMaxPeers];
+	int n;
+	int begin[kMaxShardedLayers], end[kMaxShardedLayers];
+};
+cudaError_t launch_scatter_layer_mask(const PeerTable &pt, const LayerPeers &lp, int P, const uint32_t *masks, cudaStream_t st);
+struct LayerRows {  // this rank's layer sections to clear
+	int n;
+	float *rows[kMaxShardedLayers];
+};
+cudaError_t launch_layer_zero_rows(GeomView g, int n, const LayerRows &t, cudaStream_t st);
+struct LayerGatherTable {  // the live layers (those with a gradient) in table order; sec[k].grad2d[p] = rank p's section of layer k
+	int n;
+	int begin[kMaxShardedLayers], end[kMaxShardedLayers];
+	float *sink[kMaxShardedLayers];
+	PeerTable sec[kMaxShardedLayers];
+};
+cudaError_t launch_layer_gather(int P, const PeerTable &pt, const LayerGatherTable &t, const int32_t *radii, const uint32_t *masks, float *out,
+                                float *dL_dmeans2D, cudaStream_t st);
 cudaError_t launch_project_scatter(const FrameDev &f, const PeerTable &pt, const float *means3D, const float *shs,
                                    const float *colors_precomp, const float *opacities, const float *scales, const float *rotations,
                                    const float *cov3D_precomp, int32_t *radii_local, GaussRec *rec_local, float4 *jac_local,
@@ -402,6 +476,8 @@ cudaError_t launch_preprocess_bwd(const FrameDev &f, const PeerTable *pt, const 
 // render layers (layers.cu)
 cudaError_t launch_layer_lists(const FrameDev &f, ImgView main_img, BinView main_bin, int begin, int end, ImgView layer_img, uint32_t *layer_list,
                                cudaStream_t st);
+cudaError_t launch_layer_lists_masked(const FrameDev &f, ImgView main_img, BinView main_bin, const uint8_t *mask, int bit, ImgView layer_img,
+                                      uint32_t *layer_list, cudaStream_t st);
 cudaError_t launch_layer_fill(const FrameDev &f, const float *bg, float *color, float *depth, float *alpha, cudaStream_t st);
 cudaError_t launch_layer_stash(const float *grad2d, int lo, int hi, float *stash, bool restore, float *dL_dmeans2D, cudaStream_t st);
 cudaError_t launch_layer_merge(float *grad2d, const SgrLayerGrad *layers, int n, cudaStream_t st);

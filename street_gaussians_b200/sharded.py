@@ -33,8 +33,8 @@ import torch.nn as nn
 from . import _capi
 from ._capi import ptr
 from .training import PARAM_NAMES, _attr, _install, _param_slots, _segment, _stat_segment
-from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, InstanceCapacity, TileRowBand, _copy_status, _ForwardState,
-                         _backward_blend_impl, _backward_geom_impl, _fit_grads, _fp32_inputs, _geom_grad_buffers, _image_grads,
+from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, InstanceCapacity, TileRowBand, _check_layers, _copy_status,
+                         _ForwardState, _backward_blend_impl, _backward_geom_impl, _fit_grads, _fp32_inputs, _geom_grad_buffers, _image_grads,
                          _input_shapes, _make_frame, _reference_inputs)
 
 
@@ -214,21 +214,22 @@ def _align(n: int, a: int = 256) -> int:
 
 
 class PeerWorkspace:
-    """Per-rank buffer [geom_state | radii_all | grad2d | sem | gsem | pose_acc | loss | barrier pad] that every rank of the group can
-    address (include/sgr.h, SgrPeers).
+    """Per-rank buffer [geom_state | radii_all | grad2d | sem | gsem | pose_acc | loss | layer_mask | layer_grad2d | barrier pad] that
+    every rank of the group can address (include/sgr.h, SgrPeers).  The two layer sections exist with `layers` > 0 (render layers of
+    the fused step, GaussianShardedRasterizer.forward_layers).
 
     Real multi-GPU: ONE torch symmetric-memory allocation per rank (CUDA VMM mapped into every process; NVLink loads and
     stores), rendezvous'ed once; `barrier()` is the device-side signal-pad barrier of that allocation (a few microseconds
     over NVLink).  `emulate(...)` builds `world` ordinary buffers on ONE device that point at each other, so the exchange
     kernels can be tested without a second GPU."""
 
-    def __init__(self, settings, chunk: int, world: int, rank: int, device, group=None, _buffers=None, S: int = 0):
+    def __init__(self, settings, chunk: int, world: int, rank: int, device, group=None, _buffers=None, S: int = 0, layers: int = 0):
         self.chunk, self.world, self.rank, self.P_total = int(chunk), int(world), int(rank), int(chunk) * int(world)
-        self.S = int(S)
+        self.S, self.layers = int(S), int(layers)
         if world > _capi.MAX_PEERS:
             raise _capi.SgrError(f"peer exchange supports at most {_capi.MAX_PEERS} ranks, got {world}")
         self.geom_bytes, self.img_bytes, self.off_radii, self.off_grad, self.off_flags, self.total = self.layout(settings, self.P_total, device,
-                                                                                                                 self.S)
+                                                                                                                 self.S, layers=self.layers)
         self.off_sem, self.off_gsem = self.feature_offsets(self.off_grad, self.P_total, self.S)
         self.off_pose = self.pose_offset(self.off_grad, self.P_total, self.S)
         self.off_loss, self.loss_bytes = self.loss_offset(self.off_grad, self.P_total, self.S), self.loss_section_bytes(settings)
@@ -266,6 +267,17 @@ class PeerWorkspace:
             self.peers.pose_acc[p] = ptrs[p] + self.off_pose
             self.peers.loss[p] = ptrs[p] + self.off_loss
         self.peers.loss_bytes = self.loss_bytes
+        self.off_layer_mask, self.off_layer_grad = self.layer_offsets(settings, self.off_grad, self.P_total, self.S)
+        self.layer_peers = _capi.SgrLayerPeers()
+        self.layer_peers.layers = self.layers
+        if self.layers:
+            for p in range(self.world):
+                self.layer_peers.layer_mask[p] = ptrs[p] + self.off_layer_mask
+                self.layer_peers.layer_grad2d[p] = ptrs[p] + self.off_layer_grad
+        self.layer_mask = self.buf[self.off_layer_mask: self.off_layer_mask + self.P_total * (self.layers > 0)]
+        nl = 48 * self.P_total * self.layers
+        self.layer_grad2d = self.buf[self.off_layer_grad: self.off_layer_grad + nl].view(torch.float32).view(self.layers, self.P_total, 12)
+        self._layer_states = []
         nsem = self.P_total * self.S
         self.sem = self.buf[self.off_sem: self.off_sem + 4 * nsem].view(torch.float32).view(self.P_total, self.S)
         self.gsem = self.buf[self.off_gsem: self.off_gsem + 4 * nsem].view(torch.float32).view(self.P_total, self.S)
@@ -298,26 +310,37 @@ class PeerWorkspace:
         return n
 
     @staticmethod
-    def layout(settings, P_total: int, device, S: int = 0):
+    def layer_offsets(settings, off_grad: int, P_total: int, S: int):
+        """Offsets of the render layers' sections, after the band losses' section and before the barrier pad: layer_mask (one byte per
+        slot, bit k = layer k) and layer_grad2d (rows of 12 fp32 per slot, P_total rows per layer)."""
+        off_mask = _align(PeerWorkspace.loss_offset(off_grad, P_total, S) + PeerWorkspace.loss_section_bytes(settings))
+        return off_mask, _align(off_mask + P_total)
+
+    @staticmethod
+    def layout(settings, P_total: int, device, S: int = 0, layers: int = 0):
         """(geom_bytes, img_bytes, offset of radii_all, offset of grad2d, offset of the barrier pad, total bytes) of the per-rank buffer.
         With S feature channels the sections sem and gsem (feature_offsets) sit before the pad; S = 0 leaves them empty.  The composer's
-        accumulator section (pose_offset) follows them, then the band losses' section (loss_offset, loss_section_bytes)."""
+        accumulator section (pose_offset) follows them, then the band losses' section (loss_offset, loss_section_bytes), then with
+        `layers` render layers their mask and gradient sections (layer_offsets)."""
         fr, keep = _make_frame(settings, P_total, 0, 0, device, None)
         gb, ib = C.c_size_t(0), C.c_size_t(0)
         _capi.call("sgr_state_sizes", None, C.byref(fr), C.byref(gb), C.byref(ib))
         del keep
         off_radii = _align(gb.value)
         off_grad = _align(off_radii + 4 * P_total)
-        off_flags = _align(PeerWorkspace.loss_offset(off_grad, P_total, S) + PeerWorkspace.loss_section_bytes(settings))
+        if layers:
+            off_flags = _align(PeerWorkspace.layer_offsets(settings, off_grad, P_total, S)[1] + 48 * P_total * int(layers))
+        else:
+            off_flags = _align(PeerWorkspace.loss_offset(off_grad, P_total, S) + PeerWorkspace.loss_section_bytes(settings))
         return gb.value, ib.value, off_radii, off_grad, off_flags, off_flags + 256
 
     @classmethod
-    def emulate(cls, settings, chunk: int, world: int, device, S: int = 0):
+    def emulate(cls, settings, chunk: int, world: int, device, S: int = 0, layers: int = 0):
         """`world` workspaces on ONE device whose peer tables point at each other (tests; world == 1 module path)."""
-        total = cls.layout(settings, int(chunk) * int(world), device, S)[-1]
+        total = cls.layout(settings, int(chunk) * int(world), device, S, layers=layers)[-1]
         bufs = [torch.empty(total, dtype=torch.uint8, device=device) for _ in range(world)]
         ptrs = [b.data_ptr() for b in bufs]
-        return [cls(settings, chunk, world, r, device, _buffers=(bufs[r], ptrs), S=S) for r in range(world)]
+        return [cls(settings, chunk, world, r, device, _buffers=(bufs[r], ptrs), S=S, layers=layers) for r in range(world)]
 
     def barrier(self):
         """Device-side barrier of the STAGED path (torch symmetric memory's signal pad)."""
@@ -342,6 +365,18 @@ class PeerWorkspace:
         if b["binning"] is None or b["binning"].numel() < capacity_bytes:
             b["binning"] = torch.empty((capacity_bytes,), device=dev, dtype=torch.uint8)
         return b
+
+    def layer_states(self, n: int, state_bytes: int):
+        """The states of `n` render layers (sgr_sharded_layer_state_sizes bytes each), kept from a fused forward to its backward like
+        step_buffers."""
+        dev = self.buf.device
+        st = self._layer_states
+        while len(st) < n:
+            st.append(torch.empty((0,), device=dev, dtype=torch.uint8))
+        for k in range(n):
+            if st[k].numel() < state_bytes:
+                st[k] = torch.empty((state_bytes,), device=dev, dtype=torch.uint8)
+        return st[:n]
 
 
 def scatter_records(settings, ws: PeerWorkspace, rec_local, radii_local, P_local: int):
@@ -471,10 +506,12 @@ class _GaussianShardedRasterize(torch.autograd.Function):
 
 
 def sharded_forward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, capacity: int, gaussian_capacity: int, status_word=None,
-                        semantics=None):
+                        semantics=None, layers=None):
     """One sgr_sharded_forward call on the current stream (used by the autograd path and, with emulated workspaces on
     separate streams, by the single-GPU tests).  Returns (color, depth, alpha, step buffers).  semantics [P, S] (this rank's rows,
-    S = ws.S): sgr_sharded_forward_features, and the banded feature image [S, H, W] is returned as a fifth value."""
+    S = ws.S): sgr_sharded_forward_features, and the banded feature image [S, H, W] is returned as a fifth value.  layers: (begin, end,
+    bg) per render layer in this rank's rows (at most ws.layers): sgr_sharded_forward_layers, and the list of every layer's (color,
+    depth, alpha), zero outside the band, is returned as a fifth value; the layer states stay in the workspace for the backward."""
     L = _capi.lib()
     device = tensors["means3D"].device
     H, W = int(settings.image_height), int(settings.image_width)
@@ -497,6 +534,20 @@ def sharded_forward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, ca
         sem_in = _capi.f32(semantics, device)
         semantic = z(S)
         _capi.call("sgr_sharded_forward_features", device, *args, ptr(sem_in), ptr(semantic))
+    elif layers is not None:
+        if not 0 < len(layers) <= ws.layers:
+            raise ValueError(f"the workspace carries {ws.layers} render layers, the call {len(layers)}")
+        nb = C.c_size_t(0)
+        _capi.call("sgr_sharded_layer_state_sizes", None, C.byref(fr), capacity, C.byref(nb))
+        states = ws.layer_states(len(layers), nb.value)
+        table = (_capi.SgrShardedLayer * len(layers))()
+        outs, bgs = [], []
+        for k, (b, e, bg) in enumerate(layers):
+            bgs.append(_capi.f32(bg, device, align16=True))
+            outs.append((z(3), z(1), z(1)))
+            table[k] = _capi.SgrShardedLayer(b, e, bgs[-1].data_ptr(), states[k].data_ptr(), states[k].numel(), *(t.data_ptr() for t in outs[-1]))
+        _capi.call("sgr_sharded_forward_layers", device, *args, C.byref(ws.layer_peers), table, len(layers))
+        semantic = outs
     else:
         _capi.call("sgr_sharded_forward", device, *args)
     if status_word is not None:  # the status of the gathered frame (P_total slots)
@@ -505,13 +556,15 @@ def sharded_forward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, ca
         del keep2
     del keep
     ws.fwd_pending = True
-    return (color, depth, alpha, bufs, semantic) if S else (color, depth, alpha, bufs)
+    return (color, depth, alpha, bufs, semantic) if S or layers is not None else (color, depth, alpha, bufs)
 
 
-def sharded_backward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, capacity: int, alpha, gc, gd, ga, gs=None):
+def sharded_backward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, capacity: int, alpha, gc, gd, ga, gs=None, layers=None):
     """One sgr_sharded_backward call on the current stream.  Returns the 8 gradients in _backward_geom_impl's order.  gs [S, H, W]
     (the feature image's upstream gradient, after a forward with semantics): sgr_sharded_backward_features, and dL/dsemantics [P, S]
-    of this rank's own Gaussians is returned as a ninth value."""
+    of this rank's own Gaussians is returned as a ninth value.  layers (after a forward with layers, the same table): (begin, end, bg,
+    alpha, (g_color, g_depth, g_alpha) or None, means2D sink [end - begin, 3] fp32 or None) per layer: sgr_sharded_backward_layers,
+    which writes each layer's own screen-space gradient into its sink."""
     dev = alpha.device
     sh, colors, scales, rots, cov = (tensors[k] for k in ("sh", "colors_precomp", "scales", "rotations", "cov3Ds_precomp"))
     M = int(sh.shape[1]) if sh is not None else 0
@@ -527,6 +580,21 @@ def sharded_backward_raw(settings, band, ws: "PeerWorkspace", tensors, P: int, c
     if S:
         g_sem = torch.empty((P, S), device=dev, dtype=torch.float32)
         _capi.call("sgr_sharded_backward_features", dev, *args, ptr(_capi.f32(gs, dev)), ptr(g_sem))
+    elif layers is not None:
+        frs = _make_frame(settings, P, M, 0, dev, band)
+        nb = C.c_size_t(0)
+        _capi.call("sgr_sharded_layer_state_sizes", None, C.byref(frs[0]), capacity, C.byref(nb))
+        states = ws.layer_states(len(layers), nb.value)
+        table = (_capi.SgrShardedLayer * len(layers))()
+        keep_alive = []
+        for k, (b, e, bg, l_alpha, grads, sink) in enumerate(layers):
+            bg = _capi.f32(bg, dev, align16=True)
+            gl = (None,) * 3 if grads is None else tuple(_capi.f32(g, dev, align16=True) for g in grads)
+            keep_alive += [bg, *gl]
+            table[k] = _capi.SgrShardedLayer(b, e, bg.data_ptr(), states[k].data_ptr(), states[k].numel(), None, None, l_alpha.data_ptr(),
+                                             *(None if g is None else g.data_ptr() for g in gl), None if sink is None else sink.data_ptr())
+        _capi.call("sgr_sharded_backward_layers", dev, *args, C.byref(ws.layer_peers), table, len(layers))
+        del keep_alive, frs
     else:
         _capi.call("sgr_sharded_backward", dev, *args)
     del keep
@@ -580,6 +648,64 @@ def _fused_backward(ctx, grad_color, grad_depth, grad_alpha, grad_semantic):
     return _fit_grads(shapes, (g_means3D, g_means2D, g_sh, g_colors, g_sem, g_opac, g_scales, g_rots, g_cov)) + (None, None, None)
 
 
+class _GaussianShardedLayers(torch.autograd.Function):
+    """The fused step with render layers (sgr_sharded_forward_layers / sgr_sharded_backward_layers).  Outputs (color, radii, depth,
+    alpha, semantic), then (color, depth, alpha) per layer; `layers` holds _check_layers' tuples and `sinks` their means2D tensors."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, sh, colors_precomp, semantics, opacities, scales, rotations, cov3Ds_precomp, settings, owner,
+                differentiable, layers, *sinks):
+        # an output without upstream gradient arrives as None, so a layer without one costs nothing in backward
+        ctx.set_materialize_grads(False)
+        tensors = _local_tensors(means3D, sh, colors_precomp, None, opacities, scales, rotations, cov3Ds_precomp)
+        device, P = means3D.device, int(means3D.shape[0])
+        owner.chunk_for(P)
+        # (checked before workspace() may replace a workspace whose forward still awaits its backward)
+        if owner._ws is not None and owner._ws.in_flight:
+            raise _capi.SgrError("GaussianShardedRasterizer(exchange='p2p') owns ONE peer workspace: run backward() of the previous "
+                                 "forward (or call release_workspace()) before the next forward, or use one rasterizer per camera")
+        ws = owner.workspace(device, 0, len(layers))
+        cap = owner.capacity
+        if not cap.frozen:
+            cap.check()
+        H, W = int(settings.image_height), int(settings.image_width)
+        capacity = int(cap.capacity)
+        gcap = int(cap.gaussian_capacity) if cap.gaussian_capacity is not None else ws.P_total
+        color, depth, alpha, bufs, louts = sharded_forward_raw(settings, owner.band, ws, tensors, P, capacity, gcap,
+                                                               layers=[(b, e, bg) for b, e, bg, _ in layers])
+        if not cap.frozen:
+            frt, keep = _make_frame(settings, ws.P_total, 0, 0, device, owner.band)
+            cap.record_status(frt, ws.geom, device)
+            del keep
+        ws.in_flight = bool(differentiable)
+        ctx.settings, ctx.owner, ctx.ws, ctx.P, ctx.capacity, ctx.tensors, ctx.layers = settings, owner, ws, P, capacity, tensors, layers
+        ctx.shapes = _input_shapes(means3D, means2D, sh, colors_precomp, semantics, opacities, scales, rotations, cov3Ds_precomp)
+        ctx.save_for_backward(alpha, *(a for _, _, a in louts))
+        radii_out = bufs["radii"][:P]
+        ctx.mark_non_differentiable(radii_out)
+        return (color, radii_out, depth, alpha, torch.zeros((0, H, W), device=device, dtype=torch.float32), *(t for o in louts for t in o))
+
+    @staticmethod
+    def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha, grad_semantic, *grad_layers):
+        alpha, *layer_alphas = ctx.saved_tensors
+        settings, owner, ws, P, tensors = ctx.settings, ctx.owner, ctx.ws, ctx.P, ctx.tensors
+        dev = alpha.device
+        gc, gd, ga = (_capi.f32(g, dev, align16=True) for g in _image_grads(settings, dev, (grad_color, grad_depth, grad_alpha), (3, 1, 1)))
+        table = []
+        for k, (b, e, bg, sink) in enumerate(ctx.layers):
+            g3 = grad_layers[3 * k: 3 * k + 3]
+            grads = None if all(g is None for g in g3) else _image_grads(settings, dev, g3, (3, 1, 1))
+            sg = None
+            if grads is not None and sink is not None and ctx.needs_input_grad[13 + k]:
+                sg = torch.empty((e - b, 3), device=dev, dtype=torch.float32)
+            table.append((b, e, bg, layer_alphas[k], grads, sg))
+        out = sharded_backward_raw(settings, owner.band, ws, tensors, P, ctx.capacity, alpha, gc, gd, ga, layers=table)
+        ws.in_flight = False
+        g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rots, g_cov = out
+        return (_fit_grads(ctx.shapes, (g_means3D, g_means2D, g_sh, g_colors, None, g_opac, g_scales, g_rots, g_cov)) + (None,) * 4
+                + tuple(None if t[5] is None else t[5].to(dtype=l[3].dtype, device=l[3].device) for t, l in zip(table, ctx.layers)))
+
+
 class GaussianShardedRasterizer(nn.Module):
     """Same call signature as GaussianRasterizer.forward, but every argument holds only THIS rank's Gaussians and the
     returned radii / gradients cover only them; the images cover this rank's tile rows (zeros elsewhere).  The gathered
@@ -616,14 +742,16 @@ class GaussianShardedRasterizer(nn.Module):
         self.chunk = int(chunk) if chunk is not None else chunk_size(P_local, self.group)
         return self.chunk
 
-    def workspace(self, device, S: int = 0) -> "PeerWorkspace":
+    def workspace(self, device, S: int = 0, layers: int = 0) -> "PeerWorkspace":
         """COLLECTIVE on first use, after repartition() and when the number of feature channels the fused step carries changes:
-        allocate + rendezvous the peer-mapped buffer (keyed on (chunk, S))."""
-        if self._ws is None or self._ws.chunk != self.chunk or self._ws.S != S:
+        allocate + rendezvous the peer-mapped buffer (keyed on (chunk, S)).  A forward with render layers needs their sections: a
+        workspace with fewer is replaced, one with more is kept."""
+        if self._ws is None or self._ws.chunk != self.chunk or self._ws.S != S or self._ws.layers < layers:
+            layers = max(layers, self._ws.layers if self._ws is not None and self._ws.chunk == self.chunk and self._ws.S == S else 0)
             if self.world > 1:
-                self._ws = PeerWorkspace(self.raster_settings, self.chunk, self.world, self.rank, device, self.group, S=S)
+                self._ws = PeerWorkspace(self.raster_settings, self.chunk, self.world, self.rank, device, self.group, S=S, layers=layers)
             else:
-                self._ws = PeerWorkspace.emulate(self.raster_settings, self.chunk, 1, device, S)[0]
+                self._ws = PeerWorkspace.emulate(self.raster_settings, self.chunk, 1, device, S, layers)[0]
         return self._ws
 
     def pose_workspace(self) -> "PeerWorkspace":
@@ -656,8 +784,35 @@ class GaussianShardedRasterizer(nn.Module):
         if self.capacity is not None:
             self.capacity.check(wait=True)
 
-    def forward_layers(self, *args, **kwargs):
-        raise _capi.SgrError("render layers are single-GPU only: use GaussianRasterizer")
+    def forward_layers(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None,
+                       semantics=None, *, layers):
+        """forward() plus render layers, as GaussianRasterizer.forward_layers returns them: ``layers`` is a sequence of RenderLayer whose
+        ranges are in THIS rank's rows, and each layer's (color, depth, alpha) holds this rank's band of the layer rendered from the rows
+        of every rank (zeros elsewhere; the ranks' images sum to the single-GPU layer of the rank-major concatenation of their rows).
+        Every rank passes the same number of layers with the same bg, and every rank's loss must give the same layers a gradient (or
+        none): an owner gathers the other ranks' layer rows only for the layers whose outputs got a gradient on its own rank.  Only the fused peer-memory step renders layers:
+        exchange="p2p", fused=True, an InstanceCapacity that has learnt its capacity (a plain forward first), no feature channels and
+        at most two layers."""
+        mode = ("render layers under Gaussian sharding need the fused peer-memory step (elsewhere they are single-GPU: GaussianRasterizer): "
+                "exchange='p2p', fused=True, an InstanceCapacity")
+        exchange, fused, capacity = getattr(self, "exchange", None), getattr(self, "fused", False), getattr(self, "capacity", None)
+        if exchange != "p2p" or not fused:
+            raise _capi.SgrError(f"{mode} (this rasterizer has exchange={exchange!r}, fused={fused})")
+        if capacity is None or capacity.capacity is None:
+            raise _capi.SgrError(f"{mode} whose capacity is known: run a plain forward first")
+        if semantics is not None:
+            raise _capi.SgrError(f"{mode}, and no feature channels in the call")
+        if len(layers) > _capi.MAX_SHARDED_LAYERS:
+            raise _capi.SgrError(f"{mode}, and at most {_capi.MAX_SHARDED_LAYERS} layers (got {len(layers)})")
+        layers = tuple(_check_layers(layers, int(means3D.shape[0])))
+        shs, colors_precomp, scales, rotations, cov3D_precomp, _ = _reference_inputs(means3D, shs, colors_precomp, scales, rotations,
+                                                                                     cov3D_precomp, None)
+        if not means3D.is_cuda:
+            raise _capi.SgrError("street_gaussians_b200 rasterizer needs CUDA tensors (there is no CPU fallback)")
+        args = (means3D, means2D, shs, colors_precomp, None, opacities, scales, rotations, cov3D_precomp)
+        differentiable = torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in args)
+        out = _GaussianShardedLayers.apply(*args, self.raster_settings, self, differentiable, layers, *(l[3] for l in layers))
+        return tuple(out[:5]) + (tuple(tuple(out[5 + 3 * k: 8 + 3 * k]) for k in range(len(layers))),)
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None,
                 semantics=None):

@@ -25,6 +25,10 @@ With the argument `compose` (NCCL all_reduce of the accumulator rows) or `compos
 leg runs (run_compose): compose(..., group= / rasterizer=) on each rank's rows of a config-C-like scene, before and after the rebalanced
 split.  It has run at world 1 only, not on several H100s; tests/test_sharded_compose_gpu.py emulates 2 to 8 ranks on one GPU.
 
+With the argument `layers` only the render-layer leg runs (run_layers): GaussianShardedRasterizer.forward_layers with the objects-only and
+background-only layers through the fused peer-memory step, against GaussianRasterizer.forward_layers on the whole scene.  It has run at
+world 1 only, not on several H100s; tests/test_sharded_layers_gpu.py emulates 2 to 8 ranks on one GPU.
+
 With the argument `losses-p2p` only the loss leg runs, through the p2p rasterizer: frame_losses / the losses.py wrappers with rasterizer=,
 so the halo and the sums go over its peer workspace (sgr_band_halo_exchange_peers / sgr_band_peer_sum).  Each rank's values must be the
 same bytes on every rank and the whole frame's, and its gradient rows bit-equal to the single-GPU losses'.  It has run at world 1 only,
@@ -427,6 +431,69 @@ def run_compose(rank, world, dev, exchange, n_bg=400_000, actors=(20_000, 0, 7_0
     return P
 
 
+def run_layers(rank, world, dev, P=300_000, W=1280, H=720):
+    """The objects-only and background-only layers through the fused peer-memory step (forward_layers, exchange='p2p'), against
+    GaussianRasterizer.forward_layers on the whole scene: own rows of every image bit-equal, foreign rows zero, the gradients of the own
+    Gaussians and of each layer's means2D sink within GRAD_TOL.  The objects layer gets an alpha gradient on every rank (the
+    object-accumulation loss), the background layer none."""
+    scene = synthetic.make_scene(P=P, width=W, height=H, sh_degree=3, seed=78, pose=True)
+    st = util.settings_from(sgb, scene["cam"], dev)
+    n_bkgd = P - P // 5
+    chunk = (P + world - 1) // world
+    lo, hi = min(P, rank * chunk), min(P, (rank + 1) * chunk)
+    rows = band_of_rows(H, rank, world).to(dev)
+    m = rows.view(1, H, 1).float()
+    up = {k: scene[k].to(dev) for k in ("grad_color", "grad_depth", "grad_alpha")}
+    g_obj = torch.rand(1, H, W, device=dev, generator=torch.Generator(device=dev).manual_seed(5))
+    white = (1.0, 1.0, 1.0)
+
+    def call(rast, t, m2d, layers):
+        return rast.forward_layers(means3D=t["means3D"], means2D=m2d, opacities=t["opacities"], shs=t["shs"], scales=t["scales"],
+                                   rotations=t["rotations"], layers=layers)
+
+    full = {k: scene[k].to(dev).requires_grad_(True) for k in KEYS}
+    m2d_full = torch.zeros(P, 3, device=dev, requires_grad=True)
+    sinks_full = [torch.zeros(n_bkgd, 3, device=dev, requires_grad=True), torch.zeros(P - n_bkgd, 3, device=dev, requires_grad=True)]
+    ref = call(sgb.GaussianRasterizer(st), full, m2d_full, [sgb.RenderLayer(0, n_bkgd, white, sinks_full[0]),
+                                                             sgb.RenderLayer(n_bkgd, P, white, sinks_full[1])])
+    torch.autograd.backward([ref[0], ref[2], ref[3], ref[5][1][2]], [up["grad_color"], up["grad_depth"], up["grad_alpha"], g_obj])
+    rast = GaussianShardedRasterizer(st, capacity=sgb.InstanceCapacity(), exchange="p2p")
+    worst = 0.0
+    for rep in range(3):  # pass 1: plain (learns the capacities); passes 2-3: layered
+        loc = {k: scene[k][lo:hi].to(dev).requires_grad_(True) for k in KEYS}
+        m2d = torch.zeros(hi - lo, 3, device=dev, requires_grad=True)
+        if rep == 0:
+            got = rast(means3D=loc["means3D"], means2D=m2d, opacities=loc["opacities"], shs=loc["shs"], scales=loc["scales"],
+                       rotations=loc["rotations"])
+            torch.autograd.backward([got[0], got[2], got[3]], [up["grad_color"] * m, up["grad_depth"] * m, up["grad_alpha"] * m])
+            rast.synchronize_capacity()
+            continue
+        rb, re = min(hi - lo, max(0, n_bkgd - lo)), hi - lo  # this rank's rows of each layer, in its own rows
+        sinks = [torch.zeros(rb, 3, device=dev, requires_grad=True), torch.zeros(re - rb, 3, device=dev, requires_grad=True)]
+        got = call(rast, loc, m2d, [sgb.RenderLayer(0, rb, white, sinks[0]), sgb.RenderLayer(rb, re, white, sinks[1])])
+        torch.autograd.backward([got[0], got[2], got[3], got[5][1][2]], [up["grad_color"] * m, up["grad_depth"] * m, up["grad_alpha"] * m,
+                                                                         g_obj * m])
+        rast.synchronize_capacity()
+        images = [(got[0], ref[0]), (got[2], ref[2]), (got[3], ref[3])] + [(a, b) for k in range(2) for a, b in zip(got[5][k], ref[5][k])]
+        for i, (a, b) in enumerate(images):
+            assert torch.equal(a.detach()[:, rows], b.detach()[:, rows]), f"image {i}: own rows differ"
+            assert float(a.detach()[:, ~rows].abs().max()) == 0.0 if (~rows).any() else True, f"image {i}: foreign rows not zero"
+        pairs = [(loc[k].grad, full[k].grad[lo:hi], k) for k in KEYS] + [(m2d.grad, m2d_full.grad[lo:hi], "means2D")]
+        cut = lambda g, a, b: None if g is None else g[a:b]
+        pairs += [(sinks[0].grad, cut(sinks_full[0].grad, lo, lo + rb), "background sink"),
+                  (sinks[1].grad, cut(sinks_full[1].grad, max(0, lo - n_bkgd), hi - n_bkgd), "objects sink")]
+        for a, b, name in pairs:
+            if b is None:  # (the background layer has no gradient: neither call returns one for its sink)
+                assert a is None, (name, "a gradient where the single-GPU call has none")
+                continue
+            if b.numel() == 0:
+                continue
+            e = util.rel_err(a.double().cpu().numpy(), b.double().cpu().numpy())
+            worst = max(worst, e)
+            assert e < GRAD_TOL, (name, e)
+    return worst
+
+
 def run_all(rank, world, dev, exchange):
     # the last case carries feature channels through the bounded path: with exchange=p2p its passes 2-4 are the fused step with
     # semantics (sgr_sharded_*_features, no NCCL), with exchange=nccl the staged one
@@ -462,6 +529,9 @@ def main():
             P = run_compose(rank, world, dev, "p2p" if mode == "compose-p2p" else "nccl")
             print(f"[rank {rank}/{world}] compose ({mode}): {P} Gaussians, own rows bit-equal, dL/dposes and dL/dcorrection the same bytes on "
                   "every rank and the frame's", flush=True)
+        elif mode == "layers":
+            worst = run_layers(rank, world, dev)
+            print(f"[rank {rank}/{world}] render layers (fused p2p step): own rows bit-equal, gradients rel err {worst:.2e}", flush=True)
         elif mode == "rebalance":
             P_new = run_rebalance(rank, world, dev)
             print(f"[rank {rank}/{world}] rebalance: {P_new} Gaussians, rows / moments / statistics the even split's slice bit for bit, "
