@@ -758,6 +758,36 @@ size_t sgr_band_color_correct_scratch_bytes(int32_t H, int32_t W);
 int sgr_band_color_correct_backward(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *image, const float *affine,
                                     const float *dL_dout, float *dL_dimage, double *partials, void *scratch, size_t scratch_bytes, void *stream);
 int sgr_band_color_correct_affine_grad(const double *sums, float *dL_daffine, void *stream);
+/* The sky's cube gradient summed over peer memory (the Gaussian-sharded step's SgrPeers for world, rank and the barrier pad, plus every
+ * rank's sky section): no NCCL, no host read-back, and only the cube blocks some rank's band touched cross between ranks.  A block is
+ * 32 x 32 texels of one face (clipped at the face's last rows and columns when R is not a multiple of 32): sgr_sky_grad_blocks(R) =
+ * 6 ceil(R / 32)^2 of them, block b = (face * ceil(R / 32) + row / 32) * ceil(R / 32) + column / 32.
+ *   sgr_band_sky_composite_backward_marked : sgr_band_sky_composite_backward (dL_dcube required) that also fills block_map
+ *                           [sgr_sky_grad_blocks(R)] bytes: block_map is cleared, then set to 1 at the block of every texel the
+ *                           band's atomics add into (taps wrapped onto a neighbouring face included).  Same grid as the unmarked call.
+ *   sgr_sky_grad_peer_sum  : in place on this rank's dense partial dL_dcube, which must be zero outside the blocks its block_map marks
+ *                           (as the marking backward leaves it on a zeroed dL_dcube).  Stage: the marked blocks and the map go into the
+ *                           rank's own section, device barrier.  Owner sum: block b belongs to rank b % world, which adds, for p = 0,
+ *                           1, .., world - 1, the block of every rank p that marked it (fp32, from 0.0f) into its own section, device
+ *                           barrier.  Gather: every rank copies each block some rank marked from its owner's section into dL_dcube,
+ *                           device barrier.  So every rank ends with the same bytes, blocks no rank marked stay zero, and section
+ *                           bytes no rank staged in this call are never read.  Three launches of one 256-thread CTA per block (grids
+ *                           depend on R only) and three sgr_peer_barrier barriers with the device-side count (epoch 0).
+ *   sgr_sky_peer_bytes(R)  : bytes of one rank's sky section: [6 R^2 3 fp32, padded to 256 B | sgr_sky_grad_blocks(R) map bytes],
+ *                           padded to 256 B; 0 for a bad R.  sky_peers->bytes below it: SGR_ENOMEM.
+ * Every rank of `peers` makes the same calls with the same R.  Sections and dL_dcube must be 16-byte aligned (16-byte loads and
+ * stores).  Arguments are checked before anything is enqueued. */
+typedef struct SgrSkyPeers {
+	void *sec[SGR_MAX_PEERS];           /* rank p's sky section, mapped into every rank */
+	size_t bytes;                       /* size of every rank's sky section (sgr_sky_peer_bytes) */
+} SgrSkyPeers;
+int64_t sgr_sky_grad_blocks(int32_t R);
+size_t sgr_sky_peer_bytes(int32_t R);
+int sgr_band_sky_composite_backward_marked(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t R, int32_t mode,
+                                           float fill, const float *acc, const uint8_t *sky_mask, const float *cube_map, const float *K,
+                                           const float *w2c, const float *jitter_x, const float *jitter_y, const float *dL_dout, float *dL_dacc,
+                                           float *dL_dcube, uint8_t *block_map, void *stream);
+int sgr_sky_grad_peer_sum(const SgrPeers *peers, const SgrSkyPeers *sky_peers, int32_t R, const uint8_t *block_map, float *dL_dcube, void *stream);
 /* The feature maps' finishing (sgr_finish_features_forward / _backward) on a tile-row band: the whole-frame calls' arguments plus the
  * band.  rendered, normals, semantic, dL_dnormals, dL_dsemantic and dL_drendered are whole [C, H, W] frames; only the band's pixels are
  * read and written (the caller zeroes the other rows where it needs zeros), each at its frame index, so the band's rows equal the

@@ -36,7 +36,8 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_set_nea
            "sgr_band_image_loss_grad", "sgr_band_sky_loss", "sgr_band_obj_acc_loss", "sgr_band_acc_loss_value", "sgr_band_lidar_scratch_bytes",
            "sgr_band_lidar_keys", "sgr_band_lidar_select", "sgr_band_lidar_grad", "sgr_band_peer_bytes", "sgr_band_halo_exchange_peers",
            "sgr_band_peer_sum", "sgr_band_sky_composite_forward",
-           "sgr_band_sky_composite_backward", "sgr_band_color_correct_forward", "sgr_band_color_correct_scratch_bytes",
+           "sgr_band_sky_composite_backward", "sgr_sky_grad_blocks", "sgr_sky_peer_bytes", "sgr_band_sky_composite_backward_marked",
+           "sgr_sky_grad_peer_sum", "sgr_band_color_correct_forward", "sgr_band_color_correct_scratch_bytes",
            "sgr_band_color_correct_backward", "sgr_band_color_correct_affine_grad", "sgr_band_finish_features_forward",
            "sgr_band_finish_features_backward", "sgr_eval_metrics_scratch_bytes",
            "sgr_eval_metrics_accumulate", "sgr_band_eval_metrics_accumulate", "sgr_eval_metrics_finish"]
@@ -148,6 +149,10 @@ MAX_SHARDED_LAYERS = 2  # SGR_MAX_SHARDED_LAYERS: render layers of the fused Gau
 
 class SgrLayerPeers(C.Structure):
     _fields_ = [("layers", C.c_int32), ("reserved", C.c_int32), ("layer_mask", C.c_void_p * MAX_PEERS), ("layer_grad2d", C.c_void_p * MAX_PEERS)]
+
+
+class SgrSkyPeers(C.Structure):
+    _fields_ = [("sec", C.c_void_p * MAX_PEERS), ("bytes", C.c_size_t)]
 
 
 class SgrShardedLayer(C.Structure):
@@ -343,6 +348,14 @@ def lib():
     L.sgr_band_sky_composite_forward.argtypes = [C.c_int32] * 2 + band + [C.c_int32] * 2 + [C.c_float] + [vp] * 10
     L.sgr_band_sky_composite_backward.restype = C.c_int
     L.sgr_band_sky_composite_backward.argtypes = [C.c_int32] * 2 + band + [C.c_int32] * 2 + [C.c_float] + [vp] * 11
+    L.sgr_sky_grad_blocks.restype = C.c_int64
+    L.sgr_sky_grad_blocks.argtypes = [C.c_int32]
+    L.sgr_sky_peer_bytes.restype = C.c_size_t
+    L.sgr_sky_peer_bytes.argtypes = [C.c_int32]
+    L.sgr_band_sky_composite_backward_marked.restype = C.c_int
+    L.sgr_band_sky_composite_backward_marked.argtypes = [C.c_int32] * 2 + band + [C.c_int32] * 2 + [C.c_float] + [vp] * 12
+    L.sgr_sky_grad_peer_sum.restype = C.c_int
+    L.sgr_sky_grad_peer_sum.argtypes = [C.POINTER(SgrPeers), C.POINTER(SgrSkyPeers), C.c_int32, vp, vp, vp]
     L.sgr_band_color_correct_forward.restype = C.c_int
     L.sgr_band_color_correct_forward.argtypes = [C.c_int32] * 2 + band + [vp] * 4
     L.sgr_band_color_correct_scratch_bytes.restype = C.c_size_t

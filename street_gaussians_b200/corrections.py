@@ -10,7 +10,9 @@ two rows to `compose(..., pose_correction=...)`.  CUDA tensors only: there is no
 
 color_correct's band= / group= (keyword-only, as in losses.py): the image holds the rendered rows of this rank's TileRowBand
 (sharded.py); the band's rows are corrected (sgr_band_color_correct_*), and the backward all-reduces the band's 12 fp64 sums of
-dL/daffine over `group` before rounding them, so every rank's affine gradient is the whole frame's.
+dL/daffine over `group` before rounding them, so every rank's affine gradient is the whole frame's.  rasterizer= (a
+sharded.GaussianShardedRasterizer) supplies the band and the transport as in sky.py: with exchange="p2p" the 12 sums are added over
+peer memory (band_losses.peer_sum on the loss section), in ascending rank order, with no NCCL call and no host read-back.
 """
 from __future__ import annotations
 
@@ -39,7 +41,7 @@ def _affine(a: torch.Tensor, what: str, dev) -> torch.Tensor:
 
 class _ColorCorrect(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, image, affine, band, group):
+    def forward(ctx, image, affine, band, xfer):
         _check_cuda(image, "image")
         img = _capi.f32(image)
         if img.dim() != 3 or img.shape[0] != 3:
@@ -57,7 +59,7 @@ class _ColorCorrect(torch.autograd.Function):
             _capi.call("sgr_band_color_correct_forward", img.device, H, W, *rows, ptr(img), ptr(A), ptr(out))
         ctx.save_for_backward(img, A)
         ctx.dtypes = (image.dtype, affine.dtype)
-        ctx.band, ctx.group = rows, group
+        ctx.band, ctx.xfer = rows, xfer
         return out
 
     @staticmethod
@@ -75,31 +77,34 @@ class _ColorCorrect(torch.autograd.Function):
             scratch = torch.empty(nbytes, device=dev, dtype=torch.uint8)
             _capi.call("sgr_color_correct_backward", dev, H, W, ptr(img), ptr(A), ptr(g), ptr(g_img), ptr(g_A), ptr(scratch), nbytes)
         else:
-            from .band_losses import all_reduce_sum
             g_img = torch.zeros_like(img) if ctx.needs_input_grad[0] else None
             sums = torch.empty(12, device=dev, dtype=torch.float64)
             nbytes = int(L.sgr_band_color_correct_scratch_bytes(H, W))
             scratch = torch.empty(nbytes, device=dev, dtype=torch.uint8)
             _capi.call("sgr_band_color_correct_backward", dev, H, W, *ctx.band, ptr(img), ptr(A), ptr(g), ptr(g_img), ptr(sums), ptr(scratch), nbytes)
             if ctx.needs_input_grad[1]:  # COLLECTIVE: the band's 12 sums -> the frame's, rounded once to fp32
-                all_reduce_sum(sums, ctx.group)
+                ctx.xfer.sum(sums)
                 _capi.call("sgr_band_color_correct_affine_grad", dev, ptr(sums), ptr(g_A))
         return ((g_img.to(ctx.dtypes[0]) if g_img is not None else None), (g_A.to(ctx.dtypes[1]) if ctx.needs_input_grad[1] else None), None,
                 None)
 
 
-def color_correct(image: torch.Tensor, affine: torch.Tensor, *, band=None, group=None) -> torch.Tensor:
+def color_correct(image: torch.Tensor, affine: torch.Tensor, *, band=None, group=None, rasterizer=None) -> torch.Tensor:
     """einsum('ij,jhw->ihw', affine[:3, :3], image) + affine[:3, 3, None, None] for image [3, H, W]; differentiable in both.
 
     band= / group=: image holds the rendered rows of this rank's TileRowBand (sharded.py).  The output and dL/dimage have the band's
     rows, zeros elsewhere, equal bit for bit to the whole-frame call's rows.  COLLECTIVE in the backward: the 12 fp64 sums of
     dL/daffine are all-reduced over `group` (every rank must run its backward), then rounded once, so dL/daffine is the frame's on
     every rank and does not depend on how the rows are split (it may differ from the whole-frame call's fp32-accumulated sums by
-    their rounding).  An affine from the MLP mode works unchanged: its gradient flows back into the module as usual."""
-    if band is not None:  # a bad band fails before anything else
-        from .band_losses import check_band
-        check_band(band, int(image.shape[-2]))
-    return _ColorCorrect.apply(image, affine, band, group)
+    their rounding).  An affine from the MLP mode works unchanged: its gradient flows back into the module as usual.
+
+    rasterizer= (the GaussianShardedRasterizer that rendered the rows, whose forward must have run): its band, the whole frame at world
+    1; a band= or group= that differs from its own raises ValueError.  exchange="nccl": the all-reduce above over its group.
+    exchange="p2p": COLLECTIVE in the backward over its peer memory (no NCCL call, no host synchronisation); dL/daffine is the
+    ascending-rank fp64 sum of the 12 partials, rounded once, the same on every rank."""
+    from .sky import _resolve
+    rows, xfer = _resolve(band, group, rasterizer, int(image.shape[-2]))  # a bad or mismatched band fails before anything else
+    return _ColorCorrect.apply(image, affine, rows, xfer)
 
 
 class _Reg(torch.autograd.Function):

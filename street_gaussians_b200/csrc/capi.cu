@@ -1713,6 +1713,55 @@ int sgr_band_sky_composite_backward(int32_t H, int32_t W, int32_t row_begin, int
 	return SGR_OK;
 }
 
+int64_t sgr_sky_grad_blocks(int32_t R) { return (R > 0 && R <= 16384) ? sky_block_count(R) : 0; }
+size_t sgr_sky_peer_bytes(int32_t R) { return (R > 0 && R <= 16384) ? sky_peer_bytes(R) : 0; }
+
+int sgr_band_sky_composite_backward_marked(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t R, int32_t mode,
+                                           float fill, const float *acc, const uint8_t *sky_mask, const float *cube_map, const float *K,
+                                           const float *w2c, const float *jitter_x, const float *jitter_y, const float *dL_dout, float *dL_dacc,
+                                           float *dL_dcube, uint8_t *block_map, void *stream) {
+	const char *fn = "sgr_band_sky_composite_backward_marked";
+	Band band;
+	if (int rc = loss_band(fn, H, W, row_begin, row_end, row_step, &band)) return rc;
+	if (int rc = sky_check(fn, H, W, R, mode, sky_mask)) return rc;
+	if (!acc || !cube_map || !K || !w2c || !dL_dout || !dL_dcube || !block_map) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	if (!jitter_x != !jitter_y) return fail(SGR_EINVAL, "%s: give both jitters or neither", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_sky_composite_bwd(H, W, band, R, mode, fill, acc, sky_mask, cube_map, K, w2c, jitter_x, jitter_y, dL_dout, dL_dacc, dL_dcube, st,
+	                                 block_map),
+	        fn);
+	return SGR_OK;
+}
+
+int sgr_sky_grad_peer_sum(const SgrPeers *peers, const SgrSkyPeers *sky_peers, int32_t R, const uint8_t *block_map, float *dL_dcube, void *stream) {
+	const char *fn = "sgr_sky_grad_peer_sum";
+	if (!peers) return fail(SGR_EINVAL, "%s: peers is NULL", fn);
+	if (!sky_peers) return fail(SGR_EINVAL, "%s: sky_peers is NULL", fn);
+	if (peers->world < 1 || peers->world > SGR_MAX_PEERS || peers->rank < 0 || peers->rank >= peers->world)
+		return fail(SGR_EINVAL, "%s: bad peer table: world=%d rank=%d (at most %d ranks)", fn, peers->world, peers->rank, SGR_MAX_PEERS);
+	if (R <= 0 || R > 16384) return fail(SGR_EINVAL, "%s: bad sizes R=%d", fn, R);
+	if (!block_map || !dL_dcube) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	if (int rc = check_aligned16("dL_dcube", dL_dcube)) return rc;
+	PeerTable pt = {};
+	SkyPeers sp = {};
+	pt.world = peers->world;
+	pt.rank = peers->rank;
+	for (int p = 0; p < peers->world; p++) {
+		if (!sky_peers->sec[p]) return fail(SGR_EINVAL, "%s: sky section table entry %d is NULL", fn, p);
+		if (int rc = check_aligned16("a sky section", sky_peers->sec[p])) return rc;
+		if (peers->world > 1 && !peers->flags[p]) return fail(SGR_EINVAL, "%s: peer table entry %d has no barrier pad", fn, p);
+		sp.sec[p] = reinterpret_cast<char *>(sky_peers->sec[p]);
+		pt.flags[p] = peers->flags[p];
+	}
+	if (sky_peers->bytes < sky_peer_bytes(R))
+		return fail(SGR_ENOMEM, "%s: the sky sections hold %zu bytes, %zu needed", fn, sky_peers->bytes, sky_peer_bytes(R));
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_sky_grad_peer_sum(pt, sp, R, block_map, dL_dcube, st), fn);
+	return SGR_OK;
+}
+
 int sgr_band_color_correct_forward(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *image, const float *affine,
                                    float *out, void *stream) {
 	const char *fn = "sgr_band_color_correct_forward";

@@ -278,6 +278,117 @@ cudaError_t launch_band_peer_sum(const PeerTable &pt, const LossPeers &lp, bool 
 	return peer_sum<uint32_t>(pt, lp, count, static_cast<const uint32_t *>(local), static_cast<uint32_t *>(out), st);
 }
 
+// ---- the sky cube gradient's exchange (sgr_sky_grad_peer_sum) ----
+// A rank's sky section is [6 R^2 3 fp32, padded to 256 B | one byte per block].  Block b (face f, block row br, block column bc) is
+// owned by rank b % world.  Stage: the rank copies its marked blocks and its whole map into its section.  Owner sum: the owner adds,
+// from rank 0 up, the block of every rank that marked it and writes the sum into its own section (only the owner reads block b of any
+// section, so the in-place write races with nothing).  Gather: every rank copies each block of the union from the owner's section into
+// its dense gradient.  Barriers separate the three and end the call.  Grids are one CTA per block: they depend on R only.
+constexpr int kSkyXThreads = 256;
+
+// op.vec(i) on the 16-byte aligned float4 at float offset i, op.one(i) on a single float, over every float of block b's texels: one warp
+// per texel row of the block, the row's unaligned head and tail (when 3 R is not a multiple of 4) one float at a time.
+template <class Op>
+__device__ __forceinline__ void sky_block_floats(const int b, const int R, Op &op) {
+	const int nb = sky_blocks_per_side(R), f = b / (nb * nb), br = (b / nb) % nb, bc = b % nb;
+	const int r0 = br * kSkyBlock, r1 = min(R, r0 + kSkyBlock), c0 = bc * kSkyBlock, len = (min(R, c0 + kSkyBlock) - c0) * 3;
+	const int lane = threadIdx.x & 31;
+	for (int r = r0 + (int)(threadIdx.x >> 5); r < r1; r += kSkyXThreads / 32) {
+		const size_t s = ((size_t)(f * R + r) * R + c0) * 3;
+		const int head = min(len, (int)((4 - (s & 3)) & 3)), nv = (len - head) >> 2, tail = len - head - 4 * nv;
+		if (lane < head) op.one(s + lane);
+		for (int v = lane; v < nv; v += 32) op.vec(s + head + 4 * (size_t)v);
+		if (lane < tail) op.one(s + head + 4 * (size_t)nv + lane);
+	}
+}
+
+struct SkyCopy {
+	float *__restrict__ dst;
+	const float *__restrict__ src;
+	__device__ __forceinline__ void vec(size_t i) { *reinterpret_cast<float4 *>(dst + i) = *reinterpret_cast<const float4 *>(src + i); }
+	__device__ __forceinline__ void one(size_t i) { dst[i] = src[i]; }
+};
+
+// v = 0; for p = 0 .. world - 1 (bit p of `ranks` set): v += section p — the same adds per component for a float4 and a float
+struct SkySum {
+	float *__restrict__ dst;
+	const SkyPeers *sp;
+	uint32_t ranks;
+	int world;
+	__device__ __forceinline__ void vec(size_t i) {
+		float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+		for (int p = 0; p < world; p++) {
+			if (!((ranks >> p) & 1u)) continue;
+			const float4 x = *reinterpret_cast<const float4 *>(reinterpret_cast<const float *>(sp->sec[p]) + i);
+			v.x += x.x; v.y += x.y; v.z += x.z; v.w += x.w;
+		}
+		*reinterpret_cast<float4 *>(dst + i) = v;
+	}
+	__device__ __forceinline__ void one(size_t i) {
+		float v = 0.f;
+		for (int p = 0; p < world; p++)
+			if ((ranks >> p) & 1u) v += reinterpret_cast<const float *>(sp->sec[p])[i];
+		dst[i] = v;
+	}
+};
+
+__device__ __forceinline__ uint8_t *sky_section_map(char *sec, int R) { return reinterpret_cast<uint8_t *>(sec + sky_cube_section_bytes(R)); }
+
+// bit p set: rank p's staged map marks block b
+__device__ __forceinline__ uint32_t sky_block_ranks(const SkyPeers &sp, const int world, const int R, const int b) {
+	__shared__ uint32_t s_ranks;
+	if (threadIdx.x == 0) {
+		uint32_t bits = 0u;
+		for (int p = 0; p < world; p++) bits |= sky_section_map(sp.sec[p], R)[b] ? 1u << p : 0u;
+		s_ranks = bits;
+	}
+	__syncthreads();
+	return s_ranks;
+}
+
+__global__ void __launch_bounds__(kSkyXThreads) sky_stage_kernel(const __grid_constant__ SkyPeers sp, const int R, const int rank, const uint8_t *__restrict__ map,
+                                                                 const float *__restrict__ gcube) {
+	const int b = blockIdx.x;
+	const uint8_t m = map[b];
+	char *sec = sp.sec[rank];
+	if (threadIdx.x == 0) sky_section_map(sec, R)[b] = m ? 1 : 0;
+	if (!m) return;
+	SkyCopy op{reinterpret_cast<float *>(sec), gcube};
+	sky_block_floats(b, R, op);
+}
+
+__global__ void __launch_bounds__(kSkyXThreads) sky_owner_sum_kernel(const __grid_constant__ SkyPeers sp, const int R, const int world,
+                                                                     const int rank) {
+	const int b = blockIdx.x;
+	if (b % world != rank) return;
+	const uint32_t ranks = sky_block_ranks(sp, world, R, b);
+	if (!ranks) return;
+	SkySum op{reinterpret_cast<float *>(sp.sec[rank]), &sp, ranks, world};
+	sky_block_floats(b, R, op);
+}
+
+__global__ void __launch_bounds__(kSkyXThreads) sky_gather_kernel(const __grid_constant__ SkyPeers sp, const int R, const int world, float *__restrict__ gcube) {
+	const int b = blockIdx.x;
+	if (!sky_block_ranks(sp, world, R, b)) return;  // outside the union: the rank's partial is already zero there
+	SkyCopy op{gcube, reinterpret_cast<const float *>(sp.sec[b % world])};
+	sky_block_floats(b, R, op);
+}
+
+cudaError_t launch_sky_grad_peer_sum(const PeerTable &pt, const SkyPeers &sp, int R, const uint8_t *map, float *gcube, cudaStream_t st) {
+	const unsigned nblk = (unsigned)sky_block_count(R);
+	count_launch();
+	sky_stage_kernel<<<nblk, kSkyXThreads, 0, st>>>(sp, R, pt.rank, map, gcube);
+	cudaError_t e = cudaGetLastError();
+	if (e != cudaSuccess || (e = launch_peer_barrier(pt, 0u, nullptr, st)) != cudaSuccess) return e;
+	count_launch();
+	sky_owner_sum_kernel<<<nblk, kSkyXThreads, 0, st>>>(sp, R, pt.world, pt.rank);
+	if ((e = cudaGetLastError()) != cudaSuccess || (e = launch_peer_barrier(pt, 0u, nullptr, st)) != cudaSuccess) return e;
+	count_launch();
+	sky_gather_kernel<<<nblk, kSkyXThreads, 0, st>>>(sp, R, pt.world, gcube);
+	if ((e = cudaGetLastError()) != cudaSuccess) return e;
+	return launch_peer_barrier(pt, 0u, nullptr, st);
+}
+
 cudaError_t launch_scatter_records(const FrameDev &f, const PeerTable &pt, const GaussRec *rec, const int32_t *radii, cudaStream_t st) {
 	if (pt.chunk == 0) return cudaSuccess;
 	count_launch();

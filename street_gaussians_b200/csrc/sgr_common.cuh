@@ -523,7 +523,7 @@ cudaError_t launch_sky_composite_fwd(int H, int W, Band band, int R, int mode, f
                                      cudaStream_t st);
 cudaError_t launch_sky_composite_bwd(int H, int W, Band band, int R, int mode, float fill, const float *acc, const uint8_t *mask, const float *cube,
                                      const float *K, const float *w2c, const float *jx, const float *jy, const float *gout, float *gacc,
-                                     float *gcube, cudaStream_t st);
+                                     float *gcube, cudaStream_t st, uint8_t *block_map = nullptr);
 // tracked actor poses (actor_pose.cu): the device-resident track table and one call's camera
 constexpr int kActorPoseChunk = 256;  // actors per launch: their track slots travel as a kernel parameter
 struct ActorPoseTable {
@@ -590,6 +590,17 @@ size_t band_peer_bytes(int C, int H, int W);
 cudaError_t launch_band_halo_exchange(const PeerTable &pt, const LossPeers &lp, int C, int H, int W, Band band, const float *image, float *out,
                                       cudaStream_t st);
 cudaError_t launch_band_peer_sum(const PeerTable &pt, const LossPeers &lp, bool f64, long long count, const void *local, void *out, cudaStream_t st);
+// the sky cube gradient's exchange over peer memory (peer_exchange.cu): every rank's sky section [6 R^2 3 fp32 | block map]
+// (SgrSkyPeers).  A block is kSkyBlock x kSkyBlock texels of one face, clipped at the face's last row and column.
+constexpr int kSkyBlock = 32;
+struct SkyPeers {
+	char *sec[kMaxPeers];
+};
+__host__ __device__ __forceinline__ int sky_blocks_per_side(int R) { return (R + kSkyBlock - 1) / kSkyBlock; }
+__host__ __device__ __forceinline__ int64_t sky_block_count(int R) { return 6 * (int64_t)sky_blocks_per_side(R) * sky_blocks_per_side(R); }
+__host__ __device__ __forceinline__ size_t sky_cube_section_bytes(int R) { return ((size_t)18 * R * R * sizeof(float) + 255) / 256 * 256; }
+__host__ __device__ __forceinline__ size_t sky_peer_bytes(int R) { return (sky_cube_section_bytes(R) + (size_t)sky_block_count(R) + 255) / 256 * 256; }
+cudaError_t launch_sky_grad_peer_sum(const PeerTable &pt, const SkyPeers &sp, int R, const uint8_t *map, float *gcube, cudaStream_t st);
 cudaError_t launch_image_loss_stats(int C, int H, int W, Band band, const float *img, const float *gt, const uint8_t *mask, double *acc,
                                     void *scratch, cudaStream_t st);
 cudaError_t launch_image_loss_grad(int C, int H, int W, Band band, const float *img, const float *gt, const uint8_t *mask, const double *acc,

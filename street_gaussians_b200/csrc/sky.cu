@@ -6,7 +6,8 @@
 // (face of the largest component, face coordinates inverting cube_to_dir, sky_cubemap.py:154-161, bilinear over four taps with edge
 // and corner wrap), the clamp to [0, 1] and rgb + sky (1 - acc).  The backward recomputes the ray and the taps from the saved jitter.
 // Nothing depends on how many pixels are sky: grids depend on H x W only and nothing is read back to the host.  The band forms run the
-// same kernels over the pixels of a tile-row band only (multi-GPU, DESIGN.md §8): grids depend on H x W and the band.
+// same kernels over the pixels of a tile-row band only (multi-GPU, DESIGN.md §8): grids depend on H x W and the band.  The marking band
+// backward also records which kSkyBlock x kSkyBlock blocks of the cube its atomics wrote, for the peer-memory exchange (peer_exchange.cu).
 #include "sgr_common.cuh"
 
 namespace sgr {
@@ -184,8 +185,11 @@ __global__ void __launch_bounds__(kSkyThreads) sky_composite_fwd_kernel(const in
 }
 
 // One tap's three gradient values added into texel `idx` (-1: nothing).  The warp's pixels are consecutive, so equal texels come in
-// runs of lanes: a segmented suffix sum leaves each run's total in its first lane, which issues the only atomics of the run.
-__device__ __forceinline__ void sky_scatter(const int idx, float g0, float g1, float g2, float *__restrict__ gcube) {
+// runs of lanes: a segmented suffix sum leaves each run's total in its first lane, which issues the only atomics of the run.  kMark:
+// that lane also sets the byte of the texel's kSkyBlock x kSkyBlock block in `map`, so the map holds exactly the blocks written.
+template <bool kMark>
+__device__ __forceinline__ void sky_scatter(const int idx, float g0, float g1, float g2, float *__restrict__ gcube, uint8_t *__restrict__ map,
+                                            const int R) {
 	const unsigned full = 0xffffffffu;
 	const int lane = threadIdx.x & 31;
 	const int prev = __shfl_up_sync(full, idx, 1);
@@ -202,18 +206,29 @@ __device__ __forceinline__ void sky_scatter(const int idx, float g0, float g1, f
 		atomicAdd(gcube + (size_t)idx * 3 + 1, g1);
 		atomicAdd(gcube + (size_t)idx * 3 + 2, g2);
 	}
+	if (kMark) {  // one store per distinct block of the warp, and none where the block is already marked: few blocks, many writers
+		int blk = -1;
+		if (idx >= 0 && ((heads >> lane) & 1u)) {
+			const int RR = R * R, f = idx / RR, rem = idx - f * RR, r = rem / R, c = rem - r * R, nb = sky_blocks_per_side(R);
+			blk = (f * nb + r / kSkyBlock) * nb + c / kSkyBlock;
+		}
+		const unsigned same = __match_any_sync(full, blk);
+		if (blk >= 0 && lane == __ffs(same) - 1 && !map[blk]) map[blk] = 1;
+	}
 }
 
 // dL/dacc = -sum_c sky_c g_c; dL/dcube: each tap's weight times g (1 - acc) where 0 <= s <= 1, a corner tap's weight shared by thirds
 // among the three taps that exist.  dL/drgb is dL/dout itself.  Every lane of a warp reaches sky_scatter (idx = -1 past the image or the band).
-template <bool kBand>
+// kMark (band form only): also mark the blocks of the texels written in `map` (sky_scatter).
+template <bool kBand, bool kMark = false>
 __global__ void __launch_bounds__(kSkyThreads) sky_composite_bwd_kernel(const int64_t N, const int64_t M, const Band band, const int W, const int R,
                                                                         const int mode, const float fill,
                                                                         const float *__restrict__ acc, const uint8_t *__restrict__ mask,
                                                                         const float *__restrict__ cube, const float *__restrict__ K,
                                                                         const float *__restrict__ w2c, const float *__restrict__ jx,
                                                                         const float *__restrict__ jy, const float *__restrict__ gout,
-                                                                        float *__restrict__ gacc, float *__restrict__ gcube) {
+                                                                        float *__restrict__ gacc, float *__restrict__ gcube,
+                                                                        uint8_t *__restrict__ map) {
 	const int64_t item = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
 	const int64_t pix = kBand ? band_pixel(item, band, (int64_t)kBandTileRows * W) : item;
 	const bool live = item < M && pix < N;
@@ -252,7 +267,8 @@ __global__ void __launch_bounds__(kSkyThreads) sky_composite_bwd_kernel(const in
 	}
 	if (!gcube) return;  // uniform over the grid
 #pragma unroll
-	for (int k = 0; k < 4; k++) sky_scatter(t.idx[k], __fmul_rn(t.w[k], ds[0]), __fmul_rn(t.w[k], ds[1]), __fmul_rn(t.w[k], ds[2]), gcube);
+	for (int k = 0; k < 4; k++)
+		sky_scatter<kMark>(t.idx[k], __fmul_rn(t.w[k], ds[0]), __fmul_rn(t.w[k], ds[1]), __fmul_rn(t.w[k], ds[2]), gcube, map, R);
 }
 
 static int sky_blocks(int64_t N) { return (int)((N + kSkyThreads - 1) / kSkyThreads); }
@@ -273,7 +289,7 @@ cudaError_t launch_sky_composite_bwd(int H, int W, int R, int mode, float fill, 
 	const int64_t N = (int64_t)H * W;
 	count_launch();
 	sky_composite_bwd_kernel<false><<<sky_blocks(N), kSkyThreads, 0, st>>>(N, N, Band{0, 1, 1}, W, R, mode, fill, acc, mask, cube, K, w2c, jx, jy,
-	                                                                       gout, gacc, gcube);
+	                                                                       gout, gacc, gcube, nullptr);
 	return cudaGetLastError();
 }
 
@@ -288,14 +304,23 @@ cudaError_t launch_sky_composite_fwd(int H, int W, Band band, int R, int mode, f
 	return cudaGetLastError();
 }
 
+// With a block map (sgr_band_sky_composite_backward_marked): the map is cleared first, also for an empty band, then marked.
 cudaError_t launch_sky_composite_bwd(int H, int W, Band band, int R, int mode, float fill, const float *acc, const uint8_t *mask, const float *cube,
                                      const float *K, const float *w2c, const float *jx, const float *jy, const float *gout, float *gacc,
-                                     float *gcube, cudaStream_t st) {
+                                     float *gcube, cudaStream_t st, uint8_t *block_map) {
 	const int64_t N = (int64_t)H * W, M = (int64_t)band_rows(band) * kBandTileRows * W;
+	if (block_map) {
+		cudaError_t e = cudaMemsetAsync(block_map, 0, (size_t)sky_block_count(R), st);
+		if (e != cudaSuccess) return e;
+	}
 	if (M == 0) return cudaSuccess;
 	count_launch();
-	sky_composite_bwd_kernel<true><<<sky_blocks(M), kSkyThreads, 0, st>>>(N, M, band, W, R, mode, fill, acc, mask, cube, K, w2c, jx, jy, gout, gacc,
-	                                                                      gcube);
+	if (block_map)
+		sky_composite_bwd_kernel<true, true><<<sky_blocks(M), kSkyThreads, 0, st>>>(N, M, band, W, R, mode, fill, acc, mask, cube, K, w2c, jx, jy, gout,
+		                                                                            gacc, gcube, block_map);
+	else
+		sky_composite_bwd_kernel<true><<<sky_blocks(M), kSkyThreads, 0, st>>>(N, M, band, W, R, mode, fill, acc, mask, cube, K, w2c, jx, jy, gout, gacc,
+		                                                                      gcube, nullptr);
 	return cudaGetLastError();
 }
 

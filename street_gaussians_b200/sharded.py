@@ -379,6 +379,49 @@ class PeerWorkspace:
         return st[:n]
 
 
+class SkyWorkspace:
+    """Per-rank sky section [6 R^2 3 fp32 | block map] that every rank of the group can address (include/sgr.h, SgrSkyPeers), and this
+    rank's own block map: the sky cube gradient's exchange over peer memory (sky.sky_composite with rasterizer= of a
+    GaussianShardedRasterizer(exchange="p2p"), sgr_sky_grad_peer_sum).
+
+    Its own torch symmetric-memory allocation, keyed on (R, world), so it outlives the rasterizer's PeerWorkspace across repartition();
+    it has no barrier pad: the exchange takes its barriers from the rasterizer's current workspace.  `emulate(...)` builds `world`
+    ordinary buffers on ONE device that point at each other, as PeerWorkspace.emulate does."""
+
+    def __init__(self, R: int, world: int, rank: int, device, group=None, _buffers=None):
+        self.R, self.world, self.rank = int(R), int(world), int(rank)
+        if world > _capi.MAX_PEERS:
+            raise _capi.SgrError(f"peer exchange supports at most {_capi.MAX_PEERS} ranks, got {world}")
+        self.bytes, self.blocks = self.section_bytes(self.R), int(_capi.lib().sgr_sky_grad_blocks(self.R))
+        self.hdl = None
+        if _buffers is not None:
+            self.buf, ptrs = _buffers
+        else:
+            import torch.distributed._symmetric_memory as symm
+            self.buf = symm.empty(self.bytes, dtype=torch.uint8, device=device)
+            self.hdl = symm.rendezvous(self.buf, group if group is not None else dist.group.WORLD)
+            ptrs = list(self.hdl.buffer_ptrs)
+        self.peers = _capi.SgrSkyPeers()
+        for p in range(self.world):
+            self.peers.sec[p] = ptrs[p]
+        self.peers.bytes = self.bytes
+        self.block_map = torch.zeros(self.blocks, dtype=torch.uint8, device=device)
+
+    @staticmethod
+    def section_bytes(R: int) -> int:
+        n = int(_capi.lib().sgr_sky_peer_bytes(int(R)))
+        if n == 0:
+            raise _capi.SgrError(f"bad cube map resolution R={R} for the sky section")
+        return n
+
+    @classmethod
+    def emulate(cls, R: int, world: int, device):
+        """`world` sky workspaces on ONE device whose section tables point at each other (tests)."""
+        bufs = [torch.empty(cls.section_bytes(R), dtype=torch.uint8, device=device) for _ in range(world)]
+        ptrs = [b.data_ptr() for b in bufs]
+        return [cls(R, world, r, device, _buffers=(bufs[r], ptrs)) for r in range(world)]
+
+
 def scatter_records(settings, ws: PeerWorkspace, rec_local, radii_local, P_local: int):
     """Step 2 over peer memory (sgr_scatter_records).  The caller issues ws.barrier() afterwards."""
     device = rec_local.device
@@ -725,6 +768,7 @@ class GaussianShardedRasterizer(nn.Module):
         if exchange == "p2p" and layout != "cyclic":
             raise ValueError("the peer-memory exchange needs the cyclic tile-row layout")
         self.exchange, self._ws = exchange, None
+        self._sky = None  # SkyWorkspace of sky_workspace(R), kept across repartition()
         # exchange="p2p" with a capacity object (sync-free binning) and at most 32 feature channels runs the whole forward / backward as
         # ONE C-ABI call each (sgr_sharded_forward / sgr_sharded_backward) once the capacity is known; fused=False keeps the
         # staged calls (one per step of include/sgr.h's list)
@@ -769,6 +813,21 @@ class GaussianShardedRasterizer(nn.Module):
             raise _capi.SgrError("the band losses with rasterizer= and exchange='p2p' exchange over the rasterizer's peer workspace: run "
                                  "the rasterizer's forward before the losses")
         return self._ws
+
+    def sky_workspace(self, R: int, device=None) -> "SkyWorkspace":
+        """The sky section sky.sky_composite(rasterizer=self) exchanges the cube map's gradient through (exchange="p2p"): COLLECTIVE on
+        first use and when R changes (allocate + rendezvous, keyed on (R, world)), so the sky composite's forward, which every rank
+        runs, asks for it.  It is kept across repartition(); the exchange's barriers come from the current loss_workspace()."""
+        sky = self._sky
+        if sky is None or sky.R != int(R):
+            if device is None:
+                raise _capi.SgrError("the sky section is allocated in the sky composite's forward: pass its device")
+            if self.world > 1:
+                sky = SkyWorkspace(R, self.world, self.rank, device, self.group)
+            else:
+                sky = SkyWorkspace.emulate(R, 1, device)[0]
+            self._sky = sky
+        return sky
 
     def release_workspace(self):
         """Declare that the last differentiable forward will never be back-propagated (its graph was dropped)."""

@@ -13,9 +13,16 @@ draws on the current CUDA generator.  CUDA tensors only: there is no CPU fallbac
 band= / group= (keyword-only, as in losses.py): rgb and acc hold the rendered rows of this rank's TileRowBand (sharded.py); the
 composite runs on the band's pixels only (sgr_band_sky_composite_*), the output is zero outside the band, and the backward gives
 dL/dacc on the band's rows and all-reduces the cube map's gradient over `group`, so every rank's cube_map.grad is the whole frame's.
+
+rasterizer= (a sharded.GaussianShardedRasterizer, resolved like the band losses' band_losses.resolve): its band (the whole-frame
+entries at world 1) and its transport.  With exchange="nccl" the all-reduce above over its group.  With exchange="p2p" the backward
+marks the 32 x 32-texel blocks of the cube its band touched (sgr_band_sky_composite_backward_marked) and sums only those over peer
+memory (sgr_sky_grad_peer_sum, through the rasterizer's sky_workspace): no NCCL call, no host read-back, and every rank's
+cube_map.grad holds the same bytes, the ascending-rank fp32 sum of the ranks' partials block by block.
 """
 from __future__ import annotations
 
+import ctypes as C
 from typing import Optional
 
 import torch
@@ -61,11 +68,32 @@ def _band_rows(band, H: int):
     return check_band(band, H)
 
 
+def _resolve(band, group, rasterizer, H: int):
+    """(rows or None, band_losses.Transport) of a call: band= / group= as given without a rasterizer; with one, its band and transport
+    (band_losses.resolve, which refuses a band= or group= that differs from the rasterizer's), the whole frame at world 1."""
+    from .band_losses import Transport, resolve
+    if rasterizer is None:
+        return _band_rows(band, H), Transport(group)
+    own, xfer = resolve(band, group, rasterizer, H)
+    if rasterizer.band is None:
+        return None, Transport()
+    return _band_rows(own, H), xfer
+
+
+def sky_grad_peer_sum(ws, sky_ws, g_cube: torch.Tensor) -> torch.Tensor:
+    """COLLECTIVE over the ranks of the peer workspace `ws` (sgr_sky_grad_peer_sum, on the device): in place on this rank's partial
+    g_cube [6, R, R, 3], zero outside the blocks sky_ws.block_map marks (sgr_band_sky_composite_backward_marked on a zeroed g_cube),
+    every rank ends with the marked blocks' ascending-rank sum and zeros elsewhere.  Three barriers on ws's pad."""
+    ws.next_epochs(3)
+    _capi.call("sgr_sky_grad_peer_sum", g_cube.device, C.byref(ws.peers), C.byref(sky_ws.peers), int(g_cube.shape[1]), ptr(sky_ws.block_map),
+               ptr(g_cube))
+    return g_cube
+
+
 class _SkyComposite(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, rgb, acc, cube_map, K, w2c, sky_mask, perturb: bool, fill: float, band, group):
+    def forward(ctx, rgb, acc, cube_map, K, w2c, sky_mask, perturb: bool, fill: float, rows, xfer, rasterizer):
         H, W, R = _check(rgb, acc, cube_map, K, w2c, sky_mask)
-        rows = _band_rows(band, H)
         dev = rgb.device
         rgb_c, acc_c, cube = rgb.contiguous(), acc.contiguous(), cube_map.contiguous()
         Kc, Tc = K.contiguous(), w2c.contiguous()
@@ -86,7 +114,9 @@ class _SkyComposite(torch.autograd.Function):
                        ptr(Kc), ptr(Tc), ptr(jx), ptr(jy), ptr(out))
         ctx.save_for_backward(acc_c, cube, Kc, Tc, mask, jx, jy)
         ctx.args = (H, W, R, mode, float(fill))
-        ctx.band, ctx.group = rows, group
+        ctx.band, ctx.xfer = rows, xfer
+        # exchange="p2p": the sky section is collective on first use, so it is allocated here, where every rank runs
+        ctx.sky_ws = rasterizer.sky_workspace(R, dev) if rows is not None and xfer.kind == "p2p" else None
         return out
 
     @staticmethod
@@ -101,19 +131,23 @@ class _SkyComposite(torch.autograd.Function):
             g_acc = torch.empty_like(acc) if need_acc else None
             _capi.call("sgr_sky_composite_backward", dev, H, W, R, mode, fill, ptr(acc), ptr(mask), ptr(cube), ptr(Kc), ptr(Tc), ptr(jx),
                        ptr(jy), ptr(g), ptr(g_acc), ptr(g_cube))
+        elif ctx.sky_ws is not None and need_cube:  # COLLECTIVE over peer memory: only the blocks some band touched are exchanged
+            g_acc = torch.zeros_like(acc) if need_acc else None
+            _capi.call("sgr_band_sky_composite_backward_marked", dev, H, W, *ctx.band, R, mode, fill, ptr(acc), ptr(mask), ptr(cube), ptr(Kc),
+                       ptr(Tc), ptr(jx), ptr(jy), ptr(g), ptr(g_acc), ptr(g_cube), ptr(ctx.sky_ws.block_map))
+            sky_grad_peer_sum(ctx.xfer.ws, ctx.sky_ws, g_cube)
         else:
             g_acc = torch.zeros_like(acc) if need_acc else None
             _capi.call("sgr_band_sky_composite_backward", dev, H, W, *ctx.band, R, mode, fill, ptr(acc), ptr(mask), ptr(cube), ptr(Kc), ptr(Tc),
                        ptr(jx), ptr(jy), ptr(g), ptr(g_acc), ptr(g_cube))
             if need_cube:  # COLLECTIVE: this band's partial dL/dcube -> the whole frame's, on every rank
-                from .band_losses import all_reduce_sum
-                all_reduce_sum(g_cube, ctx.group)
-        return (g_out if need_rgb else None), g_acc, g_cube, None, None, None, None, None, None, None
+                ctx.xfer.sum(g_cube)
+        return (g_out if need_rgb else None), g_acc, g_cube, None, None, None, None, None, None, None, None
 
 
 def sky_composite(rgb: torch.Tensor, acc: torch.Tensor, cube_map: torch.Tensor, K: torch.Tensor, w2c: torch.Tensor, *,
                   sky_mask: Optional[torch.Tensor] = None, perturb: bool = False, white_background: bool = True, band=None,
-                  group=None) -> torch.Tensor:
+                  group=None, rasterizer=None) -> torch.Tensor:
     """rgb [3, H, W] + sky * (1 - acc [1, H, W]) with the sky sampled from cube_map [6, R, R, 3] along the rays of K [3, 3] and
     w2c [4, 4], clamped to [0, 1]; pixels the mask rule leaves out take 1 (white_background) or 0.  Differentiable in rgb, acc and
     cube_map.  sky_mask: bool [1, H, W] or [H, W] (training with the guidance mask), None for the acc rule.  All fp32 CUDA tensors.
@@ -122,6 +156,12 @@ def sky_composite(rgb: torch.Tensor, acc: torch.Tensor, cube_map: torch.Tensor, 
     output has the band's rows, zeros elsewhere, equal bit for bit to the whole-frame call's rows; dL/dacc covers the band's rows.
     COLLECTIVE in the backward: the cube map's gradient is all-reduced over `group` (every rank must run its backward).  perturb=True
     draws the same full-frame [H, W] jitter pair, in the same order, as the whole-frame call, so a rank's rows equal the single-GPU
-    call's whenever the ranks' CUDA generators are in the same state."""
-    _band_rows(band, int(rgb.shape[-2]))  # a bad band fails before anything else
-    return _SkyComposite.apply(rgb, acc, cube_map, K, w2c, sky_mask, bool(perturb), 1.0 if white_background else 0.0, band, group)
+    call's whenever the ranks' CUDA generators are in the same state.
+
+    rasterizer= (the GaussianShardedRasterizer that rendered the rows, whose forward must have run): its band, the whole frame at world
+    1; a band= or group= that differs from its own raises ValueError.  exchange="nccl": the all-reduce above over its group.
+    exchange="p2p": COLLECTIVE in the backward over its peer memory, no NCCL call and no host synchronisation; cube_map.grad is the
+    ascending-rank fp32 sum of the ranks' partials, block by block, and the same bytes on every rank.  Every rank must ask for the cube
+    map's gradient alike."""
+    rows, xfer = _resolve(band, group, rasterizer, int(rgb.shape[-2]))  # a bad or mismatched band fails before anything else
+    return _SkyComposite.apply(rgb, acc, cube_map, K, w2c, sky_mask, bool(perturb), 1.0 if white_background else 0.0, rows, xfer, rasterizer)

@@ -33,6 +33,11 @@ With the argument `losses-p2p` only the loss leg runs, through the p2p rasterize
 so the halo and the sums go over its peer workspace (sgr_band_halo_exchange_peers / sgr_band_peer_sum).  Each rank's values must be the
 same bytes on every rank and the whole frame's, and its gradient rows bit-equal to the single-GPU losses'.  It has run at world 1 only,
 not on several H100s; tests/test_band_losses_p2p_gpu.py emulates 2 to 8 ranks on one GPU.
+
+With the argument `image-p2p` only the sky and colour-correction leg runs, through the p2p rasterizer: sky_composite / color_correct with
+rasterizer=, so the cube map's touched blocks and the colour correction's sums go over its peer memory (sgr_sky_grad_peer_sum /
+sgr_band_peer_sum).  Rows as in the NCCL leg; both parameter gradients must also be the same bytes on every rank.  It has not been run
+on several H100s; tests/test_sky_p2p_gpu.py emulates 2 to 8 ranks on one GPU.
 """
 import os
 import sys
@@ -183,15 +188,17 @@ def run_losses(rank, world, dev, W=1280, H=720, exchange="nccl"):
             assert not bool(x[:, ~rows].any()), f"{name}: foreign gradient rows not zero"
 
 
-def run_image_stages(rank, world, dev, W=1280, H=720, R=256):
+def run_image_stages(rank, world, dev, W=1280, H=720, R=256, exchange="nccl"):
     """Sky and colour-correction leg: sky_composite and color_correct with band= / group= on each rank's banded render against the
     whole-frame calls on the gathered frame.  Output and image-gradient rows bit-equal, foreign rows zero; the all-reduced cube gradient
     equal to the whole-frame one up to the order of its float atomics (1e-5 of max|ref|), and the all-reduced affine gradient within one
-    fp32 ulp of its fp64 sum."""
+    fp32 ulp of its fp64 sum.  exchange="p2p": the two stages take rasterizer= of the p2p rasterizer that rendered the rows (the cube's
+    touched blocks and the affine sums over its peer memory), and both parameter gradients must also be the same bytes on every rank; at
+    world 1 those calls are the whole-frame ones, so the affine gradient is theirs bit for bit."""
     from street_gaussians_b200 import corrections
     scene = synthetic.make_scene(P=60_001, width=W, height=H, sh_degree=3, seed=79, pose=True)
     st = util.settings_from(sgb, scene["cam"], dev)
-    rast = GaussianShardedRasterizer(st)
+    rast = GaussianShardedRasterizer(st, exchange=exchange)
     P = scene["means3D"].shape[0]
     chunk = (P + world - 1) // world
     lo, hi = min(P, rank * chunk), min(P, (rank + 1) * chunk)
@@ -216,8 +223,9 @@ def run_image_stages(rank, world, dev, W=1280, H=720, R=256):
 
     def step(rgb, a, b):
         xs = [t.detach().clone().requires_grad_(True) for t in (rgb, a, cube, affine)]
-        out = sgb.sky_composite(xs[0], xs[1], xs[2], K, w2c, sky_mask=sky_mask, band=b)
-        col = corrections.color_correct(out, xs[3], band=b)
+        kw = dict(rasterizer=rast) if b is not None and exchange == "p2p" else dict(band=b)
+        out = sgb.sky_composite(xs[0], xs[1], xs[2], K, w2c, sky_mask=sky_mask, **kw)
+        col = corrections.color_correct(out, xs[3], **kw)
         col.backward(torch.where(rows.view(1, -1, 1), up, torch.zeros_like(up)) if b is not None else up)
         return [col.detach()] + [x.grad for x in xs]
 
@@ -230,7 +238,15 @@ def run_image_stages(rank, world, dev, W=1280, H=720, R=256):
     assert float((got[3] - ref[3]).abs().max()) <= 1e-5 * float(ref[3].abs().max()), "dL/dcube"
     x64 = torch.cat([sgb.sky_composite(*full, cube, K, w2c, sky_mask=sky_mask).detach().reshape(3, -1), torch.ones(1, H * W, device=dev)]).double()
     exact = (up.reshape(3, -1).double() @ x64.T).cpu().numpy()
-    assert (np.abs(got[4].cpu().double().numpy() - exact) <= np.spacing(np.abs(exact).astype(np.float32))).all(), "dL/daffine"
+    if exchange == "p2p" and world == 1:  # rasterizer= at world 1 takes the whole-frame calls: the reference's own fp32 sums
+        assert torch.equal(bits(got[4]), bits(ref[4])), "dL/daffine"
+    else:
+        assert (np.abs(got[4].cpu().double().numpy() - exact) <= np.spacing(np.abs(exact).astype(np.float32))).all(), "dL/daffine"
+    if exchange == "p2p" and world > 1:
+        for name, x in (("dL/dcube", got[3]), ("dL/daffine", got[4])):
+            first = x.clone()
+            dist.broadcast(first, 0)
+            assert torch.equal(bits(x), bits(first)), f"{name}: bytes differ from rank 0's"
 
 
 def run_features(rank, world, dev, W=1280, H=720, K=4):
@@ -525,6 +541,10 @@ def main():
             run_losses(rank, world, dev, exchange="p2p")
             print(f"[rank {rank}/{world}] band losses over peer memory: the same values on every rank, the frame's, gradient rows bit-equal "
                   "to the single-GPU losses", flush=True)
+        elif mode == "image-p2p":
+            run_image_stages(rank, world, dev, exchange="p2p")
+            print(f"[rank {rank}/{world}] sky and colour correction over peer memory: rows bit-equal to the single-GPU calls, parameter "
+                  "gradients the frame's and the same bytes on every rank", flush=True)
         elif mode in ("compose", "compose-p2p"):
             P = run_compose(rank, world, dev, "p2p" if mode == "compose-p2p" else "nccl")
             print(f"[rank {rank}/{world}] compose ({mode}): {P} Gaussians, own rows bit-equal, dL/dposes and dL/dcorrection the same bytes on "
