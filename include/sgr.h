@@ -788,6 +788,23 @@ int sgr_band_sky_composite_backward_marked(int32_t H, int32_t W, int32_t row_beg
                                            const float *w2c, const float *jitter_x, const float *jitter_y, const float *dL_dout, float *dL_dacc,
                                            float *dL_dcube, uint8_t *block_map, void *stream);
 int sgr_sky_grad_peer_sum(const SgrPeers *peers, const SgrSkyPeers *sky_peers, int32_t R, const uint8_t *block_map, float *dL_dcube, void *stream);
+/* The marks the block-masked cube Adam (sgr_cube_sparse_adam_step below) consumes, accumulated over backward passes:
+ *   sgr_band_sky_composite_backward_or_marks : sgr_band_sky_composite_backward_marked without the clearing: the band's blocks are
+ *                           set to 1 in block_map and every other byte keeps its value (the same kernel and grid as the marking call).
+ *                           With the band of every tile row (0, ceil(H / 16), 1) its dL_dacc equals sgr_sky_composite_backward's bit
+ *                           for bit and its dL_dcube equals it up to the order of the texels' float atomics.
+ *   sgr_sky_grad_peer_sum_union : sgr_sky_grad_peer_sum that also sets union_map[b] = 1 (other bytes kept) for every block some rank's
+ *                           staged map marks.  The gather reads the union from the staged maps in the ranks' sky sections, so every
+ *                           rank writes the same bytes into its own union_map, a [sgr_sky_grad_blocks(R)]-byte device buffer distinct
+ *                           from block_map.  No rank can re-mark a staged map before every peer has read it: a section's map is written
+ *                           only by its rank's stage launch, the next one comes after this call's last barrier, and every rank reaches
+ *                           that barrier only after its gather has read all the maps.  A caller's union_map is never read by a peer. */
+int sgr_band_sky_composite_backward_or_marks(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t R, int32_t mode,
+                                             float fill, const float *acc, const uint8_t *sky_mask, const float *cube_map, const float *K,
+                                             const float *w2c, const float *jitter_x, const float *jitter_y, const float *dL_dout, float *dL_dacc,
+                                             float *dL_dcube, uint8_t *block_map, void *stream);
+int sgr_sky_grad_peer_sum_union(const SgrPeers *peers, const SgrSkyPeers *sky_peers, int32_t R, const uint8_t *block_map, float *dL_dcube,
+                                uint8_t *union_map, void *stream);
 /* The feature maps' finishing (sgr_finish_features_forward / _backward) on a tile-row band: the whole-frame calls' arguments plus the
  * band.  rendered, normals, semantic, dL_dnormals, dL_dsemantic and dL_drendered are whole [C, H, W] frames; only the band's pixels are
  * read and written (the caller zeroes the other rows where it needs zeros), each at its frame index, so the band's rows equal the
@@ -994,6 +1011,18 @@ typedef struct SgrSparseAdamSegment {
 } SgrSparseAdamSegment;
 int sgr_sparse_adam_step(const SgrSparseAdamSegment *segments, int32_t num_segments, const int32_t *radii, double beta1, double beta2,
                          double eps, void *stream);
+
+/* ---- Block-masked Adam of the sky cube map: an OPT-IN deviation from the reference (whose torch.optim.Adam steps every texel) ----
+ * One Adam step of cube->param [6, R, R, 3] (cube->numel must be 6 R^2 3) over the 32 x 32-texel blocks block_map marks, numbered as for
+ * sgr_sky_grad_blocks (block_map holds sgr_sky_grad_blocks(R) bytes, any non-zero byte marks):
+ *   marked blocks:   exactly sgr_adam_step's update of their texels (same arithmetic, same rounding: bit-equal), with cube->lr and
+ *                    cube->step; then the block's byte is set to 0, so the map comes back empty;
+ *   unmarked blocks: param, exp_avg and exp_avg_sq are not written and grad is not read.
+ * `step` is the 1-based step count after this update, as for sgr_adam_step; there are no per-block step counts.  One launch of one
+ * 256-thread CTA per block: the grid depends on R only and nothing is read back, so the call can be captured in a CUDA graph.  Traffic:
+ * 1 B per block plus 28 B per float of a marked block.  0 < R <= 16384; pointers are device memory, fp32 (scalar accesses: no alignment
+ * beyond 4 B); betas / eps are doubles for the same reason as in sgr_adam_step.  Arguments are checked before anything is enqueued. */
+int sgr_cube_sparse_adam_step(int32_t R, const SgrAdamTensor *cube, uint8_t *block_map, double beta1, double beta2, double eps, void *stream);
 
 /* present[P] (uint8 0/1) = view-space z > 0.2.  Replaces markVisible -> checkFrustum
  * (DGR/rasterize_points.cu:222-241, rasterizer_impl.cu:54-66, 141-153; pybind `mark_visible`, DGR/ext.cpp:18). */

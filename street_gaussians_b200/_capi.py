@@ -40,7 +40,8 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_set_nea
            "sgr_sky_grad_peer_sum", "sgr_band_color_correct_forward", "sgr_band_color_correct_scratch_bytes",
            "sgr_band_color_correct_backward", "sgr_band_color_correct_affine_grad", "sgr_band_finish_features_forward",
            "sgr_band_finish_features_backward", "sgr_eval_metrics_scratch_bytes",
-           "sgr_eval_metrics_accumulate", "sgr_band_eval_metrics_accumulate", "sgr_eval_metrics_finish"]
+           "sgr_eval_metrics_accumulate", "sgr_band_eval_metrics_accumulate", "sgr_eval_metrics_finish",
+           "sgr_band_sky_composite_backward_or_marks", "sgr_sky_grad_peer_sum_union", "sgr_cube_sparse_adam_step"]
 
 SKY_MASK_ACC, SKY_MASK_GIVEN = 0, 1
 SEMANTIC_LOGITS, SEMANTIC_PROBABILITIES = 0, 1
@@ -356,6 +357,10 @@ def lib():
     L.sgr_band_sky_composite_backward_marked.argtypes = [C.c_int32] * 2 + band + [C.c_int32] * 2 + [C.c_float] + [vp] * 12
     L.sgr_sky_grad_peer_sum.restype = C.c_int
     L.sgr_sky_grad_peer_sum.argtypes = [C.POINTER(SgrPeers), C.POINTER(SgrSkyPeers), C.c_int32, vp, vp, vp]
+    L.sgr_band_sky_composite_backward_or_marks.restype = C.c_int
+    L.sgr_band_sky_composite_backward_or_marks.argtypes = L.sgr_band_sky_composite_backward_marked.argtypes
+    L.sgr_sky_grad_peer_sum_union.restype = C.c_int
+    L.sgr_sky_grad_peer_sum_union.argtypes = [C.POINTER(SgrPeers), C.POINTER(SgrSkyPeers), C.c_int32, vp, vp, vp, vp]
     L.sgr_band_color_correct_forward.restype = C.c_int
     L.sgr_band_color_correct_forward.argtypes = [C.c_int32] * 2 + band + [vp] * 4
     L.sgr_band_color_correct_scratch_bytes.restype = C.c_size_t
@@ -399,6 +404,8 @@ def lib():
     L.sgr_rebalance_splice.argtypes = [C.POINTER(SgrDensifySegment), C.POINTER(SgrDensifyOutput), C.c_int32] + rebalance_tables
     L.sgr_sparse_adam_step.restype = C.c_int
     L.sgr_sparse_adam_step.argtypes = [C.POINTER(SgrSparseAdamSegment), C.c_int32, vp, C.c_double, C.c_double, C.c_double, vp]
+    L.sgr_cube_sparse_adam_step.restype = C.c_int
+    L.sgr_cube_sparse_adam_step.argtypes = [C.c_int32, C.POINTER(SgrAdamTensor), vp, C.c_double, C.c_double, C.c_double, vp]
     L.sgr_layer_state_sizes.restype = C.c_int
     L.sgr_layer_state_sizes.argtypes = [C.POINTER(SgrFrame), C.c_int64, C.POINTER(C.c_size_t)]
     L.sgr_forward_layer.restype = C.c_int

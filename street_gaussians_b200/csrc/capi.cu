@@ -1716,11 +1716,10 @@ int sgr_band_sky_composite_backward(int32_t H, int32_t W, int32_t row_begin, int
 int64_t sgr_sky_grad_blocks(int32_t R) { return (R > 0 && R <= 16384) ? sky_block_count(R) : 0; }
 size_t sgr_sky_peer_bytes(int32_t R) { return (R > 0 && R <= 16384) ? sky_peer_bytes(R) : 0; }
 
-int sgr_band_sky_composite_backward_marked(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t R, int32_t mode,
-                                           float fill, const float *acc, const uint8_t *sky_mask, const float *cube_map, const float *K,
-                                           const float *w2c, const float *jitter_x, const float *jitter_y, const float *dL_dout, float *dL_dacc,
-                                           float *dL_dcube, uint8_t *block_map, void *stream) {
-	const char *fn = "sgr_band_sky_composite_backward_marked";
+static int sky_backward_marking(const char *fn, bool clear_map, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step,
+                                int32_t R, int32_t mode, float fill, const float *acc, const uint8_t *sky_mask, const float *cube_map,
+                                const float *K, const float *w2c, const float *jitter_x, const float *jitter_y, const float *dL_dout,
+                                float *dL_dacc, float *dL_dcube, uint8_t *block_map, void *stream) {
 	Band band;
 	if (int rc = loss_band(fn, H, W, row_begin, row_end, row_step, &band)) return rc;
 	if (int rc = sky_check(fn, H, W, R, mode, sky_mask)) return rc;
@@ -1729,13 +1728,29 @@ int sgr_band_sky_composite_backward_marked(int32_t H, int32_t W, int32_t row_beg
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 	const bool debug = false;
 	SGR_TRY(launch_sky_composite_bwd(H, W, band, R, mode, fill, acc, sky_mask, cube_map, K, w2c, jitter_x, jitter_y, dL_dout, dL_dacc, dL_dcube, st,
-	                                 block_map),
+	                                 block_map, clear_map),
 	        fn);
 	return SGR_OK;
 }
 
-int sgr_sky_grad_peer_sum(const SgrPeers *peers, const SgrSkyPeers *sky_peers, int32_t R, const uint8_t *block_map, float *dL_dcube, void *stream) {
-	const char *fn = "sgr_sky_grad_peer_sum";
+int sgr_band_sky_composite_backward_marked(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t R, int32_t mode,
+                                           float fill, const float *acc, const uint8_t *sky_mask, const float *cube_map, const float *K,
+                                           const float *w2c, const float *jitter_x, const float *jitter_y, const float *dL_dout, float *dL_dacc,
+                                           float *dL_dcube, uint8_t *block_map, void *stream) {
+	return sky_backward_marking("sgr_band_sky_composite_backward_marked", true, H, W, row_begin, row_end, row_step, R, mode, fill, acc, sky_mask,
+	                            cube_map, K, w2c, jitter_x, jitter_y, dL_dout, dL_dacc, dL_dcube, block_map, stream);
+}
+
+int sgr_band_sky_composite_backward_or_marks(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, int32_t R, int32_t mode,
+                                             float fill, const float *acc, const uint8_t *sky_mask, const float *cube_map, const float *K,
+                                             const float *w2c, const float *jitter_x, const float *jitter_y, const float *dL_dout, float *dL_dacc,
+                                             float *dL_dcube, uint8_t *block_map, void *stream) {
+	return sky_backward_marking("sgr_band_sky_composite_backward_or_marks", false, H, W, row_begin, row_end, row_step, R, mode, fill, acc,
+	                            sky_mask, cube_map, K, w2c, jitter_x, jitter_y, dL_dout, dL_dacc, dL_dcube, block_map, stream);
+}
+
+static int sky_peer_sum(const char *fn, const SgrPeers *peers, const SgrSkyPeers *sky_peers, int32_t R, const uint8_t *block_map, float *dL_dcube,
+                        uint8_t *union_map, void *stream) {
 	if (!peers) return fail(SGR_EINVAL, "%s: peers is NULL", fn);
 	if (!sky_peers) return fail(SGR_EINVAL, "%s: sky_peers is NULL", fn);
 	if (peers->world < 1 || peers->world > SGR_MAX_PEERS || peers->rank < 0 || peers->rank >= peers->world)
@@ -1758,8 +1773,20 @@ int sgr_sky_grad_peer_sum(const SgrPeers *peers, const SgrSkyPeers *sky_peers, i
 		return fail(SGR_ENOMEM, "%s: the sky sections hold %zu bytes, %zu needed", fn, sky_peers->bytes, sky_peer_bytes(R));
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 	const bool debug = false;
-	SGR_TRY(launch_sky_grad_peer_sum(pt, sp, R, block_map, dL_dcube, st), fn);
+	SGR_TRY(launch_sky_grad_peer_sum(pt, sp, R, block_map, dL_dcube, st, union_map), fn);
 	return SGR_OK;
+}
+
+int sgr_sky_grad_peer_sum(const SgrPeers *peers, const SgrSkyPeers *sky_peers, int32_t R, const uint8_t *block_map, float *dL_dcube, void *stream) {
+	return sky_peer_sum("sgr_sky_grad_peer_sum", peers, sky_peers, R, block_map, dL_dcube, nullptr, stream);
+}
+
+int sgr_sky_grad_peer_sum_union(const SgrPeers *peers, const SgrSkyPeers *sky_peers, int32_t R, const uint8_t *block_map, float *dL_dcube,
+                                uint8_t *union_map, void *stream) {
+	const char *fn = "sgr_sky_grad_peer_sum_union";
+	if (!union_map) return fail(SGR_EINVAL, "%s: union_map is NULL", fn);
+	if (union_map == block_map) return fail(SGR_EINVAL, "%s: union_map must not be block_map", fn);
+	return sky_peer_sum(fn, peers, sky_peers, R, block_map, dL_dcube, union_map, stream);
 }
 
 int sgr_band_color_correct_forward(int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step, const float *image, const float *affine,
@@ -1911,6 +1938,22 @@ int sgr_adam_step(const SgrAdamTensor *tensors, int32_t num_tensors, double beta
 	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 	const bool debug = false;
 	SGR_TRY(launch_adam(tensors, num_tensors, beta1, beta2, eps, st), "adam");
+	return SGR_OK;
+}
+
+int sgr_cube_sparse_adam_step(int32_t R, const SgrAdamTensor *cube, uint8_t *block_map, double beta1, double beta2, double eps, void *stream) {
+	const char *fn = "sgr_cube_sparse_adam_step";
+	if (R <= 0 || R > 16384) return fail(SGR_EINVAL, "%s: bad sizes R=%d", fn, R);
+	if (!cube || !block_map) return fail(SGR_EINVAL, "NULL pointer passed to %s", fn);
+	if (!cube->param || !cube->grad || !cube->exp_avg || !cube->exp_avg_sq) return fail(SGR_EINVAL, "%s: the cube has a NULL pointer", fn);
+	if (cube->numel != (int64_t)18 * R * R)
+		return fail(SGR_EINVAL, "%s: numel %lld is not 6 R^2 3 = %lld for R=%d", fn, (long long)cube->numel, (long long)18 * R * R, R);
+	if (cube->step < 1) return fail(SGR_EINVAL, "%s: step %d (step counts from 1)", fn, cube->step);
+	if (!std::isfinite(cube->lr)) return fail(SGR_EINVAL, "%s: non-finite lr", fn);
+	if (!(beta1 >= 0.0 && beta1 < 1.0) || !(beta2 >= 0.0 && beta2 < 1.0)) return fail(SGR_EINVAL, "%s: betas must lie in [0, 1)", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_cube_sparse_adam(R, *cube, block_map, beta1, beta2, eps, st), fn);
 	return SGR_OK;
 }
 

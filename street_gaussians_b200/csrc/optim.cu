@@ -202,4 +202,37 @@ cudaError_t launch_sparse_adam(const SgrSparseAdamSegment *segs, int nseg, const
 	return cudaGetLastError();
 }
 
+// ---- block-masked Adam of the sky cube map ----
+// One CTA per kSkyBlock x kSkyBlock block of the cube [6, R, R, 3] (the blocks sgr_sky_grad_blocks numbers), so the grid depends on R
+// only.  Thread 0 reads the block's map byte and clears it; a block whose byte was 0 returns before touching any tensor.  A marked block
+// walks its texel rows one warp per row (3 x its width contiguous floats), each float through adam_update, so the traffic is 1 B per
+// block plus 28 B per float of a marked block.
+constexpr int kCubeAdamThreads = 256;
+
+__global__ void __launch_bounds__(kCubeAdamThreads) cube_sparse_adam_kernel(const int R, float *__restrict__ p, const float *__restrict__ g,
+                                                                           float *__restrict__ m, float *__restrict__ v,
+                                                                           uint8_t *__restrict__ map, const float omb1, const float b2,
+                                                                           const float omb2, const float eps, const float ss, const float ibc2) {
+	const int b = blockIdx.x;
+	if (!__syncthreads_or(threadIdx.x == 0 && map[b] != 0)) return;
+	if (threadIdx.x == 0) map[b] = 0;  // only thread 0 read it, before the barrier
+	const int nb = sky_blocks_per_side(R), f = b / (nb * nb), br = (b / nb) % nb, bc = b % nb;
+	const int r0 = br * kSkyBlock, r1 = min(R, r0 + kSkyBlock), c0 = bc * kSkyBlock, len = (min(R, c0 + kSkyBlock) - c0) * 3;
+	const int lane = threadIdx.x & 31;
+	for (int r = r0 + (int)(threadIdx.x >> 5); r < r1; r += kCubeAdamThreads / 32) {
+		const size_t s = ((size_t)(f * R + r) * R + c0) * 3;
+		for (int e = lane; e < len; e += 32) adam_update(p, g, m, v, s + e, omb1, b2, omb2, eps, ss, ibc2);
+	}
+}
+
+cudaError_t launch_cube_sparse_adam(int R, const SgrAdamTensor &a, uint8_t *map, double beta1, double beta2, double eps, cudaStream_t st) {
+	float ss, ibc2;
+	adam_scalars(a.lr, a.step, beta1, beta2, &ss, &ibc2);
+	count_launch();
+	cube_sparse_adam_kernel<<<(unsigned)sky_block_count(R), kCubeAdamThreads, 0, st>>>(R, a.param, a.grad, a.exp_avg, a.exp_avg_sq, map,
+	                                                                                  (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2),
+	                                                                                  (float)eps, ss, ibc2);
+	return cudaGetLastError();
+}
+
 }  // namespace sgr

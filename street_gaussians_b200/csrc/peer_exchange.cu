@@ -374,7 +374,19 @@ __global__ void __launch_bounds__(kSkyXThreads) sky_gather_kernel(const __grid_c
 	sky_block_floats(b, R, op);
 }
 
-cudaError_t launch_sky_grad_peer_sum(const PeerTable &pt, const SkyPeers &sp, int R, const uint8_t *map, float *gcube, cudaStream_t st) {
+// The gather that also sets union_map[b] for every block some rank marked (sgr_sky_grad_peer_sum_union): every rank reads the same
+// staged maps, so every rank writes the same bytes.
+__global__ void __launch_bounds__(kSkyXThreads) sky_gather_union_kernel(const __grid_constant__ SkyPeers sp, const int R, const int world,
+                                                                        float *__restrict__ gcube, uint8_t *__restrict__ union_map) {
+	const int b = blockIdx.x;
+	if (!sky_block_ranks(sp, world, R, b)) return;
+	if (threadIdx.x == 0) union_map[b] = 1;
+	SkyCopy op{gcube, reinterpret_cast<const float *>(sp.sec[b % world])};
+	sky_block_floats(b, R, op);
+}
+
+cudaError_t launch_sky_grad_peer_sum(const PeerTable &pt, const SkyPeers &sp, int R, const uint8_t *map, float *gcube, cudaStream_t st,
+                                     uint8_t *union_map) {
 	const unsigned nblk = (unsigned)sky_block_count(R);
 	count_launch();
 	sky_stage_kernel<<<nblk, kSkyXThreads, 0, st>>>(sp, R, pt.rank, map, gcube);
@@ -384,7 +396,10 @@ cudaError_t launch_sky_grad_peer_sum(const PeerTable &pt, const SkyPeers &sp, in
 	sky_owner_sum_kernel<<<nblk, kSkyXThreads, 0, st>>>(sp, R, pt.world, pt.rank);
 	if ((e = cudaGetLastError()) != cudaSuccess || (e = launch_peer_barrier(pt, 0u, nullptr, st)) != cudaSuccess) return e;
 	count_launch();
-	sky_gather_kernel<<<nblk, kSkyXThreads, 0, st>>>(sp, R, pt.world, gcube);
+	if (union_map)
+		sky_gather_union_kernel<<<nblk, kSkyXThreads, 0, st>>>(sp, R, pt.world, gcube, union_map);
+	else
+		sky_gather_kernel<<<nblk, kSkyXThreads, 0, st>>>(sp, R, pt.world, gcube);
 	if ((e = cudaGetLastError()) != cudaSuccess) return e;
 	return launch_peer_barrier(pt, 0u, nullptr, st);
 }

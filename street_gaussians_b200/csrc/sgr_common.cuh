@@ -523,7 +523,7 @@ cudaError_t launch_sky_composite_fwd(int H, int W, Band band, int R, int mode, f
                                      cudaStream_t st);
 cudaError_t launch_sky_composite_bwd(int H, int W, Band band, int R, int mode, float fill, const float *acc, const uint8_t *mask, const float *cube,
                                      const float *K, const float *w2c, const float *jx, const float *jy, const float *gout, float *gacc,
-                                     float *gcube, cudaStream_t st, uint8_t *block_map = nullptr);
+                                     float *gcube, cudaStream_t st, uint8_t *block_map = nullptr, bool clear_map = true);
 // tracked actor poses (actor_pose.cu): the device-resident track table and one call's camera
 constexpr int kActorPoseChunk = 256;  // actors per launch: their track slots travel as a kernel parameter
 struct ActorPoseTable {
@@ -600,7 +600,8 @@ __host__ __device__ __forceinline__ int sky_blocks_per_side(int R) { return (R +
 __host__ __device__ __forceinline__ int64_t sky_block_count(int R) { return 6 * (int64_t)sky_blocks_per_side(R) * sky_blocks_per_side(R); }
 __host__ __device__ __forceinline__ size_t sky_cube_section_bytes(int R) { return ((size_t)18 * R * R * sizeof(float) + 255) / 256 * 256; }
 __host__ __device__ __forceinline__ size_t sky_peer_bytes(int R) { return (sky_cube_section_bytes(R) + (size_t)sky_block_count(R) + 255) / 256 * 256; }
-cudaError_t launch_sky_grad_peer_sum(const PeerTable &pt, const SkyPeers &sp, int R, const uint8_t *map, float *gcube, cudaStream_t st);
+cudaError_t launch_sky_grad_peer_sum(const PeerTable &pt, const SkyPeers &sp, int R, const uint8_t *map, float *gcube, cudaStream_t st,
+                                     uint8_t *union_map = nullptr);
 cudaError_t launch_image_loss_stats(int C, int H, int W, Band band, const float *img, const float *gt, const uint8_t *mask, double *acc,
                                     void *scratch, cudaStream_t st);
 cudaError_t launch_image_loss_grad(int C, int H, int W, Band band, const float *img, const float *gt, const uint8_t *mask, const double *acc,
@@ -624,6 +625,7 @@ cudaError_t launch_densify_stats(const SgrStatSegment *segs, int nseg, const int
 cudaError_t launch_adam(const SgrAdamTensor *ts, int n_tensors, double beta1, double beta2, double eps, cudaStream_t st);
 cudaError_t launch_sparse_adam(const SgrSparseAdamSegment *segs, int nseg, const int32_t *radii, double beta1, double beta2, double eps,
                                cudaStream_t st);
+cudaError_t launch_cube_sparse_adam(int R, const SgrAdamTensor &a, uint8_t *map, double beta1, double beta2, double eps, cudaStream_t st);
 size_t densify_scratch_bytes(int nseg, long long P);
 cudaError_t launch_densify_plan(const SgrDensifySegment *segs, int nseg, unsigned long long seed, const float *draws, void *scratch,
                                 long long *result_host, cudaStream_t st);

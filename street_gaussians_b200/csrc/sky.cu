@@ -304,12 +304,13 @@ cudaError_t launch_sky_composite_fwd(int H, int W, Band band, int R, int mode, f
 	return cudaGetLastError();
 }
 
-// With a block map (sgr_band_sky_composite_backward_marked): the map is cleared first, also for an empty band, then marked.
+// With a block map (sgr_band_sky_composite_backward_marked): the map is cleared first, also for an empty band, then marked.  Without
+// clear_map (sgr_band_sky_composite_backward_or_marks) the marks are added to what the map holds.
 cudaError_t launch_sky_composite_bwd(int H, int W, Band band, int R, int mode, float fill, const float *acc, const uint8_t *mask, const float *cube,
                                      const float *K, const float *w2c, const float *jx, const float *jy, const float *gout, float *gacc,
-                                     float *gcube, cudaStream_t st, uint8_t *block_map) {
+                                     float *gcube, cudaStream_t st, uint8_t *block_map, bool clear_map) {
 	const int64_t N = (int64_t)H * W, M = (int64_t)band_rows(band) * kBandTileRows * W;
-	if (block_map) {
+	if (block_map && clear_map) {
 		cudaError_t e = cudaMemsetAsync(block_map, 0, (size_t)sky_block_count(R), st);
 		if (e != cudaSuccess) return e;
 	}

@@ -19,6 +19,12 @@ entries at world 1) and its transport.  With exchange="nccl" the all-reduce abov
 marks the 32 x 32-texel blocks of the cube its band touched (sgr_band_sky_composite_backward_marked) and sums only those over peer
 memory (sgr_sky_grad_peer_sum, through the rasterizer's sky_workspace): no NCCL call, no host read-back, and every rank's
 cube_map.grad holds the same bytes, the ascending-rank fp32 sum of the ranks' partials block by block.
+
+blocks= (keyword-only, with block_map(R, device)): the 32 x 32-texel blocks of the cube this call's backward adds gradient into are
+OR-ed into `blocks` (set to 1; other bytes kept), for training.CubeMapSparseAdam, which steps only those blocks and clears the map.  In
+every mode `blocks` ends up with the union over the ranks, the same bytes on every rank: the whole frame marks through
+sgr_band_sky_composite_backward_or_marks over every tile row; band= / group= sums the band's marks over the group after the gradient's
+all-reduce; rasterizer= with exchange="p2p" takes the union the peer-memory sum already forms (sgr_sky_grad_peer_sum_union).
 """
 from __future__ import annotations
 
@@ -80,21 +86,46 @@ def _resolve(band, group, rasterizer, H: int):
     return _band_rows(own, H), xfer
 
 
-def sky_grad_peer_sum(ws, sky_ws, g_cube: torch.Tensor) -> torch.Tensor:
+def block_map(R: int, device=None) -> torch.Tensor:
+    """A zeroed block map of a [6, R, R, 3] cube: sgr_sky_grad_blocks(R) = 6 ceil(R / 32)^2 uint8 bytes, one per 32 x 32-texel block,
+    for sky_composite(blocks=) and training.CubeMapSparseAdam.step."""
+    n = int(_capi.lib().sgr_sky_grad_blocks(int(R)))
+    if n <= 0:
+        raise ValueError(f"no cube block map for R={R} (0 < R <= 16384)")
+    return torch.zeros(n, dtype=torch.uint8, device=device)
+
+
+def _check_blocks(blocks, R: int, device):
+    n = int(_capi.lib().sgr_sky_grad_blocks(R))
+    if blocks.dtype != torch.uint8 or blocks.dim() != 1 or blocks.numel() != n or not blocks.is_contiguous():
+        raise ValueError(f"blocks must be a contiguous uint8 tensor of sgr_sky_grad_blocks({R}) = {n} bytes, got {blocks.dtype} "
+                         f"{tuple(blocks.shape)}")
+    if blocks.device != device:
+        raise ValueError(f"blocks is on {blocks.device}, rgb on {device}")
+
+
+def sky_grad_peer_sum(ws, sky_ws, g_cube: torch.Tensor, union: Optional[torch.Tensor] = None) -> torch.Tensor:
     """COLLECTIVE over the ranks of the peer workspace `ws` (sgr_sky_grad_peer_sum, on the device): in place on this rank's partial
     g_cube [6, R, R, 3], zero outside the blocks sky_ws.block_map marks (sgr_band_sky_composite_backward_marked on a zeroed g_cube),
-    every rank ends with the marked blocks' ascending-rank sum and zeros elsewhere.  Three barriers on ws's pad."""
+    every rank ends with the marked blocks' ascending-rank sum and zeros elsewhere.  Three barriers on ws's pad.  union: a block map
+    (block_map) into which every block some rank marked is OR-ed, the same bytes on every rank (sgr_sky_grad_peer_sum_union)."""
     ws.next_epochs(3)
-    _capi.call("sgr_sky_grad_peer_sum", g_cube.device, C.byref(ws.peers), C.byref(sky_ws.peers), int(g_cube.shape[1]), ptr(sky_ws.block_map),
-               ptr(g_cube))
+    if union is None:
+        _capi.call("sgr_sky_grad_peer_sum", g_cube.device, C.byref(ws.peers), C.byref(sky_ws.peers), int(g_cube.shape[1]),
+                   ptr(sky_ws.block_map), ptr(g_cube))
+    else:
+        _capi.call("sgr_sky_grad_peer_sum_union", g_cube.device, C.byref(ws.peers), C.byref(sky_ws.peers), int(g_cube.shape[1]),
+                   ptr(sky_ws.block_map), ptr(g_cube), ptr(union))
     return g_cube
 
 
 class _SkyComposite(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, rgb, acc, cube_map, K, w2c, sky_mask, perturb: bool, fill: float, rows, xfer, rasterizer):
+    def forward(ctx, rgb, acc, cube_map, K, w2c, sky_mask, perturb: bool, fill: float, rows, xfer, rasterizer, blocks):
         H, W, R = _check(rgb, acc, cube_map, K, w2c, sky_mask)
         dev = rgb.device
+        if blocks is not None:
+            _check_blocks(blocks, R, dev)
         rgb_c, acc_c, cube = rgb.contiguous(), acc.contiguous(), cube_map.contiguous()
         Kc, Tc = K.contiguous(), w2c.contiguous()
         mask = sky_mask.contiguous() if sky_mask is not None else None
@@ -114,7 +145,7 @@ class _SkyComposite(torch.autograd.Function):
                        ptr(Kc), ptr(Tc), ptr(jx), ptr(jy), ptr(out))
         ctx.save_for_backward(acc_c, cube, Kc, Tc, mask, jx, jy)
         ctx.args = (H, W, R, mode, float(fill))
-        ctx.band, ctx.xfer = rows, xfer
+        ctx.band, ctx.xfer, ctx.blocks = rows, xfer, blocks
         # exchange="p2p": the sky section is collective on first use, so it is allocated here, where every rank runs
         ctx.sky_ws = rasterizer.sky_workspace(R, dev) if rows is not None and xfer.kind == "p2p" else None
         return out
@@ -127,7 +158,12 @@ class _SkyComposite(torch.autograd.Function):
         g = g_out.contiguous()
         need_rgb, need_acc, need_cube = ctx.needs_input_grad[:3]
         g_cube = torch.zeros_like(cube) if need_cube else None
-        if ctx.band is None:
+        blocks = ctx.blocks if need_cube else None
+        if ctx.band is None and blocks is not None:  # the band of every tile row: the whole-frame gradient, with the blocks marked
+            g_acc = torch.empty_like(acc) if need_acc else None
+            _capi.call("sgr_band_sky_composite_backward_or_marks", dev, H, W, 0, (H + 15) // 16, 1, R, mode, fill, ptr(acc), ptr(mask),
+                       ptr(cube), ptr(Kc), ptr(Tc), ptr(jx), ptr(jy), ptr(g), ptr(g_acc), ptr(g_cube), ptr(blocks))
+        elif ctx.band is None:
             g_acc = torch.empty_like(acc) if need_acc else None
             _capi.call("sgr_sky_composite_backward", dev, H, W, R, mode, fill, ptr(acc), ptr(mask), ptr(cube), ptr(Kc), ptr(Tc), ptr(jx),
                        ptr(jy), ptr(g), ptr(g_acc), ptr(g_cube))
@@ -135,19 +171,31 @@ class _SkyComposite(torch.autograd.Function):
             g_acc = torch.zeros_like(acc) if need_acc else None
             _capi.call("sgr_band_sky_composite_backward_marked", dev, H, W, *ctx.band, R, mode, fill, ptr(acc), ptr(mask), ptr(cube), ptr(Kc),
                        ptr(Tc), ptr(jx), ptr(jy), ptr(g), ptr(g_acc), ptr(g_cube), ptr(ctx.sky_ws.block_map))
-            sky_grad_peer_sum(ctx.xfer.ws, ctx.sky_ws, g_cube)
+            if blocks is None:
+                sky_grad_peer_sum(ctx.xfer.ws, ctx.sky_ws, g_cube)
+            else:
+                sky_grad_peer_sum(ctx.xfer.ws, ctx.sky_ws, g_cube, blocks)
+        elif blocks is not None:  # COLLECTIVE: as below, then the ranks' marks summed the same way; non-zero counts are the union
+            g_acc = torch.zeros_like(acc) if need_acc else None
+            local = torch.empty_like(blocks)
+            _capi.call("sgr_band_sky_composite_backward_marked", dev, H, W, *ctx.band, R, mode, fill, ptr(acc), ptr(mask), ptr(cube), ptr(Kc),
+                       ptr(Tc), ptr(jx), ptr(jy), ptr(g), ptr(g_acc), ptr(g_cube), ptr(local))
+            ctx.xfer.sum(g_cube)
+            counts = local.to(torch.int32)
+            ctx.xfer.sum(counts)
+            blocks.logical_or_(counts)
         else:
             g_acc = torch.zeros_like(acc) if need_acc else None
             _capi.call("sgr_band_sky_composite_backward", dev, H, W, *ctx.band, R, mode, fill, ptr(acc), ptr(mask), ptr(cube), ptr(Kc), ptr(Tc),
                        ptr(jx), ptr(jy), ptr(g), ptr(g_acc), ptr(g_cube))
             if need_cube:  # COLLECTIVE: this band's partial dL/dcube -> the whole frame's, on every rank
                 ctx.xfer.sum(g_cube)
-        return (g_out if need_rgb else None), g_acc, g_cube, None, None, None, None, None, None, None, None
+        return (g_out if need_rgb else None), g_acc, g_cube, None, None, None, None, None, None, None, None, None
 
 
 def sky_composite(rgb: torch.Tensor, acc: torch.Tensor, cube_map: torch.Tensor, K: torch.Tensor, w2c: torch.Tensor, *,
                   sky_mask: Optional[torch.Tensor] = None, perturb: bool = False, white_background: bool = True, band=None,
-                  group=None, rasterizer=None) -> torch.Tensor:
+                  group=None, rasterizer=None, blocks: Optional[torch.Tensor] = None) -> torch.Tensor:
     """rgb [3, H, W] + sky * (1 - acc [1, H, W]) with the sky sampled from cube_map [6, R, R, 3] along the rays of K [3, 3] and
     w2c [4, 4], clamped to [0, 1]; pixels the mask rule leaves out take 1 (white_background) or 0.  Differentiable in rgb, acc and
     cube_map.  sky_mask: bool [1, H, W] or [H, W] (training with the guidance mask), None for the acc rule.  All fp32 CUDA tensors.
@@ -162,6 +210,12 @@ def sky_composite(rgb: torch.Tensor, acc: torch.Tensor, cube_map: torch.Tensor, 
     1; a band= or group= that differs from its own raises ValueError.  exchange="nccl": the all-reduce above over its group.
     exchange="p2p": COLLECTIVE in the backward over its peer memory, no NCCL call and no host synchronisation; cube_map.grad is the
     ascending-rank fp32 sum of the ranks' partials, block by block, and the same bytes on every rank.  Every rank must ask for the cube
-    map's gradient alike."""
+    map's gradient alike.
+
+    blocks= (block_map(R, device)): when the backward forms the cube map's gradient, it also OR-s into `blocks` the 32 x 32-texel blocks
+    that gradient touched (set to 1, other bytes kept), over every rank in the multi-GPU modes, so that marks accumulate over backward
+    passes until training.CubeMapSparseAdam.step consumes them; with several ranks, every rank must pass a map holding the same bytes.
+    The gradients are those of the call without blocks= (dL/dcube up to the order of its texels' float atomics)."""
     rows, xfer = _resolve(band, group, rasterizer, int(rgb.shape[-2]))  # a bad or mismatched band fails before anything else
-    return _SkyComposite.apply(rgb, acc, cube_map, K, w2c, sky_mask, bool(perturb), 1.0 if white_background else 0.0, rows, xfer, rasterizer)
+    return _SkyComposite.apply(rgb, acc, cube_map, K, w2c, sky_mask, bool(perturb), 1.0 if white_background else 0.0, rows, xfer, rasterizer,
+                               blocks)

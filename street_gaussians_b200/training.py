@@ -17,6 +17,9 @@
     SparseAdam(param_groups, ...).step(models, radii)
         opt-in visibility-masked Adam (no reference counterpart; it deviates from the reference): FusedAdam's update on the rows
         with radii > 0 only, every other row's parameter and moments left untouched.
+    CubeMapSparseAdam([cube_map], ...).step(blocks)
+        opt-in block-masked Adam for the sky cube map (no reference counterpart; it deviates from the reference): FusedAdam's update
+        on the 32 x 32-texel blocks sky.sky_composite(blocks=) marked, every other texel left untouched, and the map cleared.
 CUDA tensors only; there is no CPU fallback.
 """
 from __future__ import annotations
@@ -469,4 +472,79 @@ class SparseAdam(torch.optim.Optimizer):
                     s.param[:], s.grad[:], s.exp_avg[:], s.exp_avg_sq[:], s.width[:], s.lr[:], s.step[:] = f
             _capi.call("sgr_sparse_adam_step", dev, segs, len(models), ptr(r), float(betas[0]), float(betas[1]), eps)
             del keep
+        return loss
+
+
+# ---- block-masked Adam of the sky cube map ----
+class CubeMapSparseAdam(torch.optim.Optimizer):
+    """Block-masked Adam for the sky cube map: an OPT-IN alternative to FusedAdam (the reference's torch.optim.Adam(eps=1e-15) of
+    SkyCubeMap) that steps only the 32 x 32-texel blocks the frame's backward touched.  It changes training results against the
+    reference, whose Adam keeps moving every texel on its decaying momentum, so FusedAdam stays the drop-in.
+
+    It holds exactly one parameter, the contiguous fp32 CUDA cube map [6, R, R, 3].  step(blocks) — blocks: the uint8 map of
+    sky.block_map(R, device) that sky.sky_composite(..., blocks=blocks) filled:
+      * with a .grad, state["step"] goes up by one (as in FusedAdam: there are no per-block step counts), the moments are created at
+        zero on first use, and ONE sgr_cube_sparse_adam_step call gives the marked blocks FusedAdam's update bit for bit, leaves every
+        other texel's parameter and moments untouched (their gradient is not read), and clears `blocks` for the next frame;
+      * without a .grad, nothing changes, the map included.
+    The state is {step, exp_avg, exp_avg_sq}, so a state dict moves between FusedAdam and CubeMapSparseAdam in either direction, and
+    param_groups[0]["lr"] can be scheduled.  No host synchronisation and, after the first step, no allocation; the grid depends on R
+    only, so the step can be captured in a CUDA graph.  step() without a map raises TypeError: there is no dense fallback."""
+
+    def __init__(self, params, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8):
+        super().__init__(params, dict(lr=lr, betas=betas, eps=eps))
+        ps = [p for g in self.param_groups for p in g["params"]]
+        if len(ps) != 1:
+            raise ValueError(f"CubeMapSparseAdam holds exactly one parameter (the cube map), got {len(ps)}")
+        p = ps[0]
+        if p.dim() != 4 or p.shape[0] != 6 or p.shape[1] != p.shape[2] or p.shape[3] != 3:
+            raise ValueError(f"the cube map must be [6, R, R, 3], got {tuple(p.shape)}")
+        if p.dtype != torch.float32 or not p.is_contiguous():
+            raise ValueError(f"the cube map must be a contiguous fp32 tensor, got {p.dtype}")
+        self._R = int(p.shape[1])
+        self._nblocks = int(_capi.lib().sgr_sky_grad_blocks(self._R))
+        if self._nblocks <= 0:
+            raise ValueError(f"the cube map's R={self._R} is outside 0 < R <= 16384")
+        self._rec = _capi.SgrAdamTensor()  # the entry's record, refilled in place every step
+        self._rec.numel = p.numel()
+
+    @torch.no_grad()
+    def step(self, blocks: torch.Tensor = None, closure=None):
+        if blocks is None:
+            raise TypeError("CubeMapSparseAdam.step(blocks) needs the block map sky_composite(blocks=) filled; it has no dense fallback "
+                            "(use FusedAdam for a dense update)")
+        if blocks.dtype != torch.uint8 or blocks.numel() != self._nblocks or not blocks.is_contiguous():
+            raise ValueError(f"blocks must be a contiguous uint8 map of sgr_sky_grad_blocks({self._R}) = {self._nblocks} bytes, got "
+                             f"{blocks.dtype} {tuple(blocks.shape)}")
+        loss = closure() if closure is not None else None
+        group = self.param_groups[0]
+        p = group["params"][0]
+        if p.grad is None:
+            return loss
+        lr, (b1, b2), eps = float(group["lr"]), (float(b) for b in group["betas"]), float(group["eps"])
+        if not math.isfinite(lr):
+            raise ValueError(f"non-finite lr {lr}")
+        if not (0.0 <= b1 < 1.0 and 0.0 <= b2 < 1.0):
+            raise ValueError(f"betas ({b1}, {b2}) outside [0, 1)")
+        dev = p.device
+        if not p.is_cuda or blocks.device != dev:
+            raise _capi.SgrError(f"CubeMapSparseAdam needs the cube map and blocks on one CUDA device (cube on {p.device}, blocks on "
+                                 f"{blocks.device}; there is no CPU fallback)")
+        if tuple(p.shape) != (6, self._R, self._R, 3) or p.dtype != torch.float32 or not p.is_contiguous():
+            raise ValueError(f"the cube map changed to {p.dtype} {tuple(p.shape)}")
+        st = self.state[p]
+        if st:
+            m, v = st["exp_avg"], st["exp_avg_sq"]
+            for t in (m, v):
+                if t.shape != p.shape or t.dtype != torch.float32 or t.device != dev or not t.is_contiguous():
+                    raise ValueError(f"the cube map's Adam state is {t.dtype} {tuple(t.shape)} on {t.device}, the parameter "
+                                     f"{p.dtype} {tuple(p.shape)} on {dev}")
+        g = p.grad if (p.grad.dtype == torch.float32 and p.grad.is_contiguous()) else _capi.f32(p.grad)
+        if g.shape != p.shape or g.device != dev:
+            raise ValueError(f"the cube map's gradient is {tuple(g.shape)} on {g.device}, the parameter {tuple(p.shape)} on {dev}")
+        st = _advance_state(st, p)
+        r = self._rec
+        r.param, r.grad, r.exp_avg, r.exp_avg_sq = p.data_ptr(), g.data_ptr(), st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr()
+        r.lr, r.step = lr, st["step"]
+        _capi.call("sgr_cube_sparse_adam_step", dev, self._R, C.byref(r), blocks.data_ptr(), b1, b2, eps)
         return loss
