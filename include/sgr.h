@@ -805,6 +805,15 @@ int sgr_band_sky_composite_backward_or_marks(int32_t H, int32_t W, int32_t row_b
                                              float *dL_dcube, uint8_t *block_map, void *stream);
 int sgr_sky_grad_peer_sum_union(const SgrPeers *peers, const SgrSkyPeers *sky_peers, int32_t R, const uint8_t *block_map, float *dL_dcube,
                                 uint8_t *union_map, void *stream);
+/* The cube map as a lat-long image: cubemap_to_latlong (lib/models/sky_cubemap.py:178-191), which SkyCubeMap.save_state_dict
+ * (:36-46) writes as sky_latlong.png, without nvdiffrast.  Pixel (row i, column j) of the H x W image samples cube_map [6, R, R, 3] with
+ * the composite's lookup (the same taps, weights, edge wrap and corner rule as sgr_sky_composite_forward) along
+ *   (sin t sin p, cos t, -sin t cos p),  t = pi gy_i,  p = pi gx_j,  gy = linspace(1/H, 1 - 1/H, H),  gx = linspace(-1 + 1/W, 1 - 1/W, W),
+ * every step in fp32 as torch forms the reference's tensors.  latlong [H, W, 3] fp32 (may be NULL) takes the samples unclamped, as the
+ * reference returns them; latlong_u8 [H, W, 3] uint8 (may be NULL) takes (uint8)(clamp(v, 0, 1) * 255), the fp32 product truncated, as
+ * the reference's astype(np.uint8) (a NaN sample gives 0).  At least one output; no gradient.  One launch, one thread per pixel;
+ * 0 < R <= 16384, H, W > 0, H W <= (2^31 - 1) 256.  Device pointers; cube_map is read with 4-byte loads. */
+int sgr_sky_cube_to_latlong(int32_t R, const float *cube_map, int32_t H, int32_t W, float *latlong, uint8_t *latlong_u8, void *stream);
 /* The feature maps' finishing (sgr_finish_features_forward / _backward) on a tile-row band: the whole-frame calls' arguments plus the
  * band.  rendered, normals, semantic, dL_dnormals, dL_dsemantic and dL_drendered are whole [C, H, W] frames; only the band's pixels are
  * read and written (the caller zeroes the other rows where it needs zeros), each at its frame index, so the band's rows equal the

@@ -1716,6 +1716,18 @@ int sgr_band_sky_composite_backward(int32_t H, int32_t W, int32_t row_begin, int
 int64_t sgr_sky_grad_blocks(int32_t R) { return (R > 0 && R <= 16384) ? sky_block_count(R) : 0; }
 size_t sgr_sky_peer_bytes(int32_t R) { return (R > 0 && R <= 16384) ? sky_peer_bytes(R) : 0; }
 
+int sgr_sky_cube_to_latlong(int32_t R, const float *cube_map, int32_t H, int32_t W, float *latlong, uint8_t *latlong_u8, void *stream) {
+	const char *fn = "sgr_sky_cube_to_latlong";
+	// one thread per pixel in an int grid of 256-thread blocks (sky.cu's kSkyThreads): H W <= (2^31 - 1) 256
+	if (R <= 0 || R > 16384 || H <= 0 || W <= 0 || (int64_t)H * W > (int64_t)0x7fffffff * 256)
+		return fail(SGR_EINVAL, "%s: bad sizes R=%d H=%d W=%d", fn, R, H, W);
+	if (!cube_map || (!latlong && !latlong_u8)) return fail(SGR_EINVAL, "%s: cube_map and at least one output are required", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_sky_cube_to_latlong(R, cube_map, H, W, latlong, latlong_u8, st), fn);
+	return SGR_OK;
+}
+
 static int sky_backward_marking(const char *fn, bool clear_map, int32_t H, int32_t W, int32_t row_begin, int32_t row_end, int32_t row_step,
                                 int32_t R, int32_t mode, float fill, const float *acc, const uint8_t *sky_mask, const float *cube_map,
                                 const float *K, const float *w2c, const float *jitter_x, const float *jitter_y, const float *dL_dout,

@@ -524,6 +524,7 @@ cudaError_t launch_sky_composite_fwd(int H, int W, Band band, int R, int mode, f
 cudaError_t launch_sky_composite_bwd(int H, int W, Band band, int R, int mode, float fill, const float *acc, const uint8_t *mask, const float *cube,
                                      const float *K, const float *w2c, const float *jx, const float *jy, const float *gout, float *gacc,
                                      float *gcube, cudaStream_t st, uint8_t *block_map = nullptr, bool clear_map = true);
+cudaError_t launch_sky_cube_to_latlong(int R, const float *cube, int H, int W, float *out, uint8_t *u8, cudaStream_t st);
 // tracked actor poses (actor_pose.cu): the device-resident track table and one call's camera
 constexpr int kActorPoseChunk = 256;  // actors per launch: their track slots travel as a kernel parameter
 struct ActorPoseTable {

@@ -325,4 +325,56 @@ cudaError_t launch_sky_composite_bwd(int H, int W, Band band, int R, int mode, f
 	return cudaGetLastError();
 }
 
+// The lat-long image of the cube (cubemap_to_latlong, sky_cubemap.py:178-191, which SkyCubeMap.save_state_dict writes as a PNG).
+// torch.linspace(start, end, n) in fp32, as its CUDA kernel forms it: start + step k below the halfway index n / 2, end - step (n - 1 - k)
+// from it (both contracted to one fma), step = (end - start) / (n - 1); n == 1 gives start.
+struct SkyLinspace {
+	float start, end, step;
+	int n;
+};
+
+__device__ __forceinline__ float sky_linspace(const SkyLinspace &l, const int k) {
+	if (l.n == 1) return l.start;
+	return k < l.n / 2 ? __fmaf_rn(l.step, (float)k, l.start) : __fmaf_rn(-l.step, (float)(l.n - 1 - k), l.end);
+}
+
+// One thread per pixel (row i, column j): theta = gy_i pi and phi = gx_j pi rounded to fp32 as torch's gy * np.pi, the direction
+// (sin theta sin phi, cos theta, -sin theta cos phi) and the composite's lookup (sky_taps + sky_sample).  u8 (may be NULL): the
+// reference's (clamp(v, 0, 1) * 255).astype(uint8), the fp32 product truncated.
+__global__ void __launch_bounds__(kSkyThreads) sky_latlong_kernel(const int64_t N, const int W, const int R, const SkyLinspace ly,
+                                                                  const SkyLinspace lx, const float *__restrict__ cube, float *__restrict__ out,
+                                                                  uint8_t *__restrict__ u8) {
+	const int64_t pix = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (pix >= N) return;
+	const int i = (int)(pix / W), j = (int)(pix - (int64_t)i * W);
+	const float pi = 3.14159265358979323846f;
+	const float theta = __fmul_rn(sky_linspace(ly, i), pi), phi = __fmul_rn(sky_linspace(lx, j), pi);
+	const float st = sinf(theta), ct = cosf(theta), sp = sinf(phi), cp = cosf(phi);
+	const float d[3] = {__fmul_rn(st, sp), ct, -__fmul_rn(st, cp)};
+	float s[3];
+	sky_sample(sky_taps(d, R), cube, s);
+#pragma unroll
+	for (int ch = 0; ch < 3; ch++) {
+		if (out) out[pix * 3 + ch] = s[ch];
+		if (u8) u8[pix * 3 + ch] = (uint8_t)(int)__fmul_rn(fminf(fmaxf(s[ch], 0.f), 1.f), 255.f);
+	}
+}
+
+static SkyLinspace sky_linspace_of(double start, double end, int n) {
+	SkyLinspace l;
+	l.start = (float)start;
+	l.end = (float)end;
+	l.step = n > 1 ? (l.end - l.start) / (float)(n - 1) : 0.f;
+	l.n = n;
+	return l;
+}
+
+cudaError_t launch_sky_cube_to_latlong(int R, const float *cube, int H, int W, float *out, uint8_t *u8, cudaStream_t st) {
+	const int64_t N = (int64_t)H * W;
+	count_launch();
+	sky_latlong_kernel<<<sky_blocks(N), kSkyThreads, 0, st>>>(N, W, R, sky_linspace_of(0.0 + 1.0 / H, 1.0 - 1.0 / H, H),
+	                                                          sky_linspace_of(-1.0 + 1.0 / W, 1.0 - 1.0 / W, W), cube, out, u8);
+	return cudaGetLastError();
+}
+
 }  // namespace sgr

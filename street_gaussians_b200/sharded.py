@@ -23,7 +23,9 @@ fwd/bwd were about a third of the step) and the 2x91 MB all-reduce becomes a 91 
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
+import math
 from typing import List, NamedTuple, Optional, Sequence
 
 import torch
@@ -32,7 +34,7 @@ import torch.nn as nn
 
 from . import _capi
 from ._capi import ptr
-from .training import PARAM_NAMES, _attr, _install, _param_slots, _segment, _stat_segment
+from .training import ADAM_GROUP_NAMES, PARAM_NAMES, STAT_NAMES, _attr, _has, _install, _param_slots, _segment, _set, _stat_segment
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, InstanceCapacity, TileRowBand, _check_layers, _copy_status,
                          _ForwardState, _backward_blend_impl, _backward_geom_impl, _fit_grads, _fp32_inputs, _geom_grad_buffers, _image_grads,
                          _input_shapes, _make_frame, _reference_inputs)
@@ -983,6 +985,39 @@ def _rebalance_tables(L, ranges, buffers, dev):
     return (rt, len(ranges), bp, bf, nb, ptr(scratch), scratch.numel()), scratch
 
 
+def _row_table(models, optimizer, slots, dev, tr, what: str):
+    """COLLECTIVE (one all_gather): this rank's sgr_rebalance_* segments of `models` (moment bits where Adam state exists) and the
+    [world][n_models][11] table of every rank's counts, row widths and Adam steps (-1: no state), checked alike on every rank: the
+    widths and steps must agree (ValueError otherwise, on every rank).  Returns (segments, [(params, moments)] per model, table)."""
+    nm = len(models)
+    segs = (_capi.SgrDensifySegment * nm)()
+    infos = []
+    meta = torch.full((nm, 4 + _capi.DENSIFY_TENSORS), -1, dtype=torch.int64)
+    for k, m in enumerate(models):
+        seg, params, moments, widths = _segment(m, k, optimizer, slots, dev)
+        _stat_segment(seg, m, k, dev)
+        meta[k, :4] = torch.tensor([seg.count, seg.dc_width, seg.rest_width, seg.semantic_width])
+        for a, p in enumerate(params):
+            if moments[a] is not None:
+                opt = slots[id(p)][0]
+                meta[k, 4 + a] = int(opt.state[p]["step"])
+                if widths[a]:
+                    seg.moments |= 1 << a
+        segs[k] = seg
+        infos.append((params, moments))
+    table = torch.stack(tr.all_gather(meta)).tolist()  # [world][nm][11]
+    for k in range(nm):
+        for r in range(len(table)):
+            if table[r][k][1:4] != table[0][k][1:4]:
+                raise ValueError(f"model {k}: rows of {table[0][k][1:4]} (dc, rest, semantic floats) on rank 0, {table[r][k][1:4]} on rank {r}")
+            for a in range(_capi.DENSIFY_TENSORS):
+                if table[r][k][4 + a] != table[0][k][4 + a]:
+                    st = lambda v: "no Adam state" if v < 0 else f"Adam step {v}"
+                    raise ValueError(f"model {k}: {PARAM_NAMES[a]} has {st(table[0][k][4 + a])} on rank 0 and {st(table[r][k][4 + a])} on rank {r}; "
+                                     f"{what} needs the same optimizer state on every rank")
+    return segs, infos, table
+
+
 def rebalance(models: Sequence, optimizer=None, group: Optional[dist.ProcessGroup] = None, rasterizer: Optional["GaussianShardedRasterizer"] = None,
               transport=None) -> int:
     """COLLECTIVE: even out the ranks' Gaussian counts after densify_and_prune, moving rows between ranks together with their Adam
@@ -1011,31 +1046,7 @@ def rebalance(models: Sequence, optimizer=None, group: Optional[dist.ProcessGrou
     L = _capi.lib()
     dev = _attr(models[0], "_xyz").device
     slots = _param_slots(optimizer)
-    segs = (_capi.SgrDensifySegment * nm)()
-    infos = []
-    meta = torch.full((nm, 4 + _capi.DENSIFY_TENSORS), -1, dtype=torch.int64)
-    for k, m in enumerate(models):
-        seg, params, moments, widths = _segment(m, k, optimizer, slots, dev)
-        _stat_segment(seg, m, k, dev)
-        meta[k, :4] = torch.tensor([seg.count, seg.dc_width, seg.rest_width, seg.semantic_width])
-        for a, p in enumerate(params):
-            if moments[a] is not None:
-                opt = slots[id(p)][0]
-                meta[k, 4 + a] = int(opt.state[p]["step"])
-                if widths[a]:
-                    seg.moments |= 1 << a
-        segs[k] = seg
-        infos.append((params, moments))
-    table = torch.stack(tr.all_gather(meta)).tolist()  # [world][nm][11]
-    for k in range(nm):
-        for r in range(world):
-            if table[r][k][1:4] != table[0][k][1:4]:
-                raise ValueError(f"model {k}: rows of {table[0][k][1:4]} (dc, rest, semantic floats) on rank 0, {table[r][k][1:4]} on rank {r}")
-            for a in range(_capi.DENSIFY_TENSORS):
-                if table[r][k][4 + a] != table[0][k][4 + a]:
-                    st = lambda v: "no Adam state" if v < 0 else f"Adam step {v}"
-                    raise ValueError(f"model {k}: {PARAM_NAMES[a]} has {st(table[0][k][4 + a])} on rank 0 and {st(table[r][k][4 + a])} on rank {r}; "
-                                     "rebalance needs the same optimizer state on every rank")
+    segs, infos, table = _row_table(models, optimizer, slots, dev, tr, "rebalance")
     plan = rebalance_plan([[row[0] for row in table[r]] for r in range(world)])
     P_new = sum(plan.counts[rank])
     if rasterizer is not None:
@@ -1086,3 +1097,288 @@ def rebalance(models: Sequence, optimizer=None, group: Optional[dist.ProcessGrou
     for k, m in enumerate(models):
         _install(m, infos[k][0], *new[k], slots)
     return P_new
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Checkpoints under Gaussian sharding (DESIGN.md §8): the files io.save_checkpoint / io.save_ply write on one GPU, and resuming from them
+# at any world size
+# ---------------------------------------------------------------------------------------------------------------------
+def even_slices(totals: Sequence[int], world: int) -> List[List[tuple]]:
+    """Rank r's rows [lo, hi) of every sub-model (totals[m] rows each, composition order) under the even split of the model-major global
+    array that rebalance() leaves: rank r owns the global rows [B_r, B_{r+1}), the first P % world ranks one row more."""
+    totals = [int(n) for n in totals]
+    if world < 1 or any(n < 0 for n in totals):
+        raise ValueError(f"even_slices needs world >= 1 and non-negative counts, got world={world}, {totals}")
+    base, extra = divmod(sum(totals), world)
+    B = [r * base + min(r, extra) for r in range(world + 1)]
+    out = []
+    for r in range(world):
+        row, g0 = [], 0
+        for n in totals:
+            lo = min(max(B[r], g0), g0 + n)
+            row.append((lo - g0, max(lo, min(B[r + 1], g0 + n)) - g0))
+            g0 += n
+        out.append(row)
+    return out
+
+
+def gather_pieces(counts: Sequence[Sequence[int]], row_bytes: Sequence[int], piece_bytes: int) -> List[tuple]:
+    """The pieces gather_state sends: (source rank, [(model, first local row, rows), ...]) in rank-major, then model, then row order, every
+    local row of every rank exactly once, each piece at most piece_bytes (row_bytes[m] bytes per row of model m; a model no rank holds rows
+    of may have any width)."""
+    need = max((int(row_bytes[k]) for row in counts for k, n in enumerate(row) if n), default=0)
+    if piece_bytes < max(need, 1):
+        raise ValueError(f"piece_bytes={piece_bytes} is smaller than one row ({need} bytes)")
+    pieces = []
+    for s, row in enumerate(counts):
+        cur, used = [], 0
+        for k, n in enumerate(row):
+            at = 0
+            while at < n:
+                take = min((piece_bytes - used) // int(row_bytes[k]), n - at)
+                if take == 0:
+                    pieces.append((s, cur))
+                    cur, used = [], 0
+                    continue
+                cur.append((k, at, take))
+                used += take * int(row_bytes[k])
+                at += take
+        if cur:
+            pieces.append((s, cur))
+    return pieces
+
+
+def _unpack_rows(flat: torch.Tensor, ranges, seg_info, host, at_rank):
+    """Scatter a received piece (host fp32, the sgr_rebalance_pack block format) into the host arrays of every model at its global rows."""
+    off = 0
+    for k, first, rows in ranges:
+        widths, moment_bits = seg_info[k]
+        dst = host[k]
+        g = at_rank[k] + first
+        order = [dst[PARAM_NAMES[a]] for a in range(len(PARAM_NAMES)) if widths[a]]
+        order += [dst["adam"][PARAM_NAMES[a]]["exp_avg"] for a in moment_bits]
+        order += [dst["adam"][PARAM_NAMES[a]]["exp_avg_sq"] for a in moment_bits]
+        order += [dst[s] for s in STAT_NAMES]
+        for t in order:
+            w = int(math.prod(t.shape[1:]))
+            t.view(t.shape[0], w)[g:g + rows] = flat[off:off + rows * w].view(rows, w)
+            off += rows * w
+
+
+def gather_state(models: Sequence, optimizer=None, *, dst: int = 0, group=None, transport=None, piece_bytes: int = 1 << 30):
+    """COLLECTIVE: every rank's rows of every sub-model, with their Adam moments and densification statistics, assembled on rank `dst` as
+    the global tensors a single-GPU run of the same rows holds (rank-major order, as GaussianShardedRasterizer composes them).
+
+    models: this rank's sub-models in composition order (the seven parameters and max_radii2D, xyz_gradient_accum, denom), the same list
+      on every rank; a sub-model may have 0 local rows.  optimizer: one optimizer or a list; a parameter's moments are gathered where it has
+      Adam state, and its step must be equal on every rank.  As in rebalance(), one all_gather of the per-model table comes first and a
+      width or step mismatch raises ValueError on every rank before any row moves.
+    Then the rows travel in pieces (gather_pieces) of at most piece_bytes: the owner packs one piece with sgr_rebalance_pack into a buffer
+      it reuses, sends it to dst (transport.exchange), and dst copies it to the host and scatters it into the global host tensors.  Extra
+      device memory is one piece buffer per rank (dst's own rows take the same path without the send); no live tensor is replaced.
+    Returns on dst one dict per model: the seven parameters and three statistics by attribute name (CPU fp32), and "adam": {parameter name:
+      {"step": int, "exp_avg", "exp_avg_sq"}} for the parameters with Adam state.  Other ranks return None."""
+    tr = transport if transport is not None else ProcessGroupTransport(group)
+    world, rank = int(tr.world), int(tr.rank)
+    models = list(models)
+    nm = len(models)
+    if nm == 0:
+        raise ValueError("gather_state needs the sub-models (background, then actors)")
+    if not 0 <= int(dst) < world:
+        raise ValueError(f"dst={dst} is not a rank of a group of {world}")
+    if int(piece_bytes) <= 0:
+        raise ValueError(f"piece_bytes must be positive, got {piece_bytes}")
+    L = _capi.lib()
+    dev = _attr(models[0], "_xyz").device
+    slots = _param_slots(optimizer)
+    segs, infos, table = _row_table(models, optimizer, slots, dev, tr, "gather_state")
+    counts = [[row[0] for row in table[r]] for r in range(world)]
+    rf = [int(L.sgr_rebalance_row_floats(C.byref(segs[k]))) for k in range(nm)]
+    pieces = gather_pieces(counts, [4 * f for f in rf], int(piece_bytes))
+    floats = lambda ranges: sum(rows * rf[k] for k, _, rows in ranges)
+    cap = max((floats(r) for s, r in pieces if s == rank or rank == dst), default=0)
+    buf = torch.empty((cap,), dtype=torch.float32, device=dev) if cap else None
+    host = at_rank = seg_info = None
+    if rank == dst:
+        host, seg_info = [], []
+        for k, (params, moments) in enumerate(infos):
+            n = sum(counts[r][k] for r in range(world))
+            h = {a: torch.empty((n,) + tuple(p.shape[1:]), dtype=torch.float32) for a, p in zip(PARAM_NAMES, params)}
+            h.update(max_radii2D=torch.empty(n), xyz_gradient_accum=torch.empty(n, 2), denom=torch.empty(n, 1))
+            h["adam"] = {PARAM_NAMES[a]: dict(step=table[0][k][4 + a], exp_avg=torch.empty_like(h[PARAM_NAMES[a]]),
+                                              exp_avg_sq=torch.empty_like(h[PARAM_NAMES[a]]))
+                         for a in range(len(PARAM_NAMES)) if table[0][k][4 + a] >= 0}
+            host.append(h)
+            w = [int(math.prod(p.shape[1:])) for p in params]
+            seg_info.append((w, [a for a in range(len(PARAM_NAMES)) if (segs[k].moments >> a) & 1]))
+        at_rank = [[sum(counts[q][k] for q in range(r)) for k in range(nm)] for r in range(world)]
+    for s, ranges in pieces:
+        n = floats(ranges)
+        if rank == s:
+            args, scratch = _rebalance_tables(L, [(k, 0, first, 0, rows) for k, first, rows in ranges], [buf[:n]], dev)
+            _capi.call("sgr_rebalance_pack", dev, segs, nm, *args)
+        if s != dst:
+            tr.exchange({dst: buf[:n]} if rank == s else {}, {s: buf[:n]} if rank == dst else {})
+        if rank == dst:
+            _unpack_rows(buf[:n].cpu(), ranges, seg_info, host, at_rank[s])
+    return host
+
+
+# Host storage address -> the location torch.save records for it.  save_checkpoint assembles the global tensors on the host (so the device
+# memory of dst stays bounded) but writes them as the single-GPU file holds them, on dst's CUDA device, so that a bare torch.load (the
+# reference's train.py:42, scene.py:42) puts them there.  The tagger answers only while save_checkpoint is writing (_SAVE_AS non-empty).
+_SAVE_AS = {}
+_tagger = []
+
+
+def _tag_host_storage(storage):
+    if _SAVE_AS and storage.device.type == "cpu":
+        return _SAVE_AS.get(storage.data_ptr())
+    return None
+
+
+@contextlib.contextmanager
+def _saved_on(tensors, device):
+    """torch.save inside the block records the host storages of `tensors` at `device` (torch.serialization.register_package)."""
+    if not _tagger:
+        torch.serialization.register_package(1, _tag_host_storage, lambda storage, location: None)
+        _tagger.append(_tag_host_storage)
+    for t in tensors:
+        if t.device.type == "cpu" and t.numel():
+            _SAVE_AS[t.untyped_storage().data_ptr()] = f"cuda:{device.index if device.index is not None else torch.cuda.current_device()}"
+    try:
+        yield
+    finally:
+        _SAVE_AS.clear()
+
+
+def _checkpoint_entries(model, st, optimizer, is_final: bool, extra, dev, on_device: list):
+    """One sub-model's entries of io.save_checkpoint from its gathered state: the parameters as nn.Parameters (the model's requires_grad),
+    and unless is_final the training extras in GaussianModel.state_dict's order (gaussian_model.py:180-205), then the caller's `extra`.
+    The gathered host tensors are appended to `on_device` (written at dev's location); an empty one is made on dev itself."""
+    from .training import adam_state_dict
+
+    def dev_tensor(t):
+        if t.numel() == 0:
+            return torch.empty(t.shape, dtype=t.dtype, device=dev)
+        on_device.append(t)
+        return t
+
+    params = {a: nn.Parameter(dev_tensor(st[a]), requires_grad=_attr(model, a).requires_grad) for a in PARAM_NAMES}
+    e = {}
+    if not is_final:
+        if _has(model, "spatial_lr_scale"):
+            e["spatial_lr_scale"] = _attr(model, "spatial_lr_scale")
+        e["denom"], e["max_radii2D"], e["xyz_gradient_accum"] = (dev_tensor(st[s]) for s in ("denom", "max_radii2D", "xyz_gradient_accum"))
+        if _has(model, "active_sh_degree"):
+            e["active_sh_degree"] = _attr(model, "active_sh_degree")
+        if optimizer is not None:
+            adam = {a: dict(step=v["step"], exp_avg=dev_tensor(v["exp_avg"]), exp_avg_sq=dev_tensor(v["exp_avg_sq"])) for a, v in st["adam"].items()}
+            e["optimizer"] = adam_state_dict(model, optimizer, state=adam)
+    e.update(extra or {})
+    return params, e
+
+
+def save_checkpoint(path: str, named_models, iteration: int, optimizer=None, *, is_final: bool = False, extras=None, dst: int = 0, group=None,
+                    transport=None, piece_bytes: int = 1 << 30, **other) -> None:
+    """COLLECTIVE: rank `dst` writes the .pth of train.py:218-223 that io.save_checkpoint writes on one GPU for the rank-major concatenation
+    of the ranks' rows (gather_state).  named_models: {model_name: this rank's sub-model} in composition order, the same names on every
+    rank.  Per model: the seven parameters and, unless is_final, spatial_lr_scale and active_sh_degree (where the model has them), denom,
+    max_radii2D, xyz_gradient_accum and 'optimizer', the model's state in torch.optim.Adam.state_dict() format with the reference's group
+    names (training.adam_state_dict, from the groups of this rank's `optimizer`).  extras: {model_name: {key: value}} added to a model's
+    entries; **other (actor_pose, sky_cubemap, color_correction, pose_correction, ...: replicated state) is written by dst only.
+
+    The file is the single-GPU one as the reference reads it with a bare torch.load: the parameters are nn.Parameters with the requires_grad
+    of dst's model, and the parameters, moments and statistics are recorded at dst's CUDA device (the Adam steps on the CPU, as torch keeps
+    them), although dst assembles them on the host and never holds the whole model on the device."""
+    names = list(named_models)
+    objs = [named_models[n] for n in names]
+    state = gather_state(objs, None if is_final else optimizer, dst=dst, group=group, transport=transport, piece_bytes=piece_bytes)
+    if state is None:
+        return
+    from . import io
+    dev = _attr(objs[0], "_xyz").device
+    models, ex, on_device = {}, {}, []
+    for n, m, st in zip(names, objs, state):
+        models[n], ex[n] = _checkpoint_entries(m, st, None if is_final else optimizer, is_final, (extras or {}).get(n), dev, on_device)
+    with _saved_on(on_device, dev):
+        io.save_checkpoint(path, models, iteration, ex, **other)
+
+
+def save_ply(path: str, named_models, *, dst: int = 0, group=None, transport=None, piece_bytes: int = 1 << 30) -> None:
+    """COLLECTIVE: rank `dst` writes the point_cloud.ply of Scene.save (street_gaussian_model.py:94-105), the bytes io.save_ply writes on one
+    GPU for the rank-major concatenation of the ranks' rows.  named_models as for save_checkpoint; statistics are not needed."""
+    names = list(named_models)
+    objs = []
+    for n in names:
+        m = named_models[n]
+        d = {a: _attr(m, a) for a in PARAM_NAMES}  # with zero statistics where the model has none: the row format carries them
+        cnt, dev = int(d["_xyz"].shape[0]), d["_xyz"].device
+        for s, shape in zip(STAT_NAMES, ((cnt,), (cnt, 2), (cnt, 1))):
+            d[s] = _attr(m, s) if _has(m, s) else torch.zeros(shape, device=dev)
+        objs.append(d)
+    state = gather_state(objs, None, dst=dst, group=group, transport=transport, piece_bytes=piece_bytes)
+    if state is None:
+        return
+    from . import io
+    io.save_ply(path, {n: {a: st[a] for a in PARAM_NAMES} for n, st in zip(names, state)})
+
+
+_CKPT_KEYS = ("xyz", "feature_dc", "feature_rest", "opacity", "scaling", "rotation", "semantic")  # gaussian_model.py:182-190, by PARAM_NAMES
+
+
+def load_checkpoint(path: str, models, optimizer=None, *, group=None, transport=None, rasterizer: Optional["GaussianShardedRasterizer"] = None) -> int:
+    """Resume from a .pth written by save_checkpoint, io.save_checkpoint or the reference's train.py, at any world size.  Returns the local
+    Gaussian count.
+
+    models: {model_name: this rank's sub-model} in composition order.  Rank r takes the global rows [B_r, B_{r+1}) of the even split of the
+      model-major array (even_slices, the split rebalance() leaves; a sub-model may get 0 rows).  The file is opened with torch.load(mmap=True)
+      and only this rank's slices are copied to the device of the model's _xyz, so no rank holds the whole model on the device.
+    Parameters are replaced by new nn.Parameters (same requires_grad), in their groups of `optimizer` too (found by identity, as rebalance()
+      does); where the file's 'optimizer' holds state for a parameter (matched by the reference's group names), its state becomes {step, the
+      slices of exp_avg and exp_avg_sq}, otherwise any old state is dropped.  max_radii2D, xyz_gradient_accum and denom take their slices, or
+      zeros when the file is final.  Group learning rates and every other entry of the file are left to the caller.
+    rasterizer: its repartition() is called with the largest rank's count (no collective: every rank computes it from the file).
+    transport / group: only for this rank's index and the world size (ProcessGroupTransport); nothing is exchanged."""
+    tr = transport if transport is not None else ProcessGroupTransport(group)
+    world, rank = int(tr.world), int(tr.rank)
+    names = list(models)
+    objs = [models[n] for n in names]
+    if not objs:
+        raise ValueError("load_checkpoint needs the sub-models (background, then actors)")
+    sd = torch.load(path, map_location="cpu", mmap=True, weights_only=False)
+    for n in names:
+        if n not in sd or not isinstance(sd[n], dict) or "xyz" not in sd[n]:
+            raise KeyError(f"{path} has no Gaussian model '{n}' (it holds {sorted(k for k, v in sd.items() if isinstance(v, dict) and 'xyz' in v)})")
+    slices = even_slices([int(sd[n]["xyz"].shape[0]) for n in names], world)
+    dev = _attr(objs[0], "_xyz").device
+    slots = _param_slots(optimizer)
+    for n, m, (lo, hi) in zip(names, objs, slices[rank]):
+        e = sd[n]
+        opt_state = {}
+        if optimizer is not None and isinstance(e.get("optimizer"), dict):
+            osd = e["optimizer"]
+            for g in osd["param_groups"]:
+                if g.get("name") in ADAM_GROUP_NAMES and len(g["params"]) == 1 and g["params"][0] in osd["state"]:
+                    opt_state[PARAM_NAMES[ADAM_GROUP_NAMES.index(g["name"])]] = osd["state"][g["params"][0]]
+        for a, key in zip(PARAM_NAMES, _CKPT_KEYS):
+            old = _attr(m, a)
+            t = e[key][lo:hi].to(device=dev, dtype=torch.float32).contiguous()
+            p = nn.Parameter(t, requires_grad=old.requires_grad)
+            if id(old) in slots:
+                opt, grp, j = slots[id(old)]
+                grp["params"][j] = p
+                opt.state.pop(old, None)
+                s = opt_state.get(a)
+                if s is not None:
+                    step = s["step"].clone() if isinstance(s["step"], torch.Tensor) else s["step"]
+                    opt.state[p] = dict(step=step, **{mk: s[mk][lo:hi].to(device=dev, dtype=torch.float32).contiguous()
+                                                      for mk in ("exp_avg", "exp_avg_sq")})
+            _set(m, a, p)
+        for s, shape in zip(STAT_NAMES, ((hi - lo,), (hi - lo, 2), (hi - lo, 1))):
+            t = e[s][lo:hi].to(device=dev, dtype=torch.float32).reshape(shape).contiguous() if s in e else torch.zeros(shape, device=dev)
+            _set(m, s, t)
+    P_local = sum(hi - lo for lo, hi in slices[rank])
+    if rasterizer is not None:
+        rasterizer.repartition(P_local, chunk=max(sum(hi - lo for lo, hi in row) for row in slices))
+    return P_local

@@ -219,3 +219,65 @@ def sky_composite(rgb: torch.Tensor, acc: torch.Tensor, cube_map: torch.Tensor, 
     rows, xfer = _resolve(band, group, rasterizer, int(rgb.shape[-2]))  # a bad or mismatched band fails before anything else
     return _SkyComposite.apply(rgb, acc, cube_map, K, w2c, sky_mask, bool(perturb), 1.0 if white_background else 0.0, rows, xfer, rasterizer,
                                blocks)
+
+
+# ---- the lat-long export (SkyCubeMap.save_state_dict, lib/models/sky_cubemap.py:36-46) ----
+def _latlong(cube_map: torch.Tensor, res, want_f32: bool, want_u8: bool):
+    if cube_map.dim() != 4 or cube_map.shape[0] != 6 or cube_map.shape[3] != 3 or cube_map.shape[1] != cube_map.shape[2]:
+        raise ValueError(f"cube_map must be [6, R, R, 3], got {tuple(cube_map.shape)}")
+    if cube_map.dtype != torch.float32:
+        raise ValueError(f"cube_map must be float32, got {cube_map.dtype}")
+    if not cube_map.is_cuda:
+        raise _capi.SgrError(f"street_gaussians_b200.sky needs CUDA tensors (cube_map is on {cube_map.device}; there is no CPU fallback)")
+    if len(res) != 2 or any(int(n) != n or int(n) <= 0 for n in res):
+        raise ValueError(f"res must be two positive integers (height, width), got {res}")
+    H, W = int(res[0]), int(res[1])
+    dev = cube_map.device
+    cube = cube_map.detach().contiguous()
+    out = torch.empty((H, W, 3), device=dev, dtype=torch.float32) if want_f32 else None
+    u8 = torch.empty((H, W, 3), device=dev, dtype=torch.uint8) if want_u8 else None
+    _capi.call("sgr_sky_cube_to_latlong", dev, int(cube.shape[1]), ptr(cube), H, W, ptr(out), ptr(u8))
+    return out, u8
+
+
+def cubemap_to_latlong(cube_map: torch.Tensor, res) -> torch.Tensor:
+    """cubemap_to_latlong (lib/models/sky_cubemap.py:178-191): the cube map [6, R, R, 3] sampled along the rows of latitude and columns
+    of longitude of a res = (H, W) image -> [H, W, 3] fp32, unclamped, on the cube's device.  One kernel (sgr_sky_cube_to_latlong) with
+    sky_composite's lookup; no nvdiffrast, and no gradient (the reference uses the result only as an image)."""
+    return _latlong(cube_map, res, True, False)[0]
+
+
+def latlong_u8(cube_map: torch.Tensor, res=None) -> torch.Tensor:
+    """The bytes of the reference's sky_latlong.png: (cubemap_to_latlong(cube_map, res).clamp(0, 1) * 255).astype(uint8), [H, W, 3] uint8 on
+    the cube's device, formed in the same kernel.  res defaults to (R, 2 R), as SkyCubeMap.save_state_dict uses."""
+    R = int(cube_map.shape[1]) if cube_map.dim() == 4 else 0
+    return _latlong(cube_map, (R, 2 * R) if res is None else res, False, True)[1]
+
+
+def png_bytes(rgb) -> bytes:
+    """An 8-bit RGB PNG of rgb [H, W, 3] uint8 (numpy or a CPU tensor): signature, IHDR, one zlib IDAT of filter-0 rows, IEND."""
+    import struct
+    import zlib
+
+    import numpy as np
+
+    a = np.ascontiguousarray(rgb.numpy() if isinstance(rgb, torch.Tensor) else rgb)
+    if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3 or a.shape[0] == 0 or a.shape[1] == 0:
+        raise ValueError(f"a PNG image must be a non-empty uint8 [H, W, 3] array, got {a.dtype} {a.shape}")
+    H, W = a.shape[:2]
+    raw = np.concatenate([np.zeros((H, 1), np.uint8), a.reshape(H, 3 * W)], axis=1).tobytes()
+
+    def chunk(kind: bytes, data: bytes) -> bytes:
+        return struct.pack(">I", len(data)) + kind + data + struct.pack(">I", zlib.crc32(kind + data) & 0xFFFFFFFF)
+
+    return (b"\x89PNG\r\n\x1a\n" + chunk(b"IHDR", struct.pack(">IIBBBBB", W, H, 8, 2, 0, 0, 0)) + chunk(b"IDAT", zlib.compress(raw, 6))
+            + chunk(b"IEND", b""))
+
+
+def save_latlong_png(path: str, cube_map: torch.Tensor, res=None) -> None:
+    """Write the reference's sky_latlong.png (SkyCubeMap.save_state_dict, sky_cubemap.py:43-45) for cube_map [6, R, R, 3] at res = (H, W),
+    by default (R, 2 R): latlong_u8 as an 8-bit RGB PNG (png_bytes; no imageio).  The pixels are the reference's; the compressed bytes
+    are zlib's, not imageio's."""
+    data = png_bytes(latlong_u8(cube_map, res).cpu())
+    with open(path, "wb") as f:
+        f.write(data)

@@ -227,6 +227,33 @@ def _install(model, params, new_params, new_moments, new_stats, slots):
         _set(model, name, t)
 
 
+ADAM_GROUP_NAMES = ("xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation", "semantic")  # gaussian_model.py:289-297, by PARAM_NAMES
+
+
+def adam_state_dict(model, optimizer, *, state=None) -> dict:
+    """One sub-model's optimizer state in the format torch.optim.Adam.state_dict() gives for the reference's per-model optimizer
+    (GaussianModel.training_setup, gaussian_model.py:286-303): seven groups named xyz, f_dc, f_rest, opacity, scaling, rotation, semantic,
+    parameter i in group i, each group with the lr, betas and eps of the group of `optimizer` (one optimizer or a list, e.g. a FusedAdam
+    or SparseAdam over several sub-models) that holds the model's tensor, found by identity; state[i] = {step (fp32 CPU scalar tensor, as
+    torch keeps it), exp_avg, exp_avg_sq} for the tensors with Adam state.  The moments are the optimizer's tensors, not copies.  state:
+    {parameter name: {"step", "exp_avg", "exp_avg_sq"}} to use instead of the optimizer's (sharded.gather_state's "adam").  What
+    GaussianModel.state_dict stores as 'optimizer', so a torch.optim.Adam built as the reference builds it load_state_dict()s it."""
+    slots = _param_slots(optimizer)
+    groups, packed = [], {}
+    for i, (a, name) in enumerate(zip(PARAM_NAMES, ADAM_GROUP_NAMES)):
+        p = _attr(model, a)
+        if id(p) not in slots:
+            raise ValueError(f"{a} is not held by the optimizer")
+        opt, g, _ = slots[id(p)]
+        groups.append(dict(params=[torch.zeros(0)], lr=g["lr"], betas=tuple(g["betas"]), eps=g["eps"], name=name))
+        st = opt.state.get(p) if state is None else state.get(a)
+        if st:
+            packed[i] = dict(step=torch.tensor(float(int(st["step"])), dtype=torch.float32), exp_avg=st["exp_avg"], exp_avg_sq=st["exp_avg_sq"])
+    sd = torch.optim.Adam(groups, lr=0.0, eps=1e-15).state_dict()
+    sd["state"] = packed
+    return sd
+
+
 def _densify(models, max_grad, min_opacity, prune_big_points, optimizer=None, grad_abs=False, seed=None, noise=None, keep_masks=False):
     L = _capi.lib()
     models = list(models)

@@ -21,6 +21,10 @@ kernels.
 With the argument `rebalance` only the rebalance leg runs (run_rebalance): sharded.rebalance over NCCL on an uneven split, against the
 global arrays each rank restates.  It has run at world 1 only, not on several H100s; tests/test_rebalance_gpu.py emulates 2 to 8 ranks.
 
+With the argument `checkpoint` only the checkpoint leg runs (run_checkpoint): sharded.save_checkpoint at world N over torch.distributed,
+sharded.load_checkpoint at the same world N into fresh models, and the next training step against the uninterrupted one.  It has run at
+world 1 only, not on several H100s; tests/test_sharded_checkpoint_gpu.py emulates 1 to 8 ranks on one GPU.
+
 With the argument `compose` (NCCL all_reduce of the accumulator rows) or `compose-p2p` (the rasterizer's peer workspace) only the composer
 leg runs (run_compose): compose(..., group= / rasterizer=) on each rank's rows of a config-C-like scene, before and after the rebalanced
 split.  It has run at world 1 only, not on several H100s; tests/test_sharded_compose_gpu.py emulates 2 to 8 ranks on one GPU.
@@ -387,6 +391,102 @@ def run_rebalance(rank, world, dev, W=640, H=400):
     return P_new
 
 
+def run_checkpoint(rank, world, dev, W=640, H=400):
+    """Checkpoint leg (argument `checkpoint`): every rank owns the even split of a with_raw scene and steps FusedAdam three times on it;
+    sharded.save_checkpoint gathers the rows to rank 0 over torch.distributed (ProcessGroupTransport: the all_gather of the table, then one
+    batch_isend_irecv per piece of at most 1 MiB) and writes the file; every rank then resumes into fresh models and a fresh FusedAdam with
+    sharded.load_checkpoint.  The resumed rows, moments and statistics must be the uninterrupted run's bit for bit, and one training step
+    (compose -> GaussianShardedRasterizer -> loss -> backward -> FusedAdam) on both must give bit-equal own image rows and parameter
+    gradients within GRAD_TOL of each other (their float atomics add in any order, so the steps' bytes may differ)."""
+    import tempfile
+    import types
+    from street_gaussians_b200 import sharded, training
+    names, stats = training.PARAM_NAMES, training.STAT_NAMES
+    scene = synthetic.make_scene(P=200_000, width=W, height=H, sh_degree=3, seed=83, n_vehicles=4, per_vehicle=20_000, with_raw=True,
+                                 scale_med=0.02)
+    raw = scene["raw"]
+    poses, idft = raw["poses"].to(dev), raw["idft"].to(dev)
+    g = torch.Generator().manual_seed(10)
+    glob = []
+    for r in raw["models"]:
+        n = r["xyz"].shape[0]
+        m = {"_" + a: v.to(dev).contiguous() for a, v in r.items()}
+        m["_semantic"] = torch.rand(n, 2, generator=g).to(dev)
+        m["max_radii2D"], m["xyz_gradient_accum"], m["denom"] = (torch.rand(n, generator=g).to(dev), torch.rand(n, 2, generator=g).to(dev),
+                                                                 torch.rand(n, 1, generator=g).to(dev) + 1)
+        glob.append(m)
+    rows = sharded.even_slices([m["_xyz"].shape[0] for m in glob], world)[rank]
+    grads = [[torch.randn(m[a].shape, generator=g).to(dev) * 1e-2 for a in names] for m in glob]
+
+    def model(m, lo, hi):
+        return types.SimpleNamespace(**{a: torch.nn.Parameter(m[a][lo:hi].clone()) for a in names}, **{s: m[s][lo:hi].clone() for s in stats},
+                                     spatial_lr_scale=1.0, active_sh_degree=3)
+
+    def adam(objs):
+        return training.FusedAdam([{"params": [getattr(o, a)], "lr": 1e-3 * (1 + i), "name": a} for o in objs for i, a in enumerate(names)],
+                                  eps=1e-15)
+
+    mine = [model(m, lo, hi) for m, (lo, hi) in zip(glob, rows)]
+    opt = adam(mine)
+    for it in range(3):
+        for k, o in enumerate(mine):
+            for a, gk in zip(names, grads[k]):
+                getattr(o, a).grad = gk[rows[k][0]:rows[k][1]] * (1 + it)
+        opt.step()
+    st = util.settings_from(sgb, scene["cam"], dev)
+    gw = torch.Generator(device=dev).manual_seed(4)
+    wc = torch.randn((3, H, W), generator=gw, device=dev)
+    img_rows = band_of_rows(H, rank, world).to(dev)
+    path = [os.path.join(tempfile.mkdtemp(prefix="sgr_ckpt_"), "iteration_3.pth")] if rank == 0 else [None]
+    if world > 1:
+        dist.broadcast_object_list(path, src=0)
+    path = path[0]
+    named = lambda objs: {f"m{k}": o for k, o in enumerate(objs)}
+    sharded.save_checkpoint(path, named(mine), 3, opt, piece_bytes=1 << 20)
+    if world > 1:
+        dist.barrier()
+    new = [model(m, 0, 1) for m in glob]
+    nopt = adam(new)
+    rast = GaussianShardedRasterizer(st)
+    P = sharded.load_checkpoint(path, named(new), nopt, rasterizer=rast)
+    assert P == sum(hi - lo for lo, hi in rows) and rast.chunk == max(sum(hi - lo for lo, hi in r) for r in sharded.even_slices(
+        [m["_xyz"].shape[0] for m in glob], world)), (P, rast.chunk)
+    bits = lambda t: t.detach().contiguous().view(torch.int32)
+    for k, (o, q) in enumerate(zip(new, mine)):
+        for a in names:
+            p, pq = getattr(o, a), getattr(q, a)
+            assert torch.equal(bits(p), bits(pq)), ("resumed", k, a)
+            assert any(p is x for grp in nopt.param_groups for x in grp["params"]) and int(nopt.state[p]["step"]) == 3
+            for mk in ("exp_avg", "exp_avg_sq"):
+                assert torch.equal(bits(nopt.state[p][mk]), bits(opt.state[pq][mk])), ("resumed", k, a, mk)
+        for s in stats:
+            assert torch.equal(bits(getattr(o, s)), bits(getattr(q, s))), ("resumed", k, s)
+
+    def train_step(objs, o, r):
+        o.zero_grad(set_to_none=True)
+        xyz, rot, scale, opac, sh = sgb.compose(objs, poses, idft)
+        color = r(means3D=xyz, means2D=None, opacities=opac, shs=sh, scales=scale, rotations=rot)[0]
+        (color * wc).sum().backward()
+        gr = [None if getattr(x, a).grad is None else getattr(x, a).grad.clone() for x in objs for a in names[:6]]
+        o.step()
+        return color.detach(), gr
+
+    c0, g0 = train_step(mine, opt, GaussianShardedRasterizer(st))
+    c1, g1 = train_step(new, nopt, rast)
+    assert torch.equal(c0[:, img_rows], c1[:, img_rows]), "resumed step: own image rows differ"
+    worst = 0.0
+    for a, b in zip(g0, g1):
+        assert (a is None) == (b is None), "resumed step: a gradient is missing"
+        if a is not None and a.numel():
+            err = float((a - b).abs().max()) / max(float(a.abs().max()), 1e-30)
+            worst = max(worst, err)
+    assert worst <= GRAD_TOL, ("resumed step: gradients", worst)
+    if rank == 0:
+        os.remove(path)
+        os.rmdir(os.path.dirname(path))
+    return P, worst
+
+
 def run_compose(rank, world, dev, exchange, n_bg=400_000, actors=(20_000, 0, 7_000, 35_000, 1_000, 12_000, 3, 50_000)):
     """compose(..., rasterizer=) on this rank's rows of a config-C-like scene (background, 8 tracked actors, flip mask, pose correction)
     against compose() of the whole scene: own composed rows and raw gradient rows bit-equal, dL/dposes and dL/dcorrection the same bytes on
@@ -552,6 +652,10 @@ def main():
         elif mode == "layers":
             worst = run_layers(rank, world, dev)
             print(f"[rank {rank}/{world}] render layers (fused p2p step): own rows bit-equal, gradients rel err {worst:.2e}", flush=True)
+        elif mode == "checkpoint":
+            P, worst = run_checkpoint(rank, world, dev)
+            print(f"[rank {rank}/{world}] checkpoint: saved at world {world} and resumed, {P} Gaussians, rows / moments / statistics bit for "
+                  f"bit, the next step's own image rows bit-equal, gradients rel err {worst:.2e}", flush=True)
         elif mode == "rebalance":
             P_new = run_rebalance(rank, world, dev)
             print(f"[rank {rank}/{world}] rebalance: {P_new} Gaussians, rows / moments / statistics the even split's slice bit for bit, "
