@@ -994,6 +994,26 @@ int sgr_rebalance_pack(const SgrDensifySegment *segments, int32_t num_segments, 
 int sgr_rebalance_splice(const SgrDensifySegment *segments, const SgrDensifyOutput *outputs, int32_t num_segments, const SgrRebalanceRange *ranges,
                          int32_t num_ranges, const float *const *buffers, const int64_t *buffer_floats, int32_t num_buffers, void *scratch,
                          size_t scratch_bytes, void *stream);
+/* One round of moving buffers between ranks through the Gaussian-sharded step's peer workspace (sharded.PeerTransport: rebalance's
+ * table all-gather and row moves), with no NCCL call.  Rank p's STAGING region is the first staging_bytes bytes from peers->records[p]
+ * (the workspace's record, radii and grad2d sections, which hold nothing between a backward and the next forward).
+ *   stage : ONE launch copies each `stage` piece (rank == this rank) from `local` into this rank's staging region at `offset`;
+ *   device barrier (sgr_peer_barrier with the device-side count);
+ *   pull  : ONE launch copies each `pull` piece from rank `rank`'s staging region at `offset` into `local` (peer memory, NVLink).
+ * There is no barrier after the pull: the caller issues one (sgr_peer_barrier) before any rank rewrites a staging region a peer may still
+ * read.  Offsets and lengths are in floats; every offset is a multiple of 4 and every `local` with floats > 0 is 16-byte aligned (the
+ * copies use 16-byte loads and stores; a piece's last floats past a multiple of 4 are copied one by one), pieces lie inside staging_bytes,
+ * and each side has at most SGR_MAX_PEERS pieces (the table travels as the kernel's argument).  Pieces of one launch must not overlap
+ * in their destination.  Traffic: 2 x 4 B per float on each side.  Arguments are checked before anything is enqueued. */
+typedef struct SgrPeerPiece {
+	int32_t rank;      /* rank whose staging region holds the piece (stage: this rank) */
+	int32_t reserved;
+	int64_t offset;    /* first float of the piece in that staging region */
+	int64_t floats;
+	float *local;      /* device: the staged floats' source, or the pulled floats' destination, in this rank's memory */
+} SgrPeerPiece;
+int sgr_peer_exchange_round(const SgrPeers *peers, size_t staging_bytes, const SgrPeerPiece *stage, int32_t num_stage, const SgrPeerPiece *pull,
+                            int32_t num_pull, void *stream);
 
 /* ---- Visibility-masked ("sparse") Adam: an OPT-IN deviation from the reference (no counterpart there) ----
  * One Adam step that updates only the rows of the Gaussians this frame rendered.  Segments are the sub-models in composition order

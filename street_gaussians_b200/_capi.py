@@ -42,7 +42,7 @@ SYMBOLS = ["sgr_abi_version", "sgr_last_error", "sgr_launch_count", "sgr_set_nea
            "sgr_band_finish_features_backward", "sgr_eval_metrics_scratch_bytes",
            "sgr_eval_metrics_accumulate", "sgr_band_eval_metrics_accumulate", "sgr_eval_metrics_finish",
            "sgr_band_sky_composite_backward_or_marks", "sgr_sky_grad_peer_sum_union", "sgr_cube_sparse_adam_step",
-           "sgr_sky_cube_to_latlong"]
+           "sgr_sky_cube_to_latlong", "sgr_peer_exchange_round"]
 
 SKY_MASK_ACC, SKY_MASK_GIVEN = 0, 1
 SEMANTIC_LOGITS, SEMANTIC_PROBABILITIES = 0, 1
@@ -134,6 +134,10 @@ class SgrRebalanceRange(C.Structure):
 
 
 SPARSE_ADAM_MAX_WIDTH = 8388607   # floats per row
+
+
+class SgrPeerPiece(C.Structure):
+    _fields_ = [("rank", C.c_int32), ("reserved", C.c_int32), ("offset", C.c_int64), ("floats", C.c_int64), ("local", C.c_void_p)]
 
 
 class SgrSparseAdamSegment(C.Structure):
@@ -405,6 +409,8 @@ def lib():
     L.sgr_rebalance_pack.argtypes = [C.POINTER(SgrDensifySegment), C.c_int32] + rebalance_tables
     L.sgr_rebalance_splice.restype = C.c_int
     L.sgr_rebalance_splice.argtypes = [C.POINTER(SgrDensifySegment), C.POINTER(SgrDensifyOutput), C.c_int32] + rebalance_tables
+    L.sgr_peer_exchange_round.restype = C.c_int
+    L.sgr_peer_exchange_round.argtypes = [C.POINTER(SgrPeers), C.c_size_t, C.POINTER(SgrPeerPiece), C.c_int32, C.POINTER(SgrPeerPiece), C.c_int32, vp]
     L.sgr_sparse_adam_step.restype = C.c_int
     L.sgr_sparse_adam_step.argtypes = [C.POINTER(SgrSparseAdamSegment), C.c_int32, vp, C.c_double, C.c_double, C.c_double, vp]
     L.sgr_cube_sparse_adam_step.restype = C.c_int

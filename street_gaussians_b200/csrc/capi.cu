@@ -2252,6 +2252,59 @@ int sgr_rebalance_splice(const SgrDensifySegment *segments, const SgrDensifyOutp
 	return rebalance_copy(fn, spans, num_ranges, scratch, scratch_bytes, stream);
 }
 
+// the piece table of one side of sgr_peer_exchange_round: pieces checked against the staging regions, the empty ones dropped
+static int peer_pieces(const char *fn, const char *side, const SgrPeers *peers, size_t staging_bytes, const SgrPeerPiece *pieces, int32_t num,
+                       bool stage, PieceTable &t, long long &blocks) {
+	t.n = 0;
+	if (num < 0 || num > SGR_MAX_PEERS) return fail(SGR_EINVAL, "%s: %d %s pieces (at most %d)", fn, num, side, SGR_MAX_PEERS);
+	if (num > 0 && !pieces) return fail(SGR_EINVAL, "%s: the %s pieces are NULL", fn, side);
+	const long long cap = (long long)(staging_bytes / sizeof(float));
+	for (int i = 0; i < num; i++) {
+		const SgrPeerPiece &p = pieces[i];
+		if (p.rank < 0 || p.rank >= peers->world || (stage && p.rank != peers->rank))
+			return fail(SGR_EINVAL, "%s: %s piece %d names rank %d (this rank %d of %d)", fn, side, i, p.rank, peers->rank, peers->world);
+		if (p.floats < 0 || p.offset < 0 || (p.offset & 3) || p.offset > cap - p.floats)
+			return fail(SGR_EINVAL, "%s: %s piece %d: floats [%lld, +%lld) do not lie 16-byte aligned inside the %lld floats of a staging region", fn, side,
+			            i, (long long)p.offset, (long long)p.floats, cap);
+		if (p.floats == 0) continue;
+		if (!p.local) return fail(SGR_EINVAL, "%s: %s piece %d has a NULL buffer", fn, side, i);
+		if (int rc = check_aligned16("a piece's buffer", p.local)) return rc;
+		float *region = reinterpret_cast<float *>(peers->records[p.rank]) + p.offset;
+		t.src[t.n] = stage ? p.local : region;
+		t.dst[t.n] = stage ? region : p.local;
+		t.floats[t.n] = p.floats;
+		blocks += peer_piece_blocks(p.floats);
+		t.n++;
+	}
+	return SGR_OK;
+}
+
+int sgr_peer_exchange_round(const SgrPeers *peers, size_t staging_bytes, const SgrPeerPiece *stage, int32_t num_stage, const SgrPeerPiece *pull,
+                            int32_t num_pull, void *stream) {
+	const char *fn = "sgr_peer_exchange_round";
+	if (!peers) return fail(SGR_EINVAL, "%s: peers is NULL", fn);
+	if (peers->world < 1 || peers->world > SGR_MAX_PEERS || peers->rank < 0 || peers->rank >= peers->world)
+		return fail(SGR_EINVAL, "%s: bad peer table: world=%d rank=%d (at most %d ranks)", fn, peers->world, peers->rank, SGR_MAX_PEERS);
+	PeerTable pt = {};
+	pt.world = peers->world;
+	pt.rank = peers->rank;
+	for (int p = 0; p < peers->world; p++) {
+		if (!peers->records[p]) return fail(SGR_EINVAL, "%s: peer table entry %d has no staging region", fn, p);
+		if (int rc = check_aligned16("a staging region", peers->records[p])) return rc;
+		if (peers->world > 1 && !peers->flags[p]) return fail(SGR_EINVAL, "%s: peer table entry %d has no barrier pad", fn, p);
+		pt.flags[p] = peers->flags[p];
+	}
+	PieceTable ts = {}, tp = {};
+	long long blocks_stage = 0, blocks_pull = 0;
+	if (int rc = peer_pieces(fn, "stage", peers, staging_bytes, stage, num_stage, true, ts, blocks_stage)) return rc;
+	if (int rc = peer_pieces(fn, "pull", peers, staging_bytes, pull, num_pull, false, tp, blocks_pull)) return rc;
+	if (blocks_stage > 0x7fffffffLL || blocks_pull > 0x7fffffffLL) return fail(SGR_EUNSUPPORTED, "%s: more than 2^31-1 blocks of floats to copy", fn);
+	cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+	const bool debug = false;
+	SGR_TRY(launch_peer_exchange_round(pt, ts, tp, st), fn);
+	return SGR_OK;
+}
+
 int sgr_sparse_adam_step(const SgrSparseAdamSegment *segments, int32_t num_segments, const int32_t *radii, double beta1, double beta2,
                          double eps, void *stream) {
 	if (!segments || num_segments <= 0) return fail(SGR_EINVAL, "segment table is empty");

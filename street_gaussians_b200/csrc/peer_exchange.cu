@@ -404,6 +404,56 @@ cudaError_t launch_sky_grad_peer_sum(const PeerTable &pt, const SkyPeers &sp, in
 	return launch_peer_barrier(pt, 0u, nullptr, st);
 }
 
+// ---- buffers moved through the staging regions (sgr_peer_exchange_round) ----
+// One CTA copies kPieceVec x 256 consecutive float4 of one piece: every thread issues its kPieceVec 16-B loads before its first store,
+// and the lanes of a warp touch consecutive 16-B pieces, so every load request is whole 128-B lines (over NVLink in the pull).  The
+// piece's last (floats mod 4) floats are copied one by one by the CTA that holds its end.
+constexpr int kPieceThreads = 256, kPieceVec = 4;
+constexpr long long kPieceFloats = 4LL * kPieceThreads * kPieceVec;
+long long peer_piece_blocks(long long floats) { return (floats + kPieceFloats - 1) / kPieceFloats; }
+
+__global__ void __launch_bounds__(kPieceThreads) copy_pieces_kernel(const __grid_constant__ PieceTable t) {
+	int i = 0;
+	while (i + 1 < t.n && (int)blockIdx.x >= t.block_start[i + 1]) i++;
+	const long long e0 = (long long)(blockIdx.x - t.block_start[i]) * kPieceFloats;
+	const long long n = min(kPieceFloats, t.floats[i] - e0);
+	const int nv = (int)(n >> 2);
+	const float4 *src = reinterpret_cast<const float4 *>(t.src[i] + e0);
+	float4 *dst = reinterpret_cast<float4 *>(t.dst[i] + e0);
+	float4 v[kPieceVec];
+#pragma unroll
+	for (int j = 0; j < kPieceVec; j++) {
+		const int k = threadIdx.x + j * kPieceThreads;
+		if (k < nv) v[j] = src[k];
+	}
+#pragma unroll
+	for (int j = 0; j < kPieceVec; j++) {
+		const int k = threadIdx.x + j * kPieceThreads;
+		if (k < nv) dst[k] = v[j];
+	}
+	if (threadIdx.x < (int)(n & 3)) t.dst[i][e0 + 4 * nv + threadIdx.x] = t.src[i][e0 + 4 * nv + threadIdx.x];
+}
+
+static cudaError_t launch_pieces(PieceTable &t, cudaStream_t st) {
+	long long blocks = 0;
+	for (int i = 0; i < t.n; i++) {
+		t.block_start[i] = (int)blocks;
+		blocks += peer_piece_blocks(t.floats[i]);
+	}
+	t.block_start[t.n] = (int)blocks;
+	if (blocks == 0) return cudaSuccess;
+	count_launch();
+	copy_pieces_kernel<<<(unsigned)blocks, kPieceThreads, 0, st>>>(t);
+	return cudaGetLastError();
+}
+
+// stage launch, barrier, pull launch (the pieces without floats are dropped by the caller; a side without pieces launches nothing)
+cudaError_t launch_peer_exchange_round(const PeerTable &pt, PieceTable stage, PieceTable pull, cudaStream_t st) {
+	cudaError_t e = launch_pieces(stage, st);
+	if (e != cudaSuccess || (e = launch_peer_barrier(pt, 0u, nullptr, st)) != cudaSuccess) return e;
+	return launch_pieces(pull, st);
+}
+
 cudaError_t launch_scatter_records(const FrameDev &f, const PeerTable &pt, const GaussRec *rec, const int32_t *radii, cudaStream_t st) {
 	if (pt.chunk == 0) return cudaSuccess;
 	count_launch();

@@ -439,6 +439,17 @@ cudaError_t launch_project_scatter(const FrameDev &f, const PeerTable &pt, const
 cudaError_t launch_scatter_records(const FrameDev &f, const PeerTable &pt, const GaussRec *rec, const int32_t *radii, cudaStream_t st);
 cudaError_t launch_gather_grad2d(const FrameDev &f, const PeerTable &pt, const GaussRec *rec, const int32_t *radii, float *out,
                                  cudaStream_t st);
+// sgr_peer_exchange_round (peer_exchange.cu): up to kMaxPeers copies of n[i] floats from src[i] to dst[i] (16-byte aligned) in one
+// launch; block_start[i] = first CTA of copy i, block_start[n] = the grid (filled by launch_peer_exchange_round)
+struct PieceTable {
+	int n;
+	const float *src[kMaxPeers];
+	float *dst[kMaxPeers];
+	long long floats[kMaxPeers];
+	int block_start[kMaxPeers + 1];
+};
+long long peer_piece_blocks(long long floats);
+cudaError_t launch_peer_exchange_round(const PeerTable &pt, PieceTable stage, PieceTable pull, cudaStream_t st);
 // Gaussian-sharded mode: tile counts / depth keys of gathered records against this rank's band (binning.cu)
 cudaError_t launch_count_tiles(const FrameDev &f, GeomView g, const int32_t *radii, cudaStream_t st, float *zero_rows = nullptr);
 size_t geom_temp_bytes(int P);

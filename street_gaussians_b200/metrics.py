@@ -14,7 +14,10 @@ a device slot, and `ViewMetrics.result()` turns every slot into values with ONE 
 
 On a tile-row band (the multi-GPU rasterizers return images whose rows outside the rank's band are zero), `band=` / `group=` make each
 `add` fetch the rows within the SSIM window's reach from the neighbouring ranks (band_losses.exchange_halo) and `result()` sum every
-slot over the ranks with one all-reduce; every rank gets the whole frame's numbers, without gathering a frame.
+slot over the ranks with one all-reduce; every rank gets the whole frame's numbers, without gathering a frame.  `rasterizer=` (the
+GaussianShardedRasterizer that rendered the rows) takes its band and transport as the band losses do (band_losses.resolve): with
+exchange="p2p" the halo and the sum go over the loss section of its peer workspace (sgr_band_halo_exchange_peers, sgr_band_peer_sum),
+with no NCCL call.
 """
 from __future__ import annotations
 
@@ -98,14 +101,18 @@ class ViewMetrics:
     ssim_masked  with a mask, SSIM of the images zeroed outside it (ssim(mask=)); otherwise SSIM of the whole images, as metrics.py;
     band, group  the rank's TileRowBand and process group of a multi-GPU renderer: `add` is then COLLECTIVE (a halo exchange with the
                  neighbouring ranks) and `result` COLLECTIVE (one all-reduce of every slot).
+    rasterizer   the sharded.GaussianShardedRasterizer that rendered the rows instead: its band (the whole image at world 1), and with
+                 exchange="p2p" the halo and the sum of the slots over the loss section of the workspace its forward set up, which
+                 must hold the [V, 5] fp64 slots of `result` (ValueError otherwise); a band= or group= that differs from it raises.
 
     L1 and PSNR average over the masked pixels' elements (every pixel without a mask); SSIM over all pixels."""
 
-    def __init__(self, clamp: bool = True, quantize8: bool = False, ssim_masked: bool = True, band=None, group=None):
+    def __init__(self, clamp: bool = True, quantize8: bool = False, ssim_masked: bool = True, band=None, group=None, rasterizer=None):
         self.flags = _flags(clamp, quantize8, ssim_masked)
-        self.band, self.group = band, group
+        self.band, self.group, self.rasterizer = band, group, rasterizer
         self._sums: Optional[torch.Tensor] = None
         self._n = 0
+        self._H = 0  # image height of the views added (band_losses.resolve takes it for the rasterizer's band)
 
     def __len__(self) -> int:
         return self._n
@@ -129,18 +136,31 @@ class ViewMetrics:
             raise ValueError(f"image / gt must both be [C, H, W], got {tuple(image.shape)} and {tuple(gt.shape)}")
         dev = image.device
         Cn, H, W = (int(v) for v in image.shape)
-        if self.band is not None:
-            band_losses.check_band(self.band, H)
-            img = band_losses.exchange_halo(image.detach(), self.band, self.group)
+        band = self.band
+        self._H = H
+        if self.rasterizer is not None:
+            band, xfer = band_losses.resolve(self.band, self.group, self.rasterizer, H)
+            band_losses.check_band(band, H)
+            img = xfer.halo(image.detach(), band)
+        elif band is not None:
+            band_losses.check_band(band, H)
+            img = band_losses.exchange_halo(image.detach(), band, self.group)
         else:
             img = _capi.f32(image.detach())
-        accumulate(img[None], _capi.f32(gt.detach(), dev)[None], _mask_u8(mask, H, W, dev), self._slot(dev), self.flags, self.band)
+        accumulate(img[None], _capi.f32(gt.detach(), dev)[None], _mask_u8(mask, H, W, dev), self._slot(dev), self.flags, band)
 
     @torch.no_grad()
     def result(self) -> dict:
         """The scores of the views added so far, and a fresh start: {"psnr", "ssim", "l1": float32 [V], "n": int64 [V] (masked elements),
-        "mean": {"psnr", "ssim", "l1"}}, on the host after one read.  With a band, COLLECTIVE: one all-reduce of the slots."""
+        "mean": {"psnr", "ssim", "l1"}}, on the host after one read.  With a band, COLLECTIVE: one all-reduce of the slots (with a p2p
+        rasterizer, one peer-memory sum)."""
         V, sums = self._n, self._sums
+        xfer = None
+        if V and self.rasterizer is not None:
+            _, xfer = band_losses.resolve(self.band, self.group, self.rasterizer, self._H)
+            if xfer.kind == "p2p" and V * _capi.EVAL_SUMS * 8 > xfer.ws.loss_bytes:
+                raise ValueError(f"the sums of {V} views ({V * _capi.EVAL_SUMS * 8} bytes) do not fit the peer workspace's loss section of "
+                                 f"{xfer.ws.loss_bytes} bytes: call result() after fewer views")
         self._sums, self._n = None, 0
         if V == 0:
             nan = float("nan")
@@ -148,7 +168,9 @@ class ViewMetrics:
             return {"psnr": empty, "ssim": empty, "l1": empty, "n": torch.empty(0, dtype=torch.int64),
                     "mean": {"psnr": nan, "ssim": nan, "l1": nan}}
         sums = sums[:V]
-        if self.band is not None:
+        if xfer is not None:
+            xfer.sum(sums)
+        elif self.band is not None:
             band_losses.all_reduce_sum(sums, self.group)
         # one transfer: the fp32 values and the exact fp64 counts
         both = torch.cat([finish(sums).double().reshape(-1), sums[:, 3]]).cpu()

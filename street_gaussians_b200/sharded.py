@@ -948,7 +948,8 @@ def rebalance_plan(counts: Sequence[Sequence[int]]) -> RebalancePlan:
 
 class ProcessGroupTransport:
     """rebalance()'s two exchanges over torch.distributed (NCCL or gloo): an all_gather of a small int64 table and the packed row
-    buffers.  Tests substitute an object with the same four members that exchanges between emulated ranks."""
+    buffers.  Tests substitute an object with the same four members that exchanges between emulated ranks; PeerTransport is the
+    peer-memory implementation."""
 
     def __init__(self, group=None):
         self.group = group
@@ -972,6 +973,141 @@ class ProcessGroupTransport:
         if ops:
             for req in dist.batch_isend_irecv(ops):
                 req.wait()
+
+
+class PeerPiece(NamedTuple):
+    """`floats` floats of the buffer rank `src` sends to rank `dst`, from float `buf_at` of the send buffer (the same float of the receive
+    buffer), staged at float `stage_at` of the source's staging region."""
+    src: int
+    dst: int
+    stage_at: int
+    buf_at: int
+    floats: int
+
+
+def peer_rounds(sizes: Sequence[Sequence[int]], capacity: int) -> List[List[PeerPiece]]:
+    """The rounds in which PeerTransport.exchange moves sizes[s][d] floats from every rank s to every rank d through staging regions of
+    `capacity` floats.  Each source lays its outgoing buffers out one after the other in ascending destination order, each from a multiple
+    of 4 floats (16-byte loads), and round k stages floats [k C, (k + 1) C) of that layout, C = capacity rounded down to a multiple of 4;
+    a rank with nothing to send has no piece but takes every round's barriers.  Every float moves exactly once, and the schedule depends on
+    `sizes` and `capacity` only, so every rank that holds them computes the same rounds (and issues the same barriers)."""
+    world = len(sizes)
+    sizes = [[int(v) for v in row] for row in sizes]
+    if any(len(row) != world for row in sizes) or any(v < 0 for row in sizes for v in row) or any(sizes[s][s] for s in range(world)):
+        raise ValueError(f"sizes must be [world][world] non-negative float counts with an empty diagonal, got {sizes}")
+    cap = int(capacity) // 4 * 4
+    offs, ends = [], []
+    for row in sizes:
+        at, end, o = 0, 0, []
+        for n in row:
+            o.append(at)
+            if n:
+                end = at + n
+                at = (end + 3) // 4 * 4
+        offs.append(o)
+        ends.append(end)
+    if max(ends, default=0) == 0:
+        return []
+    if cap <= 0:
+        raise ValueError(f"a staging region of {capacity} floats cannot hold a piece")
+    rounds = []
+    for k in range(-(-max(ends) // cap)):
+        lo_k, hi_k = k * cap, (k + 1) * cap
+        pieces = []
+        for s in range(world):
+            for d in range(world):
+                lo, hi = max(offs[s][d], lo_k), min(offs[s][d] + sizes[s][d], hi_k)
+                if lo < hi:
+                    pieces.append(PeerPiece(s, d, lo - lo_k, lo - offs[s][d], hi - lo))
+        rounds.append(pieces)
+    return rounds
+
+
+class PeerTransport:
+    """rebalance()'s transport over the peer workspace of a GaussianShardedRasterizer(exchange="p2p") (DESIGN.md §8): device-side
+    barriers and NVLink loads, no NCCL call.  Opt-in: rebalance(..., transport=PeerTransport(rasterizer)) right after densify_and_prune,
+    with every rank's backward done.
+
+    The transport keeps the workspace the rasterizer holds when it is made, although rebalance() repartitions the rasterizer before it
+    exchanges (the next forward sets up a new workspace when the slot count changed), and never sets one up itself.  Its staging
+    region on each rank is that workspace's record, radii and grad2d sections, which hold nothing between a backward and the next
+    forward; the workspace does not grow.
+      all_gather : the table goes into this rank's staging region, device barrier, every rank's table is pulled into one device array,
+                   which is read back (rebalance's only host read).  The next forward on the workspace takes its leading barrier.
+      exchange   : device barrier, then per round of peer_rounds(): every rank stages its outgoing floats of the round, device barrier,
+                   every rank pulls its pieces from the sources' staging regions (one launch for every source), device barrier.
+    Raises SgrError, before anything is enqueued, for a rasterizer with exchange="nccl", one whose workspace a forward has not set up
+    yet, and one with a forward in flight (its backward needs the records)."""
+
+    def __init__(self, rasterizer: "GaussianShardedRasterizer"):
+        if getattr(rasterizer, "exchange", None) != "p2p":
+            raise _capi.SgrError("PeerTransport moves rows over the peer workspace of a GaussianShardedRasterizer(exchange='p2p'); this "
+                                 f"rasterizer has exchange={getattr(rasterizer, 'exchange', None)!r}: use ProcessGroupTransport")
+        ws = rasterizer._ws
+        if ws is None:
+            raise _capi.SgrError("PeerTransport stages the rows in the rasterizer's peer workspace: run the rasterizer's forward and backward first")
+        self.ws = ws
+        self.world, self.rank = ws.world, ws.rank
+        self.staging_bytes = (ws.off_grad + 48 * ws.P_total) // 16 * 16
+        self._check_idle()
+
+    def _check_idle(self):
+        if self.ws.in_flight:
+            raise _capi.SgrError("PeerTransport reuses the records of the rasterizer's peer workspace: run backward() of the last forward (or "
+                                 "call release_workspace()) before rebalancing")
+
+    def _round(self, stage, pull):
+        tab = lambda ps: (_capi.SgrPeerPiece * max(1, len(ps)))(*ps)
+        _capi.call("sgr_peer_exchange_round", self.ws.buf.device, C.byref(self.ws.peers), self.staging_bytes, tab(stage), len(stage), tab(pull),
+                   len(pull))
+
+    def all_gather(self, t: torch.Tensor) -> List[torch.Tensor]:
+        """Every rank's `t` (a CPU tensor of a whole number of floats), as CPU tensors in rank order."""
+        self._check_idle()
+        if self.world == 1:
+            return [t]
+        ws, dev = self.ws, self.ws.buf.device
+        flat = t.contiguous().view(-1).view(torch.uint8)
+        if flat.numel() % 4:
+            raise ValueError(f"all_gather moves whole floats, got {flat.numel()} bytes")
+        n = flat.numel() // 4
+        slot = (n + 3) // 4 * 4
+        if 4 * n > self.staging_bytes:
+            raise ValueError(f"a table of {4 * n} bytes does not fit the staging region of {self.staging_bytes} bytes")
+        local = flat.view(torch.float32).to(dev)
+        out = torch.empty((self.world, slot), dtype=torch.float32, device=dev)
+        ws.next_epochs(1)
+        self._round([_capi.SgrPeerPiece(self.rank, 0, 0, n, local.data_ptr())],
+                    [_capi.SgrPeerPiece(p, 0, 0, n, out[p].data_ptr()) for p in range(self.world)])
+        ws.fwd_pending = True  # peers may still read this rank's table: the next forward's delivery waits for its leading barrier
+        # into pinned memory, then a wait on this stream alone: a copy into pageable memory would block inside the driver until the
+        # barrier lets the pull through, and ranks emulated by threads of one process need the driver to enqueue their own work meanwhile
+        host = out
+        if dev.type == "cuda":
+            host = torch.empty(out.shape, dtype=out.dtype, pin_memory=True)
+            host.copy_(out, non_blocking=True)
+            torch.cuda.current_stream(dev).synchronize()
+        return [host[p, :n].clone().view(t.dtype).view(t.shape) for p in range(self.world)]
+
+    def exchange(self, sends: dict, recvs: dict, sizes: Sequence[Sequence[int]]) -> None:
+        """sends[dst] (fp32 device buffers) goes to rank dst and recvs[src] is filled from rank src.  sizes[s][d]: the floats rank s sends
+        rank d, the same table on every rank (rebalance derives it from its plan), from which every rank computes the same rounds."""
+        self._check_idle()
+        me = self.rank
+        for d in range(self.world):
+            for bufs, n, what in ((sends, sizes[me][d], "send"), (recvs, sizes[d][me], "receive")):
+                b = bufs.get(d)
+                if (b.numel() if b is not None else 0) != n or (b is not None and (b.dtype != torch.float32 or not b.is_contiguous())):
+                    raise ValueError(f"the {what} buffer of rank {d} must be {n} contiguous fp32 floats")
+        rounds = peer_rounds(sizes, self.staging_bytes // 4)
+        ws, dev = self.ws, self.ws.buf.device
+        ws.next_epochs(1 + 2 * len(rounds))
+        _capi.call("sgr_peer_barrier", dev, C.byref(ws.peers), 0)  # a peer may still gather grad2d rows or read the table from this region
+        for pieces in rounds:
+            self._round([_capi.SgrPeerPiece(me, 0, p.stage_at, p.floats, sends[p.dst].data_ptr() + 4 * p.buf_at) for p in pieces if p.src == me],
+                        [_capi.SgrPeerPiece(p.src, 0, p.stage_at, p.floats, recvs[p.src].data_ptr() + 4 * p.buf_at) for p in pieces if p.dst == me])
+            _capi.call("sgr_peer_barrier", dev, C.byref(ws.peers), 0)  # every pull of the round is done before a region is rewritten
+        ws.fwd_pending = False
 
 
 def _rebalance_tables(L, ranges, buffers, dev):
@@ -1031,10 +1167,12 @@ def rebalance(models: Sequence, optimizer=None, group: Optional[dist.ProcessGrou
       by identity, and their state moves to the new key with the moments of the rows they now hold; step is unchanged and must be equal
       on every rank (ValueError otherwise, on every rank).
     rasterizer: its repartition() is called with the new counts' maximum (no further collective).
-    transport: see ProcessGroupTransport; default ProcessGroupTransport(group).
+    transport: see ProcessGroupTransport; default ProcessGroupTransport(group).  PeerTransport(rasterizer) moves the table and the rows
+      over the peer workspace of a GaussianShardedRasterizer(exchange="p2p") instead, with no NCCL call.
 
     Communication: one all_gather of a [n_models, 11] int64 table (counts, row widths, Adam steps), the only host read, and, when some
-    row moves, one batch_isend_irecv of one packed buffer per (source, destination) pair.  The rows are packed by one
+    row moves, one exchange of one packed buffer per (source, destination) pair (ProcessGroupTransport: one batch_isend_irecv;
+    PeerTransport: the rounds of peer_rounds over its staging regions).  The rows are packed by one
     sgr_rebalance_pack launch and the new tensors written by one sgr_rebalance_splice launch; when no row moves (world 1, or ranks
     already balanced) nothing is launched."""
     tr = transport if transport is not None else ProcessGroupTransport(group)
@@ -1066,7 +1204,13 @@ def rebalance(models: Sequence, optimizer=None, group: Optional[dist.ProcessGrou
         args, scratch = _rebalance_tables(L, [(mv.model, dsts.index(mv.dst), mv.src_row_begin, 0, mv.src_row_end - mv.src_row_begin)
                                               for mv in sends], send_bufs, dev)
         _capi.call("sgr_rebalance_pack", dev, segs, nm, *args)
-    tr.exchange(dict(zip(dsts, send_bufs)), dict(zip(srcs, recv_bufs)))
+    if isinstance(tr, PeerTransport):  # it moves the rows in rounds that every rank must count alike: it takes every pair's size
+        sizes = [[0] * world for _ in range(world)]
+        for mv in plan.moves:
+            sizes[mv.src][mv.dst] += (mv.src_row_end - mv.src_row_begin) * rf[mv.model]
+        tr.exchange(dict(zip(dsts, send_bufs)), dict(zip(srcs, recv_bufs)), sizes)
+    else:
+        tr.exchange(dict(zip(dsts, send_bufs)), dict(zip(srcs, recv_bufs)))
     # splice: per model [received from lower ranks | kept | received from higher ranks]
     ranges = [(mv.model, srcs.index(mv.src), 0, mv.dst_row_begin, mv.src_row_end - mv.src_row_begin) for mv in recvs]
     ranges += [(mv.model, -1, mv.src_row_begin, mv.dst_row_begin, mv.src_row_end - mv.src_row_begin) for mv in plan.kept if mv.src == rank]

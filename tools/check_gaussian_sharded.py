@@ -20,6 +20,9 @@ kernels.
 
 With the argument `rebalance` only the rebalance leg runs (run_rebalance): sharded.rebalance over NCCL on an uneven split, against the
 global arrays each rank restates.  It has run at world 1 only, not on several H100s; tests/test_rebalance_gpu.py emulates 2 to 8 ranks.
+With `rebalance-p2p` the same leg renders through GaussianShardedRasterizer(exchange="p2p") and rebalances with
+transport=sharded.PeerTransport(rasterizer): the table and the rows go over the rasterizer's peer workspace, with no NCCL call.  It has
+not been run on several H100s; tests/test_rebalance_p2p_gpu.py emulates 2 to 8 ranks on one GPU.
 
 With the argument `checkpoint` only the checkpoint leg runs (run_checkpoint): sharded.save_checkpoint at world N over torch.distributed,
 sharded.load_checkpoint at the same world N into fresh models, and the next training step against the uninterrupted one.  It has run at
@@ -292,9 +295,10 @@ def run_features(rank, world, dev, W=1280, H=720, K=4):
             assert not bool(x[:, ~rows].any()), f"{mode} {name}: foreign rows not zero"
 
 
-def run_rebalance(rank, world, dev, W=640, H=400):
+def run_rebalance(rank, world, dev, W=640, H=400, exchange="nccl"):
     """Rebalance leg (argument `rebalance`): every rank builds the same with_raw scene, owns an uneven share of it (rank r weighted r + 1,
-    the last rank three times more), steps FusedAdam three times on it and calls sharded.rebalance (NCCL all_gather and batch_isend_irecv).
+    the last rank three times more), steps FusedAdam three times on it and calls sharded.rebalance (NCCL all_gather and batch_isend_irecv;
+    with exchange="p2p" the rasterizer's peer workspace through sharded.PeerTransport, after the render has set the workspace up).
     Each rank restates the global arrays and their Adam steps on its own GPU (the update is elementwise), so afterwards its new rows of
     every parameter, both moments and the statistics must be the even split's slice of them, bit for bit; one more step too.  The
     Gaussian-sharded render before and after has the single-GPU render's own rows bit for bit; densify_and_prune runs on the result."""
@@ -352,7 +356,7 @@ def run_rebalance(rank, world, dev, W=640, H=400):
     with torch.no_grad():
         xyz, rot, scale, opac, sh = sgb.compose(full, poses, idft)
         ref = sgb.GaussianRasterizer(st)(means3D=xyz, means2D=None, opacities=opac, shs=sh, scales=scale, rotations=rot)
-    rast = GaussianShardedRasterizer(st)
+    rast = GaussianShardedRasterizer(st, exchange=exchange)
 
     def render_own_rows(tag):
         with torch.no_grad():
@@ -362,7 +366,7 @@ def run_rebalance(rank, world, dev, W=640, H=400):
             assert torch.equal(a[:, img_rows], b[:, img_rows]), f"rebalance {tag}: {name} own rows differ"
 
     render_own_rows("before")
-    P_new = sharded.rebalance(mine, opt, rasterizer=rast)
+    P_new = sharded.rebalance(mine, opt, rasterizer=rast, transport=sharded.PeerTransport(rast) if exchange == "p2p" else None)
     base, extra = divmod(P, world)
     Bn = [r * base + min(r, extra) for r in range(world + 1)]
     assert P_new == Bn[rank + 1] - Bn[rank] and rast.chunk == base + (extra > 0), (P_new, rast.chunk)
@@ -656,9 +660,9 @@ def main():
             P, worst = run_checkpoint(rank, world, dev)
             print(f"[rank {rank}/{world}] checkpoint: saved at world {world} and resumed, {P} Gaussians, rows / moments / statistics bit for "
                   f"bit, the next step's own image rows bit-equal, gradients rel err {worst:.2e}", flush=True)
-        elif mode == "rebalance":
-            P_new = run_rebalance(rank, world, dev)
-            print(f"[rank {rank}/{world}] rebalance: {P_new} Gaussians, rows / moments / statistics the even split's slice bit for bit, "
+        elif mode in ("rebalance", "rebalance-p2p"):
+            P_new = run_rebalance(rank, world, dev, exchange="p2p" if mode == "rebalance-p2p" else "nccl")
+            print(f"[rank {rank}/{world}] {mode}: {P_new} Gaussians, rows / moments / statistics the even split's slice bit for bit, "
                   "own image rows bit-equal before and after", flush=True)
         else:
             run_all(rank, world, dev, mode)
