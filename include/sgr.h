@@ -190,7 +190,10 @@ int sgr_backward_geom(const SgrFrame *frame, const float *means3D, const float *
 
 /* Convenience: stage 1 + stage 2 on one device.  Replaces RasterizeGaussiansBackwardCUDA ->
  * CudaRasterizer::Rasterizer::backward (DGR/rasterize_points.cu:126-220, rasterizer_impl.cu:396-506; pybind name
- * `rasterize_gaussians_backward`, DGR/ext.cpp:17).  grad2d_scratch is P*12 floats of caller scratch. */
+ * `rasterize_gaussians_backward`, DGR/ext.cpp:17).  grad2d_scratch is P*12 floats of caller scratch: unlike sgr_backward_blend,
+ * only the rows of the Gaussians the forward reached (emitted an instance of, or whose inputs are not all finite) are cleared and read
+ * back, so its other rows keep whatever they held; the gradients equal those of sgr_backward_blend + sgr_backward_geom.  geom_state
+ * must come from sgr_forward, sgr_forward_bounded or sgr_forward_records. */
 int sgr_backward(const SgrFrame *frame, int64_t num_instances, const float *means3D, const float *shs,
                  const float *colors_precomp, const float *semantics, const float *scales, const float *rotations,
                  const float *cov3D_precomp, const int32_t *radii, const void *geom_state, const void *binning_state,

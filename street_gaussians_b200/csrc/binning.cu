@@ -84,10 +84,11 @@ __device__ __forceinline__ void zero_grad2d_row(float4 *__restrict__ rows, size_
 // zero_rows (nullable): this rank's partial grad2d[P,12].  The rows of the Gaussians delivered to this rank (radius != 0 <=>
 // rectangle meets the band) are the only ones its blend_bwd can touch and the only ones their owners read back, so they are
 // zeroed here — 48 B x (Gaussians in the band) instead of a 48 B x P_total memset in front of every backward.
+// reached: every Gaussian with a radius starts reached — the inputs of its chain rule were projected elsewhere and are not checked here.
 __global__ void __launch_bounds__(256) count_tiles_kernel(const FrameDev f, const GaussRec *__restrict__ rec,
                                                          const int32_t *__restrict__ radii, uint32_t *__restrict__ tiles_touched,
                                                          uint32_t *__restrict__ depth_key, uint32_t *__restrict__ iota,
-                                                         float4 *__restrict__ zero_rows) {
+                                                         uint32_t *__restrict__ reached, float4 *__restrict__ zero_rows) {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	const bool in_range = idx < f.P;
 	bool ok = false;
@@ -108,12 +109,13 @@ __global__ void __launch_bounds__(256) count_tiles_kernel(const FrameDev f, cons
 		tiles_touched[idx] = count;
 		depth_key[idx] = count > 0 ? __float_as_uint(depth) : 0xffffffffu;
 		iota[idx] = (uint32_t)idx;
+		reached[idx] = ok ? 1u : 0u;
 	}
 }
 cudaError_t launch_count_tiles(const FrameDev &f, GeomView g, const int32_t *radii, cudaStream_t st, float *zero_rows) {
 	if (f.P == 0) return cudaSuccess;
 	count_launch();
-	count_tiles_kernel<<<(f.P + 255) / 256, 256, 0, st>>>(f, g.rec, radii, g.tiles_touched, g.depth_key, g.iota,
+	count_tiles_kernel<<<(f.P + 255) / 256, 256, 0, st>>>(f, g.rec, radii, g.tiles_touched, g.depth_key, g.iota, g.reached,
 	                                                      reinterpret_cast<float4 *>(zero_rows));
 	return cudaGetLastError();
 }
@@ -246,11 +248,13 @@ constexpr uint32_t kEmitStage = 512;  // instances staged per warp (2 x 2 KB of 
 // only the Gaussians before the split emit; the far pass passes its own offsets, dev_cap -> the end of the emitted sequence,
 // dev_floor -> the near pass's end (the Gaussians before the split then have empty ranges there) and the KeepUnsaturated predicate.
 // A pass whose device-side cap does not exceed its floor (0 without one) has nothing to emit: the whole grid returns.
+// reached (nullable): set for every Gaussian with a non-empty range in this pass — the Gaussians the per-tile lists can hold, so the only
+// ones a blend backward can add to (the ranges already exclude what the bounded mode drops and, in the far pass, the saturated tiles).
 template <typename KeyT, typename Keep = KeepAll>
 __global__ void __launch_bounds__(256) emit_pairs_kernel(const FrameDev f, const GaussRec *__restrict__ rec, const int32_t *__restrict__ radii,
                                                         const uint32_t *__restrict__ perm, const uint32_t *__restrict__ offsets, KeyT *__restrict__ keys,
                                                         uint32_t *__restrict__ vals, uint32_t *__restrict__ big_list,
-                                                        uint32_t *__restrict__ big_count, uint32_t cap, const int n_order,
+                                                        uint32_t *__restrict__ big_count, uint32_t *__restrict__ reached, uint32_t cap, const int n_order,
                                                         const uint32_t *__restrict__ dev_cap = nullptr,
                                                         const uint32_t *__restrict__ dev_floor = nullptr, const Keep keep = Keep()) {
 	if (dev_cap && *dev_cap <= (dev_floor ? *dev_floor : 0u)) return;
@@ -284,6 +288,7 @@ __global__ void __launch_bounds__(256) emit_pairs_kernel(const FrameDev f, const
 			gidx = perm[t];  // (padding slots of the compacted order have end == off and a meaningless perm)
 			fp = rec_footprint(f, rec[gidx], radii[gidx]);
 			active = true;
+			if (reached) reached[gidx] = 1u;
 		}
 	}
 	const uint32_t warp_first = __shfl_sync(0xffffffffu, off, 0);
@@ -326,7 +331,8 @@ static cudaError_t launch_emit(const FrameDev &f, GeomView g, const int32_t *rad
 	KeyT *keys = reinterpret_cast<KeyT *>(b.keys_in);
 	count_launch(2);
 	emit_pairs_kernel<KeyT, Keep><<<(unsigned)((n_order + 255) / 256), 256, 0, st>>>(f, g.rec, radii, g.perm, offsets, keys, b.vals_in,
-	                                                                               g.big_list, status, cap32, n_order, dev_cap, dev_floor, keep);
+	                                                                               g.big_list, status, g.reached, cap32, n_order, dev_cap, dev_floor,
+	                                                                               keep);
 	// persistent-style grid for the deferred large rectangles
 	emit_big_kernel<KeyT, Keep><<<kNumSMs * 4, 256, 0, st>>>(f, g.rec, radii, g.perm, offsets, keys, b.vals_in, g.big_list, status, cap32, keep);
 	return cudaGetLastError();

@@ -294,9 +294,11 @@ __global__ void __launch_bounds__(256) blend_bwd_kernel(const FrameDev f, const 
 
 cudaError_t launch_blend_bwd(const FrameDev &f, GeomView g, BinView b, ImgView img, const float *semantics,
                              const float *out_alpha, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
-                             const float *dL_dsem, float *grad2d, float *dL_dsemantics, cudaStream_t st, bool grad2d_zeroed) {
+                             const float *dL_dsem, float *grad2d, float *dL_dsemantics, cudaStream_t st, bool grad2d_zeroed,
+                             const uint32_t *reached) {
 	if (f.P == 0) return cudaSuccess;
-	if (f.S <= 0) return launch_blend_bwd2(f, g, b, img, out_alpha, dL_dcolor, dL_ddepth, dL_dalpha, grad2d, st, grad2d_zeroed);  // two-phase fast path
+	if (f.S <= 0)  // two-phase fast path
+		return launch_blend_bwd2(f, g, b, img, out_alpha, dL_dcolor, dL_ddepth, dL_dalpha, grad2d, st, grad2d_zeroed, reached);
 	cudaError_t e = cudaMemsetAsync(grad2d, 0, (size_t)f.P * kNComp * sizeof(float), st);
 	if (e != cudaSuccess) return e;
 	if (f.S > 0 && (e = cudaMemsetAsync(dL_dsemantics, 0, (size_t)f.P * f.S * sizeof(float), st)) != cudaSuccess) return e;

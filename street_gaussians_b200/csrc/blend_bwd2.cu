@@ -305,11 +305,28 @@ __global__ void __launch_bounds__(256, 3) blend_bwd2_kernel(const FrameDev f, co
 	}
 }
 
+// zeroes the grad2d rows of the reached Gaussians: on a frame whose image comes from a few thousand near splats that is 4 B read per
+// Gaussian instead of 48 B written
+__global__ void __launch_bounds__(256) clear_reached_rows_kernel(const int P, const uint32_t *__restrict__ reached, float4 *__restrict__ rows) {
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= P || reached[i] == 0u) return;
+	const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+	rows[3 * (size_t)i] = z; rows[3 * (size_t)i + 1] = z; rows[3 * (size_t)i + 2] = z;
+}
+
 cudaError_t launch_blend_bwd2(const FrameDev &f, GeomView g, BinView b, ImgView img, const float *out_alpha, const float *dL_dcolor,
-                              const float *dL_ddepth, const float *dL_dalpha, float *grad2d, cudaStream_t st, bool grad2d_zeroed) {
+                              const float *dL_ddepth, const float *dL_dalpha, float *grad2d, cudaStream_t st, bool grad2d_zeroed,
+                              const uint32_t *reached) {
 	if (f.P == 0) return cudaSuccess;
 	// (grad2d_zeroed: sgr_sharded_forward already cleared the rows this band can touch — see count_tiles_kernel)
-	cudaError_t e = grad2d_zeroed ? cudaSuccess : cudaMemsetAsync(grad2d, 0, (size_t)f.P * 12 * sizeof(float), st);
+	cudaError_t e = cudaSuccess;
+	if (!grad2d_zeroed && reached) {
+		count_launch();
+		clear_reached_rows_kernel<<<(unsigned)((f.P + 255) / 256), 256, 0, st>>>(f.P, reached, reinterpret_cast<float4 *>(grad2d));
+		e = cudaGetLastError();
+	} else if (!grad2d_zeroed) {
+		e = cudaMemsetAsync(grad2d, 0, (size_t)f.P * 12 * sizeof(float), st);
+	}
 	if (e != cudaSuccess) return e;
 	const int rows = band_rows(f.band);
 	if (rows <= 0 || f.gx <= 0) return cudaSuccess;

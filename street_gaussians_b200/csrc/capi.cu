@@ -61,6 +61,7 @@ GeomView carve_geom(void *base, int P) {
 	g.jac = take<float4>(p, 3 * n);
 	g.ckey = take<uint32_t>(p, n);
 	g.cval = take<uint32_t>(p, n);
+	g.reached = g.cval;
 	g.temp_bytes = memo_bytes((int64_t)P, [](int64_t n) { return geom_temp_bytes((int)n); });
 	g.temp = take<char>(p, g.temp_bytes);
 	g.total_bytes = (size_t)(p - reinterpret_cast<char *>(base));
@@ -568,7 +569,8 @@ static int sharded_forward(const SgrFrame *frame, const SgrPeers *peers, const f
 		if ((rc = check_gaussian_inputs(fl, shs, colors_precomp, scales, rotations, cov3D_precomp)) != SGR_OK) return rc;
 	}
 	void *geom_state = pt.rec[pt.rank];  // this rank's gathered records ARE the head of its geom state
-	const GeomView g = carve_geom(geom_state, ft.P);
+	GeomView g = carve_geom(geom_state, ft.P);
+	g.reached = nullptr;  // (cval holds the compacted depth-sort input, which the layer rows' reset reads after the binning)
 	const ImgView img = carve_img(img_state, ft.W, ft.H);
 	if (geom_bytes < g.total_bytes) return fail(SGR_ENOMEM, "geom_state too small: %zu < %zu", geom_bytes, g.total_bytes);
 	if (!img_state || img_bytes < img.total_bytes) return fail(SGR_ENOMEM, "img_state too small: %zu < %zu", img_bytes, img.total_bytes);
@@ -798,10 +800,12 @@ int sgr_forward_status(const SgrFrame *frame, const void *geom_state, int64_t *n
 	return SGR_OK;
 }
 
-int sgr_backward_blend(const SgrFrame *frame, int64_t num_instances, const float *semantics, const void *geom_state,
-                       const void *binning_state, const void *img_state, const float *out_alpha, const float *dL_dcolor,
-                       const float *dL_ddepth, const float *dL_dalpha, const float *dL_dsemantic, float *grad2d,
-                       float *dL_dsemantics, void *stream) {
+// shared body of sgr_backward_blend (every grad2d row written) and sgr_backward (grad2d is scratch for the chain rule: `reached_only`
+// clears the rows of the Gaussians the forward reached, and only those are read back)
+static int backward_blend(const SgrFrame *frame, int64_t num_instances, const float *semantics, const void *geom_state,
+                          const void *binning_state, const void *img_state, const float *out_alpha, const float *dL_dcolor,
+                          const float *dL_ddepth, const float *dL_dalpha, const float *dL_dsemantic, float *grad2d,
+                          float *dL_dsemantics, bool reached_only, void *stream) {
 	FrameDev f;
 	int rc = make_frame(frame, f);
 	if (rc) return rc;
@@ -816,19 +820,28 @@ int sgr_backward_blend(const SgrFrame *frame, int64_t num_instances, const float
 	const GeomView g = carve_geom(const_cast<void *>(geom_state), f.P);
 	const ImgView img = carve_img(const_cast<void *>(img_state), f.W, f.H);
 	const BinView b = carve_bin(const_cast<void *>(binning_state), num_instances);
-	SGR_TRY(launch_blend_bwd(f, g, b, img, semantics, out_alpha, dL_dcolor, dL_ddepth, dL_dalpha, dL_dsemantic, grad2d, dL_dsemantics, st),
+	SGR_TRY(launch_blend_bwd(f, g, b, img, semantics, out_alpha, dL_dcolor, dL_ddepth, dL_dalpha, dL_dsemantic, grad2d, dL_dsemantics, st,
+	                         false, reached_only ? g.reached : nullptr),
 	        "blend_bwd");
 	return SGR_OK;
+}
+int sgr_backward_blend(const SgrFrame *frame, int64_t num_instances, const float *semantics, const void *geom_state,
+                       const void *binning_state, const void *img_state, const float *out_alpha, const float *dL_dcolor,
+                       const float *dL_ddepth, const float *dL_dalpha, const float *dL_dsemantic, float *grad2d,
+                       float *dL_dsemantics, void *stream) {
+	return backward_blend(frame, num_instances, semantics, geom_state, binning_state, img_state, out_alpha, dL_dcolor, dL_ddepth, dL_dalpha,
+	                      dL_dsemantic, grad2d, dL_dsemantics, false, stream);
 }
 
 // shared body of sgr_backward_geom (no layer table) and sgr_backward_geom_layered; `fn` names the entry point in error messages.
 // With a live layer (grad2d set, non-empty range) the layers' rows are merged into grad2d before the chain rule, and the main
-// dL_dmeans2D of their range is restored from the pre-merge rows afterwards.
+// dL_dmeans2D of their range is restored from the pre-merge rows afterwards.  reached_only (sgr_backward, no layers): only the rows of
+// the Gaussians the forward reached are read.
 static int backward_geom(const char *fn, const SgrFrame *frame, const float *means3D, const float *shs, const float *colors_precomp,
                          const float *scales, const float *rotations, const float *cov3D_precomp, const int32_t *radii,
                          const void *geom_state, float *grad2d, const SgrLayerGrad *layers, int32_t num_layers, float *scratch,
                          float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh, float *dL_dcolors_precomp, float *dL_dopacity,
-                         float *dL_dscales, float *dL_drotations, float *dL_dcov3D, void *stream) {
+                         float *dL_dscales, float *dL_drotations, float *dL_dcov3D, void *stream, bool reached_only = false) {
 	FrameDev f;
 	int rc = make_frame(frame, f);
 	if (rc) return rc;
@@ -855,7 +868,8 @@ static int backward_geom(const char *fn, const SgrFrame *frame, const float *mea
 	}
 	SGR_TRY(launch_preprocess_bwd(f, nullptr, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii, g.jac, grad2d, dL_dmeans3D,
 	                              dL_dmeans2D, shs ? dL_dsh : nullptr, dL_dcolors_precomp, dL_dopacity,
-	                              cov3D_precomp ? nullptr : dL_dscales, cov3D_precomp ? nullptr : dL_drotations, dL_dcov3D, st),
+	                              cov3D_precomp ? nullptr : dL_dscales, cov3D_precomp ? nullptr : dL_drotations, dL_dcov3D, st,
+	                              reached_only ? g.reached : nullptr),
 	        "preprocess_bwd");
 	if (hi > lo) SGR_TRY(launch_layer_stash(grad2d, lo, hi, scratch, true, dL_dmeans2D, st), "layer restore");
 	return SGR_OK;
@@ -879,12 +893,12 @@ int sgr_backward(const SgrFrame *frame, int64_t num_instances, const float *mean
                  const float *dL_dalpha, const float *dL_dsemantic, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh,
                  float *dL_dcolors_precomp, float *dL_dsemantics, float *dL_dopacity, float *dL_dscales,
                  float *dL_drotations, float *dL_dcov3D, float *grad2d_scratch, void *stream) {
-	int rc = sgr_backward_blend(frame, num_instances, semantics, geom_state, binning_state, img_state, out_alpha, dL_dcolor, dL_ddepth,
-	                            dL_dalpha, dL_dsemantic, grad2d_scratch, dL_dsemantics, stream);
+	int rc = backward_blend(frame, num_instances, semantics, geom_state, binning_state, img_state, out_alpha, dL_dcolor, dL_ddepth,
+	                        dL_dalpha, dL_dsemantic, grad2d_scratch, dL_dsemantics, true, stream);
 	if (rc) return rc;
-	return sgr_backward_geom(frame, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii, geom_state, grad2d_scratch,
-	                         dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors_precomp, dL_dopacity, dL_dscales, dL_drotations, dL_dcov3D,
-	                         stream);
+	return backward_geom("sgr_backward", frame, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii, geom_state,
+	                     grad2d_scratch, nullptr, 0, nullptr, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors_precomp, dL_dopacity, dL_dscales,
+	                     dL_drotations, dL_dcov3D, stream, true);
 }
 
 // ---- render layers ----

@@ -27,6 +27,9 @@ namespace sgr {
 constexpr int kShRow = 49;  // padded smem row (floats) for up to 16 x 3 SH coefficients
 constexpr int kBwdStride = 52;  // row stride (floats) of the TMA variant's stage: 208 B
 
+// reached (nullable, !GATHER only): the forward's reached words (GeomView::reached).  A Gaussian without one loads nothing but its word
+// and writes zeros: its grad2d row may hold anything (launch_blend_bwd cleared only the reached rows), and with a zero row and finite
+// inputs its chain rule gives zeros (+-0) anyway — the forward marked every visible Gaussian whose inputs are not all finite.
 // GATHER = true (sgr_sharded_backward): grad2d is not a local array — the 12 sums of local Gaussian idx (global id
 // rank*chunk + idx) are read from the partial grad2d of every rank whose cyclic band its rectangle meets (NVLink peer loads)
 // and added in ascending rank order, exactly what sgr_gather_grad2d produced as a separate pass.
@@ -36,14 +39,16 @@ __global__ void __launch_bounds__(256) preprocess_bwd_kernel(
     const float *__restrict__ scales, const float *__restrict__ rotations, const float *__restrict__ cov3D_precomp,
     const int32_t *__restrict__ radii, const float4 *__restrict__ jac, const float *__restrict__ grad2d,
     float *__restrict__ dL_dmeans3D, float *__restrict__ dL_dmeans2D, float *__restrict__ dL_dsh, float *__restrict__ dL_dcolors,
-    float *__restrict__ dL_dopacity, float *__restrict__ dL_dscales, float *__restrict__ dL_drot, float *__restrict__ dL_dcov3D) {
+    float *__restrict__ dL_dopacity, float *__restrict__ dL_dscales, float *__restrict__ dL_drot, float *__restrict__ dL_dcov3D,
+    const uint32_t *__restrict__ reached) {
 	extern __shared__ float s_sh[];  // [warps][32][kShRow] when STAGED
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const bool in_range = idx < f.P;
+	const bool need = in_range && (GATHER || reached == nullptr || reached[idx] != 0u);
 	const size_t i = (size_t)idx;
 	const int nsh = f.M * 3;
-	const bool visible = in_range && radii[idx] > 0;
+	const bool visible = need && radii[idx] > 0;
 	float *srow = STAGED ? (s_sh + ((size_t)warp * 32 + lane) * kShRow) : nullptr;
 
 	float4 g0v = make_float4(0.f, 0.f, 0.f, 0.f), g1v = g0v, g2v = g0v;
@@ -54,7 +59,7 @@ __global__ void __launch_bounds__(256) preprocess_bwd_kernel(
 		gather_runs(pt, mask, rs, s_g, g0v, g1v, g2v);
 	}
 	if (in_range) {
-		if (!GATHER) {
+		if (!GATHER && need) {
 			g0v = reinterpret_cast<const float4 *>(grad2d)[3 * i];      // mean2D.x, .y, .z(abs), conic.xx
 			g1v = reinterpret_cast<const float4 *>(grad2d)[3 * i + 1];  // conic.xy, conic.yy, opacity, color.r
 			g2v = reinterpret_cast<const float4 *>(grad2d)[3 * i + 2];  // color.g, color.b, depth, pad
@@ -174,12 +179,14 @@ __global__ void __launch_bounds__(256, 3) preprocess_bwd_tma_kernel(
     const float *__restrict__ rotations, const float *__restrict__ cov3D_precomp, const int32_t *__restrict__ radii,
     const float4 *__restrict__ jac, const float *__restrict__ grad2d, float *__restrict__ dL_dmeans3D, float *__restrict__ dL_dmeans2D,
     float *__restrict__ dL_dsh, float *__restrict__ dL_dopacity, float *__restrict__ dL_dscales, float *__restrict__ dL_drot,
-    float *__restrict__ dL_dcov3D) {
+    float *__restrict__ dL_dcov3D, const uint32_t *__restrict__ reached) {
 	extern __shared__ __align__(16) unsigned char s_stage[];
 	__shared__ float s_cam[36];
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const bool in_range = idx < f.P;
+	// (an unreached Gaussian keeps radius 0 below: every gradient it writes is then the zero of a culled one)
+	const bool need = in_range && (GATHER || reached == nullptr || reached[idx] != 0u);
 	const size_t i = (size_t)idx;
 	const int nsh = f.M * 3;
 	const uint32_t row_bytes = (uint32_t)nsh * 4u;
@@ -192,7 +199,7 @@ __global__ void __launch_bounds__(256, 3) preprocess_bwd_tma_kernel(
 	float4 q = make_float4(1.f, 0.f, 0.f, 0.f);
 	float c6[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
 	ColorJac cj = {g0v, g0v, g0v};
-	if (in_range) {
+	if (need) {
 		radius = radii[idx];
 		mean = make_float3(means3D[3 * i], means3D[3 * i + 1], means3D[3 * i + 2]);
 		if (cov3D_precomp != nullptr) {
@@ -304,9 +311,11 @@ constexpr size_t kBwdStageBytes = (size_t)8 * 32 * kBwdStride * sizeof(float);
 cudaError_t launch_preprocess_bwd(const FrameDev &f, const PeerTable *pt, const float *means3D, const float *shs, const float *colors_precomp,
                                   const float *scales, const float *rotations, const float *cov3D_precomp, const int32_t *radii,
                                   const float4 *jac, const float *grad2d, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh,
-                                  float *dL_dcolors, float *dL_dopacity, float *dL_dscales, float *dL_drot, float *dL_dcov3D, cudaStream_t st) {
+                                  float *dL_dcolors, float *dL_dopacity, float *dL_dscales, float *dL_drot, float *dL_dcov3D, cudaStream_t st,
+                                  const uint32_t *reached) {
 	if (f.P == 0) return cudaSuccess;
 	const bool gather = pt != nullptr;  // pt == nullptr: the local path, grad2d holds this process's screen-space sums
+	if (gather) reached = nullptr;      // (the gathered sums come from other ranks' emissions)
 	const PeerTable peers = gather ? *pt : PeerTable{};
 	const unsigned grid = (unsigned)((f.P + 255) / 256);
 	cudaError_t e;
@@ -316,7 +325,7 @@ cudaError_t launch_preprocess_bwd(const FrameDev &f, const PeerTable *pt, const 
 		if ((e = ensure_dynamic_smem(kernel, (int)kBwdStageBytes, configured[gather])) != cudaSuccess) return e;
 		count_launch();
 		kernel<<<grid, 256, kBwdStageBytes, st>>>(f, peers, means3D, scales, rotations, cov3D_precomp, radii, jac, grad2d, dL_dmeans3D,
-		                                          dL_dmeans2D, dL_dsh, dL_dopacity, dL_dscales, dL_drot, dL_dcov3D);
+		                                          dL_dmeans2D, dL_dsh, dL_dopacity, dL_dscales, dL_drot, dL_dcov3D, reached);
 		return cudaGetLastError();
 	}
 	const bool staged = shs != nullptr && f.M <= 16;  // rows of up to 48 floats fit the padded smem row
@@ -329,7 +338,7 @@ cudaError_t launch_preprocess_bwd(const FrameDev &f, const PeerTable *pt, const 
 	}
 	count_launch();
 	kernel<<<grid, 256, smem, st>>>(f, peers, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, radii, jac, grad2d, dL_dmeans3D,
-	                                dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drot, dL_dcov3D);
+	                                dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drot, dL_dcov3D, reached);
 	return cudaGetLastError();
 }
 

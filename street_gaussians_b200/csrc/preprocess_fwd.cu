@@ -10,7 +10,10 @@
 // contribution (exact opacity-aware row-span cull, tile_visit.cuh) and that lie in this process's tile-row band,
 // (4) large rectangles are counted warp-cooperatively instead of by one thread, (5) a 32-bit depth key per Gaussian
 // feeds the depth pre-sort of binning.cu, (6) the SH colour's 3 x 3 direction Jacobian (+ clamp bits) is stored for the backward,
-// which then never reads the coefficient rows.  The per-Gaussian geometry it shares with the backward is in gaussian_geom.cuh.
+// which then never reads the coefficient rows, (7) the reached word (GeomView::reached) starts here: 1 for a visible Gaussian whose
+// chain-rule inputs (position, shape, camera, colour Jacobian) are not all finite, so that the backward runs its chain rule on a zero
+// row exactly as it runs every other one and turns a non-finite input into the same NaN / Inf; 0 otherwise, until the emission marks it.
+// The per-Gaussian geometry it shares with the backward is in gaussian_geom.cuh.
 #include "gaussian_geom.cuh"
 #include "tile_visit.cuh"
 
@@ -126,7 +129,8 @@ __global__ void __launch_bounds__(256) preprocess_fwd_kernel(const FrameDev f, c
                                                              const float *__restrict__ rotations, const float *__restrict__ cov3D_precomp,
                                                              int32_t *__restrict__ radii, GaussRec *__restrict__ rec,
                                                              float4 *__restrict__ jac, uint32_t *__restrict__ tiles_touched, uint32_t *__restrict__ depth_key,
-                                                             uint32_t *__restrict__ iota, const size_t cnt_offset = 0) {
+                                                             uint32_t *__restrict__ iota, uint32_t *__restrict__ reached,
+                                                             const size_t cnt_offset = 0) {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	const bool in_range = idx < f.P;
 	// every small per-Gaussian input is requested up front, before any arithmetic: one DRAM round trip instead of three
@@ -148,8 +152,18 @@ __global__ void __launch_bounds__(256) preprocess_fwd_kernel(const FrameDev f, c
 	if (threadIdx.x < 16) s_cam[threadIdx.x] = f.view[threadIdx.x];
 	else if (threadIdx.x < 32) s_cam[threadIdx.x] = f.proj[threadIdx.x - 16];
 	else if (threadIdx.x < 35) s_cam[threadIdx.x] = f.campos[threadIdx.x - 32];
-	__syncthreads();
+	const bool cam_finite = __syncthreads_and(threadIdx.x >= 35 || isfinite(s_cam[threadIdx.x])) &&
+	                        isfinite(f.fx + f.fy + f.tanx + f.tany + f.mod);
 	if (in_range) pr = project_gaussian(f, s_cam, s_cam + 16, p, shape, cov3D_precomp != nullptr);
+	// the inputs of the backward's chain rule (the colour Jacobian's entries are added below): a sum of finite values that overflows
+	// marks a Gaussian too, which only costs it the shortcut
+	float in_sum = p.x + p.y + p.z;
+	if (cov3D_precomp != nullptr) {
+#pragma unroll
+		for (int k = 0; k < 6; k++) in_sum += shape.c6[k];
+	} else {
+		in_sum += shape.s.x + shape.s.y + shape.s.z + shape.q.x + shape.q.y + shape.q.z + shape.q.w;
+	}
 	GaussRec rec_out;
 	rec_out.q0 = rec_out.q1 = rec_out.q2 = make_float4(0.f, 0.f, 0.f, 0.f);
 	if (in_range) {
@@ -170,6 +184,8 @@ __global__ void __launch_bounds__(256) preprocess_fwd_kernel(const FrameDev f, c
 				float J[9];
 				sh_color_jacobian(f.D, x, y, z, c, J);
 				store_color_jac(jac + 3 * (size_t)idx, J, clamp_bits);
+#pragma unroll
+				for (int k = 0; k < 9; k++) in_sum += J[k];
 			} else {
 				rgb = make_float3(colors_precomp[3 * (size_t)idx], colors_precomp[3 * (size_t)idx + 1], colors_precomp[3 * (size_t)idx + 2]);
 			}
@@ -236,6 +252,7 @@ __global__ void __launch_bounds__(256) preprocess_fwd_kernel(const FrameDev f, c
 		// sort key of the depth pre-sort: Gaussians that emit nothing go to the very end
 		depth_key[idx] = count > 0 ? __float_as_uint(pr.depth) : 0xffffffffu;
 		iota[idx] = (uint32_t)idx;
+		reached[idx] = pr.ok && !(cam_finite && isfinite(in_sum)) ? 1u : 0u;
 	}
 }
 
@@ -268,7 +285,8 @@ cudaError_t launch_preprocess_fwd(const FrameDev &f, const float *means3D, const
 	if (f.P == 0) return cudaSuccess;
 	count_launch();
 	preprocess_fwd_kernel<true><<<(f.P + 255) / 256, 256, 0, st>>>(f, PeerTable{}, means3D, shs, colors_precomp, opacities, scales, rotations,
-	                                                                  cov3D_precomp, radii, g.rec, g.jac, g.tiles_touched, g.depth_key, g.iota);
+	                                                                  cov3D_precomp, radii, g.rec, g.jac, g.tiles_touched, g.depth_key, g.iota,
+	                                                                  g.reached);
 	return cudaGetLastError();
 }
 cudaError_t launch_project(const FrameDev &f, const float *means3D, const float *shs, const float *colors_precomp,
@@ -277,7 +295,7 @@ cudaError_t launch_project(const FrameDev &f, const float *means3D, const float 
 	if (f.P == 0) return cudaSuccess;
 	count_launch();
 	preprocess_fwd_kernel<false><<<(f.P + 255) / 256, 256, 0, st>>>(f, PeerTable{}, means3D, shs, colors_precomp, opacities, scales, rotations,
-	                                                                   cov3D_precomp, radii, rec, jac, nullptr, nullptr, nullptr);
+	                                                                   cov3D_precomp, radii, rec, jac, nullptr, nullptr, nullptr, nullptr);
 	return cudaGetLastError();
 }
 cudaError_t launch_project_scatter(const FrameDev &f, const PeerTable &pt, const float *means3D, const float *shs,
@@ -288,7 +306,8 @@ cudaError_t launch_project_scatter(const FrameDev &f, const PeerTable &pt, const
 	count_launch();
 	const unsigned nblk = (unsigned)((pt.chunk + kRunBlock - 1) / kRunBlock);
 	preprocess_fwd_kernel<false, true><<<nblk, 256, 0, st>>>(f, pt, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-	                                                         radii_local, rec_local, jac_local, nullptr, masks_local, nullptr, cnt_offset);
+	                                                         radii_local, rec_local, jac_local, nullptr, masks_local, nullptr, nullptr,
+	                                                         cnt_offset);
 	return cudaGetLastError();
 }
 cudaError_t launch_filter(const FrameDev &f, const float *means3D, const float *scales, const float *rotations,

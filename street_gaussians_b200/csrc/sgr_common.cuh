@@ -42,6 +42,9 @@ struct GeomView {
 	float4 *jac;              // per Gaussian with SH colour: 3 float4, d colour / d view direction + clamp bits (gaussian_geom.cuh)
 	uint32_t *ckey, *cval;    // compacted depth-sort input (keys / Gaussian indices), Gaussian-sharded forward only; the saturation
 	                          // split's far offsets live in ckey (and its far counts in iota, dead after the depth sort)
+	uint32_t *reached;        // per Gaussian: non-zero if the backward must read its grad2d row and run its chain rule — the forward
+	                          // emitted an instance of it, or one of its inputs is not finite.  Lives in cval (carve_geom); nullptr in
+	                          // the fused Gaussian-sharded forward, whose cval is live.  See launch_preprocess_fwd / emit_pairs_kernel.
 	void *temp;               // cub temp storage: max(scan, depth sort)
 	size_t temp_bytes;
 	size_t total_bytes;
@@ -474,16 +477,24 @@ cudaError_t launch_blend_fwd(const FrameDev &f, GeomView g, BinView b, ImgView i
                              float *out_depth, float *out_alpha, float *out_sem, cudaStream_t st, BlendPass pass = kBlendFull);
 cudaError_t launch_blend_bwd(const FrameDev &f, GeomView g, BinView b, ImgView img, const float *semantics,
                              const float *out_alpha, const float *dL_dcolor, const float *dL_ddepth, const float *dL_dalpha,
-                             const float *dL_dsem, float *grad2d, float *dL_dsemantics, cudaStream_t st, bool grad2d_zeroed = false);
+                             const float *dL_dsem, float *grad2d, float *dL_dsemantics, cudaStream_t st, bool grad2d_zeroed = false,
+                             const uint32_t *reached = nullptr);
+// grad2d_zeroed: the caller cleared the rows the blend can touch.  Otherwise reached == nullptr clears all f.P rows, and reached = the
+// forward's reached words (GeomView) clears only the rows of reached Gaussians: the others stay as they were, so grad2d is then scratch
+// for launch_preprocess_bwd with the same words (S > 0, blend_bwd_kernel: every row and dL_dsemantics are cleared whatever `reached`).
 cudaError_t launch_blend_bwd2(const FrameDev &f, GeomView g, BinView b, ImgView img, const float *out_alpha, const float *dL_dcolor,
-                              const float *dL_ddepth, const float *dL_dalpha, float *grad2d, cudaStream_t st, bool grad2d_zeroed = false);
+                              const float *dL_ddepth, const float *dL_dalpha, float *grad2d, cudaStream_t st, bool grad2d_zeroed = false,
+                              const uint32_t *reached = nullptr);
 // pt == nullptr: grad2d holds the f.P x 12 screen-space sums of this process.  With a peer table (sgr_sharded_backward, with
 // sgr_gather_grad2d fused in) the sums of each local Gaussian are summed from the ranks that rendered it while the chain rule runs,
 // and grad2d carries instead the destination masks (u32[f.P]) the forward stored.
+// reached (pt == nullptr only; nullable): the forward's reached words.  The row of a Gaussian without one is taken as zero and not read,
+// so it may hold anything (launch_blend_bwd with the same words), and the chain rule of such a Gaussian, all zeros, is not run.
 cudaError_t launch_preprocess_bwd(const FrameDev &f, const PeerTable *pt, const float *means3D, const float *shs, const float *colors_precomp,
                                   const float *scales, const float *rotations, const float *cov3D_precomp, const int32_t *radii,
                                   const float4 *jac, const float *grad2d, float *dL_dmeans3D, float *dL_dmeans2D, float *dL_dsh,
-                                  float *dL_dcolors, float *dL_dopacity, float *dL_dscales, float *dL_drot, float *dL_dcov3D, cudaStream_t st);
+                                  float *dL_dcolors, float *dL_dopacity, float *dL_dscales, float *dL_drot, float *dL_dcov3D, cudaStream_t st,
+                                  const uint32_t *reached = nullptr);
 // render layers (layers.cu)
 cudaError_t launch_layer_lists(const FrameDev &f, ImgView main_img, BinView main_bin, int begin, int end, ImgView layer_img, uint32_t *layer_list,
                                cudaStream_t st);

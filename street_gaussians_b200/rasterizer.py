@@ -406,6 +406,30 @@ def _backward_geom_impl(settings, band, st: _ForwardState, tensors, radii, grad2
     return grads
 
 
+def _backward_impl(settings, band, st: _ForwardState, tensors, radii, alpha, grad_color, grad_depth, grad_alpha, grad_semantic,
+                   grad2d_scratch: Optional[torch.Tensor] = None):
+    """Both stages in one call (sgr_backward): returns (the 8 chain-rule outputs of _backward_geom_impl, dL_dsemantics[P,S]).  The
+    grad2d rows are scratch of the call (a fresh tensor unless `grad2d_scratch` is given), so only those of the Gaussians the forward
+    reached are cleared and read."""
+    means3D = tensors["means3D"]
+    device, P = means3D.device, means3D.shape[0]
+    S = int(tensors["semantics"].shape[1]) if tensors["semantics"] is not None else 0
+    sh, colors, scales, rots, cov = (tensors[k] for k in ("sh", "colors_precomp", "scales", "rotations", "cov3Ds_precomp"))
+    M = int(sh.shape[1]) if sh is not None else 0
+    fr, keep = _make_frame(settings, P, M, S, device, band)
+    grad2d = grad2d_scratch if grad2d_scratch is not None else torch.empty((P, 12), device=device, dtype=torch.float32)
+    g_sem = torch.empty((P, S), device=device, dtype=torch.float32)
+    gc, gd, ga = (_capi.f32(g, device, align16=True) for g in (grad_color, grad_depth, grad_alpha))
+    gs = _capi.f32(grad_semantic, device, align16=True) if S > 0 else None
+    g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rots, g_cov = grads = _geom_grad_buffers(tensors, P, device)
+    _capi.call("sgr_backward", device, C.byref(fr), st.num_instances, ptr(means3D), ptr(sh), ptr(colors), ptr(tensors["semantics"]),
+               ptr(scales), ptr(rots), ptr(cov), ptr(radii), ptr(st.geom), ptr(st.binning), ptr(st.img), ptr(alpha), ptr(gc), ptr(gd),
+               ptr(ga), ptr(gs), ptr(g_means3D), ptr(g_means2D), ptr(g_sh), ptr(g_colors), ptr(g_sem), ptr(g_opac), ptr(g_scales),
+               ptr(g_rots), ptr(g_cov), ptr(grad2d))
+    del keep
+    return grads, g_sem
+
+
 def _forward_or_dump(means3D, sh, colors_precomp, semantics, opacities, scales, rotations, cov3Ds_precomp, raster_settings, band, capacity):
     try:
         return _forward_impl(means3D, sh, colors_precomp, semantics, opacities, scales, rotations, cov3Ds_precomp, raster_settings, band,
@@ -491,6 +515,12 @@ class _RasterizeGaussians(torch.autograd.Function):
         grad_color, grad_depth, grad_alpha, grad_semantic = _image_grads(settings, tensors["means3D"].device,
                                                                          (grad_color, grad_depth, grad_alpha, grad_semantic), (3, 1, 1, S))
         try:
+            if ctx.grad_reduce is None and not n and st.geom is not None:
+                # the screen-space sums stay inside this call: sgr_backward clears and reads only the reached Gaussians' rows
+                grads, g_sem = _backward_impl(settings, band, st, tensors, radii, alpha, grad_color, grad_depth, grad_alpha, grad_semantic)
+                g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rots, g_cov = grads
+                return _fit_grads(shapes, (g_means3D, g_means2D, g_sh, g_colors, g_sem if S > 0 else None, g_opac, g_scales, g_rots,
+                                           g_cov)) + nones
             grad2d, g_sem = _backward_blend_impl(settings, band, st, tensors, alpha, grad_color, grad_depth, grad_alpha, grad_semantic)
             if ctx.grad_reduce is not None:  # multi-GPU: sum the per-band partial sums across ranks (one collective)
                 grad2d, g_sem = ctx.grad_reduce(grad2d, g_sem)
